@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the B200-native FastSpeech2 + HiFi-GAN inference path (driver contract in the task brief).
+"""bench.py -- throughput of the H100-native FastSpeech2 + HiFi-GAN inference path.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            our arm (N>1: launched under torchrun, one rank per GPU)
   python bench.py --impl reference [...]                          CPU reference arm (oracle port of the reference, host cores)
+  python bench.py ... --dump-outputs DIR                          also write what the last timed step computed as DIR/<name>.npy
 
 A "step" is one pass of the hot path over one synthetic batch per GPU: FastSpeech2.forward (phonemes -> mel, including the
 single host sync on max(mel_len)) followed by hifigan Generator.forward (mel -> 22.05 kHz fp32 waveform), i.e.
@@ -11,6 +12,7 @@ BASELINE.json configs[2]; the mel-only configs[1] number is reported in `extra`.
 from __future__ import annotations
 
 import argparse
+import atexit
 import gc
 import json
 import os
@@ -50,7 +52,36 @@ def parse():
     ap.add_argument("--voc-pair-kmax", type=int, default=None, help="override hifigan.Generator.pair_kmax (largest kernel size run as fused pairs)")
     ap.add_argument("--voc-pair-mask", type=int, default=None, help="override hifigan.Generator.pair_mask (A/B of the per-pair fused launches)")
     ap.add_argument("--fs2-f8", type=int, default=None, choices=[0, 1], help="override the decoder / PostNet operand split (A/B)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step (rank 0) as DIR/<name>.npy (float32 / float64, <= 64 MB)")
     return ap.parse_args()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, out, wav):
+    """What a caller of the timed path receives from one step: FastSpeech2.forward's outputs (the masks are implied by mel_lens /
+    src_lens) and the waveform.  Integer outputs are stored as float64.  Arrays are written whole while they fit the budget; a larger one
+    is replaced by a fixed, seeded sample of its flattened elements (`<name>.npy`) with their flat indices (`<name>_index.npy`)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    names = ("mel", "postnet_mel", "pitch", "energy", "log_duration", "duration_rounded")
+    arrays = {n: out[i] for i, n in enumerate(names)}
+    arrays["src_lens"], arrays["mel_lens"], arrays["wav"] = out[8], out[9], wav
+    budget = DUMP_LIMIT_BYTES
+    for name, t in arrays.items():                           # (small arrays first: the waveform is last)
+        a = t.detach().cpu()
+        a = (a.double() if not a.is_floating_point() else a.float()).numpy()
+        if a.nbytes <= budget:
+            np.save(os.path.join(dirname, name + ".npy"), a)
+            budget -= a.nbytes
+            continue
+        k = max(1, min(a.size, budget // 12))                # value (4 B) + index (8 B) per sampled element
+        idx = np.sort(np.random.default_rng(0).choice(a.size, size=k, replace=False))
+        np.save(os.path.join(dirname, name + ".npy"), a.reshape(-1)[idx])
+        np.save(os.path.join(dirname, name + "_index.npy"), idx.astype(np.float64))
+        budget -= k * 12
 
 
 def peaks():
@@ -59,12 +90,14 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"], "tflops_sustained": d["bf16_tflops_sustained"],
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0,
+            "source": "NVIDIA H100 SXM data sheet (dense BF16, 700 W card), not measured"}
 
 
 _NVML_LOOP = r"""
-import sys, time
+import os, sys, time
 import pynvml as N
+parent = os.getppid()
 N.nvmlInit()
 h = N.nvmlDeviceGetHandleByIndex(int(sys.argv[1]))
 period, light = float(sys.argv[3]) / 1e3, sys.argv[4] == "clocks"
@@ -72,7 +105,7 @@ mx = N.nvmlDeviceGetMaxClockInfo(h, N.NVML_CLOCK_SM)
 get_reasons = getattr(N, "nvmlDeviceGetCurrentClocksEventReasons", None) or N.nvmlDeviceGetCurrentClocksThrottleReasons
 out = open(sys.argv[2], "w")
 k = 0
-while True:
+while os.getppid() == parent:         # ends with the benchmark process, however that ends
     t0 = time.perf_counter()
     full = not light or k % 5 == 0          # "clocks": power and event reasons on every 5th sample only
     r = get_reasons(h) if full else -1
@@ -115,6 +148,12 @@ class ClockSampler:
                 self.mode = "nvidia-smi"
             except Exception:
                 self.proc = None
+        atexit.register(self._kill)          # no helper outlives the benchmark, also when it fails before stop()
+
+    def _kill(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.kill()
+            self.proc.wait()
 
     def stop(self):
         if self.proc is None:
@@ -409,8 +448,11 @@ def run_ours(args):
     del out, wav                                      # (timed() keeps at most one previous result set alive, like the warm-up loop)
 
     # N > 1: the asynchronous gather of the last step completes inside the timed region (flush before the closing event)
-    ms_total, launches, _ = timed(step_device, args.steps) if gather is None else _timed_with_flush(timed, step_device, gather, args.steps, args.prime)
+    ms_total, launches, last = timed(step_device, args.steps) if gather is None else _timed_with_flush(timed, step_device, gather, args.steps, args.prime)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last)
+    del last
     spread_device = dict(timed.spread)
     value = samples_step * args.steps / (ms_total * 1e-3)
 
@@ -433,7 +475,7 @@ def run_ours(args):
         return list(ms), list(fl), list(cnt)
 
     def tensor_roofline(fn, ms_step):
-        """Roofline of the dominant kernel class = the tcgen05 kernels (implicit-GEMM conv1d + fused ResBlock group).  Bracketing every
+        """Roofline of the dominant kernel class = the tensor-core kernels (implicit-GEMM conv1d + fused ResBlock group).  Bracketing every
         launch with two events costs a bubble per launch, so the class's duration inside the TIMED region is its share of the
         bracketed pass times the event-timed step; the raw bracketed figure is reported next to it."""
         ms, fl, cnt = class_profile(fn)
@@ -449,18 +491,12 @@ def run_ours(args):
     roof = None
     if rank == 0:
         r = tensor_roofline(step_local, ms_total / args.steps)
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "r02", "step_traffic.json")
-        if os.path.exists(tp):
-            tj = json.load(open(tp))
-            traffic, traffic_src = tj.get("tcgen05_class_dram_bytes_per_launch"), tj.get("source")
-        roof = {"kernel": "tcgen05 kernel class: conv_tc_kernel (implicit-GEMM conv1d: FFT-block projections / conv-FFN of encoder and decoder, "
+        roof = {"kernel": "tensor-core kernel class: conv_tc_kernel (implicit-GEMM conv1d: FFT-block projections / conv-FFN of encoder and decoder, "
                           "variance predictors, PostNet, HiFi-GAN convs) + resstack_kernel (fused ResBlock group / pairs); attention, layer norm "
                           "and the few fp32 CUDA-core launches are separate classes (other_classes_ms) and NOT counted",
                 "bound": "tensor", "achieved": r["achieved"], "peak": pk["tflops_sustained"], "unit": "TFLOP/s", "frac": r["frac"],
-                "peak_source": pk["source"] + ", bf16 sustained (kernels timed inside a long step); two MMAs per useful MMA-equivalent in the "
+                "peak_source": pk["source"] + "; two MMAs per useful MMA-equivalent in the "
                                               "f16+f8 operand split, three in the split-fp16 one: 0.50 / 0.33 of the peak is the ceiling",
-                "traffic": traffic, "traffic_source": traffic_src,
                 "timing": "class share from one untimed step with CUDA events around every launch x the event-timed step", **{k: v for k, v in r.items() if k not in ("achieved", "frac")}}
 
     # ------------------------------------------------------------------ the other BASELINE.json configs (N = 1: all of them; N > 1: the configs[4] shard)
@@ -574,6 +610,8 @@ def _timed_with_flush(timed, step, gather, steps, prime):
 def main():
     args = parse()
     if args.impl == "reference":
+        if args.dump_outputs:
+            sys.exit("bench.py: --dump-outputs applies to the GPU arm (--impl ours) only")
         run_reference(args)
         return
     if args.gpus > 1 and "RANK" not in os.environ:

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfs2b200.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 MAX_LAYERS, MAX_POSTNET, MAX_STAGES, MAX_RESBLOCKS, MAX_DIL = 12, 8, 8, 32, 4
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_LRELU = 0, 1, 2, 3
 CONV_AUTO, CONV_SIMT, CONV_TC = 0, 1, 2
@@ -162,6 +162,7 @@ EXPORTS = {
     "fs2_profile_end": (i32, [C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(i64)]),
     "fs2_conv1d": (i32, [C.POINTER(Conv1dArgs), fp]),
     "fs2_conv_tc_block": (i32, [i32]),
+    "fs2_conv_tc_block_f8": (i32, [i32]),
     "fs2_conv_tc_plan": (i32, [C.c_void_p, i32, C.c_void_p]),
     "fs2_layernorm": (i32, [C.POINTER(LayerNormArgs), fp]),
     "fs2_attention": (i32, [C.POINTER(AttentionArgs), fp]),

@@ -1,8 +1,7 @@
-"""Compile the CUDA sources under csrc/ into fastspeech2_b200/libfs2b200.so for sm_100a (in-tree, so it ships with gpurun).
+"""Compile the CUDA sources under csrc/ into fastspeech2_b200/libfs2b200.so for the H100 (sm_90a), next to the Python package.
 
 Each .cu is compiled to an object in parallel (build/obj/, git-ignored) and the objects are linked with nvcc --shared.
-FS2_TC_TRACE=1 in the environment compiles the per-role timeline stamps into the tcgen05 conv kernel (scripts/tc_trace.py);
-FS2_DEBUG_KNOBS=1 compiles the fs2_debug_set_* tuning knobs that scripts/tc_*.py use (the shipped library has neither).
+FS2_DEBUG_KNOBS=1 compiles the fs2_debug_set_* tuning knobs that scripts/tc_*.py use (the shipped library has none).
 """
 from __future__ import annotations
 
@@ -17,9 +16,9 @@ ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "libfs2b200.so")
 OBJ = os.path.join(ROOT, "build", "obj")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
-         "-I", os.path.join(ROOT, "include")] + (["-DFS2_TC_TRACE", "-DFS2_DEBUG_KNOBS"] if os.environ.get("FS2_TC_TRACE") == "1" else []) \
-        + (["-DFS2_DEBUG_KNOBS"] if os.environ.get("FS2_DEBUG_KNOBS") == "1" and os.environ.get("FS2_TC_TRACE") != "1" else [])
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include")] \
+        + (["-DFS2_DEBUG_KNOBS"] if os.environ.get("FS2_DEBUG_KNOBS") == "1" else [])
 
 
 def sources():
@@ -58,7 +57,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose:
             print(f"== {os.path.basename(src)}\n{r.stdout}{r.stderr}")
     objs = [os.path.join(OBJ, os.path.basename(s)[:-3] + ".o") for s in srcs]
-    r = subprocess.run([NVCC, "--shared", "-gencode", "arch=compute_100a,code=sm_100a"] + objs + ["-o", LIB], capture_output=True, text=True)
+    r = subprocess.run([NVCC, "--shared"] + ARCH + objs + ["-o", LIB], capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)
         raise RuntimeError("nvcc failed linking libfs2b200.so")

@@ -1,30 +1,28 @@
 // Fused self-attention of one FFT block on the tensor cores (transformer/Modules.py:14-25 + key mask Models.py:79, heads as
-// SubLayers.py:39-44): S = Q K^T, softmax and O = P V in ONE persistent tcgen05 kernel -- the score matrix lives in tensor memory
-// and never reaches HBM (the GEMM path of attention_tc.cu materialises S [B*H][T][Tk] in fp32: 535 MB per layer at B = 64).
+// SubLayers.py:39-44): S = Q K^T, softmax and O = P V in ONE persistent wgmma kernel -- the score matrix lives in registers and
+// never reaches HBM (the GEMM path of attention_tc.cu materialises S [B*H][T][Tk] in fp32: 535 MB per layer at B = 64).
 //
 //   work item = (utterance b, head h, 128 query rows); K and V come as the per-utterance operand tiles that pack_k/v_tiles_kernel
 //   (attention_tc.cu) write once per layer (fp16 hi/lo, three-MMA split: attention keeps fp32-class operands).
-//   pass 1: for every block of 128 keys  S = Q K_j^T (TMEM, double-buffered)  ->  row maximum (thread == query row; the two warps
-//           that share a row's halves combine through shared memory once per item).
+//   pass 1: for every block of 128 keys  S = Q K_j^T (register accumulators)  ->  row maximum (a row's columns are spread over the
+//           four lanes of a quad: two shuffles).
 //   pass 2: S again -> p = exp2(s*c - m) (keys >= key_len masked to 0) -> fp16 hi/lo operand planes in shared memory ->
-//           O += P V_j (TMEM accumulator), row sums alongside.  No rescaling of O is ever needed because the maximum is final.
+//           O += P V_j (register accumulators), row sums alongside.  No rescaling of O is ever needed because the maximum is final.
 //   epilogue: O / l -> ctx[b, t, h*128 .. +128]; query rows t >= key_len[b] are written as 0 (contract of fs2_attention).
-//   Recomputing S costs 1/3 more MMAs than a one-pass online softmax and removes the O-rescale round trips through TMEM.
+//   Recomputing S costs 1/3 more MMAs than a one-pass online softmax and removes the O rescaling.
 //
-// Roles: warp 0 streams K / V stages (cp.async.bulk), warp 1 issues the MMAs, warps 2-9 are "row" warps (TMEM lane quarter =
-// warp % 4, column half = (warp-2)/4): Q conversion, both softmax passes, the epilogue.
+// Roles: warp 8 streams K / V stages (cp.async.bulk) in the order they are consumed; warps 0-7 are two consumer warpgroups that
+// own 64 query rows each: Q conversion, the MMAs, both softmax passes and the epilogue.
 #include "conv_tc_kernel.cuh"
 
 namespace fs2 {
 
 int pack_kv_tiles(const fs2_attention_args* a, unsigned char* kt, unsigned char* vt, long long tstride, cudaStream_t s);   // attention_tc.cu
 
-constexpr int AF_THREADS = 320;
+constexpr int AF_THREADS = 288;
 constexpr int AF_SB = 8;                         // K / V stage ring depth
 constexpr uint32_t AF_STAGE = 8192;              // one stage: [hi | lo][2 chunks][128][16 B]
 constexpr float AF_WSCALE = 16.f;                // operand scale of the packed K / V tiles (attention_tc.cu::AT_WSCALE)
-
-__device__ __forceinline__ void row_warps_sync_af() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the 8 row warps only
 
 struct AfP {
   const float* qkv; float* ctx;
@@ -50,6 +48,8 @@ __device__ __forceinline__ void af_store16(unsigned char* kblk, int row, const f
   *reinterpret_cast<uint4*>(p0 + 6144) = make_uint4(lw[4], lw[5], lw[6], lw[7]);          // lo, chunk 1
 }
 
+__device__ __forceinline__ void af_wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }   // one warpgroup
+
 __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const AfP p) {
   constexpr uint32_t KBLK = 8192;                // one 16-wide K-block of an A operand: hi plane 4 KB + lo plane 4 KB (128 rows)
   constexpr uint32_t PLANES = 8 * KBLK;          // 128 x 128 operand: 64 KB
@@ -58,37 +58,19 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
   unsigned char* qa = smem_raw;                  // Q operand planes
   unsigned char* pa = qa + PLANES;               // P operand planes
   unsigned char* ring = pa + PLANES;
-  float* xch = reinterpret_cast<float*>(ring + (size_t)AF_SB * AF_STAGE);   // [2 halves][128 rows] row max, then row sums
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xch + 256);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)AF_SB * AF_STAGE);
   uint64_t* fullB = bars;                        // [AF_SB]
   uint64_t* emptyB = fullB + AF_SB;              // [AF_SB]
-  uint64_t* sFull = emptyB + AF_SB;              // [2] S buffer written
-  uint64_t* sEmpty = sFull + 2;                  // [2] S buffer read by all row warps
-  uint64_t* qReady = sEmpty + 2;                 // Q planes written (and O of the previous item drained)
-  uint64_t* pReady = qReady + 1;                 // P planes of a key block written
-  uint64_t* pFree = pReady + 1;                  // the PV MMAs that read them have retired
-  uint64_t* oFull = pFree + 1;                   // O complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(oFull + 1);
 
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < AF_SB; i++) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(&sFull[i], 1); mbar_init(&sEmpty[i], 8); }
-    mbar_init(qReady, 8); mbar_init(pReady, 8); mbar_init(pFree, 1); mbar_init(oFull, 1);
+  if (tid == 0) {
+    for (int i = 0; i < AF_SB; i++) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t s_col[2] = {0u, 128u}, o_col = 256u;
   const int nkb = p.Tk / 128;                    // key blocks
 
-  if (warp == 0) {
-    // ===================== K / V stage producer, in the order the MMA warp consumes them =====================
+  if (warp == 8) {
+    // ===================== K / V stage producer, in the order the consumers read them =====================
     if (lane == 0) {
       Ring rb;
       auto push = [&](const unsigned char* src) {
@@ -103,186 +85,160 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
         const unsigned char* vt = p.vt + (long long)bh * p.tstride + TC_HDR;   // [key/16][8 KB]
         for (int j = 0; j < nkb; j++)                                            // pass 1
           for (int kb = 0; kb < 8; kb++) push(kt + ((size_t)j * 8 + kb) * AF_STAGE);
-        for (int kb = 0; kb < 8; kb++) push(kt + (size_t)kb * AF_STAGE);         // pass 2: S(0)
-        for (int j = 0; j < nkb; j++) {
-          if (j + 1 < nkb)
-            for (int kb = 0; kb < 8; kb++) push(kt + ((size_t)(j + 1) * 8 + kb) * AF_STAGE);   // S(j+1)
-          for (int kb = 0; kb < 8; kb++) push(vt + ((size_t)j * 8 + kb) * AF_STAGE);           // P V_j
+        for (int j = 0; j < nkb; j++) {                                          // pass 2
+          for (int kb = 0; kb < 8; kb++) push(kt + ((size_t)j * 8 + kb) * AF_STAGE);   // S(j)
+          for (int kb = 0; kb < 8; kb++) push(vt + ((size_t)j * 8 + kb) * AF_STAGE);   // P V_j
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    const uint32_t idesc = umma_idesc_f16(128);
-    const uint64_t desc_c = umma_desc(0, 2048, 128);     // A and B alike: chunk stride 128 rows * 16 B, 8-row groups 128 B apart
-    const uint32_t qa16 = smem_u32(qa) >> 4, pa16 = smem_u32(pa) >> 4;
-    Ring rb;
-    uint32_t s_use[2] = {0, 0};                  // uses of each S buffer so far (phase of sEmpty / sFull)
-    uint32_t q_phase = 0, p_phase = 0, pf_phase = 0;
-    // D[tmem col] (+)= A(planes a16, 8 K-blocks) x B(next 8 ring stages), three-MMA split
-    auto gemm = [&](uint32_t a16, uint32_t dcol, bool overwrite) {
-      for (int kb = 0; kb < 8; kb++, rb.advance(AF_SB)) {
-        mbar_wait(&fullB[rb.idx], rb.phase);
-        tc_fence_after();
-        if (leader) {
-          const uint64_t a_hi = desc_c | (uint64_t)((a16 + kb * (KBLK >> 4)) & 0x3fff), a_lo = a_hi + (4096 >> 4);
-          const uint64_t b_hi = desc_c | (uint64_t)(smem_u32(ring + (size_t)rb.idx * AF_STAGE) >> 4), b_lo = b_hi + (4096 >> 4);
-          tc_mma_f16(tmem + dcol, a_lo, b_hi, idesc, (overwrite && kb == 0) ? 0u : 1u);
-          tc_mma_f16(tmem + dcol, a_hi, b_hi, idesc, 1u);
-          tc_mma_f16(tmem + dcol, a_hi, b_lo, idesc, 1u);
-          tc_commit(&emptyB[rb.idx]);
-        }
-        __syncwarp();
-      }
-    };
-    auto issue_s = [&](int j) {                  // S(j) into buffer j & 1
-      const int sb = j & 1;
-      if (s_use[sb] > 0) mbar_wait(&sEmpty[sb], (s_use[sb] - 1) & 1);      // the previous contents have been read
-      tc_fence_after();
-      gemm(qa16, s_col[sb], true);
-      if (leader) tc_commit(&sFull[sb]);
-      __syncwarp();
-      s_use[sb]++;
-    };
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-      mbar_wait(qReady, q_phase); q_phase ^= 1;
-      tc_fence_after();
-      for (int j = 0; j < nkb; j++) issue_s(j);                             // pass 1
-      issue_s(0);                                                           // pass 2
-      for (int j = 0; j < nkb; j++) {
-        if (j + 1 < nkb) issue_s(j + 1);
-        mbar_wait(pReady, p_phase); p_phase ^= 1;
-        tc_fence_after();
-        gemm(pa16, o_col, j == 0);
-        if (leader) { tc_commit(pFree); if (j == nkb - 1) tc_commit(oFull); }
-        __syncwarp();
-      }
-      (void)pf_phase;
+    return;
+  }
+  // ===================== consumer warpgroups =====================
+  const int g = warp >> 2, w = warp & 3;
+  const int D = p.H * 128;
+  const float c = p.scale * (1.f / AF_WSCALE) * 1.4426950408889634f;      // s*c = scaled score in log2 units (K tiles carry x16)
+  const uint64_t desc_c = wgmma_desc(0, 2048, 128);    // A and B alike: chunk stride 128 rows * 16 B, 8-row groups 128 B apart
+  const uint32_t qa16 = (smem_u32(qa) >> 4) + 64 * g, pa16 = (smem_u32(pa) >> 4) + 64 * g;
+  Ring rb;
+  // D (+)= A(planes a16, 8 K-blocks) x B(next 8 ring stages), three-MMA split; stages are released one MMA group late
+  auto gemm = [&](uint32_t a16, float (&d)[64]) {
+    int pend = -1;
+    for (int kb = 0; kb < 8; kb++, rb.advance(AF_SB)) {
+      mbar_wait(&fullB[rb.idx], rb.phase);
+      wgmma_fence();
+      const uint64_t a_hi = desc_c | (uint64_t)((a16 + kb * (KBLK >> 4)) & 0x3fff), a_lo = a_hi + (4096 >> 4);
+      const uint64_t b_hi = desc_c | (uint64_t)(smem_u32(ring + (size_t)rb.idx * AF_STAGE) >> 4), b_lo = b_hi + (4096 >> 4);
+      Wgmma<128>::f16(d, a_lo, b_hi, kb == 0 ? 0u : 1u);
+      Wgmma<128>::f16(d, a_hi, b_hi, 1u);
+      Wgmma<128>::f16(d, a_hi, b_lo, 1u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (pend >= 0) tc_release(&emptyB[pend]);
+      pend = (int)rb.idx;
     }
-  } else {
-    // ===================== row warps =====================
-    const int q = warp & 3, h = (warp - 2) >> 2;
-    const int r128 = q * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    const int D = p.H * 128;
-    const float c = p.scale * (1.f / AF_WSCALE) * 1.4426950408889634f;      // s*c = scaled score in log2 units (K tiles carry x16)
-    uint32_t s_phase[2] = {0, 0}, pf_phase = 0, o_phase = 0;
-    bool p_written = false;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-      const int bh = item / p.qtiles, qt = item - bh * p.qtiles;
-      const int b = bh / p.H, hd = bh - b * p.H;
-      const int t = qt * 128 + r128;
-      const int len = p.key_lens ? min(p.key_lens[b], p.T) : p.T;
-      // ---- Q rows -> operand planes (this warp: d columns 64h .. 64h+63 = K-blocks 4h .. 4h+3)
-      {
-        const float* src = p.qkv + ((long long)b * p.T + t) * 3 * D + hd * 128 + h * 64;
+    wgmma_wait<0>();
+    wgmma_keep<128>(d);
+    tc_release(&emptyB[pend]);
+  };
+  const int qr = (tid & 127) >> 1, qhalf = tid & 1;    // Q conversion: row, 64-column half
+  for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+    const int bh = item / p.qtiles, qt = item - bh * p.qtiles;
+    const int b = bh / p.H, hd = bh - b * p.H;
+    const int len = p.key_lens ? min(p.key_lens[b], p.T) : p.T;
+    // ---- Q rows of this warpgroup -> operand planes (the previous item's MMAs have all retired)
+    {
+      const int t = qt * 128 + 64 * g + qr;
+      const float* src = p.qkv + ((long long)b * p.T + t) * 3 * D + hd * 128 + qhalf * 64;
 #pragma unroll
-        for (int g = 0; g < 4; g++) {
-          float v[16];
-          if (t < p.T) {
-#pragma unroll
-            for (int k4 = 0; k4 < 4; k4++) {
-              const float4 u = __ldg(reinterpret_cast<const float4*>(src + g * 16) + k4);
-              v[4 * k4] = u.x; v[4 * k4 + 1] = u.y; v[4 * k4 + 2] = u.z; v[4 * k4 + 3] = u.w;
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < 16; k++) v[k] = 0.f;
-          }
-          af_store16(qa + (size_t)(h * 4 + g) * KBLK, r128, v);
-        }
-        fence_proxy_async();
-        tc_fence_before();                         // (also orders the previous item's O reads before the next O overwrite)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(qReady);
-      }
-      // ---- pass 1: row maximum of the masked, scaled scores over this warp's key halves
-      float m = -INFINITY;
-      for (int j = 0; j < nkb; j++) {
-        const int sb = j & 1;
-        mbar_wait(&sFull[sb], s_phase[sb]); s_phase[sb] ^= 1;
-        tc_fence_after();
-#pragma unroll
-        for (int g = 0; g < 2; g++) {
-          uint32_t sv[32];
-          tc_ld32(tmem + lane_base + s_col[sb] + h * 64 + g * 32, sv);
-          const int key0 = j * 128 + h * 64 + g * 32;
-#pragma unroll
-          for (int k = 0; k < 32; k++)
-            if (key0 + k < len) m = fmaxf(m, __uint_as_float(sv[k]) * c);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sEmpty[sb]);
-      }
-      xch[h * 128 + r128] = m;
-      row_warps_sync_af();
-      m = fmaxf(xch[r128], xch[128 + r128]);
-      row_warps_sync_af();                          // xch is reused for the row sums
-      // ---- pass 2: p = exp2(s*c - m) -> P operand planes (this warp: keys 64h .. 64h+63 of the block = K-blocks 4h .. 4h+3)
-      float l = 0.f;
-      for (int j = 0; j < nkb; j++) {
-        const int sb = j & 1;
-        mbar_wait(&sFull[sb], s_phase[sb]); s_phase[sb] ^= 1;
-        tc_fence_after();
-        if (p_written) { mbar_wait(pFree, pf_phase); pf_phase ^= 1; }      // the previous block's PV MMAs have read the planes
-#pragma unroll
-        for (int g = 0; g < 2; g++) {
-          uint32_t sv[32];
-          tc_ld32(tmem + lane_base + s_col[sb] + h * 64 + g * 32, sv);
-          const int key0 = j * 128 + h * 64 + g * 32;
-#pragma unroll
-          for (int half = 0; half < 2; half++) {
-            float pv[16];
-#pragma unroll
-            for (int k = 0; k < 16; k++) {
-              const float e = key0 + half * 16 + k < len ? exp2f(fmaf(__uint_as_float(sv[half * 16 + k]), c, -m)) : 0.f;
-              pv[k] = e;
-              l += e;
-            }
-            af_store16(pa + (size_t)(h * 4 + g * 2 + half) * KBLK, r128, pv);
-          }
-        }
-        tc_fence_before();
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) { mbar_arrive(&sEmpty[sb]); mbar_arrive(pReady); }
-        p_written = true;
-      }
-      xch[h * 128 + r128] = l;
-      row_warps_sync_af();
-      l = xch[r128] + xch[128 + r128];
-      // ---- epilogue: O / l (V tiles carry x16), rows beyond the utterance are zero
-      mbar_wait(oFull, o_phase); o_phase ^= 1;
-      tc_fence_after();
-      const float inv = (t < len) ? (1.f / AF_WSCALE) / l : 0.f;
-      float* dst = p.ctx + ((long long)b * p.T + t) * D + hd * 128 + h * 64;
-#pragma unroll
-      for (int g = 0; g < 2; g++) {
-        uint32_t ov[32];
-        tc_ld32(tmem + lane_base + o_col + h * 64 + g * 32, ov);
+      for (int k = 0; k < 4; k++) {
+        float v[16];
         if (t < p.T) {
 #pragma unroll
-          for (int k4 = 0; k4 < 8; k4++)
-            reinterpret_cast<float4*>(dst + g * 32)[k4] = make_float4(__uint_as_float(ov[4 * k4]) * inv, __uint_as_float(ov[4 * k4 + 1]) * inv,
-                                                                      __uint_as_float(ov[4 * k4 + 2]) * inv, __uint_as_float(ov[4 * k4 + 3]) * inv);
+          for (int k4 = 0; k4 < 4; k4++) {
+            const float4 u = __ldg(reinterpret_cast<const float4*>(src + k * 16) + k4);
+            v[4 * k4] = u.x; v[4 * k4 + 1] = u.y; v[4 * k4 + 2] = u.z; v[4 * k4 + 3] = u.w;
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 16; i++) v[i] = 0.f;
+        }
+        af_store16(qa + (size_t)(qhalf * 4 + k) * KBLK, 64 * g + qr, v);
+      }
+      fence_proxy_async();
+      af_wg_sync(g);
+    }
+    float sacc[64];
+    // ---- pass 1: row maxima of the masked, scaled scores (rows lane/4 and lane/4 + 8 of this warp's 16)
+    float m[2] = {-INFINITY, -INFINITY};
+    for (int j = 0; j < nkb; j++) {
+      gemm(qa16, sacc);
+#pragma unroll
+      for (int jj = 0; jj < 16; jj++)
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const int key = j * 128 + 8 * jj + 2 * (lane & 3) + e;
+          if (key < len) {
+            m[0] = fmaxf(m[0], sacc[4 * jj + e] * c);
+            m[1] = fmaxf(m[1], sacc[4 * jj + 2 + e] * c);
+          }
+        }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
+      m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
+    }
+    // ---- pass 2: p = exp2(s*c - m) -> P operand planes -> O += P V_j
+    float oacc[64];
+    float l[2] = {0.f, 0.f};
+    const int prow = 64 * g + 16 * w + (lane >> 2);
+    for (int j = 0; j < nkb; j++) {
+      gemm(qa16, sacc);
+#pragma unroll
+      for (int jj = 0; jj < 16; jj++) {
+        const int k0 = 8 * jj + 2 * (lane & 3);          // key inside the block
+        unsigned char* base = pa + (size_t)(k0 >> 4) * KBLK + ((k0 >> 3) & 1) * 2048 + (k0 & 7) * 2;
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          float e[2];
+#pragma unroll
+          for (int q = 0; q < 2; q++) {
+            e[q] = j * 128 + k0 + q < len ? exp2f(fmaf(sacc[4 * jj + 2 * h + q], c, -m[h])) : 0.f;
+            l[h] += e[q];
+          }
+          const uint32_t hw = cvt_f16x2_sat(e[0], e[1]);
+          const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw));
+          const uint32_t lw = cvt_f16x2_sat(e[0] - hf.x, e[1] - hf.y);
+          unsigned char* rowp = base + (size_t)(prow + 8 * h) * 16;
+          *reinterpret_cast<uint32_t*>(rowp) = hw;
+          *reinterpret_cast<uint32_t*>(rowp + 4096) = lw;
         }
       }
-      row_warps_sync_af();                          // xch free for the next item
+      fence_proxy_async();
+      af_wg_sync(g);                                   // every thread's P values are in place before the warpgroup's MMAs read them
+      if (j == 0) {
+#pragma unroll
+        for (int i = 0; i < 64; i++) oacc[i] = 0.f;
+      }
+      {
+        // O += P V_j: the first K-block of the first key block overwrites (gemm's kb == 0), later key blocks accumulate
+        int pend = -1;
+        for (int kb = 0; kb < 8; kb++, rb.advance(AF_SB)) {
+          mbar_wait(&fullB[rb.idx], rb.phase);
+          wgmma_fence();
+          const uint64_t a_hi = desc_c | (uint64_t)((pa16 + kb * (KBLK >> 4)) & 0x3fff), a_lo = a_hi + (4096 >> 4);
+          const uint64_t b_hi = desc_c | (uint64_t)(smem_u32(ring + (size_t)rb.idx * AF_STAGE) >> 4), b_lo = b_hi + (4096 >> 4);
+          Wgmma<128>::f16(oacc, a_lo, b_hi, 1u);
+          Wgmma<128>::f16(oacc, a_hi, b_hi, 1u);
+          Wgmma<128>::f16(oacc, a_hi, b_lo, 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (pend >= 0) tc_release(&emptyB[pend]);
+          pend = (int)rb.idx;
+        }
+        wgmma_wait<0>();
+        wgmma_keep<128>(oacc);
+        tc_release(&emptyB[pend]);
+      }
+      af_wg_sync(g);                                   // the P planes are rewritten by the next key block
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
+    // ---- epilogue: O / l (V tiles carry x16), rows beyond the utterance are zero
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+      const int t = qt * 128 + prow + 8 * h;
+      if (t >= p.T) continue;
+      const float inv = t < len ? (1.f / AF_WSCALE) / l[h] : 0.f;
+      float* dst = p.ctx + ((long long)b * p.T + t) * D + hd * 128 + 2 * (lane & 3);
+#pragma unroll
+      for (int jj = 0; jj < 16; jj++)
+        *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(oacc[4 * jj + 2 * h] * inv, oacc[4 * jj + 2 * h + 1] * inv);
+    }
   }
 }
 
-static constexpr size_t AF_SMEM = 2 * 65536 + (size_t)AF_SB * AF_STAGE + 256 * 4 + (2 * AF_SB + 10) * 8 + 16;
+static constexpr size_t AF_SMEM = 2 * 65536 + (size_t)AF_SB * AF_STAGE + 2 * AF_SB * 8 + 16;
 
 static inline long long af_tile_stride(int Tk) { return TC_HDR + (long long)Tk * 512; }
 

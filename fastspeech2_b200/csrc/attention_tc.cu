@@ -1,5 +1,5 @@
 // Self-attention of the decoder FFT blocks on the tensor cores (transformer/Modules.py:14-25, key mask Models.py:79),
-// built from the split-FP16 tcgen05 GEMM engine in conv_tc.cu:
+// built from the split-FP16 tensor-core GEMM engine in conv_tc.cu:
 //
 //   1. pack_kv_tiles : per (utterance, head) re-tile K and V (fp32, inside the packed qkv rows) into the GEMM's weight-tile
 //                      image (fp16 hi/lo, 128-byte header) -- K as the [d x keys] operand of S = Q K^T, V as the [keys x d]
@@ -10,8 +10,8 @@
 //                      following LayerNorm, transformer/Layers.py:25).
 //   4. O = P V        : conv_tc GEMM with C_in = Tk keys, written straight into the head's 128 columns of ctx [B][T][D].
 //
-// The score matrix is materialised once in fp32 (the reference writes it four times); a fused flash-style tcgen05 kernel
-// that keeps S in TMEM is the planned replacement.  The exact fp32 kernel (attention_simt.cu) stays in use for the encoder.
+// The score matrix is materialised once in fp32 (the reference writes it four times); the fused kernel (attention_fused.cu)
+// keeps S in registers instead.  The exact fp32 kernel (attention_simt.cu) stays in use for the encoder.
 #include <cuda_fp16.h>
 
 #include "common.cuh"

@@ -2,7 +2,7 @@
 //
 // This is the exact-precision path (plain fp32 FMA, fp32 accumulate): it serves every layer upstream of the
 // discrete duration / pitch-bucket decisions, where the parity budget is ~1e-6 (SURVEY.md section 7, hard part 2),
-// and is the fallback for shapes the tcgen05 path does not take.  One kernel covers nn.Linear (taps = 1),
+// and is the fallback for shapes the tensor-core path does not take.  One kernel covers nn.Linear (taps = 1),
 // nn.Conv1d with dilation, and a phase group of ConvTranspose1d (see fs2b200.h).
 //
 // Tiling: CTA = 128 (or 64, for small problems) rows (time) x BN output channels, BK = 16, 256 threads, TM x TN register tile per thread,
@@ -206,9 +206,13 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   p.alpha = a->alpha; p.accumulate = a->accumulate;
   p.row_lens = a->row_lens;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
+  int derr = FS2_OK;
+  DevState* dv = dev_state(&derr);                      // SM count of the current device
+  if (!dv) return derr;
+  const long long num_sms = dv->num_sms.load(std::memory_order_relaxed);
   // 128-row tiles by default; 64-row tiles when the grid would not even give every SM two CTAs (encoder / predictors: 2048 rows)
   const int nblk = a->N > 64 ? (a->N + 127) / 128 : 1;
-  const bool small = (long long)((a->T + 127) / 128) * a->B * nblk < 2LL * 148;
+  const bool small = (long long)((a->T + 127) / 128) * a->B * nblk < 2LL * num_sms;
   const int bm = small ? 64 : 128;
   p.tiles_per_batch = (a->T + bm - 1) / bm;
   const long long gx = (long long)p.tiles_per_batch * a->B;
@@ -224,8 +228,8 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
 #define FS2_SIMT_LAUNCH(BN_, grid_)                   \
   if (small) { FS2_SIMT_ACT(64, BN_, grid_) } else { FS2_SIMT_ACT(128, BN_, grid_) }
   // narrow outputs on small problems (FFN w_2, predictor convs: 2048 rows x 256 channels): 64-column CTAs double the CTA count
-  // (64 -> 128 on 148 SMs)
-  const bool narrow_small = small && a->N > 64 && (long long)gx * ((a->N + 127) / 128) < 148;
+  // while the 128-column grid leaves SMs idle
+  const bool narrow_small = small && a->N > 64 && (long long)gx * ((a->N + 127) / 128) < num_sms;
   if (a->N > 64 && !narrow_small) {
     dim3 grid((unsigned)gx, (a->N + 127) / 128);
     FS2_SIMT_LAUNCH(128, grid)

@@ -1,94 +1,71 @@
-// Host side of the tcgen05 implicit-GEMM Conv1d: shape support, work-item / ring heuristics, launch.
-// Device code: conv_tc_kernel.cuh (instantiated in conv_tc_mt{1,2,4}.cu).
+// Host side of the wgmma implicit-GEMM Conv1d: shape support, work-item / ring heuristics, launch.
+// Device code: conv_tc_kernel.cuh (instantiated in conv_tc_nb*.cu).
 #include "conv_tc_kernel.cuh"
 
 namespace fs2 {
 
 // ------------------------------------------------------------------ host side
-#ifdef FS2_DEBUG_KNOBS
-long long* g_tc_trace = nullptr;  // debug: set through fs2_debug_set_tc_trace (per-item role timeline)
-#else
-static constexpr long long* g_tc_trace = nullptr;
-#endif
-
-static int pow2_cols(int c) {
-  int v = 32;
-  while (v < c) v <<= 1;
-  return v;
-}
-
-int conv_tc_nb(int N) {  // output channels per work item: NB <= 128 keeps two accumulator sets of MT=2 tiles inside TMEM
+// Output channels per work item: NB <= 128 keeps a consumer thread's accumulators at <= 64 registers.  The f8 split asks for
+// nb_max = 64: Hopper accumulates E4M3 products with reduced precision, so its correction term needs an accumulator of its own.
+int conv_tc_nb(int N, int nb_max) {
   if (N % 16) return 0;
-  if (N <= 128) return N;
-  for (int nb = 128; nb >= 16; nb -= 16)
+  if (N <= nb_max) return N;
+  for (int nb = nb_max; nb >= 16; nb -= 16)
     if (N % nb == 0) return nb;
   return 0;
 }
 
 bool conv_tc_supported(const fs2_conv1d_args* a) {
-  if (!a || a->Cin % TC_KB || a->N % 16 || conv_tc_nb(a->N) == 0) return false;
+  if (!a || a->Cin % TC_KB || a->N % 16 || conv_tc_nb(a->N, 128) == 0) return false;
   if ((a->x_row_stride & 7) || (a->x_batch_stride & 7) || (reinterpret_cast<uintptr_t>(a->x) & 31u)) return false;   // 256-bit loads
   if ((a->y_row_stride & 3) || (a->y_batch_stride & 3)) return false;
   if ((long long)(TC_LD * TC_TTHREADS) * a->x_row_stride > 0x7fffffffLL) return false;                                // 32-bit row offsets
   if (a->res && ((a->res_row_stride & 3) || (a->res_batch_stride & 3))) return false;
   if (a->in_act != FS2_ACT_NONE && a->in_act != FS2_ACT_LRELU) return false;
   if (a->in_act == FS2_ACT_LRELU && !(a->in_slope >= 0.f && a->in_slope <= 1.f)) return false;   // max(x, slope*x) form
-  if ((a->taps - 1) * a->dilation > TC_LD * TC_TTHREADS / TC_CHUNKS - 128) return false;
+  if ((a->taps - 1) * a->dilation > TC_LD * TC_TTHREADS / TC_CHUNKS - 128) return false;   // slab rows the transform warps hold
   return true;
 }
 
 #ifdef FS2_DEBUG_KNOBS
-int g_tc_pdl = 0;                  // programmatic dependent launch: 0 = off (default), 1 = short launches only, 2 = every launch.
-                                   // Measured with the three modes interleaved step by step (scripts/pdl_ab.py,
-                                   // profiles/r01_pdl_ab.txt): no gain on either forward (39.5 / 40.8 / 42.2 ms per step), so it
-                                   // stays off; debug switch fs2_debug_set_tc_pdl
+int g_tc_pdl = 0;                  // programmatic dependent launch: 0 = off (default), 1 = short launches only, 2 = every launch;
+                                   // debug switch fs2_debug_set_tc_pdl
 int g_tc_tune[4] = {0, 0, 0, 0};   // debug overrides: SA, SB, TPS, grid (0 = heuristic); set through fs2_debug_set_tc_tuning
 #else                              // shipped build: no mutable process-wide state
 static constexpr int g_tc_pdl = 0;
 static constexpr int g_tc_tune[4] = {0, 0, 0, 0};
 #endif
 
-// Shape-derived launch plan (pure host logic, no CUDA calls): work-item shape, accumulator grouping, ring depths, shared /
-// tensor memory budget, grid.  Returns FS2_OK or FS2_ERR_UNSUPPORTED.  Exposed as fs2_conv_tc_plan so that the heuristics'
-// invariants are testable without a GPU (tests/test_abi.py).
+// Shape-derived launch plan (pure host logic, no CUDA calls): work-item shape, accumulator grouping, ring depths, shared-memory
+// budget, grid.  Returns FS2_OK or FS2_ERR_UNSUPPORTED.  Exposed as fs2_conv_tc_plan so that the heuristics' invariants are
+// testable without a GPU (tests/test_abi.py).
 static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& smem, int& grid) {
   const bool nb64 = (a->tc_variant & FS2_TC_VARIANT_NB64) != 0;   // 64-channel work items: separate accumulators for hi*hi and the cross terms
-  p.NB = nb64 ? (a->N % 64 == 0 ? 64 : (a->N < 64 && a->N % 16 == 0 ? a->N : 0)) : conv_tc_nb(a->N);
+  const bool f8 = (a->tc_variant & FS2_TC_VARIANT_F8) != 0;
+  p.NB = nb64 ? (a->N % 64 == 0 ? 64 : (a->N < 64 && a->N % 16 == 0 ? a->N : 0)) : conv_tc_nb(a->N, f8 ? 64 : 128);
   if (p.NB == 0) return FS2_ERR_UNSUPPORTED;
-  p.acc_stride = (p.NB + 31) & ~31;
   const int halo = (a->taps - 1) * a->dilation;
-  const int tiles128 = (a->T + 127) / 128;
-  int mt = 2;                                          // two accumulator sets of MT tiles: 2*MT*TG*acc_stride <= 512 columns
-  if (p.acc_stride <= 64 && tiles128 >= 4 && 4 * 128 + halo <= 5 * TC_TTHREADS / TC_CHUNKS) mt = 4;   // narrow layers: amortise per-item handshakes
-  if (g_tc_tune[3] == -1) mt = 2;                      // debug: force MT = 2
-  if (nb64 && mt > 2) mt = 2;                          // keeps TG = 2 (two accumulator sets of MT*2 tiles of 64 columns = 512)
-  if (mt > tiles128) mt = tiles128 >= 2 ? 2 : 1;
-  if (mt == 2 && mt * 128 + halo > TC_LD * TC_TTHREADS / TC_CHUNKS) mt = 1;   // rows one register-ring slot can hold
-  // small problems (decoder projections, attention PV): prefer more, smaller work items when MT = 2 would leave SMs idle
-  if (mt == 2 && 2LL * (a->N / p.NB) * a->B * ((a->T + 255) / 256) <= num_sms) mt = 1;   // measured: helps at <= 1/2 wave, hurts K-heavy layers at ~1 wave
-  int R = mt * 128 + halo;
+  // One 128-row tile per work item, split between the two consumer warpgroups.  Narrow blocks (NB <= 64): hi*hi and the two cross
+  // terms accumulate in separate register sets (summed in fp32 round-to-nearest by the epilogue) at the same register cost as NB = 128.
+  int R = 128 + halo;
   R += (12 - (R & 7)) & 7;                             // R % 8 == 4: conflict-free transform stores (2 chunks per row)
-  p.MT = mt; p.R = R;
-  // narrow layers: hi*hi and the two cross terms accumulate in separate TMEM tiles (summed in fp32 round-to-nearest by the
-  // epilogue) while two accumulator sets still fit in 512 columns
-  p.TG = (mt == 4 ? p.acc_stride <= 32 : p.acc_stride <= 64) ? 2 : 1;
-  const size_t fixed = 4 * TC_STAGE_FLOATS * sizeof(float) + (2 * TC_SA_MAX + 2 * TC_SB_MAX + 4) * 8 + 16;
+  if (R > TC_LD * TC_TTHREADS / TC_CHUNKS + 7) return FS2_ERR_UNSUPPORTED;
+  p.MT = 1; p.R = R;
+  p.TG = p.NB <= 64 ? 2 : 1;
+  const size_t fixed = (2 * TC_SA_MAX + 2 * TC_SB_MAX) * 8 + 16;
   const size_t tap_bytes = (size_t)2 * TC_CHUNKS * p.NB * 16;
-  // Taps per weight stage: measured (scripts/tc_tune.py, profiles/r01_tc_tune.txt) -- grouping 4 taps per bulk copy / handshake
-  // is 10-25 % faster for the k = 5..11 layers at every channel width; k <= 3 layers are best with one tap per stage.
-  int tps = a->taps >= 5 ? 4 : 1;
+  int tps = a->taps >= 5 ? 4 : 1;                      // taps per weight stage: wide kernels share one bulk copy / handshake
   if (g_tc_tune[2] > 0) tps = g_tc_tune[2];
   if (tps > a->taps) tps = a->taps;
   p.TPS = tps;
   const size_t a_stage = (size_t)2 * TC_CHUNKS * R * 16, b_stage = (size_t)tps * tap_bytes;
   const size_t budget = 226 * 1024;
   const int kblocks = a->Cin / TC_KB;
-  // Slab ring depth, measured per shape class (scripts/tc_tune_sa.py, profiles/r01_tc_tune_sa.txt): the ring spans work items, so
-  // even 2-K-block layers want 3 stages (-10..-14 % on the 32-channel stage against 2); k <= 3 layers like 5 (-4..-6 %); a
-  // 4th MT=4 stage is not worth shrinking the weight ring for.
+  // Slab ring depth: the ring spans work items, so even 2-K-block layers want 3 stages; short kernels have the least MMA work per
+  // slab and the deepest ring.
   int sa = 3, sb = tps > 1 ? 4 : TC_SB_MAX;
-  if (mt < 4 && a->taps <= 3) sa = 5;
-  else if (mt < 4 && kblocks >= 4) sa = 4;
+  if (a->taps <= 3) sa = 5;
+  else if (kblocks >= 4) sa = 4;
   while (fixed + sa * a_stage + sb * b_stage > budget && sa > 3) sa--;
   while (fixed + sa * a_stage + sb * b_stage > budget && sb > 3) sb--;
   while (fixed + sa * a_stage + sb * b_stage > budget && sa > 2) sa--;
@@ -99,8 +76,7 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
   if (fixed + sa * a_stage + sb * b_stage > budget) return FS2_ERR_UNSUPPORTED;
   p.SA = sa; p.SB = sb;
   smem = fixed + sa * a_stage + sb * b_stage;
-  p.tmem_cols = pow2_cols(2 * mt * p.TG * p.acc_stride);
-  p.tiles_per_batch = (a->T + mt * 128 - 1) / (mt * 128);
+  p.tiles_per_batch = (a->T + 127) / 128;
   const long long n_items = (long long)(a->N / p.NB) * a->B * p.tiles_per_batch;
   if (n_items > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   p.n_items = (int)n_items;
@@ -110,7 +86,7 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
   return FS2_OK;
 }
 
-// out[12] = {NB, MT, TG, SA, SB, TPS, R, tmem_cols, tiles_per_batch, n_items, grid, dynamic smem bytes}
+// out[12] = {NB, MT, TG, SA, SB, TPS, R, accumulator registers per consumer thread, tiles_per_batch, n_items, grid, dynamic smem bytes}
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out) {
   if (!a || !out || num_sms <= 0 || a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
@@ -119,7 +95,7 @@ int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out) {
   int grid = 0;
   const int rc = conv_tc_plan(a, num_sms, p, smem, grid);
   if (rc != FS2_OK) return rc;
-  const int v[12] = {p.NB, p.MT, p.TG, p.SA, p.SB, p.TPS, p.R, p.tmem_cols, p.tiles_per_batch, p.n_items, grid, (int)smem};
+  const int v[12] = {p.NB, p.MT, p.TG, p.SA, p.SB, p.TPS, p.R, p.TG * p.NB / 2, p.tiles_per_batch, p.n_items, grid, (int)smem};
   for (int i = 0; i < 12; i++) out[i] = v[i];
   return FS2_OK;
 }
@@ -149,9 +125,10 @@ int conv1d_tc(const fs2_conv1d_args* a, const float* wt, unsigned variant, cudaS
     DevOnce once;
     if (!dv->conv_tc_ready.load(std::memory_order_relaxed)) {
       const int mx = 227 * 1024;
-      cudaError_t e = conv_tc_prepare_mt1(mx);
-      if (e == cudaSuccess) e = conv_tc_prepare_mt2(mx);
-      if (e == cudaSuccess) e = conv_tc_prepare_mt4(mx);
+      cudaError_t e = cudaSuccess;
+      for (cudaError_t (*prep)(int) : {conv_tc_prepare_nb16, conv_tc_prepare_nb32, conv_tc_prepare_nb48, conv_tc_prepare_nb64,
+                                       conv_tc_prepare_nb80, conv_tc_prepare_nb96, conv_tc_prepare_nb112, conv_tc_prepare_nb128})
+        if (e == cudaSuccess) e = prep(mx);
       if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
       dv->conv_tc_ready.store(true, std::memory_order_release);
     }
@@ -167,18 +144,23 @@ int conv1d_tc(const fs2_conv1d_args* a, const float* wt, unsigned variant, cudaS
   p.res = a->res; p.rbs = a->res_batch_stride; p.rrs = a->res_row_stride;
   p.alpha = a->alpha; p.accumulate = a->accumulate; p.row_lens = a->row_lens;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
-  p.trace = g_tc_trace;
   p.variant = variant;
   p.f8 = (variant & FS2_TC_VARIANT_F8) ? 1 : 0;
   size_t smem = 0;
   int grid = 0;
   const int rc = conv_tc_plan(plan_args, g_num_sms, p, smem, grid);
   if (rc != FS2_OK) return rc;
-  const int mt = p.MT;
   prof_before(s);
-  if (mt == 4) conv_tc_launch_mt4(p, (unsigned)grid, smem, s);
-  else if (mt == 2) conv_tc_launch_mt2(p, (unsigned)grid, smem, s);
-  else conv_tc_launch_mt1(p, (unsigned)grid, smem, s);
+  switch (p.NB) {
+    case 16: conv_tc_launch_nb16(p, (unsigned)grid, smem, s); break;
+    case 32: conv_tc_launch_nb32(p, (unsigned)grid, smem, s); break;
+    case 48: conv_tc_launch_nb48(p, (unsigned)grid, smem, s); break;
+    case 64: conv_tc_launch_nb64(p, (unsigned)grid, smem, s); break;
+    case 80: conv_tc_launch_nb80(p, (unsigned)grid, smem, s); break;
+    case 96: conv_tc_launch_nb96(p, (unsigned)grid, smem, s); break;
+    case 112: conv_tc_launch_nb112(p, (unsigned)grid, smem, s); break;
+    default: conv_tc_launch_nb128(p, (unsigned)grid, smem, s); break;
+  }
   prof_after(s, 0, 2.0 * a->B * a->T * (double)a->Cin * a->taps * a->N);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

@@ -62,10 +62,9 @@ size_t attention_gemm_workspace(int B, int T, int H);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
-int conv_tc_nb(int N);
+int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out);
 #ifdef FS2_DEBUG_KNOBS
-extern long long* g_tc_trace;
 extern int g_tc_tune[4];
 extern int g_tc_pdl;
 #endif
@@ -133,7 +132,7 @@ static int ln(cudaStream_t s, const float* x, float* y, int B, int T, int C, con
 // input channels is cut into (tap, 256-channel) slices; each slice is one work unit of 16 K-steps with separate accumulators for
 // the hi*hi term and the cross terms (FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED, one launch per conv), and the slices are added in
 // fp32 round-to-nearest by the epilogue's accumulate path.  That bounds the tensor core's truncating accumulation to 16 steps per chain (a single k = 9 launch has 432) and
-// brings the error back to the fp32 CUDA-core kernel's level (profiles/r02/flip_census_*.jsonl).  `w_seg`: taps * (Cin/256) tile
+// brings the error back to the fp32 CUDA-core kernel's level (scripts/flip_census.py).  `w_seg`: taps * (Cin/256) tile
 // buffers of 128 + 1024*N bytes (packing.pack_conv_tc_segments).  y = bias + sum_slices + res, rows >= row_lens zeroed; no output
 // activation (a following ReLU is applied by the consumer: in_act of the next conv / pre_relu of the LayerNorm).
 static int conv_seg(cudaStream_t s, const float* x, int B, int T, int Cin, const float* w_seg, const float* bias, int N, int taps, int pad,
@@ -185,7 +184,7 @@ static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_
   at.scale = 1.0f / sqrtf((float)(D / m->n_head));
   if (tc && f.att_ws && (m->tc_mask & FS2_TC_ATTENTION_GEMM) && attention_gemm_usable(B, T, m->n_head)) {
     FS2_TRY(attention_gemm(&at, f.att_ws, f.att_bytes, s));          // round-1 path: S materialised, two GEMM launches per head
-  } else if (tc && f.att_ws && T >= 128) {                            // one fused tcgen05 kernel: S stays in tensor memory, any length
+  } else if (tc && f.att_ws && T >= 128) {                            // one fused tensor-core kernel: S stays in registers, any length
     FS2_TRY(attention_fused(&at, f.att_ws, f.att_bytes, s));
   } else {
     FS2_TRY(attention_simt(&at, s));
@@ -453,8 +452,9 @@ using namespace fs2;
 
 extern "C" {
 
-int fs2_abi_version(void) { return 8; }
-int fs2_conv_tc_block(int N) { return conv_tc_nb(N); }
+int fs2_abi_version(void) { return 9; }
+int fs2_conv_tc_block(int N) { return conv_tc_nb(N, 128); }
+int fs2_conv_tc_block_f8(int N) { return conv_tc_nb(N, 64); }
 int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_tc_plan_query(a, num_sms, out); }
 int64_t fs2_kernel_launch_count(void) { return (int64_t)g_launch_count.load(); }
 size_t fs2_struct_size(int which) {
@@ -481,7 +481,6 @@ size_t fs2_struct_size(int which) {
 #ifdef FS2_DEBUG_KNOBS
 /* tuning / tracing knobs for scripts/tc_*.py -- compiled in only with -DFS2_DEBUG_KNOBS (FS2_DEBUG_KNOBS=1 python -m fastspeech2_b200.build):
  * the shipped library has no mutable process-wide state behind the ABI */
-void fs2_debug_set_tc_trace(long long* buf) { g_tc_trace = buf; }
 void fs2_debug_set_tc_pdl(int on) { g_tc_pdl = on; }
 void fs2_debug_set_tc_tuning(int sa, int sb, int tps, int grid) { g_tc_tune[0] = sa; g_tc_tune[1] = sb; g_tc_tune[2] = tps; g_tc_tune[3] = grid; }
 #endif
@@ -507,7 +506,7 @@ int fs2_profile_end(double* ms, double* flops, int64_t* launches) {
   g_prof.clear();
   return rc;
 }
-const char* fs2_build_info(void) { return "fs2b200 sm_100a (tcgen05 split-FP16 conv + attention GEMMs, fp32 CUDA-core kernels), built " __DATE__ " " __TIME__; }
+const char* fs2_build_info(void) { return "fs2b200 sm_90a (wgmma split-FP16 conv + attention, fp32 CUDA-core kernels), built " __DATE__ " " __TIME__; }
 
 int fs2_conv1d(const fs2_conv1d_args* a, fs2_stream_t st) { return conv1d_dispatch(a, S(st)); }
 int fs2_layernorm(const fs2_layernorm_args* a, fs2_stream_t st) { return layernorm(a, S(st)); }

@@ -1,4 +1,4 @@
-"""Make the reference's `import model` / `import hifigan` resolve to the B200-native drop-ins.
+"""Make the reference's `import model` / `import hifigan` resolve to the H100-native drop-ins.
 
     import fastspeech2_b200.dropin as dropin; dropin.install()           # programmatic
     python -m fastspeech2_b200.dropin synthesize.py --text ... -p ... -m ... -t ...   # run the untouched reference CLI
@@ -36,7 +36,7 @@ def vocoder_infer(mels, vocoder, model_config, preprocess_config, lengths=None):
 
     from . import ops
     if model_config["vocoder"]["model"] != "HiFi-GAN":
-        raise NotImplementedError("the B200-native path serves the vendored HiFi-GAN vocoder only (MelGAN needs a network fetch upstream)")
+        raise NotImplementedError("the H100-native path serves the vendored HiFi-GAN vocoder only (MelGAN needs a network fetch upstream)")
     with torch.no_grad():
         wav = vocoder(mels)                                    # [B, 1, N] fp32 on the device
     scale = float(preprocess_config["preprocessing"]["audio"]["max_wav_value"])

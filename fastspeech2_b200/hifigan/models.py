@@ -1,6 +1,6 @@
 """Drop-in `hifigan.models.Generator` (HiFi-GAN V1 generator): same constructor argument, checkpoint key layout
 (weight_g / weight_v / bias), `remove_weight_norm()` and `forward(mel[B,80,T]) -> wav[B,1,256*T]` as the reference
-(hifigan/models.py:112-174); forward is hand-written sm_100a CUDA behind fs2_vocoder_forward.  No PyTorch fallback.
+(hifigan/models.py:112-174); forward is hand-written sm_90a CUDA behind fs2_vocoder_forward.  No PyTorch fallback.
 """
 from __future__ import annotations
 
@@ -33,24 +33,19 @@ class Generator(nn.Module):
         self.num_kernels = len(self._hd["resblock_kernel_sizes"])
         self.num_upsamples = len(self._hd["upsample_rates"])
         self._weight_norm = True
-        self.use_tensor_cores = True     # split-FP16 tcgen05 kernel for every conv it supports; False = fp32 CUDA-core kernels only
+        self.use_tensor_cores = True     # split-FP16 tensor-core kernel for every conv it supports; False = fp32 CUDA-core kernels only
         # Operand split per part (bit 0 = conv_pre, bit 1+i = upsample stage i): set = fp16 main term + one E4M3 correction MMA
-        # (2/3 of the tensor time), clear = three fp16 MMAs.  Default: every upsample stage, NOT conv_pre -- measured with the shipped
-        # checkpoints (tests/test_gpu_model.py::test_hifigan_real_checkpoint_vs_reference, profiles/r02/parity_report_*.jsonl): all
-        # stages 1.0e-5 (LJSpeech) / 4.2e-5 (universal) of the 1e-4 bar, but conv_pre as well (its input is the raw log-mel, |x| up to
-        # 11.5) 1.2e-4 on the universal checkpoint.  CPU emulation of the split: scripts/emul_split_precision.py.
+        # (half the tensor-core work of the three-MMA split), clear = three fp16 MMAs.  Default: every upsample stage, NOT conv_pre --
+        # its input is the raw log-mel (|x| up to 11.5), where the E4M3 correction of the shipped universal checkpoint misses the 1e-4
+        # waveform bar (tests/test_gpu_model.py::test_hifigan_real_checkpoint_vs_reference; CPU emulation: scripts/emul_split_precision.py).
         self.f8_mask = 0b11110
         # Stages (bit i) whose ResBlock group runs as ONE persistent kernel with every intermediate on chip (fs2_resstack, available for
         # the 64- and 32-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).  Default: the 32-channel
-        # stage, where it beats the 18 per-layer launches (5.7 vs 6.3 ms at B = 16 x 1012 frames, 27x less HBM traffic); on the
-        # 64-channel stage the three-tile slab leaves no room to overlap epilogues with MMAs and the per-layer path is faster
-        # (profiles/r02/resstack_*.txt), so it stays opt-in there (fused_mask |= 0b0100).
+        # stage, the most memory-bound one; the 64-channel stage stays on the per-layer path unless fused_mask |= 0b0100.
         self.fused_mask = 0b1000
-        # Stages (bit i) where every (dilated conv, conv, +x) pair with kernel size <= pair_kmax runs as ONE fs2_resstack launch: the
-        # k = 3 layers of the 64-channel stage move 0.7 of the HBM peak as single layers (profiles/r02/conv_layer_bench_warm.txt);
-        # fused per pair the intermediate never leaves the SM.  Measured per pair (profiles/r02/pair_bench.txt): k = 3 556 vs 587 us
-        # for the two launches, but k = 7 842-902 vs 665 and k = 11 1133-1264 vs 801 -- one item in flight per SM serialises the
-        # pair's MMAs and epilogues, which only the HBM-bound k = 3 pairs can afford -- hence pair_kmax = 3.
+        # Stages (bit i) where every (dilated conv, conv, +x) pair with kernel size <= pair_kmax runs as ONE fs2_resstack launch, so
+        # that the intermediate never leaves the SM: worthwhile for the memory-bound k = 3 pairs of the 64-channel stage, while the
+        # longer kernels are tensor-bound and keep their per-layer launches -- hence pair_kmax = 3.
         self.pair_mask = 0b0100
         self.pair_kmax = 3
         populate(self, hifigan_spec(self._hd, weight_norm=True))
@@ -109,7 +104,7 @@ class Generator(nn.Module):
         hd = self._hd
         dev = get(self, "conv_pre.bias").device
         if dev.type != "cuda":
-            raise L.Fs2Error("hifigan.Generator (B200-native) needs its parameters on a CUDA device; there is no CPU path")
+            raise L.Fs2Error("hifigan.Generator (H100-native) needs its parameters on a CUDA device; there is no CPU path")
         m = L.VocoderModel()
         m.n_mel, m.c0 = 80, hd["upsample_initial_channel"]
         m.n_stages, m.n_kernels = self.num_upsamples, self.num_kernels
@@ -124,7 +119,7 @@ class Generator(nn.Module):
                 m.rb_dil[j][d] = dv
         for i, (u, k) in enumerate(zip(hd["upsample_rates"], hd["upsample_kernel_sizes"])):
             if k != 2 * u or u % 2:
-                raise L.Fs2Error("ConvTranspose1d stage needs kernel = 2*stride and even stride on the sm_100a path")
+                raise L.Fs2Error("ConvTranspose1d stage needs kernel = 2*stride and even stride on the sm_90a path")
             m.rates[i], m.up_k[i] = u, k
         m.fused_mask = 0
         if self.use_tensor_cores:
@@ -165,7 +160,7 @@ class Generator(nn.Module):
 
     def _forward(self, x):
         if self.training:
-            raise NotImplementedError("B200-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
+            raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
         lib = L.lib()
         m, _keep, dev, up = self._packed or self._pack()
         if x.dim() != 3 or x.shape[1] != m.n_mel:

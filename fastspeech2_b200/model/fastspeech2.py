@@ -1,5 +1,5 @@
 """Drop-in `model.fastspeech2.FastSpeech2`: same constructor, state_dict keys, forward signature and 10-tuple as the
-reference (model/fastspeech2.py:13-110); the forward itself is hand-written sm_100a CUDA behind the C ABI
+reference (model/fastspeech2.py:13-110); the forward itself is hand-written sm_90a CUDA behind the C ABI
 (include/fs2b200.h: fs2_acoustic_encode + fs2_acoustic_decode).  Inference only; there is no PyTorch fallback.
 """
 from __future__ import annotations
@@ -18,7 +18,7 @@ from ..synth import sinusoid_table
 
 
 class FastSpeech2(nn.Module):
-    """FastSpeech2 acoustic model, B200-native forward.
+    """FastSpeech2 acoustic model, H100-native forward.
 
     Arguments, parameter names and return values mirror the reference class (model/fastspeech2.py:16-41,:43-110).
     """
@@ -50,14 +50,13 @@ class FastSpeech2(nn.Module):
                         torch.exp(torch.linspace(np.log(stats["energy"][0]), np.log(stats["energy"][1]), n)))
         self.multi_speaker = bool(model_config["multi_speaker"])
         self.max_seq_len = int(model_config["max_seq_len"])
-        # Which sub-networks run on the tcgen05 kernels (L.TC_* bits; cleared = exact fp32 CUDA-core kernels).
+        # Which sub-networks run on the tensor-core kernels (L.TC_* bits; cleared = exact fp32 CUDA-core kernels).
         #  * decoder FFT blocks, mel_linear, PostNet: two-MMA operand split (*_F8: fp16 main term + one E4M3 correction MMA), fused attention.
         #  * encoder FFT blocks and the three variance predictors feed the DISCRETE duration / pitch / energy-bucket decisions (SURVEY.md
-        #    section 7, hard part 2).  A single long tensor-core accumulation (432 truncating steps for the k = 9 conv) left 1.8e-5 on the
-        #    predictions and flipped 7 / 13 buckets per 24.5k phonemes (fp32 kernels: 3.6e-6, 2 / 0).  They therefore run K-SEGMENTED
-        #    (fs2b200.h: every (tap, 256-channel) slice is its own 16-step launch with a separate hi*hi accumulator, slices summed in fp32
-        #    round-to-nearest): 2.1e-6, 2 / 1 flips -- the fp32 kernels' level -- and 0.7 ms less per step
-        #    (scripts/flip_census.py, profiles/r02/flip_census_encoder_predictors*.jsonl).  Clear the two bits for the fp32 kernels.
+        #    section 7, hard part 2).  A single long tensor-core accumulation (432 truncating steps for the k = 9 conv) flips buckets
+        #    noticeably more often than the fp32 kernels.  They therefore run K-SEGMENTED (fs2b200.h: every (tap, 256-channel) slice is
+        #    its own 16-step work unit with a separate hi*hi accumulator, slices summed in fp32 round-to-nearest), which brings the flips
+        #    back to the fp32 kernels' level (scripts/flip_census.py).  Clear the two bits for the fp32 kernels.
         self.tc_mask = (L.TC_DECODER | L.TC_POSTNET | L.TC_DECODER_F8 | L.TC_POSTNET_F8 | L.TC_ENCODER | L.TC_PREDICTORS)
         self._packed = None          # (AcousticModel struct, keep-alive tensors, device)
         self._pos_long = {}          # device position tables longer than max_seq_len, keyed by width
@@ -88,10 +87,10 @@ class FastSpeech2(nn.Module):
         tr = self.model_config["transformer"]
         vp = self.model_config["variance_predictor"]
         if tr["encoder_hidden"] != tr["decoder_hidden"] or tr["encoder_head"] != tr["decoder_head"]:
-            raise L.Fs2Error("encoder/decoder width or head count differ: unsupported by the sm_100a kernels")
+            raise L.Fs2Error("encoder/decoder width or head count differ: unsupported by the sm_90a kernels")
         dev = get(self, "mel_linear.weight").device
         if dev.type != "cuda":
-            raise L.Fs2Error("FastSpeech2 (B200-native) needs its parameters on a CUDA device; there is no CPU path")
+            raise L.Fs2Error("FastSpeech2 (H100-native) needs its parameters on a CUDA device; there is no CPU path")
         n_post = 0
         while f"postnet.convolutions.{n_post}.0.conv.weight" in self._keys():
             n_post += 1
@@ -174,7 +173,7 @@ class FastSpeech2(nn.Module):
     def _forward(self, speakers, texts, src_lens, max_src_len, mels=None, mel_lens=None, max_mel_len=None,
                  p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0):
         if self.training:
-            raise NotImplementedError("B200-native FastSpeech2 is inference-only: call .eval() (utils/model.py:32)")
+            raise NotImplementedError("H100-native FastSpeech2 is inference-only: call .eval() (utils/model.py:32)")
         p_frame = self.pitch_feature_level == "frame_level"
         e_frame = self.energy_feature_level == "frame_level"
         lib = L.lib()

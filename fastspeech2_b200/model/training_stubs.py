@@ -6,7 +6,7 @@ Training is outside this path's scope (SURVEY.md section 2.1 rows 11-13); the na
 
 class _TrainingOnly:
     def __init__(self, *a, **k):
-        raise NotImplementedError(f"{type(self).__name__}: the B200-native drop-in covers inference only")
+        raise NotImplementedError(f"{type(self).__name__}: the H100-native drop-in covers inference only")
 
 
 class FastSpeech2Loss(_TrainingOnly):

@@ -1,4 +1,4 @@
-"""Weight re-layout for the sm_100a kernels (pure tensor permutations, device-agnostic, run once per load).
+"""Weight re-layout for the sm_90a kernels (pure tensor permutations, device-agnostic, run once per load).
 
 Inputs are reference-keyed tensors (SURVEY.md Appendix C); outputs are the layouts include/fs2b200.h documents:
 conv / linear weights as [taps][C_in][C_out] (C_out contiguous), QKV concatenated, eval BatchNorm folded into the
@@ -24,13 +24,14 @@ def lin_w(w: Tensor) -> Tensor:
     return w.t().contiguous()
 
 
-def conv_tc_block(n_out: int) -> int:
-    """Output channels per CTA of the tcgen05 kernel (mirror of conv_tc_nb in csrc/conv_tc.cu); 0 = unsupported."""
+def conv_tc_block(n_out: int, nb_max: int = 128) -> int:
+    """Output channels per work item of the tensor-core kernel (mirror of conv_tc_nb in csrc/conv_tc.cu); 0 = unsupported.
+    The f8 split uses nb_max = 64 (its correction term needs an accumulator of its own)."""
     if n_out % 16:
         return 0
-    if n_out <= 128:
+    if n_out <= nb_max:
         return n_out
-    for nb in range(128, 15, -16):
+    for nb in range(nb_max, 15, -16):
         if n_out % nb == 0:
             return nb
     return 0
@@ -60,16 +61,16 @@ def _e4m3_bytes(x: Tensor) -> Tensor:
 
 
 def pack_conv_tc(w: Tensor, f8: bool = False, nb: int | None = None):
-    """[taps][Cin][N] fp32 -> byte buffer for the tcgen05 kernel (see include/fs2b200.h):
+    """[taps][Cin][N] fp32 -> byte buffer for the tensor-core kernel (see include/fs2b200.h):
          128-byte header (float32[0] = 1/scale, int32[1] = format)  |  [N/NB][Cin/16][taps][2 planes][2 K-chunks][NB][16 bytes]
-    Every (tap, 16-channel K-block) stage is one contiguous 64*NB-byte smem image (UMMA no-swizzle K-major).
+    Every (tap, 16-channel K-block) stage is one contiguous 64*NB-byte smem image (no-swizzle K-major).
       f8 = False (format 0): plane 0 = fp16 hi, plane 1 = fp16 lo; a chunk row holds 8 channels.
       f8 = True  (format 1, FS2_TC_VARIANT_F8): plane 0 = fp16 hi; plane 1 = E4M3 with chunk 0 = hi * 2^-12 and chunk 1 = lo of the
-        K-block's 16 channels -- the B operand of one K = 32 kind::f8f6f4 MMA against the activations' [lo * 2^12 | hi].
+        K-block's 16 channels -- the B operand of one K = 32 E4M3 MMA against the activations' [lo * 2^12 | hi]; NB <= 64.
     Returns None when the shape is not served by the tensor-core kernel."""
     taps, cin, n = w.shape
     if nb is None:
-        nb = conv_tc_block(n)
+        nb = conv_tc_block(n, 64 if f8 else 128)
     elif n % nb or nb % 16:
         return None
     if nb == 0 or cin % 16:

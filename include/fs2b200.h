@@ -1,4 +1,4 @@
-/* fs2b200.h -- C ABI of the B200-native FastSpeech2 + HiFi-GAN inference path.
+/* fs2b200.h -- C ABI of the H100-native FastSpeech2 + HiFi-GAN inference path.
  *
  * The reference (ming024/FastSpeech2) has no FFI: its "plugin API" for this path is two nn.Module
  * classes.  This library is what a native binding underneath those two classes calls:
@@ -43,19 +43,21 @@ enum {
 
 enum { FS2_ACT_NONE = 0, FS2_ACT_RELU = 1, FS2_ACT_TANH = 2, FS2_ACT_LRELU = 3 };
 enum { FS2_CONV_AUTO = 0, FS2_CONV_SIMT = 1, FS2_CONV_TC = 2 };
-/* which parts of the acoustic model may use the split-FP16 tcgen05 kernel (fs2_acoustic_model.tc_mask) */
+/* which parts of the acoustic model may use the split-FP16 tensor-core kernel (fs2_acoustic_model.tc_mask) */
 enum { FS2_TC_ENCODER = 1, FS2_TC_PREDICTORS = 2, FS2_TC_DECODER = 4, FS2_TC_POSTNET = 8,
        /* the decoder's / PostNet's w_*_tc tiles are in the f16+f8 format (see FS2_TC_VARIANT_F8) */
        FS2_TC_DECODER_F8 = 16, FS2_TC_POSTNET_F8 = 32,
        /* decoder attention through the round-1 GEMM path (scores materialised in HBM) instead of the fused kernel */
        FS2_TC_ATTENTION_GEMM = 64 };
 /* fs2_conv1d_args.tc_variant bits.  F8: w_tc holds the two-MMA operand split -- fp16 hi tiles as in the three-MMA split, and in
- * place of the fp16 lo tiles E4M3 tiles [hi * 2^-12 | lo] that one K = 32 kind::f8f6f4 MMA multiplies with the activations'
+ * place of the fp16 lo tiles E4M3 tiles [hi * 2^-12 | lo] that one K = 32 E4M3 MMA multiplies with the activations'
  * [lo * 2^12 | hi]: y ~ a_hi.w_hi + (a_lo.w_hi + a_hi.w_lo) with the bracket at E4M3 precision (relative error ~2^-16 instead
- * of ~2^-22; 2/3 of the tensor-pipe time and shared-memory operand traffic).  Activations beyond +-448 saturate in the correction. */
+ * of ~2^-22; half the tensor-core work of the three-MMA split).  The correction accumulates separately from the main term (Hopper
+ * adds E4M3 products with reduced precision), so F8 tiles use NB = fs2_conv_tc_block_f8(N) <= 64 output channels per work item.
+ * Activations beyond +-448 saturate in the correction. */
 enum { FS2_TC_VARIANT_F8 = 1,
        /* w_tc is tiled for 64 output channels per work item (pack_conv_tc(w, nb=64)): the hi*hi term and the two cross terms then
-        * accumulate in separate tensor-memory tiles.  Used by the K-segmented encoder / predictor path (see fs2_acoustic_model). */
+        * accumulate in separate register accumulators.  Used by the K-segmented encoder / predictor path (see fs2_acoustic_model). */
        FS2_TC_VARIANT_NB64 = 2,
        /* with NB64: w_tc holds taps * (C_in / 256) one-tap tile buffers back to back (packing.pack_conv_tc_segments) and the conv is
         * evaluated K-SEGMENTED inside one launch: every (tile, tap, 256-channel chunk) is a work unit with a fresh 16-step accumulator,
@@ -63,16 +65,18 @@ enum { FS2_TC_VARIANT_F8 = 1,
         * pad-row mask with the last).  Needs dilation 1, alpha 1, no output activation, C_in % 256 == 0, N % 64 == 0. */
        FS2_TC_VARIANT_SEGMENTED = 4 };
 
-/* Tensor-core weight tiles.  For a conv weight w[taps][Cin][N] with NB = fs2_conv_tc_block(N) output channels per work item,
+/* Tensor-core weight tiles.  For a conv weight w[taps][Cin][N] with NB = fs2_conv_tc_block(N) output channels per work item
+ * (fs2_conv_tc_block_f8(N) for FS2_TC_VARIANT_F8 tiles, whose plane 1 holds the E4M3 [hi * 2^-12 | lo] chunks instead of fp16 lo),
  * s = a per-layer power of two, hi = fp16(s*w), lo = fp16(s*w - hi), the tiled byte buffer is
  *     128-byte header (float32[0] = 1/s)  |  [N/NB][Cin/16][taps][2: hi,lo][2: 16-byte K chunk][NB][8 halfs]
- * i.e. every (K-block, tap) stage is one contiguous 64*NB-byte smem image (UMMA no-swizzle K-major, fp16), fetched by one
+ * i.e. every (K-block, tap) stage is one contiguous 64*NB-byte smem image (no-swizzle K-major, fp16), fetched by one
  * cp.async.bulk.  fastspeech2_b200/packing.py::pack_conv_tc builds it. */
-int fs2_conv_tc_block(int N); /* 0 when N is not supported by the tensor-core kernel */
+int fs2_conv_tc_block(int N);    /* 0 when N is not supported by the tensor-core kernel */
+int fs2_conv_tc_block_f8(int N); /* the same for FS2_TC_VARIANT_F8 tiles: the largest multiple of 16 <= 64 that divides N (N itself if N <= 64) */
 struct fs2_conv1d_args;
-/* Launch plan the tcgen05 kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are
+/* Launch plan the tensor-core kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are
  * only checked for alignment): out[12] = {NB, MT (128-row tiles per work item), TG (accumulators per tile), slab stages, weight
- * stages, taps per weight stage, slab rows, TMEM columns, work items per utterance, work items, grid, dynamic shared memory bytes}.
+ * stages, taps per weight stage, slab rows, accumulator registers per consumer thread, work items per utterance, work items, grid, dynamic shared memory bytes}.
  * Returns FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
 int fs2_conv_tc_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out);
 
@@ -88,18 +92,18 @@ int fs2_conv_tc_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out)
  * rows outside [0,T) read as zero (Conv1d zero padding); rows t >= row_lens[b] are written as exact 0 when row_lens != NULL.
  * Strides are in elements.  Covers nn.Linear (taps=1), nn.Conv1d (any odd k, dilation), and one phase group of
  * ConvTranspose1d (two taps, y_row_stride = u*C_out; see fs2_vocoder_model).
- * Both kernels: Cin % 16 == 0, pointers 16-byte aligned, strides % 4 == 0.  The tcgen05 kernel additionally needs w_tc,
+ * Both kernels: Cin % 16 == 0, pointers 16-byte aligned, strides % 4 == 0.  The tensor-core kernel additionally needs w_tc,
  * N % 16 == 0, x 32-byte aligned with x strides % 8 == 0 (256-bit loads), in_act in {NONE, LRELU with 0 <= slope <= 1} and
  * (taps-1)*dilation <= 256; anything else is served by the exact kernel under FS2_CONV_AUTO and refused (FS2_ERR_UNSUPPORTED)
- * under FS2_CONV_TC.  Activations beyond +-65504 saturate in the fp16 hi/lo split of the tcgen05 kernel. */
+ * under FS2_CONV_TC.  Activations beyond +-65504 saturate in the fp16 hi/lo split of the tensor-core kernel. */
 typedef struct fs2_conv1d_args {
   const float* x; int64_t x_batch_stride, x_row_stride;
   int B, T, Cin;
   const float* w;    /* [taps][Cin][N] */
   const float* bias; /* [N] or NULL */
   int N, taps, dilation, pad_left;
-  const float* w_tc; /* NULL, or the same weights in the tcgen05 tile layout (see "tensor-core weight tiles" below) */
-  int backend;       /* FS2_CONV_AUTO: split-FP16 tcgen05 kernel when w_tc is given and the shape qualifies, else the fp32 CUDA-core kernel */
+  const float* w_tc; /* NULL, or the same weights in the tensor-core tile layout (see "tensor-core weight tiles" below) */
+  int backend;       /* FS2_CONV_AUTO: split-FP16 tensor-core kernel when w_tc is given and the shape qualifies, else the fp32 CUDA-core kernel */
   unsigned tc_variant; /* FS2_TC_VARIANT_* bits describing the format of w_tc */
   int in_act; float in_slope;
   int out_act; float out_slope;
@@ -126,7 +130,7 @@ typedef struct fs2_attention_args {
   const float* qkv; float* ctx; int B, T, H, Dh;
   const int32_t* key_lens; float scale;
   int backend;                  /* 0 = exact fp32 flash-style kernel; 1 = tensor-core GEMMs + row softmax (scores in HBM, T <= 4096); 2 = ONE fused
-                                   tcgen05 kernel (QK^T, softmax, PV; scores stay in tensor memory, any T).  1 and 2 need the workspace */
+                                   tensor-core kernel (QK^T, softmax, PV; scores stay in registers, any T).  1 and 2 need the workspace */
   void* workspace; size_t workspace_bytes;   /* backend 1 only: >= fs2_attention_workspace_bytes(B, T, H) */
 } fs2_attention_args;
 int fs2_attention(const fs2_attention_args* a, fs2_stream_t stream);
@@ -181,7 +185,7 @@ int fs2_conv_post(const fs2_conv_post_args* a, fs2_stream_t stream);
 /* HiFi-GAN multi-receptive-field ResBlock group of one upsample stage as ONE persistent kernel (hifigan/models.py:154-160, ResBlock.forward
  * :96-103):   y = (1/n_kernels) * sum_j R_j(x),   R_j: x <- conv_{k_j,1}( lrelu( conv_{k_j,dil_jd}( lrelu(x) ) + b1 ) ) + b2 + x  for d = 0..n_dil-1,
  * lrelu slope 0.1, "same" zero padding at the utterance ends.  x, y: contiguous [B][N][C], C in {32, 64} (the 64- / 32-channel stages);
- * every intermediate stays in shared / tensor memory (halo recompute), weights are the f16+f8 tiles of the per-layer kernel
+ * every intermediate stays in shared memory / registers (halo recompute), weights are the f16+f8 tiles of the per-layer kernel
  * (FS2_TC_VARIANT_F8 with N = C: pack_conv_tc(w, f8=True)).  (k-1)*dil/2 <= 32 per conv.  Other shapes: FS2_ERR_UNSUPPORTED.
  * x and y must not overlap (work items re-read halo rows of x): FS2_ERR_ARG. */
 typedef struct fs2_resstack_args {
@@ -196,8 +200,8 @@ typedef struct fs2_resstack_args {
 } fs2_resstack_args;
 int fs2_resstack(const fs2_resstack_args* a, fs2_stream_t stream);
 /* launch plan (pure host logic): out[12] = {128-row tiles per slab, halo rows per side, output rows per work item, work items, grid,
- * weight ring stages, dynamic shared memory bytes, TMEM columns, rows per output TMA box, output boxes per tile, conv taps per weight stage,
- * independent-tile mode (single kernel size with a small halo: every 128-row tile carries its own halo)} */
+ * weight ring stages, dynamic shared memory bytes, accumulator registers per consumer thread, rows per output TMA box, output boxes per tile, conv taps per weight stage,
+ * 0 (reserved: every work item is one slab with its halo at the two ends)} */
 int fs2_resstack_plan(const fs2_resstack_args* a, int num_sms, int32_t* out);
 
 /* out[b,t] = t < lens[b] ? (int16) trunc(wav[b,t] * scale) : 0   -- the device half of utils.model.vocoder_infer (utils/model.py:82-90:
@@ -236,7 +240,7 @@ typedef struct fs2_predictor_weights {
 
 /* Encoder / predictors on the tensor cores (tc_mask bits FS2_TC_ENCODER / FS2_TC_PREDICTORS): these layers feed the discrete duration and
  * pitch / energy bucket decisions, where the truncating tensor-core accumulator of a long K loop (432 accumulation steps for the k = 9
- * conv) costs 5x the error of the fp32 CUDA-core kernel (profiles/r02/flip_census_*.jsonl).  They therefore run K-SEGMENTED: every
+ * conv) costs 5x the error of the fp32 CUDA-core kernel (scripts/flip_census.py).  They therefore run K-SEGMENTED: every
  * (tap, 256-input-channel) slice is its own launch of 16 K-steps whose hi*hi term has its own accumulator (FS2_TC_VARIANT_NB64), and the
  * slices are summed in fp32 round-to-nearest by the epilogue's accumulate path.  Their w_*_tc pointers then hold
  * taps * (C_in / 256) tile buffers back to back (segment (tap, kc) at index tap * (C_in/256) + kc, each 128 + 1024 * N bytes:
@@ -328,14 +332,14 @@ int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, f
 /* ------------------------------------------------------------------ misc */
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
-const char* fs2_build_info(void);          /* "sm_100a ..." */
+const char* fs2_build_info(void);          /* "sm_90a ..." */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the
  * device that owns the stream current before calling -- (b) the launch counter above and (c) the profiling state below, which is
  * per host thread.  Tuning / tracing knobs exist only in builds with -DFS2_DEBUG_KNOBS.
  * Per-kernel-class device timing for bench.py's roofline (CUDA events recorded around each launch on the launch stream).
- * Classes: 0 tcgen05 kernels (conv1d implicit GEMM + fused ResBlock group), 1 attention, 2 layernorm, 3 everything else, 4 fp32 CUDA-core conv1d.  begin() arms it, end() synchronises the
+ * Classes: 0 tensor-core kernels (conv1d implicit GEMM + fused ResBlock group), 1 attention, 2 layernorm, 3 everything else, 4 fp32 CUDA-core conv1d.  begin() arms it, end() synchronises the
  * recorded events, fills ms/flops/launches per class (arrays of FS2_PROF_CLASSES) and disarms.  Not for timed regions. */
 #define FS2_PROF_CLASSES 5
 int fs2_profile_begin(void);

@@ -105,5 +105,91 @@ def main():
         json.dump(keys, f, indent=0, sort_keys=True)
 
 
+def live_cases():
+    """tests/golden/reference_cases.npz: the reference's outputs for the inputs of test_oracle_golden.py's multi-speaker / teacher-forced /
+    vocoder case and its frame-level case (inputs are regenerated from the same seeds by the tests)."""
+    import copy
+    FastSpeech2, hifigan = ref_import.load()
+    scratch = tempfile.mkdtemp()
+    z = {}
+    pc, mc = configs.make_configs("LibriTTS", scratch)
+    sd = synth.fastspeech2_state_dict(pc, mc, seed=31)
+    ref = FastSpeech2(pc, mc)
+    ref.load_state_dict(sd, strict=True)
+    ref.eval()
+    spk, texts, lens, L = synth.make_batch(3, 36, seed=32, n_speakers=904, min_len=10)
+    with torch.no_grad():
+        want = ref(spk, texts, lens, L, p_control=0.9, d_control=1.2)
+        ml = want[9]
+        want2 = ref(spk, texts, lens, L, None, ml, int(ml.max()), want[2], want[3], want[5].long())
+    for i in (0, 1, 2, 3, 4, 5, 9):
+        z[f"free_{i}"] = want[i].numpy()
+    for i in (0, 1, 4):      # fed its own predictions, the teacher-forced mel and log-durations equal the free-running ones bit for bit
+        assert torch.equal(want2[i], want[i])
+    for i in (2, 3):
+        z[f"forced_{i}"] = want2[i].numpy()
+    h = hifigan.AttrDict(configs.HIFIGAN_CONFIG)
+    gen = hifigan.Generator(h)
+    gen.load_state_dict(synth.hifigan_state_dict(h, seed=33), strict=True)
+    gen.eval()
+    gen.remove_weight_norm()
+    with torch.no_grad():
+        z["wav"] = gen(synth.make_mel(1, 30, seed=34)).numpy()
+    pc, mc = configs.make_configs("LJSpeech", scratch)
+    pc = copy.deepcopy(pc)
+    pc["preprocessing"]["pitch"]["feature"] = "frame_level"
+    pc["preprocessing"]["energy"]["feature"] = "frame_level"
+    ref = FastSpeech2(pc, mc)
+    ref.load_state_dict(synth.fastspeech2_state_dict(pc, mc, seed=41), strict=True)
+    ref.eval()
+    spk, texts, lens, L = synth.make_batch(2, 22, seed=42, min_len=13)
+    with torch.no_grad():
+        want = ref(spk, texts, lens, L, p_control=1.2)
+    for i in (0, 1, 2, 3, 4, 9):
+        z[f"frame_{i}"] = want[i].numpy()
+    np.savez_compressed(os.path.join(OUT, "reference_cases.npz"), **z)
+
+
+def frontend_cases():
+    """tests/golden/frontend_reference_batches.npz: the three `preprocessed_data/*/val.txt` files the reference ships, the token
+    sequences its `text_to_sequence` makes of every line, and the batches of its TextDataset + DataLoader(batch_size=8).  Runs the
+    reference's modules (`text`, `dataset`) from its own tree, so call it in a process of its own."""
+    ref_import._stub()
+    ref = ref_import.REFERENCE_ROOT
+    sys.path.insert(0, ref)
+    os.chdir(ref)
+    import yaml
+    from torch.utils.data import DataLoader
+    from dataset import TextDataset as RefTextDataset
+    from text import text_to_sequence
+    z = {}
+    as_bytes = lambda s: np.frombuffer(s.encode("utf-8") if isinstance(s, str) else s, dtype=np.uint8)
+    for ds in ("LJSpeech", "LibriTTS", "AISHELL3"):
+        pc = yaml.safe_load(open(f"config/{ds}/preprocess.yaml"))
+        pre = pc["path"]["preprocessed_path"]
+        src = os.path.join(pre, "val.txt")
+        cleaners = pc["preprocessing"]["text"]["text_cleaners"]
+        data = RefTextDataset(src, pc)
+        seqs = [np.asarray(text_to_sequence(t, cleaners), dtype=np.int64) for t in data.text]
+        z[f"{ds}__val"] = as_bytes(open(src, "rb").read())
+        z[f"{ds}__speakers"] = as_bytes(open(os.path.join(pre, "speakers.json"), "rb").read())
+        z[f"{ds}__seq"] = np.concatenate(seqs)
+        z[f"{ds}__seq_len"] = np.array([len(s) for s in seqs], dtype=np.int64)
+        meta = {"cleaners": cleaners, "batches": [], "item5": None}
+        for i, (ids, raws, spk, texts, lens, mx) in enumerate(DataLoader(data, batch_size=8, collate_fn=data.collate_fn)):
+            meta["batches"].append({"ids": ids, "raw": raws, "max": int(mx), "max_type": type(mx).__name__})
+            z[f"{ds}__b{i}__spk"], z[f"{ds}__b{i}__texts"], z[f"{ds}__b{i}__lens"] = spk, texts, lens
+        it = data[5]
+        assert np.array_equal(it[2], seqs[5])
+        meta["item5"] = [it[0], int(it[1]), it[3]]
+        z[f"{ds}__meta"] = as_bytes(json.dumps(meta))
+    np.savez_compressed(os.path.join(OUT, "frontend_reference_batches.npz"), **z)
+
+
 if __name__ == "__main__":
-    main()
+    if "--frontend" in sys.argv:
+        frontend_cases()
+    elif "--cases" in sys.argv:
+        live_cases()
+    else:
+        main()

@@ -1,4 +1,4 @@
-"""Warm timings of single HiFi-GAN-shaped fs2_conv1d layers on the tcgen05 kernel (B = 16 x 1017 frames), both operand splits.
+"""Warm timings of single HiFi-GAN-shaped fs2_conv1d layers on the tensor-core kernel (B = 16 x 1017 frames), both operand splits.
 Usage: python scripts/conv_layer_bench.py [one]   (one = a single (C=128, k=3, f8) layer in a loop, for ncu)"""
 import sys, os, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

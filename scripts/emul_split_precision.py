@@ -1,8 +1,8 @@
 """CPU emulation of candidate tensor-core operand splits on the HiFi-GAN generator (exact fp64 accumulation of the rounded
-operands), against the fp64 oracle.  Decides which split the tcgen05 conv kernel may use.
+operands), against the fp64 oracle.  Decides which split the tensor-core conv kernel may use.
 
-  split3 : a = hi + lo (fp16, fp16), w likewise:  ah*wh + al*wh + ah*wl                 (3 kind::f16 MMAs, round 1)
-  f16f8  : main ah*wh in fp16; correction [al8 | ah8] . [wh8 ; wl8] in e4m3            (1 kind::f16 + 1 kind::f8f6f4 MMA)
+  split3 : a = hi + lo (fp16, fp16), w likewise:  ah*wh + al*wh + ah*wl                 (3 FP16 MMAs, round 1)
+  f16f8  : main ah*wh in fp16; correction [al8 | ah8] . [wh8 ; wl8] in e4m3            (1 FP16 + 1 E4M3 MMA)
   f16    : ah*wh only
 
 Usage: python scripts/emul_split_precision.py [--real] [--frames 60]

@@ -1,6 +1,6 @@
 """Decision-flip census (SURVEY.md section 7, hard part 2; VERDICT r01 item 6): durations round(exp(logd) - 1) and the pitch / energy
 buckets are discrete, so fp32-level differences can flip them.  For >= 10k phonemes per config this counts, against the CPU oracle,
-the flips of (a) the exact fp32 CUDA-core encoder + predictors and (b) the tcgen05 three-MMA-split encoder + predictors, with the
+the flips of (a) the exact fp32 CUDA-core encoder + predictors and (b) the tensor-core three-MMA-split encoder + predictors, with the
 distance of every flipped value to its decision boundary.  One JSON line per (config, path).  Usage: python scripts/flip_census.py [seeds]"""
 import json, os, sys, tempfile
 import torch
@@ -15,7 +15,7 @@ torch.set_num_threads(16)
 base = L.TC_DECODER | L.TC_POSTNET | L.TC_DECODER_F8 | L.TC_POSTNET_F8
 for ds, nspk, Lmax, minlen in (("LJSpeech", 1, 128, None), ("LibriTTS", 904, 192, 64)):
     pc, mc = configs.make_configs(ds, tempfile.mkdtemp())
-    for path, mask in (("fp32_cuda_cores", base), ("tcgen05_k_segmented", base | L.TC_ENCODER | L.TC_PREDICTORS)):
+    for path, mask in (("fp32_cuda_cores", base), ("tensor_core_k_segmented", base | L.TC_ENCODER | L.TC_PREDICTORS)):
         tot = {"config": ds, "encoder_predictors": path, "phonemes": 0, "duration_flips": 0, "pitch_bucket_flips": 0, "energy_bucket_flips": 0,
                "max_err_logd": 0.0, "max_err_pitch": 0.0, "max_err_energy": 0.0, "flip_margins": []}
         for seed in range(seeds):

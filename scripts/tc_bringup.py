@@ -1,4 +1,4 @@
-"""GPU bring-up of the tcgen05 conv kernel: every case runs in its own subprocess (a wedged kernel cannot take the
+"""GPU bring-up of the tensor-core conv kernel: every case runs in its own subprocess (a wedged kernel cannot take the
 rest down) for each descriptor variant; prints max-abs error against an fp64 CPU evaluation of the fs2_conv1d contract."""
 import json
 import os

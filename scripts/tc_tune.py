@@ -1,4 +1,4 @@
-"""A/B the tcgen05 conv kernel's ring depths / taps-per-stage inside ONE process (box-to-box noise is ~10-20 %)."""
+"""A/B the tensor-core conv kernel's ring depths / taps-per-stage inside ONE process (box-to-box noise is ~10-20 %)."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

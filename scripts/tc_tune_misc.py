@@ -1,5 +1,5 @@
-"""Re-tune after the instruction trim, inside ONE process: taps per weight stage (TPS) for small-k layers, MT=4 vs MT=2 for narrow layers,
-weight ring depth.  Debug hook fs2_debug_set_tc_tuning(sa, sb, tps, grid) with grid = -1 forcing MT = 2."""
+"""Tune the tensor-core conv kernel inside ONE process: taps per weight stage (TPS) and weight ring depth per HiFi-GAN layer shape.
+Debug hook fs2_debug_set_tc_tuning(sa, sb, tps, grid) (library built with FS2_DEBUG_KNOBS=1; 0 = the heuristic's choice)."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -12,7 +12,7 @@ shapes = [("s3 C32 k3", 32, 32, 3, 1, 262144, False), ("s3 C32 k7 res", 32, 32, 
           ("ups2 C128->64 k2", 128, 64, 2, 1, 65536, False), ("s1 C128 k3", 128, 128, 3, 1, 65536, False), ("s1 C128 k7", 128, 128, 7, 1, 65536, False),
           ("s1 C128 k11", 128, 128, 11, 1, 65536, False), ("s0 C256 k3", 256, 256, 3, 1, 8192, False), ("s0 C256 k7", 256, 256, 7, 1, 8192, False)]
 settings = [("default", (0, 0, 0, 0)), ("tps1", (0, 0, 1, 0)), ("tps2", (0, 0, 2, 0)), ("tps3", (0, 0, 3, 0)), ("tps4", (0, 0, 4, 0)), ("tps6", (0, 0, 6, 0)),
-            ("MT2", (0, 0, 0, -1)), ("sb2", (0, 2, 0, 0)), ("sb3", (0, 3, 0, 0)), ("sb6", (0, 6, 0, 0)), ("default", (0, 0, 0, 0))]
+            ("sb2", (0, 2, 0, 0)), ("sb3", (0, 3, 0, 0)), ("sb6", (0, 6, 0, 0)), ("default", (0, 0, 0, 0))]
 for name, Cin, N, k, dil, T, res in shapes:
     B = 16
     x = torch.randn(B, T, Cin, generator=g).cuda()

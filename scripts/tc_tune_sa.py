@@ -1,4 +1,4 @@
-"""Sweep the activation-slab ring depth (SA) of the tcgen05 conv kernel per layer shape inside ONE process (debug tuning hook)."""
+"""Sweep the activation-slab ring depth (SA) of the tensor-core conv kernel per layer shape inside ONE process (debug tuning hook)."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -9,19 +9,19 @@ if ROOT not in sys.path:
 
 
 def pytest_sessionstart(session):
-    # the CPU oracle is ATen: on many-core hosts (the B200 box has 128) more threads than the small test problems can feed is slower
+    # the CPU oracle is ATen: on many-core hosts more threads than the small test problems can feed is slower
     import torch
     torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: select with `-m gpu`)")
     config.addinivalue_line("markers", "reference: needs the reference tree at /root/reference (absent on the GPU box)")
 
 
 def pytest_collection_modifyitems(config, items):
     """`gpu` tests are skipped (not failed) on a host without a CUDA device or without the built library, so a plain `pytest tests`
-    works on CPU-only CI; the driver selects them with `-m gpu` on the B200 box."""
+    works on CPU-only CI; `-m gpu` selects them on an H100."""
     import torch
     lib = os.path.join(ROOT, "fastspeech2_b200", "libfs2b200.so")
     why = None

@@ -21,7 +21,7 @@ def test_library_builds_and_loads():
     assert os.path.exists(path)
     h = _lib.lib()
     assert h.fs2_abi_version() == _lib.ABI_VERSION
-    assert b"sm_100a" in h.fs2_build_info()
+    assert b"sm_90a" in h.fs2_build_info()
 
 
 def test_every_declared_symbol_is_exported_and_bound():
@@ -60,19 +60,19 @@ def test_host_side_argument_checks_need_no_gpu():
     assert h.fs2_resstack(ctypes.byref(r), None) == -1           # misaligned y
 
 
-def _plan(h, B, T, Cin, N, taps, dil=1, num_sms=148, x=0x1000, x_row_stride=None):
+def _plan(h, B, T, Cin, N, taps, dil=1, num_sms=132, x=0x1000, x_row_stride=None):
     a = _lib.Conv1dArgs(x=x, x_batch_stride=T * (x_row_stride or Cin), x_row_stride=x_row_stride or Cin, B=B, T=T, Cin=Cin, w=0x1000, N=N, taps=taps,
                         dilation=dil, pad_left=(taps - 1) * dil // 2, w_tc=0x1000, y=0x1000, y_batch_stride=T * N, y_row_stride=N, alpha=1.0)
     out = (ctypes.c_int32 * 12)()
     rc = h.fs2_conv_tc_plan(ctypes.byref(a), num_sms, out)
-    keys = ("NB", "MT", "TG", "SA", "SB", "TPS", "R", "tmem_cols", "tiles_per_batch", "n_items", "grid", "smem")
+    keys = ("NB", "MT", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")
     return rc, dict(zip(keys, out))
 
 
-def test_tcgen05_launch_plan_respects_the_hardware_limits():
-    """Host-side heuristics of the tcgen05 conv (work-item shape, ring depths, TMEM / shared-memory budget) for every layer shape of
-    both models at the BASELINE batch sizes, plus a sweep: no plan may exceed 227 KB of shared memory, 512 TMEM columns, the
-    register-ring row capacity or the ring maxima, and the work items must cover the problem exactly."""
+def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
+    """Host-side heuristics of the wgmma conv (work-item shape, ring depths, register / shared-memory budget) for every layer shape of
+    both models at the BASELINE batch sizes, plus a sweep: no plan may exceed 227 KB of shared memory, 64 accumulator registers per
+    consumer thread, the register-ring row capacity or the ring maxima, and the work items must cover the problem exactly."""
     h = _lib.lib()
     shapes = []
     for B, T in ((1, 7), (1, 1012), (16, 1012), (64, 2032)):
@@ -85,22 +85,28 @@ def test_tcgen05_launch_plan_respects_the_hardware_limits():
             t, c = t * u, c // 2
             shapes += [(B, t, c, c, k, d) for k in (3, 7, 11) for d in (1, 3, 5)]
     for (B, T, Cin, N, k, d) in shapes:
-        rc, p = _plan(h, B, T, Cin, N, k, d)
+        rc, p = _plan(h, B, T, Cin, N, k, d, num_sms=132)
         assert rc == 0, (B, T, Cin, N, k, d, rc)
         assert p["NB"] % 16 == 0 and 16 <= p["NB"] <= 128 and N % p["NB"] == 0
-        assert p["MT"] in (1, 2, 4) and p["TG"] in (1, 2)
-        acc_stride = (p["NB"] + 31) // 32 * 32
-        assert 2 * p["MT"] * p["TG"] * acc_stride <= p["tmem_cols"] <= 512 and p["tmem_cols"] & (p["tmem_cols"] - 1) == 0
+        assert p["MT"] == 1 and p["TG"] == (2 if p["NB"] <= 64 else 1)
+        assert p["acc_regs"] == p["TG"] * p["NB"] // 2 <= 64
         assert p["smem"] <= 227 * 1024
         assert 2 <= p["SA"] <= 8 and 2 <= p["SB"] <= 8 and 1 <= p["TPS"] <= k
-        assert p["R"] % 8 == 4 and p["R"] >= p["MT"] * 128 + (k - 1) * d
-        assert p["R"] <= (5 if p["MT"] == 4 else 3) * 256 // 2 + 7               # rows the transform warps' register ring can hold
-        assert p["tiles_per_batch"] * p["MT"] * 128 >= T > (p["tiles_per_batch"] - 1) * p["MT"] * 128
-        assert p["n_items"] == (N // p["NB"]) * B * p["tiles_per_batch"] and p["grid"] == min(p["n_items"], 148)
-    # the measured shape classes keep their tuned plans (profiles/r01_tc_tune_sa.txt, r01_tc_ab_mt4.txt)
-    assert _plan(h, 16, 259072, 32, 32, 3)[1]["MT"] == 4 and _plan(h, 16, 259072, 32, 32, 3)[1]["SA"] == 3
+        assert p["R"] % 8 == 4 and p["R"] >= 128 + (k - 1) * d
+        assert p["R"] <= 3 * 256 // 2 + 7                                      # rows the transform warps' register ring can hold
+        assert p["tiles_per_batch"] * 128 >= T > (p["tiles_per_batch"] - 1) * 128
+        assert p["n_items"] == (N // p["NB"]) * B * p["tiles_per_batch"] and p["grid"] == min(p["n_items"], 132)
+    # the packer and the kernel agree on the work-item width of both tile formats (F8 tiles: at most 64 channels)
+    from fastspeech2_b200 import packing
+    for n in range(0, 1100, 8):
+        assert h.fs2_conv_tc_block(n) == packing.conv_tc_block(n) and h.fs2_conv_tc_block_f8(n) == packing.conv_tc_block(n, 64), n
+        if n and n % 16 == 0:
+            a = _lib.Conv1dArgs(x=0x1000, x_batch_stride=256 * 16, x_row_stride=16, B=1, T=256, Cin=16, w=0x1000, N=n, taps=1,
+                                w_tc=0x1000, y=0x1000, y_batch_stride=256 * n, y_row_stride=n, alpha=1.0, tc_variant=_lib.TC_VARIANT_F8)
+            out = (ctypes.c_int32 * 12)()
+            assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, out) == 0 and out[0] == h.fs2_conv_tc_block_f8(n) and out[2] == 2, n
+    # ring depths per shape class: short kernels get the deepest slab ring, wide kernels share one weight stage between four taps
     assert _plan(h, 16, 64768, 128, 128, 3)[1]["SA"] == 5 and _plan(h, 16, 64768, 128, 128, 11, 5)[1]["TPS"] == 4
-    assert _plan(h, 16, 1012, 1024, 128, 1)[1]["MT"] == 1                       # half a wave of MT=2 items: smaller items
     # refused shapes: C_in % 16, N % 16, misaligned or oddly strided x, halo beyond the slab
     assert _plan(h, 1, 128, 24, 16, 1)[0] == -2 and _plan(h, 1, 128, 16, 24, 1)[0] == -2
     assert _plan(h, 1, 128, 16, 16, 1, x=0x1010)[0] == -2 and _plan(h, 1, 128, 16, 16, 1, x_row_stride=20)[0] == -2
@@ -109,8 +115,8 @@ def test_tcgen05_launch_plan_respects_the_hardware_limits():
 
 def test_fused_resblock_plan_respects_the_hardware_limits():
     """fs2_resstack_plan (pure host logic) over the shipped generator's kernel / dilation sets, every single-pair shape and a sweep of
-    lengths: the halo covers the receptive radius, the output boxes tile the work item exactly in whole swizzle atoms, shared memory and
-    TMEM stay inside the SM's budget, and the independent-tile mode is chosen exactly where it was measured to pay."""
+    lengths: the halo covers the receptive radius, the output boxes tile the work item exactly in whole swizzle atoms, and shared memory
+    and the consumer threads' accumulator + residual registers stay inside the SM's budget."""
     h = _lib.lib()
 
     def plan(C, N, ks, dils, B=16):
@@ -120,8 +126,8 @@ def test_fused_resblock_plan_respects_the_hardware_limits():
             for d, dv in enumerate(dils[j]):
                 a.dil[j][d] = dv
         out = (ctypes.c_int32 * 12)()
-        rc = h.fs2_resstack_plan(ctypes.byref(a), 148, out)
-        keys = ("MT", "H", "TILE", "items", "grid", "SB", "smem", "tmem_cols", "obox", "n_oboxes", "TPS", "indep")
+        rc = h.fs2_resstack_plan(ctypes.byref(a), 132, out)
+        keys = ("MT", "H", "TILE", "items", "grid", "SB", "smem", "regs", "obox", "n_oboxes", "TPS", "indep")
         return rc, dict(zip(keys, out))
 
     cases = [(C, N, (3, 7, 11), ((1, 3, 5),) * 3) for C in (32, 64) for N in (1, 50, 392, 1000, 129536, 259072)]
@@ -133,14 +139,10 @@ def test_fused_resblock_plan_respects_the_hardware_limits():
         radius = max(sum((k - 1) * d // 2 + (k - 1) // 2 for d in dd) for k, dd in zip(ks, dils))
         assert p["H"] >= radius and p["H"] % 4 == 0
         assert p["obox"] % 8 == 0 and 8 <= p["obox"] <= 256 and p["n_oboxes"] * p["obox"] == p["TILE"] and p["n_oboxes"] <= 12
-        if p["indep"]:
-            assert C == 32 and len(ks) == 1 and p["H"] <= 16 and p["obox"] == 128 - 2 * p["H"] and p["n_oboxes"] == p["MT"]
-        else:
-            assert p["TILE"] == p["MT"] * 128 - 2 * p["H"]
-        assert p["indep"] == int(C == 32 and len(ks) == 1 and (radius + 3) // 4 * 4 <= 16)
-        assert p["smem"] <= 227 * 1024 and 2 * p["MT"] * C <= p["tmem_cols"] <= 512
+        assert p["indep"] == 0 and p["TILE"] == p["MT"] * 128 - 2 * p["H"]
+        assert p["smem"] <= 227 * 1024 and p["regs"] == p["MT"] * C <= 128
         assert 2 <= p["SB"] <= 8 and p["TPS"] * 64 * C == 8192
-        assert p["items"] == 16 * -(-N // p["TILE"]) and p["grid"] == min(p["items"], 148)
+        assert p["items"] == 16 * -(-N // p["TILE"]) and p["grid"] == min(p["items"], 132)
     # refused: other widths, even kernels, taps reaching more than 32 rows outside a tile, table overflow
     assert plan(128, 1000, (3,), ((1,),))[0] == -2 and plan(32, 1000, (4,), ((1,),))[0] == -2
     assert plan(32, 1000, (11,), ((7,),))[0] == -2 and plan(32, 0, (3,), ((1,),))[0] == -1

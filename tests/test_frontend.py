@@ -2,7 +2,6 @@
 (dataset.py:149-198, synthesize.py:191-198, utils/tools.py:58-65), and its own host logic (bucketing, sharding, prefetch thread)."""
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -131,53 +130,52 @@ def test_device_batches_on_cuda_stage_through_pinned_slots(tmp_path):
         assert torch.equal(s_t, torch.from_numpy(spk)) and torch.equal(t_t, torch.from_numpy(texts)) and torch.equal(l_t, torch.from_numpy(lens))
 
 
-def test_against_the_reference_dataloader_on_its_shipped_val_files():
-    """The three `preprocessed_data/*/val.txt` files the reference ships (512 utterances each, English ARPAbet and Mandarin pinyin),
-    through the reference's own TextDataset + DataLoader(batch_size=8) + to_device, against TextBatches / device_batches and against
-    OUR TextDataset under the same stock DataLoader.  Runs in a subprocess: the reference's module names (`text`, `utils`, `dataset`)
-    must resolve to its tree."""
-    from oracle import ref_import
-    if not ref_import.available():
-        pytest.skip("reference tree not present")
-    code = r'''
-import sys, os
-sys.path.insert(0, %r)
-from oracle import ref_import
-ref_import._stub()
-REF = ref_import.REFERENCE_ROOT
-sys.path.insert(0, REF); os.chdir(REF)
-import numpy as np, torch, yaml
-from torch.utils.data import DataLoader
-from dataset import TextDataset as RefTextDataset
-from utils.tools import to_device
-from text import text_to_sequence
-from fastspeech2_b200 import frontend
-n = 0
-for ds_name in ("LJSpeech", "LibriTTS", "AISHELL3"):
-    pc = yaml.safe_load(open(f"config/{ds_name}/preprocess.yaml"))
-    src = os.path.join(pc["path"]["preprocessed_path"], "val.txt")
-    ref = RefTextDataset(src, pc)
-    want = list(DataLoader(ref, batch_size=8, collate_fn=ref.collate_fn))
-    ours_ds = frontend.TextDataset(src, pc)                      # default text_to_sequence: the tree's own `text` package
-    via_loader = list(DataLoader(ours_ds, batch_size=8, collate_fn=ours_ds.collate_fn))
-    tb = frontend.TextBatches(src, pc, batch_size=8, text_to_sequence=text_to_sequence)
-    direct, dev = list(tb), list(tb.device_batches("cpu"))
-    assert len(want) == len(via_loader) == len(direct) == len(dev) == 64
-    for w, a, b, d in zip(want, via_loader, direct, dev):
-        for got in (a, b):
-            assert got[0] == w[0] and got[1] == w[1] and got[5] == w[5] and type(got[5]) is type(w[5])
-            for i in (2, 3, 4):
-                assert got[i].dtype == w[i].dtype and got[i].shape == w[i].shape and np.array_equal(got[i], w[i]), (ds_name, i)
-        wd = to_device(w, torch.device("cpu"))
-        assert d[0] == wd[0] and d[1] == wd[1] and d[5] == wd[5]
-        for i in (2, 3, 4):
-            assert d[i].dtype == wd[i].dtype and torch.equal(d[i], wd[i])
-        n += len(w[0])
-    item_r, item_o = ref[5], ours_ds[5]
-    assert item_r[0] == item_o[0] and item_r[1] == item_o[1] and np.array_equal(item_r[2], item_o[2]) and item_r[3] == item_o[3]
-    print(ds_name, "padding", round(tb.padded_fraction(), 3), "->", round(frontend.TextBatches(src, pc, batch_size=8, bucket=True, text_to_sequence=text_to_sequence).padded_fraction(), 3))
-print("compared", n)
-''' % ROOT
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "compared 1536" in r.stdout, r.stdout + r.stderr
-    print(r.stdout)
+def test_against_the_reference_dataloader_on_its_shipped_val_files(tmp_path):
+    """The three `preprocessed_data/*/val.txt` files the reference ships (512 utterances each, English ARPAbet and Mandarin pinyin) and
+    the batches the reference's own TextDataset + DataLoader(batch_size=8) + to_device made of them (tests/golden/
+    frontend_reference_batches.npz, oracle/gen_golden.py --frontend), against TextBatches / device_batches and against OUR TextDataset
+    under the same stock DataLoader.  text_to_sequence is replayed from the reference's recorded sequences of every line."""
+    import torch
+    from torch.utils.data import DataLoader
+    z = np.load(os.path.join(ROOT, "tests", "golden", "frontend_reference_batches.npz"))
+    n = 0
+    for ds in ("LJSpeech", "LibriTTS", "AISHELL3"):
+        meta = json.loads(z[f"{ds}__meta"].tobytes().decode("utf-8"))
+        pre = tmp_path / ds
+        pre.mkdir()
+        src = pre / "val.txt"
+        src.write_bytes(z[f"{ds}__val"].tobytes())
+        (pre / "speakers.json").write_bytes(z[f"{ds}__speakers"].tobytes())
+        cleaners = meta["cleaners"]
+        pc = {"preprocessing": {"text": {"text_cleaners": cleaners}}, "path": {"preprocessed_path": str(pre)}}
+        lines = src.read_text(encoding="utf-8").splitlines()
+        seqs = np.split(z[f"{ds}__seq"], np.cumsum(z[f"{ds}__seq_len"])[:-1])
+        table = {}
+        for line, s in zip(lines, seqs):
+            assert table.setdefault(line.split("|")[2], s.tolist()) == s.tolist()
+
+        def t2s(text, cl):
+            assert cl == cleaners
+            return table[text]
+
+        want = [(b["ids"], b["raw"], z[f"{ds}__b{i}__spk"], z[f"{ds}__b{i}__texts"], z[f"{ds}__b{i}__lens"], b["max"])
+                for i, b in enumerate(meta["batches"])]
+        ours_ds = frontend.TextDataset(str(src), pc, text_to_sequence=t2s)
+        via_loader = list(DataLoader(ours_ds, batch_size=8, collate_fn=ours_ds.collate_fn))
+        tb = frontend.TextBatches(str(src), pc, batch_size=8, text_to_sequence=t2s)
+        direct, dev = list(tb), list(tb.device_batches("cpu"))
+        assert len(want) == len(via_loader) == len(direct) == len(dev) == 64
+        for w, b, a, c, d in zip(want, meta["batches"], via_loader, direct, dev):
+            for got in (a, c):
+                assert got[0] == w[0] and got[1] == w[1] and got[5] == w[5] and type(got[5]).__name__ == b["max_type"]
+                for i in (2, 3, 4):
+                    assert got[i].dtype == w[i].dtype and got[i].shape == w[i].shape and np.array_equal(got[i], w[i]), (ds, i)
+            # the reference's to_device (utils/tools.py:58-65): speakers / texts .long(), lengths as they are
+            wd = (torch.from_numpy(w[2]).long(), torch.from_numpy(w[3]).long(), torch.from_numpy(w[4]))
+            assert d[0] == w[0] and d[1] == w[1] and d[5] == w[5]
+            for i, x in zip((2, 3, 4), wd):
+                assert d[i].dtype == x.dtype and torch.equal(d[i], x)
+            n += len(w[0])
+        item = ours_ds[5]
+        assert [item[0], item[1], item[3]] == meta["item5"] and np.array_equal(item[2], seqs[5])
+    assert n == 1536

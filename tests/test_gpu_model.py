@@ -114,7 +114,7 @@ def test_fastspeech2_ragged_multispeaker_long(libri_configs, parity_log):
 def test_fastspeech2_full_size_vs_oracle(libri_configs, parity_log):
     """BASELINE.json configs[3] at FULL size (LibriTTS multi-speaker, B = 64, mixed 64-256 phonemes with padding masks, Tmax ~ 2000)
     against the CPU oracle on the whole batch (tens of seconds of ATen on the box's cores): decisions exact, mel within the bar,
-    padded rows follow the reference's padding semantics.  Exercises MT = 4 tiles, Tk > 1000 attention and the long position table."""
+    padded rows follow the reference's padding semantics.  Exercises many 128-row tiles per utterance, Tk > 1000 attention and the long position table."""
     pc, mc = libri_configs
     sd = synth.fastspeech2_state_dict(pc, mc, seed=21)
     m = FastSpeech2(pc, mc); m.load_state_dict(sd); m = m.to(DEV).eval()
@@ -137,7 +137,7 @@ def test_fastspeech2_config4_shard_vs_oracle(lj_configs, parity_log):
 
 @pytest.mark.parametrize("cfg", ["lj", "libri"])
 def test_fastspeech2_tensor_core_encoder_and_predictors(cfg, lj_configs, libri_configs, parity_log):
-    """Both settings of FS2_TC_ENCODER | FS2_TC_PREDICTORS (default: set): encoder FFT blocks and the three variance predictors on tcgen05, K-SEGMENTED (every
+    """Both settings of FS2_TC_ENCODER | FS2_TC_PREDICTORS (default: set): encoder FFT blocks and the three variance predictors on tensor-core, K-SEGMENTED (every
     (tap, 256-channel) slice its own 16-step accumulation, slices summed in fp32 by the epilogue) so that the truncating tensor-core
     accumulator cannot move the discrete decisions more than the fp32 kernels do.  Same flip-aware protocol as the full-size tests."""
     from fastspeech2_b200 import _lib as L
@@ -283,7 +283,7 @@ def test_hifigan_vs_oracle(B, T, parity_log):
 def test_hifigan_full_size_vs_oracle(B, parity_log):
     """BASELINE.json configs[2] (B = 16) and one GPU's shard of configs[4] (B = 64): the vocoder at FULL size (x 1012 frames ->
     259072 samples per utterance).  Generator rows are independent (no cross-utterance op), so the CPU oracle is run on the first
-    and last utterance of the batch and compared with those rows of the GPU result: tile indexing, MT = 4 work items and the
+    and last utterance of the batch and compared with those rows of the GPU result: tile indexing, the resstack slabs and the
     batch strides are exercised at the benchmarked shape while the check stays a few seconds of CPU."""
     gen, sd = _generator(seed=5)
     mel = synth.make_mel(B, 1012, seed=6)

@@ -53,16 +53,16 @@ def test_conv1d(case):
 
 
 TC_CASES = [
-    # B, T, Cin, N, taps, dil, pad, in_act, out_act, res, alpha, accumulate, lens      (tcgen05 split-FP16 kernel, backend = 2)
-    (1, 128, 16, 128, 1, 1, 0, 0, 0, False, 1.0, False, False),      # one tile, one K-block (MT = 1)
-    (2, 300, 64, 128, 3, 1, 1, 0, 0, False, 1.0, False, False),      # ragged tail tile (MT = 2)
+    # B, T, Cin, N, taps, dil, pad, in_act, out_act, res, alpha, accumulate, lens      (tensor-core split-FP16 kernel, backend = 2)
+    (1, 128, 16, 128, 1, 1, 0, 0, 0, False, 1.0, False, False),      # one tile, one K-block
+    (2, 300, 64, 128, 3, 1, 1, 0, 0, False, 1.0, False, False),      # ragged tail tile
     (2, 700, 128, 128, 11, 5, 25, 3, 3, True, 1.0, False, False),    # HiFi-GAN stage-1 conv1 shape: dilation 5, lrelu in/out
     (2, 520, 256, 256, 7, 1, 3, 0, 0, True, 1.0 / 3, True, False),   # two N-blocks, residual + scaled accumulate
     (2, 333, 512, 80, 5, 1, 2, 0, 0, True, 1.0, False, False),       # PostNet last conv: N = 80 (16-column tail block)
     (2, 260, 256, 1024, 9, 1, 4, 0, 1, False, 1.0, False, False),    # conv-FFN w_1 + ReLU, 8 N-blocks
     (3, 200, 1024, 256, 1, 1, 0, 0, 0, True, 1.0, False, True),      # conv-FFN w_2 + residual + pad-row mask
-    (2, 1500, 32, 32, 3, 3, 3, 3, 3, False, 1.0, False, False),      # 32 channels: MT = 4, two accumulator groups
-    (2, 777, 64, 64, 7, 1, 3, 3, 0, True, 1.0, False, False),        # 64 channels: MT = 4
+    (2, 1500, 32, 32, 3, 3, 3, 3, 3, False, 1.0, False, False),      # 32 channels: two accumulator groups
+    (2, 777, 64, 64, 7, 1, 3, 3, 0, True, 1.0, False, False),        # 64 channels: two accumulator groups
     (2, 150, 80, 512, 7, 1, 3, 0, 0, False, 1.0, False, False),      # conv_pre: C_in = 80
     (2, 257, 64, 64, 2, 1, 1, 3, 0, False, 1.0, False, False),       # ConvTranspose phase group (2 taps)
     (1, 40, 256, 80, 1, 1, 0, 0, 2, False, 1.0, False, False),       # short sequence, tanh epilogue
@@ -71,7 +71,7 @@ TC_CASES = [
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv1d_tensor_core(case):
-    """fs2_conv1d through the tcgen05 kernel against an fp64 evaluation of the same contract.  Error budget: the split
+    """fs2_conv1d through the tensor-core kernel against an fp64 evaluation of the same contract.  Error budget: the split
     keeps 22 bits; what remains is the tensor core's truncating fp32 accumulator (~0.5 ulp per K=16 step)."""
     B, T, Cin, N, taps, dil, pad, in_act, out_act, use_res, alpha, acc, use_lens = case
     x = rnd(B, T, Cin, seed=1)
@@ -243,7 +243,7 @@ def test_resstack_single_pair_accumulate(C, k, dils, N):
 
 
 def test_conv1d_tensor_core_alignment_contract():
-    """The tcgen05 kernel reads activations with 256-bit loads: a 16-byte-but-not-32-byte aligned x is refused by the explicit
+    """The tensor-core kernel reads activations with 256-bit loads: a 16-byte-but-not-32-byte aligned x is refused by the explicit
     backend and silently served by the exact fp32 kernel under FS2_CONV_AUTO (same contract, fp32 accuracy)."""
     from fastspeech2_b200._lib import Fs2Error
     B, T, Cin, N = 2, 200, 64, 64
@@ -323,7 +323,7 @@ def test_attention(T, lens):
 
 @pytest.mark.parametrize("T,lens", [(300, [300, 129, 1]), (1000, [1000, 777, 513]), (1100, [1100, 64, 1037])])
 def test_attention_tensor_core_path(T, lens):
-    """S = QK^T / PV as split-FP16 tcgen05 GEMMs + row softmax (decoder path): fp32-class accuracy expected."""
+    """S = QK^T / PV as split-FP16 tensor-core GEMMs + row softmax (decoder path): fp32-class accuracy expected."""
     qkv = rnd(3, T, 768, seed=2)
     kl = torch.tensor(lens, dtype=torch.int32)
     want = E.attention(qkv.double(), 2, kl)
@@ -337,7 +337,7 @@ def test_attention_tensor_core_path(T, lens):
 
 @pytest.mark.parametrize("T,lens", [(128, [128, 5, 77]), (300, [300, 129, 1]), (1017, [1017, 777, 513]), (1100, [1100, 64, 1037]), (4200, [4200, 4097, 9])])
 def test_attention_fused_kernel(T, lens):
-    """fs2_attention backend 2: QK^T, softmax and PV in ONE tcgen05 kernel (scores stay in tensor memory; two-pass softmax; no length
+    """fs2_attention backend 2: QK^T, softmax and PV in ONE tensor-core kernel (scores stay in registers; two-pass softmax; no length
     limit) against an fp64 evaluation of transformer/Modules.py:14-25 with the key mask of Models.py:79.  Same budget as the GEMM path."""
     qkv = rnd(3, T, 768, seed=3)
     kl = torch.tensor(lens, dtype=torch.int32)

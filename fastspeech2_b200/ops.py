@@ -39,12 +39,13 @@ def conv1d(x, w, bias=None, *, dilation=1, pad_left=0, in_act=L.ACT_NONE, in_slo
     return out
 
 
-def layernorm(x, gamma, beta, row_lens=None, eps=1e-5):
+def layernorm(x, gamma, beta, row_lens=None, eps=1e-5, pre_relu=False):
+    """LayerNorm over the last dim of x (or of relu(x) with pre_relu), rows t >= row_lens[b] zeroed."""
     _need_cuda(x)
     B, T, Cc = x.shape
     y = torch.empty_like(x)
     a = L.LayerNormArgs(x=x.data_ptr(), y=y.data_ptr(), B=B, T=T, C=Cc, gamma=gamma.data_ptr(), beta=beta.data_ptr(), eps=eps,
-                        row_lens=L.ptr(row_lens))
+                        row_lens=L.ptr(row_lens), pre_relu=int(pre_relu))
     L.check(L.lib().fs2_layernorm(C.byref(a), _stream(x.device)), "fs2_layernorm")
     return y
 
@@ -72,6 +73,15 @@ def embed_positions(ids, table, pos):
                     n_vocab=table.shape[0])
     L.check(L.lib().fs2_embed_positions(C.byref(a), _stream(ids.device)), "fs2_embed_positions")
     return y
+
+
+def add_positions_(x, pos):
+    """x[b,t,:] += pos[t,:] in place (fs2_add_positions); x contiguous [B,T,D], pos [>= T, D]."""
+    _need_cuda(x)
+    B, T, D = x.shape
+    assert x.is_contiguous() and pos.is_contiguous() and pos.shape[0] >= T and pos.shape[1] == D
+    L.check(L.lib().fs2_add_positions(x.data_ptr(), pos.data_ptr(), B, T, D, _stream(x.device)), "fs2_add_positions")
+    return x
 
 
 def add_speaker_(x, table, idx):

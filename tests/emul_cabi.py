@@ -54,6 +54,49 @@ def conv1d_epilogue(acc, bias, out_act=ACT_NONE, out_slope=0.0, res=None, alpha=
     return v
 
 
+def f8_operands(x, w, in_act=ACT_NONE, in_slope=0.0):
+    """The operands the f16 + f8 tensor-core kernel multiplies, evaluated exactly: returns (a_hi, w_hi, a_lo8, w_hi8, a_hi8, w_lo8, scale)
+    in fp64 so that  y*scale = a_hi.w_hi + a_lo8.w_hi8 + a_hi8.w_lo8  (conv_tc_kernel.cuh::tc_convert_store, packing.pack_conv_tc)."""
+    from fastspeech2_b200 import packing
+    e4 = lambda t: t.float().clamp(-448, 448).to(torch.float8_e4m3fn).double()
+    a = x.float()
+    if in_act == ACT_LRELU:
+        a = torch.maximum(a, a * in_slope)
+    ah = a.half().float()
+    al = a - ah
+    hi, _, s = packing.split_fp16(w)
+    wl = w.float() * s - hi.float()
+    return (ah.double(), hi.double(), e4(al * 4096.0) / 4096.0, e4(hi.float() * 2.0 ** -12) * 4096.0, e4(ah), e4(wl), s)
+
+
+def conv1d_f8(x, w, bias, dilation=1, pad_left=0, in_act=ACT_NONE, in_slope=0.0, out_act=ACT_NONE, out_slope=0.0,
+              res=None, alpha=1.0, y_prev=None, row_lens=None, fp16_only=False):
+    """fs2_conv1d with the f16 + f8 tile format (FS2_TC_VARIANT_F8) in fp64 on the rounded operands: what the kernel computes up to
+    its fp32 accumulation.  x is rounded to fp32 first, as the kernel reads it.  fp16_only: drop the E4M3 correction term (a
+    single-pass fp16 convolution), the error a kernel that lost the correction would make."""
+    ah, wh, al8, wh8, ah8, wl8, s = f8_operands(x, w, in_act, in_slope)
+    lin = lambda a_, w_: conv1d(a_, w_, None, dilation, pad_left)
+    pre = lin(ah, wh) if fp16_only else lin(ah, wh) + lin(al8, wh8) + lin(ah8, wl8)
+    d = lambda t: None if t is None else t.double()
+    return conv1d_epilogue(pre / s, d(bias), out_act, out_slope, d(res), alpha, d(y_prev), row_lens)
+
+
+def resblock_group(x, kernels, dils, w1, b1, w2, b2, conv=conv1d):
+    """fs2_resstack as the per-layer calls of model.cu's unfused vocoder path:  r <- conv2(conv1(r, lrelu in / out) ) + r  per
+    dilation, the last conv of each kernel size scaled by 1/n_kernels and accumulated into the sum.  w1 / w2 [j][d]: [k][C][C]."""
+    nk = len(kernels)
+    xs = None
+    for j, k in enumerate(kernels):
+        r = x
+        for d, dv in enumerate(dils[j]):
+            t = conv(r, w1[j][d], b1[j][d], dv, (k - 1) * dv // 2, ACT_LRELU, 0.1, ACT_LRELU, 0.1)
+            last = d == len(dils[j]) - 1
+            r = conv(t, w2[j][d], b2[j][d], 1, (k - 1) // 2, res=r, alpha=1.0 / nk if last else 1.0,
+                     y_prev=xs if last and j > 0 else None)
+        xs = r
+    return xs
+
+
 def layernorm(x, g, b, row_lens=None):
     y = torch.nn.functional.layer_norm(x, (x.shape[-1],), g, b, 1e-5)
     if row_lens is not None:

@@ -60,9 +60,10 @@ def test_host_side_argument_checks_need_no_gpu():
     assert h.fs2_resstack(ctypes.byref(r), None) == -1           # misaligned y
 
 
-def _plan(h, B, T, Cin, N, taps, dil=1, num_sms=132, x=0x1000, x_row_stride=None):
+def _plan(h, B, T, Cin, N, taps, dil=1, num_sms=132, x=0x1000, x_row_stride=None, tc_variant=0):
     a = _lib.Conv1dArgs(x=x, x_batch_stride=T * (x_row_stride or Cin), x_row_stride=x_row_stride or Cin, B=B, T=T, Cin=Cin, w=0x1000, N=N, taps=taps,
-                        dilation=dil, pad_left=(taps - 1) * dil // 2, w_tc=0x1000, y=0x1000, y_batch_stride=T * N, y_row_stride=N, alpha=1.0)
+                        dilation=dil, pad_left=(taps - 1) * dil // 2, w_tc=0x1000, y=0x1000, y_batch_stride=T * N, y_row_stride=N, alpha=1.0,
+                        tc_variant=tc_variant)
     out = (ctypes.c_int32 * 12)()
     rc = h.fs2_conv_tc_plan(ctypes.byref(a), num_sms, out)
     keys = ("NB", "MT", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")
@@ -113,23 +114,66 @@ def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
     assert _plan(h, 1, 4096, 16, 16, 11, 30)[0] == -2
 
 
+def _rs_plan(C, N, ks, dils, B=16):
+    a = _lib.ResstackArgs(B=B, N=N, C=C, n_kernels=len(ks), n_dil=len(dils[0]))
+    for j, k in enumerate(ks):
+        a.k[j] = k
+        for d, dv in enumerate(dils[j]):
+            a.dil[j][d] = dv
+    out = (ctypes.c_int32 * 12)()
+    rc = _lib.lib().fs2_resstack_plan(ctypes.byref(a), 132, out)
+    keys = ("MT", "H", "TILE", "items", "grid", "SB", "smem", "regs", "obox", "n_oboxes", "TPS", "indep")
+    return rc, dict(zip(keys, out))
+
+
+def test_gpu_case_tables_reach_every_tile_width_and_the_persistent_loop():
+    """The GPU op tests (tests/test_gpu_ops.py) launch every work-item width the conv dispatcher instantiates in both tile formats, give
+    every CTA of a 132-SM grid at least two work items (some cases four) in each format, sit at the limits of the conv halo and of the
+    ResBlock kernel's reach, and put the ResBlock group at one tile +- 1 row.  Checked here, without a GPU, so that a later edit cannot
+    quietly shrink those tables."""
+    from fastspeech2_b200 import packing
+    from tests import test_gpu_ops as G
+    h = _lib.lib()
+    # every NB: split3 {16, ..., 128}, f8 {16, 32, 48, 64}
+    assert {packing.conv_tc_block(c[3]) for c in G.TC_CASES} == set(range(16, 129, 16))
+    assert {packing.conv_tc_block(c[3], 64) for c in G.TC_CASES} == {16, 32, 48, 64}
+    # the persistent loop: >= 2 work items per CTA at 132 SMs in every format, >= 4 in at least one case of each
+    tables = {0: G.TC_PERSISTENT_CASES, _lib.TC_VARIANT_F8: G.TC_PERSISTENT_CASES,
+              _lib.TC_VARIANT_NB64 | _lib.TC_VARIANT_SEGMENTED: [(B, T, Cin, N, taps, 1) for B, T, Cin, N, taps, *_ in G.SEG_PERSISTENT_CASES]}
+    for variant, cases in tables.items():
+        items = []
+        for B, T, Cin, N, taps, dil, *_ in cases:
+            rc, p = _plan(h, B, T, Cin, N, taps, dil, tc_variant=variant)
+            assert rc == 0 and p["grid"] == 132, (variant, B, T, Cin, N)
+            items.append(p["n_items"])
+        assert min(items) >= 2 * 132 and max(items) >= 4 * 132, (variant, items)
+    assert len(G.TC_PERSISTENT_CASES) >= 5 and len(G.SEG_PERSISTENT_CASES) >= 3
+    assert all(c in G.TC_CASES for c in G.TC_PERSISTENT_CASES) and all(c in G.SEG_CASES for c in G.SEG_PERSISTENT_CASES)
+    assert any(B * 2 * -(-T // 128) >= 2 * 132 for T, lens in G.ATT_BATCHED_CASES for B in [len(lens)])     # fused attention items
+    # conv halo (taps - 1) * dilation: 256 is planned (both 2 x 256 and 3 x 128 are in the table), 257 is refused
+    halos = {(c[4], c[5]) for c in G.TC_CASES if (c[4] - 1) * c[5] == 256}
+    assert {(2, 256), (3, 128)} <= halos
+    assert {c[6] for c in G.TC_CASES if (c[4] - 1) * c[5] == 256} >= {0, 128, 256}                 # pad_left 0, centred, = halo
+    for taps, dil in halos:
+        assert _plan(h, 2, 700, 32, 64, taps, dil)[0] == 0
+    assert _plan(h, 2, 700, 32, 64, 2, 257)[0] == -2 and _plan(h, 2, 700, 32, 64, 3, 129)[0] == -2
+    # ResBlock: the tile of the shipped group, and single pairs whose taps reach exactly 32 rows (33 is refused)
+    ship_k, ship_d = (3, 7, 11), ((1, 3, 5),) * 3
+    for C, tile in G.RESSTACK_TILE.items():
+        assert _rs_plan(C, 1000, ship_k, ship_d)[1]["TILE"] == tile
+        assert {N for _, N, c, k, d in G.RESSTACK_CASES if c == C and k == ship_k and d == ship_d} >= {1, tile - 1, tile + 1}
+    reach32 = {(C, k) for C, k, dils, N in G.SINGLE_PAIR_CASES if max((k - 1) * d // 2 for d in dils) == 32}
+    assert reach32 == {(C, k) for C in (32, 64) for k in (3, 5, 9)}
+    for C, k in reach32:
+        assert _rs_plan(C, 1000, (k,), ((64 // (k - 1),),))[0] == 0
+    assert _rs_plan(32, 1000, (3,), ((33,),))[0] == -2
+
+
 def test_fused_resblock_plan_respects_the_hardware_limits():
     """fs2_resstack_plan (pure host logic) over the shipped generator's kernel / dilation sets, every single-pair shape and a sweep of
     lengths: the halo covers the receptive radius, the output boxes tile the work item exactly in whole swizzle atoms, and shared memory
     and the consumer threads' accumulator + residual registers stay inside the SM's budget."""
-    h = _lib.lib()
-
-    def plan(C, N, ks, dils, B=16):
-        a = _lib.ResstackArgs(B=B, N=N, C=C, n_kernels=len(ks), n_dil=len(dils[0]))
-        for j, k in enumerate(ks):
-            a.k[j] = k
-            for d, dv in enumerate(dils[j]):
-                a.dil[j][d] = dv
-        out = (ctypes.c_int32 * 12)()
-        rc = h.fs2_resstack_plan(ctypes.byref(a), 132, out)
-        keys = ("MT", "H", "TILE", "items", "grid", "SB", "smem", "regs", "obox", "n_oboxes", "TPS", "indep")
-        return rc, dict(zip(keys, out))
-
+    plan = _rs_plan
     cases = [(C, N, (3, 7, 11), ((1, 3, 5),) * 3) for C in (32, 64) for N in (1, 50, 392, 1000, 129536, 259072)]
     cases += [(C, N, (k,), ((d,),)) for C in (32, 64) for N in (40, 1000, 259072) for k in (3, 5, 7, 11) for d in (1, 3, 5)]
     cases += [(C, 5000, (3,), ((1, 3, 5),)) for C in (32, 64)] + [(64, 50, (3, 5), ((1, 2), (2, 6)))]

@@ -11,13 +11,12 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfs2b200.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 MAX_LAYERS, MAX_POSTNET, MAX_STAGES, MAX_RESBLOCKS, MAX_DIL = 12, 8, 8, 32, 4
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_LRELU = 0, 1, 2, 3
 CONV_AUTO, CONV_SIMT, CONV_TC = 0, 1, 2
 TC_ENCODER, TC_PREDICTORS, TC_DECODER, TC_POSTNET = 1, 2, 4, 8
 TC_DECODER_F8, TC_POSTNET_F8 = 16, 32
-TC_ATTENTION_GEMM = 64
 TC_VARIANT_F8 = 1
 TC_VARIANT_NB64 = 2
 TC_VARIANT_SEGMENTED = 4

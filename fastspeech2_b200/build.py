@@ -1,7 +1,6 @@
 """Compile the CUDA sources under csrc/ into fastspeech2_b200/libfs2b200.so for the H100 (sm_90a), next to the Python package.
 
 Each .cu is compiled to an object in parallel (build/obj/, git-ignored) and the objects are linked with nvcc --shared.
-FS2_DEBUG_KNOBS=1 compiles the fs2_debug_set_* tuning knobs that scripts/tc_*.py use (the shipped library has none).
 """
 from __future__ import annotations
 
@@ -17,8 +16,7 @@ LIB = os.path.join(HERE, "libfs2b200.so")
 OBJ = os.path.join(ROOT, "build", "obj")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
-FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include")] \
-        + (["-DFS2_DEBUG_KNOBS"] if os.environ.get("FS2_DEBUG_KNOBS") == "1" else [])
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include")]
 
 
 def sources():

@@ -1,9 +1,10 @@
 // Fused self-attention of one FFT block on the tensor cores (transformer/Modules.py:14-25 + key mask Models.py:79, heads as
 // SubLayers.py:39-44): S = Q K^T, softmax and O = P V in ONE persistent wgmma kernel -- the score matrix lives in registers and
-// never reaches HBM (the GEMM path of attention_tc.cu materialises S [B*H][T][Tk] in fp32: 535 MB per layer at B = 64).
+// never reaches HBM (the reference writes S [2B][T][T] in fp32 four times).
 //
-//   work item = (utterance b, head h, 128 query rows); K and V come as the per-utterance operand tiles that pack_k/v_tiles_kernel
-//   (attention_tc.cu) write once per layer (fp16 hi/lo, three-MMA split: attention keeps fp32-class operands).
+//   pack_kv_tiles_kernel, once per layer: K and V of every (utterance, head) -> fp16 hi/lo operand tiles (three-MMA split: attention
+//   keeps fp32-class operands), one bulk-copy stage per 16 rows of the MMA's K dimension.
+//   work item = (utterance b, head h, 128 query rows).
 //   pass 1: for every block of 128 keys  S = Q K_j^T (register accumulators)  ->  row maximum (a row's columns are spread over the
 //           four lanes of a quad: two shuffles).
 //   pass 2: S again -> p = exp2(s*c - m) (keys >= key_len masked to 0) -> fp16 hi/lo operand planes in shared memory ->
@@ -17,12 +18,96 @@
 
 namespace fs2 {
 
-int pack_kv_tiles(const fs2_attention_args* a, unsigned char* kt, unsigned char* vt, long long tstride, cudaStream_t s);   // attention_tc.cu
-
 constexpr int AF_THREADS = 288;
 constexpr int AF_SB = 8;                         // K / V stage ring depth
 constexpr uint32_t AF_STAGE = 8192;              // one stage: [hi | lo][2 chunks][128][16 B]
-constexpr float AF_WSCALE = 16.f;                // operand scale of the packed K / V tiles (attention_tc.cu::AT_WSCALE)
+constexpr float AF_WSCALE = 16.f;                // power-of-two operand scale of the packed K / V tiles (|k|, |v| < 4094 stay inside fp16)
+
+// ------------------------------------------------------------------ K / V operand tiles
+// Per (utterance, head) one buffer of af_tile_stride(Tk) bytes: TC_HDR header (float 1 / AF_WSCALE), then the stages; keys are padded
+// to Tk, a multiple of 128, with zeros.
+__device__ __forceinline__ void split8(const float (&f)[8], float scale, uint4& hi, uint4& lo) {
+  uint32_t hw[4], lw[4];
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    const float a0 = fminf(fmaxf(f[2 * j] * scale, -65504.f), 65504.f);
+    const float a1 = fminf(fmaxf(f[2 * j + 1] * scale, -65504.f), 65504.f);
+    const __half2 h2 = __floats2half2_rn(a0, a1);
+    const float2 hf = __half22float2(h2);
+    const __half2 l2 = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
+    hw[j] = *reinterpret_cast<const uint32_t*>(&h2);
+    lw[j] = *reinterpret_cast<const uint32_t*>(&l2);
+  }
+  hi = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+  lo = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+}
+
+// K tiles: B operand W[c = d][n = key] of S = Q K^T, layout  header | [key/128][d/16][hi|lo][2 chunks][128 keys][8 halfs]
+__device__ __forceinline__ void pack_k_tiles(const float* __restrict__ qkv, unsigned char* __restrict__ tiles, int B, int T, int Tk, int H,
+                                             long long tile_stride, long long idx) {   // idx = (bh, key, dchunk)
+  const long long total = (long long)B * H * Tk * (128 / 8);
+  if (idx >= total) return;
+  const int dchunk = (int)(idx % (128 / 8));
+  const long long r = idx / (128 / 8);
+  const int key = (int)(r % Tk);
+  const int bh = (int)(r / Tk);
+  const int b = bh / H, h = bh - b * H;
+  const int D = H * 128;
+  float f[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) f[j] = 0.f;
+  if (key < T) {
+    const float4* src = reinterpret_cast<const float4*>(qkv + ((long long)b * T + key) * 3 * D + D + h * 128 + dchunk * 8);
+    const float4 u = __ldg(src), v = __ldg(src + 1);
+    f[0] = u.x; f[1] = u.y; f[2] = u.z; f[3] = u.w; f[4] = v.x; f[5] = v.y; f[6] = v.z; f[7] = v.w;
+  }
+  uint4 hi, lo;
+  split8(f, AF_WSCALE, hi, lo);
+  unsigned char* base = tiles + (long long)bh * tile_stride;
+  if (key == 0 && dchunk == 0) *reinterpret_cast<float*>(base) = 1.f / AF_WSCALE;
+  const int nblk = key / 128, nn = key - nblk * 128, kb = dchunk >> 1, chunk = dchunk & 1;
+  const size_t b_plane = AF_STAGE / 2, kbl = 128 / 16;
+  unsigned char* dst = base + TC_HDR + ((size_t)nblk * kbl + kb) * AF_STAGE + ((size_t)chunk * 128 + nn) * 16;
+  *reinterpret_cast<uint4*>(dst) = hi;
+  *reinterpret_cast<uint4*>(dst + b_plane) = lo;
+}
+
+// V tiles: B operand W[c = key][n = d] of O = P V, layout  header | [key/16][hi|lo][2 chunks of 8 keys][128 d][8 halfs (keys)]
+__device__ __forceinline__ void pack_v_tiles(const float* __restrict__ qkv, unsigned char* __restrict__ tiles, int B, int T, int Tk, int H,
+                                             long long tile_stride, long long idx) {   // idx = (bh, key8, d)
+  const long long total = (long long)B * H * (Tk / 8) * 128;
+  if (idx >= total) return;
+  const int d = (int)(idx % 128);
+  const long long r = idx / 128;
+  const int k8 = (int)(r % (Tk / 8));
+  const int bh = (int)(r / (Tk / 8));
+  const int b = bh / H, h = bh - b * H;
+  const int D = H * 128;
+  float f[8];
+#pragma unroll
+  for (int e = 0; e < 8; e++) {
+    const int key = k8 * 8 + e;
+    f[e] = key < T ? __ldg(qkv + ((long long)b * T + key) * 3 * D + 2 * D + h * 128 + d) : 0.f;
+  }
+  uint4 hi, lo;
+  split8(f, AF_WSCALE, hi, lo);
+  unsigned char* base = tiles + (long long)bh * tile_stride;
+  if (k8 == 0 && d == 0) *reinterpret_cast<float*>(base) = 1.f / AF_WSCALE;
+  const int kb = k8 >> 1, chunk = k8 & 1;
+  const size_t b_plane = AF_STAGE / 2;
+  unsigned char* dst = base + TC_HDR + (size_t)kb * AF_STAGE + ((size_t)chunk * 128 + d) * 16;
+  *reinterpret_cast<uint4*>(dst) = hi;
+  *reinterpret_cast<uint4*>(dst + b_plane) = lo;
+}
+
+// One launch writes both operand-tile sets: blocks [0, k_blocks) the K tiles, the rest the V tiles.
+__global__ void pack_kv_tiles_kernel(const float* __restrict__ qkv, unsigned char* __restrict__ kt, unsigned char* __restrict__ vt, int B, int T,
+                                     int Tk, int H, long long tile_stride, unsigned k_blocks) {
+  if (blockIdx.x < k_blocks) pack_k_tiles(qkv, kt, B, T, Tk, H, tile_stride, (long long)blockIdx.x * blockDim.x + threadIdx.x);
+  else pack_v_tiles(qkv, vt, B, T, Tk, H, tile_stride, (long long)(blockIdx.x - k_blocks) * blockDim.x + threadIdx.x);
+}
+
+// ------------------------------------------------------------------ attention kernel
 
 struct AfP {
   const float* qkv; float* ctx;
@@ -270,7 +355,14 @@ int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cuda
   const size_t tile_bytes = ((size_t)a->B * a->H * tstride + 255) & ~(size_t)255;
   unsigned char* kt = reinterpret_cast<unsigned char*>(base);
   unsigned char* vt = kt + tile_bytes;
-  FS2_TRY(pack_kv_tiles(a, kt, vt, tstride, s));
+  {
+    const long long nk = (long long)a->B * a->H * Tk * (128 / 8), nv = (long long)a->B * a->H * (Tk / 8) * 128;
+    const unsigned kb = (unsigned)((nk + 255) / 256), vb = (unsigned)((nv + 255) / 256);
+    prof_before(s);
+    pack_kv_tiles_kernel<<<kb + vb, 256, 0, s>>>(a->qkv, kt, vt, a->B, a->T, Tk, a->H, tstride, kb);
+    prof_after(s, 1, 0.0);
+    FS2_LAUNCH_CHECK();
+  }
   AfP p{};
   p.qkv = a->qkv; p.ctx = a->ctx; p.kt = kt; p.vt = vt; p.tstride = tstride;
   p.B = a->B; p.T = a->T; p.H = a->H; p.Tk = Tk; p.key_lens = a->key_lens; p.scale = a->scale;

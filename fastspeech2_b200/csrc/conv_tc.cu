@@ -27,15 +27,6 @@ bool conv_tc_supported(const fs2_conv1d_args* a) {
   return true;
 }
 
-#ifdef FS2_DEBUG_KNOBS
-int g_tc_pdl = 0;                  // programmatic dependent launch: 0 = off (default), 1 = short launches only, 2 = every launch;
-                                   // debug switch fs2_debug_set_tc_pdl
-int g_tc_tune[4] = {0, 0, 0, 0};   // debug overrides: SA, SB, TPS, grid (0 = heuristic); set through fs2_debug_set_tc_tuning
-#else                              // shipped build: no mutable process-wide state
-static constexpr int g_tc_pdl = 0;
-static constexpr int g_tc_tune[4] = {0, 0, 0, 0};
-#endif
-
 // Shape-derived launch plan (pure host logic, no CUDA calls): work-item shape, accumulator grouping, ring depths, shared-memory
 // budget, grid.  Returns FS2_OK or FS2_ERR_UNSUPPORTED.  Exposed as fs2_conv_tc_plan so that the heuristics' invariants are
 // testable without a GPU (tests/test_abi.py).
@@ -50,12 +41,11 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
   int R = 128 + halo;
   R += (12 - (R & 7)) & 7;                             // R % 8 == 4: conflict-free transform stores (2 chunks per row)
   if (R > TC_LD * TC_TTHREADS / TC_CHUNKS + 7) return FS2_ERR_UNSUPPORTED;
-  p.MT = 1; p.R = R;
+  p.R = R;
   p.TG = p.NB <= 64 ? 2 : 1;
   const size_t fixed = (2 * TC_SA_MAX + 2 * TC_SB_MAX) * 8 + 16;
   const size_t tap_bytes = (size_t)2 * TC_CHUNKS * p.NB * 16;
   int tps = a->taps >= 5 ? 4 : 1;                      // taps per weight stage: wide kernels share one bulk copy / handshake
-  if (g_tc_tune[2] > 0) tps = g_tc_tune[2];
   if (tps > a->taps) tps = a->taps;
   p.TPS = tps;
   const size_t a_stage = (size_t)2 * TC_CHUNKS * R * 16, b_stage = (size_t)tps * tap_bytes;
@@ -71,22 +61,17 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
   while (fixed + sa * a_stage + sb * b_stage > budget && sa > 2) sa--;
   while (fixed + sa * a_stage + sb * b_stage > budget && sb > 2) sb--;
   if (fixed + sa * a_stage + sb * b_stage > budget) return FS2_ERR_UNSUPPORTED;
-  if (g_tc_tune[0] > 0) sa = g_tc_tune[0] > TC_SA_MAX ? TC_SA_MAX : g_tc_tune[0];
-  if (g_tc_tune[1] > 0) sb = g_tc_tune[1] > TC_SB_MAX ? TC_SB_MAX : g_tc_tune[1];
-  if (fixed + sa * a_stage + sb * b_stage > budget) return FS2_ERR_UNSUPPORTED;
   p.SA = sa; p.SB = sb;
   smem = fixed + sa * a_stage + sb * b_stage;
   p.tiles_per_batch = (a->T + 127) / 128;
   const long long n_items = (long long)(a->N / p.NB) * a->B * p.tiles_per_batch;
   if (n_items > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   p.n_items = (int)n_items;
-  p.pdl = g_tc_pdl == 2 || (g_tc_pdl == 1 && n_items <= 4LL * num_sms);
   grid = n_items < num_sms ? (int)n_items : num_sms;
-  if (g_tc_tune[3] > 0 && g_tc_tune[3] < grid) grid = g_tc_tune[3];
   return FS2_OK;
 }
 
-// out[12] = {NB, MT, TG, SA, SB, TPS, R, accumulator registers per consumer thread, tiles_per_batch, n_items, grid, dynamic smem bytes}
+// out[11] = {NB, TG, SA, SB, TPS, R, accumulator registers per consumer thread, tiles_per_batch, n_items, grid, dynamic smem bytes}
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out) {
   if (!a || !out || num_sms <= 0 || a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
@@ -95,23 +80,23 @@ int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out) {
   int grid = 0;
   const int rc = conv_tc_plan(a, num_sms, p, smem, grid);
   if (rc != FS2_OK) return rc;
-  const int v[12] = {p.NB, p.MT, p.TG, p.SA, p.SB, p.TPS, p.R, p.TG * p.NB / 2, p.tiles_per_batch, p.n_items, grid, (int)smem};
-  for (int i = 0; i < 12; i++) out[i] = v[i];
+  const int v[11] = {p.NB, p.TG, p.SA, p.SB, p.TPS, p.R, p.TG * p.NB / 2, p.tiles_per_batch, p.n_items, grid, (int)smem};
+  for (int i = 0; i < 11; i++) out[i] = v[i];
   return FS2_OK;
 }
 
-// `wt` must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h)
-int conv1d_tc(const fs2_conv1d_args* a, const float* wt, unsigned variant, cudaStream_t s, long long wt_batch_stride) {
-  if (!a || !a->x || !wt || !a->y) return FS2_ERR_ARG;
+// a->w_tc must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h) in the format a->tc_variant names
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
+  if (!a || !a->x || !a->w_tc || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
-  if (!aligned16(a->x) || !aligned16(wt) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
+  if (!aligned16(a->x) || !aligned16(a->w_tc) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
+  const unsigned variant = a->tc_variant;
   // K-segmented evaluation in ONE launch (FS2_TC_VARIANT_SEGMENTED): the work units are (tile, tap, 256-channel chunk)
   fs2_conv1d_args seg_args;
   int nseg = 1, seg_nkc = 1;
   if (variant & FS2_TC_VARIANT_SEGMENTED) {
-    if (!(variant & FS2_TC_VARIANT_NB64) || a->Cin % 256 || a->N % 64 || a->dilation != 1 || a->alpha != 1.f || a->out_act != FS2_ACT_NONE ||
-        wt_batch_stride != 0)
+    if (!(variant & FS2_TC_VARIANT_NB64) || a->Cin % 256 || a->N % 64 || a->dilation != 1 || a->alpha != 1.f || a->out_act != FS2_ACT_NONE)
       return FS2_ERR_UNSUPPORTED;
     seg_nkc = a->Cin / 256; nseg = a->taps * seg_nkc;
     seg_args = *a;
@@ -137,14 +122,13 @@ int conv1d_tc(const fs2_conv1d_args* a, const float* wt, unsigned variant, cudaS
   TcP p{};
   p.x = a->x; p.xbs = a->x_batch_stride; p.xrs = a->x_row_stride;
   p.B = a->B; p.T = a->T; p.Cin = plan_args->Cin;
-  p.wt = wt; p.wt_bstride = wt_batch_stride; p.bias = a->bias; p.N = a->N;
+  p.wt = a->w_tc; p.bias = a->bias; p.N = a->N;
   p.taps = plan_args->taps; p.dil = a->dilation; p.pad = a->pad_left;
   p.nseg = nseg; p.seg_nkc = seg_nkc; p.seg_wbytes = TC_HDR + (long long)1024 * a->N;
   p.in_act = a->in_act; p.in_slope = a->in_slope; p.out_act = a->out_act; p.out_slope = a->out_slope;
   p.res = a->res; p.rbs = a->res_batch_stride; p.rrs = a->res_row_stride;
   p.alpha = a->alpha; p.accumulate = a->accumulate; p.row_lens = a->row_lens;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
-  p.variant = variant;
   p.f8 = (variant & FS2_TC_VARIANT_F8) ? 1 : 0;
   size_t smem = 0;
   int grid = 0;

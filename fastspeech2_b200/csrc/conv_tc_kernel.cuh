@@ -49,7 +49,6 @@ struct TcP {
   const float* x; long long xbs, xrs;
   int B, T, Cin;
   const float* wt;                 // tiled weights, see packing.pack_conv_tc
-  long long wt_bstride;            // bytes between the tile buffers of consecutive utterances (0 = shared weights)
   const float* bias;
   int N;                           // total output channels
   int NB;                          // output channels per work item (MMA N), N % NB == 0, NB % 16 == 0, NB <= 128
@@ -60,15 +59,12 @@ struct TcP {
   float alpha; int accumulate;
   const int* row_lens;
   float* y; long long ybs, yrs;
-  int MT;                          // 128-row tiles per work item (1)
   int TG;                          // accumulators per tile: 1 = all split terms together, 2 = {hi*hi | the two cross terms}
   int SA, SB;                      // ring depths
   int TPS;                         // conv taps per weight stage (small NB: several taps share one bulk copy / one handshake)
-  int R;                           // slab rows held in smem (>= MT*128 + (taps-1)*dil, R % 8 == 4)
+  int R;                           // slab rows held in smem (>= 128 + (taps-1)*dil, R % 8 == 4)
   int tiles_per_batch;             // work items per utterance
   int n_items;                     // total work items = (N/NB) * B * tiles_per_batch
-  unsigned variant;                // reserved for A/B experiments (unused by the shipped kernel)
-  int pdl;                         // launched with programmatic stream serialisation: wait for the previous grid before touching its data
   int nseg;                        // K-segments per output tile (1 = plain conv).  > 1: the conv is the sum of nseg one-tap slices over p.Cin (= 256)
                                    // input channels each, slice s = (tap = s / seg_nkc, channel chunk = s % seg_nkc); every slice is its own work unit with a
                                    // fresh accumulator, and the units of one tile run back to back on one CTA, adding into y in fp32 (FS2_TC_VARIANT_SEGMENTED)
@@ -105,11 +101,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// Programmatic dependent launch: the grid may start while its predecessor in the stream is still draining; everything that
-// reads or writes memory the predecessor touches comes after grid_dep_wait() (returns once the predecessor has completed and
-// flushed).  grid_dep_launch() lets the successor's CTAs be scheduled onto SMs as this grid's CTAs exit.
-__device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // 8 consecutive floats (one 32-byte sector) as two 128-bit read-only loads
 __device__ __forceinline__ void ldg256(float (&d)[8], const float* src) {
@@ -145,7 +136,7 @@ __device__ __forceinline__ Item decode_item(const TcP& p, int item) {
   it.nblk = item / per_blk;
   const int rem = item - it.nblk * per_blk;
   it.b = rem / p.tiles_per_batch;
-  it.t0 = (rem - it.b * p.tiles_per_batch) * p.MT * 128;
+  it.t0 = (rem - it.b * p.tiles_per_batch) * 128;
   return it;
 }
 
@@ -276,13 +267,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (p.pdl) {
-    grid_dep_launch();
-    // Static weights were written before the stream reached this layer, so the producer warp starts prefetching weight stages
-    // while the predecessor drains; per-utterance "weights" (attention K / V tiles) come from the previous kernel.  Everything
-    // else (activation loads, residual / accumulate loads, stores) waits.
-    if (warp != CWARPS || p.wt_bstride != 0) grid_dep_wait();
-  }
 
   if (warp == CWARPS) {
     // ===================== weight-stage producer (TMA bulk copies) =====================
@@ -292,9 +276,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
       const int per_blk = p.B * p.tiles_per_batch;
       int nblk = (int)blockIdx.x / per_blk, rem = (int)blockIdx.x - nblk * per_blk;
       for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-        const long long wb = p.wt_bstride ? (long long)(rem / p.tiles_per_batch) * p.wt_bstride : 0;
         for (int seg = 0; seg < p.nseg; seg++) {
-          const unsigned char* src = reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes + wb + TC_HDR +
+          const unsigned char* src = reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes + TC_HDR +
                                      (size_t)nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
           for (int kb = 0; kb < KBLOCKS; kb++) {
             for (int tap = 0; tap < p.taps; tap += p.TPS) {
@@ -318,7 +301,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     // so the tensor core always has the next stage's MMAs queued while the previous ones retire.
     const int g = warp >> 2;                             // 64-row half of the tile
     const uint64_t a_const = wgmma_desc(0, (uint32_t)R * 16, 128), b_const = wgmma_desc(0, (uint32_t)NB * 16, 128);
-    const float inv_ws0 = __ldg(p.wt);                 // header: 1 / (power-of-two weight scale); identical for every utterance
+    const float inv_ws0 = __ldg(p.wt);                 // header: 1 / (power-of-two weight scale)
     Ring ra, rb;
     for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
       const Item it = decode_item(p, item);
@@ -481,20 +464,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   }
 }
 
-inline void conv_tc_launch(void (*kern)(const TcP), const TcP& p, unsigned grid, size_t smem, cudaStream_t s) {
-  if (!p.pdl) {
-    kern<<<grid, TC_THREADS, smem, s>>>(p);
-    return;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  cudaLaunchKernelEx(&cfg, kern, p);
-}
-
 // The NB instantiations live in their own translation units (conv_tc_nb*.cu) so that the library builds in parallel.
 // conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.
 #define FS2_CONV_TC_NB_DECL(nb)                        \
@@ -509,7 +478,7 @@ FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CON
     return cudaFuncSetAttribute(conv_tc_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
   }                                                                                                     \
   void conv_tc_launch_nb##nb(const TcP& p, unsigned grid, size_t smem, cudaStream_t s) {                \
-    conv_tc_launch(conv_tc_kernel<nb>, p, grid, smem, s);                                              \
+    conv_tc_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                                               \
   }
 
 }  // namespace fs2

@@ -56,24 +56,18 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 
 // kernels / launchers defined in the other translation units
 int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s);
-int conv1d_tc(const fs2_conv1d_args* a, const float* wt, unsigned variant, cudaStream_t s, long long wt_batch_stride = 0);
-int attention_gemm(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s);
-size_t attention_gemm_workspace(int B, int T, int H);
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
 int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out);
-#ifdef FS2_DEBUG_KNOBS
-extern int g_tc_tune[4];
-extern int g_tc_pdl;
-#endif
 
 // backend dispatch of the fs2_conv1d contract
 static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s) {
   if (!a) return FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_TC) return a->w_tc ? conv1d_tc(a, a->w_tc, a->tc_variant, s) : FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, a->w_tc, a->tc_variant, s);
+  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s);
+  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s);
   return conv1d_simt(a, s);
 }
 int attention_simt(const fs2_attention_args* a, cudaStream_t s);
@@ -146,16 +140,10 @@ static int conv_seg(cudaStream_t s, const float* x, int B, int T, int Cin, const
   a.res = res; a.res_batch_stride = (int64_t)T * N; a.res_row_stride = N;
   a.alpha = 1.f; a.accumulate = 0; a.row_lens = row_lens;
   a.y = y; a.y_batch_stride = (int64_t)T * N; a.y_row_stride = N;
-  return conv1d_tc(&a, a.w_tc, a.tc_variant, s);
+  return conv1d_tc(&a, s);
 }
 
 struct FftBufs { float *x, *tmp, *qkv, *ctx, *hid; void* att_ws; size_t att_bytes; };
-
-// The GEMM attention materialises S [B*H][T][Tk] in fp32 and keeps a score row in registers: it serves 192 <= T <= 4096 with a
-// workspace of at most 8 GB; anything longer / larger runs the exact flash-style kernel, which has no length limit.
-static bool attention_gemm_usable(int B, int T, int H) {
-  return T >= 192 && T <= 4096 && attention_gemm_workspace(B, T, H) <= ((size_t)8 << 30);
-}
 
 // One FFT block in place on bufs.x  (transformer/Layers.py:21-30)
 static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_block_weights& w, const FftBufs& f, int B, int T,
@@ -182,9 +170,7 @@ static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_
   fs2_attention_args at{};
   at.qkv = f.qkv; at.ctx = f.ctx; at.B = B; at.T = T; at.H = m->n_head; at.Dh = D / m->n_head; at.key_lens = lens;
   at.scale = 1.0f / sqrtf((float)(D / m->n_head));
-  if (tc && f.att_ws && (m->tc_mask & FS2_TC_ATTENTION_GEMM) && attention_gemm_usable(B, T, m->n_head)) {
-    FS2_TRY(attention_gemm(&at, f.att_ws, f.att_bytes, s));          // round-1 path: S materialised, two GEMM launches per head
-  } else if (tc && f.att_ws && T >= 128) {                            // one fused tensor-core kernel: S stays in registers, any length
+  if (tc && f.att_ws && T >= 128) {                                   // one fused tensor-core kernel: S stays in registers, any length
     FS2_TRY(attention_fused(&at, f.att_ws, f.att_bytes, s));
   } else {
     FS2_TRY(attention_simt(&at, s));
@@ -209,10 +195,7 @@ static bool model_ok(const fs2_acoustic_model* m) {
 static FftBufs fft_bufs(Arena& ar, const fs2_acoustic_model* m, size_t rows, int B = 0, int T = 0, bool tc_attention = false) {
   FftBufs f;
   f.att_ws = nullptr; f.att_bytes = 0;
-  if (tc_attention && (m->tc_mask & FS2_TC_ATTENTION_GEMM) && attention_gemm_usable(B, T, m->n_head)) {
-    f.att_bytes = attention_gemm_workspace(B, T, m->n_head);
-    f.att_ws = ar.take(f.att_bytes);
-  } else if (tc_attention && T >= 128) {
+  if (tc_attention && T >= 128) {
     f.att_bytes = attention_fused_workspace(B, T, m->n_head);
     f.att_ws = ar.take(f.att_bytes);
   }
@@ -452,7 +435,7 @@ using namespace fs2;
 
 extern "C" {
 
-int fs2_abi_version(void) { return 9; }
+int fs2_abi_version(void) { return 10; }
 int fs2_conv_tc_block(int N) { return conv_tc_nb(N, 128); }
 int fs2_conv_tc_block_f8(int N) { return conv_tc_nb(N, 64); }
 int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_tc_plan_query(a, num_sms, out); }
@@ -478,12 +461,6 @@ size_t fs2_struct_size(int which) {
     default: return 0;
   }
 }
-#ifdef FS2_DEBUG_KNOBS
-/* tuning / tracing knobs for scripts/tc_*.py -- compiled in only with -DFS2_DEBUG_KNOBS (FS2_DEBUG_KNOBS=1 python -m fastspeech2_b200.build):
- * the shipped library has no mutable process-wide state behind the ABI */
-void fs2_debug_set_tc_pdl(int on) { g_tc_pdl = on; }
-void fs2_debug_set_tc_tuning(int sa, int sb, int tps, int grid) { g_tc_tune[0] = sa; g_tc_tune[1] = sb; g_tc_tune[2] = tps; g_tc_tune[3] = grid; }
-#endif
 int fs2_profile_begin(void) {
   g_prof.clear();
   g_prof_on = true;
@@ -511,14 +488,14 @@ const char* fs2_build_info(void) { return "fs2b200 sm_90a (wgmma split-FP16 conv
 int fs2_conv1d(const fs2_conv1d_args* a, fs2_stream_t st) { return conv1d_dispatch(a, S(st)); }
 int fs2_layernorm(const fs2_layernorm_args* a, fs2_stream_t st) { return layernorm(a, S(st)); }
 int fs2_attention(const fs2_attention_args* a, fs2_stream_t st) {
-  if (a && a->backend == 1) return attention_gemm(a, a->workspace, a->workspace_bytes, S(st));
-  if (a && a->backend == 2) return attention_fused(a, a->workspace, a->workspace_bytes, S(st));
-  return attention_simt(a, S(st));
+  if (!a) return FS2_ERR_ARG;
+  if (a->backend == 0) return attention_simt(a, S(st));
+  if (a->backend == 2) return attention_fused(a, a->workspace, a->workspace_bytes, S(st));
+  return FS2_ERR_ARG;
 }
-size_t fs2_attention_workspace_bytes(int B, int T, int H) {      // enough for either tensor-core backend
+size_t fs2_attention_workspace_bytes(int B, int T, int H) {      // backend 2
   if (!(B > 0 && T > 0 && H > 0)) return 0;
-  const size_t g = attention_gemm_workspace(B, T, H), f = attention_fused_workspace(B, T, H);
-  return g > f ? g : f;
+  return attention_fused_workspace(B, T, H);
 }
 int fs2_embed_positions(const fs2_embed_args* a, fs2_stream_t st) { return embed_positions(a, S(st)); }
 int fs2_add_speaker(const fs2_rowbias_args* a, fs2_stream_t st) { return add_speaker(a, S(st)); }

@@ -56,7 +56,7 @@ def attention(qkv, n_head, key_lens=None, backend=0):
     D = D3 // 3
     ctx = torch.empty(B, T, D, dtype=torch.float32, device=qkv.device)
     ws = None
-    if backend in (1, 2):
+    if backend == 2:
         ws = torch.empty(L.lib().fs2_attention_workspace_bytes(B, T, n_head), dtype=torch.uint8, device=qkv.device)
     a = L.AttentionArgs(qkv=qkv.data_ptr(), ctx=ctx.data_ptr(), B=B, T=T, H=n_head, Dh=D // n_head, key_lens=L.ptr(key_lens),
                         scale=float((D // n_head) ** -0.5), backend=backend, workspace=L.ptr(ws),

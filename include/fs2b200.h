@@ -46,9 +46,7 @@ enum { FS2_CONV_AUTO = 0, FS2_CONV_SIMT = 1, FS2_CONV_TC = 2 };
 /* which parts of the acoustic model may use the split-FP16 tensor-core kernel (fs2_acoustic_model.tc_mask) */
 enum { FS2_TC_ENCODER = 1, FS2_TC_PREDICTORS = 2, FS2_TC_DECODER = 4, FS2_TC_POSTNET = 8,
        /* the decoder's / PostNet's w_*_tc tiles are in the f16+f8 format (see FS2_TC_VARIANT_F8) */
-       FS2_TC_DECODER_F8 = 16, FS2_TC_POSTNET_F8 = 32,
-       /* decoder attention through the round-1 GEMM path (scores materialised in HBM) instead of the fused kernel */
-       FS2_TC_ATTENTION_GEMM = 64 };
+       FS2_TC_DECODER_F8 = 16, FS2_TC_POSTNET_F8 = 32 };
 /* fs2_conv1d_args.tc_variant bits.  F8: w_tc holds the two-MMA operand split -- fp16 hi tiles as in the three-MMA split, and in
  * place of the fp16 lo tiles E4M3 tiles [hi * 2^-12 | lo] that one K = 32 E4M3 MMA multiplies with the activations'
  * [lo * 2^12 | hi]: y ~ a_hi.w_hi + (a_lo.w_hi + a_hi.w_lo) with the bracket at E4M3 precision (relative error ~2^-16 instead
@@ -75,8 +73,9 @@ int fs2_conv_tc_block(int N);    /* 0 when N is not supported by the tensor-core
 int fs2_conv_tc_block_f8(int N); /* the same for FS2_TC_VARIANT_F8 tiles: the largest multiple of 16 <= 64 that divides N (N itself if N <= 64) */
 struct fs2_conv1d_args;
 /* Launch plan the tensor-core kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are
- * only checked for alignment): out[12] = {NB, MT (128-row tiles per work item), TG (accumulators per tile), slab stages, weight
- * stages, taps per weight stage, slab rows, accumulator registers per consumer thread, work items per utterance, work items, grid, dynamic shared memory bytes}.
+ * only checked for alignment; a work item is one 128-row tile x NB output channels): out[11] = {NB, TG (accumulators per tile), slab
+ * stages, weight stages, taps per weight stage, slab rows, accumulator registers per consumer thread, work items per utterance, work items,
+ * grid, dynamic shared memory bytes}.
  * Returns FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
 int fs2_conv_tc_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out);
 
@@ -129,9 +128,9 @@ int fs2_layernorm(const fs2_layernorm_args* a, fs2_stream_t stream);
 typedef struct fs2_attention_args {
   const float* qkv; float* ctx; int B, T, H, Dh;
   const int32_t* key_lens; float scale;
-  int backend;                  /* 0 = exact fp32 flash-style kernel; 1 = tensor-core GEMMs + row softmax (scores in HBM, T <= 4096); 2 = ONE fused
-                                   tensor-core kernel (QK^T, softmax, PV; scores stay in registers, any T).  1 and 2 need the workspace */
-  void* workspace; size_t workspace_bytes;   /* backend 1 only: >= fs2_attention_workspace_bytes(B, T, H) */
+  int backend;                  /* 0 = exact fp32 flash-style kernel; 2 = ONE fused tensor-core kernel (QK^T, softmax, PV; scores stay in
+                                   registers, any T).  Any other value: FS2_ERR_ARG */
+  void* workspace; size_t workspace_bytes;   /* backend 2: >= fs2_attention_workspace_bytes(B, T, H) bytes; backend 0 ignores it */
 } fs2_attention_args;
 int fs2_attention(const fs2_attention_args* a, fs2_stream_t stream);
 size_t fs2_attention_workspace_bytes(int B, int T, int H);
@@ -337,7 +336,7 @@ size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the
  * device that owns the stream current before calling -- (b) the launch counter above and (c) the profiling state below, which is
- * per host thread.  Tuning / tracing knobs exist only in builds with -DFS2_DEBUG_KNOBS.
+ * per host thread.
  * Per-kernel-class device timing for bench.py's roofline (CUDA events recorded around each launch on the launch stream).
  * Classes: 0 tensor-core kernels (conv1d implicit GEMM + fused ResBlock group), 1 attention, 2 layernorm, 3 everything else, 4 fp32 CUDA-core conv1d.  begin() arms it, end() synchronises the
  * recorded events, fills ms/flops/launches per class (arrays of FS2_PROF_CLASSES) and disarms.  Not for timed regions. */

@@ -58,15 +58,18 @@ def test_host_side_argument_checks_need_no_gpu():
     assert h.fs2_resstack(ctypes.byref(r), None) == -1           # overlapping x / y (the kernel re-reads halo rows of x)
     r.y = 0x10008
     assert h.fs2_resstack(ctypes.byref(r), None) == -1           # misaligned y
+    for backend in (1, 3):                                       # attention backends are 0 (exact) and 2 (fused tensor-core kernel)
+        at = _lib.AttentionArgs(qkv=0x1000, ctx=0x1000, B=1, T=4, H=2, Dh=128, scale=1.0, backend=backend)
+        assert h.fs2_attention(ctypes.byref(at), None) == -1
 
 
 def _plan(h, B, T, Cin, N, taps, dil=1, num_sms=132, x=0x1000, x_row_stride=None, tc_variant=0):
     a = _lib.Conv1dArgs(x=x, x_batch_stride=T * (x_row_stride or Cin), x_row_stride=x_row_stride or Cin, B=B, T=T, Cin=Cin, w=0x1000, N=N, taps=taps,
                         dilation=dil, pad_left=(taps - 1) * dil // 2, w_tc=0x1000, y=0x1000, y_batch_stride=T * N, y_row_stride=N, alpha=1.0,
                         tc_variant=tc_variant)
-    out = (ctypes.c_int32 * 12)()
+    out = (ctypes.c_int32 * 11)()
     rc = h.fs2_conv_tc_plan(ctypes.byref(a), num_sms, out)
-    keys = ("NB", "MT", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")
+    keys = ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")
     return rc, dict(zip(keys, out))
 
 
@@ -78,7 +81,8 @@ def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
     shapes = []
     for B, T in ((1, 7), (1, 1012), (16, 1012), (64, 2032)):
         shapes += [(B, T, 256, 768, 1, 1), (B, T, 256, 256, 1, 1), (B, T, 256, 1024, 9, 1), (B, T, 1024, 256, 1, 1), (B, T, 256, 80, 1, 1),
-                   (B, T, 80, 512, 5, 1), (B, T, 512, 512, 5, 1), (B, T, 512, 80, 5, 1), (B, T, 128, 2048, 1, 1), (B, T, 2048, 128, 1, 1)]
+                   (B, T, 80, 512, 5, 1), (B, T, 512, 512, 5, 1), (B, T, 512, 80, 5, 1)]
+        shapes += [(B, T, 128, 2048, 1, 1), (B, T, 2048, 128, 1, 1)]          # sweep: wide N, long C_in
         t, c = T, 512
         shapes.append((B, T, 80, 512, 7, 1))                                   # conv_pre
         for u in (8, 8, 2, 2):
@@ -89,7 +93,7 @@ def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
         rc, p = _plan(h, B, T, Cin, N, k, d, num_sms=132)
         assert rc == 0, (B, T, Cin, N, k, d, rc)
         assert p["NB"] % 16 == 0 and 16 <= p["NB"] <= 128 and N % p["NB"] == 0
-        assert p["MT"] == 1 and p["TG"] == (2 if p["NB"] <= 64 else 1)
+        assert p["TG"] == (2 if p["NB"] <= 64 else 1)
         assert p["acc_regs"] == p["TG"] * p["NB"] // 2 <= 64
         assert p["smem"] <= 227 * 1024
         assert 2 <= p["SA"] <= 8 and 2 <= p["SB"] <= 8 and 1 <= p["TPS"] <= k
@@ -104,8 +108,8 @@ def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
         if n and n % 16 == 0:
             a = _lib.Conv1dArgs(x=0x1000, x_batch_stride=256 * 16, x_row_stride=16, B=1, T=256, Cin=16, w=0x1000, N=n, taps=1,
                                 w_tc=0x1000, y=0x1000, y_batch_stride=256 * n, y_row_stride=n, alpha=1.0, tc_variant=_lib.TC_VARIANT_F8)
-            out = (ctypes.c_int32 * 12)()
-            assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, out) == 0 and out[0] == h.fs2_conv_tc_block_f8(n) and out[2] == 2, n
+            out = (ctypes.c_int32 * 11)()
+            assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, out) == 0 and out[0] == h.fs2_conv_tc_block_f8(n) and out[1] == 2, n
     # ring depths per shape class: short kernels get the deepest slab ring, wide kernels share one weight stage between four taps
     assert _plan(h, 16, 64768, 128, 128, 3)[1]["SA"] == 5 and _plan(h, 16, 64768, 128, 128, 11, 5)[1]["TPS"] == 4
     # refused shapes: C_in % 16, N % 16, misaligned or oddly strided x, halo beyond the slab

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfs2b200.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 MAX_LAYERS, MAX_POSTNET, MAX_STAGES, MAX_RESBLOCKS, MAX_DIL = 12, 8, 8, 32, 4
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_LRELU = 0, 1, 2, 3
 CONV_AUTO, CONV_SIMT, CONV_TC = 0, 1, 2
@@ -36,7 +36,8 @@ class Conv1dArgs(C.Structure):
                 ("res", fp), ("res_batch_stride", i64), ("res_row_stride", i64),
                 ("alpha", f32), ("accumulate", i32),
                 ("row_lens", fp),
-                ("y", fp), ("y_batch_stride", i64), ("y_row_stride", i64)]
+                ("y", fp), ("y_batch_stride", i64), ("y_row_stride", i64),
+                ("x_lens", fp), ("lens_scale", i32)]
 
 
 class LayerNormArgs(C.Structure):
@@ -75,7 +76,7 @@ class LengthRegulateArgs(C.Structure):
 
 class ConvPostArgs(C.Structure):
     _fields_ = [("x", fp), ("B", i32), ("T", i32), ("C", i32), ("w", fp), ("bias", fp), ("taps", i32),
-                ("in_slope", f32), ("wav", fp)]
+                ("in_slope", f32), ("wav", fp), ("lens", fp), ("lens_scale", i32)]
 
 
 class FftBlockWeights(C.Structure):
@@ -139,7 +140,7 @@ class ResstackArgs(C.Structure):
                 ("k", i32 * (MAX_DIL + 4)), ("dil", (i32 * MAX_DIL) * (MAX_DIL + 4)),
                 ("w1_tc", (fp * MAX_DIL) * (MAX_DIL + 4)), ("b1", (fp * MAX_DIL) * (MAX_DIL + 4)),
                 ("w2_tc", (fp * MAX_DIL) * (MAX_DIL + 4)), ("b2", (fp * MAX_DIL) * (MAX_DIL + 4)),
-                ("alpha", f32), ("accumulate", i32)]
+                ("alpha", f32), ("accumulate", i32), ("lens", fp), ("lens_scale", i32)]
 
 
 class WavInt16Args(C.Structure):
@@ -148,7 +149,7 @@ class WavInt16Args(C.Structure):
 
 class VocoderArgs(C.Structure):
     _fields_ = [("B", i32), ("T", i32), ("mel", fp), ("mel_batch_stride", i64), ("mel_row_stride", i64),
-                ("wav", fp), ("workspace", fp), ("workspace_bytes", C.c_size_t)]
+                ("wav", fp), ("workspace", fp), ("workspace_bytes", C.c_size_t), ("mel_lens", fp)]
 
 
 EXPORTS = {

@@ -59,6 +59,13 @@ __device__ __forceinline__ float apply_act(float v, int act, float slope) {
   }
 }
 
+// Ragged batches (x_lens / lens of fs2_conv1d, fs2_resstack, fs2_conv_post): utterance b has n_b = clamp(lens[b] * scale, 0, cap) rows.
+// Device lengths are clamped, never trusted.
+__device__ __forceinline__ int ragged_rows(const int* lens, int scale, int cap, int b) {
+  const long long n = (long long)__ldg(lens + b) * scale;
+  return n <= 0 ? 0 : (n >= cap ? cap : (int)n);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -26,6 +26,7 @@ struct ConvP {
   const int* row_lens;
   float* y; long long ybs, yrs;
   int tiles_per_batch;
+  const int* x_lens; int lens_scale;   // ragged batch (fs2_conv1d_args::x_lens) or NULL
 };
 
 template <int BM, int BN, int ACT>
@@ -47,6 +48,9 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   const int b = blockIdx.x / p.tiles_per_batch;
   const int t0 = (blockIdx.x % p.tiles_per_batch) * BM;
   const int n0 = blockIdx.y * BN;
+  // ragged batch: input rows t >= n_b read as zero, and a tile lying wholly at or beyond n_b has nothing to compute (its rows are unspecified)
+  const int tend = p.x_lens ? ragged_rows(p.x_lens, p.lens_scale, p.T, b) : p.T;
+  if (t0 >= tend) return;
 
   const float* xb = p.x + (long long)b * p.xbs;
   const int kc = p.Cin / BK;               // k-steps per tap
@@ -71,7 +75,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
       const int row = f >> 2, c4 = f & 3;
       const int t = t0 + row + shift;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (t >= 0 && t < p.T) {
+      if (t >= 0 && t < tend) {
         v = __ldg(reinterpret_cast<const float4*>(xb + (long long)t * p.xrs + c0 + c4 * 4));
         if (p.in_act == FS2_ACT_LRELU) {
           v.x = v.x > 0.f ? v.x : v.x * p.in_slope;
@@ -205,6 +209,7 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   p.res = a->res; p.rbs = a->res_batch_stride; p.rrs = a->res_row_stride;
   p.alpha = a->alpha; p.accumulate = a->accumulate;
   p.row_lens = a->row_lens;
+  p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // SM count of the current device

@@ -130,6 +130,7 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
   p.alpha = a->alpha; p.accumulate = a->accumulate; p.row_lens = a->row_lens;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
   p.f8 = (variant & FS2_TC_VARIANT_F8) ? 1 : 0;
+  p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;   // the plan below stays the padded one: the host never reads device lengths
   size_t smem = 0;
   int grid = 0;
   const int rc = conv_tc_plan(plan_args, g_num_sms, p, smem, grid);

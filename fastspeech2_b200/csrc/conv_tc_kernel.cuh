@@ -71,6 +71,8 @@ struct TcP {
   int seg_nkc;                     // channel chunks per tap
   long long seg_wbytes;            // bytes between the tile buffers of consecutive slices
   int f8;                          // operand split: 0 = three FP16 MMAs (hi*hi + lo*hi + hi*lo), 1 = FP16 main term + ONE E4M3 (K = 32) correction MMA
+  const int* x_lens;               // ragged batch (fs2_conv1d_args::x_lens) or NULL; n_items / tiles_per_batch then only bound the grid
+  int lens_scale;
 };
 
 // ------------------------------------------------------------------ PTX wrappers
@@ -140,6 +142,32 @@ __device__ __forceinline__ Item decode_item(const TcP& p, int item) {
   return it;
 }
 
+// Ragged batch (TcP::x_lens, RsP::lens): utterance b has n_b = ragged_rows(...) rows, and the work items of one channel block are the
+// live `tile`-row tiles of utterance 0, 1, ... back to back: sum_b ceil(n_b / tile) of them, so no tile lying wholly in the padding is
+// ever scheduled.
+// Monotone cursor over that compacted sequence.  Every role visits its items in increasing order (item = blockIdx.x, + gridDim.x, ...),
+// so the cursor only moves forward and each length is loaded once per channel block: no table, no cap on B, no host sync.
+struct RaggedWalk {
+  int live;                        // live tiles per channel block
+  int nblk, b, before, rows;       // cursor: channel block, utterance, live tiles of utterances < b in the block, n_b
+  __device__ __forceinline__ void init(const int* lens, int scale, int cap, int B, int tile) {
+    live = 0;
+    for (int i = 0; i < B; i++) live += (ragged_rows(lens, scale, cap, i) + tile - 1) / tile;
+    nblk = 0; b = 0; before = 0; rows = ragged_rows(lens, scale, cap, 0);
+  }
+  __device__ __forceinline__ Item item(const int* lens, int scale, int cap, int tile, int i) {   // i < live * channel blocks
+    const int blk = i / live, rem = i - blk * live;
+    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = ragged_rows(lens, scale, cap, 0); }
+    for (int nt = (rows + tile - 1) / tile; rem >= before + nt; nt = (rows + tile - 1) / tile) {
+      before += nt;
+      rows = ragged_rows(lens, scale, cap, ++b);
+    }
+    Item it;
+    it.nblk = blk; it.b = b; it.t0 = (rem - before) * tile;
+    return it;
+  }
+};
+
 template <int ACT>
 __device__ __forceinline__ float tc_act(float v, float slope) {
   if (ACT == FS2_ACT_RELU) return fmaxf(v, 0.f);
@@ -196,9 +224,10 @@ __device__ __forceinline__ void tc_convert_store(const float (&src)[LD][8], cons
 
 // Epilogue of one consumer warpgroup: its 64 rows of the tile straight from the accumulator fragments (see wgmma.cuh): thread
 // (warp w, lane l) owns rows 16w + l/4 and +8, column pairs 8j + 2(l%4).  The split-term accumulators are summed here in fp32
-// round-to-nearest.  bias / res / row_lens may be NULL; acc_in: add alpha*value to y instead of overwriting it.
+// round-to-nearest.  bias / res / row_lens may be NULL; acc_in: add alpha*value to y instead of overwriting it.  Rows >= tend (T, or n_b
+// of a ragged batch) are not written.
 template <int ACT, int NB, int TG>
-__device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 2], const Item& it, int row_base, const float* bias,
+__device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 2], const Item& it, int row_base, int tend, const float* bias,
                                             const float* res, const int* row_lens, int acc_in, float inv_ws) {
   const int lane = threadIdx.x & 31;
   const int n0 = it.nblk * NB + 2 * (lane & 3);
@@ -207,7 +236,7 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 #pragma unroll
   for (int h = 0; h < 2; h++) {
     const int t = row_base + (lane >> 2) + 8 * h;
-    if (t >= p.T) continue;
+    if (t >= tend) continue;
     const bool live = t < len_b;
     float* yrow = p.y + (long long)it.b * p.ybs + (long long)t * p.yrs + n0;
     const float* rrow = res ? res + (long long)it.b * p.rbs + (long long)t * p.rrs + n0 : nullptr;
@@ -242,7 +271,9 @@ __device__ __forceinline__ void tc_release(uint64_t* bar) {
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-template <int NB>
+// RAG: ragged batch (TcP::x_lens != NULL).  A template parameter rather than a runtime branch: the cursor state would otherwise raise the
+// padded path's spills (every NB is at the 96-register cap of one 544-thread CTA per SM).
+template <int NB, bool RAG>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -260,6 +291,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
+  // Ragged batch: every role walks the compacted item sequence (RaggedWalk) in the same order, which keeps the rings' stage / phase
+  // sequence identical across the three roles.
+  constexpr bool rag = RAG;
+  RaggedWalk walk{};
+  int n_items = p.n_items;
+  if (rag) { walk.init(p.x_lens, p.lens_scale, p.T, p.B, 128); n_items = walk.live * (p.N / p.NB); }
 
   if (tid == 0) {
     for (int i = 0; i < TC_SA_MAX; i++) { mbar_init(&fullA[i], TC_TW); mbar_init(&emptyA[i], CWARPS); }
@@ -273,9 +310,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     if (lane == 0) {
       const uint32_t stage_bytes = 2 * b_plane;   // one tap of one K-block (hi + lo)
       Ring rb;
-      const int per_blk = p.B * p.tiles_per_batch;
+      const int per_blk = rag ? max(walk.live, 1) : p.B * p.tiles_per_batch;
       int nblk = (int)blockIdx.x / per_blk, rem = (int)blockIdx.x - nblk * per_blk;
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
         for (int seg = 0; seg < p.nseg; seg++) {
           const unsigned char* src = reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes + TC_HDR +
                                      (size_t)nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
@@ -303,8 +340,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     const uint64_t a_const = wgmma_desc(0, (uint32_t)R * 16, 128), b_const = wgmma_desc(0, (uint32_t)NB * 16, 128);
     const float inv_ws0 = __ldg(p.wt);                 // header: 1 / (power-of-two weight scale)
     Ring ra, rb;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-      const Item it = decode_item(p, item);
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      const Item it = rag ? walk.item(p.x_lens, p.lens_scale, p.T, 128, item) : decode_item(p, item);
+      const int tend = rag ? walk.rows : p.T;
       for (int seg = 0; seg < p.nseg; seg++) {
         float acc[TG][NB / 2];
 #pragma unroll
@@ -362,10 +400,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
             : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes));
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
         switch (p.out_act) {                           // uniform branch: keeps tanhf out of the other variants' inner loops
-          case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, bias, res, lens, acc_in, inv_ws); break;
-          case FS2_ACT_TANH: tc_epilogue<FS2_ACT_TANH, NB, TG>(p, acc, it, row_base, bias, res, lens, acc_in, inv_ws); break;
-          case FS2_ACT_LRELU: tc_epilogue<FS2_ACT_LRELU, NB, TG>(p, acc, it, row_base, bias, res, lens, acc_in, inv_ws); break;
-          default: tc_epilogue<FS2_ACT_NONE, NB, TG>(p, acc, it, row_base, bias, res, lens, acc_in, inv_ws); break;
+          case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
+          case FS2_ACT_TANH: tc_epilogue<FS2_ACT_TANH, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
+          case FS2_ACT_LRELU: tc_epilogue<FS2_ACT_LRELU, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
+          default: tc_epilogue<FS2_ACT_NONE, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
         }
       }
     }
@@ -396,16 +434,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     }
     // load cursor (runs TC_DEPTH K-blocks ahead of the store cursor); no divisions on the per-K-block path
     int l_item = blockIdx.x, l_kb = 0, l_seg = 0;
-    const float* l_xrow = nullptr;                     // &x[b][t0 - pad][0]; rows outside [0, T) are never dereferenced
-    int l_tfirst = 0;
+    const float* l_xrow = nullptr;                     // &x[b][t0 - pad][0]; rows outside [0, l_tend) are never dereferenced
+    int l_tfirst = 0, l_tend = p.T;                    // l_tend: T, or n_b of a ragged batch
     bool l_interior = false;                           // warp-uniform: every slab row of the item exists
     auto l_set_item = [&]() {
-      if (l_item < p.n_items) {
-        const Item it = decode_item(p, l_item);
+      if (l_item < n_items) {
+        const Item it = rag ? walk.item(p.x_lens, p.lens_scale, p.T, 128, l_item) : decode_item(p, l_item);
+        if (rag) l_tend = walk.rows;
         const int s_tap = l_seg / p.seg_nkc, s_kc = l_seg - s_tap * p.seg_nkc;   // K-segment: one tap, one 256-channel chunk (0, 0 when nseg == 1)
         l_tfirst = it.t0 - p.pad + s_tap;
         l_xrow = p.x + (long long)it.b * p.xbs + (long long)l_tfirst * p.xrs + s_kc * p.Cin;
-        l_interior = l_tfirst >= 0 && l_tfirst + rows_needed <= p.T;
+        l_interior = l_tfirst >= 0 && l_tfirst + rows_needed <= l_tend;
       }
     };
     l_set_item();
@@ -419,7 +458,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
 #pragma unroll
         for (int u = 0; u < LD; u++) {
           const int t = l_tfirst + rowu[u];
-          if (rowu[u] >= 0 && t >= 0 && t < p.T) {
+          if (rowu[u] >= 0 && t >= 0 && t < l_tend) {
             ldg256(dst[u], xk + goff[u]);
           } else {
 #pragma unroll
@@ -433,7 +472,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
         l_set_item();
       }
     };
-    const int my_items = (p.n_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    const int my_items = (n_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // >= 0: blockIdx.x < gridDim.x
     const int total = my_items * p.nseg * KBLOCKS;
 #pragma unroll
     for (int d = 0; d < DEPTH; d++)
@@ -475,10 +514,12 @@ FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CON
 
 #define FS2_CONV_TC_NB_DEF(nb)                                                                          \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes) {                                                  \
-    return cudaFuncSetAttribute(conv_tc_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+    return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
   }                                                                                                     \
   void conv_tc_launch_nb##nb(const TcP& p, unsigned grid, size_t smem, cudaStream_t s) {                \
-    conv_tc_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                                               \
+    if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                          \
+    else conv_tc_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);                                  \
   }
 
 }  // namespace fs2

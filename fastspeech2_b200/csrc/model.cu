@@ -66,6 +66,7 @@ int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out);
 // backend dispatch of the fs2_conv1d contract
 static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s) {
   if (!a) return FS2_ERR_ARG;
+  if (a->x_lens && a->lens_scale < 1) return FS2_ERR_ARG;
   if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s);
   if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s);
   return conv1d_simt(a, s);
@@ -103,7 +104,7 @@ struct Arena {
 static int conv(cudaStream_t s, const float* x, int B, int T, int Cin, const float* w, const float* w_tc, const float* bias, int N,
                 int taps, int dil, int pad, int out_act, float out_slope, float* y, const float* res = nullptr,
                 int in_act = FS2_ACT_NONE, float in_slope = 0.f, float alpha = 1.f, int accumulate = 0,
-                const int32_t* row_lens = nullptr, unsigned tc_variant = 0) {
+                const int32_t* row_lens = nullptr, unsigned tc_variant = 0, const int32_t* x_lens = nullptr, int lens_scale = 1) {
   fs2_conv1d_args a{};
   a.w_tc = w_tc; a.backend = FS2_CONV_AUTO; a.tc_variant = tc_variant;
   a.x = x; a.x_batch_stride = (int64_t)T * Cin; a.x_row_stride = Cin;
@@ -113,6 +114,7 @@ static int conv(cudaStream_t s, const float* x, int B, int T, int Cin, const flo
   a.res = res; a.res_batch_stride = (int64_t)T * N; a.res_row_stride = N;
   a.alpha = alpha; a.accumulate = accumulate; a.row_lens = row_lens;
   a.y = y; a.y_batch_stride = (int64_t)T * N; a.y_row_stride = N;
+  a.x_lens = x_lens; a.lens_scale = lens_scale;
   return conv1d_dispatch(&a, s);
 }
 
@@ -349,6 +351,11 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
   float* r2 = ar.f32(n);
   if (ar.dry) return FS2_OK;
   if (!bx || !bu || !bt || !r1 || !r2) return FS2_ERR_WORKSPACE;
+  // Ragged mode: every layer bounds utterance b by mel_lens[b] frames times its rows per mel frame (`scale`), so each utterance is
+  // synthesised as if alone and the tiles of the padding are never computed.  Rows beyond an utterance are left unspecified in the
+  // intermediates; conv_post writes them as zeros.
+  const int32_t* lens = a->mel_lens;
+  int scale = 1;
 
   {  // conv_pre reads the (possibly strided) channels-last mel view
     fs2_conv1d_args c{};
@@ -356,6 +363,7 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
     c.B = B; c.T = T; c.Cin = m->n_mel; c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.N = m->c0; c.taps = 7;
     c.dilation = 1; c.pad_left = 3; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
     c.alpha = 1.f; c.y = bx; c.y_batch_stride = (int64_t)T * m->c0; c.y_row_stride = m->c0;
+    c.x_lens = lens; c.lens_scale = scale;
     FS2_TRY(conv1d_dispatch(&c, s));
   }
   int Ti = T, C = m->c0;
@@ -374,9 +382,10 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
       c.N = (u / 2) * Co; c.taps = 2; c.dilation = 1; c.pad_left = g == 0 ? 1 : 0;
       c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.alpha = 1.f; c.tc_variant = tcv;
       c.y = bu + (size_t)g * (u / 2) * Co; c.y_batch_stride = (int64_t)Ti * u * Co; c.y_row_stride = (int64_t)u * Co;
+      c.x_lens = lens; c.lens_scale = scale;          // [B][Ti][u*Co]: input and output rows have the same n_b
       FS2_TRY(conv1d_dispatch(&c, s));
     }
-    Ti *= u; C = Co;
+    Ti *= u; C = Co; scale *= u;
     // ---- mean of the multi-receptive-field ResBlocks (models.py:154-160, ResBlock.forward :96-103)
     if ((m->fused_mask >> i) & 1) {                    // one persistent kernel for the whole group: intermediates never leave the SM
       if (!tcv) return FS2_ERR_ARG;
@@ -391,6 +400,7 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
           ra.w2_tc[j][d] = m->w_rb2_tc[rb][d]; ra.b2[j][d] = m->b_rb2[rb][d];
         }
       }
+      ra.lens = lens; ra.lens_scale = scale;
       FS2_TRY(resstack(&ra, s));
       continue;
     }
@@ -409,21 +419,22 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
           ra.w1_tc[0][0] = m->w_rb1_tc[rb][d]; ra.b1[0][0] = m->b_rb1[rb][d];
           ra.w2_tc[0][0] = m->w_rb2_tc[rb][d]; ra.b2[0][0] = m->b_rb2[rb][d];
           ra.alpha = lastp ? inv_nk : 1.f; ra.accumulate = lastp && j > 0;
+          ra.lens = lens; ra.lens_scale = scale;
           FS2_TRY(resstack(&ra, s));
           r = dstp;
           continue;
         }
         FS2_TRY(conv(s, r, B, Ti, C, m->w_rb1[rb][d], m->w_rb1_tc[rb][d], m->b_rb1[rb][d], C, k, dil, (k * dil - dil) / 2, FS2_ACT_LRELU,
-                     0.1f, bt, nullptr, FS2_ACT_LRELU, 0.1f, 1.f, 0, nullptr, tcv));
+                     0.1f, bt, nullptr, FS2_ACT_LRELU, 0.1f, 1.f, 0, nullptr, tcv, lens, scale));
         const bool last = d == m->n_dil - 1;
         float* dst = last ? bx : (r == r1 ? r2 : r1);
         FS2_TRY(conv(s, bt, B, Ti, C, m->w_rb2[rb][d], m->w_rb2_tc[rb][d], m->b_rb2[rb][d], C, k, 1, (k - 1) / 2, FS2_ACT_NONE, 0.f, dst,
-                     r, FS2_ACT_NONE, 0.f, last ? inv_nk : 1.f, last && j > 0, nullptr, tcv));
+                     r, FS2_ACT_NONE, 0.f, last ? inv_nk : 1.f, last && j > 0, nullptr, tcv, lens, scale));
         r = dst;
       }
     }
   }
-  fs2_conv_post_args p{bx, B, Ti, C, m->w_post, m->b_post, 7, 0.01f, a->wav};
+  fs2_conv_post_args p{bx, B, Ti, C, m->w_post, m->b_post, 7, 0.01f, a->wav, lens, scale};
   return conv_post(&p, s);
 }
 
@@ -435,7 +446,7 @@ using namespace fs2;
 
 extern "C" {
 
-int fs2_abi_version(void) { return 10; }
+int fs2_abi_version(void) { return 11; }
 int fs2_conv_tc_block(int N) { return conv_tc_nb(N, 128); }
 int fs2_conv_tc_block_f8(int N) { return conv_tc_nb(N, 64); }
 int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_tc_plan_query(a, num_sms, out); }

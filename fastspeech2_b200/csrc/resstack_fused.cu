@@ -48,6 +48,7 @@ struct RsP {
   int OBOX, n_oboxes;            // rows per output box (TILE = n_oboxes * OBOX, OBOX % 8 == 0)
   int TPS;                       // conv taps per weight stage (one bulk copy / one handshake)
   int accumulate;                // the first kernel size reduce-adds into y too
+  const int* lens; int lens_scale;   // ragged batch (fs2_resstack_args::lens) or NULL; n_items then only bounds the grid
 };
 
 // ------------------------------------------------------------------ TMA (tensor-map) wrappers
@@ -91,7 +92,8 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
   *reinterpret_cast<unsigned short*>(kblk + 3 * chunk_bytes + cc) = (unsigned short)h8;
 }
 
-template <int C, int MT>
+// RAG: ragged batch (RsP::lens != NULL), a template parameter so that the padded path's code and register allocation stay as they are.
+template <int C, int MT, bool RAG>
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmy,
                                                                  const RsP p) {
   constexpr int KB = C / 16, R = MT * 128, NH = C / 32, NJ = C / 8;   // NJ: 8-column fragment groups of a row
@@ -123,12 +125,16 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
   }
   fence_proxy_async();
   __syncthreads();
+  // ragged batch: the producer and both consumer warpgroups walk the same compacted item sequence (RaggedWalk, conv_tc_kernel.cuh)
+  RaggedWalk walk{};
+  int n_items = p.n_items;
+  if (RAG) { walk.init(p.lens, p.lens_scale, p.N, p.B, p.TILE); n_items = walk.live; }
 
   if (warp == 8) {
     // ===================== weight producer: every conv's stages once per work item and kernel size =====================
     if (lane == 0) {
       Ring rb;
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x)
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x)
         for (int j = 0; j < p.n_kernels; j++)
           for (int d = 0; d < p.n_dil; d++)
             for (int c2 = 0; c2 < 2; c2++) {
@@ -160,9 +166,15 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
   Ring rb;
   uint32_t round_phase = 0;
   bool stores_pending = false;
-  for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-    const int b = item / p.tiles_per_b;
-    const int t0 = (item - b * p.tiles_per_b) * p.TILE;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    int b, t0, nrows = p.N;                         // nrows: rows of utterance b (n_b of a ragged batch); the convs pad at its end
+    if (RAG) {
+      const Item it = walk.item(p.lens, p.lens_scale, p.N, p.TILE, item);
+      b = it.b; t0 = it.t0; nrows = walk.rows;
+    } else {
+      b = item / p.tiles_per_b;
+      t0 = (item - b * p.tiles_per_b) * p.TILE;
+    }
     for (int j = 0; j < p.n_kernels; j++) {
       // ---- input: TMA boxes of x -> XT (idle: the last conv that read it has retired), then residual stream -> registers, lrelu(x) -> XA
       if (io) {
@@ -182,7 +194,8 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
 #pragma unroll
           for (int jj = 0; jj < NJ; jj++) {
             const int c = cbase + 8 * jj;
-            const float2 u = *reinterpret_cast<const float2*>(xt + (size_t)((c >> 5) * MT + m) * XBOX + sw128(r128, (c & 31) >> 2) + (c & 3) * 4);
+            float2 u = *reinterpret_cast<const float2*>(xt + (size_t)((c >> 5) * MT + m) * XBOX + sw128(r128, (c & 31) >> 2) + (c & 3) * 4);
+            if (RAG && t0 - p.H + row >= nrows) u = make_float2(0.f, 0.f);   // the padding of a ragged batch reads as zero
             xr(i, 4 * jj + 2 * h) = u.x;
             xr(i, 4 * jj + 2 * h + 1) = u.y;
             rs_store2(xa, CHUNK, row, c, rs_lrelu(u.x), rs_lrelu(u.y));   // rows outside the utterance arrive as zeros (TMA fill)
@@ -238,7 +251,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
               for (int h = 0; h < 2; h++) {
                 const int row = rbase + 64 * i + 8 * h;
                 const int gr = t0 - p.H + row;
-                const bool in = gr >= 0 && gr < p.N;
+                const bool in = gr >= 0 && gr < nrows;
                 const float s0 = acc[i][4 * jj + 2 * h] + corr[i][4 * jj + 2 * h], s1 = acc[i][4 * jj + 2 * h + 1] + corr[i][4 * jj + 2 * h + 1];
                 float v0 = fmaf(s0, inv_s, bv.x), v1 = fmaf(s1, inv_s, bv.y);
                 if (c2 == 0) {
@@ -361,6 +374,7 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
   if (!a || !a->x || !a->y) return FS2_ERR_ARG;
   if (!aligned16(a->x) || !aligned16(a->y)) return FS2_ERR_ARG;
   if (a->B <= 0 || a->N <= 0 || a->C <= 0) return FS2_ERR_ARG;
+  if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
   {  // not in place: a work item re-reads halo rows of x that its neighbours' results would already have overwritten
     const unsigned char *xb = reinterpret_cast<const unsigned char*>(a->x), *yb = reinterpret_cast<const unsigned char*>(a->y);
     const size_t bytes = (size_t)a->B * a->N * a->C * sizeof(float);
@@ -375,8 +389,10 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
     DevOnce once;
     if (!dv->fused_ready.load(std::memory_order_relaxed)) {
       const int mx = 227 * 1024;
-      cudaError_t e = cudaFuncSetAttribute(resstack_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+      cudaError_t e = cudaFuncSetAttribute(resstack_kernel<32, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<32, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
       if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
       dv->fused_ready.store(true, std::memory_order_release);
     }
@@ -395,12 +411,18 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
     }
   p.H = plan[1]; p.TILE = plan[2]; p.tiles_per_b = (a->N + p.TILE - 1) / p.TILE; p.n_items = plan[3];
   p.alpha = a->alpha > 0.f ? a->alpha : 1.f / (float)a->n_kernels; p.accumulate = a->accumulate; p.SB = plan[5]; p.OBOX = plan[8]; p.n_oboxes = plan[9]; p.TPS = plan[10];
+  p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
   alignas(64) CUtensorMap tmx, tmy;
   FS2_TRY(make_map(&tmx, a->x, a->B, a->N, a->C, 128));
   FS2_TRY(make_map(&tmy, a->y, a->B, a->N, a->C, p.OBOX));
   prof_before(s);
-  if (a->C == 32) resstack_kernel<32, 4><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
-  else resstack_kernel<64, 2><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+  if (a->C == 32) {
+    if (a->lens) resstack_kernel<32, 4, true><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+    else resstack_kernel<32, 4, false><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+  } else {
+    if (a->lens) resstack_kernel<64, 2, true><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+    else resstack_kernel<64, 2, false><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+  }
   prof_after(s, 0, flops);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

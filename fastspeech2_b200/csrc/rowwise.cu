@@ -331,6 +331,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
   float* xs = cp_smem + a.taps * C;       // [CP_ROWS + taps - 1][C + 1]
   const int b = blockIdx.x / tiles_per_batch;
   const int t0 = (blockIdx.x % tiles_per_batch) * CP_ROWS;
+  const int nin = a.lens ? ragged_rows(a.lens, a.lens_scale, a.T, b) : a.T;   // ragged batch: rows >= n_b read as zero, wav there is 0
   for (int i = threadIdx.x; i < a.taps * C; i += blockDim.x) wsm[i] = a.w[i];
   const int rows = CP_ROWS + a.taps - 1, C4 = C / 4;
   const float4* xb = reinterpret_cast<const float4*>(a.x) + (long long)b * a.T * C4;
@@ -338,7 +339,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
     const int r = i / C4, c4 = i - r * C4;
     const int t = t0 - pad + r;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t >= 0 && t < a.T) {
+    if (t >= 0 && t < nin) {
       v = __ldg(xb + (long long)t * C4 + c4);
       v.x = v.x > 0.f ? v.x : v.x * a.in_slope;
       v.y = v.y > 0.f ? v.y : v.y * a.in_slope;
@@ -358,7 +359,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 #pragma unroll 8
     for (int c = 0; c < C; c++) acc = fmaf(xr[c], wj[c], acc);
   }
-  a.wav[(long long)b * a.T + t] = tanhf(acc);
+  a.wav[(long long)b * a.T + t] = t < nin ? tanhf(acc) : 0.f;
 }
 
 // The generator's own shape (32 channels, 7 taps, hifigan/models.py:131): no shared memory at all.  Eight lanes own one time row (one
@@ -368,7 +369,8 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 // full 32-byte sectors.  (The staged kernel above issues two shared-memory loads per FMA and measured 263 us = 2.0 TB/s at
 // B = 16 x 259k samples; this one is bound by the single read of x.)
 constexpr int CPF_BLOCKS = 18;                         // row blocks of TAPS rows per 8-lane group
-template <int TAPS>
+// RAG: ragged batch (a.lens != NULL); a template parameter so that the padded path keeps its code and registers
+template <int TAPS, bool RAG>
 __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups) {
   constexpr int PAD = (TAPS - 1) / 2, ROWS = CPF_BLOCKS * TAPS - 2 * PAD;     // output rows per group (120 for 7 taps: a multiple of 8)
   static_assert(ROWS % 8 == 0, "full 8-sample stores");
@@ -380,6 +382,7 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
   const int t0 = (int)(grp - (long long)b * groups_per_batch) * ROWS;
   const int T = live ? a.T : 0;
   const int tend = min(t0 + ROWS, T);
+  const int nin = RAG ? ragged_rows(a.lens, a.lens_scale, T, b) : T;   // ragged batch: rows >= n_b read as zero, wav there is 0
   float4 w[TAPS];
 #pragma unroll
   for (int j = 0; j < TAPS; j++) w[j] = __ldg(reinterpret_cast<const float4*>(a.w + j * 32) + sub);
@@ -397,7 +400,7 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
 #pragma unroll
     for (int i = 0; i < TAPS; i++) {
       const int r = rb + i;
-      x[i] = (r >= 0 && r < T) ? __ldg(xb + (long long)r * 8) : make_float4(0.f, 0.f, 0.f, 0.f);
+      x[i] = (r >= 0 && r < nin) ? __ldg(xb + (long long)r * 8) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
     for (int i = 0; i < TAPS; i++) {
@@ -422,7 +425,7 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
         const int o = (t - t0) & 7;
         if (o == sub) keep = tot;
         if (o == 7 || t == tend - 1) {
-          if (sub <= o) wb[t - o + sub] = tanhf(keep + bias);
+          if (sub <= o) wb[t - o + sub] = (!RAG || t - o + sub < nin) ? tanhf(keep + bias) : 0.f;
         }
       }
     }
@@ -431,13 +434,15 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
 
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s) {
   if (!a || !a->x || !a->w || !a->bias || !a->wav || a->B <= 0 || a->T <= 0 || a->C <= 0 || a->taps <= 0) return FS2_ERR_ARG;
+  if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
   if (a->C == 32 && a->taps == 7 && (reinterpret_cast<uintptr_t>(a->x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15u) == 0) {
     constexpr int ROWS = CPF_BLOCKS * 7 - 6;
     const int gpb = (a->T + ROWS - 1) / ROWS;
     const long long n_groups = (long long)gpb * a->B, blocks = (n_groups * 8 + 255) / 256;
     if (blocks > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
     prof_before(s);
-    conv_post_c32_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups);
+    if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups);
+    else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups);
     prof_after(s, 3, 2.0 * (double)a->B * a->T * a->taps * a->C);
     FS2_LAUNCH_CHECK();
     return FS2_OK;

@@ -2,6 +2,7 @@
 
     import fastspeech2_b200.dropin as dropin; dropin.install()           # programmatic
     python -m fastspeech2_b200.dropin synthesize.py --text ... -p ... -m ... -t ...   # run the untouched reference CLI
+    python -m fastspeech2_b200.dropin --ragged-vocoder synthesize.py --mode batch ...  # ... vocoding each utterance on its own frames
 
 `utils/model.py:7-8` does `import hifigan` and `from model import FastSpeech2, ScheduledOptim`; both names are bound here
 to `fastspeech2_b200.hifigan` / `fastspeech2_b200.model`, whose classes keep the reference's constructor arguments,
@@ -9,6 +10,7 @@ state_dict keys, forward signatures and return values (see INTEGRATION.md).
 """
 from __future__ import annotations
 
+import functools
 import os
 import runpy
 import sys
@@ -27,18 +29,34 @@ def install(force: bool = False) -> None:
 _pinned = {}
 
 
-def vocoder_infer(mels, vocoder, model_config, preprocess_config, lengths=None):
+def vocoder_infer(mels, vocoder, model_config, preprocess_config, lengths=None, ragged=False):
     """Drop-in for the reference's `utils.model.vocoder_infer` (utils/model.py:74-92), same arguments and return value (a list of
     int16 numpy arrays, one per utterance, trimmed to `lengths[i]` samples).  The reference copies the fp32 waveform to the host
     and converts / trims there; here `x max_wav_value -> int16` and the trim run on the device (fs2_wav_to_int16), so 2 bytes per
-    sample cross PCIe, into pinned memory, asynchronously on the compute stream."""
+    sample cross PCIe, into pinned memory, asynchronously on the compute stream.
+
+    ragged=True vocodes every utterance on its own lengths[i] / prod(upsample_rates) mel frames (Generator.forward's mel_lens):
+    the padded frames of a batch are neither read nor computed, so a short utterance no longer depends on its batch neighbours
+    and the result equals the utterance synthesised alone.  Needs `lengths`, each a multiple of prod(upsample_rates)
+    (the reference passes mel_lens * hop_length); ValueError otherwise."""
     import torch
 
     from . import ops
     if model_config["vocoder"]["model"] != "HiFi-GAN":
         raise NotImplementedError("the H100-native path serves the vendored HiFi-GAN vocoder only (MelGAN needs a network fetch upstream)")
+    mel_lens = None
+    if ragged:
+        if lengths is None:
+            raise ValueError("ragged vocoding needs the per-utterance lengths")
+        up = 1
+        for u in vocoder.h["upsample_rates"] if isinstance(vocoder.h, dict) else vocoder.h.upsample_rates:
+            up *= int(u)
+        lens = torch.as_tensor(lengths).long()
+        if bool((lens % up != 0).any()):
+            raise ValueError(f"ragged vocoding needs lengths that are multiples of prod(upsample_rates) = {up}")
+        mel_lens = lens // up
     with torch.no_grad():
-        wav = vocoder(mels)                                    # [B, 1, N] fp32 on the device
+        wav = vocoder(mels) if mel_lens is None else vocoder(mels, mel_lens=mel_lens)   # [B, 1, N] fp32 on the device
     scale = float(preprocess_config["preprocessing"]["audio"]["max_wav_value"])
     B, _, N = wav.shape
     lens_d = None if lengths is None else torch.as_tensor(lengths).to(wav.device)
@@ -54,14 +72,15 @@ def vocoder_infer(mels, vocoder, model_config, preprocess_config, lengths=None):
     return [arr[i, : (N if lens_h is None else lens_h[i])].copy() for i in range(B)]
 
 
-def patch_vocoder_infer() -> bool:
+def patch_vocoder_infer(ragged: bool = False) -> bool:
     """Rebind `utils.model.vocoder_infer` of the (already importable) reference tree to the device-side version; `utils.tools.synth_samples`
-    looks the name up at call time (utils/tools.py:200), so the shipped CLI picks it up unchanged."""
+    looks the name up at call time (utils/tools.py:200), so the shipped CLI picks it up unchanged.  ragged=True binds the version
+    that vocodes each utterance on its own frames (vocoder_infer(..., ragged=True))."""
     try:
         import utils.model as um
     except Exception:
         return False
-    um.vocoder_infer = vocoder_infer
+    um.vocoder_infer = functools.partial(vocoder_infer, ragged=True) if ragged else vocoder_infer
     return True
 
 
@@ -79,13 +98,17 @@ def patch_text_dataset() -> bool:
 
 def main(argv=None) -> None:
     argv = list(sys.argv[1:] if argv is None else argv)
+    ragged = False
+    while argv and argv[0] == "--ragged-vocoder":      # our flags come before the script path; everything after it is the script's
+        ragged = True
+        argv.pop(0)
     if not argv:
-        raise SystemExit("usage: python -m fastspeech2_b200.dropin <reference script, e.g. synthesize.py> [script args...]")
+        raise SystemExit("usage: python -m fastspeech2_b200.dropin [--ragged-vocoder] <reference script, e.g. synthesize.py> [script args...]")
     script = os.path.abspath(argv[0])
     install()
     sys.argv = [script] + argv[1:]
     sys.path.insert(0, os.path.dirname(script))       # the reference resolves `utils`, `text`, `dataset` relative to itself
-    patch_vocoder_infer()
+    patch_vocoder_infer(ragged=ragged)
     patch_text_dataset()
     runpy.run_path(script, run_name="__main__")
 

@@ -152,13 +152,20 @@ class Generator(nn.Module):
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
-    def forward(self, x):
-        """x: mel [B, 80, T] (any strides; the usual caller passes postnet_mel.transpose(1, 2), utils/tools.py:202)."""
+    def forward(self, x, mel_lens=None):
+        """x: mel [B, 80, T] (any strides; the usual caller passes postnet_mel.transpose(1, 2), utils/tools.py:202).
+
+        mel_lens (optional): integer tensor [B] of valid frames per utterance, on any device (FastSpeech2's out[9] can be passed
+        straight in).  Utterance b is then synthesised exactly as `self(x[b:b+1, :, :mel_lens[b]])` would synthesise it alone: frames
+        at or beyond mel_lens[b] are never read, the vocoder skips the work of the padding, and wav[b, 0, t] = 0 for
+        t >= mel_lens[b] * prod(upsample_rates).  The output shape stays [B, 1, prod(upsample_rates) * T].  Without mel_lens every
+        utterance is synthesised over all T frames, padding included, as the reference does.  A CPU tensor is range-checked
+        (ValueError outside [0, T]); device values are clamped to [0, T] by the kernels."""
         dev = get(self, "conv_pre.bias").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):   # per-device kernel setup: CURRENT device
-            return self._forward(x)
+            return self._forward(x, mel_lens)
 
-    def _forward(self, x):
+    def _forward(self, x, mel_lens=None):
         if self.training:
             raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
         lib = L.lib()
@@ -167,6 +174,14 @@ class Generator(nn.Module):
             raise ValueError(f"expected mel of shape [B, {m.n_mel}, T]")
         x = x.to(device=dev, dtype=torch.float32)
         B, _, T = x.shape
+        lens_d = None
+        if mel_lens is not None:
+            mel_lens = torch.as_tensor(mel_lens)
+            if mel_lens.dtype.is_floating_point or mel_lens.dtype.is_complex or mel_lens.dtype == torch.bool or mel_lens.shape != (B,):
+                raise ValueError(f"mel_lens must be an integer tensor of shape [{B}]")
+            if mel_lens.device.type == "cpu" and B and not bool(((mel_lens >= 0) & (mel_lens <= T)).all()):
+                raise ValueError(f"mel_lens must lie in [0, {T}]")
+            lens_d = mel_lens.to(device=dev, dtype=torch.int32).contiguous()
         stream = torch.cuda.current_stream(dev).cuda_stream
         if x.stride(1) == 1 and x.stride(2) % 4 == 0 and x.stride(0) % 4 == 0 and x.data_ptr() % 16 == 0 and x.stride(2) >= m.n_mel:
             mel_cl, bs, rs = x, x.stride(0), x.stride(2)       # already a channels-last view
@@ -180,6 +195,6 @@ class Generator(nn.Module):
         if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
             self._ws = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
         va = L.VocoderArgs(B=B, T=T, mel=mel_cl.data_ptr(), mel_batch_stride=bs, mel_row_stride=rs, wav=wav.data_ptr(),
-                           workspace=self._ws.data_ptr(), workspace_bytes=self._ws.numel())
+                           workspace=self._ws.data_ptr(), workspace_bytes=self._ws.numel(), mel_lens=L.ptr(lens_d))
         L.check(lib.fs2_vocoder_forward(C.byref(m), C.byref(va), stream), "fs2_vocoder_forward")
         return wav

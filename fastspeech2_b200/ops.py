@@ -19,8 +19,11 @@ def _need_cuda(t):
 
 
 def conv1d(x, w, bias=None, *, dilation=1, pad_left=0, in_act=L.ACT_NONE, in_slope=0.0, out_act=L.ACT_NONE, out_slope=0.0,
-           res=None, alpha=1.0, out=None, accumulate=False, row_lens=None, w_tc=None, backend=L.CONV_AUTO, tc_variant=0):
-    """x [B,T,Cin] (row-strided ok), w [taps][Cin][N] -> y [B,T,N].  `out` may be a strided [B,T,N] view."""
+           res=None, alpha=1.0, out=None, accumulate=False, row_lens=None, w_tc=None, backend=L.CONV_AUTO, tc_variant=0,
+           x_lens=None, lens_scale=1):
+    """x [B,T,Cin] (row-strided ok), w [taps][Cin][N] -> y [B,T,N].  `out` may be a strided [B,T,N] view.
+    x_lens: int32 [B] on the device (ragged batch): utterance b is computed on its first min(x_lens[b] * lens_scale, T) rows only,
+    as if alone; the output rows after them are unspecified."""
     _need_cuda(x)
     B, T, Cin = x.shape
     taps, _, N = w.shape
@@ -34,7 +37,8 @@ def conv1d(x, w, bias=None, *, dilation=1, pad_left=0, in_act=L.ACT_NONE, in_slo
                      res=L.ptr(res), res_batch_stride=res.stride(0) if res is not None else 0,
                      res_row_stride=res.stride(1) if res is not None else 0,
                      alpha=alpha, accumulate=int(accumulate), row_lens=L.ptr(row_lens),
-                     y=out.data_ptr(), y_batch_stride=out.stride(0), y_row_stride=out.stride(1))
+                     y=out.data_ptr(), y_batch_stride=out.stride(0), y_row_stride=out.stride(1),
+                     x_lens=L.ptr(x_lens), lens_scale=int(lens_scale))
     L.check(L.lib().fs2_conv1d(C.byref(a), _stream(x.device)), "fs2_conv1d")
     return out
 
@@ -128,25 +132,28 @@ def length_regulate(x, cum, T, pos=None):
     return y
 
 
-def conv_post(x, w, bias, in_slope=0.01):
+def conv_post(x, w, bias, in_slope=0.01, lens=None, lens_scale=1):
+    """tanh(conv(lrelu(x))) -> wav [B,T].  lens: int32 [B] on the device (ragged batch): wav[b, t] = 0 for t >= lens[b] * lens_scale,
+    and the rows before that are computed as if the utterance were alone."""
     _need_cuda(x)
     B, T, Cc = x.shape
     wav = torch.empty(B, T, dtype=torch.float32, device=x.device)
     a = L.ConvPostArgs(x=x.data_ptr(), B=B, T=T, C=Cc, w=w.data_ptr(), bias=bias.data_ptr(), taps=w.shape[0], in_slope=in_slope,
-                       wav=wav.data_ptr())
+                       wav=wav.data_ptr(), lens=L.ptr(lens), lens_scale=int(lens_scale))
     L.check(L.lib().fs2_conv_post(C.byref(a), _stream(x.device)), "fs2_conv_post")
     return wav
 
 
-def resstack(x, kernels, dilations, w1_tc, b1, w2_tc, b2, alpha=0.0, out=None, accumulate=False):
+def resstack(x, kernels, dilations, w1_tc, b1, w2_tc, b2, alpha=0.0, out=None, accumulate=False, lens=None, lens_scale=1):
     """Fused multi-receptive-field ResBlock group (fs2_resstack).  x [B,N,C] contiguous; kernels [k_j]; dilations [[d...] per j];
-    w1_tc / w2_tc [j][d]: pack_conv_tc(w, f8=True) tiles; b1 / b2 [j][d]: biases."""
+    w1_tc / w2_tc [j][d]: pack_conv_tc(w, f8=True) tiles; b1 / b2 [j][d]: biases.  lens: int32 [B] on the device (ragged batch):
+    utterance b is computed on its first min(lens[b] * lens_scale, N) rows as if alone; the output rows after them are unspecified."""
     _need_cuda(x)
     B, N, Cc = x.shape
     assert x.is_contiguous()
     y = torch.empty_like(x) if out is None else out
     a = L.ResstackArgs(x=x.data_ptr(), y=y.data_ptr(), B=B, N=N, C=Cc, n_kernels=len(kernels), n_dil=len(dilations[0]),
-                       alpha=float(alpha), accumulate=int(accumulate))
+                       alpha=float(alpha), accumulate=int(accumulate), lens=L.ptr(lens), lens_scale=int(lens_scale))
     for j, k in enumerate(kernels):
         a.k[j] = k
         for d, dv in enumerate(dilations[j]):

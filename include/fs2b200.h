@@ -110,6 +110,13 @@ typedef struct fs2_conv1d_args {
   float alpha; int accumulate;
   const int32_t* row_lens; /* [B] or NULL */
   float* y; int64_t y_batch_stride, y_row_stride;
+  /* Ragged batch: NULL, or [B] per-utterance lengths.  Utterance b then has n_b = clamp(x_lens[b] * lens_scale, 0, T) rows: input rows
+   * t >= n_b read as zero (as rows outside [0, T) do), output rows t >= n_b are unspecified (row_lens still zeroes rows >= row_lens[b]
+   * where they are written), and no work item lying wholly at or beyond n_b runs -- so utterance b is computed exactly as a B = 1 call
+   * on its first n_b rows.  lens_scale (rows per length unit, e.g. 256 when x_lens holds mel frames and the rows are audio samples)
+   * must be >= 1 when x_lens is given (FS2_ERR_ARG before any CUDA call).  The tensor-core kernel's grid is still sized from the padded
+   * shape (the host never reads device lengths); CTAs left without work exit. */
+  const int32_t* x_lens; int lens_scale;
 } fs2_conv1d_args;
 int fs2_conv1d(const fs2_conv1d_args* a, fs2_stream_t stream);
 
@@ -175,9 +182,13 @@ typedef struct fs2_length_regulate_args {
 } fs2_length_regulate_args;
 int fs2_length_regulate(const fs2_length_regulate_args* a, fs2_stream_t stream);
 
-/* wav[b,t] = tanh( *bias + sum_{j<taps} sum_c lrelu_slope(x[b,t+j-pad,c]) * w[j][c] )   (hifigan/models.py:161-163) */
+/* wav[b,t] = tanh( *bias + sum_{j<taps} sum_c lrelu_slope(x[b,t+j-pad,c]) * w[j][c] )   (hifigan/models.py:161-163)
+ * lens: NULL, or [B] per-utterance lengths with n_b = clamp(lens[b] * lens_scale, 0, T) (lens_scale >= 1, else FS2_ERR_ARG): rows
+ * t >= n_b of x read as zero and wav[b,t] = 0 exactly for t >= n_b, i.e. each utterance is the waveform of a B = 1 call on its first
+ * n_b rows followed by silence. */
 typedef struct fs2_conv_post_args {
   const float* x; int B, T, C; const float* w; const float* bias; int taps; float in_slope; float* wav;
+  const int32_t* lens; int lens_scale;
 } fs2_conv_post_args;
 int fs2_conv_post(const fs2_conv_post_args* a, fs2_stream_t stream);
 
@@ -196,6 +207,10 @@ typedef struct fs2_resstack_args {
   float alpha;     /* weight of every kernel size's result; <= 0: 1/n_kernels (the mean) */
   int accumulate;  /* 1: y += ... (also for the first kernel size) instead of y = ...; with n_kernels = n_dil = 1 the call is ONE fused
                       conv pair  y (+)= alpha * (conv_k,1(lrelu(conv_k,d(lrelu(x)))) + x)  -- the per-pair mode of the 64-channel stage */
+  /* Ragged batch: NULL, or [B] per-utterance lengths, n_b = clamp(lens[b] * lens_scale, 0, N) rows (lens_scale >= 1, else FS2_ERR_ARG):
+   * rows >= n_b of x read as zero and every conv pads at row n_b, rows >= n_b of y are unspecified, and only the work items that
+   * hold a row < n_b run.  The grid is sized from the padded shape (fs2_resstack_plan does not read lengths); CTAs without work exit. */
+  const int32_t* lens; int lens_scale;
 } fs2_resstack_args;
 int fs2_resstack(const fs2_resstack_args* a, fs2_stream_t stream);
 /* launch plan (pure host logic): out[12] = {128-row tiles per slab, halo rows per side, output rows per work item, work items, grid,
@@ -324,6 +339,11 @@ typedef struct fs2_vocoder_args {
   const float* mel; int64_t mel_batch_stride, mel_row_stride; /* channels-last view [B][T][n_mel] */
   float* wav;                                                  /* [B][T*prod(rates)] */
   void* workspace; size_t workspace_bytes;
+  /* Ragged mode: NULL (every utterance is synthesised over all T frames, as the reference does), or [B] mel-frame lengths (device,
+   * clamped to [0, T]): utterance b is then synthesised exactly as a B = 1 call on its first mel_lens[b] frames, frames at or beyond
+   * mel_lens[b] are never read, and wav[b, t] = 0 for t >= mel_lens[b] * prod(rates).  Every layer bounds its rows by the same array
+   * (fs2_conv1d x_lens / fs2_resstack lens / fs2_conv_post lens with the layer's frames-to-rows factor as lens_scale). */
+  const int32_t* mel_lens;
 } fs2_vocoder_args;
 size_t fs2_vocoder_workspace_bytes(const fs2_vocoder_model* m, int B, int T);
 int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, fs2_stream_t stream);

@@ -341,14 +341,8 @@ int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cuda
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);
   if (!dv) return derr;
-  if (!dv->att_fused_ready.load(std::memory_order_acquire)) {
-    DevOnce once;
-    if (!dv->att_fused_ready.load(std::memory_order_relaxed)) {
-      cudaError_t e = cudaFuncSetAttribute(attention_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AF_SMEM);
-      if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
-      dv->att_fused_ready.store(true, std::memory_order_release);
-    }
-  }
+  FS2_TRY(dev_once(dv->att_fused_ready,
+                   [] { return cudaFuncSetAttribute(attention_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AF_SMEM); }));
   const int Tk = (a->T + 127) / 128 * 128;
   char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
   const long long tstride = af_tile_stride(Tk);

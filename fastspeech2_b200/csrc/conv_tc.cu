@@ -106,18 +106,14 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // state of the CURRENT device: the caller's stream must belong to it
   if (!dv) return derr;
-  if (!dv->conv_tc_ready.load(std::memory_order_acquire)) {
-    DevOnce once;
-    if (!dv->conv_tc_ready.load(std::memory_order_relaxed)) {
-      const int mx = 227 * 1024;
-      cudaError_t e = cudaSuccess;
-      for (cudaError_t (*prep)(int) : {conv_tc_prepare_nb16, conv_tc_prepare_nb32, conv_tc_prepare_nb48, conv_tc_prepare_nb64,
-                                       conv_tc_prepare_nb80, conv_tc_prepare_nb96, conv_tc_prepare_nb112, conv_tc_prepare_nb128})
-        if (e == cudaSuccess) e = prep(mx);
-      if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
-      dv->conv_tc_ready.store(true, std::memory_order_release);
-    }
-  }
+  FS2_TRY(dev_once(dv->conv_tc_ready, [] {
+    const int mx = 227 * 1024;
+    cudaError_t e = cudaSuccess;
+    for (cudaError_t (*prep)(int) : {conv_tc_prepare_nb16, conv_tc_prepare_nb32, conv_tc_prepare_nb48, conv_tc_prepare_nb64,
+                                     conv_tc_prepare_nb80, conv_tc_prepare_nb96, conv_tc_prepare_nb112, conv_tc_prepare_nb128})
+      if (e == cudaSuccess) e = prep(mx);
+    return e;
+  }));
   const int g_num_sms = dv->num_sms.load(std::memory_order_relaxed);
   TcP p{};
   p.x = a->x; p.xbs = a->x_batch_stride; p.xrs = a->x_row_stride;

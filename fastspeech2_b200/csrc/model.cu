@@ -32,8 +32,15 @@ DevState* dev_state(int* err) {
   }
   return d;
 }
-DevOnce::DevOnce() { g_dev_mutex.lock(); }
-DevOnce::~DevOnce() { g_dev_mutex.unlock(); }
+int dev_once(std::atomic<bool>& ready, cudaError_t (*setup)()) {
+  if (ready.load(std::memory_order_acquire)) return FS2_OK;
+  std::lock_guard<std::mutex> lock(g_dev_mutex);
+  if (ready.load(std::memory_order_relaxed)) return FS2_OK;
+  const cudaError_t e = setup();
+  if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
+  ready.store(true, std::memory_order_release);
+  return FS2_OK;
+}
 
 // ------------------------------------------------------------------ per-launch profiling (off unless armed; state is per host thread)
 thread_local bool g_prof_on = false;
@@ -100,92 +107,84 @@ struct Arena {
   }
 };
 
-// contiguous [B][T][C] convolution helper
-static int conv(cudaStream_t s, const float* x, int B, int T, int Cin, const float* w, const float* w_tc, const float* bias, int N,
-                int taps, int dil, int pad, int out_act, float out_slope, float* y, const float* res = nullptr,
-                int in_act = FS2_ACT_NONE, float in_slope = 0.f, float alpha = 1.f, int accumulate = 0,
-                const int32_t* row_lens = nullptr, unsigned tc_variant = 0, const int32_t* x_lens = nullptr, int lens_scale = 1) {
-  fs2_conv1d_args a{};
-  a.w_tc = w_tc; a.backend = FS2_CONV_AUTO; a.tc_variant = tc_variant;
-  a.x = x; a.x_batch_stride = (int64_t)T * Cin; a.x_row_stride = Cin;
-  a.B = B; a.T = T; a.Cin = Cin;
-  a.w = w; a.bias = bias; a.N = N; a.taps = taps; a.dilation = dil; a.pad_left = pad;
-  a.in_act = in_act; a.in_slope = in_slope; a.out_act = out_act; a.out_slope = out_slope;
-  a.res = res; a.res_batch_stride = (int64_t)T * N; a.res_row_stride = N;
-  a.alpha = alpha; a.accumulate = accumulate; a.row_lens = row_lens;
-  a.y = y; a.y_batch_stride = (int64_t)T * N; a.y_row_stride = N;
-  a.x_lens = x_lens; a.lens_scale = lens_scale;
-  return conv1d_dispatch(&a, s);
-}
-
-static int ln(cudaStream_t s, const float* x, float* y, int B, int T, int C, const float* g, const float* b, const int32_t* lens,
-              int pre_relu = 0) {
-  fs2_layernorm_args a{x, y, B, T, C, g, b, 1e-5f, lens, pre_relu};
-  return layernorm(&a, s);
-}
-
-// K-segmented tensor-core convolution for the layers that feed the discrete decisions (encoder, predictors): the sum over taps and
-// input channels is cut into (tap, 256-channel) slices; each slice is one work unit of 16 K-steps with separate accumulators for
-// the hi*hi term and the cross terms (FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED, one launch per conv), and the slices are added in
-// fp32 round-to-nearest by the epilogue's accumulate path.  That bounds the tensor core's truncating accumulation to 16 steps per chain (a single k = 9 launch has 432) and
-// brings the error back to the fp32 CUDA-core kernel's level (scripts/flip_census.py).  `w_seg`: taps * (Cin/256) tile
-// buffers of 128 + 1024*N bytes (packing.pack_conv_tc_segments).  y = bias + sum_slices + res, rows >= row_lens zeroed; no output
-// activation (a following ReLU is applied by the consumer: in_act of the next conv / pre_relu of the LayerNorm).
-static int conv_seg(cudaStream_t s, const float* x, int B, int T, int Cin, const float* w_seg, const float* bias, int N, int taps, int pad,
-                    float* y, const float* res, int in_act, float in_slope, const int32_t* row_lens) {
+// fs2_conv1d arguments for contiguous [B][T][Cin] input, [B][T][N] output and residual, `taps` with "same" padding at dilation 1.
+// The rest starts at its identity: bias and residual off, alpha 1, no activations, FS2_CONV_AUTO, no row_lens / x_lens.
+// Call sites set the weights and whatever else differs by field name.
+static fs2_conv1d_args conv_args(const float* x, int B, int T, int Cin, int N, int taps, float* y) {
   fs2_conv1d_args a{};
   a.x = x; a.x_batch_stride = (int64_t)T * Cin; a.x_row_stride = Cin;
   a.B = B; a.T = T; a.Cin = Cin;
-  a.w = nullptr; a.w_tc = w_seg; a.backend = FS2_CONV_TC; a.tc_variant = FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED;
-  a.bias = bias; a.N = N; a.taps = taps; a.dilation = 1; a.pad_left = pad;
-  a.in_act = in_act; a.in_slope = in_slope; a.out_act = FS2_ACT_NONE;
-  a.res = res; a.res_batch_stride = (int64_t)T * N; a.res_row_stride = N;
-  a.alpha = 1.f; a.accumulate = 0; a.row_lens = row_lens;
+  a.N = N; a.taps = taps; a.dilation = 1; a.pad_left = (taps - 1) / 2;
+  a.backend = FS2_CONV_AUTO; a.alpha = 1.f;
+  a.res_batch_stride = (int64_t)T * N; a.res_row_stride = N;
   a.y = y; a.y_batch_stride = (int64_t)T * N; a.y_row_stride = N;
-  return conv1d_tc(&a, s);
+  a.lens_scale = 1;
+  return a;
 }
+
+// How the convs of one FFT block, variance predictor or the decoder's mel_linear + PostNet run, decided once per block.
+//  EXACT:     fp32 CUDA-core kernel (w_tc is not passed).
+//  TC:        split-precision tensor-core kernel with variant `tcv` wherever conv1d_dispatch supports the shape.
+//  SEGMENTED: K-segmented tensor-core convolution for the layers that feed the discrete decisions (encoder, predictors): the sum over
+//             taps and input channels is cut into (tap, 256-channel) slices; each slice is one work unit of 16 K-steps with separate
+//             accumulators for the hi*hi term and the cross terms (FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED, one launch per
+//             conv), and the slices are added in fp32 round-to-nearest by the epilogue's accumulate path.  That bounds the tensor
+//             core's truncating accumulation to 16 steps per chain (a single k = 9 launch has 432) and brings the error back to the
+//             fp32 CUDA-core kernel's level (scripts/flip_census.py).  w_tc: taps * (Cin/256) tile buffers of 128 + 1024*N bytes
+//             (packing.pack_conv_tc_segments).  No output activation: a following ReLU is applied by the consumer (in_act of the
+//             next conv / pre_relu of the LayerNorm).
+struct ConvMode {
+  enum { EXACT, TC, SEGMENTED } path;
+  unsigned tcv;
+  void weights(fs2_conv1d_args& a, const float* w, const float* w_tc, const float* bias) const {
+    a.bias = bias;
+    if (path == SEGMENTED) {
+      a.w = nullptr; a.w_tc = w_tc; a.backend = FS2_CONV_TC; a.tc_variant = FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED;
+    } else {
+      a.w = w; a.w_tc = path == TC ? w_tc : nullptr; a.tc_variant = tcv;
+    }
+  }
+};
 
 struct FftBufs { float *x, *tmp, *qkv, *ctx, *hid; void* att_ws; size_t att_bytes; };
 
 // One FFT block in place on bufs.x  (transformer/Layers.py:21-30)
 static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_block_weights& w, const FftBufs& f, int B, int T,
-                     const int32_t* lens, bool tc, unsigned tcv, bool segmented = false) {
+                     const int32_t* lens, ConvMode mode) {
   const int D = m->d_model, F = m->d_inner;
-  const float* none = nullptr;
-  if (segmented) {                                     // encoder on the tensor cores: K-segmented convs, exact attention
-    if (!w.w_qkv_tc || !w.w_o_tc || !w.w_1_tc || !w.w_2_tc || m->k2 != 1) return FS2_ERR_ARG;
-    FS2_TRY(conv_seg(s, f.x, B, T, D, w.w_qkv_tc, w.b_qkv, 3 * D, 1, 0, f.qkv, nullptr, FS2_ACT_NONE, 0.f, nullptr));
-    fs2_attention_args at{};
-    at.qkv = f.qkv; at.ctx = f.ctx; at.B = B; at.T = T; at.H = m->n_head; at.Dh = D / m->n_head; at.key_lens = lens;
-    at.scale = 1.0f / sqrtf((float)(D / m->n_head));
-    FS2_TRY(attention_simt(&at, s));
-    FS2_TRY(conv_seg(s, f.ctx, B, T, D, w.w_o_tc, w.b_o, D, 1, 0, f.tmp, f.x, FS2_ACT_NONE, 0.f, nullptr));
-    FS2_TRY(ln(s, f.tmp, f.x, B, T, D, w.ln1_g, w.ln1_b, lens));
-    // conv-FFN: w_1 leaves the pre-activation hidden, the ReLU is w_2's input activation (leaky_relu with slope 0)
-    FS2_TRY(conv_seg(s, f.x, B, T, D, w.w_1_tc, w.b_1, F, m->k1, (m->k1 - 1) / 2, f.hid, nullptr, FS2_ACT_NONE, 0.f, nullptr));
-    FS2_TRY(conv_seg(s, f.hid, B, T, F, w.w_2_tc, w.b_2, D, 1, 0, f.tmp, f.x, FS2_ACT_LRELU, 0.f, nullptr));
-    FS2_TRY(ln(s, f.tmp, f.x, B, T, D, w.ln2_g, w.ln2_b, lens));
-    return FS2_OK;
-  }
-  FS2_TRY(conv(s, f.x, B, T, D, w.w_qkv, tc ? w.w_qkv_tc : none, w.b_qkv, 3 * D, 1, 1, 0, FS2_ACT_NONE, 0.f, f.qkv, nullptr, FS2_ACT_NONE, 0.f,
-               1.f, 0, nullptr, tcv));
+  const bool seg = mode.path == ConvMode::SEGMENTED;
+  if (seg && (!w.w_qkv_tc || !w.w_o_tc || !w.w_1_tc || !w.w_2_tc || m->k2 != 1)) return FS2_ERR_ARG;
+  fs2_conv1d_args c = conv_args(f.x, B, T, D, 3 * D, 1, f.qkv);
+  mode.weights(c, w.w_qkv, w.w_qkv_tc, w.b_qkv);
+  FS2_TRY(conv1d_dispatch(&c, s));
   fs2_attention_args at{};
   at.qkv = f.qkv; at.ctx = f.ctx; at.B = B; at.T = T; at.H = m->n_head; at.Dh = D / m->n_head; at.key_lens = lens;
   at.scale = 1.0f / sqrtf((float)(D / m->n_head));
-  if (tc && f.att_ws && T >= 128) {                                   // one fused tensor-core kernel: S stays in registers, any length
+  if (mode.path == ConvMode::TC && f.att_ws && T >= 128) {           // one fused tensor-core kernel: S stays in registers, any length
     FS2_TRY(attention_fused(&at, f.att_ws, f.att_bytes, s));
   } else {
     FS2_TRY(attention_simt(&at, s));
   }
-  FS2_TRY(conv(s, f.ctx, B, T, D, w.w_o, tc ? w.w_o_tc : none, w.b_o, D, 1, 1, 0, FS2_ACT_NONE, 0.f, f.tmp, f.x, FS2_ACT_NONE, 0.f, 1.f, 0, nullptr,
-               tcv));
-  FS2_TRY(ln(s, f.tmp, f.x, B, T, D, w.ln1_g, w.ln1_b, lens));
-  FS2_TRY(conv(s, f.x, B, T, D, w.w_1, tc ? w.w_1_tc : none, w.b_1, F, m->k1, 1, (m->k1 - 1) / 2, FS2_ACT_RELU, 0.f, f.hid, nullptr, FS2_ACT_NONE,
-               0.f, 1.f, 0, nullptr, tcv));
-  FS2_TRY(conv(s, f.hid, B, T, F, w.w_2, tc ? w.w_2_tc : none, w.b_2, D, m->k2, 1, (m->k2 - 1) / 2, FS2_ACT_NONE, 0.f, f.tmp, f.x, FS2_ACT_NONE,
-               0.f, 1.f, 0, nullptr, tcv));
-  FS2_TRY(ln(s, f.tmp, f.x, B, T, D, w.ln2_g, w.ln2_b, lens));
-  return FS2_OK;
+  c = conv_args(f.ctx, B, T, D, D, 1, f.tmp);
+  mode.weights(c, w.w_o, w.w_o_tc, w.b_o);
+  c.res = f.x;
+  FS2_TRY(conv1d_dispatch(&c, s));
+  fs2_layernorm_args n{};                                           // both LayerNorms: tmp -> x, padded rows zeroed
+  n.x = f.tmp; n.y = f.x; n.B = B; n.T = T; n.C = D; n.eps = 1e-5f; n.row_lens = lens;
+  n.gamma = w.ln1_g; n.beta = w.ln1_b;
+  FS2_TRY(layernorm(&n, s));
+  // conv-FFN.  K-segmented: w_1 leaves the pre-activation hidden and the ReLU is w_2's input activation (leaky_relu with slope 0)
+  c = conv_args(f.x, B, T, D, F, m->k1, f.hid);
+  mode.weights(c, w.w_1, w.w_1_tc, w.b_1);
+  if (!seg) c.out_act = FS2_ACT_RELU;
+  FS2_TRY(conv1d_dispatch(&c, s));
+  c = conv_args(f.hid, B, T, F, D, m->k2, f.tmp);
+  mode.weights(c, w.w_2, w.w_2_tc, w.b_2);
+  c.res = f.x;
+  if (seg) { c.in_act = FS2_ACT_LRELU; c.in_slope = 0.f; }
+  FS2_TRY(conv1d_dispatch(&c, s));
+  n.gamma = w.ln2_g; n.beta = w.ln2_b;
+  return layernorm(&n, s);
 }
 
 static bool model_ok(const fs2_acoustic_model* m) {
@@ -209,27 +208,31 @@ static FftBufs fft_bufs(Arena& ar, const fs2_acoustic_model* m, size_t rows, int
   return f;
 }
 
-// VariancePredictor.forward (+ bucketize / embedding add when bins != NULL) on rows [B][T]  (model/modules.py:242-250, :80-100)
-static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_predictor_weights& w, const float* x, int B, int T,
-                         const int32_t* lens, float control, const float* target, const float* bins, const float* emb, float* x_acc,
-                         float* pred_out, float* h1, float* h2) {
-  const int k = m->vp_kernel, D = m->d_model, VF = m->vp_filter;
-  if ((m->tc_mask & FS2_TC_PREDICTORS) && w.w_c1_tc && w.w_c2_tc) {   // tensor cores, K-segmented (conv_seg); ReLU applied by the LayerNorm
-    FS2_TRY(conv_seg(s, x, B, T, D, w.w_c1_tc, w.b_c1, VF, k, (k - 1) / 2, h1, nullptr, FS2_ACT_NONE, 0.f, nullptr));
-    FS2_TRY(ln(s, h1, h2, B, T, VF, w.ln1_g, w.ln1_b, nullptr, 1));
-    FS2_TRY(conv_seg(s, h2, B, T, VF, w.w_c2_tc, w.b_c2, VF, k, 1, h1, nullptr, FS2_ACT_NONE, 0.f, nullptr));   // padding=1 is hard-coded upstream
-    FS2_TRY(ln(s, h1, h2, B, T, VF, w.ln2_g, w.ln2_b, nullptr, 1));
-  } else {
-    FS2_TRY(conv(s, x, B, T, D, w.w_c1, nullptr, w.b_c1, VF, k, 1, (k - 1) / 2, FS2_ACT_RELU, 0.f, h1));
-    FS2_TRY(ln(s, h1, h2, B, T, VF, w.ln1_g, w.ln1_b, nullptr));
-    FS2_TRY(conv(s, h2, B, T, VF, w.w_c2, nullptr, w.b_c2, VF, k, 1, 1, FS2_ACT_RELU, 0.f, h1));  // padding=1 is hard-coded upstream
-    FS2_TRY(ln(s, h1, h2, B, T, VF, w.ln2_g, w.ln2_b, nullptr));
-  }
-  fs2_variance_head_args v{};
-  v.h = h2; v.w = w.w_out; v.b = w.b_out; v.B = B; v.L = T; v.C = VF;
-  v.lens = lens; v.control = control; v.target = target;
-  v.bins = bins; v.n_edges = m->n_bins - 1; v.emb = emb; v.D = D; v.x = x_acc; v.pred_out = pred_out;
-  return variance_head(&v, s);
+// VariancePredictor.forward (+ bucketize / embedding add when bins != NULL) on rows [B][T]  (model/modules.py:242-250, :80-100).
+// `head` carries the caller's part of the head's arguments: B, L = T, lens, control, target, bins, emb, pred_out, and x, which is
+// both the predictor's input and where the embedding is added.
+static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_predictor_weights& w, fs2_variance_head_args head,
+                         float* h1, float* h2) {
+  const int B = head.B, T = head.L, k = m->vp_kernel, D = m->d_model, VF = m->vp_filter;
+  const bool seg = (m->tc_mask & FS2_TC_PREDICTORS) && w.w_c1_tc && w.w_c2_tc;   // K-segmented: the ReLU is applied by the LayerNorm
+  const ConvMode mode{seg ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};
+  fs2_layernorm_args n{};                                           // both LayerNorms: h1 -> h2, unmasked
+  n.x = h1; n.y = h2; n.B = B; n.T = T; n.C = VF; n.eps = 1e-5f; n.pre_relu = seg;
+  fs2_conv1d_args c = conv_args(head.x, B, T, D, VF, k, h1);
+  mode.weights(c, w.w_c1, w.w_c1_tc, w.b_c1);
+  if (!seg) c.out_act = FS2_ACT_RELU;
+  FS2_TRY(conv1d_dispatch(&c, s));
+  n.gamma = w.ln1_g; n.beta = w.ln1_b;
+  FS2_TRY(layernorm(&n, s));
+  c = conv_args(h2, B, T, VF, VF, k, h1);
+  mode.weights(c, w.w_c2, w.w_c2_tc, w.b_c2);
+  c.pad_left = 1;                                                   // padding=1 is hard-coded upstream
+  if (!seg) c.out_act = FS2_ACT_RELU;
+  FS2_TRY(conv1d_dispatch(&c, s));
+  n.gamma = w.ln2_g; n.beta = w.ln2_b;
+  FS2_TRY(layernorm(&n, s));
+  head.h = h2; head.w = w.w_out; head.b = w.b_out; head.C = VF; head.n_edges = m->n_bins - 1; head.D = D;
+  return variance_head(&head, s);
 }
 
 // ------------------------------------------------------------------ phase 1
@@ -243,12 +246,15 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
   if (!f.x || !f.tmp || !f.qkv || !f.ctx || !f.hid || !h1 || !h2) return FS2_ERR_WORKSPACE;
   if (L > m->enc_pos_rows) return FS2_ERR_ARG;
 
-  fs2_embed_args e{a->texts, m->word_emb, m->enc_pos, f.x, B, L, D, m->n_vocab};
+  fs2_embed_args e{};
+  e.ids = a->texts; e.table = m->word_emb; e.pos = m->enc_pos; e.y = f.x; e.B = B; e.L = L; e.D = D; e.n_vocab = m->n_vocab;
   FS2_TRY(embed_positions(&e, s));
-  for (int i = 0; i < m->n_enc; i++) FS2_TRY(fft_block(s, m, m->enc[i], f, B, L, a->src_lens, false, 0, (m->tc_mask & FS2_TC_ENCODER) != 0));
+  const ConvMode enc_mode{(m->tc_mask & FS2_TC_ENCODER) ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};   // exact attention either way
+  for (int i = 0; i < m->n_enc; i++) FS2_TRY(fft_block(s, m, m->enc[i], f, B, L, a->src_lens, enc_mode));
   if (m->spk_emb) {
     if (!a->speakers) return FS2_ERR_ARG;
-    fs2_rowbias_args r{f.x, m->spk_emb, a->speakers, B, L, D, m->n_speakers};
+    fs2_rowbias_args r{};
+    r.x = f.x; r.table = m->spk_emb; r.idx = a->speakers; r.B = B; r.L = L; r.D = D; r.n_rows = m->n_speakers;
     FS2_TRY(add_speaker(&r, s));
   }
   // x_adapted starts as the encoder output; pitch / energy embeddings are added in place (modules.py:117-126)
@@ -256,16 +262,19 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
   if (ce != cudaSuccess) return FS2_ERR_CUDA - (int)ce;
 
   // duration on the un-embedded x; pitch on x; energy on x + pitch embedding.  energy uses p_control (modules.py:124).
-  FS2_TRY(run_predictor(s, m, m->dur, a->x_adapted, B, L, a->src_lens, 1.f, nullptr, nullptr, nullptr, a->x_adapted, a->logd_pred, h1, h2));
+  fs2_variance_head_args v{};
+  v.x = a->x_adapted; v.B = B; v.L = L; v.lens = a->src_lens; v.control = 1.f; v.pred_out = a->logd_pred;
+  FS2_TRY(run_predictor(s, m, m->dur, v, h1, h2));
+  v.control = a->p_control;
   if (!m->pitch_frame_level) {
     if (!a->p_pred) return FS2_ERR_ARG;
-    FS2_TRY(run_predictor(s, m, m->pitch, a->x_adapted, B, L, a->src_lens, a->p_control, a->p_target, m->pitch_bins, m->pitch_emb,
-                          a->x_adapted, a->p_pred, h1, h2));
+    v.target = a->p_target; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred;
+    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2));
   }
   if (!m->energy_frame_level) {
     if (!a->e_pred) return FS2_ERR_ARG;
-    FS2_TRY(run_predictor(s, m, m->energy, a->x_adapted, B, L, a->src_lens, a->p_control, a->e_target, m->energy_bins, m->energy_emb,
-                          a->x_adapted, a->e_pred, h1, h2));
+    v.target = a->e_target; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred;
+    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2));
   }
 
   fs2_durations_args d{};
@@ -294,44 +303,79 @@ static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cu
   if (T > m->dec_pos_rows) return FS2_ERR_ARG;
 
   const bool frame_level = m->pitch_frame_level || m->energy_frame_level;
-  fs2_length_regulate_args lr{a->x_adapted, a->cum_dur, frame_level ? nullptr : m->dec_pos, f.x, B, a->L, T, D};
+  fs2_length_regulate_args lr{};
+  lr.x = a->x_adapted; lr.cum = a->cum_dur; lr.pos = frame_level ? nullptr : m->dec_pos; lr.y = f.x; lr.B = B; lr.L = a->L; lr.T = T; lr.D = D;
   FS2_TRY(length_regulate(&lr, s));
   if (frame_level) {                                   // frame-level pitch / energy (model/modules.py:139-148), then the position add
     float* h1 = f.hid;                                 // [rows][d_inner] is free here and d_inner >= 2 * vp_filter is checked below
     float* h2 = f.hid + rows * m->vp_filter;
     if ((size_t)m->d_inner < 2 * (size_t)m->vp_filter) return FS2_ERR_UNSUPPORTED;
+    fs2_variance_head_args v{};
+    v.x = f.x; v.B = B; v.L = T; v.lens = a->mel_mask_lens; v.control = a->p_control;
     if (m->pitch_frame_level) {
       if (!a->p_pred_frames) return FS2_ERR_ARG;
-      FS2_TRY(run_predictor(s, m, m->pitch, f.x, B, T, a->mel_mask_lens, a->p_control, a->p_target_frames, m->pitch_bins, m->pitch_emb, f.x,
-                            a->p_pred_frames, h1, h2));
+      v.target = a->p_target_frames; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred_frames;
+      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2));
     }
     if (m->energy_frame_level) {
       if (!a->e_pred_frames) return FS2_ERR_ARG;
-      FS2_TRY(run_predictor(s, m, m->energy, f.x, B, T, a->mel_mask_lens, a->p_control, a->e_target_frames, m->energy_bins, m->energy_emb, f.x,
-                            a->e_pred_frames, h1, h2));
+      v.target = a->e_target_frames; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred_frames;
+      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2));
     }
     FS2_TRY(add_positions(f.x, m->dec_pos, B, T, D, s));
   }
-  for (int i = 0; i < m->n_dec; i++) FS2_TRY(fft_block(s, m, m->dec[i], f, B, T, a->mel_mask_lens, (m->tc_mask & FS2_TC_DECODER) != 0,
-                                                     (m->tc_mask & FS2_TC_DECODER_F8) ? FS2_TC_VARIANT_F8 : 0));
-  const bool tcp = (m->tc_mask & FS2_TC_POSTNET) != 0;
-  const unsigned tcpv = (m->tc_mask & FS2_TC_POSTNET_F8) ? FS2_TC_VARIANT_F8 : 0;
-  FS2_TRY(conv(s, f.x, B, T, D, m->w_mel, tcp ? m->w_mel_tc : nullptr, m->b_mel, m->n_mel, 1, 1, 0, FS2_ACT_NONE, 0.f, a->mel, nullptr, FS2_ACT_NONE,
-               0.f, 1.f, 0, nullptr, tcpv));
+  const ConvMode dec_mode{(m->tc_mask & FS2_TC_DECODER) ? ConvMode::TC : ConvMode::EXACT,
+                          (m->tc_mask & FS2_TC_DECODER_F8) ? FS2_TC_VARIANT_F8 : 0u};
+  for (int i = 0; i < m->n_dec; i++) FS2_TRY(fft_block(s, m, m->dec[i], f, B, T, a->mel_mask_lens, dec_mode));
+  const ConvMode post_mode{(m->tc_mask & FS2_TC_POSTNET) ? ConvMode::TC : ConvMode::EXACT,
+                           (m->tc_mask & FS2_TC_POSTNET_F8) ? FS2_TC_VARIANT_F8 : 0u};
+  fs2_conv1d_args c = conv_args(f.x, B, T, D, m->n_mel, 1, a->mel);
+  post_mode.weights(c, m->w_mel, m->w_mel_tc, m->b_mel);
+  FS2_TRY(conv1d_dispatch(&c, s));
   // PostNet: eval BatchNorm folded into (w, b) by the packer; unmasked, tanh on all but the last (Layers.py:129-137)
   const float* cur = a->mel;
   for (int i = 0; i < m->n_postnet; i++) {
     const bool last = i == m->n_postnet - 1;
     float* dst = last ? a->postnet_mel : ((i & 1) ? pb : pa);
-    FS2_TRY(conv(s, cur, B, T, m->post_cin[i], m->w_post[i], tcp ? m->w_post_tc[i] : nullptr, m->b_post[i], m->post_cout[i], m->post_k, 1,
-                 (m->post_k - 1) / 2,
-                 last ? FS2_ACT_NONE : FS2_ACT_TANH, 0.f, dst, last ? a->mel : nullptr, FS2_ACT_NONE, 0.f, 1.f, 0, nullptr, tcpv));
+    c = conv_args(cur, B, T, m->post_cin[i], m->post_cout[i], m->post_k, dst);
+    post_mode.weights(c, m->w_post[i], m->w_post_tc[i], m->b_post[i]);
+    if (last) c.res = a->mel;
+    else c.out_act = FS2_ACT_TANH;
+    FS2_TRY(conv1d_dispatch(&c, s));
     cur = dst;
   }
   return FS2_OK;
 }
 
 // ------------------------------------------------------------------ vocoder
+// fs2_resstack arguments for stage i's ResBlock group on [B][N][C] rows: every kernel size and dilation, utterance b bounded by
+// lens[b] * scale rows.  x, y, alpha and accumulate are the caller's (alpha 0: the kernel takes the mean over the n_kernels ResBlocks).
+static fs2_resstack_args resblock_args(const fs2_vocoder_model* m, int i, int B, int N, int C, const int32_t* lens, int scale) {
+  fs2_resstack_args a{};
+  a.B = B; a.N = N; a.C = C; a.n_kernels = m->n_kernels; a.n_dil = m->n_dil;
+  for (int j = 0; j < m->n_kernels; j++) {
+    const int rb = i * m->n_kernels + j;
+    a.k[j] = m->rb_k[j];
+    for (int d = 0; d < m->n_dil; d++) {
+      a.dil[j][d] = m->rb_dil[j][d];
+      a.w1_tc[j][d] = m->w_rb1_tc[rb][d]; a.b1[j][d] = m->b_rb1[rb][d];
+      a.w2_tc[j][d] = m->w_rb2_tc[rb][d]; a.b2[j][d] = m->b_rb2[rb][d];
+    }
+  }
+  a.lens = lens; a.lens_scale = scale;
+  return a;
+}
+
+// The same arguments narrowed to the one (dilated conv, conv) pair (j, d); fs2_resstack reads only the first n_kernels x n_dil entries.
+static fs2_resstack_args resblock_pair(const fs2_resstack_args& g, int j, int d) {
+  fs2_resstack_args a = g;
+  a.n_kernels = 1; a.n_dil = 1;
+  a.k[0] = g.k[j]; a.dil[0][0] = g.dil[j][d];
+  a.w1_tc[0][0] = g.w1_tc[j][d]; a.b1[0][0] = g.b1[j][d];
+  a.w2_tc[0][0] = g.w2_tc[j][d]; a.b2[0][0] = g.b2[j][d];
+  return a;
+}
+
 static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, cudaStream_t s, Arena& ar) {
   const int B = a->B, T = a->T;
   size_t per_frame = (size_t)m->c0;  // floats per mel frame of the widest activation
@@ -357,15 +401,13 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
   const int32_t* lens = a->mel_lens;
   int scale = 1;
 
-  {  // conv_pre reads the (possibly strided) channels-last mel view
-    fs2_conv1d_args c{};
-    c.x = a->mel; c.x_batch_stride = a->mel_batch_stride; c.x_row_stride = a->mel_row_stride;
-    c.B = B; c.T = T; c.Cin = m->n_mel; c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.N = m->c0; c.taps = 7;
-    c.dilation = 1; c.pad_left = 3; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
-    c.alpha = 1.f; c.y = bx; c.y_batch_stride = (int64_t)T * m->c0; c.y_row_stride = m->c0;
-    c.x_lens = lens; c.lens_scale = scale;
-    FS2_TRY(conv1d_dispatch(&c, s));
-  }
+  // conv_pre reads the (possibly strided) channels-last mel view
+  fs2_conv1d_args c = conv_args(a->mel, B, T, m->n_mel, m->c0, 7, bx);
+  c.x_batch_stride = a->mel_batch_stride; c.x_row_stride = a->mel_row_stride;
+  c.res_batch_stride = c.res_row_stride = 0;                        // no residual
+  c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
+  c.x_lens = lens; c.lens_scale = scale;
+  FS2_TRY(conv1d_dispatch(&c, s));
   int Ti = T, C = m->c0;
   const float inv_nk = 1.f / (float)m->n_kernels;
   for (int i = 0; i < m->n_stages; i++) {
@@ -374,34 +416,25 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
     const unsigned tcv = (m->f8_mask & (2 << i)) ? FS2_TC_VARIANT_F8 : 0;
     // ---- lrelu + ConvTranspose1d as two 2-tap phase-group convolutions (hifigan/models.py:152-153)
     for (int g = 0; g < 2; g++) {
-      fs2_conv1d_args c{};
-      c.x = bx; c.x_batch_stride = (int64_t)Ti * C; c.x_row_stride = C; c.B = B; c.T = Ti; c.Cin = C;
+      const size_t off = (size_t)g * (u / 2) * Co;    // group g writes output channels [off, off + (u/2)*Co) of each [u*Co] row
+      c = conv_args(bx, B, Ti, C, (u / 2) * Co, 2, bu + off);
+      c.y_batch_stride = (int64_t)Ti * u * Co; c.y_row_stride = (int64_t)u * Co;
+      c.res_batch_stride = c.res_row_stride = 0;                    // no residual
+      c.pad_left = g == 0 ? 1 : 0;
       c.w = g == 0 ? m->w_up_a[i] : m->w_up_b[i];
       c.w_tc = g == 0 ? m->w_up_a_tc[i] : m->w_up_b_tc[i];
-      c.bias = m->b_up[i] + (size_t)g * (u / 2) * Co;
-      c.N = (u / 2) * Co; c.taps = 2; c.dilation = 1; c.pad_left = g == 0 ? 1 : 0;
-      c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.alpha = 1.f; c.tc_variant = tcv;
-      c.y = bu + (size_t)g * (u / 2) * Co; c.y_batch_stride = (int64_t)Ti * u * Co; c.y_row_stride = (int64_t)u * Co;
+      c.bias = m->b_up[i] + off;
+      c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
       c.x_lens = lens; c.lens_scale = scale;          // [B][Ti][u*Co]: input and output rows have the same n_b
       FS2_TRY(conv1d_dispatch(&c, s));
     }
     Ti *= u; C = Co; scale *= u;
     // ---- mean of the multi-receptive-field ResBlocks (models.py:154-160, ResBlock.forward :96-103)
+    fs2_resstack_args group = resblock_args(m, i, B, Ti, C, lens, scale);
     if ((m->fused_mask >> i) & 1) {                    // one persistent kernel for the whole group: intermediates never leave the SM
       if (!tcv) return FS2_ERR_ARG;
-      fs2_resstack_args ra{};
-      ra.x = bu; ra.y = bx; ra.B = B; ra.N = Ti; ra.C = C; ra.n_kernels = m->n_kernels; ra.n_dil = m->n_dil;
-      for (int j = 0; j < m->n_kernels; j++) {
-        ra.k[j] = m->rb_k[j];
-        for (int d = 0; d < m->n_dil; d++) {
-          const int rb = i * m->n_kernels + j;
-          ra.dil[j][d] = m->rb_dil[j][d];
-          ra.w1_tc[j][d] = m->w_rb1_tc[rb][d]; ra.b1[j][d] = m->b_rb1[rb][d];
-          ra.w2_tc[j][d] = m->w_rb2_tc[rb][d]; ra.b2[j][d] = m->b_rb2[rb][d];
-        }
-      }
-      ra.lens = lens; ra.lens_scale = scale;
-      FS2_TRY(resstack(&ra, s));
+      group.x = bu; group.y = bx;
+      FS2_TRY(resstack(&group, s));
       continue;
     }
     for (int j = 0; j < m->n_kernels; j++) {
@@ -409,32 +442,35 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
       const float* r = bu;
       const bool pairs = ((m->pair_mask >> i) & 1) && tcv && (C == 32 || C == 64) && k <= m->pair_kmax;
       for (int d = 0; d < m->n_dil; d++) {
-        const int dil = m->rb_dil[j][d];
-        if (pairs) {                                   // one launch per (dilated conv, conv, +x) pair: the intermediate stays on chip
-          const bool lastp = d == m->n_dil - 1;
-          float* dstp = lastp ? bx : (r == r1 ? r2 : r1);
-          fs2_resstack_args ra{};
-          ra.x = r; ra.y = dstp; ra.B = B; ra.N = Ti; ra.C = C; ra.n_kernels = 1; ra.n_dil = 1;
-          ra.k[0] = k; ra.dil[0][0] = dil;
-          ra.w1_tc[0][0] = m->w_rb1_tc[rb][d]; ra.b1[0][0] = m->b_rb1[rb][d];
-          ra.w2_tc[0][0] = m->w_rb2_tc[rb][d]; ra.b2[0][0] = m->b_rb2[rb][d];
-          ra.alpha = lastp ? inv_nk : 1.f; ra.accumulate = lastp && j > 0;
-          ra.lens = lens; ra.lens_scale = scale;
-          FS2_TRY(resstack(&ra, s));
-          r = dstp;
-          continue;
-        }
-        FS2_TRY(conv(s, r, B, Ti, C, m->w_rb1[rb][d], m->w_rb1_tc[rb][d], m->b_rb1[rb][d], C, k, dil, (k * dil - dil) / 2, FS2_ACT_LRELU,
-                     0.1f, bt, nullptr, FS2_ACT_LRELU, 0.1f, 1.f, 0, nullptr, tcv, lens, scale));
-        const bool last = d == m->n_dil - 1;
+        const bool last = d == m->n_dil - 1;            // the last layer adds its share of the mean over the n_kernels ResBlocks into bx
         float* dst = last ? bx : (r == r1 ? r2 : r1);
-        FS2_TRY(conv(s, bt, B, Ti, C, m->w_rb2[rb][d], m->w_rb2_tc[rb][d], m->b_rb2[rb][d], C, k, 1, (k - 1) / 2, FS2_ACT_NONE, 0.f, dst,
-                     r, FS2_ACT_NONE, 0.f, last ? inv_nk : 1.f, last && j > 0, nullptr, tcv, lens, scale));
+        const float alpha = last ? inv_nk : 1.f;
+        const int accumulate = last && j > 0;
+        if (pairs) {                                   // one launch per (dilated conv, conv, +x) pair: the intermediate stays on chip
+          fs2_resstack_args p = resblock_pair(group, j, d);
+          p.x = r; p.y = dst; p.alpha = alpha; p.accumulate = accumulate;
+          FS2_TRY(resstack(&p, s));
+        } else {                                       // the two convs through bt
+          const int dil = m->rb_dil[j][d];
+          c = conv_args(r, B, Ti, C, C, k, bt);
+          c.w = m->w_rb1[rb][d]; c.w_tc = m->w_rb1_tc[rb][d]; c.bias = m->b_rb1[rb][d]; c.tc_variant = tcv;
+          c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
+          c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
+          c.x_lens = lens; c.lens_scale = scale;
+          FS2_TRY(conv1d_dispatch(&c, s));
+          c = conv_args(bt, B, Ti, C, C, k, dst);
+          c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
+          c.res = r; c.alpha = alpha; c.accumulate = accumulate;
+          c.x_lens = lens; c.lens_scale = scale;
+          FS2_TRY(conv1d_dispatch(&c, s));
+        }
         r = dst;
       }
     }
   }
-  fs2_conv_post_args p{bx, B, Ti, C, m->w_post, m->b_post, 7, 0.01f, a->wav, lens, scale};
+  fs2_conv_post_args p{};
+  p.x = bx; p.B = B; p.T = Ti; p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f; p.wav = a->wav;
+  p.lens = lens; p.lens_scale = scale;
   return conv_post(&p, s);
 }
 

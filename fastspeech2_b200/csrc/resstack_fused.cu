@@ -385,18 +385,14 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
   if (!dv) return derr;
   int plan[12];
   FS2_TRY(resstack_plan(a, dv->num_sms.load(std::memory_order_relaxed), plan));
-  if (!dv->fused_ready.load(std::memory_order_acquire)) {
-    DevOnce once;
-    if (!dv->fused_ready.load(std::memory_order_relaxed)) {
-      const int mx = 227 * 1024;
-      cudaError_t e = cudaFuncSetAttribute(resstack_kernel<32, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<32, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-      if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
-      dv->fused_ready.store(true, std::memory_order_release);
-    }
-  }
+  FS2_TRY(dev_once(dv->fused_ready, [] {
+    const int mx = 227 * 1024;
+    cudaError_t e = cudaFuncSetAttribute(resstack_kernel<32, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<32, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    return e;
+  }));
   RsP p{};
   p.B = a->B; p.N = a->N;
   p.n_kernels = a->n_kernels; p.n_dil = a->n_dil;

@@ -142,7 +142,7 @@ typedef struct fs2_attention_args {
 int fs2_attention(const fs2_attention_args* a, fs2_stream_t stream);
 size_t fs2_attention_workspace_bytes(int B, int T, int H);
 
-/* y[b,l,:] = table[ids[b,l]] + pos[l]   (+ spk[speakers[b]] when spk != NULL: not used by the encoder, kept for tests) */
+/* y[b,l,:] = table[ids[b,l]] + pos[l]   (the speaker embedding is added separately, by fs2_add_speaker) */
 typedef struct fs2_embed_args {
   const int64_t* ids; const float* table; const float* pos; float* y; int B, L, D, n_vocab;
 } fs2_embed_args;
@@ -352,7 +352,7 @@ int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, f
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
 const char* fs2_build_info(void);          /* "sm_90a ..." */
-size_t fs2_struct_size(int which);
+size_t fs2_struct_size(int which);         /* sizeof of the i-th struct above, in declaration order (binding self-check) */
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the
  * device that owns the stream current before calling -- (b) the launch counter above and (c) the profiling state below, which is
@@ -362,7 +362,7 @@ size_t fs2_struct_size(int which);
  * recorded events, fills ms/flops/launches per class (arrays of FS2_PROF_CLASSES) and disarms.  Not for timed regions. */
 #define FS2_PROF_CLASSES 5
 int fs2_profile_begin(void);
-int fs2_profile_end(double* ms, double* flops, int64_t* launches);         /* sizeof of the i-th struct above, in declaration order (binding self-check) */
+int fs2_profile_end(double* ms, double* flops, int64_t* launches);
 
 #ifdef __cplusplus
 }

@@ -182,6 +182,8 @@ EXPORTS = {
     "fs2_acoustic_encode": (i32, [C.POINTER(AcousticModel), C.POINTER(EncodeArgs), fp]),
     "fs2_decode_workspace_bytes": (C.c_size_t, [C.POINTER(AcousticModel), i32, i32]),
     "fs2_acoustic_decode": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), fp]),
+    "fs2_acoustic_encode_ragged": (i32, [C.POINTER(AcousticModel), C.POINTER(EncodeArgs), fp]),
+    "fs2_acoustic_decode_ragged": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), fp]),
     "fs2_vocoder_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderArgs), fp]),
 }

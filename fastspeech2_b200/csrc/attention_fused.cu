@@ -12,6 +12,13 @@
 //   epilogue: O / l -> ctx[b, t, h*128 .. +128]; query rows t >= key_len[b] are written as 0 (contract of fs2_attention).
 //   Recomputing S costs 1/3 more MMAs than a one-pass online softmax and removes the O rescaling.
 //
+// Ragged mode (template parameter RAG; the padded instantiation keeps its code): utterance b is computed exactly as a B = 1 call
+// with T = n_b = key_lens[b].  Only utterances with n_b >= AF_MIN_ROWS are taken (a B = 1 call with a shorter T runs the exact
+// kernel, which takes the others); their work items are the live query tiles, compacted per head by the RaggedWalk cursor of the
+// conv kernel, and each streams ceil(n_b / 128) key blocks in both passes.  The packer packs only those key blocks, with rows at
+// or beyond n_b as zero; Q rows at or beyond n_b load as zero (0 * a stale NaN would still be NaN in P V), and ctx rows there are
+// not written.
+//
 // Roles: warp 8 streams K / V stages (cp.async.bulk) in the order they are consumed; warps 0-7 are two consumer warpgroups that
 // own 64 query rows each: Q conversion, the MMAs, both softmax passes and the epilogue.
 #include "conv_tc_kernel.cuh"
@@ -22,6 +29,7 @@ constexpr int AF_THREADS = 288;
 constexpr int AF_SB = 8;                         // K / V stage ring depth
 constexpr uint32_t AF_STAGE = 8192;              // one stage: [hi | lo][2 chunks][128][16 B]
 constexpr float AF_WSCALE = 16.f;                // power-of-two operand scale of the packed K / V tiles (|k|, |v| < 4094 stay inside fp16)
+constexpr int AF_MIN_ROWS = 128;                 // shortest utterance the ragged kernel takes (a B = 1 call takes T >= 128)
 
 // ------------------------------------------------------------------ K / V operand tiles
 // Per (utterance, head) one buffer of af_tile_stride(Tk) bytes: TC_HDR header (float 1 / AF_WSCALE), then the stages; keys are padded
@@ -43,8 +51,18 @@ __device__ __forceinline__ void split8(const float (&f)[8], float scale, uint4& 
 }
 
 // K tiles: B operand W[c = d][n = key] of S = Q K^T, layout  header | [key/128][d/16][hi|lo][2 chunks][128 keys][8 halfs]
+// Ragged: keys of utterance b at or beyond n_b pack as zero, and key blocks beyond ceil(n_b / 128) (every block when n_b < AF_MIN_ROWS)
+// are not packed: the attention kernel never reads them.
+template <bool RAG>
+__device__ __forceinline__ int af_key_rows(const int* key_lens, int T, int b) {
+  if (!RAG) return T;
+  const int n = ragged_rows(key_lens, 1, T, b);
+  return n < AF_MIN_ROWS ? 0 : n;
+}
+
+template <bool RAG>
 __device__ __forceinline__ void pack_k_tiles(const float* __restrict__ qkv, unsigned char* __restrict__ tiles, int B, int T, int Tk, int H,
-                                             long long tile_stride, long long idx) {   // idx = (bh, key, dchunk)
+                                             long long tile_stride, long long idx, const int* key_lens) {   // idx = (bh, key, dchunk)
   const long long total = (long long)B * H * Tk * (128 / 8);
   if (idx >= total) return;
   const int dchunk = (int)(idx % (128 / 8));
@@ -53,10 +71,12 @@ __device__ __forceinline__ void pack_k_tiles(const float* __restrict__ qkv, unsi
   const int bh = (int)(r / Tk);
   const int b = bh / H, h = bh - b * H;
   const int D = H * 128;
+  const int rows = af_key_rows<RAG>(key_lens, T, b);
+  if (RAG && key >= (rows + 127) / 128 * 128) return;
   float f[8];
 #pragma unroll
   for (int j = 0; j < 8; j++) f[j] = 0.f;
-  if (key < T) {
+  if (key < rows) {
     const float4* src = reinterpret_cast<const float4*>(qkv + ((long long)b * T + key) * 3 * D + D + h * 128 + dchunk * 8);
     const float4 u = __ldg(src), v = __ldg(src + 1);
     f[0] = u.x; f[1] = u.y; f[2] = u.z; f[3] = u.w; f[4] = v.x; f[5] = v.y; f[6] = v.z; f[7] = v.w;
@@ -73,8 +93,9 @@ __device__ __forceinline__ void pack_k_tiles(const float* __restrict__ qkv, unsi
 }
 
 // V tiles: B operand W[c = key][n = d] of O = P V, layout  header | [key/16][hi|lo][2 chunks of 8 keys][128 d][8 halfs (keys)]
+template <bool RAG>
 __device__ __forceinline__ void pack_v_tiles(const float* __restrict__ qkv, unsigned char* __restrict__ tiles, int B, int T, int Tk, int H,
-                                             long long tile_stride, long long idx) {   // idx = (bh, key8, d)
+                                             long long tile_stride, long long idx, const int* key_lens) {   // idx = (bh, key8, d)
   const long long total = (long long)B * H * (Tk / 8) * 128;
   if (idx >= total) return;
   const int d = (int)(idx % 128);
@@ -83,11 +104,13 @@ __device__ __forceinline__ void pack_v_tiles(const float* __restrict__ qkv, unsi
   const int bh = (int)(r / (Tk / 8));
   const int b = bh / H, h = bh - b * H;
   const int D = H * 128;
+  const int rows = af_key_rows<RAG>(key_lens, T, b);
+  if (RAG && k8 * 8 >= (rows + 127) / 128 * 128) return;
   float f[8];
 #pragma unroll
   for (int e = 0; e < 8; e++) {
     const int key = k8 * 8 + e;
-    f[e] = key < T ? __ldg(qkv + ((long long)b * T + key) * 3 * D + 2 * D + h * 128 + d) : 0.f;
+    f[e] = key < rows ? __ldg(qkv + ((long long)b * T + key) * 3 * D + 2 * D + h * 128 + d) : 0.f;
   }
   uint4 hi, lo;
   split8(f, AF_WSCALE, hi, lo);
@@ -101,10 +124,11 @@ __device__ __forceinline__ void pack_v_tiles(const float* __restrict__ qkv, unsi
 }
 
 // One launch writes both operand-tile sets: blocks [0, k_blocks) the K tiles, the rest the V tiles.
+template <bool RAG>
 __global__ void pack_kv_tiles_kernel(const float* __restrict__ qkv, unsigned char* __restrict__ kt, unsigned char* __restrict__ vt, int B, int T,
-                                     int Tk, int H, long long tile_stride, unsigned k_blocks) {
-  if (blockIdx.x < k_blocks) pack_k_tiles(qkv, kt, B, T, Tk, H, tile_stride, (long long)blockIdx.x * blockDim.x + threadIdx.x);
-  else pack_v_tiles(qkv, vt, B, T, Tk, H, tile_stride, (long long)(blockIdx.x - k_blocks) * blockDim.x + threadIdx.x);
+                                     int Tk, int H, long long tile_stride, unsigned k_blocks, const int* key_lens) {
+  if (blockIdx.x < k_blocks) pack_k_tiles<RAG>(qkv, kt, B, T, Tk, H, tile_stride, (long long)blockIdx.x * blockDim.x + threadIdx.x, key_lens);
+  else pack_v_tiles<RAG>(qkv, vt, B, T, Tk, H, tile_stride, (long long)(blockIdx.x - k_blocks) * blockDim.x + threadIdx.x, key_lens);
 }
 
 // ------------------------------------------------------------------ attention kernel
@@ -135,6 +159,7 @@ __device__ __forceinline__ void af_store16(unsigned char* kblk, int row, const f
 
 __device__ __forceinline__ void af_wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }   // one warpgroup
 
+template <bool RAG>
 __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const AfP p) {
   constexpr uint32_t KBLK = 8192;                // one 16-wide K-block of an A operand: hi plane 4 KB + lo plane 4 KB (128 rows)
   constexpr uint32_t PLANES = 8 * KBLK;          // 128 x 128 operand: 64 KB
@@ -152,7 +177,12 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int nkb = p.Tk / 128;                    // key blocks
+  const int nkb = p.Tk / 128;                    // key blocks (ragged: per item, ceil(n_b / 128))
+  // Ragged: items are (head, utterance, live query tile), heads as the block dimension of the compacted sequence; every role walks
+  // it in the same order.
+  RaggedWalkT<AF_MIN_ROWS> walk{};
+  int n_items = p.n_items;
+  if (RAG) { walk.init(p.key_lens, 1, p.T, p.B, 128); n_items = walk.live * p.H; }
 
   if (warp == 8) {
     // ===================== K / V stage producer, in the order the consumers read them =====================
@@ -164,13 +194,17 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
         bulk_g2s(ring + (size_t)rb.idx * AF_STAGE, src, AF_STAGE, &fullB[rb.idx]);
         rb.advance(AF_SB);
       };
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-        const int bh = item / p.qtiles;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        int bh = item / p.qtiles, nkb_i = nkb;
+        if (RAG) {
+          const Item it = walk.item(p.key_lens, 1, p.T, 128, item);
+          bh = it.b * p.H + it.nblk; nkb_i = (walk.rows + 127) / 128;
+        }
         const unsigned char* kt = p.kt + (long long)bh * p.tstride + TC_HDR;   // [key block][d/16][8 KB]
         const unsigned char* vt = p.vt + (long long)bh * p.tstride + TC_HDR;   // [key/16][8 KB]
-        for (int j = 0; j < nkb; j++)                                            // pass 1
+        for (int j = 0; j < nkb_i; j++)                                          // pass 1
           for (int kb = 0; kb < 8; kb++) push(kt + ((size_t)j * 8 + kb) * AF_STAGE);
-        for (int j = 0; j < nkb; j++) {                                          // pass 2
+        for (int j = 0; j < nkb_i; j++) {                                        // pass 2
           for (int kb = 0; kb < 8; kb++) push(kt + ((size_t)j * 8 + kb) * AF_STAGE);   // S(j)
           for (int kb = 0; kb < 8; kb++) push(vt + ((size_t)j * 8 + kb) * AF_STAGE);   // P V_j
         }
@@ -206,10 +240,16 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     tc_release(&emptyB[pend]);
   };
   const int qr = (tid & 127) >> 1, qhalf = tid & 1;    // Q conversion: row, 64-column half
-  for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-    const int bh = item / p.qtiles, qt = item - bh * p.qtiles;
-    const int b = bh / p.H, hd = bh - b * p.H;
-    const int len = p.key_lens ? min(p.key_lens[b], p.T) : p.T;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    int bh = item / p.qtiles, qt = item - bh * p.qtiles;
+    int b = bh / p.H, hd = bh - b * p.H;
+    int len = p.key_lens ? min(p.key_lens[b], p.T) : p.T;
+    int nkb_i = nkb, rows = p.T;                   // rows that exist: the utterance's own in ragged mode
+    if (RAG) {
+      const Item it = walk.item(p.key_lens, 1, p.T, 128, item);
+      b = it.b; hd = it.nblk; qt = it.t0 / 128; bh = b * p.H + hd;
+      len = rows = walk.rows; nkb_i = (len + 127) / 128;
+    }
     // ---- Q rows of this warpgroup -> operand planes (the previous item's MMAs have all retired)
     {
       const int t = qt * 128 + 64 * g + qr;
@@ -217,7 +257,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
 #pragma unroll
       for (int k = 0; k < 4; k++) {
         float v[16];
-        if (t < p.T) {
+        if (t < rows) {
 #pragma unroll
           for (int k4 = 0; k4 < 4; k4++) {
             const float4 u = __ldg(reinterpret_cast<const float4*>(src + k * 16) + k4);
@@ -235,7 +275,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     float sacc[64];
     // ---- pass 1: row maxima of the masked, scaled scores (rows lane/4 and lane/4 + 8 of this warp's 16)
     float m[2] = {-INFINITY, -INFINITY};
-    for (int j = 0; j < nkb; j++) {
+    for (int j = 0; j < nkb_i; j++) {
       gemm(qa16, sacc);
 #pragma unroll
       for (int jj = 0; jj < 16; jj++)
@@ -257,7 +297,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     float oacc[64];
     float l[2] = {0.f, 0.f};
     const int prow = 64 * g + 16 * w + (lane >> 2);
-    for (int j = 0; j < nkb; j++) {
+    for (int j = 0; j < nkb_i; j++) {
       gemm(qa16, sacc);
 #pragma unroll
       for (int jj = 0; jj < 16; jj++) {
@@ -313,7 +353,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
       l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
       l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
       const int t = qt * 128 + prow + 8 * h;
-      if (t >= p.T) continue;
+      if (t >= rows) continue;
       const float inv = t < len ? (1.f / AF_WSCALE) / l[h] : 0.f;
       float* dst = p.ctx + ((long long)b * p.T + t) * D + hd * 128 + 2 * (lane & 3);
 #pragma unroll
@@ -333,7 +373,7 @@ size_t attention_fused_workspace(int B, int T, int H) {
   return 2 * tile_bytes + 256;
 }
 
-int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s) {
+int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged) {
   if (!a || !a->qkv || !a->ctx || !ws || a->B <= 0 || a->T <= 0 || a->H <= 0) return FS2_ERR_ARG;
   if (a->Dh != 128) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->qkv) || !aligned16(a->ctx)) return FS2_ERR_ARG;
@@ -341,8 +381,11 @@ int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cuda
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);
   if (!dv) return derr;
-  FS2_TRY(dev_once(dv->att_fused_ready,
-                   [] { return cudaFuncSetAttribute(attention_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AF_SMEM); }));
+  if (ragged && !a->key_lens) return FS2_ERR_ARG;
+  FS2_TRY(dev_once(dv->att_fused_ready, [] {
+    const cudaError_t e = cudaFuncSetAttribute(attention_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AF_SMEM);
+    return e == cudaSuccess ? cudaFuncSetAttribute(attention_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AF_SMEM) : e;
+  }));
   const int Tk = (a->T + 127) / 128 * 128;
   char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
   const long long tstride = af_tile_stride(Tk);
@@ -353,7 +396,8 @@ int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cuda
     const long long nk = (long long)a->B * a->H * Tk * (128 / 8), nv = (long long)a->B * a->H * (Tk / 8) * 128;
     const unsigned kb = (unsigned)((nk + 255) / 256), vb = (unsigned)((nv + 255) / 256);
     prof_before(s);
-    pack_kv_tiles_kernel<<<kb + vb, 256, 0, s>>>(a->qkv, kt, vt, a->B, a->T, Tk, a->H, tstride, kb);
+    if (ragged) pack_kv_tiles_kernel<true><<<kb + vb, 256, 0, s>>>(a->qkv, kt, vt, a->B, a->T, Tk, a->H, tstride, kb, a->key_lens);
+    else pack_kv_tiles_kernel<false><<<kb + vb, 256, 0, s>>>(a->qkv, kt, vt, a->B, a->T, Tk, a->H, tstride, kb, nullptr);
     prof_after(s, 1, 0.0);
     FS2_LAUNCH_CHECK();
   }
@@ -367,7 +411,8 @@ int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cuda
   const int num_sms = dv->num_sms.load(std::memory_order_relaxed);
   const int grid = items < num_sms ? (int)items : num_sms;
   prof_before(s);
-  attention_fused_kernel<<<grid, AF_THREADS, AF_SMEM, s>>>(p);
+  if (ragged) attention_fused_kernel<true><<<grid, AF_THREADS, AF_SMEM, s>>>(p);   // grid from the padded shape: CTAs without work exit
+  else attention_fused_kernel<false><<<grid, AF_THREADS, AF_SMEM, s>>>(p);
   // algorithmic count as the reference computes it (dense T x T): 4*T*T*Dh per (b, h)
   prof_after(s, 1, 4.0 * a->B * a->H * (double)a->T * a->T * 128);
   FS2_LAUNCH_CHECK();

@@ -14,7 +14,11 @@ namespace fs2 {
 constexpr int ATT_BQ = 64, ATT_BK = 64, ATT_D = 128, ATT_LD = ATT_D + 4, ATT_PLD = ATT_BK + 4;
 constexpr size_t ATT_SMEM = (size_t)(ATT_BQ * ATT_LD + ATT_BK * ATT_LD + ATT_BK * ATT_D) * sizeof(float);
 
-__global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attention_args a) {
+// RAG: ragged batch.  Utterance b is computed exactly as a B = 1 call with T = len: Q / K / V rows at or beyond len load as zero
+// (they are not computed upstream and may hold anything), query tiles wholly at or beyond len and the rows there are not written, and
+// an utterance with len >= fused_from (> 0) is left to the fused kernel.  A template parameter, so the padded kernel keeps its code.
+template <bool RAG>
+__global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attention_args a, int fused_from) {
   extern __shared__ __align__(16) float smem[];
   float* Qs = smem;                       // [64][132]
   float* Ks = Qs + ATT_BQ * ATT_LD;       // [64][132]  (reused as P [64][68])
@@ -29,7 +33,9 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
   const float* base = a.qkv + (long long)b * a.T * row_stride;
   const int len = a.key_lens ? min(a.key_lens[b], a.T) : a.T;
   float* out = a.ctx + (long long)b * a.T * D + h * ATT_D;
+  const int rows = RAG ? len : a.T;       // rows that exist: the utterance's own in ragged mode
 
+  if (RAG && (q0 >= len || (fused_from > 0 && len >= fused_from))) return;
   if (q0 >= len) {  // whole query tile is padding: the reference zeroes these rows after the LayerNorm
     for (int f = tid; f < ATT_BQ * (ATT_D / 4); f += 256) {
       const int r = f / (ATT_D / 4), c = f % (ATT_D / 4);
@@ -42,7 +48,7 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
   for (int f = tid; f < ATT_BQ * (ATT_D / 4); f += 256) {
     const int r = f / (ATT_D / 4), c = f % (ATT_D / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (q0 + r < a.T) v = __ldg(reinterpret_cast<const float4*>(base + (long long)(q0 + r) * row_stride + h * ATT_D) + c);
+    if (q0 + r < rows) v = __ldg(reinterpret_cast<const float4*>(base + (long long)(q0 + r) * row_stride + h * ATT_D) + c);
     *reinterpret_cast<float4*>(Qs + r * ATT_LD + c * 4) = v;
   }
 
@@ -62,7 +68,7 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
     for (int f = tid; f < ATT_BK * (ATT_D / 4); f += 256) {
       const int r = f / (ATT_D / 4), c = f % (ATT_D / 4);
       float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
-      if (k0 + r < a.T) {
+      if (k0 + r < rows) {
         const float* rowp = base + (long long)(k0 + r) * row_stride + h * ATT_D;
         kv = __ldg(reinterpret_cast<const float4*>(rowp + D) + c);
         vv = __ldg(reinterpret_cast<const float4*>(rowp + 2 * D) + c);
@@ -155,7 +161,7 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
 #pragma unroll
   for (int i = 0; i < 4; i++) {
     const int q = q0 + ty + 16 * i;
-    if (q >= a.T) continue;
+    if (q >= rows) continue;
     float* orow = out + (long long)q * D;
     if (q >= len) {
       *reinterpret_cast<float4*>(orow + tx * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -168,18 +174,21 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
   }
 }
 
-int attention_simt(const fs2_attention_args* a, cudaStream_t s) {
+int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged, int fused_from) {
   if (!a || !a->qkv || !a->ctx || a->B <= 0 || a->T <= 0 || a->H <= 0) return FS2_ERR_ARG;
   if (a->Dh != ATT_D) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->qkv) || !aligned16(a->ctx)) return FS2_ERR_ARG;
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);
   if (!dv) return derr;
-  FS2_TRY(dev_once(dv->att_simt_ready,
-                   [] { return cudaFuncSetAttribute(attention_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM); }));
+  FS2_TRY(dev_once(dv->att_simt_ready, [] {
+    const cudaError_t e = cudaFuncSetAttribute(attention_simt_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);
+    return e == cudaSuccess ? cudaFuncSetAttribute(attention_simt_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM) : e;
+  }));
   dim3 grid((a->T + ATT_BQ - 1) / ATT_BQ, a->H, a->B);
   prof_before(s);
-  attention_simt_kernel<<<grid, 256, ATT_SMEM, s>>>(*a);
+  if (ragged) attention_simt_kernel<true><<<grid, 256, ATT_SMEM, s>>>(*a, fused_from);
+  else attention_simt_kernel<false><<<grid, 256, ATT_SMEM, s>>>(*a, 0);
   prof_after(s, 1, 4.0 * a->B * a->H * (double)a->T * a->T * ATT_D);  // dense T x T count, as the reference computes it
   FS2_LAUNCH_CHECK();
   return FS2_OK;

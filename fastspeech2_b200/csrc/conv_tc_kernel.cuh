@@ -147,26 +147,34 @@ __device__ __forceinline__ Item decode_item(const TcP& p, int item) {
 // ever scheduled.
 // Monotone cursor over that compacted sequence.  Every role visits its items in increasing order (item = blockIdx.x, + gridDim.x, ...),
 // so the cursor only moves forward and each length is loaded once per channel block: no table, no cap on B, no host sync.
-struct RaggedWalk {
+// MIN_ROWS > 0: an utterance with fewer rows counts as empty (the fused attention kernel leaves those to the exact one).
+template <int MIN_ROWS>
+struct RaggedWalkT {
   int live;                        // live tiles per channel block
   int nblk, b, before, rows;       // cursor: channel block, utterance, live tiles of utterances < b in the block, n_b
+  __device__ __forceinline__ static int rows_of(const int* lens, int scale, int cap, int b) {
+    const int n = ragged_rows(lens, scale, cap, b);
+    if constexpr (MIN_ROWS > 0) return n < MIN_ROWS ? 0 : n;
+    return n;
+  }
   __device__ __forceinline__ void init(const int* lens, int scale, int cap, int B, int tile) {
     live = 0;
-    for (int i = 0; i < B; i++) live += (ragged_rows(lens, scale, cap, i) + tile - 1) / tile;
-    nblk = 0; b = 0; before = 0; rows = ragged_rows(lens, scale, cap, 0);
+    for (int i = 0; i < B; i++) live += (rows_of(lens, scale, cap, i) + tile - 1) / tile;
+    nblk = 0; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0);
   }
   __device__ __forceinline__ Item item(const int* lens, int scale, int cap, int tile, int i) {   // i < live * channel blocks
     const int blk = i / live, rem = i - blk * live;
-    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = ragged_rows(lens, scale, cap, 0); }
+    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0); }
     for (int nt = (rows + tile - 1) / tile; rem >= before + nt; nt = (rows + tile - 1) / tile) {
       before += nt;
-      rows = ragged_rows(lens, scale, cap, ++b);
+      rows = rows_of(lens, scale, cap, ++b);
     }
     Item it;
     it.nblk = blk; it.b = b; it.t0 = (rem - before) * tile;
     return it;
   }
 };
+using RaggedWalk = RaggedWalkT<0>;
 
 template <int ACT>
 __device__ __forceinline__ float tc_act(float v, float slope) {

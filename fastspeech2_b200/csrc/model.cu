@@ -64,7 +64,7 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 // kernels / launchers defined in the other translation units
 int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s);
 int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s);
-int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s);
+int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
 int conv_tc_nb(int N, int nb_max);
@@ -78,12 +78,12 @@ static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s) {
   if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s);
   return conv1d_simt(a, s);
 }
-int attention_simt(const fs2_attention_args* a, cudaStream_t s);
+int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = false, int fused_from = 0);
 int embed_positions(const fs2_embed_args* a, cudaStream_t s);
 int add_speaker(const fs2_rowbias_args* a, cudaStream_t s);
 int layernorm(const fs2_layernorm_args* a, cudaStream_t s);
 int variance_head(const fs2_variance_head_args* a, cudaStream_t s);
-int durations(const fs2_durations_args* a, cudaStream_t s);
+int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr);
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s);
 int resstack(const fs2_resstack_args* a, cudaStream_t s);
@@ -91,6 +91,7 @@ int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, int* out);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
 int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s);
+int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cudaStream_t s);
 
 // ------------------------------------------------------------------ workspace bump allocator
 struct Arena {
@@ -148,26 +149,36 @@ struct ConvMode {
 
 struct FftBufs { float *x, *tmp, *qkv, *ctx, *hid; void* att_ws; size_t att_bytes; };
 
+// Ragged mode (fs2_acoustic_encode_ragged / fs2_acoustic_decode_ragged): utterance b is bounded by lens[b] rows in every layer, so it is
+// computed exactly as a B = 1 call on those rows would compute it.  Each conv gets the lengths as x_lens (lens_scale 1): it reads rows
+// at or beyond lens[b] as zero and leaves its output rows there unspecified; the LayerNorms zero them.  `rag` is that x_lens, or NULL.
+static const int32_t* ragged_lens(bool ragged, const int32_t* lens) { return ragged ? lens : nullptr; }
+
 // One FFT block in place on bufs.x  (transformer/Layers.py:21-30)
 static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_block_weights& w, const FftBufs& f, int B, int T,
-                     const int32_t* lens, ConvMode mode) {
+                     const int32_t* lens, ConvMode mode, bool ragged) {
   const int D = m->d_model, F = m->d_inner;
   const bool seg = mode.path == ConvMode::SEGMENTED;
+  const int32_t* rag = ragged_lens(ragged, lens);
   if (seg && (!w.w_qkv_tc || !w.w_o_tc || !w.w_1_tc || !w.w_2_tc || m->k2 != 1)) return FS2_ERR_ARG;
   fs2_conv1d_args c = conv_args(f.x, B, T, D, 3 * D, 1, f.qkv);
   mode.weights(c, w.w_qkv, w.w_qkv_tc, w.b_qkv);
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   fs2_attention_args at{};
   at.qkv = f.qkv; at.ctx = f.ctx; at.B = B; at.T = T; at.H = m->n_head; at.Dh = D / m->n_head; at.key_lens = lens;
   at.scale = 1.0f / sqrtf((float)(D / m->n_head));
   if (mode.path == ConvMode::TC && f.att_ws && T >= 128) {           // one fused tensor-core kernel: S stays in registers, any length
-    FS2_TRY(attention_fused(&at, f.att_ws, f.att_bytes, s));
+    FS2_TRY(attention_fused(&at, f.att_ws, f.att_bytes, s, ragged));
+    // ragged: the fused kernel takes the utterances of >= 128 rows, the exact kernel the shorter ones -- the backends a B = 1 call picks
+    if (ragged) FS2_TRY(attention_simt(&at, s, true, 128));
   } else {
-    FS2_TRY(attention_simt(&at, s));
+    FS2_TRY(attention_simt(&at, s, ragged, 0));
   }
   c = conv_args(f.ctx, B, T, D, D, 1, f.tmp);
   mode.weights(c, w.w_o, w.w_o_tc, w.b_o);
   c.res = f.x;
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   fs2_layernorm_args n{};                                           // both LayerNorms: tmp -> x, padded rows zeroed
   n.x = f.tmp; n.y = f.x; n.B = B; n.T = T; n.C = D; n.eps = 1e-5f; n.row_lens = lens;
@@ -177,11 +188,13 @@ static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_
   c = conv_args(f.x, B, T, D, F, m->k1, f.hid);
   mode.weights(c, w.w_1, w.w_1_tc, w.b_1);
   if (!seg) c.out_act = FS2_ACT_RELU;
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   c = conv_args(f.hid, B, T, F, D, m->k2, f.tmp);
   mode.weights(c, w.w_2, w.w_2_tc, w.b_2);
   c.res = f.x;
   if (seg) { c.in_act = FS2_ACT_LRELU; c.in_slope = 0.f; }
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   n.gamma = w.ln2_g; n.beta = w.ln2_b;
   return layernorm(&n, s);
@@ -210,17 +223,19 @@ static FftBufs fft_bufs(Arena& ar, const fs2_acoustic_model* m, size_t rows, int
 
 // VariancePredictor.forward (+ bucketize / embedding add when bins != NULL) on rows [B][T]  (model/modules.py:242-250, :80-100).
 // `head` carries the caller's part of the head's arguments: B, L = T, lens, control, target, bins, emb, pred_out, and x, which is
-// both the predictor's input and where the embedding is added.
+// both the predictor's input and where the embedding is added.  Ragged: the convs and LayerNorms are bounded by head.lens.
 static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_predictor_weights& w, fs2_variance_head_args head,
-                         float* h1, float* h2) {
+                         float* h1, float* h2, bool ragged) {
   const int B = head.B, T = head.L, k = m->vp_kernel, D = m->d_model, VF = m->vp_filter;
   const bool seg = (m->tc_mask & FS2_TC_PREDICTORS) && w.w_c1_tc && w.w_c2_tc;   // K-segmented: the ReLU is applied by the LayerNorm
   const ConvMode mode{seg ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};
-  fs2_layernorm_args n{};                                           // both LayerNorms: h1 -> h2, unmasked
-  n.x = h1; n.y = h2; n.B = B; n.T = T; n.C = VF; n.eps = 1e-5f; n.pre_relu = seg;
+  const int32_t* rag = ragged_lens(ragged, head.lens);
+  fs2_layernorm_args n{};                                           // both LayerNorms: h1 -> h2, unmasked (ragged: masked)
+  n.x = h1; n.y = h2; n.B = B; n.T = T; n.C = VF; n.eps = 1e-5f; n.pre_relu = seg; n.row_lens = rag;
   fs2_conv1d_args c = conv_args(head.x, B, T, D, VF, k, h1);
   mode.weights(c, w.w_c1, w.w_c1_tc, w.b_c1);
   if (!seg) c.out_act = FS2_ACT_RELU;
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   n.gamma = w.ln1_g; n.beta = w.ln1_b;
   FS2_TRY(layernorm(&n, s));
@@ -228,6 +243,7 @@ static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_
   mode.weights(c, w.w_c2, w.w_c2_tc, w.b_c2);
   c.pad_left = 1;                                                   // padding=1 is hard-coded upstream
   if (!seg) c.out_act = FS2_ACT_RELU;
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   n.gamma = w.ln2_g; n.beta = w.ln2_b;
   FS2_TRY(layernorm(&n, s));
@@ -236,7 +252,8 @@ static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_
 }
 
 // ------------------------------------------------------------------ phase 1
-static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cudaStream_t s, Arena& ar) {
+// ragged: utterance b has src_lens[b] phonemes; x_adapted rows at or beyond it are left unspecified.
+static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cudaStream_t s, Arena& ar, bool ragged) {
   const int B = a->B, L = a->L, D = m->d_model, VF = m->vp_filter;
   const size_t rows = (size_t)B * L;
   FftBufs f = fft_bufs(ar, m, rows);
@@ -250,7 +267,7 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
   e.ids = a->texts; e.table = m->word_emb; e.pos = m->enc_pos; e.y = f.x; e.B = B; e.L = L; e.D = D; e.n_vocab = m->n_vocab;
   FS2_TRY(embed_positions(&e, s));
   const ConvMode enc_mode{(m->tc_mask & FS2_TC_ENCODER) ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};   // exact attention either way
-  for (int i = 0; i < m->n_enc; i++) FS2_TRY(fft_block(s, m, m->enc[i], f, B, L, a->src_lens, enc_mode));
+  for (int i = 0; i < m->n_enc; i++) FS2_TRY(fft_block(s, m, m->enc[i], f, B, L, a->src_lens, enc_mode, ragged));
   if (m->spk_emb) {
     if (!a->speakers) return FS2_ERR_ARG;
     fs2_rowbias_args r{};
@@ -264,24 +281,24 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
   // duration on the un-embedded x; pitch on x; energy on x + pitch embedding.  energy uses p_control (modules.py:124).
   fs2_variance_head_args v{};
   v.x = a->x_adapted; v.B = B; v.L = L; v.lens = a->src_lens; v.control = 1.f; v.pred_out = a->logd_pred;
-  FS2_TRY(run_predictor(s, m, m->dur, v, h1, h2));
+  FS2_TRY(run_predictor(s, m, m->dur, v, h1, h2, ragged));
   v.control = a->p_control;
   if (!m->pitch_frame_level) {
     if (!a->p_pred) return FS2_ERR_ARG;
     v.target = a->p_target; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred;
-    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2));
+    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged));
   }
   if (!m->energy_frame_level) {
     if (!a->e_pred) return FS2_ERR_ARG;
     v.target = a->e_target; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred;
-    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2));
+    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged));
   }
 
   fs2_durations_args d{};
   d.src = a->d_target ? a->d_target : a->logd_pred; d.use_target = a->d_target != nullptr; d.d_control = a->d_control;
   d.B = B; d.L = L; d.d_rounded = a->d_target ? nullptr : a->d_rounded; d.cum = a->cum_dur; d.mel_lens = a->mel_lens;
   d.mel_lens32 = a->mel_lens32; d.len_stats = a->len_stats;
-  FS2_TRY(durations(&d, s));
+  FS2_TRY(durations(&d, s, ragged_lens(ragged, a->src_lens)));
   if (a->len_stats_host) {
     ce = cudaMemcpyAsync(a->len_stats_host, a->len_stats, 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
     if (ce != cudaSuccess) return FS2_ERR_CUDA - (int)ce;
@@ -290,7 +307,8 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
 }
 
 // ------------------------------------------------------------------ phase 2
-static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cudaStream_t s, Arena& ar) {
+// ragged: utterance b has mel_mask_lens[b] frames; mel and postnet_mel rows at or beyond it are zeroed.
+static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cudaStream_t s, Arena& ar, bool ragged) {
   const int B = a->B, T = a->T, D = m->d_model;
   const size_t rows = (size_t)B * T;
   FftBufs f = fft_bufs(ar, m, rows, B, T, (m->tc_mask & FS2_TC_DECODER) != 0);
@@ -315,22 +333,24 @@ static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cu
     if (m->pitch_frame_level) {
       if (!a->p_pred_frames) return FS2_ERR_ARG;
       v.target = a->p_target_frames; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred_frames;
-      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2));
+      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged));
     }
     if (m->energy_frame_level) {
       if (!a->e_pred_frames) return FS2_ERR_ARG;
       v.target = a->e_target_frames; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred_frames;
-      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2));
+      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged));
     }
     FS2_TRY(add_positions(f.x, m->dec_pos, B, T, D, s));
   }
   const ConvMode dec_mode{(m->tc_mask & FS2_TC_DECODER) ? ConvMode::TC : ConvMode::EXACT,
                           (m->tc_mask & FS2_TC_DECODER_F8) ? FS2_TC_VARIANT_F8 : 0u};
-  for (int i = 0; i < m->n_dec; i++) FS2_TRY(fft_block(s, m, m->dec[i], f, B, T, a->mel_mask_lens, dec_mode));
+  for (int i = 0; i < m->n_dec; i++) FS2_TRY(fft_block(s, m, m->dec[i], f, B, T, a->mel_mask_lens, dec_mode, ragged));
   const ConvMode post_mode{(m->tc_mask & FS2_TC_POSTNET) ? ConvMode::TC : ConvMode::EXACT,
                            (m->tc_mask & FS2_TC_POSTNET_F8) ? FS2_TC_VARIANT_F8 : 0u};
+  const int32_t* rag = ragged_lens(ragged, a->mel_mask_lens);
   fs2_conv1d_args c = conv_args(f.x, B, T, D, m->n_mel, 1, a->mel);
   post_mode.weights(c, m->w_mel, m->w_mel_tc, m->b_mel);
+  c.x_lens = rag;
   FS2_TRY(conv1d_dispatch(&c, s));
   // PostNet: eval BatchNorm folded into (w, b) by the packer; unmasked, tanh on all but the last (Layers.py:129-137)
   const float* cur = a->mel;
@@ -341,9 +361,11 @@ static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cu
     post_mode.weights(c, m->w_post[i], m->w_post_tc[i], m->b_post[i]);
     if (last) c.res = a->mel;
     else c.out_act = FS2_ACT_TANH;
+    c.x_lens = rag;
     FS2_TRY(conv1d_dispatch(&c, s));
     cur = dst;
   }
+  if (ragged) return zero_tail(a->mel, a->postnet_mel, a->mel_mask_lens, B, T, m->n_mel, s);   // the convs left those rows unspecified
   return FS2_OK;
 }
 
@@ -563,11 +585,11 @@ size_t fs2_encode_workspace_bytes(const fs2_acoustic_model* m, int B, int L) {
   Arena ar(nullptr, 0);
   fs2_encode_args a{};
   a.B = B; a.L = L;
-  encode_impl(m, &a, nullptr, ar);
+  encode_impl(m, &a, nullptr, ar, false);
   return ar.off + 256;
 }
 
-int fs2_acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) {
+static int acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st, bool ragged) {
   if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0) return FS2_ERR_ARG;
   if (!a->texts || !a->src_lens || !a->logd_pred || !a->mel_lens || !a->cum_dur || !a->x_adapted ||
       !a->len_stats || !a->workspace)
@@ -575,25 +597,29 @@ int fs2_acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, f
   if (!a->d_target && !a->d_rounded) return FS2_ERR_ARG;
   if (m->d_model / m->n_head != 128) return FS2_ERR_UNSUPPORTED;
   Arena ar(a->workspace, a->workspace_bytes);
-  return encode_impl(m, a, S(st), ar);
+  return encode_impl(m, a, S(st), ar, ragged);
 }
+int fs2_acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return acoustic_encode(m, a, st, false); }
+int fs2_acoustic_encode_ragged(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return acoustic_encode(m, a, st, true); }
 
 size_t fs2_decode_workspace_bytes(const fs2_acoustic_model* m, int B, int T) {
   if (!model_ok(m) || B <= 0 || T <= 0) return 0;
   Arena ar(nullptr, 0);
   fs2_decode_args a{};
   a.B = B; a.T = T;
-  decode_impl(m, &a, nullptr, ar);
+  decode_impl(m, &a, nullptr, ar, false);
   return ar.off + 256;
 }
 
-int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) {
+static int acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st, bool ragged) {
   if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0 || a->T <= 0) return FS2_ERR_ARG;
   if (!a->x_adapted || !a->cum_dur || !a->mel_mask_lens || !a->mel || !a->postnet_mel || !a->workspace) return FS2_ERR_ARG;
   if (m->d_model / m->n_head != 128) return FS2_ERR_UNSUPPORTED;
   Arena ar(a->workspace, a->workspace_bytes);
-  return decode_impl(m, a, S(st), ar);
+  return decode_impl(m, a, S(st), ar, ragged);
 }
+int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return acoustic_decode(m, a, st, false); }
+int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return acoustic_decode(m, a, st, true); }
 
 static bool vocoder_ok(const fs2_vocoder_model* m) {
   if (!(m && m->n_stages > 0 && m->n_stages <= FS2_MAX_STAGES && m->n_kernels > 0 && m->n_kernels <= FS2_MAX_DIL + 4 &&

@@ -206,18 +206,23 @@ int variance_head(const fs2_variance_head_args* a, cudaStream_t s) {
 
 // ------------------------------------------------------------------ durations (modules.py:132-135, :185-187)
 // One CTA per utterance: round-half-even (rintf == torch.round), truncate, block-wide inclusive scan.
-__global__ void durations_kernel(const fs2_durations_args a) {
+// RAG: ragged batch, columns l >= src_lens[b] do not exist: they are not read, count as 0 frames and d_rounded there is 0.
+template <bool RAG>
+__global__ void durations_kernel(const fs2_durations_args a, const int* __restrict__ src_lens) {
   __shared__ int warp_tot[32];
   __shared__ int carry_s;
   const int b = blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int nw = blockDim.x >> 5;
+  const int n = RAG ? ragged_rows(src_lens, 1, a.L, b) : a.L;
   if (tid == 0) carry_s = 0;
   __syncthreads();
   for (int base = 0; base < a.L; base += blockDim.x) {
     const int l = base + tid;
     int reps = 0;
-    if (l < a.L) {
+    if (RAG && l >= n && l < a.L) {
+      if (!a.use_target && a.d_rounded) a.d_rounded[(long long)b * a.L + l] = 0.f;
+    } else if (l < a.L) {
       const float s = a.src[(long long)b * a.L + l];
       float d;
       if (a.use_target) {
@@ -266,11 +271,33 @@ __global__ void durations_kernel(const fs2_durations_args a) {
   }
 }
 
-int durations(const fs2_durations_args* a, cudaStream_t s) {
+int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens) {
   if (!a || !a->src || !a->cum || !a->mel_lens || !a->len_stats || a->B <= 0 || a->L <= 0) return FS2_ERR_ARG;
   cudaError_t e = cudaMemsetAsync(a->len_stats, 0, 3 * sizeof(int), s);
   if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
-  durations_kernel<<<a->B, 256, 0, s>>>(*a);
+  if (src_lens) durations_kernel<true><<<a->B, 256, 0, s>>>(*a, src_lens);
+  else durations_kernel<false><<<a->B, 256, 0, s>>>(*a, nullptr);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+// ------------------------------------------------------------------ y0[b,t,:] = y1[b,t,:] = 0 for t >= lens[b] (ragged acoustic outputs)
+__global__ void zero_tail_kernel(float* __restrict__ y0, float* __restrict__ y1, const int* __restrict__ lens, long long rows, int T, int C4) {
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int b = (int)(row / T), t = (int)(row - (long long)b * T);
+  if (t < ragged_rows(lens, 1, T, b)) return;
+  const int lane = threadIdx.x & 31;
+  float4* o0 = reinterpret_cast<float4*>(y0) + row * C4;
+  float4* o1 = reinterpret_cast<float4*>(y1) + row * C4;
+  for (int c = lane; c < C4; c += 32) { o0[c] = make_float4(0.f, 0.f, 0.f, 0.f); o1[c] = make_float4(0.f, 0.f, 0.f, 0.f); }
+}
+
+int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cudaStream_t s) {
+  if (!y0 || !y1 || !lens || B <= 0 || T <= 0 || C <= 0) return FS2_ERR_ARG;
+  if (C % 4 || !aligned16(y0) || !aligned16(y1)) return FS2_ERR_UNSUPPORTED;
+  const long long rows = (long long)B * T;
+  zero_tail_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(y0, y1, lens, rows, T, C / 4);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

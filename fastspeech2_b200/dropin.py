@@ -3,6 +3,7 @@
     import fastspeech2_b200.dropin as dropin; dropin.install()           # programmatic
     python -m fastspeech2_b200.dropin synthesize.py --text ... -p ... -m ... -t ...   # run the untouched reference CLI
     python -m fastspeech2_b200.dropin --ragged-vocoder synthesize.py --mode batch ...  # ... vocoding each utterance on its own frames
+    python -m fastspeech2_b200.dropin --ragged synthesize.py --mode batch ...          # ... and synthesising its mel as if alone
 
 `utils/model.py:7-8` does `import hifigan` and `from model import FastSpeech2, ScheduledOptim`; both names are bound here
 to `fastspeech2_b200.hifigan` / `fastspeech2_b200.model`, whose classes keep the reference's constructor arguments,
@@ -98,14 +99,18 @@ def patch_text_dataset() -> bool:
 
 def main(argv=None) -> None:
     argv = list(sys.argv[1:] if argv is None else argv)
-    ragged = False
-    while argv and argv[0] == "--ragged-vocoder":      # our flags come before the script path; everything after it is the script's
+    ragged = ragged_acoustic = False
+    while argv and argv[0] in ("--ragged-vocoder", "--ragged"):   # our flags come before the script path; everything after it is the script's
         ragged = True
-        argv.pop(0)
+        ragged_acoustic |= argv.pop(0) == "--ragged"
     if not argv:
-        raise SystemExit("usage: python -m fastspeech2_b200.dropin [--ragged-vocoder] <reference script, e.g. synthesize.py> [script args...]")
+        raise SystemExit("usage: python -m fastspeech2_b200.dropin [--ragged | --ragged-vocoder] <reference script, e.g. synthesize.py> "
+                         "[script args...]")
     script = os.path.abspath(argv[0])
     install()
+    if ragged_acoustic:                                # every FastSpeech2 the script builds runs ragged (FastSpeech2.ragged)
+        import fastspeech2_b200.model as b_model
+        b_model.FastSpeech2.ragged = True
     sys.argv = [script] + argv[1:]
     sys.path.insert(0, os.path.dirname(script))       # the reference resolves `utils`, `text`, `dataset` relative to itself
     patch_vocoder_infer(ragged=ragged)

@@ -23,6 +23,12 @@ class FastSpeech2(nn.Module):
     Arguments, parameter names and return values mirror the reference class (model/fastspeech2.py:16-41,:43-110).
     """
 
+    # Ragged mode, per instance or for the class (forward's `ragged` overrides it per call): utterance b is synthesised from its own
+    # src_lens[b] phonemes and mel_lens[b] frames only, bit for bit as it would be alone, and the padding's work is skipped
+    # (fs2_acoustic_encode_ragged in fs2b200.h).  Off: the reference's batched semantics, in which padded rows reach the last phonemes
+    # and frames of every shorter utterance.
+    ragged = False
+
     def __init__(self, preprocess_config, model_config):
         super().__init__()
         self.model_config = model_config
@@ -163,15 +169,16 @@ class FastSpeech2(nn.Module):
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
     def forward(self, speakers, texts, src_lens, max_src_len, mels=None, mel_lens=None, max_mel_len=None,
-                p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0):
+                p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0, ragged=None):
+        """The reference's forward; `ragged` (None: the module's `ragged` attribute) selects the ragged mode described in __init__."""
         # the C ABI sets up per-device kernel attributes for the CURRENT device: make the model's device current
         dev = get(self, "mel_linear.weight").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
             return self._forward(speakers, texts, src_lens, max_src_len, mels, mel_lens, max_mel_len, p_targets, e_targets, d_targets,
-                                 p_control, e_control, d_control)
+                                 p_control, e_control, d_control, self.ragged if ragged is None else bool(ragged))
 
     def _forward(self, speakers, texts, src_lens, max_src_len, mels=None, mel_lens=None, max_mel_len=None,
-                 p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0):
+                 p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0, ragged=False):
         if self.training:
             raise NotImplementedError("H100-native FastSpeech2 is inference-only: call .eval() (utils/model.py:32)")
         p_frame = self.pitch_feature_level == "frame_level"
@@ -213,7 +220,8 @@ class FastSpeech2(nn.Module):
                           d_rounded=d_rounded.data_ptr(), mel_lens=mel_lens_out.data_ptr(), mel_lens32=mel_lens32.data_ptr(),
                           cum_dur=cum.data_ptr(), x_adapted=x_adapted.data_ptr(), len_stats=stats_dev.data_ptr(),
                           len_stats_host=self._stats_host.data_ptr(), workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        L.check(lib.fs2_acoustic_encode(C.byref(m), C.byref(ea), stream), "fs2_acoustic_encode")
+        encode = lib.fs2_acoustic_encode_ragged if ragged else lib.fs2_acoustic_encode
+        L.check(encode(C.byref(m), C.byref(ea), stream), "fs2_acoustic_encode")
 
         if max_mel_len is not None:
             T = int(max_mel_len)
@@ -250,7 +258,8 @@ class FastSpeech2(nn.Module):
                           p_pred_frames=p_pred.data_ptr() if p_frame else 0, e_pred_frames=e_pred.data_ptr() if e_frame else 0,
                           mel=mel.data_ptr(), postnet_mel=post.data_ptr(),
                           workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        L.check(lib.fs2_acoustic_decode(C.byref(m), C.byref(da), stream), "fs2_acoustic_decode")
+        decode = lib.fs2_acoustic_decode_ragged if ragged else lib.fs2_acoustic_decode
+        L.check(decode(C.byref(m), C.byref(da), stream), "fs2_acoustic_decode")
 
         src_masks = torch.arange(Lmax, device=dev)[None, :] >= src_lens32[:, None]
         mel_masks = torch.arange(T, device=dev)[None, :] >= mask_lens32[:, None]

@@ -310,6 +310,21 @@ typedef struct fs2_decode_args {
 size_t fs2_decode_workspace_bytes(const fs2_acoustic_model* m, int B, int T);
 int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t stream);
 
+/* Ragged mode of the pair above: same models, arguments and workspace sizes.  Utterance b is bounded by src_lens[b] phonemes in the
+ * encoder and the predictors and by mel_mask_lens[b] frames in the decoder, so it is computed exactly -- bit for bit -- as a B = 1
+ * call of fs2_acoustic_encode / fs2_acoustic_decode with L = src_lens[b] and T = mel_mask_lens[b] on its own inputs would compute it:
+ *   - no value at or beyond an utterance's length (token ids, targets, durations, whatever the workspace holds) reaches its valid
+ *     outputs, and no work item lying wholly in the padding is computed (every conv gets the lengths as x_lens);
+ *   - p_pred / e_pred / logd_pred / d_rounded / cum_dur are valid on the first src_lens[b] columns (frame-level predictions: on the
+ *     first mel_mask_lens[b]); d_rounded is 0 beyond, durations beyond src_lens[b] count as 0 frames;
+ *   - mel and postnet_mel are exact zeros in rows >= mel_mask_lens[b];
+ *   - x_adapted rows at or beyond src_lens[b] are unspecified;
+ *   - the decoder's attention picks its backend per utterance as a B = 1 call would: the fused tensor-core kernel for utterances of
+ *     >= 128 frames, the exact kernel for shorter ones.
+ * Device lengths are clamped to [0, L] / [0, T] and never read by the host; position-table rows are shared by all utterances. */
+int fs2_acoustic_encode_ragged(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t stream);
+int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ vocoder (hifigan Generator.forward) */
 
 typedef struct fs2_vocoder_model {

@@ -164,6 +164,7 @@ EXPORTS = {
     "fs2_conv_tc_block": (i32, [i32]),
     "fs2_conv_tc_block_f8": (i32, [i32]),
     "fs2_conv_tc_plan": (i32, [C.c_void_p, i32, C.c_void_p]),
+    "fs2_conv_simt_plan": (i32, [C.c_void_p, i32, C.c_void_p]),
     "fs2_layernorm": (i32, [C.POINTER(LayerNormArgs), fp]),
     "fs2_attention": (i32, [C.POINTER(AttentionArgs), fp]),
     "fs2_attention_workspace_bytes": (C.c_size_t, [i32, i32, i32]),

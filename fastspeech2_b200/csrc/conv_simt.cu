@@ -191,6 +191,26 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   }
 }
 
+// Tile choice of the launcher (pure host logic, no CUDA call; exposed as fs2_conv_simt_plan so that the GPU tests' coverage of the six
+// (BM, BN) instantiations is checkable without a GPU): out[4] = {BM, BN, grid.x, grid.y}.
+int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int* out) {
+  if (!a || !out || num_sms <= 0) return FS2_ERR_ARG;
+  if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
+  if (a->Cin % BK != 0 || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
+  // 128-row tiles by default; 64-row tiles when the grid would not even give every SM two CTAs (encoder / predictors: 2048 rows)
+  const int nblk = a->N > 64 ? (a->N + 127) / 128 : 1;
+  const bool small = (long long)((a->T + 127) / 128) * a->B * nblk < 2LL * num_sms;
+  const int bm = small ? 64 : 128;
+  const long long gx = (long long)((a->T + bm - 1) / bm) * a->B;
+  if (gx > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
+  // narrow outputs on small problems (FFN w_2, predictor convs: 2048 rows x 256 channels): 64-column CTAs double the CTA count
+  // while the 128-column grid leaves SMs idle
+  const bool narrow_small = small && a->N > 64 && gx * ((a->N + 127) / 128) < num_sms;
+  const int bn = (a->N > 64 && !narrow_small) ? 128 : a->N > 32 ? 64 : 32;
+  out[0] = bm; out[1] = bn; out[2] = (int)gx; out[3] = (a->N + bn - 1) / bn;
+  return FS2_OK;
+}
+
 int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
@@ -214,36 +234,27 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // SM count of the current device
   if (!dv) return derr;
-  const long long num_sms = dv->num_sms.load(std::memory_order_relaxed);
-  // 128-row tiles by default; 64-row tiles when the grid would not even give every SM two CTAs (encoder / predictors: 2048 rows)
-  const int nblk = a->N > 64 ? (a->N + 127) / 128 : 1;
-  const bool small = (long long)((a->T + 127) / 128) * a->B * nblk < 2LL * num_sms;
-  const int bm = small ? 64 : 128;
-  p.tiles_per_batch = (a->T + bm - 1) / bm;
-  const long long gx = (long long)p.tiles_per_batch * a->B;
-  if (gx > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
+  int plan[4];
+  FS2_TRY(conv_simt_plan(a, dv->num_sms.load(std::memory_order_relaxed), plan));
+  const int bm = plan[0], bn = plan[1];
+  p.tiles_per_batch = plan[2] / a->B;
+  const dim3 grid((unsigned)plan[2], (unsigned)plan[3]);
   prof_before(s);
-#define FS2_SIMT_ACT(BM_, BN_, grid_)                                                                      \
-  switch (a->out_act) {                                                                                    \
-    case FS2_ACT_RELU: conv_simt_kernel<BM_, BN_, FS2_ACT_RELU><<<grid_, 256, 0, s>>>(p); break;           \
-    case FS2_ACT_TANH: conv_simt_kernel<BM_, BN_, FS2_ACT_TANH><<<grid_, 256, 0, s>>>(p); break;           \
-    case FS2_ACT_LRELU: conv_simt_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid_, 256, 0, s>>>(p); break;         \
-    default: conv_simt_kernel<BM_, BN_, FS2_ACT_NONE><<<grid_, 256, 0, s>>>(p); break;                     \
+#define FS2_SIMT_ACT(BM_, BN_)                                                                            \
+  switch (a->out_act) {                                                                                   \
+    case FS2_ACT_RELU: conv_simt_kernel<BM_, BN_, FS2_ACT_RELU><<<grid, 256, 0, s>>>(p); break;           \
+    case FS2_ACT_TANH: conv_simt_kernel<BM_, BN_, FS2_ACT_TANH><<<grid, 256, 0, s>>>(p); break;           \
+    case FS2_ACT_LRELU: conv_simt_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); break;         \
+    default: conv_simt_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p); break;                     \
   }
-#define FS2_SIMT_LAUNCH(BN_, grid_)                   \
-  if (small) { FS2_SIMT_ACT(64, BN_, grid_) } else { FS2_SIMT_ACT(128, BN_, grid_) }
-  // narrow outputs on small problems (FFN w_2, predictor convs: 2048 rows x 256 channels): 64-column CTAs double the CTA count
-  // while the 128-column grid leaves SMs idle
-  const bool narrow_small = small && a->N > 64 && (long long)gx * ((a->N + 127) / 128) < num_sms;
-  if (a->N > 64 && !narrow_small) {
-    dim3 grid((unsigned)gx, (a->N + 127) / 128);
-    FS2_SIMT_LAUNCH(128, grid)
-  } else if (a->N > 32) {
-    dim3 grid((unsigned)gx, (a->N + 63) / 64);
-    FS2_SIMT_LAUNCH(64, grid)
+#define FS2_SIMT_LAUNCH(BN_) \
+  if (bm == 64) { FS2_SIMT_ACT(64, BN_) } else { FS2_SIMT_ACT(128, BN_) }
+  if (bn == 128) {
+    FS2_SIMT_LAUNCH(128)
+  } else if (bn == 64) {
+    FS2_SIMT_LAUNCH(64)
   } else {
-    dim3 grid((unsigned)gx, 1);
-    FS2_SIMT_LAUNCH(32, grid)
+    FS2_SIMT_LAUNCH(32)
   }
 #undef FS2_SIMT_LAUNCH
 #undef FS2_SIMT_ACT

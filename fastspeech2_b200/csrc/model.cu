@@ -63,6 +63,7 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 
 // kernels / launchers defined in the other translation units
 int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s);
+int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int* out);
 int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
@@ -508,6 +509,7 @@ int fs2_abi_version(void) { return 11; }
 int fs2_conv_tc_block(int N) { return conv_tc_nb(N, 128); }
 int fs2_conv_tc_block_f8(int N) { return conv_tc_nb(N, 64); }
 int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_tc_plan_query(a, num_sms, out); }
+int fs2_conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_simt_plan(a, num_sms, out); }
 int64_t fs2_kernel_launch_count(void) { return (int64_t)g_launch_count.load(); }
 size_t fs2_struct_size(int which) {
   switch (which) {

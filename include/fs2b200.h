@@ -78,6 +78,10 @@ struct fs2_conv1d_args;
  * grid, dynamic shared memory bytes}.
  * Returns FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
 int fs2_conv_tc_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out);
+/* Tile the exact fp32 kernel (FS2_CONV_SIMT) would use for this call on a device with num_sms SMs (pure host logic, no CUDA call,
+ * pointers are not read): out[4] = {BM (rows per CTA: 64 or 128), BN (output channels per CTA: 32, 64 or 128), grid.x, grid.y}.
+ * Returns FS2_ERR_ARG / FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
+int fs2_conv_simt_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out);
 
 #define FS2_MAX_LAYERS 12
 #define FS2_MAX_POSTNET 8

@@ -173,6 +173,52 @@ def test_gpu_case_tables_reach_every_tile_width_and_the_persistent_loop():
     assert _rs_plan(32, 1000, (3,), ((33,),))[0] == -2
 
 
+def test_gpu_case_tables_reach_every_exact_conv_tile():
+    """The exact fp32 conv tests (tests/test_gpu_ops.py::test_conv1d, ::test_conv1d_ragged) reach, on a 132-SM device, all six (BM, BN)
+    tiles of conv_simt_kernel, each with all four output activations, a partial row tile and a partial column tile; plus T = 1, one
+    K-step, 11 dilated taps, pad_left 0 and off-centre, alpha / residual / accumulate, row_lens, strided views, LRELU input with slopes
+    0 and 0.1, and ragged lengths 0, 1, BM - 1, BM, BM + 1 and T with lens_scale 1 and 8.  Checked here against fs2_conv_simt_plan."""
+    from tests import test_gpu_ops as G
+    seen = {}
+    for case in G.CONV_CASES:
+        case, opts = G._case_opts(case)
+        B, T, Cin, N, taps, dil, pad, in_act, out_act = case[:9]
+        bm, bn = G.simt_plan(B, T, Cin, N, taps)
+        s = seen.setdefault((bm, bn), {"acts": set(), "T_tail": False, "N_tail": False})
+        s["acts"].add(out_act)
+        s["T_tail"] |= T % bm != 0
+        s["N_tail"] |= N % bn != 0
+    assert set(seen) == G.SIMT_TILES
+    for tile, s in seen.items():
+        assert s["acts"] == {0, 1, 2, 3} and s["T_tail"] and s["N_tail"], (tile, s)
+    cases = [G._case_opts(c) for c in G.CONV_CASES]
+    assert any(c[1] == 1 for c, _ in cases) and any(c[2] == 16 for c, _ in cases)
+    assert any(c[4] == 11 and c[5] > 1 for c, _ in cases)
+    pads = {"zero": any(c[6] == 0 and c[4] > 1 for c, _ in cases), "off_centre": any(c[6] not in (0, (c[4] - 1) * c[5] // 2) for c, _ in cases)}
+    assert all(pads.values()), pads
+    assert any(c[9] and c[10] != 1.0 and c[11] for c, _ in cases) and any(c[12] for c, _ in cases)
+    assert any(o.get("strided") for _, o in cases)
+    assert {o.get("in_slope", 0.1) for c, o in cases if c[7] == 3} == {0.0, 0.1}
+    assert {G.simt_plan(*c[:5])[1] for c, _ in cases if c[3] % 4 == 0 and c[3] <= 32} == {32}     # GW = 2 stores
+    # ragged: row counts 0, 1, BM - 1, BM, BM + 1, T in both row tiles (lens_scale 1), and lens_scale 8
+    for bm in (64, 128):
+        rows = set()
+        for B, T, Cin, N, taps, *_, scale, xl in G.RAGGED_CONV_CASES:
+            if G.simt_plan(B, T, Cin, N, taps)[0] == bm and scale == 1:
+                rows |= {min(l * scale, T) for l in xl} | ({"T"} if T in xl else set())
+        assert {0, 1, bm - 1, bm, bm + 1, "T"} <= rows, (bm, rows)
+    assert {c[9] for c in G.RAGGED_CONV_CASES} == {1, 8}
+    assert any(l * c[9] > c[1] for c in G.RAGGED_CONV_CASES for l in c[10])
+    # the tile choice itself: 64-row tiles below two CTAs per SM, 64-column tiles when 128 would leave SMs idle
+    assert G.simt_plan(16, 1000, 256, 1024, 9) == (128, 128) and G.simt_plan(2, 131, 1024, 256, 1) == (64, 64)
+    h = _lib.lib()
+    a = _lib.Conv1dArgs(x=16, w=16, y=16, B=1, T=128, Cin=24, N=16, taps=1)
+    out = (ctypes.c_int32 * 4)()
+    assert h.fs2_conv_simt_plan(ctypes.byref(a), 132, out) == -2
+    a.Cin, a.T = 16, 0
+    assert h.fs2_conv_simt_plan(ctypes.byref(a), 132, out) == -1
+
+
 def test_fused_resblock_plan_respects_the_hardware_limits():
     """fs2_resstack_plan (pure host logic) over the shipped generator's kernel / dilation sets, every single-pair shape and a sweep of
     lengths: the halo covers the receptive radius, the output boxes tile the work item exactly in whole swizzle atoms, and shared memory

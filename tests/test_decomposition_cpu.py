@@ -144,3 +144,114 @@ def test_conv_post_sliding_window_schedule():
                                 assert np.isnan(out[t - o + sub])
                                 out[t - o + sub] = np.tanh(keep[sub] + 0.05)
         assert not np.isnan(out).any() and np.abs(out - want).max() < 1e-12, T
+
+
+# The exact-kernel bars of tests/test_gpu_ops.py against the faults they are there to catch, emulated in fp64 on the same cases: each
+# must put some element at least 100x past its bar, so a kernel with that fault fails its test.
+REJECT = 100.0
+
+
+def test_exact_conv_bar_rejects_a_dropped_k_step():
+    """One 16-channel K-step left out, at the longest sum of test_conv1d's table (K = 9216): every 64-row tile is caught."""
+    from tests import test_gpu_ops as G
+    case = max((G._case_opts(c)[0] for c in G.CONV_CASES), key=lambda c: c[2] * c[4])
+    assert case[2] * case[4] == 9216
+    B, T, Cin, N, taps, dil, pad, in_act, out_act, _, alpha, _, _ = case
+    x, w, bias, res, y0, lens = G._conv_case(case)
+    want = E.conv1d(x.double(), w.double(), bias.double(), dil, pad, in_act, 0.1, out_act, 0.1)
+    scale = G.conv_scale(x, w, bias, dil, pad, in_act, 0.1, None, alpha, None, None)
+    wf = w.clone()
+    wf[taps // 2, 7 * 16:8 * 16] = 0.0
+    fault = E.conv1d(x.double(), wf.double(), bias.double(), dil, pad, in_act, 0.1, out_act, 0.1)
+    bm = G.simt_plan(B, T, Cin, N, taps)[0]
+    tiles = [G.normalised_err(fault[b:b + 1, s:s + bm], want[b:b + 1, s:s + bm], scale[b:b + 1, s:s + bm]) for b in range(B) for s in range(0, T, bm)]
+    assert min(tiles) > REJECT * G.CONV_EXACT_C, (min(tiles), G.CONV_EXACT_C)
+
+
+def test_exact_conv_bar_rejects_a_halo_row_off_by_one():
+    """The first row of the second 64-row tile reading its first tap's input one row late (a halo load off by one at a tile edge)."""
+    from tests import test_gpu_ops as G
+    case, opts = next(G._case_opts(c) for c in G.CONV_CASES if G._case_opts(c)[0][:5] == (2, 300, 64, 48, 5))
+    B, T, Cin, N, taps, dil, pad, in_act, out_act, _, alpha, _, _ = case
+    slope = opts.get("in_slope", 0.1)
+    x, w, bias, _, _, _ = G._conv_case(case)
+    bm = G.simt_plan(B, T, Cin, N, taps)[0]
+    t, shift = bm, -pad
+    xd, wd = x.double(), w.double()
+    acc = E.conv1d(xd, wd, None, dil, pad, in_act, slope)
+    want = E.conv1d_epilogue(acc, bias.double(), out_act, 0.1)
+    xa = E._act(xd, in_act, slope)
+    acc[:, t] += (xa[:, t + shift + 1] - xa[:, t + shift]) @ wd[0]
+    fault = E.conv1d_epilogue(acc, bias.double(), out_act, 0.1)
+    scale = G.conv_scale(x, w, bias, dil, pad, in_act, slope, None, alpha, None, None)
+    for b in range(B):
+        e = G.normalised_err(fault[b:b + 1, t:t + 1], want[b:b + 1, t:t + 1], scale[b:b + 1, t:t + 1])
+        assert e > REJECT * G.CONV_EXACT_C, (b, e)
+
+
+def _tiled_softmax_attention(qkv, lens, rescale=True, mask_before_max=True):
+    """The exact attention kernel's online softmax over 64-key tiles in fp64, with p = exp(s - m) rounded through fp32 as the kernel
+    computes it.  rescale=False: O and l are not rescaled when a later tile raises the running max.  mask_before_max=False: the max
+    is taken over every key of the visited tiles, the masked ones past n in the last tile included."""
+    B, T, _ = qkv.shape
+    q, k, v = (qkv[..., i * 256:(i + 1) * 256].double().reshape(B, T, 2, 128).permute(0, 2, 1, 3) for i in range(3))
+    out = torch.zeros(B, 2, T, 128, dtype=torch.float64)
+    for b, n in enumerate(lens):
+        n = min(max(n, 0), T)
+        if n == 0:
+            continue
+        s = q[b] @ k[b].transpose(-1, -2) / 128 ** 0.5
+        key = torch.arange(T)
+        m = torch.full((2, T, 1), float("-inf"), dtype=torch.float64)
+        l = torch.zeros(2, T, 1, dtype=torch.float64)
+        o = torch.zeros(2, T, 128, dtype=torch.float64)
+        for k0 in range(0, n, 64):
+            st = s[:, :, k0:k0 + 64]
+            valid = key[k0:k0 + 64] < n
+            m_tile = (st if not mask_before_max else st.masked_fill(~valid, float("-inf"))).amax(-1, keepdim=True)
+            m_new = torch.maximum(m, m_tile)
+            p = torch.exp((st - m_new).float()).double().masked_fill(~valid, 0.0)
+            c = torch.exp(m - m_new) if rescale else torch.ones_like(m)
+            l = l * c + p.sum(-1, keepdim=True)
+            o = o * c + p @ v[b][:, k0:k0 + 64]
+            m = m_new
+        out[b] = o / l
+        out[b, :, n:] = 0.0
+    return out.permute(0, 2, 1, 3).reshape(B, T, 256)
+
+
+def test_attention_bar_rejects_a_missing_rescale_and_a_max_over_masked_keys():
+    """On test_attention_adversarial_scores' cases: the emulated kernel matches fp64 within the bar as it is; without the online
+    rescale (row max in the last key tile) or with masked keys in the max (they hold the largest scores), every utterance with more
+    than one key tile, respectively with masked keys in its last tile, is caught."""
+    from tests import test_gpu_ops as G
+    bar = max(G.ATT_EXACT_C.values())
+    for kind, fault in (("last_tile_max", dict(rescale=False)), ("masked_max", dict(mask_before_max=False))):
+        T, lens = next((T, lens) for k, T, lens in G.ATT_ADV_CASES if k == kind)
+        qkv = G.attention_qkv(kind, lens, T)
+        kl = torch.tensor(lens, dtype=torch.int32)
+        want = E.attention(qkv.double(), 2, kl)
+        scale = G.attention_bar_scale(qkv, kl)
+        good = _tiled_softmax_attention(qkv, lens)
+        bad = _tiled_softmax_attention(qkv, lens, **fault)
+        for b, n in enumerate(lens):
+            n = min(max(n, 0), T)
+            e_good = G.attention_normalised_err(good[b:b + 1], want[b:b + 1], scale[b:b + 1])
+            assert e_good < bar / 4, (kind, b, e_good)
+            if (kind == "last_tile_max" and n > 64) or (kind == "masked_max" and 0 < n < T and n % 64):
+                e = G.attention_normalised_err(bad[b:b + 1], want[b:b + 1], scale[b:b + 1])
+                assert e > REJECT * bar, (kind, b, n, e)
+
+
+def test_layernorm_bar_rejects_a_one_pass_variance():
+    """E[x^2] - E[x]^2 in fp32 on test_layernorm's rows with |mean| / std up to 1e4."""
+    from tests import test_gpu_ops as G
+    for C in (80, 256, 1024):
+        x = G.layernorm_rows(C)
+        gm, bt = 1 + G.rnd(C, seed=2, scale=0.1), G.rnd(C, seed=3, scale=0.1)
+        want = E.layernorm(x.double(), gm.double(), bt.double())
+        mean = x.mean(-1, keepdim=True)
+        var = ((x * x).mean(-1, keepdim=True) - mean * mean).clamp_min(0.0)
+        fault = (x - mean) * torch.rsqrt(var + 1e-5) * gm + bt
+        e = G.normalised_err(fault, want, G.ln_scale(x, gm, bt))
+        assert e > REJECT * G.LN_C, (C, e)

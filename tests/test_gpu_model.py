@@ -32,17 +32,19 @@ def _cmp(out, ref):
     return errs
 
 
-def _free_running_then_teacher_forced(m, sd, batch, name, parity_log, **kw):
+def _free_running_then_teacher_forced(m, sd, batch, name, parity_log, oracle=None, mel_tol=MEL_TOL, raw_heads=False, **kw):
     """SURVEY.md section 7, hard part 2: pitch / energy buckets are discrete decisions -- a prediction that lies within fp32 summation
     noise (~3e-6) of one of the 255 bin edges can land in different buckets on the GPU and in the CPU oracle (with ~10^4 phonemes
     per batch that happens for roughly one batch in four; the reference itself flips between thread counts), which swaps an
     embedding row and changes that utterance's whole mel.  Protocol: (A) free-running -- durations exact, continuous predictions
     within 1e-4, every bucket difference must be such a boundary case (margin < 2e-5) and is logged; (B) if any bucket differs, the
     mel is compared teacher-forced on the oracle's own decisions (p / e / d targets), which cannot hide a real error.  The same holds
-    for a duration that sits on a rounding boundary of round(exp(logd) - 1) (margin < 2e-4 frames)."""
+    for a duration that sits on a rounding boundary of round(exp(logd) - 1) (margin < 2e-4 frames).  oracle: the oracle's free-running
+    and teacher-forced outputs for this batch when the caller has them already.  raw_heads: pitch / energy are unnormalised (Hz and
+    energy in the hundreds, config/LJSpeech_paper), so their bar (5e-4) and their bin-edge margin are relative to 1 + |oracle value|."""
     spk, texts, lens, Lm = batch
     dev = lambda t: t.to(DEV)
-    ref = O.fastspeech2_forward(sd, spk, texts, lens, Lm, **kw)
+    ref = oracle[0] if oracle else O.fastspeech2_forward(sd, spk, texts, lens, Lm, **kw)
     out = m(dev(spk), dev(texts), dev(lens), Lm, **kw)
     flips = 0
     for b, l in (out[5].cpu() != ref[5]).nonzero().tolist():          # a duration on a rounding boundary (round-half-even of exp(logd) - 1)
@@ -52,23 +54,41 @@ def _free_running_then_teacher_forced(m, sd, batch, name, parity_log, **kw):
         flips += 1
     if not flips:
         assert torch.equal(out[9].cpu(), ref[9]) and torch.equal(out[7].cpu(), ref[7])
-    e = {k: (out[i].cpu() - ref[i]).abs().max().item() for i, k in ((2, "pitch"), (3, "energy"), (4, "logd"))}
-    assert max(e["pitch"], e["energy"], e["logd"]) < 1e-4, e
+    unit = lambda r: 1 + r.abs() if raw_heads else 1.0
+    err = lambda o, r: ((o.cpu() - r).abs() / unit(r)).max().item()
+    # raw-valued heads: the fp32 noise the 100-250x head weights amplify is ~2e-4 of 1 + |value| (the relative bar of the paper config's
+    # golden test), so a bucket may differ wherever the oracle's value lies within that of an edge
+    cont_tol, edge_tol = (5e-4, 5e-4) if raw_heads else (1e-4, 2e-5)
+    e = {"logd": (out[4].cpu() - ref[4]).abs().max().item()}
+    assert e["logd"] < 1e-4, e
+    # Each decision changes what the later predictors see: the energy predictor's input holds the pitch embedding, and frame-level
+    # predictors run on the duration-expanded sequence.  So a prediction is compared free-running only while every decision before it
+    # matched; after a boundary flip it is compared teacher-forced, where its input is the oracle's again.
+    same_inputs = not flips or ref[2].shape == texts.shape
     for i, nm in ((2, "pitch"), (3, "energy")):
+        if not same_inputs:
+            break
+        e[nm] = err(out[i], ref[i])
+        assert e[nm] < cont_tol, e
         edges = sd[f"variance_adaptor.{nm}_bins"]
         bo, br = torch.bucketize(out[i].cpu(), edges), torch.bucketize(ref[i], edges)
         diff = (bo != br).nonzero()
         for b, l in diff.tolist():
-            margin = (edges - ref[i][b, l]).abs().min().item()
-            assert margin < 2e-5, f"{nm} bucket differs away from a bin edge: utterance {b} phoneme {l} margin {margin}"
+            margin = ((edges - ref[i][b, l]).abs().min() / unit(ref[i][b, l])).item()
+            assert margin < edge_tol, f"{nm} bucket differs away from a bin edge: utterance {b} position {l} margin {margin}"
         flips += diff.shape[0]
+        same_inputs = diff.shape[0] == 0
+    e_free = e
     if flips:
         T = int(ref[9].max())
-        ref = O.fastspeech2_forward(sd, spk, texts, lens, Lm, None, ref[9], T, ref[2], ref[3], ref[5].long(), **kw)
+        ref = oracle[1] if oracle else O.fastspeech2_forward(sd, spk, texts, lens, Lm, None, ref[9], T, ref[2], ref[3], ref[5].long(), **kw)
         out = m(dev(spk), dev(texts), dev(lens), Lm, None, dev(ref[9]), T, dev(ref[2]), dev(ref[3]), dev(ref[5].long()), **kw)
+        e_tf = {nm: err(out[i], ref[i]) for i, nm in ((2, "pitch"), (3, "energy"))}
+        assert max(e_tf.values()) < cont_tol, e_tf
     e = _cmp(out, ref)
-    parity_log(name, **e, decision_flips_at_boundaries=flips, tmax=int(ref[9].max()), frames=int(ref[9].sum()))
-    assert e["mel"] < MEL_TOL and e["postnet"] < MEL_TOL, e
+    parity_log(name, **e, **{f"free_running_{k}": v for k, v in e_free.items()}, decision_flips_at_boundaries=flips, tmax=int(ref[9].max()),
+               frames=int(ref[9].sum()))
+    assert e["mel"] < mel_tol and e["postnet"] < mel_tol, e
     return out, ref
 
 

@@ -164,7 +164,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
   constexpr uint32_t KBLK = 8192;                // one 16-wide K-block of an A operand: hi plane 4 KB + lo plane 4 KB (128 rows)
   constexpr uint32_t PLANES = 8 * KBLK;          // 128 x 128 operand: 64 KB
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = warp_uniform_id(), lane = tid & 31;
   unsigned char* qa = smem_raw;                  // Q operand planes
   unsigned char* pa = qa + PLANES;               // P operand planes
   unsigned char* ring = pa + PLANES;

@@ -123,6 +123,12 @@ __device__ __forceinline__ uint32_t cvt_e4m3x2_sat(float a0, float a1) {
   return (uint32_t)h;
 }
 
+// Warp index of the calling thread, in a form ptxas knows to be warp-uniform.  threadIdx.x >> 5 is uniform only because the
+// block is one-dimensional, which ptxas cannot assume: a role branch on it counts as divergent, and every wgmma under such a
+// branch is then serialised (warning C7520: a warpgroup arrive and a full wait around each MMA, so commit groups and
+// wait_group<1> stop overlapping anything).  A shuffle from lane 0 is uniform by construction.
+__device__ __forceinline__ int warp_uniform_id() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
+
 // mbarrier ring cursor without runtime div/mod (an integer division per tap was on the MMA issuer's critical path)
 struct Ring {
   uint32_t idx = 0, phase = 0;
@@ -279,13 +285,13 @@ __device__ __forceinline__ void tc_release(uint64_t* bar) {
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-// RAG: ragged batch (TcP::x_lens != NULL).  A template parameter rather than a runtime branch: the cursor state would otherwise raise the
-// padded path's spills (every NB is at the 96-register cap of one 544-thread CTA per SM).
+// RAG: ragged batch (TcP::x_lens != NULL).  A template parameter rather than a runtime branch: the cursor state would otherwise cost the
+// padded path registers (every NB is at or near the 96-register cap of one 544-thread CTA per SM).
 template <int NB, bool RAG>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = warp_uniform_id(), lane = tid & 31;
   const int R = p.R, SA = p.SA, SB = p.SB;
   const uint32_t a_plane = (uint32_t)TC_CHUNKS * R * 16;          // bytes of one hi (or lo) slab
   const uint32_t b_plane = (uint32_t)TC_CHUNKS * NB * 16;         // bytes of one hi (or lo) weight tile

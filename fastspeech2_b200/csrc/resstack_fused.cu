@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
   static_assert(SLAB == (uint32_t)R * C * 4, "an operand slab has exactly the size of the fp32 tile it is built from");
   static_assert(MT * (C / 2) * 256 * 4 == SLAB, "the residual stream has the size of a slab");
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = warp_uniform_id(), lane = tid & 31;
   unsigned char* smem0 = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms are 1024 bytes
   unsigned char* xa = smem0 + RS_GUARD;          // 1024-byte aligned: doubles as the swizzled staging area of the result
   unsigned char* xt = xa + SLAB;                 //                    doubles as the landing area of the fp32 input boxes

@@ -40,12 +40,13 @@ class Generator(nn.Module):
         # waveform bar (tests/test_gpu_model.py::test_hifigan_real_checkpoint_vs_reference; CPU emulation: scripts/emul_split_precision.py).
         self.f8_mask = 0b11110
         # Stages (bit i) whose ResBlock group runs as ONE persistent kernel with every intermediate on chip (fs2_resstack, available for
-        # the 64- and 32-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).  Default: the 32-channel
-        # stage, the most memory-bound one; the 64-channel stage stays on the per-layer path unless fused_mask |= 0b0100.
-        self.fused_mask = 0b1000
+        # the 64- and 32-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).  Default: both (on an
+        # H100 SXM at 400 W, bench.py configs[2]: 127 ms per step against 133 ms with the 64-channel stage on per-layer launches and
+        # fused k = 3 pairs).
+        self.fused_mask = 0b1100
         # Stages (bit i) where every (dilated conv, conv, +x) pair with kernel size <= pair_kmax runs as ONE fs2_resstack launch, so
-        # that the intermediate never leaves the SM: worthwhile for the memory-bound k = 3 pairs of the 64-channel stage, while the
-        # longer kernels are tensor-bound and keep their per-layer launches -- hence pair_kmax = 3.
+        # that the intermediate never leaves the SM.  Only stages outside fused_mask use it: by default none, and with the 64-channel
+        # stage taken out of fused_mask its memory-bound k = 3 pairs.
         self.pair_mask = 0b0100
         self.pair_kmax = 3
         populate(self, hifigan_spec(self._hd, weight_norm=True))

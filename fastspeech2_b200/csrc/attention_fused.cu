@@ -14,14 +14,14 @@
 //
 // Ragged mode (template parameter RAG; the padded instantiation keeps its code): utterance b is computed exactly as a B = 1 call
 // with T = n_b = key_lens[b].  Only utterances with n_b >= AF_MIN_ROWS are taken (a B = 1 call with a shorter T runs the exact
-// kernel, which takes the others); their work items are the live query tiles, compacted per head by the RaggedWalk cursor of the
-// conv kernel, and each streams ceil(n_b / 128) key blocks in both passes.  The packer packs only those key blocks, with rows at
+// kernel, which takes the others); their work items are the live query tiles, compacted per head by the RaggedWalk cursor
+// (tc_pipeline.cuh), and each streams ceil(n_b / 128) key blocks in both passes.  The packer packs only those key blocks, with rows at
 // or beyond n_b as zero; Q rows at or beyond n_b load as zero (0 * a stale NaN would still be NaN in P V), and ctx rows there are
 // not written.
 //
 // Roles: warp 8 streams K / V stages (cp.async.bulk) in the order they are consumed; warps 0-7 are two consumer warpgroups that
 // own 64 query rows each: Q conversion, the MMAs, both softmax passes and the epilogue.
-#include "conv_tc_kernel.cuh"
+#include "tc_pipeline.cuh"
 
 namespace fs2 {
 
@@ -38,13 +38,9 @@ __device__ __forceinline__ void split8(const float (&f)[8], float scale, uint4& 
   uint32_t hw[4], lw[4];
 #pragma unroll
   for (int j = 0; j < 4; j++) {
-    const float a0 = fminf(fmaxf(f[2 * j] * scale, -65504.f), 65504.f);
+    const float a0 = fminf(fmaxf(f[2 * j] * scale, -65504.f), 65504.f);   // also maps NaN to -65504
     const float a1 = fminf(fmaxf(f[2 * j + 1] * scale, -65504.f), 65504.f);
-    const __half2 h2 = __floats2half2_rn(a0, a1);
-    const float2 hf = __half22float2(h2);
-    const __half2 l2 = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
-    hw[j] = *reinterpret_cast<const uint32_t*>(&h2);
-    lw[j] = *reinterpret_cast<const uint32_t*>(&l2);
+    hw[j] = split_f16x2(a0, a1, lw[j]);
   }
   hi = make_uint4(hw[0], hw[1], hw[2], hw[3]);
   lo = make_uint4(lw[0], lw[1], lw[2], lw[3]);
@@ -145,11 +141,7 @@ struct AfP {
 __device__ __forceinline__ void af_store16(unsigned char* kblk, int row, const float (&a)[16]) {
   uint32_t hw[8], lw[8];
 #pragma unroll
-  for (int j = 0; j < 8; j++) {
-    hw[j] = cvt_f16x2_sat(a[2 * j], a[2 * j + 1]);
-    const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw[j]));
-    lw[j] = cvt_f16x2_sat(a[2 * j] - hf.x, a[2 * j + 1] - hf.y);
-  }
+  for (int j = 0; j < 8; j++) hw[j] = split_f16x2(a[2 * j], a[2 * j + 1], lw[j]);
   unsigned char* p0 = kblk + (size_t)row * 16;
   *reinterpret_cast<uint4*>(p0) = make_uint4(hw[0], hw[1], hw[2], hw[3]);                 // hi, chunk 0
   *reinterpret_cast<uint4*>(p0 + 2048) = make_uint4(hw[4], hw[5], hw[6], hw[7]);          // hi, chunk 1
@@ -173,8 +165,8 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
   uint64_t* emptyB = fullB + AF_SB;              // [AF_SB]
 
   if (tid == 0) {
-    for (int i = 0; i < AF_SB; i++) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    ring_init(fullB, emptyB, AF_SB, 1, 8);
+    mbar_init_fence();
   }
   __syncthreads();
   const int nkb = p.Tk / 128;                    // key blocks (ragged: per item, ceil(n_b / 128))
@@ -188,12 +180,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     // ===================== K / V stage producer, in the order the consumers read them =====================
     if (lane == 0) {
       Ring rb;
-      auto push = [&](const unsigned char* src) {
-        mbar_wait(&emptyB[rb.idx], rb.phase ^ 1);
-        mbar_expect_tx(&fullB[rb.idx], AF_STAGE);
-        bulk_g2s(ring + (size_t)rb.idx * AF_STAGE, src, AF_STAGE, &fullB[rb.idx]);
-        rb.advance(AF_SB);
-      };
+      auto push = [&](const unsigned char* src) { ring_push(fullB, emptyB, rb, AF_SB, ring + (size_t)rb.idx * AF_STAGE, src, AF_STAGE); };
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
         int bh = item / p.qtiles, nkb_i = nkb;
         if (RAG) {
@@ -219,25 +206,19 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
   const uint64_t desc_c = wgmma_desc(0, 2048, 128);    // A and B alike: chunk stride 128 rows * 16 B, 8-row groups 128 B apart
   const uint32_t qa16 = (smem_u32(qa) >> 4) + 64 * g, pa16 = (smem_u32(pa) >> 4) + 64 * g;
   Ring rb;
-  // D (+)= A(planes a16, 8 K-blocks) x B(next 8 ring stages), three-MMA split; stages are released one MMA group late
-  auto gemm = [&](uint32_t a16, float (&d)[64]) {
+  // D (+)= A(planes a16, 8 K-blocks) x B(next 8 ring stages), three-MMA split.  acc0 = 0: the first MMA overwrites D.
+  auto gemm = [&](uint32_t a16, float (&d)[64], uint32_t acc0) {
     int pend = -1;
-    for (int kb = 0; kb < 8; kb++, rb.advance(AF_SB)) {
-      mbar_wait(&fullB[rb.idx], rb.phase);
-      wgmma_fence();
-      const uint64_t a_hi = desc_c | (uint64_t)((a16 + kb * (KBLK >> 4)) & 0x3fff), a_lo = a_hi + (4096 >> 4);
-      const uint64_t b_hi = desc_c | (uint64_t)(smem_u32(ring + (size_t)rb.idx * AF_STAGE) >> 4), b_lo = b_hi + (4096 >> 4);
-      Wgmma<128>::f16(d, a_lo, b_hi, kb == 0 ? 0u : 1u);
-      Wgmma<128>::f16(d, a_hi, b_hi, 1u);
-      Wgmma<128>::f16(d, a_hi, b_lo, 1u);
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (pend >= 0) tc_release(&emptyB[pend]);
-      pend = (int)rb.idx;
-    }
-    wgmma_wait<0>();
+    for (int kb = 0; kb < 8; kb++, rb.advance(AF_SB))
+      ring_step(fullB, emptyB, rb, pend, [&](uint32_t sb) {
+        const uint64_t a_hi = desc_c | (uint64_t)((a16 + kb * (KBLK >> 4)) & 0x3fff), a_lo = a_hi + (4096 >> 4);
+        const uint64_t b_hi = desc_c | (uint64_t)(smem_u32(ring + (size_t)sb * AF_STAGE) >> 4), b_lo = b_hi + (4096 >> 4);
+        Wgmma<128>::f16(d, a_lo, b_hi, kb == 0 ? acc0 : 1u);
+        Wgmma<128>::f16(d, a_hi, b_hi, 1u);
+        Wgmma<128>::f16(d, a_hi, b_lo, 1u);
+      });
+    ring_drain(emptyB, pend);
     wgmma_keep<128>(d);
-    tc_release(&emptyB[pend]);
   };
   const int qr = (tid & 127) >> 1, qhalf = tid & 1;    // Q conversion: row, 64-column half
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -276,7 +257,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     // ---- pass 1: row maxima of the masked, scaled scores (rows lane/4 and lane/4 + 8 of this warp's 16)
     float m[2] = {-INFINITY, -INFINITY};
     for (int j = 0; j < nkb_i; j++) {
-      gemm(qa16, sacc);
+      gemm(qa16, sacc, 0u);
 #pragma unroll
       for (int jj = 0; jj < 16; jj++)
 #pragma unroll
@@ -298,7 +279,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     float l[2] = {0.f, 0.f};
     const int prow = 64 * g + 16 * w + (lane >> 2);
     for (int j = 0; j < nkb_i; j++) {
-      gemm(qa16, sacc);
+      gemm(qa16, sacc, 0u);
 #pragma unroll
       for (int jj = 0; jj < 16; jj++) {
         const int k0 = 8 * jj + 2 * (lane & 3);          // key inside the block
@@ -311,9 +292,8 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
             e[q] = j * 128 + k0 + q < len ? exp2f(fmaf(sacc[4 * jj + 2 * h + q], c, -m[h])) : 0.f;
             l[h] += e[q];
           }
-          const uint32_t hw = cvt_f16x2_sat(e[0], e[1]);
-          const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw));
-          const uint32_t lw = cvt_f16x2_sat(e[0] - hf.x, e[1] - hf.y);
+          uint32_t lw;
+          const uint32_t hw = split_f16x2(e[0], e[1], lw);
           unsigned char* rowp = base + (size_t)(prow + 8 * h) * 16;
           *reinterpret_cast<uint32_t*>(rowp) = hw;
           *reinterpret_cast<uint32_t*>(rowp + 4096) = lw;
@@ -325,26 +305,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
 #pragma unroll
         for (int i = 0; i < 64; i++) oacc[i] = 0.f;
       }
-      {
-        // O += P V_j: the first K-block of the first key block overwrites (gemm's kb == 0), later key blocks accumulate
-        int pend = -1;
-        for (int kb = 0; kb < 8; kb++, rb.advance(AF_SB)) {
-          mbar_wait(&fullB[rb.idx], rb.phase);
-          wgmma_fence();
-          const uint64_t a_hi = desc_c | (uint64_t)((pa16 + kb * (KBLK >> 4)) & 0x3fff), a_lo = a_hi + (4096 >> 4);
-          const uint64_t b_hi = desc_c | (uint64_t)(smem_u32(ring + (size_t)rb.idx * AF_STAGE) >> 4), b_lo = b_hi + (4096 >> 4);
-          Wgmma<128>::f16(oacc, a_lo, b_hi, 1u);
-          Wgmma<128>::f16(oacc, a_hi, b_hi, 1u);
-          Wgmma<128>::f16(oacc, a_hi, b_lo, 1u);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (pend >= 0) tc_release(&emptyB[pend]);
-          pend = (int)rb.idx;
-        }
-        wgmma_wait<0>();
-        wgmma_keep<128>(oacc);
-        tc_release(&emptyB[pend]);
-      }
+      gemm(pa16, oacc, 1u);                            // O += P V_j (zeroed above for the first key block)
       af_wg_sync(g);                                   // the P planes are rewritten by the next key block
     }
     // ---- epilogue: O / l (V tiles carry x16), rows beyond the utterance are zero

@@ -25,10 +25,7 @@
 //               accumulators (or one FP16 + one E4M3 K = 32 MMA, TcP::f8), then the epilogue straight from the accumulator
 //               fragments: bias / activation / residual / alpha / accumulate / pad-row mask -> global stores.
 #pragma once
-#include <cuda_fp16.h>
-
-#include "common.cuh"
-#include "wgmma.cuh"
+#include "tc_pipeline.cuh"
 
 namespace fs2 {
 
@@ -43,7 +40,6 @@ constexpr int TC_CTHREADS = TC_CWG * 128;
 constexpr int TC_THREADS = TC_CTHREADS + 32 + TC_TTHREADS;   // consumer warpgroups, producer warp, transform warps
 constexpr int TC_DEPTH = 2;         // K-blocks of activation loads in flight per transform thread (register ring)
 constexpr int TC_LD = 3;           // (row, K-chunk) items (2 float4 loads each) per transform thread per K-block: 256 * 3 / 2 >= 384 rows
-constexpr int TC_HDR = 128;        // bytes of header in front of the weight tiles: float[0] = 1 / weight scale
 
 struct TcP {
   const float* x; long long xbs, xrs;
@@ -75,69 +71,12 @@ struct TcP {
   int lens_scale;
 };
 
-// ------------------------------------------------------------------ PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // 8 consecutive floats (one 32-byte sector) as two 128-bit read-only loads
 __device__ __forceinline__ void ldg256(float (&d)[8], const float* src) {
   const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src) + 1);
   d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
 }
-// fp16x2 {lo = a0, hi = a1}, round-to-nearest, |x| > 65504 saturates instead of becoming inf: SASS F2FP.SATFINITE.F16.F32.PACK_AB
-__device__ __forceinline__ uint32_t cvt_f16x2_sat(float a0, float a1) {
-  uint32_t h;
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(a1), "f"(a0));
-  return h;
-}
 
-// e4m3x2 {byte 0 = a0, byte 1 = a1}, round-to-nearest, saturating at +-448
-__device__ __forceinline__ uint32_t cvt_e4m3x2_sat(float a0, float a1) {
-  unsigned short h;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h) : "f"(a1), "f"(a0));
-  return (uint32_t)h;
-}
-
-// Warp index of the calling thread, in a form ptxas knows to be warp-uniform.  threadIdx.x >> 5 is uniform only because the
-// block is one-dimensional, which ptxas cannot assume: a role branch on it counts as divergent, and every wgmma under such a
-// branch is then serialised (warning C7520: a warpgroup arrive and a full wait around each MMA, so commit groups and
-// wait_group<1> stop overlapping anything).  A shuffle from lane 0 is uniform by construction.
-__device__ __forceinline__ int warp_uniform_id() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
-
-// mbarrier ring cursor without runtime div/mod (an integer division per tap was on the MMA issuer's critical path)
-struct Ring {
-  uint32_t idx = 0, phase = 0;
-  __device__ __forceinline__ void advance(uint32_t n) {
-    if (++idx == n) { idx = 0; phase ^= 1u; }
-  }
-};
-
-struct Item { int nblk, b, t0; };
 __device__ __forceinline__ Item decode_item(const TcP& p, int item) {
   const int per_blk = p.B * p.tiles_per_batch;
   Item it;
@@ -148,40 +87,6 @@ __device__ __forceinline__ Item decode_item(const TcP& p, int item) {
   return it;
 }
 
-// Ragged batch (TcP::x_lens, RsP::lens): utterance b has n_b = ragged_rows(...) rows, and the work items of one channel block are the
-// live `tile`-row tiles of utterance 0, 1, ... back to back: sum_b ceil(n_b / tile) of them, so no tile lying wholly in the padding is
-// ever scheduled.
-// Monotone cursor over that compacted sequence.  Every role visits its items in increasing order (item = blockIdx.x, + gridDim.x, ...),
-// so the cursor only moves forward and each length is loaded once per channel block: no table, no cap on B, no host sync.
-// MIN_ROWS > 0: an utterance with fewer rows counts as empty (the fused attention kernel leaves those to the exact one).
-template <int MIN_ROWS>
-struct RaggedWalkT {
-  int live;                        // live tiles per channel block
-  int nblk, b, before, rows;       // cursor: channel block, utterance, live tiles of utterances < b in the block, n_b
-  __device__ __forceinline__ static int rows_of(const int* lens, int scale, int cap, int b) {
-    const int n = ragged_rows(lens, scale, cap, b);
-    if constexpr (MIN_ROWS > 0) return n < MIN_ROWS ? 0 : n;
-    return n;
-  }
-  __device__ __forceinline__ void init(const int* lens, int scale, int cap, int B, int tile) {
-    live = 0;
-    for (int i = 0; i < B; i++) live += (rows_of(lens, scale, cap, i) + tile - 1) / tile;
-    nblk = 0; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0);
-  }
-  __device__ __forceinline__ Item item(const int* lens, int scale, int cap, int tile, int i) {   // i < live * channel blocks
-    const int blk = i / live, rem = i - blk * live;
-    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0); }
-    for (int nt = (rows + tile - 1) / tile; rem >= before + nt; nt = (rows + tile - 1) / tile) {
-      before += nt;
-      rows = rows_of(lens, scale, cap, ++b);
-    }
-    Item it;
-    it.nblk = blk; it.b = b; it.t0 = (rem - before) * tile;
-    return it;
-  }
-};
-using RaggedWalk = RaggedWalkT<0>;
-
 template <int ACT>
 __device__ __forceinline__ float tc_act(float v, float slope) {
   if (ACT == FS2_ACT_RELU) return fmaxf(v, 0.f);
@@ -189,13 +94,6 @@ __device__ __forceinline__ float tc_act(float v, float slope) {
   if (ACT == FS2_ACT_LRELU) return v > 0.f ? v : v * slope;
   return v;
 }
-
-// Operand scales of the f16 + f8 split (TcP::f8): activation lo * 2^12 and hi (unscaled) are rounded to E4M3; the packer stores
-// weight hi * 2^-12 and lo (unscaled) in E4M3 (packing.pack_conv_tc), so both correction products carry the main term's scale.
-// |x| <= 448 stays inside E4M3; beyond that the correction of that element saturates (the result degrades towards single-pass
-// fp16 accuracy for it, never to garbage).
-constexpr float TC_F8_LO_SCALE = 4096.f;
-constexpr float TC_F8_HI_SCALE = 1.f;
 
 // One K-block of one transform thread: input activation, operand split, stores into the slab planes.
 //   F8 = false: plane 0 = fp16 hi, plane 1 = fp16 lo, both [16-byte K-chunk of 8 channels][row][8 halfs].
@@ -215,15 +113,13 @@ __device__ __forceinline__ void tc_convert_store(const float (&src)[LD][8], cons
         a0 = fmaxf(a0, a0 * in_slope);                 // leaky_relu for 0 <= slope <= 1
         a1 = fmaxf(a1, a1 * in_slope);
       }
-      hw[j] = cvt_f16x2_sat(a0, a1);
-      const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw[j]));
       if (F8) {
-        const uint32_t l8 = cvt_e4m3x2_sat((a0 - hf.x) * TC_F8_LO_SCALE, (a1 - hf.y) * TC_F8_LO_SCALE);   // a - hi is exact in fp32
-        const uint32_t h8 = cvt_e4m3x2_sat(hf.x, hf.y);                                                    // TC_F8_HI_SCALE == 1
+        uint32_t l8, h8;
+        hw[j] = split_f8x2(a0, a1, l8, h8);
         if (j & 1) { lw[j >> 1] |= l8 << 16; lw[2 + (j >> 1)] |= h8 << 16; }
         else { lw[j >> 1] = l8; lw[2 + (j >> 1)] = h8; }
       } else {
-        lw[j] = cvt_f16x2_sat(a0 - hf.x, a1 - hf.y);
+        hw[j] = split_f16x2(a0, a1, lw[j]);
       }
     }
     *reinterpret_cast<uint4*>(hi + offu[u]) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
@@ -279,12 +175,6 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
   }
 }
 
-// Releases a slab / weight stage once every consumer warp has seen its MMAs retire (one arrival per consumer warp).
-__device__ __forceinline__ void tc_release(uint64_t* bar) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
-}
-
 // RAG: ragged batch (TcP::x_lens != NULL).  A template parameter rather than a runtime branch: the cursor state would otherwise cost the
 // padded path registers (every NB is at or near the 96-register cap of one 544-thread CTA per SM).
 template <int NB, bool RAG>
@@ -313,9 +203,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   if (rag) { walk.init(p.x_lens, p.lens_scale, p.T, p.B, 128); n_items = walk.live * (p.N / p.NB); }
 
   if (tid == 0) {
-    for (int i = 0; i < TC_SA_MAX; i++) { mbar_init(&fullA[i], TC_TW); mbar_init(&emptyA[i], CWARPS); }
-    for (int i = 0; i < TC_SB_MAX; i++) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], CWARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    ring_init(fullA, emptyA, TC_SA_MAX, TC_TW, CWARPS);
+    ring_init(fullB, emptyB, TC_SB_MAX, 1, CWARPS);
+    mbar_init_fence();
   }
   __syncthreads();
 
@@ -332,13 +222,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
                                      (size_t)nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
           for (int kb = 0; kb < KBLOCKS; kb++) {
             for (int tap = 0; tap < p.taps; tap += p.TPS) {
-              const int n = min(p.TPS, p.taps - tap);
-              const uint32_t bytes = (uint32_t)n * stage_bytes;
-              mbar_wait(&emptyB[rb.idx], rb.phase ^ 1);
-              mbar_expect_tx(&fullB[rb.idx], bytes);
-              bulk_g2s(b_base + (size_t)rb.idx * p.TPS * stage_bytes, src, bytes, &fullB[rb.idx]);
+              const uint32_t bytes = (uint32_t)min(p.TPS, p.taps - tap) * stage_bytes;
+              ring_push(fullB, emptyB, rb, SB, b_base + (size_t)rb.idx * p.TPS * stage_bytes, src, bytes);
               src += bytes;
-              rb.advance(SB);
             }
           }
         }
@@ -348,8 +234,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     }
   } else if (warp < CWARPS) {
     // ===================== consumer warpgroups: MMAs + epilogue =====================
-    // Every operand is a precomputed descriptor base plus a constant.  A stage is released one MMA group late (wgmma.wait_group 1),
-    // so the tensor core always has the next stage's MMAs queued while the previous ones retire.
+    // Every operand is a precomputed descriptor base plus a constant.
     const int g = warp >> 2;                             // 64-row half of the tile
     const uint64_t a_const = wgmma_desc(0, (uint32_t)R * 16, 128), b_const = wgmma_desc(0, (uint32_t)NB * 16, 128);
     const float inv_ws0 = __ldg(p.wt);                 // header: 1 / (power-of-two weight scale)
@@ -371,29 +256,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
           const uint64_t a_lo = a_hi + (a_plane >> 4);
           uint32_t row_off = 0;
           for (int tap = 0; tap < p.taps; tap += p.TPS, rb.advance(SB)) {
-            const uint32_t sb = rb.idx;
             const int n = min(p.TPS, p.taps - tap);
-            mbar_wait(&fullB[sb], rb.phase);
-            wgmma_fence();
-            uint64_t b_hi = b_const | (uint64_t)(smem_u32(b_base + (size_t)sb * p.TPS * 2 * b_plane) >> 4);
-            for (int j = 0; j < n; j++, b_hi += (2 * b_plane) >> 4, row_off += (uint32_t)p.dil) {
-              const uint64_t b_lo = b_hi + (b_plane >> 4);
-              const uint64_t ah0 = a_hi + row_off, al0 = a_lo + row_off;
-              const uint32_t first = (kb | tap | j) ? 1u : 0u;
-              if (TG == 2 && p.f8) {                         // (the host plans f8 work items with NB <= 64, i.e. TG == 2)
-                Wgmma<NB>::f16(acc[0], ah0, b_hi, first);                        // fp16: A_hi * B_hi
-                Wgmma<NB>::e4m3(acc[TG - 1], al0, b_lo, first);                  // E4M3, K = 32: [A_lo | A_hi] * [B_hi ; B_lo]
-              } else {
-                Wgmma<NB>::f16(acc[TG - 1], al0, b_hi, first);                   // A_lo * B_hi
-                Wgmma<NB>::f16(acc[0], ah0, b_hi, TG >= 2 ? first : 1u);         // A_hi * B_hi
-                Wgmma<NB>::f16(acc[TG - 1], ah0, b_lo, 1u);                      // A_hi * B_lo
+            ring_step(fullB, emptyB, rb, pend_b, [&](uint32_t sb) {
+              uint64_t b_hi = b_const | (uint64_t)(smem_u32(b_base + (size_t)sb * p.TPS * 2 * b_plane) >> 4);
+              for (int j = 0; j < n; j++, b_hi += (2 * b_plane) >> 4, row_off += (uint32_t)p.dil) {
+                const uint64_t b_lo = b_hi + (b_plane >> 4);
+                const uint64_t ah0 = a_hi + row_off, al0 = a_lo + row_off;
+                const uint32_t first = (kb | tap | j) ? 1u : 0u;
+                if (TG == 2 && p.f8) {                         // (the host plans f8 work items with NB <= 64, i.e. TG == 2)
+                  Wgmma<NB>::f16(acc[0], ah0, b_hi, first);                        // fp16: A_hi * B_hi
+                  Wgmma<NB>::e4m3(acc[TG - 1], al0, b_lo, first);                  // E4M3, K = 32: [A_lo | A_hi] * [B_hi ; B_lo]
+                } else {
+                  Wgmma<NB>::f16(acc[TG - 1], al0, b_hi, first);                   // A_lo * B_hi
+                  Wgmma<NB>::f16(acc[0], ah0, b_hi, TG >= 2 ? first : 1u);         // A_hi * B_hi
+                  Wgmma<NB>::f16(acc[TG - 1], ah0, b_lo, 1u);                      // A_hi * B_lo
+                }
               }
-            }
-            wgmma_commit();
-            wgmma_wait<1>();                           // the previous group has retired: its stages may be refilled
-            if (pend_b >= 0) tc_release(&emptyB[pend_b]);
-            if (pend_a >= 0) { tc_release(&emptyA[pend_a]); pend_a = -1; }
-            pend_b = (int)sb;
+            });
+            if (pend_a >= 0) { tc_release(&emptyA[pend_a]); pend_a = -1; }   // its last group retired in ring_step
           }
           pend_a = (int)sa;
         }
@@ -507,8 +387,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
             else tc_convert_store<false, false, LD>(v[d], rowu, offu, off8, hi, hi + a_plane, (uint32_t)R * 16, in_slope);
           }
           fence_proxy_async();                         // generic-proxy stores -> visible to the tensor core (async proxy)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&fullA[ra.idx]);   // one arrival per transform warp
+          tc_release(&fullA[ra.idx]);                  // one arrival per transform warp
           ra.advance(SA);
           if (seq + DEPTH < total) issue_loads(v[d]);
         }

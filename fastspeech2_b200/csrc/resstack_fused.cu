@@ -19,7 +19,7 @@
 //     same fragment order (each thread reads back only what it wrote).  Epilogue = accumulators -> bias / residual / lrelu ->
 //     operand split -> st.shared into the other slab; a named barrier over both warpgroups publishes it (the next conv's taps
 //     read the neighbours' rows).
-//   * weights stream through a cp.async.bulk ring exactly as in conv_tc_kernel.cuh (same tile images: the packer's f8 format).
+//   * weights stream through the cp.async.bulk stage ring of tc_pipeline.cuh (the same tile images as conv_tc_kernel.cuh: the packer's f8 format).
 //   * global I/O is TMA with tensor maps: the fp32 tile of x arrives as 3-D boxes [1][128 rows][32 channels] (128-byte swizzle;
 //     rows outside [0, N) are zero-filled by the hardware = the conv's zero padding, and there is no bleed between utterances)
 //     into XT while it is idle; the result leaves as boxes staged in XA with a TMA store (first kernel size) or TMA reduce-add
@@ -28,7 +28,7 @@
 // Roles: warps 0-7 two consumer warpgroups (conversion, MMAs, epilogues; thread 0 issues the tensor-map copies), warp 8 weight producer.
 #include <cuda.h>
 
-#include "conv_tc_kernel.cuh"
+#include "tc_pipeline.cuh"
 
 namespace fs2 {
 
@@ -81,10 +81,8 @@ __device__ __forceinline__ float rs_lrelu(float v) { return fmaxf(v, 0.1f * v); 
 // channels c, c+1 (c even) of slab row `row` -> the operand planes (fp16 hi; E4M3 [lo * 2^12 | hi]).  `a0`, `a1` already carry the
 // activation and the out-of-utterance zeroing.
 __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_bytes, int row, int c, float a0, float a1) {
-  const uint32_t hw = cvt_f16x2_sat(a0, a1);
-  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hw));
-  const uint32_t l8 = cvt_e4m3x2_sat((a0 - hf.x) * TC_F8_LO_SCALE, (a1 - hf.y) * TC_F8_LO_SCALE);
-  const uint32_t h8 = cvt_e4m3x2_sat(hf.x, hf.y);          // TC_F8_HI_SCALE == 1
+  uint32_t l8, h8;
+  const uint32_t hw = split_f8x2(a0, a1, l8, h8);
   const int cc = c & 15;
   unsigned char* kblk = slab + (size_t)(c >> 4) * 4 * chunk_bytes + (size_t)row * 16;
   *reinterpret_cast<uint32_t*>(kblk + (cc >> 3) * chunk_bytes + (cc & 7) * 2) = hw;
@@ -117,15 +115,15 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
 
   for (int i = tid; i < RS_GUARD / 16; i += RS_THREADS) reinterpret_cast<uint4*>(smem0)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
-    for (int i = 0; i < RS_SB_MAX; i++) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 8); }
+    ring_init(fullB, emptyB, RS_SB_MAX, 1, 8);
     mbar_init(xLoaded, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmx)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmy)) : "memory");
   }
   fence_proxy_async();
   __syncthreads();
-  // ragged batch: the producer and both consumer warpgroups walk the same compacted item sequence (RaggedWalk, conv_tc_kernel.cuh)
+  // ragged batch: the producer and both consumer warpgroups walk the same compacted item sequence (RaggedWalk, tc_pipeline.cuh)
   RaggedWalk walk{};
   int n_items = p.n_items;
   if (RAG) { walk.init(p.lens, p.lens_scale, p.N, p.B, p.TILE); n_items = walk.live; }
@@ -143,11 +141,8 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
               for (int kb = 0; kb < KB; kb++)
                 for (int tap = 0; tap < cv.taps; tap += p.TPS) {
                   const uint32_t bytes = (uint32_t)min(p.TPS, cv.taps - tap) * WSTAGE;
-                  mbar_wait(&emptyB[rb.idx], rb.phase ^ 1);
-                  mbar_expect_tx(&fullB[rb.idx], bytes);
-                  bulk_g2s(ring + (size_t)rb.idx * stage_bytes, src, bytes, &fullB[rb.idx]);
+                  ring_push(fullB, emptyB, rb, (uint32_t)p.SB, ring + (size_t)rb.idx * stage_bytes, src, bytes);
                   src += bytes;
-                  rb.advance((uint32_t)p.SB);
                 }
             }
     }
@@ -209,36 +204,31 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
           const RsConv cv = p.conv[j][d][c2];
           const uint32_t slab16 = c2 == 0 ? xa16 : xt16;
           const int pad = (cv.taps - 1) * cv.dil / 2;
-          // ---- MMAs: every tap of every K-block for this warpgroup's MT 64-row blocks; a weight stage is released one group late
+          // ---- MMAs: every tap of every K-block for this warpgroup's MT 64-row blocks
           int pend = -1;
           for (int kb = 0; kb < KB; kb++) {
             const uint64_t a_hi = a_const | (uint64_t)((slab16 + kb * (KBLK >> 4) + 64 * MT * g) & 0x3fff);
             int row_off = -pad;
             for (int tap = 0; tap < cv.taps; tap += p.TPS, rb.advance((uint32_t)p.SB)) {
               const int n = min(p.TPS, cv.taps - tap);
-              mbar_wait(&fullB[rb.idx], rb.phase);
-              wgmma_fence();
-              uint64_t b_hi = b_const | (uint64_t)(smem_u32(ring + (size_t)rb.idx * stage_bytes) >> 4);
-              for (int t = 0; t < n; t++, b_hi += WSTAGE >> 4, row_off += cv.dil) {
-                const uint64_t b_x8 = b_hi + ((2u * C * 16u) >> 4);
-                const uint64_t ah0 = a_hi + (uint64_t)(int64_t)row_off;      // start-address field += rows (16 B each); never carries out of the field
-                const uint64_t ax0 = ah0 + (PLANE >> 4);
-                const uint32_t first = (kb | tap | t) ? 1u : 0u;
+              ring_step(fullB, emptyB, rb, pend, [&](uint32_t sb) {
+                uint64_t b_hi = b_const | (uint64_t)(smem_u32(ring + (size_t)sb * stage_bytes) >> 4);
+                for (int t = 0; t < n; t++, b_hi += WSTAGE >> 4, row_off += cv.dil) {
+                  const uint64_t b_x8 = b_hi + ((2u * C * 16u) >> 4);
+                  const uint64_t ah0 = a_hi + (uint64_t)(int64_t)row_off;      // start-address field += rows (16 B each); never carries out of the field
+                  const uint64_t ax0 = ah0 + (PLANE >> 4);
+                  const uint32_t first = (kb | tap | t) ? 1u : 0u;
 #pragma unroll
-                for (int i = 0; i < MT; i++) Wgmma<C>::f16(acc[i], ah0 + i * 64, b_hi, first);
+                  for (int i = 0; i < MT; i++) Wgmma<C>::f16(acc[i], ah0 + i * 64, b_hi, first);
 #pragma unroll
-                for (int i = 0; i < MT; i++) Wgmma<C>::e4m3(corr[i], ax0 + i * 64, b_x8, first);
-              }
-              wgmma_commit();
-              wgmma_wait<1>();
-              if (pend >= 0) tc_release(&emptyB[pend]);
-              pend = (int)rb.idx;
+                  for (int i = 0; i < MT; i++) Wgmma<C>::e4m3(corr[i], ax0 + i * 64, b_x8, first);
+                }
+              });
             }
           }
-          wgmma_wait<0>();
+          ring_drain(emptyB, pend);
 #pragma unroll
           for (int i = 0; i < MT; i++) { wgmma_keep<C>(acc[i]); wgmma_keep<C>(corr[i]); }
-          tc_release(&emptyB[pend]);
           // ---- epilogue straight from the fragments
           const float inv_s = __ldg(reinterpret_cast<const float*>(cv.w));
 #pragma unroll

@@ -1,0 +1,169 @@
+// Device code shared by the warp-specialised wgmma kernels of conv_tc_kernel.cuh, resstack_fused.cu and attention_fused.cu.
+#pragma once
+#include <cuda_fp16.h>
+
+#include "common.cuh"
+#include "wgmma.cuh"
+
+namespace fs2 {
+
+constexpr int TC_HDR = 128;        // bytes of header in front of the weight tiles: float[0] = 1 / weight scale
+
+// Operand scales of the f16 + f8 split (TcP::f8): activation lo * 2^12 and hi (unscaled) are rounded to E4M3; the packer stores
+// weight hi * 2^-12 and lo (unscaled) in E4M3 (packing.pack_conv_tc), so both correction products carry the main term's scale.
+// |x| <= 448 stays inside E4M3; beyond that the correction of that element saturates (the result degrades towards single-pass
+// fp16 accuracy for it, never to garbage).
+constexpr float TC_F8_LO_SCALE = 4096.f;
+constexpr float TC_F8_HI_SCALE = 1.f;
+
+// ------------------------------------------------------------------ PTX wrappers
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "WAIT_%=:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra DONE_%=;\n\t"
+      "bra WAIT_%=;\n\t"
+      "DONE_%=:\n\t}" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// fp16x2 {lo = a0, hi = a1}, round-to-nearest, |x| > 65504 saturates instead of becoming inf: SASS F2FP.SATFINITE.F16.F32.PACK_AB
+__device__ __forceinline__ uint32_t cvt_f16x2_sat(float a0, float a1) {
+  uint32_t h;
+  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(a1), "f"(a0));
+  return h;
+}
+
+// e4m3x2 {byte 0 = a0, byte 1 = a1}, round-to-nearest, saturating at +-448
+__device__ __forceinline__ uint32_t cvt_e4m3x2_sat(float a0, float a1) {
+  unsigned short h;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h) : "f"(a1), "f"(a0));
+  return (uint32_t)h;
+}
+
+// Operand split of {a0, a1}: returns hi = fp16(a) as fp16x2 and stores lo = fp16(a - hi) the same way (a - hi is exact in fp32).
+__device__ __forceinline__ uint32_t split_f16x2(float a0, float a1, uint32_t& lo) {
+  const uint32_t hi = cvt_f16x2_sat(a0, a1);
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  lo = cvt_f16x2_sat(a0 - hf.x, a1 - hf.y);
+  return hi;
+}
+
+// The f16 + f8 split: hi as above, and the E4M3 pairs lo8 = e4m3((a - hi) * TC_F8_LO_SCALE), hi8 = e4m3(hi * TC_F8_HI_SCALE).
+__device__ __forceinline__ uint32_t split_f8x2(float a0, float a1, uint32_t& lo8, uint32_t& hi8) {
+  static_assert(TC_F8_HI_SCALE == 1.f, "hi8 is hi rounded to E4M3 unscaled");
+  const uint32_t hi = cvt_f16x2_sat(a0, a1);
+  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  lo8 = cvt_e4m3x2_sat((a0 - hf.x) * TC_F8_LO_SCALE, (a1 - hf.y) * TC_F8_LO_SCALE);
+  hi8 = cvt_e4m3x2_sat(hf.x, hf.y);
+  return hi;
+}
+
+// Warp index of the calling thread, in a form ptxas knows to be warp-uniform.  threadIdx.x >> 5 is uniform only because the
+// block is one-dimensional, which ptxas cannot assume: a role branch on it counts as divergent, and every wgmma under such a
+// branch is then serialised (warning C7520: a warpgroup arrive and a full wait around each MMA, so commit groups and
+// wait_group<1> stop overlapping anything).  A shuffle from lane 0 is uniform by construction.
+__device__ __forceinline__ int warp_uniform_id() { return __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0); }
+
+// ------------------------------------------------------------------ stage ring
+// n shared-memory stages with a `full` and an `empty` mbarrier each; every role walks the same stage sequence with its own cursor.
+// mbarrier ring cursor without runtime div/mod (an integer division per tap was on the MMA issuer's critical path)
+struct Ring {
+  uint32_t idx = 0, phase = 0;
+  __device__ __forceinline__ void advance(uint32_t n) {
+    if (++idx == n) { idx = 0; phase ^= 1u; }
+  }
+};
+
+// One thread initialises the barrier pairs of an n-stage ring; mbar_init_fence() then orders every init before the barriers' use.
+__device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty, int n, int full_count, int empty_count) {
+  for (int i = 0; i < n; i++) { mbar_init(&full[i], full_count); mbar_init(&empty[i], empty_count); }
+}
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+
+// Producer: waits until the cursor's stage is free, then fills `bytes` of it at dst with one bulk copy from global src.
+__device__ __forceinline__ void ring_push(uint64_t* full, uint64_t* empty, Ring& r, uint32_t n, void* dst, const void* src, uint32_t bytes) {
+  mbar_wait(&empty[r.idx], r.phase ^ 1);
+  mbar_expect_tx(&full[r.idx], bytes);
+  bulk_g2s(dst, src, bytes, &full[r.idx]);
+  r.advance(n);
+}
+
+// One arrival per warp once all its lanes are done with a stage (a consumer's MMAs have retired, or a producer's stores are complete).
+__device__ __forceinline__ void tc_release(uint64_t* bar) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
+
+// Consumer warpgroup: waits for the cursor's stage, issues mmas(stage) as one wgmma group and releases the previous group's stage
+// once that has retired (so the next stage's MMAs are always queued).  pend: the last group's stage, -1 before the first step.  The
+// caller advances the cursor after the step, once it has also released what else the previous group read (the conv's slab).
+template <class Mmas>
+__device__ __forceinline__ void ring_step(uint64_t* full, uint64_t* empty, const Ring& r, int& pend, Mmas&& mmas) {
+  mbar_wait(&full[r.idx], r.phase);
+  wgmma_fence();
+  mmas(r.idx);
+  wgmma_commit();
+  wgmma_wait<1>();
+  if (pend >= 0) tc_release(&empty[pend]);
+  pend = (int)r.idx;
+}
+
+// After at least one ring_step: waits for every wgmma group and releases the last stage; then wgmma_keep the accumulators.
+__device__ __forceinline__ void ring_drain(uint64_t* empty, int pend) { wgmma_wait<0>(); tc_release(&empty[pend]); }
+
+struct Item { int nblk, b, t0; };
+
+// Ragged batch (TcP::x_lens, RsP::lens): utterance b has n_b = ragged_rows(...) rows, and the work items of one channel block are the
+// live `tile`-row tiles of utterance 0, 1, ... back to back: sum_b ceil(n_b / tile) of them, so no tile lying wholly in the padding is
+// ever scheduled.
+// Monotone cursor over that compacted sequence.  Every role visits its items in increasing order (item = blockIdx.x, + gridDim.x, ...),
+// so the cursor only moves forward and each length is loaded once per channel block: no table, no cap on B, no host sync.
+// MIN_ROWS > 0: an utterance with fewer rows counts as empty (the fused attention kernel leaves those to the exact one).
+template <int MIN_ROWS>
+struct RaggedWalkT {
+  int live;                        // live tiles per channel block
+  int nblk, b, before, rows;       // cursor: channel block, utterance, live tiles of utterances < b in the block, n_b
+  __device__ __forceinline__ static int rows_of(const int* lens, int scale, int cap, int b) {
+    const int n = ragged_rows(lens, scale, cap, b);
+    if constexpr (MIN_ROWS > 0) return n < MIN_ROWS ? 0 : n;
+    return n;
+  }
+  __device__ __forceinline__ void init(const int* lens, int scale, int cap, int B, int tile) {
+    live = 0;
+    for (int i = 0; i < B; i++) live += (rows_of(lens, scale, cap, i) + tile - 1) / tile;
+    nblk = 0; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0);
+  }
+  __device__ __forceinline__ Item item(const int* lens, int scale, int cap, int tile, int i) {   // i < live * channel blocks
+    const int blk = i / live, rem = i - blk * live;
+    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0); }
+    for (int nt = (rows + tile - 1) / tile; rem >= before + nt; nt = (rows + tile - 1) / tile) {
+      before += nt;
+      rows = rows_of(lens, scale, cap, ++b);
+    }
+    Item it;
+    it.nblk = blk; it.b = b; it.t0 = (rem - before) * tile;
+    return it;
+  }
+};
+using RaggedWalk = RaggedWalkT<0>;
+
+}  // namespace fs2

@@ -51,7 +51,7 @@ def split_fp16(w: Tensor):
     return hi, lo, s
 
 
-F8_W_HI_SCALE = 2.0 ** -12      # weight hi -> E4M3 (pairs with the kernel's activation-lo scale 2^12, conv_tc_kernel.cuh)
+F8_W_HI_SCALE = 2.0 ** -12      # weight hi -> E4M3 (pairs with the kernel's activation-lo scale 2^12, tc_pipeline.cuh)
 F8_W_LO_SCALE = 1.0             # weight lo -> E4M3 (pairs with the unscaled activation hi)
 
 

@@ -56,7 +56,7 @@ def conv1d_epilogue(acc, bias, out_act=ACT_NONE, out_slope=0.0, res=None, alpha=
 
 def f8_operands(x, w, in_act=ACT_NONE, in_slope=0.0):
     """The operands the f16 + f8 tensor-core kernel multiplies, evaluated exactly: returns (a_hi, w_hi, a_lo8, w_hi8, a_hi8, w_lo8, scale)
-    in fp64 so that  y*scale = a_hi.w_hi + a_lo8.w_hi8 + a_hi8.w_lo8  (conv_tc_kernel.cuh::tc_convert_store, packing.pack_conv_tc)."""
+    in fp64 so that  y*scale = a_hi.w_hi + a_lo8.w_hi8 + a_hi8.w_lo8  (tc_pipeline.cuh::split_f8x2, packing.pack_conv_tc)."""
     from fastspeech2_b200 import packing
     e4 = lambda t: t.float().clamp(-448, 448).to(torch.float8_e4m3fn).double()
     a = x.float()

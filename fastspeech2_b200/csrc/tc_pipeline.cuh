@@ -11,8 +11,8 @@ constexpr int TC_HDR = 128;        // bytes of header in front of the weight til
 
 // Operand scales of the f16 + f8 split (TcP::f8): activation lo * 2^12 and hi (unscaled) are rounded to E4M3; the packer stores
 // weight hi * 2^-12 and lo (unscaled) in E4M3 (packing.pack_conv_tc), so both correction products carry the main term's scale.
-// |x| <= 448 stays inside E4M3; beyond that the correction of that element saturates (the result degrades towards single-pass
-// fp16 accuracy for it, never to garbage).
+// lo * 2^12 stays inside E4M3 for |x| < 256 and hi for |x| <= 448; beyond that the correction of that element saturates (the result
+// degrades towards single-pass fp16 accuracy for it, never to garbage).
 constexpr float TC_F8_LO_SCALE = 4096.f;
 constexpr float TC_F8_HI_SCALE = 1.f;
 

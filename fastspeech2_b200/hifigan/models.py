@@ -100,6 +100,20 @@ class Generator(nn.Module):
         return out
 
     # ------------------------------------------------------------------ packing
+    def effective_masks(self):
+        """(f8_mask, fused_mask, pair_mask, pair_kmax) as the C ABI receives them (fs2_vocoder_model): fusion only for the 32- and
+        64-channel stages, pairs only outside the fused stages, and every fused or paired stage in the f16 + f8 format.  All zero
+        without tensor cores."""
+        if not self.use_tensor_cores:
+            return 0, 0, 0, 0
+        fused, ch = 0, self._hd["upsample_initial_channel"]
+        for i in range(self.num_upsamples):
+            ch //= 2
+            if (int(self.fused_mask) >> i) & 1 and ch in (32, 64):
+                fused |= 1 << i
+        pair = int(self.pair_mask) & ~fused
+        return int(self.f8_mask) | (fused << 1) | (pair << 1), fused, pair, int(self.pair_kmax)
+
     def _pack(self):
         L.lib()
         hd = self._hd
@@ -122,16 +136,8 @@ class Generator(nn.Module):
             if k != 2 * u or u % 2:
                 raise L.Fs2Error("ConvTranspose1d stage needs kernel = 2*stride and even stride on the sm_90a path")
             m.rates[i], m.up_k[i] = u, k
-        m.fused_mask = 0
-        if self.use_tensor_cores:
-            ch = m.c0
-            for i in range(m.n_stages):
-                ch //= 2
-                if (int(self.fused_mask) >> i) & 1 and ch in (32, 64):
-                    m.fused_mask |= 1 << i
-        m.pair_mask, m.pair_kmax = (int(self.pair_mask) & ~m.fused_mask, int(self.pair_kmax)) if self.use_tensor_cores else (0, 0)
-        m.f8_mask = (int(self.f8_mask) | (m.fused_mask << 1) | (m.pair_mask << 1)) if self.use_tensor_cores else 0
-        pk = packing.pack_vocoder(lambda b: self._folded(b).float(), lambda b: get(self, b + ".bias").detach().float(),
+        m.f8_mask, m.fused_mask, m.pair_mask, m.pair_kmax = self.effective_masks()
+        pk =packing.pack_vocoder(lambda b: self._folded(b).float(), lambda b: get(self, b + ".bias").detach().float(),
                                   hd["upsample_rates"], m.n_stages * m.n_kernels, m.n_dil, f8_mask=m.f8_mask)
         P = lambda k: pk[k].data_ptr()
         m.w_pre, m.b_pre, m.w_post, m.b_post = P("w_pre"), P("b_pre"), P("w_post"), P("b_post")

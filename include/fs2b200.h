@@ -52,7 +52,9 @@ enum { FS2_TC_ENCODER = 1, FS2_TC_PREDICTORS = 2, FS2_TC_DECODER = 4, FS2_TC_POS
  * [lo * 2^12 | hi]: y ~ a_hi.w_hi + (a_lo.w_hi + a_hi.w_lo) with the bracket at E4M3 precision (relative error ~2^-16 instead
  * of ~2^-22; half the tensor-core work of the three-MMA split).  The correction accumulates separately from the main term (Hopper
  * adds E4M3 products with reduced precision), so F8 tiles use NB = fs2_conv_tc_block_f8(N) <= 64 output channels per work item.
- * Activations beyond +-448 saturate in the correction. */
+ * The correction saturates from |a| = 256 on, not 448: there lo * 2^12 can leave E4M3's range (|lo| up to 2^-3 once the fp16 ulp of
+ * a is 2^-2), which costs up to 2^-14 relative (about 12 % of values in [256, 448)); from 448 on hi saturates too.  The shipped
+ * HiFi-GAN checkpoints stay below 24 on real mels (tests/test_tc_precision_cpu.py). */
 enum { FS2_TC_VARIANT_F8 = 1,
        /* w_tc is tiled for 64 output channels per work item (pack_conv_tc(w, nb=64)): the hi*hi term and the two cross terms then
         * accumulate in separate register accumulators.  Used by the K-segmented encoder / predictor path (see fs2_acoustic_model). */

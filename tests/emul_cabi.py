@@ -81,6 +81,217 @@ def conv1d_f8(x, w, bias, dilation=1, pad_left=0, in_act=ACT_NONE, in_slope=0.0,
     return conv1d_epilogue(pre / s, d(bias), out_act, out_slope, d(res), alpha, d(y_prev), row_lens)
 
 
+# ------------------------------------------------------------------ tensor-core operand formats, bit for bit, and their error bounds
+#
+# Both formats multiply rounded operands and accumulate in fp32; in fp64 the rounded products are exact, so the contract
+#     y_c = epilogue( sum_terms conv(A, W) )
+# is what the kernel computes up to its fp32 accumulation, and a list of (A, W) pairs describes every format:
+#   split3 (format 0):  (a_hi, w_hi/s) + (a_lo, w_hi/s) + (a_hi, w_lo/s)                     hi = fp16(v), lo = fp16(v - hi)
+#   f8     (format 1):  (a_hi, w_hi/s) + (e4(a_lo 2^12)/2^12, e4(w_hi 2^-12) 2^12/s) + (e4(a_hi), e4(w_lo)/s)   lo = v - hi exact
+# with a = in_act(x) in fp32, w scaled by the layer's power of two s (fp16 and E4M3 keep their subnormals; both converts saturate).
+# Two bars per output element (tc_errors): (a) |y - y_c| <= TC_ACC_C 2^-24 S and (b) |y - y64| <= TC_ACC_C 2^-24 S + R.  After the
+# operand rounding all that is left is the tensor core's fp32 accumulation: each 16-deep K-step sums its products (an error of a few
+# ulp of their absolute sum) and adds them to the accumulator with truncation (at most one ulp of the running sum).  So S = the
+# contract on absolute products, plus the accumulator mass: the sum over K-steps, in the kernel's order, of |running sum| (fp64, on
+# the contract's terms), plus the epilogue terms.  The mass follows how the accumulator actually grows: about n S / 2 for a sum of one
+# sign over n K-steps, about sqrt(n) S for random signs, so the bar stays tight on long random-signed sums without failing long
+# one-signed ones.  R = the format's stated precision (a_bounds / w_bounds) carried through the epilogue, against the unrounded y64.
+
+U24 = 2.0 ** -24
+# Largest normalised error measured over every tensor-core conv test (tests/test_gpu_tc_precision.py incl. the shipped checkpoints'
+# layers, tests/test_gpu_ops.py) on an H100 80GB HBM3 at a 700 W power limit: 5.1 (split3, weight outliers, several work items per
+# CTA; the shipped checkpoints' layers reach 4.4), so the bar leaves 3.2x.  Not more: tests/test_tc_precision_cpu.py checks that a
+# kernel without its correction terms, or without its activation lo plane, exceeds it by 10x on every shape these tests run, and the
+# longest shipped sums (HiFi-GAN stage-0 ResBlock convs, 176 K-steps) come within 1.02x of that.
+TC_ACC_C = 16.0
+# The same for the K-segmented path (16-step slices added into y in fp32 round-to-nearest): 1.04, measured likewise.
+TC_SEG_ACC_C = 4.0
+E4M3_MAX = 448.0
+
+
+def weight_scale(w):
+    """The per-layer power of two s of the tensor-core tiles: the largest 2^k with s max|w| <= 2^14 (1 for an all-zero or non-finite
+    w), derived here from frexp rather than from packing.split_fp16, so that the packer is checked against an independent definition."""
+    m = float(w.abs().max())
+    if m == 0.0 or not math.isfinite(m):
+        return 1.0
+    f, e = math.frexp(m)                      # m = f 2^e, f in [0.5, 1)
+    return 2.0 ** (14 - e + (1 if f == 0.5 else 0))
+
+
+def _f16(t):
+    """fp32 -> fp16 round-to-nearest, subnormals kept, saturating at +-65504 (cvt.rn.satfinite.f16x2.f32), as fp32."""
+    return t.clamp(-65504.0, 65504.0).half().float()
+
+
+def _e4(t):
+    """fp32 -> E4M3 round-to-nearest, subnormals kept, saturating at +-448 (cvt.rn.satfinite.e4m3x2.f32), as fp64."""
+    return t.float().clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).double()
+
+
+def _e4_err(v):
+    """Bound on |v - e4(v)| from the E4M3 definition: half an ulp of 3 mantissa bits (2^-4 |v|), half the subnormal spacing 2^-9,
+    or the saturation loss |v| - 448; never more than |v| itself below the saturation."""
+    v = v.double().abs()
+    return torch.maximum(torch.maximum(v * 2.0 ** -4, v.clamp_max(2.0 ** -10)), v - E4M3_MAX)
+
+
+def _split3_err(v):
+    """Bound on |v - (hi + lo)| of the fp16 hi / lo split: 2^-11 relative in lo, so 2^-22 |v|, and half of fp16's subnormal spacing
+    2^-24 where lo (or hi itself) is subnormal: the absolute floor 2^-25 that every |v| below about 2^-3 reaches.  Valid for |v| <= 65504."""
+    v = v.double().abs()
+    return torch.maximum(v * 2.0 ** -22, v.clamp_max(2.0 ** -25))
+
+
+def act_operand(x, in_act=ACT_NONE, in_slope=0.0):
+    """The fp32 activation the kernel splits: x read as fp32, leaky_relu as fmaxf(a, a * slope) (0 <= slope <= 1)."""
+    a = x.float()
+    if in_act == ACT_LRELU:
+        a = torch.maximum(a, a * in_slope)
+    elif in_act != ACT_NONE:
+        raise ValueError("the tensor-core kernel takes no other input activation")
+    return a
+
+
+def a_planes(a, fmt):
+    """Activation side of each term (same order as w_planes), fp64."""
+    ah = _f16(a)
+    if fmt == "split3":
+        return [ah.double(), _f16(a - ah).double(), ah.double()]
+    return [ah.double(), _e4((a - ah) * 4096.0) / 4096.0, _e4(ah)]
+
+
+def a_bounds(a, fmt):
+    """Activation side of each term of R (same order as w_bounds), fp64 and nonnegative."""
+    ah = _f16(a)
+    lo = (a - ah).double().abs()
+    if fmt == "split3":
+        e = _split3_err(a)
+        return [lo + e, a.double().abs() + e, e]
+    ea, eh = _e4_err((a - ah) * 4096.0) / 4096.0, _e4_err(ah)
+    return [ea, lo + ea, eh, ah.double().abs() + eh, lo]
+
+
+def _w_split(w, fmt):
+    s = weight_scale(w)
+    ws = w.float() * s
+    wh = ws.half().float()
+    return s, ws, wh
+
+
+def w_planes(w, fmt):
+    """Weight side of each term, with 1/s applied (exact: s is a power of two), fp64 [taps][Cin][N]."""
+    s, ws, wh = _w_split(w, fmt)
+    if fmt == "split3":
+        return [wh.double() / s, wh.double() / s, _f16(ws - wh).double() / s]
+    return [wh.double() / s, _e4(wh * 2.0 ** -12) * 4096.0 / s, _e4(ws - wh) / s]
+
+
+def w_bounds(w, fmt):
+    s, ws, wh = _w_split(w, fmt)
+    lo = (ws - wh).double().abs()
+    if fmt == "split3":
+        e = _split3_err(ws)
+        return [(lo + e) / s, e / s, ws.double().abs() / s]
+    return [wh.double().abs() / s, _e4_err(wh * 2.0 ** -12) * 4096.0 / s, lo / s, _e4_err(ws - wh) / s, lo / s]
+
+
+def _segmented(fn, w, seg_cin):
+    """fn applied to every (tap, seg_cin-channel) slice of w on its own (the K-segmented tiles: one scale per slice), reassembled."""
+    if seg_cin is None:
+        return fn(w)
+    taps, cin, _ = w.shape
+    parts = [[fn(w[t:t + 1, c:c + seg_cin]) for c in range(0, cin, seg_cin)] for t in range(taps)]
+    return [torch.cat([torch.cat([p[i] for p in row], dim=1) for row in parts], dim=0) for i in range(len(parts[0][0]))]
+
+
+def _pairs(x, w, fmt, in_act, in_slope, seg_cin):
+    a = act_operand(x, in_act, in_slope)
+    fn_w = (lambda v: w_planes(v, fmt)), (lambda v: w_bounds(v, fmt))
+    terms = list(zip(a_planes(a, fmt), _segmented(fn_w[0], w, seg_cin)))
+    bound = list(zip(a_bounds(a, fmt), _segmented(fn_w[1], w, seg_cin)))
+    return terms, bound
+
+
+def tc_contract(x, w, bias, fmt, dilation=1, pad_left=0, in_act=ACT_NONE, in_slope=0.0, out_act=ACT_NONE, out_slope=0.0, res=None,
+                alpha=1.0, y_prev=None, row_lens=None, seg_cin=None):
+    """fs2_conv1d on the tensor cores in format fmt ("split3" / "f8"), seg_cin = 256 for the K-segmented tiles.  Returns fp64
+    (y_c, y64, S, R): the rounded-operand contract, the unrounded contract, and the scales of the two bars (see above)."""
+    terms, bound = _pairs(x, w, fmt, in_act, in_slope, seg_cin)
+    lin = lambda pairs: sum(conv1d(a_, w_, None, dilation, pad_left) for a_, w_ in pairs)
+    d = lambda t: None if t is None else t.double()
+    ab = lambda t: None if t is None else t.double().abs()
+    epi = lambda acc: conv1d_epilogue(acc, d(bias), out_act, out_slope, d(res), alpha, d(y_prev), row_lens)
+    a64 = act_operand(x, in_act, in_slope).double()
+    y64 = conv1d_epilogue(conv1d(a64, w.double(), None, dilation, pad_left), d(bias), out_act, out_slope, d(res), alpha, d(y_prev), row_lens)
+    mass = accumulator_mass(terms, dilation, pad_left, seg_cin)
+    S = conv1d_epilogue(lin([(a_.abs(), w_.abs()) for a_, w_ in terms]) + mass, ab(bias), ACT_NONE, 0.0, ab(res), abs(alpha), ab(y_prev),
+                        row_lens)
+    R = conv1d_epilogue(lin(bound), None, ACT_NONE, 0.0, None, abs(alpha), None, row_lens)
+    return epi(lin(terms)), y64, S, R
+
+
+def tc_bound(x, w, fmt, dilation=1, pad_left=0, in_act=ACT_NONE, in_slope=0.0):
+    """R of tc_contract before the epilogue (alpha 1), without the other sums."""
+    _, bound = _pairs(x, w, fmt, in_act, in_slope, None)
+    return sum(conv1d(a_, w_, None, dilation, pad_left) for a_, w_ in bound)
+
+
+def accumulator_mass(terms, dilation=1, pad_left=0, seg_cin=None):
+    """Sum over the K-steps of |running sum| of the accumulator, per output element, in the order the conv kernel walks them (16-channel
+    K-block outer, tap inner; conv_tc_kernel.cuh).  K-segmented (seg_cin): every (tap, seg_cin-channel) slice has a fresh accumulator,
+    and each slice's fp32 add into y counts |y so far| once more."""
+    a0, w0 = terms[0]
+    B, T, cin = a0.shape
+    taps, _, N = w0.shape
+    mass = torch.zeros(B, T, N, dtype=torch.float64)
+    y = torch.zeros_like(mass)
+    step = lambda tap, c: sum(conv1d(a_[..., c:c + 16], w_[tap:tap + 1, c:c + 16], None, dilation, pad_left - tap * dilation)
+                              for a_, w_ in terms)
+    slices = [(range(taps), 0, cin)] if seg_cin is None else [([t], c, c + seg_cin) for t in range(taps) for c in range(0, cin, seg_cin)]
+    for tap_list, c0, c1 in slices:
+        acc = torch.zeros_like(mass)
+        for c in range(c0, c1, 16):
+            for tap in tap_list:
+                acc += step(tap, c)
+                mass += acc.abs()
+        if seg_cin is not None:
+            y += acc
+            mass += y.abs()
+    return mass
+
+
+def tc_errors(got, y_c, y64, S, R):
+    """The two normalised errors, max over elements: (a) |y - y_c| / (2^-24 S) and (b) max(0, |y - y64| - R) / (2^-24 S).  Where S = 0
+    (masked rows, all-zero products) the output must be exact.  Each must stay <= TC_ACC_C."""
+    def norm(d):
+        r = torch.where(S > 0, d / (U24 * S.clamp_min(1e-300)), torch.where(d > 0, float("inf"), 0.0))
+        return torch.nan_to_num(r, nan=float("inf")).max().item()
+    g = got.double()
+    return norm((g - y_c).abs()), norm(((g - y64).abs() - R).clamp_min(0.0))
+
+
+def unpack_conv_tc(buf, taps, cin, n, nb):
+    """Inverse of packing.pack_conv_tc for a [taps][Cin][N] weight tiled with NB output channels per work item: decodes the header
+    (1/s, format) and both planes, and returns the weight side of each term as w_planes does, from the bytes alone."""
+    buf = buf.cpu()
+    inv_s = float(buf[:4].view(torch.float32))
+    fmt = int(buf[4])
+    kb, nblk = cin // 16, n // nb
+    tiles = buf[128:].reshape(nblk, kb, taps, 2, 2 * nb * 16)
+
+    def f16_plane(p):       # [nblk][kb][tap][chunk][nn][8 halfs] -> [tap][kb * 16 + chunk * 8 + i][nblk * NB + nn]
+        h = tiles[:, :, :, p].contiguous().view(torch.float16).reshape(nblk, kb, taps, 2, nb, 8)
+        return h.permute(2, 1, 3, 5, 0, 4).reshape(taps, cin, n).double()
+
+    hi = f16_plane(0)
+    if fmt == 0:
+        return [hi * inv_s, hi * inv_s, f16_plane(1) * inv_s]
+    e = tiles[:, :, :, 1].contiguous().reshape(nblk, kb, taps, 2, nb, 16).view(torch.float8_e4m3fn).double()   # [.][h8 | l8][nn][16 ch]
+    e4 = lambda c: e[:, :, :, c].permute(2, 1, 4, 0, 3).reshape(taps, cin, n)
+    return [hi * inv_s, e4(0) * 4096.0 * inv_s, e4(1) * inv_s]
+
+
 def resblock_group(x, kernels, dils, w1, b1, w2, b2, conv=conv1d):
     """fs2_resstack as the per-layer calls of model.cu's unfused vocoder path:  r <- conv2(conv1(r, lrelu in / out) ) + r  per
     dilation, the last conv of each kernel size scaled by 1/n_kernels and accumulated into the sum.  w1 / w2 [j][d]: [k][C][C]."""
@@ -95,6 +306,33 @@ def resblock_group(x, kernels, dils, w1, b1, w2, b2, conv=conv1d):
                      y_prev=xs if last and j > 0 else None)
         xs = r
     return xs
+
+
+def resstack_contract(x, kernels, dils, w1, b1, w2, b2, alpha=None, y_prev=None):
+    """fs2_resstack (f16 + f8 operands, intermediates re-split on chip) in fp64 with the two bar scales of the group: S and R summed over
+    its layers, each layer's own (S of a conv = conv(|a|, |w|) + |b| on its exact input, R its format bound), plus |x| for the residual.
+    Carrying them through the later convs' |w| instead would multiply them by sum |w| (about 9 for the shipped layers) per conv, and
+    leave a bar that nothing could fail.  So S and R here are scales, not derived bounds: an early layer's error reaches the output
+    through the later convs with a gain this sum ignores.  Bars built on them are empirical (measured constants), and a failure is
+    not by itself proof of a kernel bug.  alpha = None: the mean over kernel sizes (the group); else y_prev + alpha * the one kernel
+    size.  Returns (y64, S, R) for tc_errors."""
+    def layer(v, w, b, dil, pad):
+        a = _act(v, ACT_LRELU, 0.1)
+        s = conv1d(a.abs(), w.double().abs(), b.double().abs(), dil, pad)
+        return conv1d(a, w.double(), b.double(), dil, pad), s, tc_bound(v, w, "f8", dil, pad, ACT_LRELU, 0.1)
+    y = S = R = 0.0
+    for j, k in enumerate(kernels):
+        r, rS, rR = x.double(), x.double().abs(), 0.0
+        for d, dv in enumerate(dils[j]):
+            t, tS, tR = layer(r, w1[j][d], b1[j][d], dv, (k - 1) * dv // 2)
+            u, uS, uR = layer(t, w2[j][d], b2[j][d], 1, (k - 1) // 2)
+            r, rS, rR = u + r, rS + tS + uS, rR + tR + uR
+        y, S, R = y + r, S + rS, R + rR
+    a = 1.0 / len(kernels) if alpha is None else alpha
+    y, S, R = a * y, abs(a) * S, abs(a) * R
+    if y_prev is not None:
+        y, S = y + y_prev.double(), S + y_prev.double().abs()
+    return y, S, R
 
 
 def layernorm(x, g, b, row_lens=None):

@@ -74,23 +74,23 @@ def test_vocoder_decomposition():
 
 def test_resblock_unfused_bar_rejects_a_single_pass_fp16_tile():
     """The GPU test of the fused ResBlock kernel (test_gpu_ops.test_resstack_fused) bounds its difference from the same group built from
-    per-layer tensor-core convs by RESSTACK_UNFUSED_BAR * max(1, |y|).  Evaluated in fp64 on the kernels' rounded operands, the group
-    with the E4M3 correction dropped (single-pass fp16) differs from the f16 + f8 contract in every 128-row block of every case by more
-    than 10x that bar, so a kernel that lost the correction in any one of its (longer) tiles fails that test; the unrounded fp64 bar
-    of the same test (3e-4 * max(1, |y|)) would not notice it."""
+    per-layer tensor-core convs by RESSTACK_UNFUSED_C 2^-24 S per element, S carried through the group (E.resstack_contract).  Evaluated
+    in fp64 on the kernels' rounded operands, the group with the E4M3 correction dropped (single-pass fp16) differs from the f16 + f8
+    contract in every 128-row block of every case by more than 10x that bar, so a kernel that lost the correction in any one of its
+    (longer) tiles fails that test."""
     import functools
     from tests import test_gpu_ops as G
+    from tests.test_gpu_tc_precision import RESSTACK_UNFUSED_C
     for case in G.RESSTACK_CASES:
         B, N, C, ks, ds = case
         x, w1, b1, w2, b2 = G._resstack_case(case)
         full = E.resblock_group(x, ks, ds, w1, b1, w2, b2, conv=E.conv1d_f8)
         fp16 = E.resblock_group(x, ks, ds, w1, b1, w2, b2, conv=functools.partial(E.conv1d_f8, fp16_only=True))
-        bar = G.RESSTACK_UNFUSED_BAR * max(1.0, full.abs().max().item())
-        diff = (full - fp16).abs()
+        _, S, _ = E.resstack_contract(x, ks, ds, w1, b1, w2, b2)
+        diff = (full - fp16).abs() / (E.U24 * S)
         blocks = [diff[b, s:s + 128].max().item() for b in range(B) for s in range(0, N, 128) if min(N - s, 128) >= 32]
         if blocks:
-            assert min(blocks) > 10 * bar, (case, min(blocks), bar)
-        assert diff.max().item() < 3e-4 * max(1.0, full.abs().max().item())
+            assert min(blocks) > 10 * RESSTACK_UNFUSED_C, (case, min(blocks))
 
 
 def test_split_conv_transpose_matches_torch():

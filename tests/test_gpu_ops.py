@@ -203,6 +203,14 @@ def _sel(t, u):
     return None if t is None else t[u]
 
 
+def tc_bars(got, u, x, w, bias, fmt, dil, pad, in_act, in_slope, out_act, res, alpha, y0, lens, seg_cin=None):
+    """The two per-element bars of the tensor-core kernels (tests/emul_cabi.py::tc_errors) on the utterances u of a batched result:
+    (a) against the rounded-operand contract, (b) against the unrounded fp64 conv; each normalised error must stay <= E.TC_ACC_C."""
+    y_c, y64, S, R = E.tc_contract(x[u], w, bias, fmt, dil, pad, in_act, in_slope, out_act, 0.1, _sel(res, u), alpha, _sel(y0, u),
+                                   _sel(lens, u), seg_cin=seg_cin)
+    return E.tc_errors(got.cpu()[u], y_c, y64, S, R)
+
+
 def _tc_call(case, x, w, bias, res, y0, lens, w_tc, variant):
     """fs2_conv1d on the tensor cores (backend = 2) for the case's epilogue settings; x, res, y0 and lens are CPU tensors."""
     _, _, _, _, _, dil, pad, in_act, out_act, _, alpha, acc, _ = case
@@ -255,40 +263,30 @@ TC_CASES += TC_PERSISTENT_CASES
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv1d_tensor_core(case, parity_log):
-    """fs2_conv1d through the tensor-core kernel against an fp64 evaluation of the same contract.  Error budget: the split
-    keeps 22 bits; what remains is the tensor core's truncating fp32 accumulator (~0.5 ulp per K=16 step)."""
+    """fs2_conv1d through the three-MMA split (FS2 tile format 0) against its rounded-operand contract and against fp64 (tc_bars)."""
     dil, pad, in_act, out_act, alpha = case[5], case[6], case[7], case[8], case[10]
     x, w, bias, res, y0, lens = _conv_case(case)
-    u = _ref_utts(x.shape[0])
-    d = lambda t: None if t is None else t[u].double()
-    want = E.conv1d(x[u].double(), w.double(), bias.double(), dil, pad, in_act, 0.1, out_act, 0.1, d(res), alpha, d(y0), _sel(lens, u))
     wtc = packing.pack_conv_tc(w)
     assert wtc is not None
     got = _tc_call(case, x, w, bias, res, y0, lens, wtc, 0)
     torch.cuda.synchronize()
-    err = (got.cpu()[u].double() - want).abs().max().item()
-    parity_log("test_conv1d_tensor_core", case=str(case[:9]), err=err, bar=6e-5)
-    assert err < 6e-5, err
+    ea, eb = tc_bars(got, _ref_utts(x.shape[0]), x, w, bias, "split3", dil, pad, in_act, 0.1, out_act, res, alpha, y0, lens)
+    parity_log("test_conv1d_tensor_core", case=str(case[:9]), err_contract=ea, err_fp64=eb, bar=E.TC_ACC_C)
+    assert ea <= E.TC_ACC_C and eb <= E.TC_ACC_C, (ea, eb)
 
 
 @pytest.mark.parametrize("case", TC_CASES)
 def test_conv1d_tensor_core_f8_split(case, parity_log):
     """FS2_TC_VARIANT_F8 (fp16 main term + one E4M3 correction MMA): (a) the kernel computes exactly the rounded-operand products of
-    its contract (checked against an fp64 evaluation of those operands, so a wrong byte order / scale / K layout cannot hide),
-    (b) against the unrounded fp64 contract the error is at the 2^-16 level (budget for the parity bars: scripts/emul_split_precision.py)."""
+    its contract up to fp32 accumulation (so a wrong byte order / scale / K layout cannot hide), (b) against the unrounded fp64 conv it
+    is within R, the E4M3 terms' stated precision (tc_bars)."""
     dil, pad, in_act, out_act, alpha = case[5], case[6], case[7], case[8], case[10]
     x, w, bias, res, y0, lens = _conv_case(case)
-    u = _ref_utts(x.shape[0])
-    d = lambda t: None if t is None else t[u].double()
-    exact = E.conv1d(x[u].double(), w.double(), bias.double(), dil, pad, in_act, 0.1, out_act, 0.1, d(res), alpha, d(y0), _sel(lens, u))
-    want = E.conv1d_f8(x[u], w, bias, dil, pad, in_act, 0.1, out_act, 0.1, _sel(res, u), alpha, _sel(y0, u), _sel(lens, u))
     got = _tc_call(case, x, w, bias, res, y0, lens, packing.pack_conv_tc(w, f8=True), 1)
     torch.cuda.synchronize()
-    err_contract = (got.cpu()[u].double() - want).abs().max().item()
-    err_exact = (got.cpu()[u].double() - exact).abs().max().item()
-    parity_log("test_conv1d_tensor_core_f8_split", case=str(case[:9]), err=err_contract, bar=6e-5, err_exact=err_exact, bar_exact=1.5e-3)
-    assert err_contract < 6e-5, (err_contract, err_exact)      # same budget as the three-MMA split: only the accumulator's rounding
-    assert err_exact < 1.5e-3, (err_contract, err_exact)       # ~2^-16 relative on O(1..10) outputs (single-pass fp16: ~2e-2 here)
+    ea, eb = tc_bars(got, _ref_utts(x.shape[0]), x, w, bias, "f8", dil, pad, in_act, 0.1, out_act, res, alpha, y0, lens)
+    parity_log("test_conv1d_tensor_core_f8_split", case=str(case[:9]), err_contract=ea, err_fp64=eb, bar=E.TC_ACC_C)
+    assert ea <= E.TC_ACC_C and eb <= E.TC_ACC_C, (ea, eb)
 
 
 SEG_CASES = [
@@ -327,22 +325,16 @@ def _seg_case(case):
 @pytest.mark.parametrize("case", SEG_CASES)
 def test_conv1d_tensor_core_k_segmented(case, parity_log):
     """FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED: one launch whose work units are (tile, tap, 256-channel chunk) slices with fresh
-    16-step accumulators, summed in fp32 through y.  Against the fp64 contract the error must be at the fp32 kernel's level (the point
-    of the segmentation: a single 432-step accumulation leaves 5x more)."""
+    16-step accumulators, summed in fp32 through y, each slice scaled back with its own header.  tc_bars with the per-slice scales."""
     B, T, Cin, N, taps, pad, in_act = case[:7]
     x, w, bias, res, lens = _seg_case(case)
-    u = _ref_utts(B)
-    want = E.conv1d(x[u].double(), w.double(), bias.double(), 1, pad, in_act, 0.0, 0, 0.0, None if res is None else res[u].double(), 1.0,
-                    None, _sel(lens, u))
     wseg = packing.pack_conv_tc_segments(w)
     assert wseg is not None and wseg.numel() == taps * (Cin // 256) * (128 + 1024 * N)
     got = _seg_call(case, x, w, bias, res, lens, wseg)
-    exact = _seg_call(case, x, w, bias, res, lens, None, backend=1)
     torch.cuda.synchronize()
-    err = (got.cpu()[u].double() - want).abs().max().item()
-    err_fp32 = (exact.cpu()[u].double() - want).abs().max().item()
-    parity_log("test_conv1d_tensor_core_k_segmented", case=str(case[:7]), err=err, bar=min(4e-6, 4 * err_fp32 + 1e-6), err_fp32=err_fp32)
-    assert err < 4e-6 and err < 4 * err_fp32 + 1e-6, (err, err_fp32)
+    ea, eb = tc_bars(got, _ref_utts(B), x, w, bias, "split3", 1, pad, in_act, 0.0, 0, res, 1.0, None, lens, seg_cin=packing.SEG_CIN)
+    parity_log("test_conv1d_tensor_core_k_segmented", case=str(case[:7]), err_contract=ea, err_fp64=eb, bar=E.TC_SEG_ACC_C)
+    assert ea <= E.TC_SEG_ACC_C and eb <= E.TC_SEG_ACC_C, (ea, eb)
 
 
 @pytest.mark.parametrize("fmt,case", [("split3", c) for c in TC_PERSISTENT_CASES] + [("f8", c) for c in TC_PERSISTENT_CASES]
@@ -391,14 +383,8 @@ def test_conv1d_tensor_core_strided_views(f8):
     torch.cuda.synchronize()
     assert torch.equal(ys, ref)
     assert torch.equal(torch.cat([yb[:, :, :4], yb[:, :, 4 + N:]], dim=2), outside)
-    u = [0, 2]
-    if f8:
-        want = E.conv1d_f8(x[u], w, bias, 1, pad, 3, 0.1, 0, 0.0, res[u], 0.5, y0[u], lens[u])
-    else:
-        d = lambda t: t.double()
-        want = E.conv1d(d(x[u]), d(w), d(bias), 1, pad, 3, 0.1, 0, 0.0, d(res[u]), 0.5, d(y0[u]), lens[u])
-    err = (ys.cpu()[u].double() - want).abs().max().item()
-    assert err < 6e-5, err
+    ea, eb = tc_bars(ys, [0, 2], x, w, bias, "f8" if f8 else "split3", 1, pad, 3, 0.1, 0, res, 0.5, y0, lens)
+    assert ea <= E.TC_ACC_C and eb <= E.TC_ACC_C, (ea, eb)
 
 
 def test_conv1d_tensor_core_halo_limit():
@@ -436,12 +422,6 @@ RESSTACK_CASES = [
 ]
 RESSTACK_TILE = {32: 392, 64: 136}      # output rows per work item of the shipped group (tests/test_abi.py checks it against the plan)
 
-# fs2_resstack against the same ResBlock group evaluated by per-layer fs2_conv1d calls on the same f8 tiles (model.cu's unfused path):
-# both compute the same rounded-operand products and differ only in fp32 accumulation order, and through it in rare roundings of an
-# intermediate's operand split.  Bar relative to max(1, |y|): the largest difference measured over RESSTACK_CASES on an H100 80GB HBM3
-# (400 W power limit) was 1.1e-7, so the bar leaves 9x headroom.  A kernel that lost the E4M3 correction term in a tile would be off
-# by the single-pass fp16 error there, which tests/test_decomposition_cpu.py shows to be more than 10x this bar in every 128-row block.
-RESSTACK_UNFUSED_BAR = 1e-6
 
 
 def _resstack_case(case):
@@ -462,41 +442,13 @@ def _resstack_case(case):
 @pytest.mark.parametrize("case", RESSTACK_CASES)
 def test_resstack_fused(case, parity_log):
     """fs2_resstack (one persistent kernel for a whole multi-receptive-field ResBlock group, intermediates on chip, halo recompute)
-    (a) against an fp64 evaluation of hifigan/models.py:96-103,:154-160 with torch conv1d.  Error budget: the f16 + f8 operand split
-    (2^-16 relative per layer) through 6 layers per kernel size.  (b) against the same group built from per-layer tensor-core convs
-    on the same tiles, which leaves only accumulation order: RESSTACK_UNFUSED_BAR."""
-    import torch.nn.functional as F
+    (b) against an fp64 evaluation of hifigan/models.py:96-103,:154-160 within R, the f16 + f8 format's bound carried through the
+    group, and (a) against the same group built from per-layer tensor-core convs on the same tiles, which leaves only accumulation order;
+    both per element, scaled by S carried through the group (tests/test_gpu_tc_precision.py::resstack_check)."""
+    from tests.test_gpu_tc_precision import resstack_check
     B, N, C, kernels, dils = case
     x, w1, b1, w2, b2 = _resstack_case(case)
-    want = torch.zeros(B, C, N, dtype=torch.float64)
-    for j, k in enumerate(kernels):
-        r = x.double().transpose(1, 2)
-        for d, dv in enumerate(dils[j]):
-            wa, wb = w1[j][d].permute(2, 1, 0).double(), w2[j][d].permute(2, 1, 0).double()     # back to [out, in, k]
-            t = F.conv1d(F.leaky_relu(r, 0.1), wa, b1[j][d].double(), dilation=dv, padding=(k - 1) * dv // 2)
-            t = F.conv1d(F.leaky_relu(t, 0.1), wb, b2[j][d].double(), padding=(k - 1) // 2)
-            r = t + r
-        want += r
-    want = (want / len(kernels)).transpose(1, 2)
-    dv = lambda ws: [[t.to(DEV) for t in row] for row in ws]
-    tiles = lambda ws: [[packing.pack_conv_tc(t, f8=True).to(DEV) for t in row] for row in ws]
-    t1, t2 = tiles(w1), tiles(w2)
-    got = ops.resstack(x.to(DEV), kernels, dils, t1, dv(b1), t2, dv(b2))
-
-    def conv(x_, wt, b_, dil, pad, in_act=0, in_slope=0.0, out_act=0, out_slope=0.0, res=None, alpha=1.0, y_prev=None):
-        return ops.conv1d(x_, wt[0], b_, dilation=dil, pad_left=pad, in_act=in_act, in_slope=in_slope, out_act=out_act, out_slope=out_slope,
-                          res=res, alpha=alpha, out=y_prev, accumulate=y_prev is not None, w_tc=wt[1], backend=2, tc_variant=1)
-    pair = lambda ws, ts: [list(zip(a, b)) for a, b in zip(dv(ws), ts)]
-    unfused = E.resblock_group(x.to(DEV), kernels, dils, pair(w1, t1), dv(b1), pair(w2, t2), dv(b2), conv=conv)
-    torch.cuda.synchronize()
-    assert torch.isfinite(got).all()
-    scale = max(1.0, want.abs().max().item())
-    err = (got.cpu().double() - want).abs().max().item()
-    err_unfused = (got - unfused).abs().max().item()
-    parity_log("test_resstack_fused", case=str(case), err=err, bar=3e-4 * scale, err_vs_unfused=err_unfused, bar_vs_unfused=RESSTACK_UNFUSED_BAR * scale,
-               err_unfused_vs_fp64=(unfused.cpu().double() - want).abs().max().item())
-    assert err < 3e-4 * scale, (err, scale)
-    assert err_unfused < RESSTACK_UNFUSED_BAR * scale, (err_unfused, scale)
+    resstack_check("test_resstack_fused", x, kernels, dils, w1, b1, w2, b2, parity_log, case=str(case))
 
 
 SINGLE_PAIR_CASES = [
@@ -596,15 +548,21 @@ def _conv_transpose_check(u, cin, cout, T, fmt, parity_log):
     ops.conv1d(xd, wb.to(DEV), bt[half * cout:].to(DEV), pad_left=0, in_act=3, in_slope=0.1, out=out[:, :, half * cout:], w_tc=tile(wb), **kw)
     torch.cuda.synchronize()
     err = (out.cpu().double().reshape(2, T * u, cout) - want).abs().max().item()
-    bar = {"fp32": 2e-5, "split3": 6e-5, "f8": 1.5e-3}[fmt]
-    vals = dict(err=err, bar=bar)
-    if fmt == "f8":
-        ya = E.conv1d_f8(x, wa, bt[: half * cout], 1, 1, 3, 0.1)
-        yb = E.conv1d_f8(x, wb, bt[half * cout:], 1, 0, 3, 0.1)
-        vals.update(err_contract=(out.cpu().double() - torch.cat([ya, yb], dim=2)).abs().max().item(), bar_contract=6e-5)
-    parity_log("test_conv1d_strided_output_conv_transpose", case=f"{fmt} u={u} {cin}->{cout} T={T}", **vals)
-    assert err < bar, vals
-    assert vals.get("err_contract", 0.0) < 6e-5, vals
+    if fmt == "fp32":
+        parity_log("test_conv1d_strided_output_conv_transpose", case=f"{fmt} u={u} {cin}->{cout} T={T}", err=err, bar=2e-5)
+        assert err < 2e-5, err
+        return
+    # the tensor-core phase groups: tc_bars on each group's columns, and the interleaved rows against torch's conv_transpose1d
+    both = [0, 1]
+    ea, eb = tc_bars(out[:, :, : half * cout], both, x, wa, bt[: half * cout], fmt, 1, 1, 3, 0.1, 0, None, 1.0, None, None)
+    ea2, eb2 = tc_bars(out[:, :, half * cout:], both, x, wb, bt[half * cout:], fmt, 1, 0, 3, 0.1, 0, None, 1.0, None, None)
+    ea, eb = max(ea, ea2), max(eb, eb2)
+    cat = torch.cat([E.conv1d(x.double(), wa.double(), bt[: half * cout].double(), 1, 1, 3, 0.1),
+                     E.conv1d(x.double(), wb.double(), bt[half * cout:].double(), 1, 0, 3, 0.1)], dim=2).reshape(2, T * u, cout)
+    assert (cat - want).abs().max().item() < 1e-12            # the phase split itself is exact
+    parity_log("test_conv1d_strided_output_conv_transpose", case=f"{fmt} u={u} {cin}->{cout} T={T}", err_contract=ea, err_fp64=eb,
+               bar=E.TC_ACC_C)
+    assert ea <= E.TC_ACC_C and eb <= E.TC_ACC_C, (ea, eb)
 
 
 def test_conv1d_strided_output_conv_transpose(parity_log):

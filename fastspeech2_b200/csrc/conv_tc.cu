@@ -27,10 +27,24 @@ bool conv_tc_supported(const fs2_conv1d_args* a) {
   return true;
 }
 
+// K-segmented evaluation in ONE launch (FS2_TC_VARIANT_SEGMENTED): the work units are (tile, tap, 256-channel chunk) slices, and the
+// plan is made for the shape of one slice (`slice`: Cin = 256, one tap).  Other variants: nseg = 1 and the plan is made for `a` itself.
+// Returns the arguments to plan on, or NULL if the segmented variant cannot take the shape.
+static const fs2_conv1d_args* conv_tc_segments(const fs2_conv1d_args* a, fs2_conv1d_args& slice, int& nseg, int& seg_nkc) {
+  nseg = seg_nkc = 1;
+  if (!(a->tc_variant & FS2_TC_VARIANT_SEGMENTED)) return a;
+  if (!(a->tc_variant & FS2_TC_VARIANT_NB64) || a->Cin % 256 || a->N % 64 || a->dilation != 1 || a->alpha != 1.f || a->out_act != FS2_ACT_NONE)
+    return nullptr;
+  seg_nkc = a->Cin / 256; nseg = a->taps * seg_nkc;
+  slice = *a;
+  slice.Cin = 256; slice.taps = 1;
+  return &slice;
+}
+
 // Shape-derived launch plan (pure host logic, no CUDA calls): work-item shape, accumulator grouping, ring depths, shared-memory
-// budget, grid.  Returns FS2_OK or FS2_ERR_UNSUPPORTED.  Exposed as fs2_conv_tc_plan so that the heuristics' invariants are
-// testable without a GPU (tests/test_abi.py).
-static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& smem, int& grid) {
+// budget, grid.  nseg: K-segments per tile (conv_tc_segments).  Returns FS2_OK or FS2_ERR_UNSUPPORTED.  Exposed as fs2_conv_tc_plan so
+// that the heuristics' invariants are testable without a GPU (tests/test_abi.py).
+static int conv_tc_plan(const fs2_conv1d_args* a, int nseg, int num_sms, TcP& p, size_t& smem, int& grid) {
   const bool nb64 = (a->tc_variant & FS2_TC_VARIANT_NB64) != 0;   // 64-channel work items: separate accumulators for hi*hi and the cross terms
   const bool f8 = (a->tc_variant & FS2_TC_VARIANT_F8) != 0;
   p.NB = nb64 ? (a->N % 64 == 0 ? 64 : (a->N < 64 && a->N % 16 == 0 ? a->N : 0)) : conv_tc_nb(a->N, f8 ? 64 : 128);
@@ -43,7 +57,8 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
   if (R > TC_LD * TC_TTHREADS / TC_CHUNKS + 7) return FS2_ERR_UNSUPPORTED;
   p.R = R;
   p.TG = p.NB <= 64 ? 2 : 1;
-  const size_t fixed = (2 * TC_SA_MAX + 2 * TC_SB_MAX) * 8 + 16;
+  // ring barriers, and the staged epilogue tiles of a conv with a residual, accumulate or K-segments (conv_tc_kernel.cuh)
+  const size_t fixed = TC_RING_BAR_BYTES + tc_stage_bytes(p.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));
   const size_t tap_bytes = (size_t)2 * TC_CHUNKS * p.NB * 16;
   int tps = a->taps >= 5 ? 4 : 1;                      // taps per weight stage: wide kernels share one bulk copy / handshake
   if (tps > a->taps) tps = a->taps;
@@ -62,6 +77,7 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
   while (fixed + sa * a_stage + sb * b_stage > budget && sb > 2) sb--;
   if (fixed + sa * a_stage + sb * b_stage > budget) return FS2_ERR_UNSUPPORTED;
   p.SA = sa; p.SB = sb;
+  p.stage_off = (int)(sa * a_stage + sb * b_stage + TC_RING_BAR_BYTES);   // [slab stages][weight stages][ring barriers][staged inputs]
   smem = fixed + sa * a_stage + sb * b_stage;
   p.tiles_per_batch = (a->T + 127) / 128;
   const long long n_items = (long long)(a->N / p.NB) * a->B * p.tiles_per_batch;
@@ -75,10 +91,14 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int num_sms, TcP& p, size_t& s
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out) {
   if (!a || !out || num_sms <= 0 || a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
+  fs2_conv1d_args slice;
+  int nseg, seg_nkc;
+  const fs2_conv1d_args* plan_args = conv_tc_segments(a, slice, nseg, seg_nkc);
+  if (!plan_args) return FS2_ERR_UNSUPPORTED;
   TcP p{};
   size_t smem = 0;
   int grid = 0;
-  const int rc = conv_tc_plan(a, num_sms, p, smem, grid);
+  const int rc = conv_tc_plan(plan_args, nseg, num_sms, p, smem, grid);
   if (rc != FS2_OK) return rc;
   const int v[11] = {p.NB, p.TG, p.SA, p.SB, p.TPS, p.R, p.TG * p.NB / 2, p.tiles_per_batch, p.n_items, grid, (int)smem};
   for (int i = 0; i < 11; i++) out[i] = v[i];
@@ -92,17 +112,10 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w_tc) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
   const unsigned variant = a->tc_variant;
-  // K-segmented evaluation in ONE launch (FS2_TC_VARIANT_SEGMENTED): the work units are (tile, tap, 256-channel chunk)
-  fs2_conv1d_args seg_args;
-  int nseg = 1, seg_nkc = 1;
-  if (variant & FS2_TC_VARIANT_SEGMENTED) {
-    if (!(variant & FS2_TC_VARIANT_NB64) || a->Cin % 256 || a->N % 64 || a->dilation != 1 || a->alpha != 1.f || a->out_act != FS2_ACT_NONE)
-      return FS2_ERR_UNSUPPORTED;
-    seg_nkc = a->Cin / 256; nseg = a->taps * seg_nkc;
-    seg_args = *a;
-    seg_args.Cin = 256; seg_args.taps = 1;          // shape of one slice: ring / tile planning happens on this
-  }
-  const fs2_conv1d_args* plan_args = nseg > 1 || (variant & FS2_TC_VARIANT_SEGMENTED) ? &seg_args : a;
+  fs2_conv1d_args slice;
+  int nseg, seg_nkc;
+  const fs2_conv1d_args* plan_args = conv_tc_segments(a, slice, nseg, seg_nkc);
+  if (!plan_args) return FS2_ERR_UNSUPPORTED;
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // state of the CURRENT device: the caller's stream must belong to it
   if (!dv) return derr;
@@ -129,7 +142,7 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
   p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;   // the plan below stays the padded one: the host never reads device lengths
   size_t smem = 0;
   int grid = 0;
-  const int rc = conv_tc_plan(plan_args, g_num_sms, p, smem, grid);
+  const int rc = conv_tc_plan(plan_args, nseg, g_num_sms, p, smem, grid);
   if (rc != FS2_OK) return rc;
   prof_before(s);
   switch (p.NB) {

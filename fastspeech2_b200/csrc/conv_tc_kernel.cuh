@@ -13,7 +13,7 @@
 // on both the synthetic and the shipped HiFi-GAN checkpoint; on the GPU the tensor core's truncating accumulator is what remains.
 //
 // Persistent, warp-specialised kernel: one CTA per SM walks a list of work items (one 128-row time tile of one utterance x one
-// block of NB <= 128 output channels); three roles overlap through mbarrier rings:
+// block of NB <= 128 output channels); four roles overlap through mbarrier rings:
 //   warp 8      weight producer: every (tap, 16-channel K-block) weight stage is ONE cp.async.bulk (TMA bulk engine) of a
 //               host-pre-split, host-pre-tiled smem image  [hi|lo][16-byte K-chunk][n][8 halfs].
 //   warps 9-16  activation transform: read the [128 + (taps-1)*dil] x 16-channel slab of a K-block ONCE from global
@@ -23,7 +23,13 @@
 //               the descriptor start address advanced by tap*dil rows: the slab is loaded and split once per K-block, not once per tap.
 //   warps 0-7   two consumer warpgroups, 64 output rows each: per weight stage 3 (split terms) wgmma m64nNBk16 with register
 //               accumulators (or one FP16 + one E4M3 K = 32 MMA, TcP::f8), then the epilogue straight from the accumulator
-//               fragments: bias / activation / residual / alpha / accumulate / pad-row mask -> global stores.
+//               fragments: bias / activation / residual / alpha / accumulate / pad-row mask -> global stores.  The residual and
+//               the y to accumulate into come from shared memory (below), so the epilogue reads only registers and shared memory.
+//   warp 17     staging (only for a conv with a residual, accumulate or K-segments): per work item and consumer warp, one
+//               cp.async.bulk per row of the residual and of the old y into that warp's 16 rows of a shared tile (TcStage), while
+//               the item's MMAs run.  Read from global in the epilogue, each of those loads sat behind the previous y store (y may
+//               alias both, so ptxas keeps them in order): one serial DRAM round trip per 8 columns with no MMA issuing.  A
+//               K-segmented conv keeps its running fp32 slice sum in the same tile instead of reading y back per slice.
 #pragma once
 #include "tc_pipeline.cuh"
 
@@ -37,7 +43,7 @@ constexpr int TC_TW = 8;            // transform warps
 constexpr int TC_TTHREADS = TC_TW * 32;
 constexpr int TC_CWG = 2;          // consumer warpgroups (64 output rows each)
 constexpr int TC_CTHREADS = TC_CWG * 128;
-constexpr int TC_THREADS = TC_CTHREADS + 32 + TC_TTHREADS;   // consumer warpgroups, producer warp, transform warps
+constexpr int TC_THREADS = TC_CTHREADS + 32 + TC_TTHREADS + 32;   // consumer warpgroups, producer warp, transform warps, staging warp
 constexpr int TC_DEPTH = 2;         // K-blocks of activation loads in flight per transform thread (register ring)
 constexpr int TC_LD = 3;           // (row, K-chunk) items (2 float4 loads each) per transform thread per K-block: 256 * 3 / 2 >= 384 rows
 
@@ -69,7 +75,18 @@ struct TcP {
   int f8;                          // operand split: 0 = three FP16 MMAs (hi*hi + lo*hi + hi*lo), 1 = FP16 main term + ONE E4M3 (K = 32) correction MMA
   const int* x_lens;               // ragged batch (fs2_conv1d_args::x_lens) or NULL; n_items / tiles_per_batch then only bound the grid
   int lens_scale;
+  int stage_off;                   // shared-memory byte offset of the staged epilogue inputs (used only if tc_stage_tiles(...) > 0)
 };
+
+// Shared-memory epilogue tiles behind the ring barriers: [full, empty mbarrier per consumer warp][residual tile if res][sum tile if
+// accumulate or nseg > 1],
+// each tile 128 rows x (NB + TC_STAGE_PAD) fp32.  The pad makes the row stride 8 or 24 banks (mod 32) for every NB, so the float2
+// reads of a half warp (4 rows x 32 bytes) fall in 32 distinct banks.  The host budgets exactly these bytes (conv_tc_plan).
+constexpr int TC_STAGE_PAD = 8;
+constexpr int TC_RING_BAR_BYTES = (2 * TC_SA_MAX + 2 * TC_SB_MAX) * 8 + 16;
+__host__ __device__ constexpr int tc_stage_tiles(bool res, bool accumulate, int nseg) { return (res ? 1 : 0) + (accumulate || nseg > 1 ? 1 : 0); }
+__host__ __device__ constexpr size_t tc_stage_tile_bytes(int NB) { return (size_t)128 * (NB + TC_STAGE_PAD) * 4; }
+__host__ __device__ constexpr size_t tc_stage_bytes(int NB, int tiles) { return tiles ? 2 * TC_CTHREADS / 32 * 8 + tiles * tc_stage_tile_bytes(NB) : 0; }
 
 // 8 consecutive floats (one 32-byte sector) as two 128-bit read-only loads
 __device__ __forceinline__ void ldg256(float (&d)[8], const float* src) {
@@ -132,45 +149,98 @@ __device__ __forceinline__ void tc_convert_store(const float (&src)[LD][8], cons
   }
 }
 
+// Staged-tile accesses through explicit 32-bit shared addresses (one register per row, immediate column offsets).  volatile: the
+// sum tile is read back by the same thread in the next K-segment, so these stay in program order.
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts_f2(uint32_t a, float2 v) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y) : "memory");
+}
+
+// The staged region (TcP::stage_off bytes into shared memory): per consumer warp a `full` and an `empty` mbarrier, then the tiles.
+// Addresses are recomputed from the kernel parameters where they are used: the consumer warps are at their register cap.
+template <int NB>
+struct TcStage {
+  static constexpr int CWARPS = TC_CTHREADS / 32;
+  static __device__ __forceinline__ uint64_t* full(const TcP& p, unsigned char* smem, int warp) {
+    return reinterpret_cast<uint64_t*>(smem + p.stage_off) + warp;
+  }
+  static __device__ __forceinline__ uint64_t* empty(const TcP& p, unsigned char* smem, int warp) { return full(p, smem, warp) + CWARPS; }
+  static __device__ __forceinline__ float* res_tile(const TcP& p, unsigned char* smem) {
+    return reinterpret_cast<float*>(smem + p.stage_off + 2 * CWARPS * 8);
+  }
+  static __device__ __forceinline__ float* sum_tile(const TcP& p, unsigned char* smem) {
+    return res_tile(p, smem) + (p.res ? tc_stage_tile_bytes(NB) / 4 : 0);
+  }
+  // Staging warp, work item `it`: for each consumer warp w, once w has released its rows of the previous item, bulk-copy the residual /
+  // old y rows of its 16 tile rows below tend (one copy per row and tile), completing on full[w].  `phase`: parity of this CTA's item.
+  static __device__ __forceinline__ void fill(const TcP& p, unsigned char* smem, const Item& it, int tend, uint32_t phase) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t row_bytes = NB * 4, per_row = (p.res ? row_bytes : 0u) + (p.accumulate ? row_bytes : 0u);
+    for (int w = 0; w < CWARPS; w++) {
+      const int row0 = 16 * w, rows = max(0, min(16, tend - (it.t0 + row0)));
+      mbar_wait(empty(p, smem, w), phase ^ 1u);
+      if (lane == 0) mbar_expect_tx(full(p, smem, w), (uint32_t)rows * per_row);
+      __syncwarp();
+      if (lane < rows) {
+        const long long t = it.t0 + row0 + lane;
+        const int srow = (row0 + lane) * (NB + TC_STAGE_PAD), n0 = it.nblk * NB;
+        if (p.res) bulk_g2s(res_tile(p, smem) + srow, p.res + it.b * p.rbs + t * p.rrs + n0, row_bytes, full(p, smem, w));
+        if (p.accumulate) bulk_g2s(sum_tile(p, smem) + srow, p.y + it.b * p.ybs + t * p.yrs + n0, row_bytes, full(p, smem, w));
+      }
+      __syncwarp();
+    }
+  }
+};
+
 // Epilogue of one consumer warpgroup: its 64 rows of the tile straight from the accumulator fragments (see wgmma.cuh): thread
 // (warp w, lane l) owns rows 16w + l/4 and +8, column pairs 8j + 2(l%4).  The split-term accumulators are summed here in fp32
-// round-to-nearest.  bias / res / row_lens may be NULL; acc_in: add alpha*value to y instead of overwriting it.  Rows >= tend (T, or n_b
-// of a ragged batch) are not written.
+// round-to-nearest.  bias / row_lens may be NULL.  The residual and the value to accumulate come from row t - t0 of the staged tiles
+// (TcStage): use_res adds the residual tile; sum_in adds alpha*value to the sum tile's value instead of overwriting it; the result goes to
+// y, or with sum_out to the sum tile (a K-segmented slice before the last).  Rows >= tend (T, or n_b of a ragged batch) are not written.
+// The tiles are addressed through 32-bit shared addresses derived from the kernel parameters (the kernel is at its 96-register cap).
 template <int ACT, int NB, int TG>
 __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 2], const Item& it, int row_base, int tend, const float* bias,
-                                            const float* res, const int* row_lens, int acc_in, float inv_ws) {
+                                            const int* row_lens, unsigned char* smem, bool use_res, bool sum_in, bool sum_out, float inv_ws) {
   const int lane = threadIdx.x & 31;
   const int n0 = it.nblk * NB + 2 * (lane & 3);
   const int len_b = row_lens ? min(row_lens[it.b], p.T) : p.T;
   const float slope = p.out_slope, alpha = p.alpha;
+  const float* brow = bias ? bias + n0 : nullptr;      // one base, immediate column offsets
 #pragma unroll
   for (int h = 0; h < 2; h++) {
     const int t = row_base + (lane >> 2) + 8 * h;
     if (t >= tend) continue;
     const bool live = t < len_b;
     float* yrow = p.y + (long long)it.b * p.ybs + (long long)t * p.yrs + n0;
-    const float* rrow = res ? res + (long long)it.b * p.rbs + (long long)t * p.rrs + n0 : nullptr;
+    // shared address of this thread's first column in the residual tile; the sum tile follows it when there is a residual
+    const uint32_t sres = smem_u32(TcStage<NB>::res_tile(p, smem)) + 4u * ((t - it.t0) * (NB + TC_STAGE_PAD) + 2 * (lane & 3));
+    const uint32_t ssum = sres + (p.res ? (uint32_t)tc_stage_tile_bytes(NB) : 0u);
 #pragma unroll
     for (int j = 0; j < NB / 8; j++) {
       float a0 = acc[0][4 * j + 2 * h], a1 = acc[0][4 * j + 2 * h + 1];
       if (TG == 2) { a0 += acc[TG - 1][4 * j + 2 * h]; a1 += acc[TG - 1][4 * j + 2 * h + 1]; }
       float2 bv = make_float2(0.f, 0.f);
-      if (bias) bv = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * j));
+      if (brow) bv = __ldg(reinterpret_cast<const float2*>(brow + 8 * j));
       float2 o;
       o.x = tc_act<ACT>(fmaf(a0, inv_ws, bv.x), slope);    // inv_ws is a power of two: exact
       o.y = tc_act<ACT>(fmaf(a1, inv_ws, bv.y), slope);
-      if (rrow) {
-        const float2 rv = *reinterpret_cast<const float2*>(rrow + 8 * j);
+      if (use_res) {
+        const float2 rv = lds_f2(sres + 32 * j);
         o.x += rv.x; o.y += rv.y;
       }
-      if (acc_in) {
-        const float2 yv = *reinterpret_cast<const float2*>(yrow + 8 * j);
+      if (sum_in) {
+        const float2 yv = lds_f2(ssum + 32 * j);
         o.x = o.x * alpha + yv.x; o.y = o.y * alpha + yv.y;
       } else {
         o.x *= alpha; o.y *= alpha;
       }
       if (!live) o = make_float2(0.f, 0.f);
-      *reinterpret_cast<float2*>(yrow + 8 * j) = o;
+      if (sum_out) sts_f2(ssum + 32 * j, o);
+      else *reinterpret_cast<float2*>(yrow + 8 * j) = o;
     }
   }
 }
@@ -192,6 +262,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   uint64_t* emptyA = fullA + TC_SA_MAX;    // [SA_MAX]
   uint64_t* fullB = emptyA + TC_SA_MAX;    // [SB_MAX]
   uint64_t* emptyB = fullB + TC_SB_MAX;    // [SB_MAX]
+  const bool staged = tc_stage_tiles(p.res != nullptr, p.accumulate != 0, p.nseg) > 0;   // the host budgeted tc_stage_bytes
+  using Stage = TcStage<NB>;
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
@@ -205,6 +277,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   if (tid == 0) {
     ring_init(fullA, emptyA, TC_SA_MAX, TC_TW, CWARPS);
     ring_init(fullB, emptyB, TC_SB_MAX, 1, CWARPS);
+    if (staged) ring_init(Stage::full(p, smem_raw, 0), Stage::empty(p, smem_raw, 0), CWARPS, 1, 1);
     mbar_init_fence();
   }
   __syncthreads();
@@ -282,23 +355,37 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
         for (int gg = 0; gg < TG; gg++) wgmma_keep<NB>(acc[gg]);
         if (pend_b >= 0) tc_release(&emptyB[pend_b]);
         if (pend_a >= 0) tc_release(&emptyA[pend_a]);
-        // K-segmented conv: unit (item, seg) adds slice seg of the tile into y -- bias with the first slice; residual, alpha-free sum
-        // and the pad-row mask with the last.  The same thread owns the same outputs in every unit, so the fp32 read-modify-write of
-        // y needs no further ordering.  No output activation (checked on the host).
+        // K-segmented conv: unit (item, seg) adds slice seg of the tile into the sum tile -- bias with the first slice; residual,
+        // alpha-free sum, the pad-row mask and the store to y with the last.  The same thread owns the same outputs in every unit, so the
+        // fp32 read-modify-write of the sum tile needs no further ordering.  No output activation (checked on the host).
         const bool first = seg == 0, last = seg == p.nseg - 1;
+        // the staging barrier completes one phase per work item of this CTA (phase parity from the item index: no register held)
+        if (staged && first) mbar_wait(Stage::full(p, smem_raw, warp), (uint32_t)((item - (int)blockIdx.x) / (int)gridDim.x) & 1u);
         const float* bias = first ? p.bias : nullptr;
-        const float* res = last ? p.res : nullptr;
         const int* lens = last ? p.row_lens : nullptr;
-        const int acc_in = (!first || p.accumulate) ? 1 : 0;
+        const bool use_res = last && p.res, sum_in = !first || p.accumulate, sum_out = !last;
         const float inv_ws = p.nseg == 1 ? inv_ws0
             : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes));
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
         switch (p.out_act) {                           // uniform branch: keeps tanhf out of the other variants' inner loops
-          case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
-          case FS2_ACT_TANH: tc_epilogue<FS2_ACT_TANH, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
-          case FS2_ACT_LRELU: tc_epilogue<FS2_ACT_LRELU, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
-          default: tc_epilogue<FS2_ACT_NONE, NB, TG>(p, acc, it, row_base, tend, bias, res, lens, acc_in, inv_ws); break;
+          case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          case FS2_ACT_TANH: tc_epilogue<FS2_ACT_TANH, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          case FS2_ACT_LRELU: tc_epilogue<FS2_ACT_LRELU, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          default: tc_epilogue<FS2_ACT_NONE, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
         }
+      }
+      if (staged) {                                    // this warp's rows are read: the staging warp may refill them
+        fence_proxy_async();                           // this lane's generic reads / writes of the rows -> before the bulk copies
+        tc_release(Stage::empty(p, smem_raw, warp));
+      }
+    }
+  } else if (warp == TC_THREADS / 32 - 1) {
+    // ===================== staging warp: residual / old-y rows of each work item -> shared memory (TcStage) =====================
+    if (staged) {
+      uint32_t phase = 0;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x, phase ^= 1u) {
+        const Item it = rag ? walk.item(p.x_lens, p.lens_scale, p.T, 128, item) : decode_item(p, item);
+        Stage::fill(p, smem_raw, it, rag ? walk.rows : p.T, phase);
       }
     }
   } else {

@@ -11,7 +11,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfs2b200.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 MAX_LAYERS, MAX_POSTNET, MAX_STAGES, MAX_RESBLOCKS, MAX_DIL = 12, 8, 8, 32, 4
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_LRELU = 0, 1, 2, 3
 CONV_AUTO, CONV_SIMT, CONV_TC = 0, 1, 2
@@ -152,6 +152,23 @@ class VocoderArgs(C.Structure):
                 ("wav", fp), ("workspace", fp), ("workspace_bytes", C.c_size_t), ("mel_lens", fp)]
 
 
+class ConvTcPlan(C.Structure):
+    _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")]
+
+
+class ConvSimtPlan(C.Structure):
+    _fields_ = [(n, i32) for n in ("BM", "BN", "grid_x", "grid_y")]
+
+
+class ResstackPlan(C.Structure):
+    _fields_ = [(n, i32) for n in ("MT", "H", "TILE", "n_items", "grid", "SB", "smem", "acc_regs", "OBOX", "n_oboxes", "TPS")]
+
+
+def fields(s):
+    """{field name: value} of a ctypes Structure (the launch plans)"""
+    return {n: getattr(s, n) for n, _ in s._fields_}
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "fs2_abi_version": (i32, []),
@@ -163,8 +180,10 @@ EXPORTS = {
     "fs2_conv1d": (i32, [C.POINTER(Conv1dArgs), fp]),
     "fs2_conv_tc_block": (i32, [i32]),
     "fs2_conv_tc_block_f8": (i32, [i32]),
-    "fs2_conv_tc_plan": (i32, [C.c_void_p, i32, C.c_void_p]),
-    "fs2_conv_simt_plan": (i32, [C.c_void_p, i32, C.c_void_p]),
+    # plan queries write a ConvTcPlan / ConvSimtPlan / ResstackPlan; the out pointer stays untyped so that a caller's int32 buffer of
+    # the plan's layout (the fields in order, as ABI 11 returned them) is still accepted
+    "fs2_conv_tc_plan": (i32, [C.POINTER(Conv1dArgs), i32, C.c_void_p]),
+    "fs2_conv_simt_plan": (i32, [C.POINTER(Conv1dArgs), i32, C.c_void_p]),
     "fs2_layernorm": (i32, [C.POINTER(LayerNormArgs), fp]),
     "fs2_attention": (i32, [C.POINTER(AttentionArgs), fp]),
     "fs2_attention_workspace_bytes": (C.c_size_t, [i32, i32, i32]),

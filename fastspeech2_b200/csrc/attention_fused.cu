@@ -4,7 +4,7 @@
 //
 //   pack_kv_tiles_kernel, once per layer: K and V of every (utterance, head) -> fp16 hi/lo operand tiles (three-MMA split: attention
 //   keeps fp32-class operands), one bulk-copy stage per 16 rows of the MMA's K dimension.
-//   work item = (utterance b, head h, 128 query rows).
+//   work item = (head h, utterance b, 128 query rows).
 //   pass 1: for every block of 128 keys  S = Q K_j^T (register accumulators)  ->  row maximum (a row's columns are spread over the
 //           four lanes of a quad: two shuffles).
 //   pass 2: S again -> p = exp2(s*c - m) (keys >= key_len masked to 0) -> fp16 hi/lo operand planes in shared memory ->
@@ -14,7 +14,7 @@
 //
 // Ragged mode (template parameter RAG; the padded instantiation keeps its code): utterance b is computed exactly as a B = 1 call
 // with T = n_b = key_lens[b].  Only utterances with n_b >= AF_MIN_ROWS are taken (a B = 1 call with a shorter T runs the exact
-// kernel, which takes the others); their work items are the live query tiles, compacted per head by the RaggedWalk cursor
+// kernel, which takes the others); their work items are the live query tiles, compacted per head by the WorkList cursor
 // (tc_pipeline.cuh), and each streams ceil(n_b / 128) key blocks in both passes.  The packer packs only those key blocks, with rows at
 // or beyond n_b as zero; Q rows at or beyond n_b load as zero (0 * a stale NaN would still be NaN in P V), and ctx rows there are
 // not written.
@@ -132,9 +132,9 @@ __global__ void pack_kv_tiles_kernel(const float* __restrict__ qkv, unsigned cha
 struct AfP {
   const float* qkv; float* ctx;
   const unsigned char* kt; const unsigned char* vt; long long tstride;     // per (b, h) tile buffers (128-byte header first)
-  int B, T, H, Tk;                               // Tk = T rounded up to 128
+  int B, T, H;
   const int* key_lens; float scale;
-  int n_items, qtiles;
+  int qtiles, n_items;                           // work items of the padded shape: per (utterance, head), in all
 };
 
 // 16 fp32 values of one row -> fp16 hi / lo operand planes of K-block kb ([2 chunks][128 rows][16 B] each)
@@ -169,24 +169,18 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     mbar_init_fence();
   }
   __syncthreads();
-  const int nkb = p.Tk / 128;                    // key blocks (ragged: per item, ceil(n_b / 128))
-  // Ragged: items are (head, utterance, live query tile), heads as the block dimension of the compacted sequence; every role walks
-  // it in the same order.
-  RaggedWalkT<AF_MIN_ROWS> walk{};
-  int n_items = p.n_items;
-  if (RAG) { walk.init(p.key_lens, 1, p.T, p.B, 128); n_items = walk.live * p.H; }
+  // Items are (head, utterance, query tile), heads as the block dimension; each streams the key blocks of its utterance's rows.
+  WorkList<RAG, AF_MIN_ROWS> work;
+  work.init(p.key_lens, 1, p.T, p.B, 128, p.qtiles, p.n_items);
 
   if (warp == 8) {
     // ===================== K / V stage producer, in the order the consumers read them =====================
     if (lane == 0) {
       Ring rb;
       auto push = [&](const unsigned char* src) { ring_push(fullB, emptyB, rb, AF_SB, ring + (size_t)rb.idx * AF_STAGE, src, AF_STAGE); };
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        int bh = item / p.qtiles, nkb_i = nkb;
-        if (RAG) {
-          const Item it = walk.item(p.key_lens, 1, p.T, 128, item);
-          bh = it.b * p.H + it.nblk; nkb_i = (walk.rows + 127) / 128;
-        }
+      for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+        const Item it = work.item(item);
+        const int bh = it.b * p.H + it.nblk, nkb_i = (it.rows + 127) / 128;
         const unsigned char* kt = p.kt + (long long)bh * p.tstride + TC_HDR;   // [key block][d/16][8 KB]
         const unsigned char* vt = p.vt + (long long)bh * p.tstride + TC_HDR;   // [key/16][8 KB]
         for (int j = 0; j < nkb_i; j++)                                          // pass 1
@@ -221,19 +215,13 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     wgmma_keep<128>(d);
   };
   const int qr = (tid & 127) >> 1, qhalf = tid & 1;    // Q conversion: row, 64-column half
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-    int bh = item / p.qtiles, qt = item - bh * p.qtiles;
-    int b = bh / p.H, hd = bh - b * p.H;
-    int len = p.key_lens ? min(p.key_lens[b], p.T) : p.T;
-    int nkb_i = nkb, rows = p.T;                   // rows that exist: the utterance's own in ragged mode
-    if (RAG) {
-      const Item it = walk.item(p.key_lens, 1, p.T, 128, item);
-      b = it.b; hd = it.nblk; qt = it.t0 / 128; bh = b * p.H + hd;
-      len = rows = walk.rows; nkb_i = (len + 127) / 128;
-    }
+  for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+    const Item it = work.item(item);
+    const int b = it.b, hd = it.nblk, rows = it.rows, nkb_i = (rows + 127) / 128;   // rows that exist: the utterance's own in ragged mode
+    const int len = p.key_lens ? min(p.key_lens[b], p.T) : p.T;                      // keys >= len are masked (ragged: len = rows)
     // ---- Q rows of this warpgroup -> operand planes (the previous item's MMAs have all retired)
     {
-      const int t = qt * 128 + 64 * g + qr;
+      const int t = it.t0 + 64 * g + qr;
       const float* src = p.qkv + ((long long)b * p.T + t) * 3 * D + hd * 128 + qhalf * 64;
 #pragma unroll
       for (int k = 0; k < 4; k++) {
@@ -313,7 +301,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
     for (int h = 0; h < 2; h++) {
       l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
       l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
-      const int t = qt * 128 + prow + 8 * h;
+      const int t = it.t0 + prow + 8 * h;
       if (t >= rows) continue;
       const float inv = t < len ? (1.f / AF_WSCALE) / l[h] : 0.f;
       float* dst = p.ctx + ((long long)b * p.T + t) * D + hd * 128 + 2 * (lane & 3);
@@ -364,8 +352,8 @@ int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cuda
   }
   AfP p{};
   p.qkv = a->qkv; p.ctx = a->ctx; p.kt = kt; p.vt = vt; p.tstride = tstride;
-  p.B = a->B; p.T = a->T; p.H = a->H; p.Tk = Tk; p.key_lens = a->key_lens; p.scale = a->scale;
-  p.qtiles = (a->T + 127) / 128;
+  p.B = a->B; p.T = a->T; p.H = a->H; p.key_lens = a->key_lens; p.scale = a->scale;
+  p.qtiles = Tk / 128;
   const long long items = (long long)a->B * a->H * p.qtiles;
   if (items > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   p.n_items = (int)items;

@@ -192,8 +192,8 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
 }
 
 // Tile choice of the launcher (pure host logic, no CUDA call; exposed as fs2_conv_simt_plan so that the GPU tests' coverage of the six
-// (BM, BN) instantiations is checkable without a GPU): out[4] = {BM, BN, grid.x, grid.y}.
-int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int* out) {
+// (BM, BN) instantiations is checkable without a GPU).
+int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out) {
   if (!a || !out || num_sms <= 0) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (a->Cin % BK != 0 || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
@@ -207,7 +207,7 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int* out) {
   // while the 128-column grid leaves SMs idle
   const bool narrow_small = small && a->N > 64 && gx * ((a->N + 127) / 128) < num_sms;
   const int bn = (a->N > 64 && !narrow_small) ? 128 : a->N > 32 ? 64 : 32;
-  out[0] = bm; out[1] = bn; out[2] = (int)gx; out[3] = (a->N + bn - 1) / bn;
+  out->BM = bm; out->BN = bn; out->grid_x = (int)gx; out->grid_y = (a->N + bn - 1) / bn;
   return FS2_OK;
 }
 
@@ -234,11 +234,11 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // SM count of the current device
   if (!dv) return derr;
-  int plan[4];
-  FS2_TRY(conv_simt_plan(a, dv->num_sms.load(std::memory_order_relaxed), plan));
-  const int bm = plan[0], bn = plan[1];
-  p.tiles_per_batch = plan[2] / a->B;
-  const dim3 grid((unsigned)plan[2], (unsigned)plan[3]);
+  fs2_conv_simt_plan_t plan;
+  FS2_TRY(conv_simt_plan(a, dv->num_sms.load(std::memory_order_relaxed), &plan));
+  const int bm = plan.BM, bn = plan.BN;
+  p.tiles_per_batch = plan.grid_x / a->B;
+  const dim3 grid((unsigned)plan.grid_x, (unsigned)plan.grid_y);
   prof_before(s);
 #define FS2_SIMT_ACT(BM_, BN_)                                                                            \
   switch (a->out_act) {                                                                                   \

@@ -44,7 +44,7 @@ static const fs2_conv1d_args* conv_tc_segments(const fs2_conv1d_args* a, fs2_con
 // Shape-derived launch plan (pure host logic, no CUDA calls): work-item shape, accumulator grouping, ring depths, shared-memory
 // budget, grid.  nseg: K-segments per tile (conv_tc_segments).  Returns FS2_OK or FS2_ERR_UNSUPPORTED.  Exposed as fs2_conv_tc_plan so
 // that the heuristics' invariants are testable without a GPU (tests/test_abi.py).
-static int conv_tc_plan(const fs2_conv1d_args* a, int nseg, int num_sms, TcP& p, size_t& smem, int& grid) {
+static int conv_tc_plan(const fs2_conv1d_args* a, int nseg, int num_sms, fs2_conv_tc_plan_t& p) {
   const bool nb64 = (a->tc_variant & FS2_TC_VARIANT_NB64) != 0;   // 64-channel work items: separate accumulators for hi*hi and the cross terms
   const bool f8 = (a->tc_variant & FS2_TC_VARIANT_F8) != 0;
   p.NB = nb64 ? (a->N % 64 == 0 ? 64 : (a->N < 64 && a->N % 16 == 0 ? a->N : 0)) : conv_tc_nb(a->N, f8 ? 64 : 128);
@@ -57,6 +57,7 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int nseg, int num_sms, TcP& p,
   if (R > TC_LD * TC_TTHREADS / TC_CHUNKS + 7) return FS2_ERR_UNSUPPORTED;
   p.R = R;
   p.TG = p.NB <= 64 ? 2 : 1;
+  p.acc_regs = p.TG * p.NB / 2;
   // ring barriers, and the staged epilogue tiles of a conv with a residual, accumulate or K-segments (conv_tc_kernel.cuh)
   const size_t fixed = TC_RING_BAR_BYTES + tc_stage_bytes(p.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));
   const size_t tap_bytes = (size_t)2 * TC_CHUNKS * p.NB * 16;
@@ -77,32 +78,26 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int nseg, int num_sms, TcP& p,
   while (fixed + sa * a_stage + sb * b_stage > budget && sb > 2) sb--;
   if (fixed + sa * a_stage + sb * b_stage > budget) return FS2_ERR_UNSUPPORTED;
   p.SA = sa; p.SB = sb;
-  p.stage_off = (int)(sa * a_stage + sb * b_stage + TC_RING_BAR_BYTES);   // [slab stages][weight stages][ring barriers][staged inputs]
-  smem = fixed + sa * a_stage + sb * b_stage;
+  p.smem = (int)(fixed + sa * a_stage + sb * b_stage);   // [slab stages][weight stages][ring barriers][staged inputs]
   p.tiles_per_batch = (a->T + 127) / 128;
   const long long n_items = (long long)(a->N / p.NB) * a->B * p.tiles_per_batch;
   if (n_items > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   p.n_items = (int)n_items;
-  grid = n_items < num_sms ? (int)n_items : num_sms;
+  p.grid = n_items < num_sms ? (int)n_items : num_sms;
   return FS2_OK;
 }
 
-// out[11] = {NB, TG, SA, SB, TPS, R, accumulator registers per consumer thread, tiles_per_batch, n_items, grid, dynamic smem bytes}
-int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out) {
+int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out) {
   if (!a || !out || num_sms <= 0 || a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
   fs2_conv1d_args slice;
   int nseg, seg_nkc;
   const fs2_conv1d_args* plan_args = conv_tc_segments(a, slice, nseg, seg_nkc);
   if (!plan_args) return FS2_ERR_UNSUPPORTED;
-  TcP p{};
-  size_t smem = 0;
-  int grid = 0;
-  const int rc = conv_tc_plan(plan_args, nseg, num_sms, p, smem, grid);
-  if (rc != FS2_OK) return rc;
-  const int v[11] = {p.NB, p.TG, p.SA, p.SB, p.TPS, p.R, p.TG * p.NB / 2, p.tiles_per_batch, p.n_items, grid, (int)smem};
-  for (int i = 0; i < 11; i++) out[i] = v[i];
-  return FS2_OK;
+  fs2_conv_tc_plan_t pl{};
+  const int rc = conv_tc_plan(plan_args, nseg, num_sms, pl);
+  if (rc == FS2_OK) *out = pl;
+  return rc;
 }
 
 // a->w_tc must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h) in the format a->tc_variant names
@@ -140,20 +135,22 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
   p.f8 = (variant & FS2_TC_VARIANT_F8) ? 1 : 0;
   p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;   // the plan below stays the padded one: the host never reads device lengths
-  size_t smem = 0;
-  int grid = 0;
-  const int rc = conv_tc_plan(plan_args, nseg, g_num_sms, p, smem, grid);
-  if (rc != FS2_OK) return rc;
+  fs2_conv_tc_plan_t pl{};
+  FS2_TRY(conv_tc_plan(plan_args, nseg, g_num_sms, pl));
+  p.SA = pl.SA; p.SB = pl.SB; p.TPS = pl.TPS; p.R = pl.R; p.tiles_per_batch = pl.tiles_per_batch; p.n_items = pl.n_items;
+  p.stage_off = pl.smem - (int)tc_stage_bytes(pl.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));   // the staged inputs end the budget
+  const unsigned grid = (unsigned)pl.grid;
+  const size_t smem = (size_t)pl.smem;
   prof_before(s);
-  switch (p.NB) {
-    case 16: conv_tc_launch_nb16(p, (unsigned)grid, smem, s); break;
-    case 32: conv_tc_launch_nb32(p, (unsigned)grid, smem, s); break;
-    case 48: conv_tc_launch_nb48(p, (unsigned)grid, smem, s); break;
-    case 64: conv_tc_launch_nb64(p, (unsigned)grid, smem, s); break;
-    case 80: conv_tc_launch_nb80(p, (unsigned)grid, smem, s); break;
-    case 96: conv_tc_launch_nb96(p, (unsigned)grid, smem, s); break;
-    case 112: conv_tc_launch_nb112(p, (unsigned)grid, smem, s); break;
-    default: conv_tc_launch_nb128(p, (unsigned)grid, smem, s); break;
+  switch (pl.NB) {
+    case 16: conv_tc_launch_nb16(p, grid, smem, s); break;
+    case 32: conv_tc_launch_nb32(p, grid, smem, s); break;
+    case 48: conv_tc_launch_nb48(p, grid, smem, s); break;
+    case 64: conv_tc_launch_nb64(p, grid, smem, s); break;
+    case 80: conv_tc_launch_nb80(p, grid, smem, s); break;
+    case 96: conv_tc_launch_nb96(p, grid, smem, s); break;
+    case 112: conv_tc_launch_nb112(p, grid, smem, s); break;
+    default: conv_tc_launch_nb128(p, grid, smem, s); break;
   }
   prof_after(s, 0, 2.0 * a->B * a->T * (double)a->Cin * a->taps * a->N);
   FS2_LAUNCH_CHECK();

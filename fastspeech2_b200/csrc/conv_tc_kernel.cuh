@@ -52,8 +52,7 @@ struct TcP {
   int B, T, Cin;
   const float* wt;                 // tiled weights, see packing.pack_conv_tc
   const float* bias;
-  int N;                           // total output channels
-  int NB;                          // output channels per work item (MMA N), N % NB == 0, NB % 16 == 0, NB <= 128
+  int N;                           // total output channels, a multiple of the kernel's NB
   int taps, dil, pad;
   int in_act; float in_slope;
   int out_act; float out_slope;
@@ -61,19 +60,17 @@ struct TcP {
   float alpha; int accumulate;
   const int* row_lens;
   float* y; long long ybs, yrs;
-  int TG;                          // accumulators per tile: 1 = all split terms together, 2 = {hi*hi | the two cross terms}
   int SA, SB;                      // ring depths
   int TPS;                         // conv taps per weight stage (small NB: several taps share one bulk copy / one handshake)
   int R;                           // slab rows held in smem (>= 128 + (taps-1)*dil, R % 8 == 4)
-  int tiles_per_batch;             // work items per utterance
-  int n_items;                     // total work items = (N/NB) * B * tiles_per_batch
-  int nseg;                        // K-segments per output tile (1 = plain conv).  > 1: the conv is the sum of nseg one-tap slices over p.Cin (= 256)
+  int tiles_per_batch, n_items;    // work items of the padded shape: per utterance ceil(T / 128), in all (N/NB) * B * tiles_per_batch
+  int nseg;                       // K-segments per output tile (1 = plain conv).  > 1: the conv is the sum of nseg one-tap slices over p.Cin (= 256)
                                    // input channels each, slice s = (tap = s / seg_nkc, channel chunk = s % seg_nkc); every slice is its own work unit with a
                                    // fresh accumulator, and the units of one tile run back to back on one CTA, adding into y in fp32 (FS2_TC_VARIANT_SEGMENTED)
   int seg_nkc;                     // channel chunks per tap
   long long seg_wbytes;            // bytes between the tile buffers of consecutive slices
   int f8;                          // operand split: 0 = three FP16 MMAs (hi*hi + lo*hi + hi*lo), 1 = FP16 main term + ONE E4M3 (K = 32) correction MMA
-  const int* x_lens;               // ragged batch (fs2_conv1d_args::x_lens) or NULL; n_items / tiles_per_batch then only bound the grid
+  const int* x_lens;               // ragged batch (fs2_conv1d_args::x_lens) or NULL
   int lens_scale;
   int stage_off;                   // shared-memory byte offset of the staged epilogue inputs (used only if tc_stage_tiles(...) > 0)
 };
@@ -92,16 +89,6 @@ __host__ __device__ constexpr size_t tc_stage_bytes(int NB, int tiles) { return 
 __device__ __forceinline__ void ldg256(float (&d)[8], const float* src) {
   const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src) + 1);
   d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
-}
-
-__device__ __forceinline__ Item decode_item(const TcP& p, int item) {
-  const int per_blk = p.B * p.tiles_per_batch;
-  Item it;
-  it.nblk = item / per_blk;
-  const int rem = item - it.nblk * per_blk;
-  it.b = rem / p.tiles_per_batch;
-  it.t0 = (rem - it.b * p.tiles_per_batch) * 128;
-  return it;
 }
 
 template <int ACT>
@@ -176,12 +163,12 @@ struct TcStage {
     return res_tile(p, smem) + (p.res ? tc_stage_tile_bytes(NB) / 4 : 0);
   }
   // Staging warp, work item `it`: for each consumer warp w, once w has released its rows of the previous item, bulk-copy the residual /
-  // old y rows of its 16 tile rows below tend (one copy per row and tile), completing on full[w].  `phase`: parity of this CTA's item.
-  static __device__ __forceinline__ void fill(const TcP& p, unsigned char* smem, const Item& it, int tend, uint32_t phase) {
+  // old y rows of its 16 tile rows below it.rows (one copy per row and tile), completing on full[w].  `phase`: parity of this CTA's item.
+  static __device__ __forceinline__ void fill(const TcP& p, unsigned char* smem, const Item& it, uint32_t phase) {
     const int lane = threadIdx.x & 31;
     const uint32_t row_bytes = NB * 4, per_row = (p.res ? row_bytes : 0u) + (p.accumulate ? row_bytes : 0u);
     for (int w = 0; w < CWARPS; w++) {
-      const int row0 = 16 * w, rows = max(0, min(16, tend - (it.t0 + row0)));
+      const int row0 = 16 * w, rows = max(0, min(16, it.rows - (it.t0 + row0)));
       mbar_wait(empty(p, smem, w), phase ^ 1u);
       if (lane == 0) mbar_expect_tx(full(p, smem, w), (uint32_t)rows * per_row);
       __syncwarp();
@@ -200,10 +187,10 @@ struct TcStage {
 // (warp w, lane l) owns rows 16w + l/4 and +8, column pairs 8j + 2(l%4).  The split-term accumulators are summed here in fp32
 // round-to-nearest.  bias / row_lens may be NULL.  The residual and the value to accumulate come from row t - t0 of the staged tiles
 // (TcStage): use_res adds the residual tile; sum_in adds alpha*value to the sum tile's value instead of overwriting it; the result goes to
-// y, or with sum_out to the sum tile (a K-segmented slice before the last).  Rows >= tend (T, or n_b of a ragged batch) are not written.
+// y, or with sum_out to the sum tile (a K-segmented slice before the last).  Rows >= it.rows (T, or n_b of a ragged batch) are not written.
 // The tiles are addressed through 32-bit shared addresses derived from the kernel parameters (the kernel is at its 96-register cap).
 template <int ACT, int NB, int TG>
-__device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 2], const Item& it, int row_base, int tend, const float* bias,
+__device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 2], const Item& it, int row_base, const float* bias,
                                             const int* row_lens, unsigned char* smem, bool use_res, bool sum_in, bool sum_out, float inv_ws) {
   const int lane = threadIdx.x & 31;
   const int n0 = it.nblk * NB + 2 * (lane & 3);
@@ -213,7 +200,7 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 #pragma unroll
   for (int h = 0; h < 2; h++) {
     const int t = row_base + (lane >> 2) + 8 * h;
-    if (t >= tend) continue;
+    if (t >= it.rows) continue;
     const bool live = t < len_b;
     float* yrow = p.y + (long long)it.b * p.ybs + (long long)t * p.yrs + n0;
     // shared address of this thread's first column in the residual tile; the sum tile follows it when there is a residual
@@ -245,8 +232,7 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
   }
 }
 
-// RAG: ragged batch (TcP::x_lens != NULL).  A template parameter rather than a runtime branch: the cursor state would otherwise cost the
-// padded path registers (every NB is at or near the 96-register cap of one 544-thread CTA per SM).
+// RAG: ragged batch (TcP::x_lens != NULL), see WorkList (every NB is at or near the 96-register cap of one 544-thread CTA per SM).
 template <int NB, bool RAG>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
@@ -267,12 +253,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
-  // Ragged batch: every role walks the compacted item sequence (RaggedWalk) in the same order, which keeps the rings' stage / phase
-  // sequence identical across the three roles.
-  constexpr bool rag = RAG;
-  RaggedWalk walk{};
-  int n_items = p.n_items;
-  if (rag) { walk.init(p.x_lens, p.lens_scale, p.T, p.B, 128); n_items = walk.live * (p.N / p.NB); }
+  WorkList<RAG> work;                                  // 128-row tiles x NB-channel blocks
+  work.init(p.x_lens, p.lens_scale, p.T, p.B, 128, p.tiles_per_batch, p.n_items);
 
   if (tid == 0) {
     ring_init(fullA, emptyA, TC_SA_MAX, TC_TW, CWARPS);
@@ -287,9 +269,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     if (lane == 0) {
       const uint32_t stage_bytes = 2 * b_plane;   // one tap of one K-block (hi + lo)
       Ring rb;
-      const int per_blk = rag ? max(walk.live, 1) : p.B * p.tiles_per_batch;
-      int nblk = (int)blockIdx.x / per_blk, rem = (int)blockIdx.x - nblk * per_blk;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+        const int nblk = work.item(item).nblk;
         for (int seg = 0; seg < p.nseg; seg++) {
           const unsigned char* src = reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes + TC_HDR +
                                      (size_t)nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
@@ -301,8 +282,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
             }
           }
         }
-        rem += (int)gridDim.x;
-        while (rem >= per_blk) { rem -= per_blk; nblk++; }
       }
     }
   } else if (warp < CWARPS) {
@@ -312,9 +291,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     const uint64_t a_const = wgmma_desc(0, (uint32_t)R * 16, 128), b_const = wgmma_desc(0, (uint32_t)NB * 16, 128);
     const float inv_ws0 = __ldg(p.wt);                 // header: 1 / (power-of-two weight scale)
     Ring ra, rb;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const Item it = rag ? walk.item(p.x_lens, p.lens_scale, p.T, 128, item) : decode_item(p, item);
-      const int tend = rag ? walk.rows : p.T;
+    for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+      const Item it = work.item(item);
       for (int seg = 0; seg < p.nseg; seg++) {
         float acc[TG][NB / 2];
 #pragma unroll
@@ -368,10 +346,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
             : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes));
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
         switch (p.out_act) {                           // uniform branch: keeps tanhf out of the other variants' inner loops
-          case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
-          case FS2_ACT_TANH: tc_epilogue<FS2_ACT_TANH, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
-          case FS2_ACT_LRELU: tc_epilogue<FS2_ACT_LRELU, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
-          default: tc_epilogue<FS2_ACT_NONE, NB, TG>(p, acc, it, row_base, tend, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          case FS2_ACT_TANH: tc_epilogue<FS2_ACT_TANH, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          case FS2_ACT_LRELU: tc_epilogue<FS2_ACT_LRELU, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
+          default: tc_epilogue<FS2_ACT_NONE, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
         }
       }
       if (staged) {                                    // this warp's rows are read: the staging warp may refill them
@@ -383,10 +361,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     // ===================== staging warp: residual / old-y rows of each work item -> shared memory (TcStage) =====================
     if (staged) {
       uint32_t phase = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x, phase ^= 1u) {
-        const Item it = rag ? walk.item(p.x_lens, p.lens_scale, p.T, 128, item) : decode_item(p, item);
-        Stage::fill(p, smem_raw, it, rag ? walk.rows : p.T, phase);
-      }
+      for (int item = blockIdx.x; item < work.count; item += gridDim.x, phase ^= 1u) Stage::fill(p, smem_raw, work.item(item), phase);
     }
   } else {
     // ===================== transform warps (activation + fp16 hi/lo split) =====================
@@ -419,9 +394,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     int l_tfirst = 0, l_tend = p.T;                    // l_tend: T, or n_b of a ragged batch
     bool l_interior = false;                           // warp-uniform: every slab row of the item exists
     auto l_set_item = [&]() {
-      if (l_item < n_items) {
-        const Item it = rag ? walk.item(p.x_lens, p.lens_scale, p.T, 128, l_item) : decode_item(p, l_item);
-        if (rag) l_tend = walk.rows;
+      if (l_item < work.count) {
+        const Item it = work.item(l_item);
+        l_tend = it.rows;
         const int s_tap = l_seg / p.seg_nkc, s_kc = l_seg - s_tap * p.seg_nkc;   // K-segment: one tap, one 256-channel chunk (0, 0 when nseg == 1)
         l_tfirst = it.t0 - p.pad + s_tap;
         l_xrow = p.x + (long long)it.b * p.xbs + (long long)l_tfirst * p.xrs + s_kc * p.Cin;
@@ -453,7 +428,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
         l_set_item();
       }
     };
-    const int my_items = (n_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // >= 0: blockIdx.x < gridDim.x
+    const int my_items = (work.count - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // >= 0: blockIdx.x < gridDim.x
     const int total = my_items * p.nseg * KBLOCKS;
 #pragma unroll
     for (int d = 0; d < DEPTH; d++)

@@ -63,13 +63,13 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 
 // kernels / launchers defined in the other translation units
 int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s);
-int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int* out);
+int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
 int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
 int conv_tc_nb(int N, int nb_max);
-int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, int* out);
+int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
 
 // backend dispatch of the fs2_conv1d contract
 static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s) {
@@ -89,7 +89,7 @@ int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s);
 int resstack(const fs2_resstack_args* a, cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
-int resstack_plan(const fs2_resstack_args* a, int num_sms, int* out);
+int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
 int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s);
 int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cudaStream_t s);
@@ -505,11 +505,11 @@ using namespace fs2;
 
 extern "C" {
 
-int fs2_abi_version(void) { return 11; }
+int fs2_abi_version(void) { return 12; }
 int fs2_conv_tc_block(int N) { return conv_tc_nb(N, 128); }
 int fs2_conv_tc_block_f8(int N) { return conv_tc_nb(N, 64); }
-int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_tc_plan_query(a, num_sms, out); }
-int fs2_conv_simt_plan(const fs2_conv1d_args* a, int num_sms, int32_t* out) { return conv_simt_plan(a, num_sms, out); }
+int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out) { return conv_tc_plan_query(a, num_sms, out); }
+int fs2_conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out) { return conv_simt_plan(a, num_sms, out); }
 int64_t fs2_kernel_launch_count(void) { return (int64_t)g_launch_count.load(); }
 size_t fs2_struct_size(int which) {
   switch (which) {
@@ -529,6 +529,9 @@ size_t fs2_struct_size(int which) {
     case 13: return sizeof(fs2_vocoder_args);
     case 14: return sizeof(fs2_resstack_args);
     case 15: return sizeof(fs2_wav_int16_args);
+    case 16: return sizeof(fs2_conv_tc_plan_t);
+    case 17: return sizeof(fs2_conv_simt_plan_t);
+    case 18: return sizeof(fs2_resstack_plan_t);
     default: return 0;
   }
 }
@@ -576,7 +579,7 @@ int fs2_length_regulate(const fs2_length_regulate_args* a, fs2_stream_t st) { re
 int fs2_conv_post(const fs2_conv_post_args* a, fs2_stream_t st) { return conv_post(a, S(st)); }
 int fs2_resstack(const fs2_resstack_args* a, fs2_stream_t st) { return resstack(a, S(st)); }
 int fs2_wav_to_int16(const fs2_wav_int16_args* a, fs2_stream_t st) { return wav_to_int16(a, S(st)); }
-int fs2_resstack_plan(const fs2_resstack_args* a, int num_sms, int32_t* out) { return out ? resstack_plan(a, num_sms, out) : FS2_ERR_ARG; }
+int fs2_resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t* out) { return out ? resstack_plan(a, num_sms, *out) : FS2_ERR_ARG; }
 int fs2_add_positions(float* x, const float* pos, int B, int T, int D, fs2_stream_t st) { return add_positions(x, pos, B, T, D, S(st)); }
 int fs2_transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, fs2_stream_t st) {
   return transpose_bct_to_btc(in, out, B, C, T, S(st));

@@ -42,13 +42,13 @@ struct RsP {
   int B, N;
   int n_kernels, n_dil;
   RsConv conv[RS_MAXK][FS2_MAX_DIL][2];
-  int H, TILE, tiles_per_b, n_items;
+  int H, TILE, tiles_per_b, n_items;   // work items of the padded shape: per utterance, in all
   float alpha;
   int SB;
   int OBOX, n_oboxes;            // rows per output box (TILE = n_oboxes * OBOX, OBOX % 8 == 0)
   int TPS;                       // conv taps per weight stage (one bulk copy / one handshake)
   int accumulate;                // the first kernel size reduce-adds into y too
-  const int* lens; int lens_scale;   // ragged batch (fs2_resstack_args::lens) or NULL; n_items then only bounds the grid
+  const int* lens; int lens_scale;   // ragged batch (fs2_resstack_args::lens) or NULL
 };
 
 // ------------------------------------------------------------------ TMA (tensor-map) wrappers
@@ -90,7 +90,7 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
   *reinterpret_cast<unsigned short*>(kblk + 3 * chunk_bytes + cc) = (unsigned short)h8;
 }
 
-// RAG: ragged batch (RsP::lens != NULL), a template parameter so that the padded path's code and register allocation stay as they are.
+// RAG: ragged batch (RsP::lens != NULL), see WorkList.
 template <int C, int MT, bool RAG>
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmy,
                                                                  const RsP p) {
@@ -123,16 +123,14 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
   }
   fence_proxy_async();
   __syncthreads();
-  // ragged batch: the producer and both consumer warpgroups walk the same compacted item sequence (RaggedWalk, tc_pipeline.cuh)
-  RaggedWalk walk{};
-  int n_items = p.n_items;
-  if (RAG) { walk.init(p.lens, p.lens_scale, p.N, p.B, p.TILE); n_items = walk.live; }
+  WorkList<RAG> work;                            // TILE-row tiles of each utterance
+  work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, p.tiles_per_b, p.n_items);
 
   if (warp == 8) {
     // ===================== weight producer: every conv's stages once per work item and kernel size =====================
     if (lane == 0) {
       Ring rb;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x)
+      for (int item = blockIdx.x; item < work.count; item += gridDim.x)
         for (int j = 0; j < p.n_kernels; j++)
           for (int d = 0; d < p.n_dil; d++)
             for (int c2 = 0; c2 < 2; c2++) {
@@ -161,15 +159,9 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
   Ring rb;
   uint32_t round_phase = 0;
   bool stores_pending = false;
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-    int b, t0, nrows = p.N;                         // nrows: rows of utterance b (n_b of a ragged batch); the convs pad at its end
-    if (RAG) {
-      const Item it = walk.item(p.lens, p.lens_scale, p.N, p.TILE, item);
-      b = it.b; t0 = it.t0; nrows = walk.rows;
-    } else {
-      b = item / p.tiles_per_b;
-      t0 = (item - b * p.tiles_per_b) * p.TILE;
-    }
+  for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+    const Item it = work.item(item);
+    const int b = it.b, t0 = it.t0, nrows = it.rows;   // nrows: rows of utterance b (n_b of a ragged batch); the convs pad at its end
     for (int j = 0; j < p.n_kernels; j++) {
       // ---- input: TMA boxes of x -> XT (idle: the last conv that read it has retired), then residual stream -> registers, lrelu(x) -> XA
       if (io) {
@@ -289,10 +281,8 @@ static size_t rs_smem_bytes(int C, int MT, int SB, int TPS) {
   return RS_GUARD + 3 * slab + (size_t)SB * TPS * 64 * C + (2 * RS_SB_MAX + 2) * 8 + 16 + 1024;   // + worst-case 1024-byte alignment slack
 }
 
-// Launch plan (pure host logic): out[12] = {MT, H (halo rows per side), TILE (output rows per work item), work items, grid, weight ring
-// stages, dynamic shared memory bytes, accumulator registers per consumer thread, rows per output box, output boxes per tile and
-// 32-channel block, taps per weight stage, independent-tile mode (0: every work item is one slab with a halo at its two ends)}
-int resstack_plan(const fs2_resstack_args* a, int num_sms, int* out) {
+// Launch plan (pure host logic, fs2_resstack_plan_t in fs2b200.h)
+int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out) {
   if (!a || a->B <= 0 || a->N <= 0 || num_sms <= 0) return FS2_ERR_ARG;
   if (a->C != 32 && a->C != 64) return FS2_ERR_UNSUPPORTED;
   if (a->n_kernels <= 0 || a->n_kernels > RS_MAXK || a->n_dil <= 0 || a->n_dil > FS2_MAX_DIL) return FS2_ERR_ARG;
@@ -328,9 +318,8 @@ int resstack_plan(const fs2_resstack_args* a, int num_sms, int* out) {
   int SB = 8;
   while (SB > 2 && rs_smem_bytes(a->C, MT, SB, TPS) > 227 * 1024) SB--;
   if (rs_smem_bytes(a->C, MT, SB, TPS) > 227 * 1024) return FS2_ERR_UNSUPPORTED;
-  out[0] = MT; out[1] = H; out[2] = TILE; out[3] = (int)items; out[4] = items < num_sms ? (int)items : num_sms; out[5] = SB;
-  out[6] = (int)rs_smem_bytes(a->C, MT, SB, TPS); out[7] = MT * a->C; out[8] = obox; out[9] = n_oboxes;
-  out[10] = TPS; out[11] = 0;
+  out.MT = MT; out.H = H; out.TILE = TILE; out.n_items = (int)items; out.grid = items < num_sms ? (int)items : num_sms; out.SB = SB;
+  out.smem = (int)rs_smem_bytes(a->C, MT, SB, TPS); out.acc_regs = MT * a->C; out.OBOX = obox; out.n_oboxes = n_oboxes; out.TPS = TPS;
   return FS2_OK;
 }
 
@@ -373,7 +362,7 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);
   if (!dv) return derr;
-  int plan[12];
+  fs2_resstack_plan_t plan;
   FS2_TRY(resstack_plan(a, dv->num_sms.load(std::memory_order_relaxed), plan));
   FS2_TRY(dev_once(dv->fused_ready, [] {
     const int mx = 227 * 1024;
@@ -395,19 +384,19 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
       p.conv[j][d][1] = RsConv{reinterpret_cast<const unsigned char*>(a->w2_tc[j][d]), a->b2[j][d], a->k[j], 1};
       flops += 2.0 * 2.0 * a->B * (double)a->N * a->C * a->C * a->k[j];
     }
-  p.H = plan[1]; p.TILE = plan[2]; p.tiles_per_b = (a->N + p.TILE - 1) / p.TILE; p.n_items = plan[3];
-  p.alpha = a->alpha > 0.f ? a->alpha : 1.f / (float)a->n_kernels; p.accumulate = a->accumulate; p.SB = plan[5]; p.OBOX = plan[8]; p.n_oboxes = plan[9]; p.TPS = plan[10];
+  p.H = plan.H; p.TILE = plan.TILE; p.tiles_per_b = plan.n_items / a->B; p.n_items = plan.n_items; p.SB = plan.SB; p.OBOX = plan.OBOX; p.n_oboxes = plan.n_oboxes; p.TPS = plan.TPS;
+  p.alpha = a->alpha > 0.f ? a->alpha : 1.f / (float)a->n_kernels; p.accumulate = a->accumulate;
   p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
   alignas(64) CUtensorMap tmx, tmy;
   FS2_TRY(make_map(&tmx, a->x, a->B, a->N, a->C, 128));
   FS2_TRY(make_map(&tmy, a->y, a->B, a->N, a->C, p.OBOX));
   prof_before(s);
   if (a->C == 32) {
-    if (a->lens) resstack_kernel<32, 4, true><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
-    else resstack_kernel<32, 4, false><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+    if (a->lens) resstack_kernel<32, 4, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_kernel<32, 4, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   } else {
-    if (a->lens) resstack_kernel<64, 2, true><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
-    else resstack_kernel<64, 2, false><<<plan[4], RS_THREADS, plan[6], s>>>(tmx, tmy, p);
+    if (a->lens) resstack_kernel<64, 2, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_kernel<64, 2, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   }
   prof_after(s, 0, flops);
   FS2_LAUNCH_CHECK();

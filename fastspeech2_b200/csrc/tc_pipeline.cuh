@@ -130,40 +130,72 @@ __device__ __forceinline__ void ring_step(uint64_t* full, uint64_t* empty, const
 // After at least one ring_step: waits for every wgmma group and releases the last stage; then wgmma_keep the accumulators.
 __device__ __forceinline__ void ring_drain(uint64_t* empty, int pend) { wgmma_wait<0>(); tc_release(&empty[pend]); }
 
-struct Item { int nblk, b, t0; };
+// ------------------------------------------------------------------ work list
+// One work item: block nblk (of output channels; of heads in attention), utterance b, first row t0 of its `tile` rows, and the rows
+// of utterance b that exist (the padded length cap, or n_b of a ragged batch): rows >= `rows` are padding.
+struct Item { int nblk, b, t0, rows; };
 
-// Ragged batch (TcP::x_lens, RsP::lens): utterance b has n_b = ragged_rows(...) rows, and the work items of one channel block are the
-// live `tile`-row tiles of utterance 0, 1, ... back to back: sum_b ceil(n_b / tile) of them, so no tile lying wholly in the padding is
-// ever scheduled.
-// Monotone cursor over that compacted sequence.  Every role visits its items in increasing order (item = blockIdx.x, + gridDim.x, ...),
-// so the cursor only moves forward and each length is loaded once per channel block: no table, no cap on B, no host sync.
-// MIN_ROWS > 0: an utterance with fewer rows counts as empty (the fused attention kernel leaves those to the exact one).
+// The work list of a persistent kernel: blocks x B utterances x `tile`-row tiles, items ordered (block, utterance, tile).  Every role
+// of a CTA walks it as  for (i = blockIdx.x; i < count; i += gridDim.x) { const Item it = work.item(i); ... }  with its own copy, so
+// all roles see the same item sequence: the mbarrier rings only work if they do.
+// init's per_b = ceil(cap / tile) and items = blocks * B * per_b are the padded shape's tiles per utterance and item count as the host
+// planned them: as kernel parameters they cost the padded instantiations no registers, computed here they did.
+// RAG: ragged batch (lens != NULL): utterance b has n_b = ragged_rows(lens, scale, cap, b) rows and only its live tiles are items,
+// sum_b ceil(n_b / tile) per block, so no tile lying wholly in the padding is ever scheduled.  MIN_ROWS > 0: an utterance with fewer
+// rows counts as empty (the fused attention kernel leaves those to the exact one).  RAG is a template parameter rather than a runtime
+// branch: the cursor state would otherwise cost the padded instantiations registers.
+template <bool RAG, int MIN_ROWS = 0>
+struct WorkList;
+
+// Padded batch: every utterance has cap rows, and an item index decodes by plain division.
 template <int MIN_ROWS>
-struct RaggedWalkT {
-  int live;                        // live tiles per channel block
-  int nblk, b, before, rows;       // cursor: channel block, utterance, live tiles of utterances < b in the block, n_b
-  __device__ __forceinline__ static int rows_of(const int* lens, int scale, int cap, int b) {
-    const int n = ragged_rows(lens, scale, cap, b);
-    if constexpr (MIN_ROWS > 0) return n < MIN_ROWS ? 0 : n;
-    return n;
+struct WorkList<false, MIN_ROWS> {
+  int count, B, tile, cap, per_b;
+  __device__ __forceinline__ void init(const int*, int, int cap_, int B_, int tile_, int per_b_, int items) {
+    cap = cap_; B = B_; tile = tile_; per_b = per_b_; count = items;
   }
-  __device__ __forceinline__ void init(const int* lens, int scale, int cap, int B, int tile) {
-    live = 0;
-    for (int i = 0; i < B; i++) live += (rows_of(lens, scale, cap, i) + tile - 1) / tile;
-    nblk = 0; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0);
-  }
-  __device__ __forceinline__ Item item(const int* lens, int scale, int cap, int tile, int i) {   // i < live * channel blocks
-    const int blk = i / live, rem = i - blk * live;
-    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(lens, scale, cap, 0); }
-    for (int nt = (rows + tile - 1) / tile; rem >= before + nt; nt = (rows + tile - 1) / tile) {
-      before += nt;
-      rows = rows_of(lens, scale, cap, ++b);
-    }
+  __device__ __forceinline__ Item item(int i) const {
+    const int per_blk = B * per_b;
     Item it;
-    it.nblk = blk; it.b = b; it.t0 = (rem - before) * tile;
+    it.nblk = i / per_blk;
+    const int rem = i - it.nblk * per_blk;
+    it.b = rem / per_b;
+    it.t0 = (rem - it.b * per_b) * tile;
+    it.rows = cap;
     return it;
   }
 };
-using RaggedWalk = RaggedWalkT<0>;
+
+// Ragged batch: a monotone cursor over the compacted sequence.  A role visits its items in increasing order, so the cursor only moves
+// forward and each length is loaded once per block: no table, no cap on B, no host sync.
+template <int MIN_ROWS>
+struct WorkList<true, MIN_ROWS> {
+  const int* lens; int scale, cap, tile;
+  int count, live;                 // items; live tiles per block
+  int nblk, b, before, rows;       // cursor: block, utterance, live tiles of utterances < b in the block, n_b
+  __device__ __forceinline__ int rows_of(int u) const {
+    const int n = ragged_rows(lens, scale, cap, u);
+    if constexpr (MIN_ROWS > 0) return n < MIN_ROWS ? 0 : n;
+    return n;
+  }
+  __device__ __forceinline__ void init(const int* lens_, int scale_, int cap_, int B, int tile_, int per_b, int items) {
+    lens = lens_; scale = scale_; cap = cap_; tile = tile_;
+    live = 0;
+    for (int u = 0; u < B; u++) live += (rows_of(u) + tile - 1) / tile;
+    count = live * (items / (B * per_b));          // live tiles x blocks
+    nblk = 0; b = 0; before = 0; rows = rows_of(0);
+  }
+  __device__ __forceinline__ Item item(int i) {   // i < count, and not below the previous call's i
+    const int blk = i / live, rem = i - blk * live;
+    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(0); }
+    for (int nt = (rows + tile - 1) / tile; rem >= before + nt; nt = (rows + tile - 1) / tile) {
+      before += nt;
+      rows = rows_of(++b);
+    }
+    Item it;
+    it.nblk = blk; it.b = b; it.t0 = (rem - before) * tile; it.rows = rows;
+    return it;
+  }
+};
 
 }  // namespace fs2

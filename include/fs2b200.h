@@ -74,16 +74,30 @@ enum { FS2_TC_VARIANT_F8 = 1,
 int fs2_conv_tc_block(int N);    /* 0 when N is not supported by the tensor-core kernel */
 int fs2_conv_tc_block_f8(int N); /* the same for FS2_TC_VARIANT_F8 tiles: the largest multiple of 16 <= 64 that divides N (N itself if N <= 64) */
 struct fs2_conv1d_args;
-/* Launch plan the tensor-core kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are
- * only checked for alignment; a work item is one 128-row tile x NB output channels): out[11] = {NB, TG (accumulators per tile), slab
- * stages, weight stages, taps per weight stage, slab rows, accumulator registers per consumer thread, work items per utterance, work items,
- * grid, dynamic shared memory bytes}.
- * Returns FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
-int fs2_conv_tc_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out);
-/* Tile the exact fp32 kernel (FS2_CONV_SIMT) would use for this call on a device with num_sms SMs (pure host logic, no CUDA call,
- * pointers are not read): out[4] = {BM (rows per CTA: 64 or 128), BN (output channels per CTA: 32, 64 or 128), grid.x, grid.y}.
- * Returns FS2_ERR_ARG / FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
-int fs2_conv_simt_plan(const struct fs2_conv1d_args* a, int num_sms, int32_t* out);
+/* Launch plan of the tensor-core kernel; a work item is one 128-row tile x NB output channels. */
+typedef struct fs2_conv_tc_plan_t {
+  int32_t NB;              /* output channels per work item */
+  int32_t TG;              /* accumulators per tile: 1 = all split terms together, 2 = {hi*hi | the cross terms} */
+  int32_t SA, SB;          /* activation slab stages, weight stages */
+  int32_t TPS;             /* conv taps per weight stage */
+  int32_t R;               /* slab rows */
+  int32_t acc_regs;        /* accumulator registers per consumer thread */
+  int32_t tiles_per_batch; /* work items per utterance and channel block */
+  int32_t n_items, grid;   /* work items (of the padded shape), CTAs */
+  int32_t smem;            /* dynamic shared memory bytes */
+} fs2_conv_tc_plan_t;
+/* The plan the tensor-core kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are
+ * only checked for alignment).  Returns FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
+int fs2_conv_tc_plan(const struct fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
+/* Tile of the exact fp32 kernel (FS2_CONV_SIMT). */
+typedef struct fs2_conv_simt_plan_t {
+  int32_t BM;              /* rows per CTA: 64 or 128 */
+  int32_t BN;              /* output channels per CTA: 32, 64 or 128 */
+  int32_t grid_x, grid_y;
+} fs2_conv_simt_plan_t;
+/* The tile the exact kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are not
+ * read).  Returns FS2_ERR_ARG / FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */
+int fs2_conv_simt_plan(const struct fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
 
 #define FS2_MAX_LAYERS 12
 #define FS2_MAX_POSTNET 8
@@ -219,10 +233,20 @@ typedef struct fs2_resstack_args {
   const int32_t* lens; int lens_scale;
 } fs2_resstack_args;
 int fs2_resstack(const fs2_resstack_args* a, fs2_stream_t stream);
-/* launch plan (pure host logic): out[12] = {128-row tiles per slab, halo rows per side, output rows per work item, work items, grid,
- * weight ring stages, dynamic shared memory bytes, accumulator registers per consumer thread, rows per output TMA box, output boxes per tile, conv taps per weight stage,
- * 0 (reserved: every work item is one slab with its halo at the two ends)} */
-int fs2_resstack_plan(const fs2_resstack_args* a, int num_sms, int32_t* out);
+/* Launch plan of fs2_resstack; a work item is one slab of MT * 128 rows: TILE output rows with H halo rows at each end. */
+typedef struct fs2_resstack_plan_t {
+  int32_t MT;              /* 128-row tiles per slab */
+  int32_t H;               /* halo rows per side */
+  int32_t TILE;            /* output rows per work item */
+  int32_t n_items, grid;   /* work items (of the padded shape), CTAs */
+  int32_t SB;              /* weight ring stages */
+  int32_t smem;            /* dynamic shared memory bytes */
+  int32_t acc_regs;        /* accumulator registers per consumer thread */
+  int32_t OBOX, n_oboxes;  /* rows per output TMA box, output boxes per tile */
+  int32_t TPS;             /* conv taps per weight stage */
+} fs2_resstack_plan_t;
+/* The plan fs2_resstack would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are not read). */
+int fs2_resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t* out);
 
 /* out[b,t] = t < lens[b] ? (int16) trunc(wav[b,t] * scale) : 0   -- the device half of utils.model.vocoder_infer (utils/model.py:82-90:
  * `(wavs.cpu().numpy() * max_wav_value).astype("int16")` then `wavs[i][:lengths[i]]`): 2 bytes per sample cross PCIe instead of 4, the
@@ -373,7 +397,10 @@ int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, f
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
 const char* fs2_build_info(void);          /* "sm_90a ..." */
-size_t fs2_struct_size(int which);         /* sizeof of the i-th struct above, in declaration order (binding self-check) */
+/* sizeof of a struct above (binding self-check), fs2_<name>[_args]: 0 conv1d, 1 layernorm, 2 attention, 3 embed, 4 rowbias,
+ * 5 variance_head, 6 durations, 7 length_regulate, 8 conv_post, 9 acoustic_model, 10 encode, 11 decode, 12 vocoder_model,
+ * 13 vocoder, 14 resstack, 15 wav_int16, 16 conv_tc_plan_t, 17 conv_simt_plan_t, 18 resstack_plan_t */
+size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the
  * device that owns the stream current before calling -- (b) the launch counter above and (c) the profiling state below, which is

@@ -37,7 +37,8 @@ def test_struct_sizes_match_the_header():
     h = _lib.lib()
     table = {0: _lib.Conv1dArgs, 1: _lib.LayerNormArgs, 2: _lib.AttentionArgs, 3: _lib.EmbedArgs, 4: _lib.RowBiasArgs,
              5: _lib.VarianceHeadArgs, 6: _lib.DurationsArgs, 7: _lib.LengthRegulateArgs, 8: _lib.ConvPostArgs,
-             9: _lib.AcousticModel, 10: _lib.EncodeArgs, 11: _lib.DecodeArgs, 12: _lib.VocoderModel, 13: _lib.VocoderArgs, 14: _lib.ResstackArgs, 15: _lib.WavInt16Args}
+             9: _lib.AcousticModel, 10: _lib.EncodeArgs, 11: _lib.DecodeArgs, 12: _lib.VocoderModel, 13: _lib.VocoderArgs, 14: _lib.ResstackArgs, 15: _lib.WavInt16Args,
+             16: _lib.ConvTcPlan, 17: _lib.ConvSimtPlan, 18: _lib.ResstackPlan}
     for i, cls in table.items():
         assert h.fs2_struct_size(i) == ctypes.sizeof(cls), cls.__name__
 
@@ -67,10 +68,9 @@ def _plan(h, B, T, Cin, N, taps, dil=1, num_sms=132, x=0x1000, x_row_stride=None
     a = _lib.Conv1dArgs(x=x, x_batch_stride=T * (x_row_stride or Cin), x_row_stride=x_row_stride or Cin, B=B, T=T, Cin=Cin, w=0x1000, N=N, taps=taps,
                         dilation=dil, pad_left=(taps - 1) * dil // 2, w_tc=0x1000, y=0x1000, y_batch_stride=T * N, y_row_stride=N, alpha=1.0,
                         tc_variant=tc_variant)
-    out = (ctypes.c_int32 * 11)()
-    rc = h.fs2_conv_tc_plan(ctypes.byref(a), num_sms, out)
-    keys = ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")
-    return rc, dict(zip(keys, out))
+    out = _lib.ConvTcPlan()
+    rc = h.fs2_conv_tc_plan(ctypes.byref(a), num_sms, ctypes.byref(out))
+    return rc, _lib.fields(out)
 
 
 def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
@@ -108,8 +108,8 @@ def test_tensor_core_conv_launch_plan_respects_the_hardware_limits():
         if n and n % 16 == 0:
             a = _lib.Conv1dArgs(x=0x1000, x_batch_stride=256 * 16, x_row_stride=16, B=1, T=256, Cin=16, w=0x1000, N=n, taps=1,
                                 w_tc=0x1000, y=0x1000, y_batch_stride=256 * n, y_row_stride=n, alpha=1.0, tc_variant=_lib.TC_VARIANT_F8)
-            out = (ctypes.c_int32 * 11)()
-            assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, out) == 0 and out[0] == h.fs2_conv_tc_block_f8(n) and out[1] == 2, n
+            out = _lib.ConvTcPlan()
+            assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, ctypes.byref(out)) == 0 and out.NB == h.fs2_conv_tc_block_f8(n) and out.TG == 2, n
     # ring depths per shape class: short kernels get the deepest slab ring, wide kernels share one weight stage between four taps
     assert _plan(h, 16, 64768, 128, 128, 3)[1]["SA"] == 5 and _plan(h, 16, 64768, 128, 128, 11, 5)[1]["TPS"] == 4
     # refused shapes: C_in % 16, N % 16, misaligned or oddly strided x, halo beyond the slab
@@ -124,10 +124,9 @@ def _rs_plan(C, N, ks, dils, B=16):
         a.k[j] = k
         for d, dv in enumerate(dils[j]):
             a.dil[j][d] = dv
-    out = (ctypes.c_int32 * 12)()
-    rc = _lib.lib().fs2_resstack_plan(ctypes.byref(a), 132, out)
-    keys = ("MT", "H", "TILE", "items", "grid", "SB", "smem", "regs", "obox", "n_oboxes", "TPS", "indep")
-    return rc, dict(zip(keys, out))
+    out = _lib.ResstackPlan()
+    rc = _lib.lib().fs2_resstack_plan(ctypes.byref(a), 132, ctypes.byref(out))
+    return rc, _lib.fields(out)
 
 
 def test_gpu_case_tables_reach_every_tile_width_and_the_persistent_loop():
@@ -213,10 +212,10 @@ def test_gpu_case_tables_reach_every_exact_conv_tile():
     assert G.simt_plan(16, 1000, 256, 1024, 9) == (128, 128) and G.simt_plan(2, 131, 1024, 256, 1) == (64, 64)
     h = _lib.lib()
     a = _lib.Conv1dArgs(x=16, w=16, y=16, B=1, T=128, Cin=24, N=16, taps=1)
-    out = (ctypes.c_int32 * 4)()
-    assert h.fs2_conv_simt_plan(ctypes.byref(a), 132, out) == -2
+    out = _lib.ConvSimtPlan()
+    assert h.fs2_conv_simt_plan(ctypes.byref(a), 132, ctypes.byref(out)) == -2
     a.Cin, a.T = 16, 0
-    assert h.fs2_conv_simt_plan(ctypes.byref(a), 132, out) == -1
+    assert h.fs2_conv_simt_plan(ctypes.byref(a), 132, ctypes.byref(out)) == -1
 
 
 def test_fused_resblock_plan_respects_the_hardware_limits():
@@ -232,11 +231,11 @@ def test_fused_resblock_plan_respects_the_hardware_limits():
         assert rc == 0, (C, N, ks, dils, rc)
         radius = max(sum((k - 1) * d // 2 + (k - 1) // 2 for d in dd) for k, dd in zip(ks, dils))
         assert p["H"] >= radius and p["H"] % 4 == 0
-        assert p["obox"] % 8 == 0 and 8 <= p["obox"] <= 256 and p["n_oboxes"] * p["obox"] == p["TILE"] and p["n_oboxes"] <= 12
-        assert p["indep"] == 0 and p["TILE"] == p["MT"] * 128 - 2 * p["H"]
-        assert p["smem"] <= 227 * 1024 and p["regs"] == p["MT"] * C <= 128
+        assert p["OBOX"] % 8 == 0 and 8 <= p["OBOX"] <= 256 and p["n_oboxes"] * p["OBOX"] == p["TILE"] and p["n_oboxes"] <= 12
+        assert p["TILE"] == p["MT"] * 128 - 2 * p["H"]
+        assert p["smem"] <= 227 * 1024 and p["acc_regs"] == p["MT"] * C <= 128
         assert 2 <= p["SB"] <= 8 and p["TPS"] * 64 * C == 8192
-        assert p["items"] == 16 * -(-N // p["TILE"]) and p["grid"] == min(p["items"], 132)
+        assert p["n_items"] == 16 * -(-N // p["TILE"]) and p["grid"] == min(p["n_items"], 132)
     # refused: other widths, even kernels, taps reaching more than 32 rows outside a tile, table overflow
     assert plan(128, 1000, (3,), ((1,),))[0] == -2 and plan(32, 1000, (4,), ((1,),))[0] == -2
     assert plan(32, 1000, (11,), ((7,),))[0] == -2 and plan(32, 0, (3,), ((1,),))[0] == -1

@@ -14,7 +14,6 @@ import pytest
 from fastspeech2_b200 import _lib
 from tests import test_sass_pipeline as S
 
-KEYS = ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")
 TILE_ROWS, PAD, CWARPS = 128, 8, 8
 
 
@@ -49,9 +48,9 @@ def _plan(B, T, Cin, N, taps, dil=1, res=False, accumulate=False, tc_variant=0):
                         pad_left=(taps - 1) * dil // 2, w_tc=0x1000, y=0x1000, y_batch_stride=T * N, y_row_stride=N, alpha=1.0,
                         res=0x2000 if res else 0, res_batch_stride=T * N if res else 0, res_row_stride=N if res else 0,
                         accumulate=int(accumulate), tc_variant=tc_variant)
-    out = (ctypes.c_int32 * 11)()
-    rc = _lib.lib().fs2_conv_tc_plan(ctypes.byref(a), 132, out)
-    return rc, dict(zip(KEYS, out))
+    out = _lib.ConvTcPlan()
+    rc = _lib.lib().fs2_conv_tc_plan(ctypes.byref(a), 132, ctypes.byref(out))
+    return rc, _lib.fields(out)
 
 
 def _shapes():

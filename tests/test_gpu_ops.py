@@ -80,9 +80,9 @@ def simt_plan(B, T, Cin, N, taps, num_sms=132):
     import ctypes
     from fastspeech2_b200 import _lib as L
     a = L.Conv1dArgs(x=16, w=16, y=16, B=B, T=T, Cin=Cin, N=N, taps=taps, alpha=1.0)
-    out = (ctypes.c_int32 * 4)()
-    assert L.lib().fs2_conv_simt_plan(ctypes.byref(a), num_sms, out) == 0
-    return out[0], out[1]
+    out = L.ConvSimtPlan()
+    assert L.lib().fs2_conv_simt_plan(ctypes.byref(a), num_sms, ctypes.byref(out)) == 0
+    return out.BM, out.BN
 
 
 def conv_scale(x, w, bias, dil, pad, in_act, in_slope, res, alpha, y0, lens):
@@ -463,8 +463,7 @@ SINGLE_PAIR_CASES = [
 
 @pytest.mark.parametrize("C,k,dils,N", SINGLE_PAIR_CASES)
 def test_resstack_single_pair_accumulate(C, k, dils, N):
-    """The single-kernel-size mode of fs2_resstack (n_kernels = 1, alpha, accumulate): y += alpha * ResBlock_k,dils(x).  With a small
-    halo the kernel runs independent 128-row tiles (each with its own halo) and prefetches the next work item's input; the long cases
+    """The single-kernel-size mode of fs2_resstack (n_kernels = 1, alpha, accumulate): y += alpha * ResBlock_k,dils(x).  The long cases
     give every CTA several work items."""
     import torch.nn.functional as F
     B = 2

@@ -11,14 +11,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 STRUCTS = (_lib.Conv1dArgs, _lib.LayerNormArgs, _lib.AttentionArgs, _lib.EmbedArgs, _lib.RowBiasArgs, _lib.VarianceHeadArgs,
            _lib.DurationsArgs, _lib.LengthRegulateArgs, _lib.ConvPostArgs, _lib.AcousticModel, _lib.EncodeArgs, _lib.DecodeArgs,
-           _lib.VocoderModel, _lib.VocoderArgs, _lib.ResstackArgs, _lib.WavInt16Args)
+           _lib.VocoderModel, _lib.VocoderArgs, _lib.ResstackArgs, _lib.WavInt16Args, _lib.ConvTcPlan, _lib.ConvSimtPlan, _lib.ResstackPlan)
 
 
 def test_ragged_entry_points_are_bound_and_the_abi_is_unchanged():
     h = _lib.lib()
     for name in ("fs2_acoustic_encode_ragged", "fs2_acoustic_decode_ragged"):
         assert name in _lib.EXPORTS and getattr(h, name).argtypes == _lib.EXPORTS[name][1]
-    assert h.fs2_abi_version() == _lib.ABI_VERSION == 11
+    assert h.fs2_abi_version() == _lib.ABI_VERSION == 12
     for i, cls in enumerate(STRUCTS):
         assert h.fs2_struct_size(i) == ctypes.sizeof(cls), cls.__name__
     assert h.fs2_struct_size(len(STRUCTS)) == 0

@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_ragged_fields_are_appended_and_sizes_match():
     h = _lib.lib()
-    assert h.fs2_abi_version() == _lib.ABI_VERSION == 11
+    assert h.fs2_abi_version() == _lib.ABI_VERSION == 12
     for i, cls, tail in ((0, _lib.Conv1dArgs, ["x_lens", "lens_scale"]), (8, _lib.ConvPostArgs, ["lens", "lens_scale"]),
                          (13, _lib.VocoderArgs, ["mel_lens"]), (14, _lib.ResstackArgs, ["lens", "lens_scale"])):
         names = [f[0] for f in cls._fields_]
@@ -44,20 +44,20 @@ def test_launch_plans_do_not_depend_on_lengths():
         a = _lib.Conv1dArgs(x=0x1000, x_batch_stride=4096 * 64, x_row_stride=64, B=3, T=4096, Cin=64, w=0x1000, N=64, taps=7,
                             pad_left=3, w_tc=0x1000, alpha=1.0, y=0x1000, y_batch_stride=4096 * 64, y_row_stride=64,
                             tc_variant=_lib.TC_VARIANT_F8, x_lens=lens, lens_scale=scale)
-        out = (ctypes.c_int32 * 11)()
-        assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, out) == 0
+        out = _lib.ConvTcPlan()
+        assert h.fs2_conv_tc_plan(ctypes.byref(a), 132, ctypes.byref(out)) == 0
         r = _lib.ResstackArgs(x=0x10000, y=0x40000, B=3, N=4096, C=64, n_kernels=3, n_dil=3, lens=lens, lens_scale=scale)
         for j, k in enumerate((3, 7, 11)):
             r.k[j] = k
             for d, dv in enumerate((1, 3, 5)):
                 r.dil[j][d] = dv
-        rp = (ctypes.c_int32 * 12)()
-        assert h.fs2_resstack_plan(ctypes.byref(r), 132, rp) == 0
+        rp = _lib.ResstackPlan()
+        assert h.fs2_resstack_plan(ctypes.byref(r), 132, ctypes.byref(rp)) == 0
         if lens == 0:
-            ref_conv, ref_rs = list(out), list(rp)
-        assert list(out) == ref_conv and list(rp) == ref_rs
-    assert ref_conv[8] == 3 * 32 and ref_conv[9] == 96         # 3 x 32 tiles of one 64-channel block: padded shape
-    assert ref_rs[3] == 3 * -(-4096 // ref_rs[2])
+            ref_conv, ref_rs = _lib.fields(out), _lib.fields(rp)
+        assert _lib.fields(out) == ref_conv and _lib.fields(rp) == ref_rs
+    assert ref_conv["n_items"] == 3 * 32 and ref_conv["grid"] == 96   # 3 x 32 tiles of one 64-channel block: padded shape
+    assert ref_rs["n_items"] == 3 * -(-4096 // ref_rs["TILE"])
 
 
 _FAKE_REFERENCE = r'''

@@ -120,6 +120,11 @@ class DecodeArgs(C.Structure):
                 ("mel", fp), ("postnet_mel", fp), ("workspace", fp), ("workspace_bytes", C.c_size_t)]
 
 
+class ControlArgs(C.Structure):
+    """fs2_control_args: per-element p / d controls of fs2_acoustic_{encode,decode}_ctl (48 bytes, pinned by a static_assert in model.cu)."""
+    _fields_ = [("p", fp), ("p_stride_b", i64), ("p_stride_l", i64), ("d", fp), ("d_stride_b", i64), ("d_stride_l", i64)]
+
+
 class VocoderModel(C.Structure):
     _fields_ = [("n_mel", i32), ("c0", i32), ("n_stages", i32), ("n_kernels", i32), ("n_dil", i32),
                 ("rates", i32 * MAX_STAGES), ("up_k", i32 * MAX_STAGES),
@@ -204,6 +209,8 @@ EXPORTS = {
     "fs2_acoustic_decode": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), fp]),
     "fs2_acoustic_encode_ragged": (i32, [C.POINTER(AcousticModel), C.POINTER(EncodeArgs), fp]),
     "fs2_acoustic_decode_ragged": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), fp]),
+    "fs2_acoustic_encode_ctl": (i32, [C.POINTER(AcousticModel), C.POINTER(EncodeArgs), C.POINTER(ControlArgs), i32, fp]),
+    "fs2_acoustic_decode_ctl": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), C.POINTER(ControlArgs), i32, fp]),
     "fs2_vocoder_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderArgs), fp]),
 }

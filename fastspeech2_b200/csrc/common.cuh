@@ -65,6 +65,13 @@ __device__ __forceinline__ int ragged_rows(const int* lens, int scale, int cap, 
   return n <= 0 ? 0 : (n >= cap ? cap : (int)n);
 }
 
+// A per-element control of fs2_control_args on the [B][L] rows of a variance head or of the durations: c[b, l] = v[b * sb + l * sl]
+// (strides in elements, 0 along a broadcast dimension).  rag: NULL, or the ragged mode's lengths -- columns l >= rag[b] are not read.
+struct ControlView {
+  const float* v; int64_t sb, sl;
+  const int32_t* rag;
+};
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -83,8 +83,8 @@ int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = fa
 int embed_positions(const fs2_embed_args* a, cudaStream_t s);
 int add_speaker(const fs2_rowbias_args* a, cudaStream_t s);
 int layernorm(const fs2_layernorm_args* a, cudaStream_t s);
-int variance_head(const fs2_variance_head_args* a, cudaStream_t s);
-int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr);
+int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl = nullptr);
+int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr);
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s);
 int resstack(const fs2_resstack_args* a, cudaStream_t s);
@@ -225,8 +225,9 @@ static FftBufs fft_bufs(Arena& ar, const fs2_acoustic_model* m, size_t rows, int
 // VariancePredictor.forward (+ bucketize / embedding add when bins != NULL) on rows [B][T]  (model/modules.py:242-250, :80-100).
 // `head` carries the caller's part of the head's arguments: B, L = T, lens, control, target, bins, emb, pred_out, and x, which is
 // both the predictor's input and where the embedding is added.  Ragged: the convs and LayerNorms are bounded by head.lens.
+// ctl: the per-element control that replaces head.control (ctl.v NULL: the scalar).
 static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_predictor_weights& w, fs2_variance_head_args head,
-                         float* h1, float* h2, bool ragged) {
+                         float* h1, float* h2, bool ragged, const ControlView& ctl = ControlView{}) {
   const int B = head.B, T = head.L, k = m->vp_kernel, D = m->d_model, VF = m->vp_filter;
   const bool seg = (m->tc_mask & FS2_TC_PREDICTORS) && w.w_c1_tc && w.w_c2_tc;   // K-segmented: the ReLU is applied by the LayerNorm
   const ConvMode mode{seg ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};
@@ -249,12 +250,19 @@ static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_
   n.gamma = w.ln2_g; n.beta = w.ln2_b;
   FS2_TRY(layernorm(&n, s));
   head.h = h2; head.w = w.w_out; head.b = w.b_out; head.C = VF; head.n_edges = m->n_bins - 1; head.D = D;
-  return variance_head(&head, s);
+  return variance_head(&head, s, &ctl);
+}
+
+// The p (pitch / energy) or d (durations) control of fs2_control_args on the phase's [B][L] rows; ragged: columns l >= lens[b] are not read.
+static ControlView control_view(const float* v, int64_t sb, int64_t sl, bool ragged, const int32_t* lens) {
+  return ControlView{v, sb, sl, v ? ragged_lens(ragged, lens) : nullptr};
 }
 
 // ------------------------------------------------------------------ phase 1
 // ragged: utterance b has src_lens[b] phonemes; x_adapted rows at or beyond it are left unspecified.
-static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cudaStream_t s, Arena& ar, bool ragged) {
+// ctl: NULL, or the per-element p / d controls that replace a->p_control / a->d_control where their pointers are set.
+static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, cudaStream_t s, Arena& ar,
+                       bool ragged) {
   const int B = a->B, L = a->L, D = m->d_model, VF = m->vp_filter;
   const size_t rows = (size_t)B * L;
   FftBufs f = fft_bufs(ar, m, rows);
@@ -284,22 +292,24 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
   v.x = a->x_adapted; v.B = B; v.L = L; v.lens = a->src_lens; v.control = 1.f; v.pred_out = a->logd_pred;
   FS2_TRY(run_predictor(s, m, m->dur, v, h1, h2, ragged));
   v.control = a->p_control;
+  const ControlView p_ctl = ctl ? control_view(ctl->p, ctl->p_stride_b, ctl->p_stride_l, ragged, a->src_lens) : ControlView{};
   if (!m->pitch_frame_level) {
     if (!a->p_pred) return FS2_ERR_ARG;
     v.target = a->p_target; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred;
-    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged));
+    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged, p_ctl));
   }
   if (!m->energy_frame_level) {
     if (!a->e_pred) return FS2_ERR_ARG;
     v.target = a->e_target; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred;
-    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged));
+    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged, p_ctl));
   }
 
   fs2_durations_args d{};
   d.src = a->d_target ? a->d_target : a->logd_pred; d.use_target = a->d_target != nullptr; d.d_control = a->d_control;
   d.B = B; d.L = L; d.d_rounded = a->d_target ? nullptr : a->d_rounded; d.cum = a->cum_dur; d.mel_lens = a->mel_lens;
   d.mel_lens32 = a->mel_lens32; d.len_stats = a->len_stats;
-  FS2_TRY(durations(&d, s, ragged_lens(ragged, a->src_lens)));
+  const ControlView d_ctl = ctl ? control_view(ctl->d, ctl->d_stride_b, ctl->d_stride_l, ragged, a->src_lens) : ControlView{};
+  FS2_TRY(durations(&d, s, ragged_lens(ragged, a->src_lens), &d_ctl));
   if (a->len_stats_host) {
     ce = cudaMemcpyAsync(a->len_stats_host, a->len_stats, 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
     if (ce != cudaSuccess) return FS2_ERR_CUDA - (int)ce;
@@ -309,7 +319,9 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, cu
 
 // ------------------------------------------------------------------ phase 2
 // ragged: utterance b has mel_mask_lens[b] frames; mel and postnet_mel rows at or beyond it are zeroed.
-static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cudaStream_t s, Arena& ar, bool ragged) {
+// ctl: NULL, or the per-frame p control that replaces a->p_control when ctl->p is set (ctl->d is not read).
+static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, cudaStream_t s, Arena& ar,
+                       bool ragged) {
   const int B = a->B, T = a->T, D = m->d_model;
   const size_t rows = (size_t)B * T;
   FftBufs f = fft_bufs(ar, m, rows, B, T, (m->tc_mask & FS2_TC_DECODER) != 0);
@@ -331,15 +343,16 @@ static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, cu
     if ((size_t)m->d_inner < 2 * (size_t)m->vp_filter) return FS2_ERR_UNSUPPORTED;
     fs2_variance_head_args v{};
     v.x = f.x; v.B = B; v.L = T; v.lens = a->mel_mask_lens; v.control = a->p_control;
+    const ControlView p_ctl = ctl ? control_view(ctl->p, ctl->p_stride_b, ctl->p_stride_l, ragged, a->mel_mask_lens) : ControlView{};
     if (m->pitch_frame_level) {
       if (!a->p_pred_frames) return FS2_ERR_ARG;
       v.target = a->p_target_frames; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred_frames;
-      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged));
+      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged, p_ctl));
     }
     if (m->energy_frame_level) {
       if (!a->e_pred_frames) return FS2_ERR_ARG;
       v.target = a->e_target_frames; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred_frames;
-      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged));
+      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged, p_ctl));
     }
     FS2_TRY(add_positions(f.x, m->dec_pos, B, T, D, s));
   }
@@ -511,6 +524,8 @@ int fs2_conv_tc_block_f8(int N) { return conv_tc_nb(N, 64); }
 int fs2_conv_tc_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out) { return conv_tc_plan_query(a, num_sms, out); }
 int fs2_conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out) { return conv_simt_plan(a, num_sms, out); }
 int64_t fs2_kernel_launch_count(void) { return (int64_t)g_launch_count.load(); }
+// fs2_control_args is not in the fs2_struct_size table (its indices are pinned at 0..18): its layout is pinned here and in the binding
+static_assert(sizeof(fs2_control_args) == 48, "fs2_control_args: two pointers and four int64 strides");
 size_t fs2_struct_size(int which) {
   switch (which) {
     case 0: return sizeof(fs2_conv1d_args);
@@ -590,41 +605,46 @@ size_t fs2_encode_workspace_bytes(const fs2_acoustic_model* m, int B, int L) {
   Arena ar(nullptr, 0);
   fs2_encode_args a{};
   a.B = B; a.L = L;
-  encode_impl(m, &a, nullptr, ar, false);
+  encode_impl(m, &a, nullptr, nullptr, ar, false);
   return ar.off + 256;
 }
 
-static int acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st, bool ragged) {
-  if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0) return FS2_ERR_ARG;
+static bool control_ok(const fs2_control_args* c, int ragged) {
+  return (ragged == 0 || ragged == 1) &&
+         (!c || (c->p_stride_b >= 0 && c->p_stride_l >= 0 && c->d_stride_b >= 0 && c->d_stride_l >= 0));
+}
+
+int fs2_acoustic_encode_ctl(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st) {
+  if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0 || !control_ok(ctl, ragged)) return FS2_ERR_ARG;
   if (!a->texts || !a->src_lens || !a->logd_pred || !a->mel_lens || !a->cum_dur || !a->x_adapted ||
       !a->len_stats || !a->workspace)
     return FS2_ERR_ARG;
   if (!a->d_target && !a->d_rounded) return FS2_ERR_ARG;
   if (m->d_model / m->n_head != 128) return FS2_ERR_UNSUPPORTED;
   Arena ar(a->workspace, a->workspace_bytes);
-  return encode_impl(m, a, S(st), ar, ragged);
+  return encode_impl(m, a, ctl, S(st), ar, ragged != 0);
 }
-int fs2_acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return acoustic_encode(m, a, st, false); }
-int fs2_acoustic_encode_ragged(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return acoustic_encode(m, a, st, true); }
+int fs2_acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return fs2_acoustic_encode_ctl(m, a, nullptr, 0, st); }
+int fs2_acoustic_encode_ragged(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return fs2_acoustic_encode_ctl(m, a, nullptr, 1, st); }
 
 size_t fs2_decode_workspace_bytes(const fs2_acoustic_model* m, int B, int T) {
   if (!model_ok(m) || B <= 0 || T <= 0) return 0;
   Arena ar(nullptr, 0);
   fs2_decode_args a{};
   a.B = B; a.T = T;
-  decode_impl(m, &a, nullptr, ar, false);
+  decode_impl(m, &a, nullptr, nullptr, ar, false);
   return ar.off + 256;
 }
 
-static int acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st, bool ragged) {
-  if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0 || a->T <= 0) return FS2_ERR_ARG;
+int fs2_acoustic_decode_ctl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st) {
+  if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0 || a->T <= 0 || !control_ok(ctl, ragged)) return FS2_ERR_ARG;
   if (!a->x_adapted || !a->cum_dur || !a->mel_mask_lens || !a->mel || !a->postnet_mel || !a->workspace) return FS2_ERR_ARG;
   if (m->d_model / m->n_head != 128) return FS2_ERR_UNSUPPORTED;
   Arena ar(a->workspace, a->workspace_bytes);
-  return decode_impl(m, a, S(st), ar, ragged);
+  return decode_impl(m, a, ctl, S(st), ar, ragged != 0);
 }
-int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return acoustic_decode(m, a, st, false); }
-int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return acoustic_decode(m, a, st, true); }
+int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return fs2_acoustic_decode_ctl(m, a, nullptr, 0, st); }
+int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return fs2_acoustic_decode_ctl(m, a, nullptr, 1, st); }
 
 static bool vocoder_ok(const fs2_vocoder_model* m) {
   if (!(m && m->n_stages > 0 && m->n_stages <= FS2_MAX_STAGES && m->n_kernels > 0 && m->n_kernels <= FS2_MAX_DIL + 4 &&

@@ -153,7 +153,10 @@ int layernorm(const fs2_layernorm_args* a, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------ variance head (modules.py:80-100, :246-250)
-__global__ void variance_head_kernel(const fs2_variance_head_args a) {
+// CTL: the prediction is scaled by the per-element control ctl instead of the scalar a.control (a template parameter so that the
+// scalar path keeps its code and registers).  Both are one fp32 multiply: a control array of fp32(c) gives the scalar c's bits.
+template <bool CTL>
+__global__ void variance_head_kernel(const fs2_variance_head_args a, const ControlView ctl) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= a.B * a.L) return;
   const int lane = threadIdx.x & 31;
@@ -172,7 +175,8 @@ __global__ void variance_head_kernel(const fs2_variance_head_args a) {
     if (a.target) {
       key = a.target[row];
     } else {
-      pred = pred * a.control;
+      if (!CTL) pred = pred * a.control;
+      else if (!(ctl.rag && l >= ctl.rag[b])) pred = pred * __ldg(ctl.v + b * ctl.sb + l * ctl.sl);
       key = pred;
     }
   }
@@ -194,12 +198,14 @@ __global__ void variance_head_kernel(const fs2_variance_head_args a) {
   }
 }
 
-int variance_head(const fs2_variance_head_args* a, cudaStream_t s) {
+// ctl: NULL or ctl->v NULL for the scalar a->control
+int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl) {
   if (!a || !a->h || !a->w || !a->b || !a->pred_out || a->B <= 0 || a->L <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->C % 4) return FS2_ERR_UNSUPPORTED;
   if (a->bins && (!a->emb || !a->x || a->n_edges <= 0 || a->D <= 0 || a->D % 4)) return FS2_ERR_ARG;
   const int rows = a->B * a->L;
-  variance_head_kernel<<<(rows + 7) / 8, 256, 0, s>>>(*a);
+  if (ctl && ctl->v) variance_head_kernel<true><<<(rows + 7) / 8, 256, 0, s>>>(*a, *ctl);
+  else variance_head_kernel<false><<<(rows + 7) / 8, 256, 0, s>>>(*a, ControlView{});
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
@@ -207,8 +213,9 @@ int variance_head(const fs2_variance_head_args* a, cudaStream_t s) {
 // ------------------------------------------------------------------ durations (modules.py:132-135, :185-187)
 // One CTA per utterance: round-half-even (rintf == torch.round), truncate, block-wide inclusive scan.
 // RAG: ragged batch, columns l >= src_lens[b] do not exist: they are not read, count as 0 frames and d_rounded there is 0.
-template <bool RAG>
-__global__ void durations_kernel(const fs2_durations_args a, const int* __restrict__ src_lens) {
+// CTL: the per-element control ctl scales the rounded durations in place of the scalar a.d_control (predicted durations only).
+template <bool RAG, bool CTL>
+__global__ void durations_kernel(const fs2_durations_args a, const int* __restrict__ src_lens, const ControlView ctl) {
   __shared__ int warp_tot[32];
   __shared__ int carry_s;
   const int b = blockIdx.x;
@@ -228,7 +235,8 @@ __global__ void durations_kernel(const fs2_durations_args a, const int* __restri
       if (a.use_target) {
         d = s;
       } else {
-        d = fmaxf(rintf(expf(s) - 1.f) * a.d_control, 0.f);
+        const float dc = CTL ? __ldg(ctl.v + b * ctl.sb + l * ctl.sl) : a.d_control;
+        d = fmaxf(rintf(expf(s) - 1.f) * dc, 0.f);
         if (a.d_rounded) a.d_rounded[(long long)b * a.L + l] = d;
       }
       // int() truncation toward zero.  A NaN / inf / absurd duration (the reference raises on int(inf) or dies allocating) is counted
@@ -271,12 +279,19 @@ __global__ void durations_kernel(const fs2_durations_args a, const int* __restri
   }
 }
 
-int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens) {
+// src_lens: the ragged mode's lengths or NULL.  ctl: NULL or ctl->v NULL for the scalar a->d_control; ignored with use_target.
+int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens, const ControlView* ctl) {
   if (!a || !a->src || !a->cum || !a->mel_lens || !a->len_stats || a->B <= 0 || a->L <= 0) return FS2_ERR_ARG;
   cudaError_t e = cudaMemsetAsync(a->len_stats, 0, 3 * sizeof(int), s);
   if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
-  if (src_lens) durations_kernel<true><<<a->B, 256, 0, s>>>(*a, src_lens);
-  else durations_kernel<false><<<a->B, 256, 0, s>>>(*a, nullptr);
+  const ControlView c = (ctl && !a->use_target) ? *ctl : ControlView{};
+  if (c.v) {
+    if (src_lens) durations_kernel<true, true><<<a->B, 256, 0, s>>>(*a, src_lens, c);
+    else durations_kernel<false, true><<<a->B, 256, 0, s>>>(*a, nullptr, c);
+  } else {
+    if (src_lens) durations_kernel<true, false><<<a->B, 256, 0, s>>>(*a, src_lens, c);
+    else durations_kernel<false, false><<<a->B, 256, 0, s>>>(*a, nullptr, c);
+  }
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

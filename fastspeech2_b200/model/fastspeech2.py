@@ -16,6 +16,42 @@ from .._modtree import get, populate
 from ..spec import fastspeech2_spec, read_dataset_files
 from ..synth import sinusoid_table
 
+_UNREAD_CONTROL = (None, 1.0, (0, 0))
+
+
+def normalize_control(control, shape, device, name="control"):
+    """A p_control / d_control argument as the C ABI takes it (fs2_control_args), for the prediction of `shape` ([B, L] phonemes or
+    [B, T] frames) that it scales as the reference's `prediction * control` does (model/modules.py:85,96,134).  Returns
+    (tensor, scalar, strides):
+      * a Python number or a one-element tensor: (None, float(control), (0, 0)), the scalar path;
+      * any other tensor: (an fp32 view on `device` broadcast to `shape`, 1.0, its two element strides).  Dimensions the tensor
+        broadcasts along (size 1, or stride 0 in an expanded view) get stride 0: the values are converted, never materialised.
+    Raises ValueError for a tensor that does not broadcast to `shape` (the reference raises too) or that would grow it, e.g.
+    [B, L, 1] (torch.broadcast_shapes(control.shape, shape) != shape; the reference would silently grow every later tensor)."""
+    if not torch.is_tensor(control) or control.numel() == 1:
+        return None, float(control), (0, 0)
+    shape = torch.Size(shape)
+    if control.is_complex():
+        raise ValueError(f"{name} must be real, got {control.dtype}")
+    try:
+        full = torch.broadcast_shapes(control.shape, shape)
+    except RuntimeError as e:
+        raise ValueError(f"{name} of shape {tuple(control.shape)} does not broadcast to the prediction's shape {tuple(shape)}") from e
+    if full != shape:
+        raise ValueError(f"{name} of shape {tuple(control.shape)} would grow the prediction's shape {tuple(shape)} to {tuple(full)}")
+    compact = control[tuple(slice(0, 1) if st == 0 else slice(None) for st in control.stride())]
+    view = compact.to(device=device, dtype=torch.float32).broadcast_to(shape)
+    return view, 1.0, tuple(view.stride())
+
+
+def _control_args(p, d):
+    c = L.ControlArgs()
+    if p[0] is not None:
+        c.p, (c.p_stride_b, c.p_stride_l) = p[0].data_ptr(), p[2]
+    if d[0] is not None:
+        c.d, (c.d_stride_b, c.d_stride_l) = d[0].data_ptr(), d[2]
+    return c
+
 
 class FastSpeech2(nn.Module):
     """FastSpeech2 acoustic model, H100-native forward.
@@ -170,7 +206,19 @@ class FastSpeech2(nn.Module):
     @torch.no_grad()
     def forward(self, speakers, texts, src_lens, max_src_len, mels=None, mel_lens=None, max_mel_len=None,
                 p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0, ragged=None):
-        """The reference's forward; `ragged` (None: the module's `ragged` attribute) selects the ragged mode described in __init__."""
+        """The reference's forward; `ragged` (None: the module's `ragged` attribute) selects the ragged mode described in __init__.
+
+        Controls, as the reference applies them (model/modules.py:85,96,132-135): a Python number, or a tensor of any real dtype on any
+        device that broadcasts, under torch rules, to the prediction it scales -- p_control to the pitch AND energy predictions
+        ([B, L]; [B, T] for frame-level predictors), d_control to the durations ([B, L]).  So [B, 1] is one value per utterance and
+        [B, L] one per phoneme.  A 1-D control of length n is per COLUMN, exactly as in the reference: [B] is not per utterance (it
+        raises unless B == L, and then scales phonemes).  A control that does not broadcast, or that would grow the prediction (e.g.
+        [B, L, 1]), raises ValueError before the phase that uses it is launched.  Controls the reference never reads are accepted
+        whatever they are: e_control always (model/modules.py:124), p_control when every predictor it scales is given its target,
+        d_control with d_targets.  Tensor values are rounded to fp32 on the model's device without a host synchronisation; the one
+        deviation from the reference is a float64 control, which the reference would let promote the prediction to float64.  Ragged
+        mode: utterance b equals its solo call with c[b] ([B, 1]) or c[b:b+1, :src_lens[b]] ([B, L]), and control columns beyond an
+        utterance's length are never read."""
         # the C ABI sets up per-device kernel attributes for the CURRENT device: make the model's device current
         dev = get(self, "mel_linear.weight").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
@@ -209,19 +257,24 @@ class FastSpeech2(nn.Module):
             self._stats_host = torch.zeros(3, dtype=torch.int32).pin_memory()
         tgt = lambda t: None if t is None else t.to(**f32).contiguous()
         p_t, e_t, d_t = tgt(p_targets), tgt(e_targets), tgt(d_targets)
+        # p_control scales the predictors without a target; e_control is never read (model/modules.py:124)
+        p_read_enc = (not p_frame and p_t is None) or (not e_frame and e_t is None)
+        p_read_dec = (p_frame and p_t is None) or (e_frame and e_t is None)
+        p_enc = normalize_control(p_control, (B, Lmax), dev, "p_control") if p_read_enc else _UNREAD_CONTROL
+        d_ctl = normalize_control(d_control, (B, Lmax), dev, "d_control") if d_t is None else _UNREAD_CONTROL
 
         m.enc_pos, m.enc_pos_rows = self._position(0, Lmax, m.d_model, dev)
         ws_bytes = lib.fs2_encode_workspace_bytes(C.byref(m), B, Lmax)
         ws = self._workspace(ws_bytes, dev)
         ea = L.EncodeArgs(B=B, L=Lmax, texts=texts.data_ptr(), speakers=L.ptr(speakers_d), src_lens=src_lens32.data_ptr(),
-                          p_control=float(p_control), e_control=float(e_control), d_control=float(d_control),
+                          p_control=p_enc[1], e_control=1.0, d_control=d_ctl[1],
                           p_target=0 if p_frame else L.ptr(p_t), e_target=0 if e_frame else L.ptr(e_t), d_target=L.ptr(d_t),
                           p_pred=0 if p_frame else p_pred.data_ptr(), e_pred=0 if e_frame else e_pred.data_ptr(), logd_pred=logd.data_ptr(),
                           d_rounded=d_rounded.data_ptr(), mel_lens=mel_lens_out.data_ptr(), mel_lens32=mel_lens32.data_ptr(),
                           cum_dur=cum.data_ptr(), x_adapted=x_adapted.data_ptr(), len_stats=stats_dev.data_ptr(),
                           len_stats_host=self._stats_host.data_ptr(), workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        encode = lib.fs2_acoustic_encode_ragged if ragged else lib.fs2_acoustic_encode
-        L.check(encode(C.byref(m), C.byref(ea), stream), "fs2_acoustic_encode")
+        ctl = _control_args(p_enc, d_ctl)
+        L.check(lib.fs2_acoustic_encode_ctl(C.byref(m), C.byref(ea), C.byref(ctl), int(ragged), stream), "fs2_acoustic_encode")
 
         if max_mel_len is not None:
             T = int(max_mel_len)
@@ -250,16 +303,17 @@ class FastSpeech2(nn.Module):
             e_pred = torch.empty(B, T, **f32)
             if e_t is not None and tuple(e_t.shape) != (B, T):
                 raise ValueError("frame-level e_targets must be [B, max_mel_len]")
+        p_dec = normalize_control(p_control, (B, T), dev, "p_control") if p_read_dec else _UNREAD_CONTROL
         ws_bytes = lib.fs2_decode_workspace_bytes(C.byref(m), B, T)
         ws = self._workspace(ws_bytes, dev)
         da = L.DecodeArgs(B=B, L=Lmax, T=T, x_adapted=x_adapted.data_ptr(), cum_dur=cum.data_ptr(),
-                          mel_mask_lens=mask_lens32.data_ptr(), p_control=float(p_control),
+                          mel_mask_lens=mask_lens32.data_ptr(), p_control=p_dec[1],
                           p_target_frames=L.ptr(p_t) if p_frame else 0, e_target_frames=L.ptr(e_t) if e_frame else 0,
                           p_pred_frames=p_pred.data_ptr() if p_frame else 0, e_pred_frames=e_pred.data_ptr() if e_frame else 0,
                           mel=mel.data_ptr(), postnet_mel=post.data_ptr(),
                           workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        decode = lib.fs2_acoustic_decode_ragged if ragged else lib.fs2_acoustic_decode
-        L.check(decode(C.byref(m), C.byref(da), stream), "fs2_acoustic_decode")
+        ctl = _control_args(p_dec, _UNREAD_CONTROL)
+        L.check(lib.fs2_acoustic_decode_ctl(C.byref(m), C.byref(da), C.byref(ctl), int(ragged), stream), "fs2_acoustic_decode")
 
         src_masks = torch.arange(Lmax, device=dev)[None, :] >= src_lens32[:, None]
         mel_masks = torch.arange(T, device=dev)[None, :] >= mask_lens32[:, None]

@@ -355,6 +355,26 @@ int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, f
 int fs2_acoustic_encode_ragged(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t stream);
 int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t stream);
 
+/* Per-utterance / per-phoneme controls (model/modules.py:85,96,132-135 broadcast `prediction * control`): device fp32 arrays that
+ * replace the scalar p_control / d_control of the phase's args where their pointer is set.  Strides are in elements, >= 0 (0 along a
+ * broadcast dimension; a negative stride is FS2_ERR_ARG).  48 bytes; the binding pins that size (it is not in fs2_struct_size).
+ *   p: pitch AND energy (modules.py:124), c[b, l] with l = phoneme (encode: [B][L] predictions) or frame (decode: frame-level
+ *      predictions on [B][T]); not read where the predictor is given its target.
+ *   d: durations, encode only, c[b, l] scales round(exp(logd) - 1) before the clamp and int() truncation; not read with d_target. */
+typedef struct fs2_control_args {
+  const float* p; int64_t p_stride_b, p_stride_l;
+  const float* d; int64_t d_stride_b, d_stride_l;
+} fs2_control_args;
+/* fs2_acoustic_{encode,decode} (ragged = 0) and fs2_acoustic_{encode,decode}_ragged (ragged = 1; other values: FS2_ERR_ARG) with
+ * controls.  ctl == NULL, or both pointers NULL: exactly the call without controls (those four entry points are this call).  In ragged
+ * mode utterance b with its slice of the controls equals its B = 1 call with c[b:b+1, :src_lens[b]] (frames: :mel_mask_lens[b]), and
+ * control columns at or beyond src_lens[b] (frames at or beyond mel_mask_lens[b]) are never read.  A control array holding fp32(c)
+ * gives the scalar c's results bit for bit.  Same workspace sizes as the calls without controls. */
+int fs2_acoustic_encode_ctl(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged,
+                            fs2_stream_t stream);
+int fs2_acoustic_decode_ctl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged,
+                            fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ vocoder (hifigan Generator.forward) */
 
 typedef struct fs2_vocoder_model {

@@ -46,6 +46,9 @@ HIFIGAN_CONFIG = {
     "num_mels": 80, "hop_size": 256, "sampling_rate": 22050,
 }
 
+# HiFi-GAN V2: V1 with upsample_initial_channel 128, so its stages are 64, 32, 16 and 8 channels wide (0.93 M parameters)
+HIFIGAN_V2_CONFIG = dict(HIFIGAN_CONFIG, upsample_initial_channel=128)
+
 
 def make_configs(dataset: str, scratch_dir: str):
     """Return (preprocess_config, model_config) and materialise stats.json / speakers.json."""

@@ -7,7 +7,8 @@
 //
 // Tiling: CTA = 128 (or 64, for small problems) rows (time) x BN output channels, BK = 16, 256 threads, TM x TN register tile per thread,
 // A tile transposed into smem so the inner product reads two broadcast float4 (A) and two conflict-free float4 (B)
-// per 64 FMAs; global->register->smem double buffering, one __syncthreads per k-step.
+// per 64 FMAs; global->register->smem double buffering, one __syncthreads per k-step.  Cin = 8 (HiFi-GAN V2's last stage): one k-step
+// per tap whose upper 8 channels load as zeros, so the sums gain only exact zeros.
 #include "common.cuh"
 
 namespace fs2 {
@@ -53,7 +54,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   if (t0 >= tend) return;
 
   const float* xb = p.x + (long long)b * p.xbs;
-  const int kc = p.Cin / BK;               // k-steps per tap
+  const int kc = (p.Cin + BK - 1) / BK;    // k-steps per tap
   const int KT = p.taps * kc;
 
   float acc[TM][NG * GW];
@@ -75,7 +76,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
       const int row = f >> 2, c4 = f & 3;
       const int t = t0 + row + shift;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (t >= 0 && t < tend) {
+      if (t >= 0 && t < tend && c0 + c4 * 4 < p.Cin) {
         v = __ldg(reinterpret_cast<const float4*>(xb + (long long)t * p.xrs + c0 + c4 * 4));
         if (p.in_act == FS2_ACT_LRELU) {
           v.x = v.x > 0.f ? v.x : v.x * p.in_slope;
@@ -94,7 +95,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
       if (f < B_F4) {
         const int k = f / (BN / 4), n4 = f % (BN / 4);
         const int n = n0 + n4 * 4;
-        if (n < p.N) v = __ldg(reinterpret_cast<const float4*>(wt + (long long)k * p.N + n));
+        if (n < p.N && c0 + k < p.Cin) v = __ldg(reinterpret_cast<const float4*>(wt + (long long)k * p.N + n));
       }
       rb[i] = v;
     }
@@ -196,7 +197,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out) {
   if (!a || !out || num_sms <= 0) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
-  if (a->Cin % BK != 0 || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
+  if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
   // 128-row tiles by default; 64-row tiles when the grid would not even give every SM two CTAs (encoder / predictors: 2048 rows)
   const int nblk = a->N > 64 ? (a->N + 127) / 128 : 1;
   const bool small = (long long)((a->T + 127) / 128) * a->B * nblk < 2LL * num_sms;
@@ -214,7 +215,7 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* 
 int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
-  if (a->Cin % BK != 0 || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
+  if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
   if ((a->x_row_stride & 3) || (a->x_batch_stride & 3) || (a->y_row_stride & 3) || (a->y_batch_stride & 3)) return FS2_ERR_UNSUPPORTED;
   if (a->res && ((a->res_row_stride & 3) || (a->res_batch_stride & 3))) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;

@@ -412,6 +412,8 @@ static fs2_resstack_args resblock_pair(const fs2_resstack_args& g, int j, int d)
   return a;
 }
 
+static bool resstack_width(int C) { return C == 8 || C == 16 || C == 32 || C == 64; }   // the channel counts fs2_resstack serves
+
 static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, cudaStream_t s, Arena& ar) {
   const int B = a->B, T = a->T;
   size_t per_frame = (size_t)m->c0;  // floats per mel frame of the widest activation
@@ -476,7 +478,7 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
     for (int j = 0; j < m->n_kernels; j++) {
       const int rb = i * m->n_kernels + j, k = m->rb_k[j];
       const float* r = bu;
-      const bool pairs = ((m->pair_mask >> i) & 1) && tcv && (C == 32 || C == 64) && k <= m->pair_kmax;
+      const bool pairs = ((m->pair_mask >> i) & 1) && tcv && resstack_width(C) && k <= m->pair_kmax;
       for (int d = 0; d < m->n_dil; d++) {
         const bool last = d == m->n_dil - 1;            // the last layer adds its share of the mean over the n_kernels ResBlocks into bx
         float* dst = last ? bx : (r == r1 ? r2 : r1);

@@ -24,6 +24,9 @@
 //     rows outside [0, N) are zero-filled by the hardware = the conv's zero padding, and there is no bleed between utterances)
 //     into XT while it is idle; the result leaves as boxes staged in XA with a TMA store (first kernel size) or TMA reduce-add
 //     (the others: the mean over kernel sizes accumulates in L2).  HBM sees x once per kernel size and y once.
+//   * widths: resstack_kernel<32, MT = 4> and <64, 2>; resstack_narrow_kernel<16> and <8> run the same body at MT = 8 (MT * C = 128
+//     throughout), with [128 rows][C] unswizzled boxes for rows narrower than 128 bytes; 8 channels are computed as 16 whose upper 8
+//     are zeros (the weights: the conv's f8 tiles zero-padded to 16 x 16).
 //
 // Roles: warps 0-7 two consumer warpgroups (conversion, MMAs, epilogues; thread 0 issues the tensor-map copies), warp 8 weight producer.
 #include <cuda.h>
@@ -75,6 +78,12 @@ __device__ __forceinline__ void tma_wait_reads() { asm volatile("cp.async.bulk.w
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // both consumer warpgroups
 // byte offset of 16-byte chunk c of row r inside a [rows][128 B] box written / read by TMA with CU_TENSOR_MAP_SWIZZLE_128B
 __device__ __forceinline__ uint32_t sw128(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
+// byte offset of channel c (even) of row r inside a box of BOXC-channel fp32 rows: 128-byte swizzled (SW, BOXC = 32) or plain
+template <bool SW, int BOXC>
+__device__ __forceinline__ uint32_t rs_box_off(int r, int c) {
+  if constexpr (SW) return sw128(r, (c & 31) >> 2) + (c & 3) * 4;
+  return (uint32_t)(r * BOXC * 4 + (c % BOXC) * 4);
+}
 
 __device__ __forceinline__ float rs_lrelu(float v) { return fmaxf(v, 0.1f * v); }   // LRELU_SLOPE = 0.1 (hifigan/models.py:7)
 
@@ -90,15 +99,21 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
   *reinterpret_cast<unsigned short*>(kblk + 3 * chunk_bytes + cc) = (unsigned short)h8;
 }
 
-// RAG: ragged batch (RsP::lens != NULL), see WorkList.
-template <int C, int MT, bool RAG>
-__global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmy,
-                                                                 const RsP p) {
-  constexpr int KB = C / 16, R = MT * 128, NH = C / 32, NJ = C / 8;   // NJ: 8-column fragment groups of a row
+// The body of both kernels.  CG: channels of x and y in global memory; C: channels computed on chip, CG itself, or 16 for CG = 8 (the
+// weights are then the 16 x 16 zero-padded tiles, and channels CG..C-1 are held at exact zero in both slabs).  Global rows of 128 bytes
+// or more travel as [128 rows][32 channels] boxes with the 128-byte swizzle; narrower rows (CG = 16: 64 B, CG = 8: 32 B) as one
+// unswizzled [rows][CG] box per 128 rows.  RAG: ragged batch (RsP::lens != NULL), see WorkList.
+template <int CG, int C, int MT, bool RAG>
+__device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUtensorMap& tmy, const RsP& p) {
+  constexpr int KB = C / 16, R = MT * 128, NJ = C / 8;                // NJ: 8-column fragment groups of a row
+  constexpr int BOXC = CG < 32 ? CG : 32, NH = CG / BOXC;             // channels per TMA box, boxes across a row
+  constexpr bool SW = BOXC == 32;                                     // 128-byte box rows: swizzled
   constexpr uint32_t CHUNK = (uint32_t)R * 16, PLANE = 2 * CHUNK, KBLK = 2 * PLANE, SLAB = KB * KBLK;
   constexpr uint32_t WSTAGE = 64u * C;
-  constexpr uint32_t XBOX = 128 * 128;                                 // bytes of one input box [128 rows][32 ch] fp32
-  static_assert(SLAB == (uint32_t)R * C * 4, "an operand slab has exactly the size of the fp32 tile it is built from");
+  constexpr uint32_t XBOX = 128 * BOXC * 4;                           // bytes of one input box [128 rows][BOXC ch] fp32
+  static_assert(CG == C || (CG == 8 && C == 16), "only the 8-channel width is zero-padded on chip");
+  static_assert(C % 16 == 0 && SLAB >= (uint32_t)R * CG * 4, "the fp32 tile lands in an operand slab");
+  static_assert(CG != C || SLAB == (uint32_t)R * C * 4, "an operand slab has exactly the size of the fp32 tile it is built from");
   static_assert(MT * (C / 2) * 256 * 4 == SLAB, "the residual stream has the size of a slab");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = warp_uniform_id(), lane = tid & 31;
@@ -168,7 +183,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
         if (stores_pending) tma_wait_reads();           // previous result boxes have been read out of XA
         mbar_expect_tx(xLoaded, (uint32_t)(MT * NH) * XBOX);
         for (int hh = 0; hh < NH; hh++)
-          for (int m = 0; m < MT; m++) tma_load_3d(xt + (size_t)(hh * MT + m) * XBOX, &tmx, hh * 32, t0 - p.H + m * 128, b, xLoaded);
+          for (int m = 0; m < MT; m++) tma_load_3d(xt + (size_t)(hh * MT + m) * XBOX, &tmx, hh * BOXC, t0 - p.H + m * 128, b, xLoaded);
       }
       stores_pending = true;
       consumers_sync();                                 // XA is free
@@ -181,7 +196,8 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
 #pragma unroll
           for (int jj = 0; jj < NJ; jj++) {
             const int c = cbase + 8 * jj;
-            float2 u = *reinterpret_cast<const float2*>(xt + (size_t)((c >> 5) * MT + m) * XBOX + sw128(r128, (c & 31) >> 2) + (c & 3) * 4);
+            if (8 * jj >= CG) { rs_store2(xa, CHUNK, row, c, 0.f, 0.f); continue; }   // zero-padded channels
+            float2 u = *reinterpret_cast<const float2*>(xt + (size_t)((c / BOXC) * MT + m) * XBOX + rs_box_off<SW, BOXC>(r128, c));
             if (RAG && t0 - p.H + row >= nrows) u = make_float2(0.f, 0.f);   // the padding of a ragged batch reads as zero
             xr(i, 4 * jj + 2 * h) = u.x;
             xr(i, 4 * jj + 2 * h + 1) = u.y;
@@ -223,10 +239,10 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
           for (int i = 0; i < MT; i++) { wgmma_keep<C>(acc[i]); wgmma_keep<C>(corr[i]); }
           // ---- epilogue straight from the fragments
           const float inv_s = __ldg(reinterpret_cast<const float*>(cv.w));
-#pragma unroll
-          for (int jj = 0; jj < NJ; jj++) {
-            const int c = cbase + 8 * jj;
-            const float2 bv = __ldg(reinterpret_cast<const float2*>(cv.b + c));
+          // The same epilogue in two loop orders.  MT = 8 (the narrow widths) walks rows outer: with column groups outer, the 16 rows'
+          // addresses and predicates stay live across both groups and push per-item state out of the 168 registers (stack spills).  The
+          // wide widths keep column groups outer, the order their register allocation was tuned in.
+          if constexpr (MT == 8) {
 #pragma unroll
             for (int i = 0; i < MT; i++)
 #pragma unroll
@@ -234,25 +250,71 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
                 const int row = rbase + 64 * i + 8 * h;
                 const int gr = t0 - p.H + row;
                 const bool in = gr >= 0 && gr < nrows;
-                const float s0 = acc[i][4 * jj + 2 * h] + corr[i][4 * jj + 2 * h], s1 = acc[i][4 * jj + 2 * h + 1] + corr[i][4 * jj + 2 * h + 1];
-                float v0 = fmaf(s0, inv_s, bv.x), v1 = fmaf(s1, inv_s, bv.y);
-                if (c2 == 0) {
-                  // conv1: lrelu -> conv2's operand slab
-                  rs_store2(xt, CHUNK, row, c, in ? rs_lrelu(v0) : 0.f, in ? rs_lrelu(v1) : 0.f);
-                } else {
-                  v0 += xr(i, 4 * jj + 2 * h); v1 += xr(i, 4 * jj + 2 * h + 1);   // + residual
-                  if (!last) {
-                    xr(i, 4 * jj + 2 * h) = v0; xr(i, 4 * jj + 2 * h + 1) = v1;
-                    rs_store2(xa, CHUNK, row, c, in ? rs_lrelu(v0) : 0.f, in ? rs_lrelu(v1) : 0.f);
-                  } else if (row >= p.H && row < p.H + p.TILE) {
-                    // result of this kernel size, alpha * x (mean over kernel sizes, models.py:154-160), staged in XA (idle since conv1
-                    // of this pair has retired) as swizzled [OBOX rows][32 channels] boxes for the TMA store / reduce-add
-                    const int ro = row - p.H, bx = ro / p.OBOX, rb_ = ro - bx * p.OBOX;
-                    unsigned char* obox = xa + (size_t)((c >> 5) * p.n_oboxes + bx) * ((size_t)p.OBOX * 128);
-                    *reinterpret_cast<float2*>(obox + sw128(rb_, (c & 31) >> 2) + (c & 3) * 4) = make_float2(v0 * p.alpha, v1 * p.alpha);
+#pragma unroll
+                for (int jj = 0; jj < NJ; jj++) {
+                  const int c = cbase + 8 * jj;
+                  if (8 * jj >= CG) {
+                    if (c2 == 0 || !last) rs_store2(c2 == 0 ? xt : xa, CHUNK, row, c, 0.f, 0.f);
+                    continue;
+                  }
+                  const float2 bv = __ldg(reinterpret_cast<const float2*>(cv.b + c));
+                  const float s0 = acc[i][4 * jj + 2 * h] + corr[i][4 * jj + 2 * h], s1 = acc[i][4 * jj + 2 * h + 1] + corr[i][4 * jj + 2 * h + 1];
+                  float v0 = fmaf(s0, inv_s, bv.x), v1 = fmaf(s1, inv_s, bv.y);
+                  if (c2 == 0) {
+                    rs_store2(xt, CHUNK, row, c, in ? rs_lrelu(v0) : 0.f, in ? rs_lrelu(v1) : 0.f);
+                  } else {
+                    v0 += xr(i, 4 * jj + 2 * h); v1 += xr(i, 4 * jj + 2 * h + 1);
+                    if (!last) {
+                      xr(i, 4 * jj + 2 * h) = v0; xr(i, 4 * jj + 2 * h + 1) = v1;
+                      rs_store2(xa, CHUNK, row, c, in ? rs_lrelu(v0) : 0.f, in ? rs_lrelu(v1) : 0.f);
+                    } else if (row >= p.H && row < p.H + p.TILE) {
+                      const int ro = row - p.H, bx = ro / p.OBOX, rb_ = ro - bx * p.OBOX;
+                      unsigned char* obox = xa + (size_t)((c / BOXC) * p.n_oboxes + bx) * ((size_t)p.OBOX * BOXC * 4);
+                      *reinterpret_cast<float2*>(obox + rs_box_off<SW, BOXC>(rb_, c)) = make_float2(v0 * p.alpha, v1 * p.alpha);
+                    }
                   }
                 }
               }
+          } else {
+#pragma unroll
+            for (int jj = 0; jj < NJ; jj++) {
+              const int c = cbase + 8 * jj;
+              if (8 * jj >= CG) {                         // zero-padded channels: exact zeros into the operand slabs, nothing to y
+                if (c2 == 0 || !last)
+#pragma unroll
+                  for (int i = 0; i < MT; i++)
+#pragma unroll
+                    for (int h = 0; h < 2; h++) rs_store2(c2 == 0 ? xt : xa, CHUNK, rbase + 64 * i + 8 * h, c, 0.f, 0.f);
+                continue;
+              }
+              const float2 bv = __ldg(reinterpret_cast<const float2*>(cv.b + c));
+#pragma unroll
+              for (int i = 0; i < MT; i++)
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                  const int row = rbase + 64 * i + 8 * h;
+                  const int gr = t0 - p.H + row;
+                  const bool in = gr >= 0 && gr < nrows;
+                  const float s0 = acc[i][4 * jj + 2 * h] + corr[i][4 * jj + 2 * h], s1 = acc[i][4 * jj + 2 * h + 1] + corr[i][4 * jj + 2 * h + 1];
+                  float v0 = fmaf(s0, inv_s, bv.x), v1 = fmaf(s1, inv_s, bv.y);
+                  if (c2 == 0) {
+                    // conv1: lrelu -> conv2's operand slab
+                    rs_store2(xt, CHUNK, row, c, in ? rs_lrelu(v0) : 0.f, in ? rs_lrelu(v1) : 0.f);
+                  } else {
+                    v0 += xr(i, 4 * jj + 2 * h); v1 += xr(i, 4 * jj + 2 * h + 1);   // + residual
+                    if (!last) {
+                      xr(i, 4 * jj + 2 * h) = v0; xr(i, 4 * jj + 2 * h + 1) = v1;
+                      rs_store2(xa, CHUNK, row, c, in ? rs_lrelu(v0) : 0.f, in ? rs_lrelu(v1) : 0.f);
+                    } else if (row >= p.H && row < p.H + p.TILE) {
+                      // result of this kernel size, alpha * x (mean over kernel sizes, models.py:154-160), staged in XA (idle since conv1
+                      // of this pair has retired) as [OBOX rows][BOXC channels] boxes for the TMA store / reduce-add
+                      const int ro = row - p.H, bx = ro / p.OBOX, rb_ = ro - bx * p.OBOX;
+                      unsigned char* obox = xa + (size_t)((c / BOXC) * p.n_oboxes + bx) * ((size_t)p.OBOX * BOXC * 4);
+                      *reinterpret_cast<float2*>(obox + rs_box_off<SW, BOXC>(rb_, c)) = make_float2(v0 * p.alpha, v1 * p.alpha);
+                    }
+                  }
+                }
+            }
           }
           fence_proxy_async();
           consumers_sync();                             // the next conv's taps read rows of both warpgroups
@@ -264,15 +326,28 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_co
         tma_wait_all();   // the previous kernel size's boxes are complete in L2 before this one's reduce-add
         for (int hh = 0; hh < NH; hh++)
           for (int bx = 0; bx < p.n_oboxes; bx++) {
-            const unsigned char* src = xa + (size_t)(hh * p.n_oboxes + bx) * ((size_t)p.OBOX * 128);
-            if (j == 0 && !p.accumulate) tma_store_3d(&tmy, hh * 32, t0 + bx * p.OBOX, b, src);
-            else tma_reduce_add_3d(&tmy, hh * 32, t0 + bx * p.OBOX, b, src);
+            const unsigned char* src = xa + (size_t)(hh * p.n_oboxes + bx) * ((size_t)p.OBOX * BOXC * 4);
+            if (j == 0 && !p.accumulate) tma_store_3d(&tmy, hh * BOXC, t0 + bx * p.OBOX, b, src);
+            else tma_reduce_add_3d(&tmy, hh * BOXC, t0 + bx * p.OBOX, b, src);
           }
         tma_commit();
       }
     }
   }
   if (io) tma_wait_all();
+}
+
+template <int C, int MT, bool RAG>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmy,
+                                                                 const RsP p) {
+  resstack_body<C, C, MT, RAG>(tmx, tmy, p);
+}
+
+// The 16- and 8-channel stages: MT = 8 keeps MT * C = 128 (the accumulator, slab and residual-stream budgets of the wide kernels).
+template <int CG, bool RAG>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                        const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<CG, 16, 8, RAG>(tmx, tmy, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -284,7 +359,8 @@ static size_t rs_smem_bytes(int C, int MT, int SB, int TPS) {
 // Launch plan (pure host logic, fs2_resstack_plan_t in fs2b200.h)
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out) {
   if (!a || a->B <= 0 || a->N <= 0 || num_sms <= 0) return FS2_ERR_ARG;
-  if (a->C != 32 && a->C != 64) return FS2_ERR_UNSUPPORTED;
+  if (a->C != 8 && a->C != 16 && a->C != 32 && a->C != 64) return FS2_ERR_UNSUPPORTED;
+  const int Cm = a->C < 16 ? 16 : a->C;         // channels computed on chip (8 is zero-padded to 16)
   if (a->n_kernels <= 0 || a->n_kernels > RS_MAXK || a->n_dil <= 0 || a->n_dil > FS2_MAX_DIL) return FS2_ERR_ARG;
   int H = 0;
   for (int j = 0; j < a->n_kernels; j++) {
@@ -299,8 +375,8 @@ int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& 
     H = hj > H ? hj : H;
   }
   H = (H + 3) & ~3;                             // output boxes are whole swizzle atoms (multiples of 8 rows)
-  // 128-row tiles per slab: the two warpgroups hold MT 64-row blocks each of fp32 main and correction accumulators (MT * C registers)
-  const int MT = a->C == 32 ? 4 : 2;
+  // 128-row tiles per slab: the two warpgroups hold MT 64-row blocks each of fp32 main and correction accumulators (MT * Cm registers)
+  const int MT = 128 / Cm;
   int TILE = 0, obox = 0, n_oboxes = 0;
   // the result leaves as TMA boxes of `obox` rows (a multiple of 8, <= 256) that tile TILE exactly: widen the halo by up to 32 rows
   // until TILE splits into at most 12 boxes (e.g. 384 - 2*4 = 376 = 47 x 8 would need 47 stores; 384 - 2*8 = 368 = 2 x 184)
@@ -314,12 +390,12 @@ int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& 
   n_oboxes = TILE / obox;
   const long long tiles_per_b = (a->N + TILE - 1) / TILE, items = tiles_per_b * a->B;
   if (items > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
-  const int TPS = a->C == 32 ? 4 : 2;           // taps per weight stage: 8 KB stages (fewer handshakes per MMA; conv_tc measured -10..-25 %)
+  const int TPS = 128 / Cm;                     // taps per weight stage: 8 KB stages (fewer handshakes per MMA; conv_tc measured -10..-25 %)
   int SB = 8;
-  while (SB > 2 && rs_smem_bytes(a->C, MT, SB, TPS) > 227 * 1024) SB--;
-  if (rs_smem_bytes(a->C, MT, SB, TPS) > 227 * 1024) return FS2_ERR_UNSUPPORTED;
+  while (SB > 2 && rs_smem_bytes(Cm, MT, SB, TPS) > 227 * 1024) SB--;
+  if (rs_smem_bytes(Cm, MT, SB, TPS) > 227 * 1024) return FS2_ERR_UNSUPPORTED;
   out.MT = MT; out.H = H; out.TILE = TILE; out.n_items = (int)items; out.grid = items < num_sms ? (int)items : num_sms; out.SB = SB;
-  out.smem = (int)rs_smem_bytes(a->C, MT, SB, TPS); out.acc_regs = MT * a->C; out.OBOX = obox; out.n_oboxes = n_oboxes; out.TPS = TPS;
+  out.smem = (int)rs_smem_bytes(Cm, MT, SB, TPS); out.acc_regs = MT * Cm; out.OBOX = obox; out.n_oboxes = n_oboxes; out.TPS = TPS;
   return FS2_OK;
 }
 
@@ -336,16 +412,17 @@ static EncodeTiledFn encode_tiled_fn() {
   }
   return reinterpret_cast<EncodeTiledFn>(f);
 }
-// fp32 [B][N][C] contiguous as a rank-3 map, boxes of [1][rows][32 channels] with the 128-byte swizzle, zero fill outside the tensor
+// fp32 [B][N][C] contiguous as a rank-3 map, zero fill outside the tensor: boxes of [1][rows][32 channels] with the 128-byte swizzle,
+// or of [1][rows][C] unswizzled for C < 32 (resstack_body's box layouts)
 static int make_map(CUtensorMap* tm, const float* base, int B, int N, int C, int box_rows) {
   EncodeTiledFn enc = encode_tiled_fn();
   if (!enc) return FS2_ERR_UNSUPPORTED;
   const cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)N, (cuuint64_t)B};
   const cuuint64_t strides[2] = {(cuuint64_t)C * 4, (cuuint64_t)N * C * 4};
-  const cuuint32_t box[3] = {32, (cuuint32_t)box_rows, 1};
+  const cuuint32_t box[3] = {(cuuint32_t)(C < 32 ? C : 32), (cuuint32_t)box_rows, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         C < 32 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? FS2_OK : FS2_ERR_CUDA - 1;
 }
 
@@ -370,6 +447,10 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<32, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_kernel<64, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     return e;
   }));
   RsP p{};
@@ -394,9 +475,15 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
   if (a->C == 32) {
     if (a->lens) resstack_kernel<32, 4, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_kernel<32, 4, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
-  } else {
+  } else if (a->C == 64) {
     if (a->lens) resstack_kernel<64, 2, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_kernel<64, 2, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+  } else if (a->C == 16) {
+    if (a->lens) resstack_narrow_kernel<16, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_narrow_kernel<16, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+  } else {
+    if (a->lens) resstack_narrow_kernel<8, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_narrow_kernel<8, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   }
   prof_after(s, 0, flops);
   FS2_LAUNCH_CHECK();

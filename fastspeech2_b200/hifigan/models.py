@@ -1,4 +1,4 @@
-"""Drop-in `hifigan.models.Generator` (HiFi-GAN V1 generator): same constructor argument, checkpoint key layout
+"""Drop-in `hifigan.models.Generator` (HiFi-GAN V1 and V2 generators): same constructor argument, checkpoint key layout
 (weight_g / weight_v / bias), `remove_weight_norm()` and `forward(mel[B,80,T]) -> wav[B,1,256*T]` as the reference
 (hifigan/models.py:112-174); forward is hand-written sm_90a CUDA behind fs2_vocoder_forward.  No PyTorch fallback.
 """
@@ -22,14 +22,21 @@ def _cfg(h, name):
     return h[name] if isinstance(h, dict) else getattr(h, name)
 
 
+# Channel counts of the stages whose ResBlock group fs2_resstack runs as one launch
+FUSED_WIDTHS = (8, 16, 32, 64)
+
+
 class Generator(nn.Module):
+    """HiFi-GAN generator for every `resblock: "1"` config the reference's Generator builds: V1 (upsample_initial_channel 512) and
+    V2 (128).  `resblock: "2"` (V3) is not in the reference's Generator and stays NotImplementedError."""
+
     def __init__(self, h):
         super().__init__()
         self.h = h
         self._hd = {k: _cfg(h, k) for k in ("upsample_rates", "upsample_kernel_sizes", "upsample_initial_channel",
                                             "resblock_kernel_sizes", "resblock_dilation_sizes")}
         if str(_cfg(h, "resblock")) != "1":
-            raise NotImplementedError("only resblock type '1' (HiFi-GAN V1, the shipped config) is supported")
+            raise NotImplementedError("only resblock type '1' (HiFi-GAN V1 and V2) is supported")
         self.num_kernels = len(self._hd["resblock_kernel_sizes"])
         self.num_upsamples = len(self._hd["upsample_rates"])
         self._weight_norm = True
@@ -40,13 +47,14 @@ class Generator(nn.Module):
         # waveform bar (tests/test_gpu_model.py::test_hifigan_real_checkpoint_vs_reference; CPU emulation: scripts/emul_split_precision.py).
         self.f8_mask = 0b11110
         # Stages (bit i) whose ResBlock group runs as ONE persistent kernel with every intermediate on chip (fs2_resstack, available for
-        # the 64- and 32-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).  Default: both (on an
-        # H100 SXM at 400 W, bench.py configs[2]: 127 ms per step against 133 ms with the 64-channel stage on per-layer launches and
-        # fused k = 3 pairs).
-        self.fused_mask = 0b1100
+        # the 64-, 32-, 16- and 8-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).  Default: every
+        # stage it serves, 0b1100 for V1 (on an H100 SXM at 400 W, bench.py configs[2]: 127 ms per step against 133 ms with the
+        # 64-channel stage on per-layer launches and fused k = 3 pairs) and 0b1111 for V2.
+        self.fused_mask = self._fusable_stages()
         # Stages (bit i) where every (dilated conv, conv, +x) pair with kernel size <= pair_kmax runs as ONE fs2_resstack launch, so
-        # that the intermediate never leaves the SM.  Only stages outside fused_mask use it: by default none, and with the 64-channel
-        # stage taken out of fused_mask its memory-bound k = 3 pairs.
+        # that the intermediate never leaves the SM.  Only stages outside fused_mask use it: by default none.  Bit 2 is V1's 64-channel
+        # stage (its memory-bound k = 3 pairs when that stage is taken out of fused_mask) and V2's 16-channel stage, so with
+        # fused_mask = 0 V2 still pairs that stage; clear pair_mask too for all-per-layer ResBlocks.
         self.pair_mask = 0b0100
         self.pair_kmax = 3
         populate(self, hifigan_spec(self._hd, weight_norm=True))
@@ -100,17 +108,22 @@ class Generator(nn.Module):
         return out
 
     # ------------------------------------------------------------------ packing
-    def effective_masks(self):
-        """(f8_mask, fused_mask, pair_mask, pair_kmax) as the C ABI receives them (fs2_vocoder_model): fusion only for the 32- and
-        64-channel stages, pairs only outside the fused stages, and every fused or paired stage in the f16 + f8 format.  All zero
-        without tensor cores."""
-        if not self.use_tensor_cores:
-            return 0, 0, 0, 0
-        fused, ch = 0, self._hd["upsample_initial_channel"]
+    def _fusable_stages(self):
+        """Bit i set when stage i's width (upsample_initial_channel / 2^(i+1)) is one fs2_resstack serves."""
+        mask, ch = 0, self._hd["upsample_initial_channel"]
         for i in range(self.num_upsamples):
             ch //= 2
-            if (int(self.fused_mask) >> i) & 1 and ch in (32, 64):
-                fused |= 1 << i
+            if ch in FUSED_WIDTHS:
+                mask |= 1 << i
+        return mask
+
+    def effective_masks(self):
+        """(f8_mask, fused_mask, pair_mask, pair_kmax) as the C ABI receives them (fs2_vocoder_model): fusion only for the
+        stages whose width fs2_resstack serves (FUSED_WIDTHS), pairs only outside the fused stages, and every fused or paired
+        stage in the f16 + f8 format.  All zero without tensor cores."""
+        if not self.use_tensor_cores:
+            return 0, 0, 0, 0
+        fused = int(self.fused_mask) & self._fusable_stages()
         pair = int(self.pair_mask) & ~fused
         return int(self.f8_mask) | (fused << 1) | (pair << 1), fused, pair, int(self.pair_kmax)
 

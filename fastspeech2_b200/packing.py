@@ -96,6 +96,18 @@ def pack_conv_tc(w: Tensor, f8: bool = False, nb: int | None = None):
     return torch.cat([hb, tiles.reshape(-1)])
 
 
+def pack_conv_tc_pad16(w: Tensor):
+    """[taps][8][8] fp32 -> the f16 + f8 tiles of the conv zero-padded to [taps][16][16]: the weights fs2_resstack reads for an
+    8-channel ResBlock group, which it computes as 16 channels whose upper 8 are zero.  The padding leaves max|w|, hence the header
+    scale, unchanged.  None for any other shape."""
+    taps, cin, n = w.shape
+    if cin != 8 or n != 8:
+        return None
+    wp = w.new_zeros(taps, 16, 16)
+    wp[:, :8, :8] = w
+    return pack_conv_tc(wp, f8=True)
+
+
 SEG_CIN = 256          # input channels per K-segment of the encoder / predictor path (16 K-steps of the tensor core)
 
 
@@ -259,5 +271,11 @@ def pack_vocoder(w_of: Callable[[str], Tensor], b_of: Callable[[str], Tensor], r
             return -1
         idx = int(k.split(".")[1])
         return idx if k.startswith("up.") else idx // nk
-    add_tc_tiles(pk, keys, [k for k in keys if f8_mask & (1 << (stage_of(k) + 1))])
+    f8_keys = [k for k in keys if f8_mask & (1 << (stage_of(k) + 1))]
+    add_tc_tiles(pk, keys, f8_keys)
+    for k in f8_keys:                        # 8-channel ResBlock convs: the zero-padded tiles of fs2_resstack (fs2_vocoder_model)
+        if k.startswith("rb.") and k + "_tc" not in pk:
+            t = pack_conv_tc_pad16(pk[k])
+            if t is not None:
+                pk[k + "_tc"] = t
     return pk

@@ -111,7 +111,8 @@ int fs2_conv_simt_plan(const struct fs2_conv1d_args* a, int num_sms, fs2_conv_si
  * rows outside [0,T) read as zero (Conv1d zero padding); rows t >= row_lens[b] are written as exact 0 when row_lens != NULL.
  * Strides are in elements.  Covers nn.Linear (taps=1), nn.Conv1d (any odd k, dilation), and one phase group of
  * ConvTranspose1d (two taps, y_row_stride = u*C_out; see fs2_vocoder_model).
- * Both kernels: Cin % 16 == 0, pointers 16-byte aligned, strides % 4 == 0.  The tensor-core kernel additionally needs w_tc,
+ * Both kernels: pointers 16-byte aligned, strides % 4 == 0; the exact kernel Cin % 16 == 0 or Cin == 8 (HiFi-GAN V2's last stage), the
+ * tensor-core kernel Cin % 16 == 0.  The tensor-core kernel additionally needs w_tc,
  * N % 16 == 0, x 32-byte aligned with x strides % 8 == 0 (256-bit loads), in_act in {NONE, LRELU with 0 <= slope <= 1} and
  * (taps-1)*dilation <= 256; anything else is served by the exact kernel under FS2_CONV_AUTO and refused (FS2_ERR_UNSUPPORTED)
  * under FS2_CONV_TC.  Activations beyond +-65504 saturate in the fp16 hi/lo split of the tensor-core kernel. */
@@ -214,9 +215,11 @@ int fs2_conv_post(const fs2_conv_post_args* a, fs2_stream_t stream);
 
 /* HiFi-GAN multi-receptive-field ResBlock group of one upsample stage as ONE persistent kernel (hifigan/models.py:154-160, ResBlock.forward
  * :96-103):   y = (1/n_kernels) * sum_j R_j(x),   R_j: x <- conv_{k_j,1}( lrelu( conv_{k_j,dil_jd}( lrelu(x) ) + b1 ) ) + b2 + x  for d = 0..n_dil-1,
- * lrelu slope 0.1, "same" zero padding at the utterance ends.  x, y: contiguous [B][N][C], C in {32, 64} (the 64- / 32-channel stages);
- * every intermediate stays in shared memory / registers (halo recompute), weights are the f16+f8 tiles of the per-layer kernel
- * (FS2_TC_VARIANT_F8 with N = C: pack_conv_tc(w, f8=True)).  (k-1)*dil/2 <= 32 per conv.  Other shapes: FS2_ERR_UNSUPPORTED.
+ * lrelu slope 0.1, "same" zero padding at the utterance ends.  x, y: contiguous [B][N][C], C in {8, 16, 32, 64} (the 64- to 8-channel
+ * stages of HiFi-GAN V1 and V2); every intermediate stays in shared memory / registers (halo recompute), weights are the f16+f8 tiles of
+ * the per-layer kernel (FS2_TC_VARIANT_F8 with N = C: pack_conv_tc(w, f8=True)).  C = 8 is computed as 16 channels whose upper 8 are
+ * zero: its weights are the f8 tiles of the conv zero-padded to 16 x 16 (packing.pack_conv_tc_pad16), while x and y stay [B][N][8] and
+ * no byte of y outside them is written.  (k-1)*dil/2 <= 32 per conv.  Other shapes: FS2_ERR_UNSUPPORTED.
  * x and y must not overlap (work items re-read halo rows of x): FS2_ERR_ARG. */
 typedef struct fs2_resstack_args {
   const float* x; float* y; int B, N, C;
@@ -393,7 +396,9 @@ typedef struct fs2_vocoder_model {
   const float *w_pre_tc, *w_up_a_tc[FS2_MAX_STAGES], *w_up_b_tc[FS2_MAX_STAGES];
   const float *w_rb1_tc[FS2_MAX_RESBLOCKS][FS2_MAX_DIL], *w_rb2_tc[FS2_MAX_RESBLOCKS][FS2_MAX_DIL];
   int f8_mask; /* bit 0: w_pre_tc, bit 1+i: every *_tc tile of stage i is in the f16+f8 format (FS2_TC_VARIANT_F8) */
-  int fused_mask; /* bit i: the ResBlock group of stage i runs as one fs2_resstack launch (needs f8_mask bit 1+i and 32 / 64 channels) */
+  int fused_mask; /* bit i: the ResBlock group of stage i runs as one fs2_resstack launch (needs f8_mask bit 1+i and a width fs2_resstack
+                     serves: 8, 16, 32 or 64 channels, i.e. the last two stages of V1 and all four of V2).  In an 8-channel stage the
+                     w_rb*_tc tiles are the 16 x 16 zero-padded ones fs2_resstack reads; its per-layer convs run on the exact kernel. */
   int pair_mask;  /* bit i: in stage i every (conv_k,d ; conv_k,1 ; +x) pair with k <= pair_kmax runs as one fs2_resstack launch (the
                      HBM-bound small-kernel layers: the pair's intermediate stays on chip); same requirements as fused_mask */
   int pair_kmax;

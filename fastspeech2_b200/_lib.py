@@ -157,6 +157,25 @@ class VocoderArgs(C.Structure):
                 ("wav", fp), ("workspace", fp), ("workspace_bytes", C.c_size_t), ("mel_lens", fp)]
 
 
+class VocoderWindowArgs(C.Structure):
+    """fs2_vocoder_window_args: one window [f0, f1) of fs2_vocoder_forward_window (80 bytes, pinned by a static_assert in model.cu)."""
+    _fields_ = [("B", i32), ("T", i32), ("mel", fp), ("mel_batch_stride", i64), ("mel_row_stride", i64),
+                ("wav", fp), ("workspace", fp), ("workspace_bytes", C.c_size_t), ("mel_lens", fp),
+                ("f0", i32), ("f1", i32), ("wav_batch_stride", i64)]
+
+
+VW_CONV_PRE, VW_UP_A, VW_UP_B, VW_RB_CONV1, VW_RB_CONV2, VW_RB_PAIR, VW_RB_GROUP, VW_CONV_POST = range(8)
+
+
+class VocoderWindowLaunch(C.Structure):
+    """fs2_vocoder_window_launch_t: one launch of fs2_vocoder_window_plan (56 bytes, pinned by a static_assert in model.cu)."""
+    _fields_ = [(n, i32) for n in ("layer", "stage", "j", "d", "scale", "y0", "y1", "x0", "x1", "src", "res_src", "pad_")] + \
+               [("flops", C.c_double)]
+
+
+VOCODER_WINDOW_ARGS_SIZE, VOCODER_WINDOW_LAUNCH_SIZE = 80, 56
+
+
 class ConvTcPlan(C.Structure):
     _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")]
 
@@ -213,6 +232,9 @@ EXPORTS = {
     "fs2_acoustic_decode_ctl": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), C.POINTER(ControlArgs), i32, fp]),
     "fs2_vocoder_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderArgs), fp]),
+    "fs2_vocoder_window_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
+    "fs2_vocoder_forward_window": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderWindowArgs), fp]),
+    "fs2_vocoder_window_plan": (i32, [C.POINTER(VocoderModel), i32, i32, i32, C.POINTER(VocoderWindowLaunch), i32]),
 }
 
 _lib = None
@@ -248,6 +270,16 @@ def check(rc: int, what: str = "fs2 call"):
     if rc <= -1000:
         raise Fs2Error(f"{what}: CUDA error {-(rc + 1000)}")
     raise Fs2Error(f"{what}: {_ERR.get(rc, rc)}")
+
+
+def vocoder_window_plan(m, T, f0, f1):
+    """The launches of window [f0, f1) of a T-frame batch (fs2_vocoder_window_plan): a list of VocoderWindowLaunch."""
+    n = lib().fs2_vocoder_window_plan(C.byref(m), T, f0, f1, None, 0)
+    if n < 0:
+        check(n, "fs2_vocoder_window_plan")
+    out = (VocoderWindowLaunch * n)()
+    check(min(0, lib().fs2_vocoder_window_plan(C.byref(m), T, f0, f1, out, n)), "fs2_vocoder_window_plan")
+    return list(out)
 
 
 def ptr(t):

@@ -65,6 +65,12 @@ __device__ __forceinline__ int ragged_rows(const int* lens, int scale, int cap, 
   return n <= 0 ? 0 : (n >= cap ? cap : (int)n);
 }
 
+// Windowed mode of one vocoder layer (fs2_vocoder_forward_window): the layer computes the logical output rows [y0, yend) and reads
+// logical input rows below xend only; rows outside [0, n_b) still read as zero, so the convs pad at the utterance ends and not at the
+// window's.  The host biases the buffer pointers by the windows' first rows, so kernels address logical rows.  The offline layer is
+// the window {0, cap, cap}.
+struct RowWindow { int y0, yend, xend; };
+
 // A per-element control of fs2_control_args on the [B][L] rows of a variance head or of the durations: c[b, l] = v[b * sb + l * sl]
 // (strides in elements, 0 along a broadcast dimension).  rag: NULL, or the ragged mode's lengths -- columns l >= rag[b] are not read.
 struct ControlView {

@@ -28,6 +28,7 @@ struct ConvP {
   float* y; long long ybs, yrs;
   int tiles_per_batch;
   const int* x_lens; int lens_scale;   // ragged batch (fs2_conv1d_args::x_lens) or NULL
+  RowWindow win;                       // rows computed and read ({0, T, T} outside the windowed mode)
 };
 
 template <int BM, int BN, int ACT>
@@ -47,11 +48,12 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
   const int b = blockIdx.x / p.tiles_per_batch;
-  const int t0 = (blockIdx.x % p.tiles_per_batch) * BM;
+  const int t0 = p.win.y0 + (blockIdx.x % p.tiles_per_batch) * BM;
   const int n0 = blockIdx.y * BN;
   // ragged batch: input rows t >= n_b read as zero, and a tile lying wholly at or beyond n_b has nothing to compute (its rows are unspecified)
-  const int tend = p.x_lens ? ragged_rows(p.x_lens, p.lens_scale, p.T, b) : p.T;
-  if (t0 >= tend) return;
+  const int n_b = p.x_lens ? ragged_rows(p.x_lens, p.lens_scale, p.T, b) : p.T;
+  if (t0 >= min(n_b, p.win.yend)) return;
+  const int tend = min(n_b, p.win.xend);
 
   const float* xb = p.x + (long long)b * p.xbs;
   const int kc = (p.Cin + BK - 1) / BK;    // k-steps per tap
@@ -165,7 +167,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   for (int i = 0; i < TM; i++) {
     const int m = (i < 4) ? (ty * 4 + i) : (64 + ty * 4 + (i - 4));
     const int t = t0 + m;
-    if (t >= p.T) continue;
+    if (t >= p.win.yend) continue;
     float* yrow = p.y + (long long)b * p.ybs + (long long)t * p.yrs;
     const float* rrow = p.res ? (p.res + (long long)b * p.rbs + (long long)t * p.rrs) : nullptr;
     const bool dead = t >= len_b;
@@ -212,7 +214,9 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* 
   return FS2_OK;
 }
 
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
+// win: NULL, or the windowed mode (RowWindow; a->T is then the full logical length): the tile is chosen for the window's rows.
+// Every output element sums its taps and channels in the same order whatever the tile, so a window computes the offline bits.
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
@@ -232,11 +236,15 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   p.row_lens = a->row_lens;
   p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
+  p.win = win ? *win : RowWindow{0, a->T, a->T};
+  fs2_conv1d_args rows = *a;
+  rows.T = p.win.yend - p.win.y0;
+  if (rows.T <= 0) return FS2_ERR_ARG;
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // SM count of the current device
   if (!dv) return derr;
   fs2_conv_simt_plan_t plan;
-  FS2_TRY(conv_simt_plan(a, dv->num_sms.load(std::memory_order_relaxed), &plan));
+  FS2_TRY(conv_simt_plan(&rows, dv->num_sms.load(std::memory_order_relaxed), &plan));
   const int bm = plan.BM, bn = plan.BN;
   p.tiles_per_batch = plan.grid_x / a->B;
   const dim3 grid((unsigned)plan.grid_x, (unsigned)plan.grid_y);
@@ -259,7 +267,7 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s) {
   }
 #undef FS2_SIMT_LAUNCH
 #undef FS2_SIMT_ACT
-  prof_after(s, 4, 2.0 * a->B * a->T * (double)a->Cin * a->taps * a->N);
+  prof_after(s, 4, 2.0 * a->B * rows.T * (double)a->Cin * a->taps * a->N);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

@@ -100,17 +100,24 @@ int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t
   return rc;
 }
 
-// a->w_tc must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h) in the format a->tc_variant names
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
+// a->w_tc must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h) in the format a->tc_variant names.
+// win: NULL, or the windowed mode (RowWindow; a->T is then the full logical length): the plan is made for the window's rows.
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win) {
   if (!a || !a->x || !a->w_tc || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w_tc) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
   const unsigned variant = a->tc_variant;
-  fs2_conv1d_args slice;
+  fs2_conv1d_args slice, rows;
   int nseg, seg_nkc;
   const fs2_conv1d_args* plan_args = conv_tc_segments(a, slice, nseg, seg_nkc);
   if (!plan_args) return FS2_ERR_UNSUPPORTED;
+  if (win) {                                            // tiles of the window only
+    if (win->yend <= win->y0) return FS2_ERR_ARG;
+    rows = *plan_args;
+    rows.T = win->yend - win->y0;
+    plan_args = &rows;
+  }
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);                      // state of the CURRENT device: the caller's stream must belong to it
   if (!dv) return derr;
@@ -139,20 +146,22 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s) {
   FS2_TRY(conv_tc_plan(plan_args, nseg, g_num_sms, pl));
   p.SA = pl.SA; p.SB = pl.SB; p.TPS = pl.TPS; p.R = pl.R; p.tiles_per_batch = pl.tiles_per_batch; p.n_items = pl.n_items;
   p.stage_off = pl.smem - (int)tc_stage_bytes(pl.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));   // the staged inputs end the budget
+  p.win = win ? *win : RowWindow{0, a->T, a->T};
   const unsigned grid = (unsigned)pl.grid;
   const size_t smem = (size_t)pl.smem;
+  const bool w = win != nullptr;
   prof_before(s);
   switch (pl.NB) {
-    case 16: conv_tc_launch_nb16(p, grid, smem, s); break;
-    case 32: conv_tc_launch_nb32(p, grid, smem, s); break;
-    case 48: conv_tc_launch_nb48(p, grid, smem, s); break;
-    case 64: conv_tc_launch_nb64(p, grid, smem, s); break;
-    case 80: conv_tc_launch_nb80(p, grid, smem, s); break;
-    case 96: conv_tc_launch_nb96(p, grid, smem, s); break;
-    case 112: conv_tc_launch_nb112(p, grid, smem, s); break;
-    default: conv_tc_launch_nb128(p, grid, smem, s); break;
+    case 16: conv_tc_launch_nb16(p, w, grid, smem, s); break;
+    case 32: conv_tc_launch_nb32(p, w, grid, smem, s); break;
+    case 48: conv_tc_launch_nb48(p, w, grid, smem, s); break;
+    case 64: conv_tc_launch_nb64(p, w, grid, smem, s); break;
+    case 80: conv_tc_launch_nb80(p, w, grid, smem, s); break;
+    case 96: conv_tc_launch_nb96(p, w, grid, smem, s); break;
+    case 112: conv_tc_launch_nb112(p, w, grid, smem, s); break;
+    default: conv_tc_launch_nb128(p, w, grid, smem, s); break;
   }
-  prof_after(s, 0, 2.0 * a->B * a->T * (double)a->Cin * a->taps * a->N);
+  prof_after(s, 0, 2.0 * a->B * plan_args->T * (double)a->Cin * a->taps * a->N);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

@@ -31,6 +31,8 @@
 //               alias both, so ptxas keeps them in order): one serial DRAM round trip per 8 columns with no MMA issuing.  A
 //               K-segmented conv keeps its running fp32 slice sum in the same tile instead of reading y back per slice.
 #pragma once
+#include <type_traits>
+
 #include "tc_pipeline.cuh"
 
 namespace fs2 {
@@ -73,6 +75,7 @@ struct TcP {
   const int* x_lens;               // ragged batch (fs2_conv1d_args::x_lens) or NULL
   int lens_scale;
   int stage_off;                   // shared-memory byte offset of the staged epilogue inputs (used only if tc_stage_tiles(...) > 0)
+  RowWindow win;                   // windowed mode (conv_tc_window_kernel only): rows computed and read, see RowWindow
 };
 
 // Shared-memory epilogue tiles behind the ring barriers: [full, empty mbarrier per consumer warp][residual tile if res][sum tile if
@@ -233,8 +236,10 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 }
 
 // RAG: ragged batch (TcP::x_lens != NULL), see WorkList (every NB is at or near the 96-register cap of one 544-thread CTA per SM).
-template <int NB, bool RAG>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
+// WIN: windowed mode, see WindowList: the tiles start at p.win.y0, rows at or beyond p.win.yend are not written and rows at or beyond
+// p.win.xend are not read (the host biases x, res and y by the window origins, so rows are logical here).
+template <int NB, bool RAG, bool WIN>
+__device__ __forceinline__ void conv_tc_body(const TcP& p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = warp_uniform_id(), lane = tid & 31;
@@ -253,8 +258,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
-  WorkList<RAG> work;                                  // 128-row tiles x NB-channel blocks
-  work.init(p.x_lens, p.lens_scale, p.T, p.B, 128, p.tiles_per_batch, p.n_items);
+  // 128-row tiles x NB-channel blocks; windowed: item.rows bounds the stores, the transform warps bound their loads at min(n_b, xend)
+  std::conditional_t<WIN, WindowList, WorkList<RAG>> work;
+  if constexpr (WIN) work.init(p.x_lens, p.lens_scale, p.T, p.B, 128, p.n_items / (p.B * p.tiles_per_batch), p.win.y0, p.win.yend, p.win.yend);
+  else work.init(p.x_lens, p.lens_scale, p.T, p.B, 128, p.tiles_per_batch, p.n_items);
 
   if (tid == 0) {
     ring_init(fullA, emptyA, TC_SA_MAX, TC_TW, CWARPS);
@@ -396,7 +403,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
     auto l_set_item = [&]() {
       if (l_item < work.count) {
         const Item it = work.item(l_item);
-        l_tend = it.rows;
+        if constexpr (WIN) l_tend = work.rows_of(it.b, p.win.xend);
+        else l_tend = it.rows;
         const int s_tap = l_seg / p.seg_nkc, s_kc = l_seg - s_tap * p.seg_nkc;   // K-segment: one tap, one 256-channel chunk (0, 0 when nseg == 1)
         l_tfirst = it.t0 - p.pad + s_tap;
         l_xrow = p.x + (long long)it.b * p.xbs + (long long)l_tfirst * p.xrs + s_kc * p.Cin;
@@ -458,11 +466,22 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   }
 }
 
+template <int NB, bool RAG>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
+  conv_tc_body<NB, RAG, false>(p);
+}
+
+// Windowed mode: its own entry point, so that the padded and ragged instantiations keep their code (lens may be NULL here).
+template <int NB>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_window_kernel(const TcP p) {
+  conv_tc_body<NB, true, true>(p);
+}
+
 // The NB instantiations live in their own translation units (conv_tc_nb*.cu) so that the library builds in parallel.
 // conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.
 #define FS2_CONV_TC_NB_DECL(nb)                        \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes); \
-  void conv_tc_launch_nb##nb(const TcP& p, unsigned grid, size_t smem, cudaStream_t s);
+  void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s);
 FS2_CONV_TC_NB_DECL(16) FS2_CONV_TC_NB_DECL(32) FS2_CONV_TC_NB_DECL(48) FS2_CONV_TC_NB_DECL(64)
 FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CONV_TC_NB_DECL(128)
 #undef FS2_CONV_TC_NB_DECL
@@ -470,10 +489,12 @@ FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CON
 #define FS2_CONV_TC_NB_DEF(nb)                                                                          \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes) {                                                  \
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+    return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_window_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
   }                                                                                                     \
-  void conv_tc_launch_nb##nb(const TcP& p, unsigned grid, size_t smem, cudaStream_t s) {                \
-    if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                          \
+  void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s) {   \
+    if (window) conv_tc_window_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                           \
+    else if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                     \
     else conv_tc_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);                                  \
   }
 

@@ -62,9 +62,10 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 }
 
 // kernels / launchers defined in the other translation units
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s);
+// win (the vocoder's windowed mode, RowWindow): NULL everywhere else
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr);
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s);
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
@@ -72,12 +73,12 @@ int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
 
 // backend dispatch of the fs2_conv1d contract
-static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s) {
+static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr) {
   if (!a) return FS2_ERR_ARG;
   if (a->x_lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s);
-  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s);
-  return conv1d_simt(a, s);
+  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win);
+  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win);
+  return conv1d_simt(a, s, win);
 }
 int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = false, int fused_from = 0);
 int embed_positions(const fs2_embed_args* a, cudaStream_t s);
@@ -86,8 +87,8 @@ int layernorm(const fs2_layernorm_args* a, cudaStream_t s);
 int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl = nullptr);
 int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr);
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s);
-int resstack(const fs2_resstack_args* a, cudaStream_t s);
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win = nullptr, int x0 = 0);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
@@ -414,6 +415,13 @@ static fs2_resstack_args resblock_pair(const fs2_resstack_args& g, int j, int d)
 
 static bool resstack_width(int C) { return C == 8 || C == 16 || C == 32 || C == 64; }   // the channel counts fs2_resstack serves
 
+// Stage i's operand format, and which of its ResBlock layers run as one fs2_resstack launch: the offline and the windowed walk share them
+static unsigned stage_tcv(const fs2_vocoder_model* m, int i) { return (m->f8_mask & (2 << i)) ? FS2_TC_VARIANT_F8 : 0; }
+static bool stage_fused(const fs2_vocoder_model* m, int i) { return (m->fused_mask >> i) & 1; }
+static bool stage_pairs(const fs2_vocoder_model* m, int i, int C, int k) {
+  return ((m->pair_mask >> i) & 1) && stage_tcv(m, i) && resstack_width(C) && k <= m->pair_kmax;
+}
+
 static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, cudaStream_t s, Arena& ar) {
   const int B = a->B, T = a->T;
   size_t per_frame = (size_t)m->c0;  // floats per mel frame of the widest activation
@@ -451,7 +459,7 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
   for (int i = 0; i < m->n_stages; i++) {
     const int u = m->rates[i], Co = C / 2;
     if (m->up_k[i] != 2 * u || (u & 1)) return FS2_ERR_UNSUPPORTED;
-    const unsigned tcv = (m->f8_mask & (2 << i)) ? FS2_TC_VARIANT_F8 : 0;
+    const unsigned tcv = stage_tcv(m, i);
     // ---- lrelu + ConvTranspose1d as two 2-tap phase-group convolutions (hifigan/models.py:152-153)
     for (int g = 0; g < 2; g++) {
       const size_t off = (size_t)g * (u / 2) * Co;    // group g writes output channels [off, off + (u/2)*Co) of each [u*Co] row
@@ -469,7 +477,7 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
     Ti *= u; C = Co; scale *= u;
     // ---- mean of the multi-receptive-field ResBlocks (models.py:154-160, ResBlock.forward :96-103)
     fs2_resstack_args group = resblock_args(m, i, B, Ti, C, lens, scale);
-    if ((m->fused_mask >> i) & 1) {                    // one persistent kernel for the whole group: intermediates never leave the SM
+    if (stage_fused(m, i)) {                           // one persistent kernel for the whole group: intermediates never leave the SM
       if (!tcv) return FS2_ERR_ARG;
       group.x = bu; group.y = bx;
       FS2_TRY(resstack(&group, s));
@@ -478,7 +486,7 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
     for (int j = 0; j < m->n_kernels; j++) {
       const int rb = i * m->n_kernels + j, k = m->rb_k[j];
       const float* r = bu;
-      const bool pairs = ((m->pair_mask >> i) & 1) && tcv && resstack_width(C) && k <= m->pair_kmax;
+      const bool pairs = stage_pairs(m, i, C, k);
       for (int d = 0; d < m->n_dil; d++) {
         const bool last = d == m->n_dil - 1;            // the last layer adds its share of the mean over the n_kernels ResBlocks into bx
         float* dst = last ? bx : (r == r1 ? r2 : r1);
@@ -510,6 +518,237 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
   p.x = bx; p.B = B; p.T = Ti; p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f; p.wav = a->wav;
   p.lens = lens; p.lens_scale = scale;
   return conv_post(&p, s);
+}
+
+// ------------------------------------------------------------------ windowed vocoder (fs2_vocoder_forward_window)
+// A window [f0, f1) is walked backward from its output samples to the rows every layer must compute (each conv: its consumers' rows
+// widened by its radius, clipped to the utterance's logical extent), then forward in the offline call's launch order, every layer
+// computing only those rows with the kernels and arithmetic the offline call uses (RowWindow).  One walk makes both the plan
+// (fs2_vocoder_window_plan) and, given a WinExec, the launches, so the two cannot disagree.
+
+struct Rows {
+  int lo, hi;
+  int n() const { return hi - lo; }
+};
+// [lo - by, hi + by) clipped to [0, cap); cap < 0: unclipped (the workspace bound of a window of hi - lo frames)
+static Rows widen(Rows r, int by, long long cap) {
+  r.lo -= by; r.hi += by;
+  if (cap >= 0) { r.lo = r.lo > 0 ? r.lo : 0; r.hi = (long long)r.hi < cap ? r.hi : (int)cap; }
+  return r;
+}
+static int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+static int pair_reach(const fs2_vocoder_model* m, int j, int d) { return (m->rb_k[j] - 1) * m->rb_dil[j][d] / 2 + (m->rb_k[j] - 1) / 2; }
+
+// A window buffer: logical rows [lo, lo + rows) of C floats each, utterances `rows` rows apart.
+struct View {
+  float* p; int lo, rows, C;
+  // logical row 0 of utterance 0: the kernels address logical rows, and never dereference one outside [lo, lo + rows)
+  float* at() const { return reinterpret_cast<float*>(reinterpret_cast<uintptr_t>(p) - (uintptr_t)lo * C * sizeof(float)); }
+  int64_t bs() const { return (int64_t)rows * C; }
+};
+
+struct WinExec {
+  const fs2_vocoder_window_args* a; cudaStream_t s;
+  float *bx, *bu, *bt, *r1, *r2;                       // the offline call's five buffers, each B * width floats
+};
+
+// fs2_conv1d arguments of a windowed launch: `cap` (a.T) is the layer's full logical length; residual off, as conv_args leaves it
+static fs2_conv1d_args win_conv_args(const float* x, int64_t xbs, int64_t xrs, int B, int cap, int Cin, const View& y, int N, int taps) {
+  fs2_conv1d_args c = conv_args(x, B, cap, Cin, N, taps, y.at());
+  c.x_batch_stride = xbs; c.x_row_stride = xrs;
+  c.y_batch_stride = y.bs(); c.y_row_stride = y.C;
+  c.res_batch_stride = c.res_row_stride = 0;
+  return c;
+}
+
+// The launches of window [f0, f1) of a T-frame batch (f1 <= T), appended to L in issue order; with ex, also issued.  T < 0: the plan of
+// an unclipped [f0, f1) (no launches), whose row counts bound those of every window of f1 - f0 frames.
+static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::vector<fs2_vocoder_window_launch_t>& L, const WinExec* ex) {
+  const int n = m->n_stages;
+  int sc[FS2_MAX_STAGES + 1];                          // rows per mel frame at stage i's input (sc[n]: the waveform)
+  sc[0] = 1;
+  for (int i = 0; i < n; i++) {
+    if (m->up_k[i] != 2 * m->rates[i] || (m->rates[i] & 1)) return FS2_ERR_UNSUPPORTED;
+    if (stage_fused(m, i) && !stage_tcv(m, i)) return FS2_ERR_ARG;
+    sc[i + 1] = sc[i] * m->rates[i];
+  }
+  auto cap = [&](int scale) { return T < 0 ? -1LL : (long long)T * scale; };
+  // ---- backward: O[i + 1] = the rows stage i's output must hold (O[0]: conv_pre's), U[i] = its ResBlocks' input, Q[i] = the
+  // ConvTranspose's phase-group rows
+  Rows O[FS2_MAX_STAGES + 1], U[FS2_MAX_STAGES], Q[FS2_MAX_STAGES];
+  const Rows post = widen(Rows{f0 * sc[n], f1 * sc[n]}, 0, cap(sc[n]));
+  O[n] = widen(post, 3, cap(sc[n]));
+  for (int i = n - 1; i >= 0; i--) {
+    int reach = 0;                                     // the widest ResBlock's receptive radius
+    for (int j = 0; j < m->n_kernels; j++) {
+      int r = 0;
+      for (int d = 0; d < m->n_dil; d++) r += pair_reach(m, j, d);
+      reach = r > reach ? r : reach;
+    }
+    const int u = m->rates[i];
+    U[i] = widen(O[i + 1], reach, cap(sc[i + 1]));
+    Q[i] = Rows{floor_div(U[i].lo, u), -floor_div(-U[i].hi, u)};
+    O[i] = widen(Q[i], 1, cap(sc[i]));
+  }
+  // ---- forward
+  auto add = [&](int layer, int stage, int j, int d, int scale, Rows y, Rows x, int src, int res_src, double flops) {
+    fs2_vocoder_window_launch_t l{};
+    l.layer = layer; l.stage = stage; l.j = j; l.d = d; l.scale = scale;
+    l.y0 = y.lo; l.y1 = y.hi; l.x0 = x.lo; l.x1 = x.hi; l.src = src; l.res_src = res_src; l.flops = flops;
+    L.push_back(l);
+    return (int)L.size() - 1;
+  };
+  const fs2_vocoder_window_args* a = ex ? ex->a : nullptr;
+  const int B = a ? a->B : 0;
+  const int32_t* lens = a ? a->mel_lens : nullptr;
+  cudaStream_t s = ex ? ex->s : nullptr;
+  int C = m->c0;
+  const Rows mel = widen(O[0], 3, cap(1));
+  int last = add(FS2_VW_CONV_PRE, -1, -1, -1, 1, O[0], mel, -1, -1, 2.0 * O[0].n() * m->n_mel * 7 * C);
+  View bx{ex ? ex->bx : nullptr, O[0].lo, O[0].n(), C};
+  if (ex) {
+    fs2_conv1d_args c = win_conv_args(a->mel, a->mel_batch_stride, a->mel_row_stride, B, T, m->n_mel, bx, C, 7);
+    c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
+    c.x_lens = lens; c.lens_scale = 1;
+    const RowWindow w{O[0].lo, O[0].hi, mel.hi};
+    FS2_TRY(conv1d_dispatch(&c, s, &w));
+  }
+  const float inv_nk = 1.f / (float)m->n_kernels;
+  for (int i = 0; i < n; i++) {
+    const int u = m->rates[i], Co = C / 2, s0 = sc[i], s1 = sc[i + 1];
+    const unsigned tcv = stage_tcv(m, i);
+    // ---- ConvTranspose phase groups: rows Q[i] of [u * Co] = the next rate's rows [Q.lo * u, Q.hi * u)
+    const double up_flops = 2.0 * Q[i].n() * C * 2 * (u / 2) * Co;
+    const View bu{ex ? ex->bu : nullptr, Q[i].lo, Q[i].n(), u * Co};
+    int up_src = -1;
+    for (int g = 0; g < 2; g++) {
+      const Rows x = widen(Rows{Q[i].lo - (g == 0), Q[i].hi + (g == 1)}, 0, cap(s0));
+      up_src = add(g == 0 ? FS2_VW_UP_A : FS2_VW_UP_B, i, -1, -1, s0, Q[i], x, last, -1, up_flops);
+      if (!ex) continue;
+      const size_t off = (size_t)g * (u / 2) * Co;
+      fs2_conv1d_args c = win_conv_args(bx.at(), bx.bs(), C, B, T * s0, C, bu, (u / 2) * Co, 2);
+      c.y += off;
+      c.pad_left = g == 0 ? 1 : 0;
+      c.w = g == 0 ? m->w_up_a[i] : m->w_up_b[i];
+      c.w_tc = g == 0 ? m->w_up_a_tc[i] : m->w_up_b_tc[i];
+      c.bias = m->b_up[i] + off;
+      c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
+      c.x_lens = lens; c.lens_scale = s0;
+      const RowWindow w{Q[i].lo, Q[i].hi, x.hi};
+      FS2_TRY(conv1d_dispatch(&c, s, &w));
+    }
+    C = Co;
+    const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
+    const long long cap1 = cap(s1);
+    if (stage_fused(m, i)) {
+      double fl = 0;
+      for (int j = 0; j < m->n_kernels; j++) {
+        Rows r = O[i + 1];
+        for (int d = m->n_dil - 1; d >= 0; d--) {
+          const int k = m->rb_k[j];
+          const Rows mid = widen(r, (k - 1) / 2, cap1);
+          fl += 2.0 * C * k * C * (mid.n() + r.n());
+          r = widen(mid, (k - 1) * m->rb_dil[j][d] / 2, cap1);
+        }
+      }
+      last = add(FS2_VW_RB_GROUP, i, -1, -1, s1, O[i + 1], U[i], up_src, -1, fl);
+      bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
+      if (ex) {
+        fs2_resstack_args g = resblock_args(m, i, B, T * s1, C, lens, s1);
+        g.x = in.p; g.y = bx.p;
+        const RowWindow w{O[i + 1].lo, O[i + 1].hi, in.lo + in.rows};
+        FS2_TRY(resstack(&g, s, &w, in.lo));
+      }
+      continue;
+    }
+    bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
+    const fs2_resstack_args group = ex ? resblock_args(m, i, B, T * s1, C, lens, s1) : fs2_resstack_args{};
+    for (int j = 0; j < m->n_kernels; j++) {
+      const int rb = i * m->n_kernels + j, k = m->rb_k[j];
+      Rows R[FS2_MAX_DIL];                             // output rows of pair d
+      R[m->n_dil - 1] = O[i + 1];
+      for (int d = m->n_dil - 1; d > 0; d--) R[d - 1] = widen(R[d], pair_reach(m, j, d), cap1);
+      View r = in;
+      int r_src = up_src;
+      for (int d = 0; d < m->n_dil; d++) {
+        const bool lastd = d == m->n_dil - 1;
+        const Rows x = widen(R[d], pair_reach(m, j, d), cap1), mid = widen(R[d], (k - 1) / 2, cap1);
+        const double f1c = 2.0 * mid.n() * C * k * C, f2c = 2.0 * R[d].n() * C * k * C;
+        const View dst{lastd ? bx.p : (ex && r.p == ex->r1 ? ex->r2 : (ex ? ex->r1 : nullptr)), R[d].lo, R[d].n(), C};
+        const float alpha = lastd ? inv_nk : 1.f;
+        const int accumulate = lastd && j > 0;
+        if (stage_pairs(m, i, C, k)) {
+          const int id = add(FS2_VW_RB_PAIR, i, j, d, s1, R[d], x, r_src, r_src, f1c + f2c);
+          if (ex) {
+            fs2_resstack_args p = resblock_pair(group, j, d);
+            p.x = r.p; p.y = dst.p; p.alpha = alpha; p.accumulate = accumulate;
+            const RowWindow w{R[d].lo, R[d].hi, r.lo + r.rows};
+            FS2_TRY(resstack(&p, s, &w, r.lo));
+          }
+          r_src = id;
+        } else {
+          const int c1 = add(FS2_VW_RB_CONV1, i, j, d, s1, mid, x, r_src, -1, f1c);
+          const int c2 = add(FS2_VW_RB_CONV2, i, j, d, s1, R[d], mid, c1, r_src, f2c);
+          if (ex) {
+            const int dil = m->rb_dil[j][d];
+            const View t{ex->bt, mid.lo, mid.n(), C};
+            fs2_conv1d_args c = win_conv_args(r.at(), r.bs(), C, B, T * s1, C, t, C, k);
+            c.w = m->w_rb1[rb][d]; c.w_tc = m->w_rb1_tc[rb][d]; c.bias = m->b_rb1[rb][d]; c.tc_variant = tcv;
+            c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
+            c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
+            c.x_lens = lens; c.lens_scale = s1;
+            const RowWindow w1{mid.lo, mid.hi, x.hi};
+            FS2_TRY(conv1d_dispatch(&c, s, &w1));
+            c = win_conv_args(t.at(), t.bs(), C, B, T * s1, C, dst, C, k);
+            c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
+            c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
+            c.alpha = alpha; c.accumulate = accumulate;
+            c.x_lens = lens; c.lens_scale = s1;
+            const RowWindow w2{R[d].lo, R[d].hi, mid.hi};
+            FS2_TRY(conv1d_dispatch(&c, s, &w2));
+          }
+          r_src = c2;
+        }
+        r = dst;
+      }
+      last = r_src;
+    }
+  }
+  add(FS2_VW_CONV_POST, -1, -1, -1, sc[n], post, O[n], last, -1, 2.0 * post.n() * C * 7);
+  if (!ex) return FS2_OK;
+  fs2_conv_post_args p{};
+  p.x = bx.at(); p.B = B; p.T = T * sc[n]; p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
+  p.wav = a->wav - post.lo;                            // sample f0 * up is the caller's wav[0]
+  p.lens = lens; p.lens_scale = sc[n];
+  const RowWindow w{post.lo, post.hi, O[n].hi};
+  return conv_post(&p, s, &w, bx.bs(), a->wav_batch_stride);
+}
+
+// Floats per utterance of each of the five buffers of a window of `frames` frames: the widest output of its unclipped plan
+static int window_width(const fs2_vocoder_model* m, int frames, size_t& width) {
+  std::vector<fs2_vocoder_window_launch_t> L;
+  FS2_TRY(window_walk(m, -1, 0, frames, L, nullptr));
+  width = 0;
+  for (const auto& l : L) {
+    size_t ch = 0;                                     // floats per output row
+    if (l.layer == FS2_VW_CONV_PRE) ch = (size_t)m->c0;
+    else if (l.layer == FS2_VW_UP_A || l.layer == FS2_VW_UP_B) ch = (size_t)m->rates[l.stage] * (m->c0 >> (l.stage + 1));
+    else if (l.layer != FS2_VW_CONV_POST) ch = (size_t)(m->c0 >> (l.stage + 1));
+    const size_t w = (size_t)(l.y1 - l.y0) * ch;
+    width = w > width ? w : width;
+  }
+  return FS2_OK;
+}
+
+static int vocoder_window_impl(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, int frames, cudaStream_t s, Arena& ar) {
+  size_t width = 0;
+  FS2_TRY(window_width(m, frames, width));
+  const size_t nf = (size_t)a->B * width;
+  WinExec ex{a, s, ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
+  if (ar.dry) return FS2_OK;
+  if (!ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
+  std::vector<fs2_vocoder_window_launch_t> L;
+  return window_walk(m, a->T, a->f0, a->f1 < a->T ? a->f1 : a->T, L, &ex);
 }
 
 }  // namespace fs2
@@ -676,6 +915,46 @@ int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, f
   if (!vocoder_ok(m) || !a || a->B <= 0 || a->T <= 0 || !a->mel || !a->wav || !a->workspace) return FS2_ERR_ARG;
   Arena ar(a->workspace, a->workspace_bytes);
   return vocoder_impl(m, a, S(st), ar);
+}
+
+// fs2_vocoder_window_args and fs2_vocoder_window_launch_t are not in the fs2_struct_size table (it stays at 0..18): pinned here and in
+// the binding
+static_assert(sizeof(fs2_vocoder_window_args) == 80, "fs2_vocoder_window_args: fs2_vocoder_args' fields, f0, f1, wav_batch_stride");
+static_assert(sizeof(fs2_vocoder_window_launch_t) == 56, "fs2_vocoder_window_launch_t: twelve int32 and a double");
+
+// Row counts of a window must fit the kernels' int rows with the halo: frames (and T) times prod(rates) below 2^30
+static bool window_rows_ok(const fs2_vocoder_model* m, long long frames) {
+  long long up = 1;
+  for (int i = 0; i < m->n_stages; i++) up *= m->rates[i];
+  return frames * up < (1LL << 30);
+}
+
+size_t fs2_vocoder_window_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
+  if (!vocoder_ok(m) || B <= 0 || frames <= 0 || !window_rows_ok(m, frames)) return 0;
+  Arena ar(nullptr, 0);
+  fs2_vocoder_window_args a{};
+  a.B = B;
+  if (vocoder_window_impl(m, &a, frames, nullptr, ar) != FS2_OK) return 0;
+  return ar.off + 256;
+}
+
+int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, fs2_stream_t st) {
+  if (!vocoder_ok(m) || !a || a->B <= 0 || a->T <= 0 || !a->mel || !a->wav || !a->workspace) return FS2_ERR_ARG;
+  if (a->f0 < 0 || a->f1 <= a->f0 || a->f0 >= a->T || !window_rows_ok(m, a->T)) return FS2_ERR_ARG;
+  const int frames = (a->f1 < a->T ? a->f1 : a->T) - a->f0;
+  long long up = 1;
+  for (int i = 0; i < m->n_stages; i++) up *= m->rates[i];
+  if (a->B > 1 && a->wav_batch_stride < frames * up) return FS2_ERR_ARG;
+  Arena ar(a->workspace, a->workspace_bytes);
+  return vocoder_window_impl(m, a, frames, S(st), ar);
+}
+
+int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, fs2_vocoder_window_launch_t* out, int max_launches) {
+  if (!vocoder_ok(m) || T <= 0 || f0 < 0 || f1 <= f0 || f0 >= T || max_launches < 0 || !window_rows_ok(m, T)) return FS2_ERR_ARG;
+  std::vector<fs2_vocoder_window_launch_t> L;
+  FS2_TRY(window_walk(m, T, f0, f1 < T ? f1 : T, L, nullptr));
+  for (int i = 0; out && i < (int)L.size() && i < max_launches; i++) out[i] = L[i];
+  return (int)L.size();
 }
 
 }  // extern "C"

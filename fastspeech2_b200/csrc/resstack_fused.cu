@@ -31,6 +31,8 @@
 // Roles: warps 0-7 two consumer warpgroups (conversion, MMAs, epilogues; thread 0 issues the tensor-map copies), warp 8 weight producer.
 #include <cuda.h>
 
+#include <type_traits>
+
 #include "tc_pipeline.cuh"
 
 namespace fs2 {
@@ -52,6 +54,8 @@ struct RsP {
   int TPS;                       // conv taps per weight stage (one bulk copy / one handshake)
   int accumulate;                // the first kernel size reduce-adds into y too
   const int* lens; int lens_scale;   // ragged batch (fs2_resstack_args::lens) or NULL
+  int x0;                            // windowed mode: logical row of the x map's row 0 (the y map's row 0 is win.y0)
+  RowWindow win;                     // windowed mode: rows computed (win.xend is not read: the x map ends the input)
 };
 
 // ------------------------------------------------------------------ TMA (tensor-map) wrappers
@@ -103,7 +107,10 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
 // weights are then the 16 x 16 zero-padded tiles, and channels CG..C-1 are held at exact zero in both slabs).  Global rows of 128 bytes
 // or more travel as [128 rows][32 channels] boxes with the 128-byte swizzle; narrower rows (CG = 16: 64 B, CG = 8: 32 B) as one
 // unswizzled [rows][CG] box per 128 rows.  RAG: ragged batch (RsP::lens != NULL), see WorkList.
-template <int CG, int C, int MT, bool RAG>
+// WIN (with RAG): windowed mode, see WindowList.  The tensor maps span the window buffers: the x map's row 0 is logical row p.x0, the
+// y map's is p.win.y0.  Its zero fill beyond the x window only reaches slab rows whose results are never stored (the host sizes the x
+// window to the stored rows' receptive field), and the y map clips the stores to the window.
+template <int CG, int C, int MT, bool RAG, bool WIN = false>
 __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUtensorMap& tmy, const RsP& p) {
   constexpr int KB = C / 16, R = MT * 128, NJ = C / 8;                // NJ: 8-column fragment groups of a row
   constexpr int BOXC = CG < 32 ? CG : 32, NH = CG / BOXC;             // channels per TMA box, boxes across a row
@@ -138,8 +145,10 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
   }
   fence_proxy_async();
   __syncthreads();
-  WorkList<RAG> work;                            // TILE-row tiles of each utterance
-  work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, p.tiles_per_b, p.n_items);
+  std::conditional_t<WIN, WindowList, WorkList<RAG>> work;   // TILE-row tiles of each utterance
+  if constexpr (WIN) work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, 1, p.win.y0, p.win.yend, p.N);
+  else work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, p.tiles_per_b, p.n_items);
+  const int xorg = WIN ? p.x0 : 0, yorg = WIN ? p.win.y0 : 0;   // map row 0
 
   if (warp == 8) {
     // ===================== weight producer: every conv's stages once per work item and kernel size =====================
@@ -183,7 +192,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
         if (stores_pending) tma_wait_reads();           // previous result boxes have been read out of XA
         mbar_expect_tx(xLoaded, (uint32_t)(MT * NH) * XBOX);
         for (int hh = 0; hh < NH; hh++)
-          for (int m = 0; m < MT; m++) tma_load_3d(xt + (size_t)(hh * MT + m) * XBOX, &tmx, hh * BOXC, t0 - p.H + m * 128, b, xLoaded);
+          for (int m = 0; m < MT; m++) tma_load_3d(xt + (size_t)(hh * MT + m) * XBOX, &tmx, hh * BOXC, t0 - p.H + m * 128 - xorg, b, xLoaded);
       }
       stores_pending = true;
       consumers_sync();                                 // XA is free
@@ -327,8 +336,8 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
         for (int hh = 0; hh < NH; hh++)
           for (int bx = 0; bx < p.n_oboxes; bx++) {
             const unsigned char* src = xa + (size_t)(hh * p.n_oboxes + bx) * ((size_t)p.OBOX * BOXC * 4);
-            if (j == 0 && !p.accumulate) tma_store_3d(&tmy, hh * BOXC, t0 + bx * p.OBOX, b, src);
-            else tma_reduce_add_3d(&tmy, hh * BOXC, t0 + bx * p.OBOX, b, src);
+            if (j == 0 && !p.accumulate) tma_store_3d(&tmy, hh * BOXC, t0 + bx * p.OBOX - yorg, b, src);
+            else tma_reduce_add_3d(&tmy, hh * BOXC, t0 + bx * p.OBOX - yorg, b, src);
           }
         tma_commit();
       }
@@ -348,6 +357,18 @@ template <int CG, bool RAG>
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                         const __grid_constant__ CUtensorMap tmy, const RsP p) {
   resstack_body<CG, 16, 8, RAG>(tmx, tmy, p);
+}
+
+// Windowed mode: entry points of their own, so that the padded and ragged instantiations keep their code (lens may be NULL here)
+template <int C, int MT>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_window_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                        const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<C, C, MT, true, true>(tmx, tmy, p);
+}
+template <int CG>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_window_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                               const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<CG, 16, 8, true, true>(tmx, tmy, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -426,21 +447,27 @@ static int make_map(CUtensorMap* tm, const float* base, int B, int N, int C, int
   return r == CUDA_SUCCESS ? FS2_OK : FS2_ERR_CUDA - 1;
 }
 
-int resstack(const fs2_resstack_args* a, cudaStream_t s) {
+// win: NULL, or the windowed mode: a->x and a->y are then the window buffers [B][x1 - x0][C] and [B][yend - y0][C] (not biased), x0 /
+// x1 the logical rows a->x holds (win->xend is x1), and a->N the full logical length.
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, int x0) {
   if (!a || !a->x || !a->y) return FS2_ERR_ARG;
   if (!aligned16(a->x) || !aligned16(a->y)) return FS2_ERR_ARG;
   if (a->B <= 0 || a->N <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
+  const int xrows = win ? win->xend - x0 : a->N, yrows = win ? win->yend - win->y0 : a->N;   // rows of the x and y buffers
+  if (xrows <= 0 || yrows <= 0) return FS2_ERR_ARG;
   {  // not in place: a work item re-reads halo rows of x that its neighbours' results would already have overwritten
     const unsigned char *xb = reinterpret_cast<const unsigned char*>(a->x), *yb = reinterpret_cast<const unsigned char*>(a->y);
-    const size_t bytes = (size_t)a->B * a->N * a->C * sizeof(float);
-    if (xb < yb + bytes && yb < xb + bytes) return FS2_ERR_ARG;
+    const size_t row = (size_t)a->B * a->C * sizeof(float);
+    if (xb < yb + row * yrows && yb < xb + row * xrows) return FS2_ERR_ARG;
   }
   int derr = FS2_OK;
   DevState* dv = dev_state(&derr);
   if (!dv) return derr;
+  fs2_resstack_args rows = *a;                  // the plan's items: tiles of the y rows
+  rows.N = yrows;
   fs2_resstack_plan_t plan;
-  FS2_TRY(resstack_plan(a, dv->num_sms.load(std::memory_order_relaxed), plan));
+  FS2_TRY(resstack_plan(&rows, dv->num_sms.load(std::memory_order_relaxed), plan));
   FS2_TRY(dev_once(dv->fused_ready, [] {
     const int mx = 227 * 1024;
     cudaError_t e = cudaFuncSetAttribute(resstack_kernel<32, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
@@ -451,6 +478,10 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_window_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_window_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_window_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_window_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     return e;
   }));
   RsP p{};
@@ -463,16 +494,22 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s) {
       if (!aligned16(a->w1_tc[j][d]) || !aligned16(a->w2_tc[j][d]) || !aligned16(a->b1[j][d]) || !aligned16(a->b2[j][d])) return FS2_ERR_ARG;
       p.conv[j][d][0] = RsConv{reinterpret_cast<const unsigned char*>(a->w1_tc[j][d]), a->b1[j][d], a->k[j], a->dil[j][d]};
       p.conv[j][d][1] = RsConv{reinterpret_cast<const unsigned char*>(a->w2_tc[j][d]), a->b2[j][d], a->k[j], 1};
-      flops += 2.0 * 2.0 * a->B * (double)a->N * a->C * a->C * a->k[j];
+      flops += 2.0 * 2.0 * a->B * (double)yrows * a->C * a->C * a->k[j];
     }
   p.H = plan.H; p.TILE = plan.TILE; p.tiles_per_b = plan.n_items / a->B; p.n_items = plan.n_items; p.SB = plan.SB; p.OBOX = plan.OBOX; p.n_oboxes = plan.n_oboxes; p.TPS = plan.TPS;
   p.alpha = a->alpha > 0.f ? a->alpha : 1.f / (float)a->n_kernels; p.accumulate = a->accumulate;
   p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
+  p.x0 = x0; p.win = win ? *win : RowWindow{0, a->N, a->N};
   alignas(64) CUtensorMap tmx, tmy;
-  FS2_TRY(make_map(&tmx, a->x, a->B, a->N, a->C, 128));
-  FS2_TRY(make_map(&tmy, a->y, a->B, a->N, a->C, p.OBOX));
+  FS2_TRY(make_map(&tmx, a->x, a->B, xrows, a->C, 128));
+  FS2_TRY(make_map(&tmy, a->y, a->B, yrows, a->C, p.OBOX));
   prof_before(s);
-  if (a->C == 32) {
+  if (win) {
+    if (a->C == 32) resstack_window_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 64) resstack_window_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 16) resstack_narrow_window_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_narrow_window_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+  } else if (a->C == 32) {
     if (a->lens) resstack_kernel<32, 4, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_kernel<32, 4, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   } else if (a->C == 64) {

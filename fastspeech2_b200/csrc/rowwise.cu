@@ -366,17 +366,21 @@ int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s) {
 // 256 + taps - 1 activated rows in shared memory with fully coalesced float4 loads (row stride C+1 floats -> conflict-free
 // column walks), then each thread reduces its own output sample from shared memory.
 constexpr int CP_ROWS = 256;
-__global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_args a, int tiles_per_batch) {
+// Batch strides of x and wav and the rows computed and read: {T * C, T} and {0, T, T} outside the windowed mode (RowWindow; a.T is then
+// the full logical length, and x / wav are biased by the windows' first rows).
+struct PostRows { long long xbs, wbs; RowWindow win; };
+__global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
   extern __shared__ float cp_smem[];
   const int C = a.C, ld = C + 1, pad = (a.taps - 1) / 2;
   float* wsm = cp_smem;                   // [taps][C]
   float* xs = cp_smem + a.taps * C;       // [CP_ROWS + taps - 1][C + 1]
   const int b = blockIdx.x / tiles_per_batch;
-  const int t0 = (blockIdx.x % tiles_per_batch) * CP_ROWS;
-  const int nin = a.lens ? ragged_rows(a.lens, a.lens_scale, a.T, b) : a.T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  const int t0 = pr.win.y0 + (blockIdx.x % tiles_per_batch) * CP_ROWS;
+  const int n_b = a.lens ? ragged_rows(a.lens, a.lens_scale, a.T, b) : a.T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  const int nin = min(n_b, pr.win.xend);
   for (int i = threadIdx.x; i < a.taps * C; i += blockDim.x) wsm[i] = a.w[i];
   const int rows = CP_ROWS + a.taps - 1, C4 = C / 4;
-  const float4* xb = reinterpret_cast<const float4*>(a.x) + (long long)b * a.T * C4;
+  const float4* xb = reinterpret_cast<const float4*>(a.x + (long long)b * pr.xbs);
   for (int i = threadIdx.x; i < rows * C4; i += blockDim.x) {
     const int r = i / C4, c4 = i - r * C4;
     const int t = t0 - pad + r;
@@ -393,7 +397,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
   }
   __syncthreads();
   const int t = t0 + threadIdx.x;
-  if (t >= a.T) return;
+  if (t >= pr.win.yend) return;
   float acc = __ldg(a.bias);
   for (int j = 0; j < a.taps; j++) {
     const float* xr = xs + (threadIdx.x + j) * ld;
@@ -401,7 +405,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 #pragma unroll 8
     for (int c = 0; c < C; c++) acc = fmaf(xr[c], wj[c], acc);
   }
-  a.wav[(long long)b * a.T + t] = t < nin ? tanhf(acc) : 0.f;
+  a.wav[(long long)b * pr.wbs + t] = t < n_b ? tanhf(acc) : 0.f;
 }
 
 // The generator's own shape (32 channels, 7 taps, hifigan/models.py:131): no shared memory at all.  Eight lanes own one time row (one
@@ -413,7 +417,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 constexpr int CPF_BLOCKS = 18;                         // row blocks of TAPS rows per 8-lane group
 // RAG: ragged batch (a.lens != NULL); a template parameter so that the padded path keeps its code and registers
 template <int TAPS, bool RAG>
-__global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups) {
+__global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups, const PostRows pr) {
   constexpr int PAD = (TAPS - 1) / 2, ROWS = CPF_BLOCKS * TAPS - 2 * PAD;     // output rows per group (120 for 7 taps: a multiple of 8)
   static_assert(ROWS % 8 == 0, "full 8-sample stores");
   const int lane = threadIdx.x & 31, sub = lane & 7;
@@ -421,16 +425,17 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
   const bool live = grp < n_groups;                     // groups past the end run along with an empty row range (full-warp shuffles below)
   grp = live ? grp : 0;
   const int b = (int)(grp / groups_per_batch);
-  const int t0 = (int)(grp - (long long)b * groups_per_batch) * ROWS;
+  const int t0 = pr.win.y0 + (int)(grp - (long long)b * groups_per_batch) * ROWS;
   const int T = live ? a.T : 0;
-  const int tend = min(t0 + ROWS, T);
-  const int nin = RAG ? ragged_rows(a.lens, a.lens_scale, T, b) : T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  const int tend = min(t0 + ROWS, live ? pr.win.yend : 0);
+  const int n_b = RAG ? ragged_rows(a.lens, a.lens_scale, T, b) : T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  const int nin = min(n_b, pr.win.xend);
   float4 w[TAPS];
 #pragma unroll
   for (int j = 0; j < TAPS; j++) w[j] = __ldg(reinterpret_cast<const float4*>(a.w + j * 32) + sub);
   const float bias = __ldg(a.bias), slope = a.in_slope;
-  const float4* xb = reinterpret_cast<const float4*>(a.x) + (long long)b * a.T * 8 + sub;
-  float* wb = a.wav + (long long)b * a.T;
+  const float4* xb = reinterpret_cast<const float4*>(a.x + (long long)b * pr.xbs) + sub;
+  float* wb = a.wav + (long long)b * pr.wbs;
   float s[TAPS];
 #pragma unroll
   for (int k = 0; k < TAPS; k++) s[k] = 0.f;
@@ -467,35 +472,40 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
         const int o = (t - t0) & 7;
         if (o == sub) keep = tot;
         if (o == 7 || t == tend - 1) {
-          if (sub <= o) wb[t - o + sub] = (!RAG || t - o + sub < nin) ? tanhf(keep + bias) : 0.f;
+          if (sub <= o) wb[t - o + sub] = (!RAG || t - o + sub < n_b) ? tanhf(keep + bias) : 0.f;
         }
       }
     }
   }
 }
 
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s) {
+// win: NULL, or the windowed mode (a->T is then the full logical length, a->x and a->wav are biased by the windows' first rows and
+// their batch strides are x_bs and wav_bs).  Both kernels add every output's taps in the same order wherever its tile starts.
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win, long long x_bs, long long wav_bs) {
   if (!a || !a->x || !a->w || !a->bias || !a->wav || a->B <= 0 || a->T <= 0 || a->C <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
+  const PostRows pr = win ? PostRows{x_bs, wav_bs, *win} : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}};
+  const int rows = pr.win.yend - pr.win.y0;
+  if (rows <= 0) return FS2_ERR_ARG;
   if (a->C == 32 && a->taps == 7 && (reinterpret_cast<uintptr_t>(a->x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15u) == 0) {
     constexpr int ROWS = CPF_BLOCKS * 7 - 6;
-    const int gpb = (a->T + ROWS - 1) / ROWS;
+    const int gpb = (rows + ROWS - 1) / ROWS;
     const long long n_groups = (long long)gpb * a->B, blocks = (n_groups * 8 + 255) / 256;
     if (blocks > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
     prof_before(s);
-    if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups);
-    else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups);
-    prof_after(s, 3, 2.0 * (double)a->B * a->T * a->taps * a->C);
+    if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    prof_after(s, 3, 2.0 * (double)a->B * rows * a->taps * a->C);
     FS2_LAUNCH_CHECK();
     return FS2_OK;
   }
   const size_t smem = ((size_t)a->taps * a->C + (size_t)(CP_ROWS + a->taps - 1) * (a->C + 1)) * sizeof(float);
   if (a->C % 4 || smem > 48 * 1024) return FS2_ERR_UNSUPPORTED;
-  const int tiles = (a->T + CP_ROWS - 1) / CP_ROWS;
-  const long long n = (long long)a->B * a->T;
+  const int tiles = (rows + CP_ROWS - 1) / CP_ROWS;
+  const long long n = (long long)a->B * rows;
   if ((long long)tiles * a->B > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   prof_before(s);
-  conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles);
+  conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   prof_after(s, 3, 2.0 * n * a->taps * a->C);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

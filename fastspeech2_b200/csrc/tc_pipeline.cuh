@@ -198,4 +198,36 @@ struct WorkList<true, MIN_ROWS> {
   }
 };
 
+// Windowed mode (fs2_vocoder_forward_window): only the logical rows [y0, yend) of each utterance are computed, in `tile`-row tiles
+// that start at y0, and only where they hold a row < n_b.  n_b = ragged_rows(lens, scale, cap, b), or cap when lens is NULL (every
+// utterance cap rows long).  An item's t0 is its tile's first logical row and its `rows` is min(n_b, lim), lim >= yend: the bound of the
+// rows the kernel stores (conv_tc), or cap (resstack, whose tensor maps bound its loads and stores); rows_of(b, end) gives another.
+// The cursor is the ragged one's.
+struct WindowList {
+  const int* lens; int scale, cap, tile, y0, yend, lim;
+  int count, live;
+  int nblk, b, before, rows;       // cursor; rows = min(n_b, lim)
+  __device__ __forceinline__ int rows_of(int u, int end) const { return min(lens ? ragged_rows(lens, scale, cap, u) : cap, end); }
+  __device__ __forceinline__ int rows_of(int u) const { return rows_of(u, lim); }
+  __device__ __forceinline__ int tiles_of(int r) const { return max(0, min(r, yend) - y0 + tile - 1) / tile; }
+  __device__ __forceinline__ void init(const int* lens_, int scale_, int cap_, int B, int tile_, int blocks, int y0_, int yend_, int lim_) {
+    lens = lens_; scale = scale_; cap = cap_; tile = tile_; y0 = y0_; yend = yend_; lim = lim_;
+    live = 0;
+    for (int u = 0; u < B; u++) live += tiles_of(rows_of(u));
+    count = live * blocks;
+    nblk = 0; b = 0; before = 0; rows = rows_of(0);
+  }
+  __device__ __forceinline__ Item item(int i) {   // i < count, and not below the previous call's i
+    const int blk = i / live, rem = i - blk * live;
+    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(0); }
+    for (int nt = tiles_of(rows); rem >= before + nt; nt = tiles_of(rows)) {
+      before += nt;
+      rows = rows_of(++b);
+    }
+    Item it;
+    it.nblk = blk; it.b = b; it.t0 = y0 + (rem - before) * tile; it.rows = rows;
+    return it;
+  }
+};
+
 }  // namespace fs2

@@ -185,11 +185,13 @@ class Generator(nn.Module):
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):   # per-device kernel setup: CURRENT device
             return self._forward(x, mel_lens)
 
-    def _forward(self, x, mel_lens=None):
+    def _inputs(self, x, mel_lens):
+        """Checks the arguments of forward / stream and converts them once: (model, packed weights, device, up, B, T, channels-last mel
+        view, its batch and row strides, device mel_lens or None, stream)."""
         if self.training:
             raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
         lib = L.lib()
-        m, _keep, dev, up = self._packed or self._pack()
+        m, keep, dev, up = self._packed or self._pack()
         if x.dim() != 3 or x.shape[1] != m.n_mel:
             raise ValueError(f"expected mel of shape [B, {m.n_mel}, T]")
         x = x.to(device=dev, dtype=torch.float32)
@@ -210,6 +212,11 @@ class Generator(nn.Module):
             mel_cl = torch.empty(B, T, m.n_mel, dtype=torch.float32, device=dev)
             L.check(lib.fs2_transpose_bct_to_btc(xc.data_ptr(), mel_cl.data_ptr(), B, m.n_mel, T, stream), "fs2_transpose")
             bs, rs = T * m.n_mel, m.n_mel
+        return m, keep, dev, up, B, T, mel_cl, bs, rs, lens_d, stream
+
+    def _forward(self, x, mel_lens=None):
+        lib = L.lib()
+        m, _keep, dev, up, B, T, mel_cl, bs, rs, lens_d, stream = self._inputs(x, mel_lens)
         wav = torch.empty(B, 1, T * up, dtype=torch.float32, device=dev)
         need = lib.fs2_vocoder_workspace_bytes(C.byref(m), B, T)
         if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
@@ -218,3 +225,37 @@ class Generator(nn.Module):
                            workspace=self._ws.data_ptr(), workspace_bytes=self._ws.numel(), mel_lens=L.ptr(lens_d))
         L.check(lib.fs2_vocoder_forward(C.byref(m), C.byref(va), stream), "fs2_vocoder_forward")
         return wav
+
+    @torch.no_grad()
+    def stream(self, x, mel_lens=None, chunk_frames=64):
+        """Synthesise in chunks of `chunk_frames` mel frames: an iterator of (first_sample, wav_chunk[B, 1, n]), the chunks in order,
+        whose concatenation along the last axis equals forward(x, mel_lens) bit for bit (fs2_vocoder_forward_window).  Each chunk is
+        computed from the frames it needs plus the generator's receptive field, in a workspace that depends on B and chunk_frames, not
+        on T, and is ready as soon as it is yielded (on the current stream), before the rest of the utterance is synthesised.  The
+        arguments are those of forward and are checked, and the mel converted, once, when stream() is called; device mel_lens are
+        never read on the host, so every utterance runs the batch's T frames in lockstep (chunks past an utterance's end are zeros)."""
+        if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
+            raise ValueError("chunk_frames must be a positive int")
+        dev = get(self, "conv_pre.bias").device
+        with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
+            inputs = self._inputs(x, mel_lens)
+        return self._stream(inputs, chunk_frames)
+
+    def _stream(self, inputs, chunk_frames):
+        lib = L.lib()
+        m, _keep, dev, up, B, T, mel_cl, bs, rs, lens_d, _ = inputs    # _keep: the packed weights stay alive while the stream runs
+        with torch.no_grad(), torch.cuda.device(dev):
+            ws = None
+            for f0 in range(0, T, chunk_frames):
+                f1 = min(f0 + chunk_frames, T)
+                if ws is None:                                 # one workspace for every chunk
+                    need = lib.fs2_vocoder_window_workspace_bytes(C.byref(m), B, f1 - f0)
+                    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                n = (f1 - f0) * up
+                wav = torch.empty(B, 1, n, dtype=torch.float32, device=dev)
+                wa = L.VocoderWindowArgs(B=B, T=T, mel=mel_cl.data_ptr(), mel_batch_stride=bs, mel_row_stride=rs, wav=wav.data_ptr(),
+                                         workspace=ws.data_ptr(), workspace_bytes=ws.numel(), mel_lens=L.ptr(lens_d),
+                                         f0=f0, f1=f1, wav_batch_stride=n)
+                L.check(lib.fs2_vocoder_forward_window(C.byref(m), C.byref(wa), torch.cuda.current_stream(dev).cuda_stream),
+                        "fs2_vocoder_forward_window")
+                yield f0 * up, wav

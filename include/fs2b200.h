@@ -418,13 +418,60 @@ typedef struct fs2_vocoder_args {
 size_t fs2_vocoder_workspace_bytes(const fs2_vocoder_model* m, int B, int T);
 int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, fs2_stream_t stream);
 
+/* Windowed (streaming) vocoder: the waveform of the mel frames [f0, f1) of every utterance of the batch, bit for bit what
+ * fs2_vocoder_forward computes there.  With up = prod(rates) and n = (min(f1, T) - f0) * up, the call writes wav[b * wav_batch_stride + i]
+ * = forward's wav[b][f0 * up + i] for i < n (so wav may point at sample f0 * up of a preallocated [B][T * up] waveform, with
+ * wav_batch_stride T * up, or at a [B][n] chunk); ragged mode (mel_lens) and padded mode as in fs2_vocoder_forward, so samples at or
+ * past mel_lens[b] * up are zeros and an utterance that ends before f0 gives an all-zero chunk.  0 <= f0 < T and f0 < f1 (f1 may
+ * exceed T), else FS2_ERR_ARG before any CUDA call.
+ *   - stateless: a window depends only on mel, mel_lens, [f0, f1) and the weights; windows may be computed in any order, or twice;
+ *   - every layer computes only the rows later layers need (fs2_vocoder_window_plan): a window reads the mel frames
+ *     [f0 - halo, f1 + halo) of [0, mel_lens[b]) and nothing else, every intermediate likewise;
+ *   - the workspace, fs2_vocoder_window_workspace_bytes(m, B, f1 - f0) or that of any wider window, does not depend on T.
+ * Every layer pads at the utterance's ends, not at the window's, and keeps the offline call's kernel choice and arithmetic per
+ * output row (f8_mask, fused_mask, pair_mask, pair_kmax and the *_tc pointers apply unchanged). */
+typedef struct fs2_vocoder_window_args {
+  int B, T;
+  const float* mel; int64_t mel_batch_stride, mel_row_stride; /* channels-last view [B][T][n_mel], as in fs2_vocoder_args */
+  float* wav;                                                  /* sample f0 * up of utterance 0; see wav_batch_stride */
+  void* workspace; size_t workspace_bytes;
+  const int32_t* mel_lens;                                     /* NULL or [B] mel-frame lengths (device), as in fs2_vocoder_args */
+  int f0, f1;                                                  /* the window's mel frames */
+  int64_t wav_batch_stride;                                    /* floats between utterances of wav (>= n) */
+} fs2_vocoder_window_args;
+size_t fs2_vocoder_window_workspace_bytes(const fs2_vocoder_model* m, int B, int frames);
+int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, fs2_stream_t stream);
+
+/* One launch of a window (fs2_vocoder_window_plan).  Rows are logical rows at the launch's rate, `scale` rows per mel frame, clipped to
+ * the utterance's logical extent [0, T * scale); input and output share the rate (the ConvTranspose runs as two phase-group convs
+ * whose row q holds the next rate's rows [q * u, q * u + u)). */
+enum { FS2_VW_CONV_PRE = 0, FS2_VW_UP_A = 1, FS2_VW_UP_B = 2, FS2_VW_RB_CONV1 = 3, FS2_VW_RB_CONV2 = 4, FS2_VW_RB_PAIR = 5,
+       FS2_VW_RB_GROUP = 6, FS2_VW_CONV_POST = 7 };
+typedef struct fs2_vocoder_window_launch_t {
+  int32_t layer;        /* FS2_VW_* */
+  int32_t stage, j, d;  /* upsample stage, kernel-size and dilation index (-1 where they do not apply) */
+  int32_t scale;        /* rows per mel frame */
+  int32_t y0, y1;       /* output rows computed */
+  int32_t x0, x1;       /* input rows read */
+  int32_t src;          /* launch that produced the input (the last one writing it); -1: the mel */
+  int32_t res_src;      /* launch that produced the residual, read at rows [y0, y1); -1: none */
+  int32_t pad_;
+  double flops;         /* algorithmic FLOPs per utterance: every conv over the rows its consumers need, no tile rounding */
+} fs2_vocoder_window_launch_t;
+/* The launches of the window [f0, f1) of a T-frame batch in issue order, walked backward from the output samples: conv_post +-3
+ * rows, a ResBlock conv (k - 1) / 2 * dilation (a fused pair or group: its total reach), a ConvTranspose phase-group pair whose output
+ * rows [a, b) at the next rate read input rows [floor(a / u) - 1, ceil(b / u) + 1), conv_pre +-3.  Writes min(count, max_launches)
+ * records to out (may be NULL) and returns the count, or FS2_ERR_ARG.  Pure host logic: no CUDA call. */
+int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, fs2_vocoder_window_launch_t* out, int max_launches);
+
 /* ------------------------------------------------------------------ misc */
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
 const char* fs2_build_info(void);          /* "sm_90a ..." */
 /* sizeof of a struct above (binding self-check), fs2_<name>[_args]: 0 conv1d, 1 layernorm, 2 attention, 3 embed, 4 rowbias,
  * 5 variance_head, 6 durations, 7 length_regulate, 8 conv_post, 9 acoustic_model, 10 encode, 11 decode, 12 vocoder_model,
- * 13 vocoder, 14 resstack, 15 wav_int16, 16 conv_tc_plan_t, 17 conv_simt_plan_t, 18 resstack_plan_t */
+ * 13 vocoder, 14 resstack, 15 wav_int16, 16 conv_tc_plan_t, 17 conv_simt_plan_t, 18 resstack_plan_t.  Like fs2_control_args,
+ * fs2_vocoder_window_args (80 bytes) and fs2_vocoder_window_launch_t (56 bytes) are not in the table: the binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

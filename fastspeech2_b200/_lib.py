@@ -176,6 +176,16 @@ class VocoderWindowLaunch(C.Structure):
 VOCODER_WINDOW_ARGS_SIZE, VOCODER_WINDOW_LAUNCH_SIZE = 80, 56
 
 
+class VocoderStreamsArgs(C.Structure):
+    """fs2_vocoder_streams_args: B streams at their own frames f0[b] (64 bytes, pinned by a static_assert in model.cu)."""
+    _fields_ = [("B", i32), ("frames", i32), ("mel", fp), ("mel_lens", fp), ("f0", fp), ("wav", fp), ("wav_batch_stride", i64),
+                ("workspace", fp), ("workspace_bytes", C.c_size_t)]
+
+
+VOCODER_STREAMS_ARGS_SIZE = 64
+assert C.sizeof(VocoderStreamsArgs) == VOCODER_STREAMS_ARGS_SIZE
+
+
 class ConvTcPlan(C.Structure):
     _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")]
 
@@ -235,6 +245,8 @@ EXPORTS = {
     "fs2_vocoder_window_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward_window": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderWindowArgs), fp]),
     "fs2_vocoder_window_plan": (i32, [C.POINTER(VocoderModel), i32, i32, i32, C.POINTER(VocoderWindowLaunch), i32]),
+    "fs2_vocoder_streams_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
+    "fs2_vocoder_forward_streams": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsArgs), fp]),
 }
 
 _lib = None

@@ -71,6 +71,18 @@ __device__ __forceinline__ int ragged_rows(const int* lens, int scale, int cap, 
 // the window {0, cap, cap}.
 struct RowWindow { int y0, yend, xend; };
 
+// Per-utterance origin mode of the windowed layers (fs2_vocoder_forward_streams): every utterance has its own window, and row r of the
+// window buffers is utterance b's logical row r + org[b] * scale.  Rows stay window-relative in the kernels, so only the bounds move:
+// utterance b's live rows are [lo, hi) = [-org[b] * scale, (max(lens[b], 0) - org[b]) * scale), clamped to +-ORIGIN_CAP, which lies
+// beyond every window's rows (an empty span when lens[b] <= 0).  Device values are clamped, never trusted.
+constexpr int ORIGIN_CAP = 1 << 30;
+struct RowSpan { int lo, hi; };
+__device__ __forceinline__ int origin_clamp(long long v) { return v < -ORIGIN_CAP ? -ORIGIN_CAP : (v > ORIGIN_CAP ? ORIGIN_CAP : (int)v); }
+__device__ __forceinline__ RowSpan origin_rows(const int* lens, const int* org, int scale, int b) {
+  const long long o = __ldg(org + b), n = max(__ldg(lens + b), 0);
+  return RowSpan{origin_clamp(-o * scale), origin_clamp((n - o) * scale)};
+}
+
 // A per-element control of fs2_control_args on the [B][L] rows of a variance head or of the durations: c[b, l] = v[b * sb + l * sl]
 // (strides in elements, 0 along a broadcast dimension).  rag: NULL, or the ragged mode's lengths -- columns l >= rag[b] are not read.
 struct ControlView {

@@ -29,10 +29,12 @@ struct ConvP {
   int tiles_per_batch;
   const int* x_lens; int lens_scale;   // ragged batch (fs2_conv1d_args::x_lens) or NULL
   RowWindow win;                       // rows computed and read ({0, T, T} outside the windowed mode)
+  const int* org;                      // per-utterance origins (conv_simt_streams_kernel only), see origin_rows
 };
 
-template <int BM, int BN, int ACT>
-__global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
+// ORG: per-utterance origin mode (origin_rows): utterance b's rows below lo_b read as zero too, and n_b is hi_b
+template <int BM, int BN, int ACT, bool ORG>
+__device__ __forceinline__ void conv_simt_body(const ConvP& p) {
   constexpr int AS_LD = BM + 4;
   constexpr int TM = BM / 16;              // 8 or 4 rows per thread
   constexpr int A_PER_THREAD = BM * BK / 4 / 256;   // float4 loads of the A tile per thread (2 or 1)
@@ -51,7 +53,14 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   const int t0 = p.win.y0 + (blockIdx.x % p.tiles_per_batch) * BM;
   const int n0 = blockIdx.y * BN;
   // ragged batch: input rows t >= n_b read as zero, and a tile lying wholly at or beyond n_b has nothing to compute (its rows are unspecified)
-  const int n_b = p.x_lens ? ragged_rows(p.x_lens, p.lens_scale, p.T, b) : p.T;
+  int n_b, lo_b = 0;
+  if constexpr (ORG) {
+    const RowSpan r = origin_rows(p.x_lens, p.org, p.lens_scale, b);
+    n_b = r.hi; lo_b = r.lo;
+    if (t0 + BM <= lo_b) return;                         // a tile wholly below the utterance: nothing to compute
+  } else {
+    n_b = p.x_lens ? ragged_rows(p.x_lens, p.lens_scale, p.T, b) : p.T;
+  }
   if (t0 >= min(n_b, p.win.yend)) return;
   const int tend = min(n_b, p.win.xend);
 
@@ -78,7 +87,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
       const int row = f >> 2, c4 = f & 3;
       const int t = t0 + row + shift;
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (t >= 0 && t < tend && c0 + c4 * 4 < p.Cin) {
+      if (t >= lo_b && t < tend && c0 + c4 * 4 < p.Cin) {
         v = __ldg(reinterpret_cast<const float4*>(xb + (long long)t * p.xrs + c0 + c4 * 4));
         if (p.in_act == FS2_ACT_LRELU) {
           v.x = v.x > 0.f ? v.x : v.x * p.in_slope;
@@ -194,6 +203,17 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   }
 }
 
+template <int BM, int BN, int ACT>
+__global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
+  conv_simt_body<BM, BN, ACT, false>(p);
+}
+
+// Per-utterance origin mode (fs2_vocoder_forward_streams): an entry point of its own, so that the other modes keep their code
+template <int BM, int BN, int ACT>
+__global__ void __launch_bounds__(256) conv_simt_streams_kernel(const ConvP p) {
+  conv_simt_body<BM, BN, ACT, true>(p);
+}
+
 // Tile choice of the launcher (pure host logic, no CUDA call; exposed as fs2_conv_simt_plan so that the GPU tests' coverage of the six
 // (BM, BN) instantiations is checkable without a GPU).
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out) {
@@ -216,7 +236,8 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* 
 
 // win: NULL, or the windowed mode (RowWindow; a->T is then the full logical length): the tile is chosen for the window's rows.
 // Every output element sums its taps and channels in the same order whatever the tile, so a window computes the offline bits.
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win) {
+// org (with win and a->x_lens): NULL, or the per-utterance origins of the origin mode (origin_rows; a->T is not used).
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, const int* org) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
@@ -224,6 +245,8 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win) 
   if (a->res && ((a->res_row_stride & 3) || (a->res_batch_stride & 3))) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
   if (a->in_act != FS2_ACT_NONE && a->in_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;
+  if (org && (!win || !a->x_lens)) return FS2_ERR_ARG;
+  if (org && a->out_act != FS2_ACT_NONE && a->out_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;   // the vocoder's activations
   ConvP p;
   p.x = a->x; p.xbs = a->x_batch_stride; p.xrs = a->x_row_stride;
   p.B = a->B; p.T = a->T; p.Cin = a->Cin;
@@ -237,6 +260,7 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win) 
   p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
   p.win = win ? *win : RowWindow{0, a->T, a->T};
+  p.org = org;
   fs2_conv1d_args rows = *a;
   rows.T = p.win.yend - p.win.y0;
   if (rows.T <= 0) return FS2_ERR_ARG;
@@ -250,11 +274,16 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win) 
   const dim3 grid((unsigned)plan.grid_x, (unsigned)plan.grid_y);
   prof_before(s);
 #define FS2_SIMT_ACT(BM_, BN_)                                                                            \
-  switch (a->out_act) {                                                                                   \
-    case FS2_ACT_RELU: conv_simt_kernel<BM_, BN_, FS2_ACT_RELU><<<grid, 256, 0, s>>>(p); break;           \
-    case FS2_ACT_TANH: conv_simt_kernel<BM_, BN_, FS2_ACT_TANH><<<grid, 256, 0, s>>>(p); break;           \
-    case FS2_ACT_LRELU: conv_simt_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); break;         \
-    default: conv_simt_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p); break;                     \
+  if (org) {                                                                                              \
+    if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); \
+    else conv_simt_streams_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p);                        \
+  } else {                                                                                                \
+    switch (a->out_act) {                                                                                 \
+      case FS2_ACT_RELU: conv_simt_kernel<BM_, BN_, FS2_ACT_RELU><<<grid, 256, 0, s>>>(p); break;         \
+      case FS2_ACT_TANH: conv_simt_kernel<BM_, BN_, FS2_ACT_TANH><<<grid, 256, 0, s>>>(p); break;         \
+      case FS2_ACT_LRELU: conv_simt_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); break;       \
+      default: conv_simt_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p); break;                   \
+    }                                                                                                     \
   }
 #define FS2_SIMT_LAUNCH(BN_) \
   if (bm == 64) { FS2_SIMT_ACT(64, BN_) } else { FS2_SIMT_ACT(128, BN_) }

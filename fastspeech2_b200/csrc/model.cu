@@ -62,10 +62,10 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 }
 
 // kernels / launchers defined in the other translation units
-// win (the vocoder's windowed mode, RowWindow): NULL everywhere else
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr);
+// win (the vocoder's windowed mode, RowWindow) and org (its per-utterance origins, origin_rows): NULL everywhere else
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr, const int* org = nullptr);
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr);
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr, const int* org = nullptr);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
@@ -73,12 +73,12 @@ int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
 
 // backend dispatch of the fs2_conv1d contract
-static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr) {
+static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr, const int* org = nullptr) {
   if (!a) return FS2_ERR_ARG;
   if (a->x_lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win);
-  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win);
-  return conv1d_simt(a, s, win);
+  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win, org);
+  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win, org);
+  return conv1d_simt(a, s, win, org);
 }
 int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = false, int fused_from = 0);
 int embed_positions(const fs2_embed_args* a, cudaStream_t s);
@@ -87,8 +87,11 @@ int layernorm(const fs2_layernorm_args* a, cudaStream_t s);
 int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl = nullptr);
 int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr);
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win = nullptr, int x0 = 0);
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0,
+              const int* org = nullptr);
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win = nullptr, int x0 = 0, const int* org = nullptr);
+int stage_mel(const float* const* mel, const int32_t* lens, const int32_t* org, int B, int x0, int rows, int n_mel, float* out,
+              cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
@@ -547,9 +550,16 @@ struct View {
   int64_t bs() const { return (int64_t)rows * C; }
 };
 
+// What a walk issues: the batch's mel view and lengths, the waveform, and the offline call's five buffers, each B * width floats.
+// org: NULL (one window for the whole batch, fs2_vocoder_forward_window), or the per-utterance origin mode (fs2_vocoder_forward_streams):
+// the walk is then the unclipped plan of [0, frames), its rows are window rows, utterance b's window starts at its frame org[b]
+// (origin_rows), and the mel is the staged window buffer.
 struct WinExec {
-  const fs2_vocoder_window_args* a; cudaStream_t s;
-  float *bx, *bu, *bt, *r1, *r2;                       // the offline call's five buffers, each B * width floats
+  int B; cudaStream_t s;
+  const float* mel; int64_t mel_bs, mel_rs;
+  const int32_t* lens; const int32_t* org;
+  float* wav; int64_t wav_bs;
+  float *bx, *bu, *bt, *r1, *r2;
 };
 
 // fs2_conv1d arguments of a windowed launch: `cap` (a.T) is the layer's full logical length; residual off, as conv_args leaves it
@@ -573,6 +583,9 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     sc[i + 1] = sc[i] * m->rates[i];
   }
   auto cap = [&](int scale) { return T < 0 ? -1LL : (long long)T * scale; };
+  // the kernels' logical length at `scale` rows per frame; the origin mode bounds every utterance by itself (origin_rows)
+  const int* org = ex ? ex->org : nullptr;
+  auto len = [&](int scale) { return org ? ORIGIN_CAP : T * scale; };
   // ---- backward: O[i + 1] = the rows stage i's output must hold (O[0]: conv_pre's), U[i] = its ResBlocks' input, Q[i] = the
   // ConvTranspose's phase-group rows
   Rows O[FS2_MAX_STAGES + 1], U[FS2_MAX_STAGES], Q[FS2_MAX_STAGES];
@@ -598,20 +611,19 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     L.push_back(l);
     return (int)L.size() - 1;
   };
-  const fs2_vocoder_window_args* a = ex ? ex->a : nullptr;
-  const int B = a ? a->B : 0;
-  const int32_t* lens = a ? a->mel_lens : nullptr;
+  const int B = ex ? ex->B : 0;
+  const int32_t* lens = ex ? ex->lens : nullptr;
   cudaStream_t s = ex ? ex->s : nullptr;
   int C = m->c0;
   const Rows mel = widen(O[0], 3, cap(1));
   int last = add(FS2_VW_CONV_PRE, -1, -1, -1, 1, O[0], mel, -1, -1, 2.0 * O[0].n() * m->n_mel * 7 * C);
   View bx{ex ? ex->bx : nullptr, O[0].lo, O[0].n(), C};
   if (ex) {
-    fs2_conv1d_args c = win_conv_args(a->mel, a->mel_batch_stride, a->mel_row_stride, B, T, m->n_mel, bx, C, 7);
+    fs2_conv1d_args c = win_conv_args(ex->mel, ex->mel_bs, ex->mel_rs, B, len(1), m->n_mel, bx, C, 7);
     c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
     c.x_lens = lens; c.lens_scale = 1;
     const RowWindow w{O[0].lo, O[0].hi, mel.hi};
-    FS2_TRY(conv1d_dispatch(&c, s, &w));
+    FS2_TRY(conv1d_dispatch(&c, s, &w, org));
   }
   const float inv_nk = 1.f / (float)m->n_kernels;
   for (int i = 0; i < n; i++) {
@@ -626,7 +638,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       up_src = add(g == 0 ? FS2_VW_UP_A : FS2_VW_UP_B, i, -1, -1, s0, Q[i], x, last, -1, up_flops);
       if (!ex) continue;
       const size_t off = (size_t)g * (u / 2) * Co;
-      fs2_conv1d_args c = win_conv_args(bx.at(), bx.bs(), C, B, T * s0, C, bu, (u / 2) * Co, 2);
+      fs2_conv1d_args c = win_conv_args(bx.at(), bx.bs(), C, B, len(s0), C, bu, (u / 2) * Co, 2);
       c.y += off;
       c.pad_left = g == 0 ? 1 : 0;
       c.w = g == 0 ? m->w_up_a[i] : m->w_up_b[i];
@@ -635,7 +647,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
       c.x_lens = lens; c.lens_scale = s0;
       const RowWindow w{Q[i].lo, Q[i].hi, x.hi};
-      FS2_TRY(conv1d_dispatch(&c, s, &w));
+      FS2_TRY(conv1d_dispatch(&c, s, &w, org));
     }
     C = Co;
     const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
@@ -654,15 +666,15 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       last = add(FS2_VW_RB_GROUP, i, -1, -1, s1, O[i + 1], U[i], up_src, -1, fl);
       bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
       if (ex) {
-        fs2_resstack_args g = resblock_args(m, i, B, T * s1, C, lens, s1);
+        fs2_resstack_args g = resblock_args(m, i, B, len(s1), C, lens, s1);
         g.x = in.p; g.y = bx.p;
         const RowWindow w{O[i + 1].lo, O[i + 1].hi, in.lo + in.rows};
-        FS2_TRY(resstack(&g, s, &w, in.lo));
+        FS2_TRY(resstack(&g, s, &w, in.lo, org));
       }
       continue;
     }
     bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
-    const fs2_resstack_args group = ex ? resblock_args(m, i, B, T * s1, C, lens, s1) : fs2_resstack_args{};
+    const fs2_resstack_args group = ex ? resblock_args(m, i, B, len(s1), C, lens, s1) : fs2_resstack_args{};
     for (int j = 0; j < m->n_kernels; j++) {
       const int rb = i * m->n_kernels + j, k = m->rb_k[j];
       Rows R[FS2_MAX_DIL];                             // output rows of pair d
@@ -683,7 +695,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
             fs2_resstack_args p = resblock_pair(group, j, d);
             p.x = r.p; p.y = dst.p; p.alpha = alpha; p.accumulate = accumulate;
             const RowWindow w{R[d].lo, R[d].hi, r.lo + r.rows};
-            FS2_TRY(resstack(&p, s, &w, r.lo));
+            FS2_TRY(resstack(&p, s, &w, r.lo, org));
           }
           r_src = id;
         } else {
@@ -692,20 +704,20 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
           if (ex) {
             const int dil = m->rb_dil[j][d];
             const View t{ex->bt, mid.lo, mid.n(), C};
-            fs2_conv1d_args c = win_conv_args(r.at(), r.bs(), C, B, T * s1, C, t, C, k);
+            fs2_conv1d_args c = win_conv_args(r.at(), r.bs(), C, B, len(s1), C, t, C, k);
             c.w = m->w_rb1[rb][d]; c.w_tc = m->w_rb1_tc[rb][d]; c.bias = m->b_rb1[rb][d]; c.tc_variant = tcv;
             c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
             c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
             c.x_lens = lens; c.lens_scale = s1;
             const RowWindow w1{mid.lo, mid.hi, x.hi};
-            FS2_TRY(conv1d_dispatch(&c, s, &w1));
-            c = win_conv_args(t.at(), t.bs(), C, B, T * s1, C, dst, C, k);
+            FS2_TRY(conv1d_dispatch(&c, s, &w1, org));
+            c = win_conv_args(t.at(), t.bs(), C, B, len(s1), C, dst, C, k);
             c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
             c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
             c.alpha = alpha; c.accumulate = accumulate;
             c.x_lens = lens; c.lens_scale = s1;
             const RowWindow w2{R[d].lo, R[d].hi, mid.hi};
-            FS2_TRY(conv1d_dispatch(&c, s, &w2));
+            FS2_TRY(conv1d_dispatch(&c, s, &w2, org));
           }
           r_src = c2;
         }
@@ -717,11 +729,11 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   add(FS2_VW_CONV_POST, -1, -1, -1, sc[n], post, O[n], last, -1, 2.0 * post.n() * C * 7);
   if (!ex) return FS2_OK;
   fs2_conv_post_args p{};
-  p.x = bx.at(); p.B = B; p.T = T * sc[n]; p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
-  p.wav = a->wav - post.lo;                            // sample f0 * up is the caller's wav[0]
+  p.x = bx.at(); p.B = B; p.T = len(sc[n]); p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
+  p.wav = ex->wav - post.lo;                           // sample f0 * up is the caller's wav[0]
   p.lens = lens; p.lens_scale = sc[n];
   const RowWindow w{post.lo, post.hi, O[n].hi};
-  return conv_post(&p, s, &w, bx.bs(), a->wav_batch_stride);
+  return conv_post(&p, s, &w, bx.bs(), ex->wav_bs, org);
 }
 
 // Floats per utterance of each of the five buffers of a window of `frames` frames: the widest output of its unclipped plan
@@ -744,11 +756,32 @@ static int vocoder_window_impl(const fs2_vocoder_model* m, const fs2_vocoder_win
   size_t width = 0;
   FS2_TRY(window_width(m, frames, width));
   const size_t nf = (size_t)a->B * width;
-  WinExec ex{a, s, ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
+  WinExec ex{a->B, s, a->mel, a->mel_batch_stride, a->mel_row_stride, a->mel_lens, nullptr, a->wav, a->wav_batch_stride,
+             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
   if (ar.dry) return FS2_OK;
   if (!ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
   std::vector<fs2_vocoder_window_launch_t> L;
   return window_walk(m, a->T, a->f0, a->f1 < a->T ? a->f1 : a->T, L, &ex);
+}
+
+// fs2_vocoder_forward_streams: the unclipped plan of [0, frames) once for the whole batch, each stream at its own origin.  The mel cone
+// (conv_pre's input rows [x0, x1) of that plan) is staged first, [B][x1 - x0][n_mel], so that conv_pre reads one batch-strided buffer.
+static int vocoder_streams_impl(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, cudaStream_t s, Arena& ar) {
+  size_t width = 0;
+  FS2_TRY(window_width(m, a->frames, width));
+  std::vector<fs2_vocoder_window_launch_t> L;
+  FS2_TRY(window_walk(m, -1, 0, a->frames, L, nullptr));
+  const int x0 = L[0].x0, rows = L[0].x1 - L[0].x0;     // launch 0 is conv_pre
+  const size_t nf = (size_t)a->B * width;
+  float* mel = ar.f32((size_t)a->B * rows * m->n_mel);
+  WinExec ex{a->B, s, nullptr, (int64_t)rows * m->n_mel, m->n_mel, a->mel_lens, a->f0, a->wav, a->wav_batch_stride,
+             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
+  if (ar.dry) return FS2_OK;
+  if (!mel || !ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
+  FS2_TRY(stage_mel(a->mel, a->mel_lens, a->f0, a->B, x0, rows, m->n_mel, mel, s));
+  ex.mel = mel - (ptrdiff_t)x0 * m->n_mel;             // window row 0 of stream 0 (the conv reads rows [x0, x1) only)
+  L.clear();
+  return window_walk(m, -1, 0, a->frames, L, &ex);
 }
 
 }  // namespace fs2
@@ -947,6 +980,28 @@ int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_win
   if (a->B > 1 && a->wav_batch_stride < frames * up) return FS2_ERR_ARG;
   Arena ar(a->workspace, a->workspace_bytes);
   return vocoder_window_impl(m, a, frames, S(st), ar);
+}
+
+static_assert(sizeof(fs2_vocoder_streams_args) == 64, "fs2_vocoder_streams_args: two int32, five pointers, an int64 and a size_t");
+
+size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
+  if (!vocoder_ok(m) || B <= 0 || frames <= 0 || !window_rows_ok(m, frames)) return 0;
+  Arena ar(nullptr, 0);
+  fs2_vocoder_streams_args a{};
+  a.B = B; a.frames = frames;
+  if (vocoder_streams_impl(m, &a, nullptr, ar) != FS2_OK) return 0;
+  return ar.off + 256;
+}
+
+int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t st) {
+  if (!vocoder_ok(m) || !a || a->B <= 0 || a->frames <= 0 || !window_rows_ok(m, a->frames)) return FS2_ERR_ARG;
+  if (!a->mel || !a->mel_lens || !a->f0 || !a->wav || !a->workspace) return FS2_ERR_ARG;
+  long long up = 1;
+  for (int i = 0; i < m->n_stages; i++) up *= m->rates[i];
+  if (a->B > 1 && a->wav_batch_stride < a->frames * up) return FS2_ERR_ARG;
+  if (a->workspace_bytes < fs2_vocoder_streams_workspace_bytes(m, a->B, a->frames)) return FS2_ERR_ARG;
+  Arena ar(a->workspace, a->workspace_bytes);
+  return vocoder_streams_impl(m, a, S(st), ar);
 }
 
 int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, fs2_vocoder_window_launch_t* out, int max_launches) {

@@ -56,6 +56,7 @@ struct RsP {
   const int* lens; int lens_scale;   // ragged batch (fs2_resstack_args::lens) or NULL
   int x0;                            // windowed mode: logical row of the x map's row 0 (the y map's row 0 is win.y0)
   RowWindow win;                     // windowed mode: rows computed (win.xend is not read: the x map ends the input)
+  const int* org;                    // per-utterance origins (the streams entry points only), see origin_rows
 };
 
 // ------------------------------------------------------------------ TMA (tensor-map) wrappers
@@ -110,7 +111,9 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
 // WIN (with RAG): windowed mode, see WindowList.  The tensor maps span the window buffers: the x map's row 0 is logical row p.x0, the
 // y map's is p.win.y0.  Its zero fill beyond the x window only reaches slab rows whose results are never stored (the host sizes the x
 // window to the stored rows' receptive field), and the y map clips the stores to the window.
-template <int CG, int C, int MT, bool RAG, bool WIN = false>
+// ORG (with WIN): per-utterance origin mode, see origin_rows.  The zero fill covers only the buffer edges, so the slab rows of x below
+// lo_b are zeroed like those at or past n_b, and every conv's rows outside [lo_b, hi_b) are held at zero as outside [0, n_b).
+template <int CG, int C, int MT, bool RAG, bool WIN = false, bool ORG = false>
 __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUtensorMap& tmy, const RsP& p) {
   constexpr int KB = C / 16, R = MT * 128, NJ = C / 8;                // NJ: 8-column fragment groups of a row
   constexpr int BOXC = CG < 32 ? CG : 32, NH = CG / BOXC;             // channels per TMA box, boxes across a row
@@ -145,8 +148,8 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
   }
   fence_proxy_async();
   __syncthreads();
-  std::conditional_t<WIN, WindowList, WorkList<RAG>> work;   // TILE-row tiles of each utterance
-  if constexpr (WIN) work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, 1, p.win.y0, p.win.yend, p.N);
+  std::conditional_t<WIN, WindowList<ORG>, WorkList<RAG>> work;   // TILE-row tiles of each utterance
+  if constexpr (WIN) work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, 1, p.win.y0, p.win.yend, p.N, p.org);
   else work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, p.tiles_per_b, p.n_items);
   const int xorg = WIN ? p.x0 : 0, yorg = WIN ? p.win.y0 : 0;   // map row 0
 
@@ -186,6 +189,8 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
   for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
     const Item it = work.item(item);
     const int b = it.b, t0 = it.t0, nrows = it.rows;   // nrows: rows of utterance b (n_b of a ragged batch); the convs pad at its end
+    int lo = 0;                                        // and at its first row: 0, or lo_b in the origin mode
+    if constexpr (ORG) lo = work.lo_of(b);
     for (int j = 0; j < p.n_kernels; j++) {
       // ---- input: TMA boxes of x -> XT (idle: the last conv that read it has retired), then residual stream -> registers, lrelu(x) -> XA
       if (io) {
@@ -207,7 +212,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
             const int c = cbase + 8 * jj;
             if (8 * jj >= CG) { rs_store2(xa, CHUNK, row, c, 0.f, 0.f); continue; }   // zero-padded channels
             float2 u = *reinterpret_cast<const float2*>(xt + (size_t)((c / BOXC) * MT + m) * XBOX + rs_box_off<SW, BOXC>(r128, c));
-            if (RAG && t0 - p.H + row >= nrows) u = make_float2(0.f, 0.f);   // the padding of a ragged batch reads as zero
+            if (RAG && (t0 - p.H + row >= nrows || (ORG && t0 - p.H + row < lo))) u = make_float2(0.f, 0.f);   // the padding of a ragged batch reads as zero
             xr(i, 4 * jj + 2 * h) = u.x;
             xr(i, 4 * jj + 2 * h + 1) = u.y;
             rs_store2(xa, CHUNK, row, c, rs_lrelu(u.x), rs_lrelu(u.y));   // rows outside the utterance arrive as zeros (TMA fill)
@@ -258,7 +263,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
               for (int h = 0; h < 2; h++) {
                 const int row = rbase + 64 * i + 8 * h;
                 const int gr = t0 - p.H + row;
-                const bool in = gr >= 0 && gr < nrows;
+                const bool in = gr >= lo && gr < nrows;
 #pragma unroll
                 for (int jj = 0; jj < NJ; jj++) {
                   const int c = cbase + 8 * jj;
@@ -303,7 +308,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
                 for (int h = 0; h < 2; h++) {
                   const int row = rbase + 64 * i + 8 * h;
                   const int gr = t0 - p.H + row;
-                  const bool in = gr >= 0 && gr < nrows;
+                  const bool in = gr >= lo && gr < nrows;
                   const float s0 = acc[i][4 * jj + 2 * h] + corr[i][4 * jj + 2 * h], s1 = acc[i][4 * jj + 2 * h + 1] + corr[i][4 * jj + 2 * h + 1];
                   float v0 = fmaf(s0, inv_s, bv.x), v1 = fmaf(s1, inv_s, bv.y);
                   if (c2 == 0) {
@@ -369,6 +374,18 @@ template <int CG>
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_window_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                                const __grid_constant__ CUtensorMap tmy, const RsP p) {
   resstack_body<CG, 16, 8, true, true>(tmx, tmy, p);
+}
+
+// Per-utterance origin mode (fs2_vocoder_forward_streams): entry points of their own as well (p.org and the lens are not NULL here)
+template <int C, int MT>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_streams_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                         const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<C, C, MT, true, true, true>(tmx, tmy, p);
+}
+template <int CG>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_streams_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                                const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<CG, 16, 8, true, true, true>(tmx, tmy, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -448,12 +465,14 @@ static int make_map(CUtensorMap* tm, const float* base, int B, int N, int C, int
 }
 
 // win: NULL, or the windowed mode: a->x and a->y are then the window buffers [B][x1 - x0][C] and [B][yend - y0][C] (not biased), x0 /
-// x1 the logical rows a->x holds (win->xend is x1), and a->N the full logical length.
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, int x0) {
+// x1 the logical rows a->x holds (win->xend is x1), and a->N the full logical length.  org (with win and a->lens): NULL, or the
+// per-utterance origins of the origin mode (origin_rows; rows are then window rows and a->N is not used).
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, int x0, const int* org) {
   if (!a || !a->x || !a->y) return FS2_ERR_ARG;
   if (!aligned16(a->x) || !aligned16(a->y)) return FS2_ERR_ARG;
   if (a->B <= 0 || a->N <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
+  if (org && (!win || !a->lens)) return FS2_ERR_ARG;
   const int xrows = win ? win->xend - x0 : a->N, yrows = win ? win->yend - win->y0 : a->N;   // rows of the x and y buffers
   if (xrows <= 0 || yrows <= 0) return FS2_ERR_ARG;
   {  // not in place: a work item re-reads halo rows of x that its neighbours' results would already have overwritten
@@ -482,6 +501,10 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_window_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_window_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_window_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_streams_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_streams_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_streams_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_streams_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     return e;
   }));
   RsP p{};
@@ -500,11 +523,17 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
   p.alpha = a->alpha > 0.f ? a->alpha : 1.f / (float)a->n_kernels; p.accumulate = a->accumulate;
   p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
   p.x0 = x0; p.win = win ? *win : RowWindow{0, a->N, a->N};
+  p.org = org;
   alignas(64) CUtensorMap tmx, tmy;
   FS2_TRY(make_map(&tmx, a->x, a->B, xrows, a->C, 128));
   FS2_TRY(make_map(&tmy, a->y, a->B, yrows, a->C, p.OBOX));
   prof_before(s);
-  if (win) {
+  if (org) {
+    if (a->C == 32) resstack_streams_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 64) resstack_streams_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 16) resstack_narrow_streams_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_narrow_streams_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+  } else if (win) {
     if (a->C == 32) resstack_window_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 64) resstack_window_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 16) resstack_narrow_window_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);

@@ -368,15 +368,23 @@ int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s) {
 constexpr int CP_ROWS = 256;
 // Batch strides of x and wav and the rows computed and read: {T * C, T} and {0, T, T} outside the windowed mode (RowWindow; a.T is then
 // the full logical length, and x / wav are biased by the windows' first rows).
-struct PostRows { long long xbs, wbs; RowWindow win; };
-__global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
+// org: NULL, or the per-utterance origins of the origin mode (origin_rows): rows and samples outside [lo_b, hi_b) read and write zero.
+struct PostRows { long long xbs, wbs; RowWindow win; const int* org; };
+template <bool ORG>
+__device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
   extern __shared__ float cp_smem[];
   const int C = a.C, ld = C + 1, pad = (a.taps - 1) / 2;
   float* wsm = cp_smem;                   // [taps][C]
   float* xs = cp_smem + a.taps * C;       // [CP_ROWS + taps - 1][C + 1]
   const int b = blockIdx.x / tiles_per_batch;
   const int t0 = pr.win.y0 + (blockIdx.x % tiles_per_batch) * CP_ROWS;
-  const int n_b = a.lens ? ragged_rows(a.lens, a.lens_scale, a.T, b) : a.T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  int n_b, lo_b = 0;
+  if constexpr (ORG) {
+    const RowSpan r = origin_rows(a.lens, pr.org, a.lens_scale, b);
+    n_b = r.hi; lo_b = r.lo;
+  } else {
+    n_b = a.lens ? ragged_rows(a.lens, a.lens_scale, a.T, b) : a.T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  }
   const int nin = min(n_b, pr.win.xend);
   for (int i = threadIdx.x; i < a.taps * C; i += blockDim.x) wsm[i] = a.w[i];
   const int rows = CP_ROWS + a.taps - 1, C4 = C / 4;
@@ -385,7 +393,10 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
     const int r = i / C4, c4 = i - r * C4;
     const int t = t0 - pad + r;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t >= 0 && t < nin) {
+    bool in;
+    if constexpr (ORG) in = t >= lo_b && t < nin;
+    else in = t >= 0 && t < nin;
+    if (in) {
       v = __ldg(xb + (long long)t * C4 + c4);
       v.x = v.x > 0.f ? v.x : v.x * a.in_slope;
       v.y = v.y > 0.f ? v.y : v.y * a.in_slope;
@@ -405,7 +416,15 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 #pragma unroll 8
     for (int c = 0; c < C; c++) acc = fmaf(xr[c], wj[c], acc);
   }
-  a.wav[(long long)b * pr.wbs + t] = t < n_b ? tanhf(acc) : 0.f;
+  a.wav[(long long)b * pr.wbs + t] = (t < n_b && (!ORG || t >= lo_b)) ? tanhf(acc) : 0.f;
+}
+
+__global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
+  conv_post_body<false>(a, tiles_per_batch, pr);
+}
+// Per-utterance origin mode (fs2_vocoder_forward_streams): entry points of their own, so that the other modes keep their code
+__global__ void __launch_bounds__(CP_ROWS) conv_post_streams_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
+  conv_post_body<true>(a, tiles_per_batch, pr);
 }
 
 // The generator's own shape (32 channels, 7 taps, hifigan/models.py:131): no shared memory at all.  Eight lanes own one time row (one
@@ -415,9 +434,10 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 // full 32-byte sectors.  (The staged kernel above issues two shared-memory loads per FMA and measured 263 us = 2.0 TB/s at
 // B = 16 x 259k samples; this one is bound by the single read of x.)
 constexpr int CPF_BLOCKS = 18;                         // row blocks of TAPS rows per 8-lane group
-// RAG: ragged batch (a.lens != NULL); a template parameter so that the padded path keeps its code and registers
-template <int TAPS, bool RAG>
-__global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups, const PostRows pr) {
+// RAG: ragged batch (a.lens != NULL); a template parameter so that the padded path keeps its code and registers.  ORG (with RAG): the
+// per-utterance origin mode.
+template <int TAPS, bool RAG, bool ORG>
+__device__ __forceinline__ void conv_post_c32_body(const fs2_conv_post_args a, int groups_per_batch, long long n_groups, const PostRows pr) {
   constexpr int PAD = (TAPS - 1) / 2, ROWS = CPF_BLOCKS * TAPS - 2 * PAD;     // output rows per group (120 for 7 taps: a multiple of 8)
   static_assert(ROWS % 8 == 0, "full 8-sample stores");
   const int lane = threadIdx.x & 31, sub = lane & 7;
@@ -428,7 +448,13 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
   const int t0 = pr.win.y0 + (int)(grp - (long long)b * groups_per_batch) * ROWS;
   const int T = live ? a.T : 0;
   const int tend = min(t0 + ROWS, live ? pr.win.yend : 0);
-  const int n_b = RAG ? ragged_rows(a.lens, a.lens_scale, T, b) : T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  int n_b, lo_b = 0;
+  if constexpr (ORG) {
+    const RowSpan r = origin_rows(a.lens, pr.org, a.lens_scale, b);
+    n_b = live ? r.hi : 0; lo_b = live ? r.lo : 0;
+  } else {
+    n_b = RAG ? ragged_rows(a.lens, a.lens_scale, T, b) : T;   // ragged batch: rows >= n_b read as zero, wav there is 0
+  }
   const int nin = min(n_b, pr.win.xend);
   float4 w[TAPS];
 #pragma unroll
@@ -447,7 +473,7 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
 #pragma unroll
     for (int i = 0; i < TAPS; i++) {
       const int r = rb + i;
-      x[i] = (r >= 0 && r < nin) ? __ldg(xb + (long long)r * 8) : make_float4(0.f, 0.f, 0.f, 0.f);
+      x[i] = (r >= lo_b && r < nin) ? __ldg(xb + (long long)r * 8) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
     for (int i = 0; i < TAPS; i++) {
@@ -472,19 +498,31 @@ __global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_
         const int o = (t - t0) & 7;
         if (o == sub) keep = tot;
         if (o == 7 || t == tend - 1) {
-          if (sub <= o) wb[t - o + sub] = (!RAG || t - o + sub < n_b) ? tanhf(keep + bias) : 0.f;
+          if (sub <= o) wb[t - o + sub] = (!RAG || (t - o + sub < n_b && (!ORG || t - o + sub >= lo_b))) ? tanhf(keep + bias) : 0.f;
         }
       }
     }
   }
 }
 
+template <int TAPS, bool RAG>
+__global__ void __launch_bounds__(256) conv_post_c32_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups, const PostRows pr) {
+  conv_post_c32_body<TAPS, RAG, false>(a, groups_per_batch, n_groups, pr);
+}
+template <int TAPS>
+__global__ void __launch_bounds__(256) conv_post_c32_streams_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups,
+                                                                    const PostRows pr) {
+  conv_post_c32_body<TAPS, true, true>(a, groups_per_batch, n_groups, pr);
+}
+
 // win: NULL, or the windowed mode (a->T is then the full logical length, a->x and a->wav are biased by the windows' first rows and
 // their batch strides are x_bs and wav_bs).  Both kernels add every output's taps in the same order wherever its tile starts.
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win, long long x_bs, long long wav_bs) {
+// org (with win and a->lens): NULL, or the per-utterance origins of the origin mode (origin_rows; a->T is not used).
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win, long long x_bs, long long wav_bs, const int* org) {
   if (!a || !a->x || !a->w || !a->bias || !a->wav || a->B <= 0 || a->T <= 0 || a->C <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  const PostRows pr = win ? PostRows{x_bs, wav_bs, *win} : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}};
+  if (org && (!win || !a->lens)) return FS2_ERR_ARG;
+  const PostRows pr = win ? PostRows{x_bs, wav_bs, *win, org} : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr};
   const int rows = pr.win.yend - pr.win.y0;
   if (rows <= 0) return FS2_ERR_ARG;
   if (a->C == 32 && a->taps == 7 && (reinterpret_cast<uintptr_t>(a->x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15u) == 0) {
@@ -493,7 +531,8 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win,
     const long long n_groups = (long long)gpb * a->B, blocks = (n_groups * 8 + 255) / 256;
     if (blocks > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
     prof_before(s);
-    if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    if (org) conv_post_c32_streams_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    else if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     prof_after(s, 3, 2.0 * (double)a->B * rows * a->taps * a->C);
     FS2_LAUNCH_CHECK();
@@ -505,8 +544,40 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win,
   const long long n = (long long)a->B * rows;
   if ((long long)tiles * a->B > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   prof_before(s);
-  conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
+  if (org) conv_post_streams_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
+  else conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   prof_after(s, 3, 2.0 * n * a->taps * a->C);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+// ------------------------------------------------------------------ mel staging of fs2_vocoder_forward_streams
+// out[b][r] = stream b's mel row org[b] + x0 + r for r < rows, zeros where that row lies outside [0, max(lens[b], 0)): the one kernel
+// that reads the per-stream pointer table, so the window kernels after it see one batch-strided buffer.  n_mel % 4 == 0 and 16-byte
+// aligned rows (float4 loads); rows outside the utterance are never dereferenced.
+__global__ void stage_mel_kernel(const float* const* mel, const int* lens, const int* org, int x0, int rows, int n4, float4* out,
+                                 long long total) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long br = i / n4;
+    const int c4 = (int)(i - br * n4);
+    const int b = (int)(br / rows), r = (int)(br - (long long)b * rows);
+    const long long t = (long long)__ldg(org + b) + x0 + r;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (t >= 0 && t < __ldg(lens + b)) v = __ldg(reinterpret_cast<const float4*>(mel[b]) + t * n4 + c4);
+    out[i] = v;
+  }
+}
+
+int stage_mel(const float* const* mel, const int32_t* lens, const int32_t* org, int B, int x0, int rows, int n_mel, float* out,
+              cudaStream_t s) {
+  if (!mel || !lens || !org || !out || B <= 0 || rows <= 0 || n_mel <= 0) return FS2_ERR_ARG;
+  if (n_mel % 4 || !aligned16(out)) return FS2_ERR_UNSUPPORTED;
+  const long long total = (long long)B * rows * (n_mel / 4);
+  const long long blocks = (total + 255) / 256;
+  prof_before(s);
+  stage_mel_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(mel, lens, org, x0, rows, n_mel / 4,
+                                                                             reinterpret_cast<float4*>(out), total);
+  prof_after(s, 3, 0.0);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }

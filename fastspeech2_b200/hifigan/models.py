@@ -7,6 +7,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -259,3 +260,107 @@ class Generator(nn.Module):
                 L.check(lib.fs2_vocoder_forward_window(C.byref(m), C.byref(wa), torch.cuda.current_stream(dev).cuda_stream),
                         "fs2_vocoder_forward_window")
                 yield f0 * up, wav
+
+    def stream_pool(self, chunk_frames=64):
+        """A pool of independent streams vocoded together (fs2_vocoder_forward_streams), for serving requests that arrive at different
+        times: StreamPool.add(mel) admits a stream, and every StreamPool.step() synthesises the next `chunk_frames` frames of every live
+        stream in one call, each at its own position.  Concatenated, one stream's chunks equal self(mel[None]) bit for bit, whatever else
+        shares the pool.  It uses the weights packed at creation, like stream(); the workspace depends on the live count and
+        chunk_frames, not on any length."""
+        if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
+            raise ValueError("chunk_frames must be a positive int")
+        if self.training:
+            raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
+        dev = get(self, "conv_pre.bias").device
+        with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
+            m, keep, dev, up = self._packed or self._pack()
+        lib = L.lib()
+        ws = [None]
+
+        def launch(ptrs, f0s, ns):
+            """One fs2_vocoder_forward_streams call on the current stream: uploads the (pointer, f0, n) table from a fresh pinned block
+            with one non_blocking copy (the caching host allocator keeps the block until the copy is done; no host sync)."""
+            B, n = len(ptrs), chunk_frames * up
+            with torch.cuda.device(dev):
+                host = torch.empty(4 * B, dtype=torch.int32, pin_memory=True)
+                h = host.numpy()
+                h[:2 * B].view(np.int64)[:] = ptrs
+                h[2 * B:3 * B] = f0s
+                h[3 * B:] = ns
+                table = host.to(dev, non_blocking=True)
+                need = lib.fs2_vocoder_streams_workspace_bytes(C.byref(m), B, chunk_frames)
+                if ws[0] is None or ws[0].numel() < need:
+                    ws[0] = torch.empty(need, dtype=torch.uint8, device=dev)
+                wav = torch.empty(B, n, dtype=torch.float32, device=dev)
+                base = table.data_ptr()
+                sa = L.VocoderStreamsArgs(B=B, frames=chunk_frames, mel=base, mel_lens=base + 12 * B, f0=base + 8 * B, wav=wav.data_ptr(),
+                                          wav_batch_stride=n, workspace=ws[0].data_ptr(), workspace_bytes=ws[0].numel())
+                L.check(lib.fs2_vocoder_forward_streams(C.byref(m), C.byref(sa), torch.cuda.current_stream(dev).cuda_stream),
+                        "fs2_vocoder_forward_streams")
+            return wav
+
+        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev)
+        pool._keep = keep                              # the packed weights stay alive while the pool runs
+        return pool
+
+
+class StreamPool:
+    """Streams vocoded together in chunks of `chunk_frames` mel frames (Generator.stream_pool).  Streams are kept in admission order;
+    each starts at frame 0 in the step after its add() and leaves after its last chunk.  `launch(ptrs, f0s, ns)` computes one step: the
+    [B, chunk_frames * up] waveform of the live streams, stream b from its frame f0s[b] of the ns[b] frames at device address ptrs[b]."""
+
+    def __init__(self, launch, n_mel, up, chunk_frames, device):
+        self._launch, self.n_mel, self.up, self.chunk_frames, self.device = launch, n_mel, up, chunk_frames, torch.device(device)
+        self._live = []                                # [handle, channels-last mel view [n, n_mel], n, next frame]
+        self._next = 0
+
+    def add(self, mel):
+        """Admits a stream.  mel: [n_mel, n] or [1, n_mel, n] on the pool's device, n >= 1.  A channels-last view with row stride n_mel
+        (FastSpeech2's postnet_mel[b, :n].T is one) is kept without a copy; any other layout is converted once.  Returns the handle."""
+        if not isinstance(mel, torch.Tensor):
+            raise ValueError("mel must be a tensor")
+        if mel.dim() == 3 and mel.shape[0] == 1:
+            mel = mel[0]
+        if mel.dim() != 2 or mel.shape[0] != self.n_mel:
+            raise ValueError(f"expected mel of shape [{self.n_mel}, n] or [1, {self.n_mel}, n]")
+        if mel.device != self.device:
+            raise ValueError(f"mel is on {mel.device}, the vocoder on {self.device}")
+        n = mel.shape[1]
+        if n < 1:
+            raise ValueError("mel has no frames")
+        rows = mel.T
+        if not (rows.dtype == torch.float32 and rows.stride(1) == 1 and (n == 1 or rows.stride(0) == self.n_mel) and rows.data_ptr() % 16 == 0):
+            rows = rows.to(torch.float32).contiguous()
+        h = self._next
+        self._next += 1
+        self._live.append([h, rows, n, 0])
+        return h
+
+    def cancel(self, h):
+        """Drops a live stream (KeyError if it is not live)."""
+        for i, s in enumerate(self._live):
+            if s[0] == h:
+                del self._live[i]
+                return
+        raise KeyError(h)
+
+    def __len__(self):
+        return len(self._live)
+
+    def step(self):
+        """One chunk of every live stream, in one launch call: a list of (handle, first_sample, wav [1, 1, m]) in admission order,
+        m = chunk_frames * up except on a stream's last chunk, which is trimmed to its end.  [] without a call when the pool is empty."""
+        if not self._live:
+            return []
+        live = self._live
+        wav = self._launch([s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live])
+        out, keep = [], []
+        for i, s in enumerate(live):
+            h, _, n, f0 = s
+            m = min(self.chunk_frames, n - f0) * self.up
+            out.append((h, f0 * self.up, wav[i:i + 1, :m].unsqueeze(0)))
+            s[3] = f0 + self.chunk_frames
+            if s[3] < n:
+                keep.append(s)
+        self._live = keep
+        return out

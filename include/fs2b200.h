@@ -464,6 +464,32 @@ typedef struct fs2_vocoder_window_launch_t {
  * records to out (may be NULL) and returns the count, or FS2_ERR_ARG.  Pure host logic: no CUDA call. */
 int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, fs2_vocoder_window_launch_t* out, int max_launches);
 
+/* Many independent streams in one call: stream b's window is its mel frames [f0[b], f0[b] + frames), each stream at its own position.
+ * With up = prod(rates), wav[b * wav_batch_stride + i] = fs2_vocoder_forward(stream b alone, a B = 1 batch of n_b = mel_lens[b]
+ * frames)'s wav[f0[b] * up + i] for 0 <= f0[b] * up + i < n_b * up, and 0 otherwise, for i < frames * up, bit for bit under every mask
+ * and policy fs2_vocoder_forward_window honours.  A stream's output does not depend on the other streams of the call.
+ *   - the host never reads f0, mel_lens or the pointer table: the launch plan is the unclipped plan of [0, frames)
+ *     (fs2_vocoder_window_plan's rows of a window that no utterance end clips), the grid is sized from B and that plan, and each
+ *     kernel bounds utterance b by its own origin: row r of a layer with `scale` rows per frame is live iff
+ *     0 <= r + f0[b] * scale < n_b * scale;
+ *   - any device values are memory-safe: stream b's mel is read only at rows of [0, n_b) inside its window's cone; f0[b] >= n_b or
+ *     n_b <= 0 gives an all-zero chunk, and rows before a negative f0[b] read as zero;
+ *   - one launch stages every stream's mel cone into the workspace ([B][cone rows][n_mel]); the rest are the launches of one
+ *     fs2_vocoder_forward_window of `frames` frames;
+ *   - B <= 0, frames <= 0, a NULL pointer, wav_batch_stride < frames * up with B > 1, or a workspace below
+ *     fs2_vocoder_streams_workspace_bytes(m, B, frames) is FS2_ERR_ARG before any CUDA call.  That bound depends on B and frames only:
+ *     the window's, plus the staged mel cone. */
+typedef struct fs2_vocoder_streams_args {
+  int B, frames;                  /* B streams, `frames` mel frames each */
+  const float* const* mel;        /* [B] device array: stream b's mel rows, n_mel contiguous floats per row, 16-byte aligned */
+  const int32_t* mel_lens;        /* [B] device: stream b's total frames n_b */
+  const int32_t* f0;              /* [B] device: stream b's first frame in this call */
+  float* wav; int64_t wav_batch_stride;   /* [B][frames * up] */
+  void* workspace; size_t workspace_bytes;
+} fs2_vocoder_streams_args;
+size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, int frames);
+int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ misc */
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
@@ -471,7 +497,8 @@ const char* fs2_build_info(void);          /* "sm_90a ..." */
 /* sizeof of a struct above (binding self-check), fs2_<name>[_args]: 0 conv1d, 1 layernorm, 2 attention, 3 embed, 4 rowbias,
  * 5 variance_head, 6 durations, 7 length_regulate, 8 conv_post, 9 acoustic_model, 10 encode, 11 decode, 12 vocoder_model,
  * 13 vocoder, 14 resstack, 15 wav_int16, 16 conv_tc_plan_t, 17 conv_simt_plan_t, 18 resstack_plan_t.  Like fs2_control_args,
- * fs2_vocoder_window_args (80 bytes) and fs2_vocoder_window_launch_t (56 bytes) are not in the table: the binding pins their sizes. */
+ * fs2_vocoder_window_args (80 bytes), fs2_vocoder_window_launch_t (56 bytes) and fs2_vocoder_streams_args (64 bytes) are not in the
+ * table: the binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

@@ -176,6 +176,15 @@ class VocoderWindowLaunch(C.Structure):
 VOCODER_WINDOW_ARGS_SIZE, VOCODER_WINDOW_LAUNCH_SIZE = 80, 56
 
 
+class ResblockRun(C.Structure):
+    """fs2_resblock_run_t: one fs2_resstack launch of a fused ResBlock stage (32 bytes, pinned by a static_assert in model.cu)."""
+    _fields_ = [(n, i32) for n in ("j", "d0", "d1", "H", "TILE", "slab")] + [("cost", C.c_double)]
+
+
+RESBLOCK_RUN_SIZE = 32
+assert C.sizeof(ResblockRun) == RESBLOCK_RUN_SIZE
+
+
 class VocoderStreamsArgs(C.Structure):
     """fs2_vocoder_streams_args: B streams at their own frames f0[b] (64 bytes, pinned by a static_assert in model.cu)."""
     _fields_ = [("B", i32), ("frames", i32), ("mel", fp), ("mel_lens", fp), ("f0", fp), ("wav", fp), ("wav_batch_stride", i64),
@@ -245,6 +254,7 @@ EXPORTS = {
     "fs2_vocoder_window_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward_window": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderWindowArgs), fp]),
     "fs2_vocoder_window_plan": (i32, [C.POINTER(VocoderModel), i32, i32, i32, C.POINTER(VocoderWindowLaunch), i32]),
+    "fs2_vocoder_resblock_runs": (i32, [C.POINTER(VocoderModel), i32, C.POINTER(ResblockRun), i32]),
     "fs2_vocoder_streams_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward_streams": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsArgs), fp]),
 }
@@ -292,6 +302,16 @@ def vocoder_window_plan(m, T, f0, f1):
     out = (VocoderWindowLaunch * n)()
     check(min(0, lib().fs2_vocoder_window_plan(C.byref(m), T, f0, f1, out, n)), "fs2_vocoder_window_plan")
     return list(out)
+
+
+def vocoder_resblock_runs(m, stage):
+    """The fs2_resstack launches of stage `stage`'s ResBlocks (fs2_vocoder_resblock_runs): a list of ResblockRun, [] outside fused_mask."""
+    n = lib().fs2_vocoder_resblock_runs(C.byref(m), stage, None, 0)
+    if n < 0:
+        check(n, "fs2_vocoder_resblock_runs")
+    out = (ResblockRun * max(n, 1))()
+    check(min(0, lib().fs2_vocoder_resblock_runs(C.byref(m), stage, out, n)), "fs2_vocoder_resblock_runs")
+    return list(out)[:n]
 
 
 def ptr(t):

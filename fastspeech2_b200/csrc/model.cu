@@ -89,11 +89,12 @@ int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_le
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0,
               const int* org = nullptr);
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win = nullptr, int x0 = 0, const int* org = nullptr);
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win = nullptr, int x0 = 0, const int* org = nullptr,
+             bool wide = false);
 int stage_mel(const float* const* mel, const int32_t* lens, const int32_t* org, int B, int x0, int rows, int n_mel, float* out,
               cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
-int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out);
+int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out, bool wide = false);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
 int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s);
 int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cudaStream_t s);
@@ -406,13 +407,17 @@ static fs2_resstack_args resblock_args(const fs2_vocoder_model* m, int i, int B,
   return a;
 }
 
-// The same arguments narrowed to the one (dilated conv, conv) pair (j, d); fs2_resstack reads only the first n_kernels x n_dil entries.
-static fs2_resstack_args resblock_pair(const fs2_resstack_args& g, int j, int d) {
+// The same arguments narrowed to ResBlock j's (dilated conv, conv) pairs [d0, d1); fs2_resstack reads only the first n_kernels x n_dil
+// entries.
+static fs2_resstack_args resblock_run(const fs2_resstack_args& g, int j, int d0, int d1) {
   fs2_resstack_args a = g;
-  a.n_kernels = 1; a.n_dil = 1;
-  a.k[0] = g.k[j]; a.dil[0][0] = g.dil[j][d];
-  a.w1_tc[0][0] = g.w1_tc[j][d]; a.b1[0][0] = g.b1[j][d];
-  a.w2_tc[0][0] = g.w2_tc[j][d]; a.b2[0][0] = g.b2[j][d];
+  a.n_kernels = 1; a.n_dil = d1 - d0;
+  a.k[0] = g.k[j];
+  for (int d = d0; d < d1; d++) {
+    a.dil[0][d - d0] = g.dil[j][d];
+    a.w1_tc[0][d - d0] = g.w1_tc[j][d]; a.b1[0][d - d0] = g.b1[j][d];
+    a.w2_tc[0][d - d0] = g.w2_tc[j][d]; a.b2[0][d - d0] = g.b2[j][d];
+  }
   return a;
 }
 
@@ -421,8 +426,88 @@ static bool resstack_width(int C) { return C == 8 || C == 16 || C == 32 || C == 
 // Stage i's operand format, and which of its ResBlock layers run as one fs2_resstack launch: the offline and the windowed walk share them
 static unsigned stage_tcv(const fs2_vocoder_model* m, int i) { return (m->f8_mask & (2 << i)) ? FS2_TC_VARIANT_F8 : 0; }
 static bool stage_fused(const fs2_vocoder_model* m, int i) { return (m->fused_mask >> i) & 1; }
+// A 128-channel stage pairs only with pair_mask bit 8 + i (its tiles are then packed at NB = 128, see fs2_vocoder_model::pair_mask)
 static bool stage_pairs(const fs2_vocoder_model* m, int i, int C, int k) {
-  return ((m->pair_mask >> i) & 1) && stage_tcv(m, i) && resstack_width(C) && k <= m->pair_kmax;
+  const bool on = C == 128 ? (m->pair_mask >> (8 + i)) & 1 : ((m->pair_mask >> i) & 1) && resstack_width(C);
+  return on && stage_tcv(m, i) && k <= m->pair_kmax;
+}
+
+// ------------------------------------------------------------------ ResBlock run planner (fs2_vocoder_resblock_runs)
+// Cost of one fs2_resstack launch in ns per output row of the stage.  A work item computes MT * 128 slab rows for TILE output rows, and
+// per slab row it spends `tap` ns per conv tap (the MMAs), `conv` ns per conv (the epilogue: operand split into shared memory, the
+// barrier) and `run` ns per kernel size (x in through TMA and its split, the result out: the fp32 round trip of an intermediate
+// between two runs is part of this term).  Fitted by least squares, by channels computed on chip, to the time of every cut of every
+// ResBlock (scripts/resblock_runs_bench.py --candidates, B = 16 x 1012 frames, padded) on an H100 80GB HBM3 (SXM) at a 700 W power
+// limit: V1's 64- and 32-channel stages (every cut within 2 % of the model) and V2's 16-channel stage (within 3 %).  The 8-channel
+// stage, computed on chip as 16 channels, uses the 16-channel rates: they overestimate it by about 40 % but rank its cuts as measured.
+struct RbNs { double tap, conv, run; };
+static RbNs rb_ns(int Cm) {
+  if (Cm >= 64) return {0.0169, 0.148, 0.215};
+  if (Cm >= 32) return {0.0055, 0.063, 0.101};
+  return {0.0026, 0.026, 0.041};
+}
+
+typedef fs2_resblock_run_t RbRun;
+constexpr int RB_MAX_RUNS = (FS2_MAX_DIL + 4) * FS2_MAX_DIL;
+
+// r.cost, H, TILE and slab of launching `a` (its j, d0, d1 are the caller's), or fs2_resstack's refusal of the shape
+static int run_cost(const fs2_resstack_args& a, RbRun& r) {
+  fs2_resstack_plan_t p;
+  FS2_TRY(resstack_plan(&a, 1, p));
+  const RbNs ns = rb_ns(a.C < 16 ? 16 : a.C);
+  double per_slab_row = 0;
+  for (int j = 0; j < a.n_kernels; j++) per_slab_row += ns.run + a.n_dil * 2 * (ns.conv + a.k[j] * ns.tap);
+  r.H = p.H; r.TILE = p.TILE; r.slab = p.MT * 128;
+  r.cost = per_slab_row * r.slab / r.TILE;
+  return FS2_OK;
+}
+
+// The launches of stage i's ResBlocks (stage i in fused_mask): the whole group, or for each ResBlock the cut of its dilations into
+// consecutive runs with the least modelled cost, whichever costs less (ties: fewer launches).  Returns the count.
+static int stage_runs(const fs2_vocoder_model* m, int i, RbRun* out) {
+  if (!resstack_width(m->c0 >> (i + 1))) return FS2_ERR_UNSUPPORTED;   // fused_mask serves 8 to 64 channels (128: pair_mask bit 8 + i)
+  const fs2_resstack_args g = resblock_args(m, i, 1, 1, m->c0 >> (i + 1), nullptr, 1);
+  RbRun whole{-1, 0, m->n_dil, 0, 0, 0, 0};
+  const bool whole_ok = run_cost(g, whole) == FS2_OK;
+  int n = 0;
+  double split = 0;
+  for (int j = 0; j < m->n_kernels; j++) {
+    RbRun best[FS2_MAX_DIL];
+    int nbest = 0;
+    double best_cost = 0;
+    for (int cuts = 0; cuts < 1 << (m->n_dil - 1); cuts++) {   // bit d: a run ends after dilation d
+      RbRun cand[FS2_MAX_DIL];
+      int nc = 0;
+      double c = 0;
+      bool ok = true;
+      for (int d0 = 0; d0 < m->n_dil && ok;) {
+        int d1 = d0 + 1;
+        while (d1 < m->n_dil && !((cuts >> (d1 - 1)) & 1)) d1++;
+        fs2_resstack_args a = resblock_run(g, j, d0, d1);
+        a.accumulate = d1 == m->n_dil && j > 0;
+        cand[nc] = RbRun{j, d0, d1, 0, 0, 0, 0};
+        ok = run_cost(a, cand[nc]) == FS2_OK;
+        c += cand[nc++].cost;
+        d0 = d1;
+      }
+      if (ok && (!nbest || c < best_cost || (c == best_cost && nc < nbest))) {
+        for (int r = 0; r < nc; r++) best[r] = cand[r];
+        nbest = nc; best_cost = c;
+      }
+    }
+    if (!nbest) {
+      if (!whole_ok) return FS2_ERR_UNSUPPORTED;
+      split = -1;
+      break;
+    }
+    for (int r = 0; r < nbest; r++) out[n++] = best[r];
+    split += best_cost;
+  }
+  if (whole_ok && (split < 0 || whole.cost <= split)) {
+    out[0] = whole;
+    return 1;
+  }
+  return n;
 }
 
 static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, cudaStream_t s, Arena& ar) {
@@ -479,11 +564,27 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
     }
     Ti *= u; C = Co; scale *= u;
     // ---- mean of the multi-receptive-field ResBlocks (models.py:154-160, ResBlock.forward :96-103)
-    fs2_resstack_args group = resblock_args(m, i, B, Ti, C, lens, scale);
-    if (stage_fused(m, i)) {                           // one persistent kernel for the whole group: intermediates never leave the SM
+    const fs2_resstack_args group = resblock_args(m, i, B, Ti, C, lens, scale);
+    if (stage_fused(m, i)) {                           // persistent kernels whose intermediates never leave the SM: the planner's runs
       if (!tcv) return FS2_ERR_ARG;
-      group.x = bu; group.y = bx;
-      FS2_TRY(resstack(&group, s));
+      RbRun runs[RB_MAX_RUNS];
+      const int nr = stage_runs(m, i, runs);
+      if (nr < 0) return nr;
+      const float* r = bu;
+      for (int q = 0; q < nr; q++) {
+        const RbRun& run = runs[q];
+        const bool last = run.d1 == m->n_dil;           // the last run of a ResBlock adds its share of the mean into bx
+        if (run.d0 == 0) r = bu;
+        float* dst = last ? bx : (r == r1 ? r2 : r1);
+        fs2_resstack_args a = group;                   // the whole group: alpha 0 (the mean), no accumulate
+        if (run.j >= 0) {
+          a = resblock_run(group, run.j, run.d0, run.d1);
+          a.alpha = last ? inv_nk : 1.f; a.accumulate = last && run.j > 0;
+        }
+        a.x = r; a.y = dst;
+        FS2_TRY(resstack(&a, s));
+        r = dst;
+      }
       continue;
     }
     for (int j = 0; j < m->n_kernels; j++) {
@@ -496,9 +597,9 @@ static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, c
         const float alpha = last ? inv_nk : 1.f;
         const int accumulate = last && j > 0;
         if (pairs) {                                   // one launch per (dilated conv, conv, +x) pair: the intermediate stays on chip
-          fs2_resstack_args p = resblock_pair(group, j, d);
+          fs2_resstack_args p = resblock_run(group, j, d, d + 1);
           p.x = r; p.y = dst; p.alpha = alpha; p.accumulate = accumulate;
-          FS2_TRY(resstack(&p, s));
+          FS2_TRY(resstack(&p, s, nullptr, 0, nullptr, C == 128));
         } else {                                       // the two convs through bt
           const int dil = m->rb_dil[j][d];
           c = conv_args(r, B, Ti, C, C, k, bt);
@@ -652,29 +753,52 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     C = Co;
     const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
     const long long cap1 = cap(s1);
-    if (stage_fused(m, i)) {
-      double fl = 0;
-      for (int j = 0; j < m->n_kernels; j++) {
-        Rows r = O[i + 1];
-        for (int d = m->n_dil - 1; d >= 0; d--) {
-          const int k = m->rb_k[j];
-          const Rows mid = widen(r, (k - 1) / 2, cap1);
-          fl += 2.0 * C * k * C * (mid.n() + r.n());
-          r = widen(mid, (k - 1) * m->rb_dil[j][d] / 2, cap1);
-        }
-      }
-      last = add(FS2_VW_RB_GROUP, i, -1, -1, s1, O[i + 1], U[i], up_src, -1, fl);
-      bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
-      if (ex) {
-        fs2_resstack_args g = resblock_args(m, i, B, len(s1), C, lens, s1);
-        g.x = in.p; g.y = bx.p;
-        const RowWindow w{O[i + 1].lo, O[i + 1].hi, in.lo + in.rows};
-        FS2_TRY(resstack(&g, s, &w, in.lo, org));
-      }
-      continue;
-    }
     bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
     const fs2_resstack_args group = ex ? resblock_args(m, i, B, len(s1), C, lens, s1) : fs2_resstack_args{};
+    // output rows of ResBlock j's pair d (R[j][d]) and the algorithmic FLOPs of its two convs
+    auto pair_rows = [&](int j, Rows* R, double* fl) {
+      const int k = m->rb_k[j];
+      R[m->n_dil - 1] = O[i + 1];
+      for (int d = m->n_dil - 1; d > 0; d--) R[d - 1] = widen(R[d], pair_reach(m, j, d), cap1);
+      for (int d = 0; d < m->n_dil; d++) fl[d] = 2.0 * C * k * C * (widen(R[d], (k - 1) / 2, cap1).n() + R[d].n());
+    };
+    if (stage_fused(m, i)) {                           // the planner's runs (fs2_vocoder_resblock_runs), each widened by its total reach
+      RbRun runs[RB_MAX_RUNS];
+      const int nr = stage_runs(m, i, runs);
+      if (nr < 0) return nr;
+      View r = in;
+      int r_src = up_src;
+      for (int q = 0; q < nr; q++) {
+        const RbRun& run = runs[q];
+        const bool lastd = run.d1 == m->n_dil;
+        Rows R[FS2_MAX_DIL], y = O[i + 1], x = U[i];
+        double fd[FS2_MAX_DIL], fl = 0;
+        for (int j = run.j < 0 ? 0 : run.j; j < (run.j < 0 ? m->n_kernels : run.j + 1); j++) {
+          pair_rows(j, R, fd);
+          for (int d = run.d0; d < run.d1; d++) fl += fd[d];
+        }
+        if (run.j >= 0) {
+          y = R[run.d1 - 1];
+          x = widen(R[run.d0], pair_reach(m, run.j, run.d0), cap1);
+        }
+        if (run.d0 == 0) { r = in; r_src = up_src; }
+        r_src = add(FS2_VW_RB_GROUP, i, run.j, run.j < 0 ? -1 : run.d0, s1, y, x, r_src, -1, fl);
+        const View dst{lastd ? bx.p : (ex && r.p == ex->r1 ? ex->r2 : (ex ? ex->r1 : nullptr)), y.lo, y.n(), C};
+        if (ex) {
+          fs2_resstack_args a = group;                 // the whole group: alpha 0 (the mean), no accumulate
+          if (run.j >= 0) {
+            a = resblock_run(group, run.j, run.d0, run.d1);
+            a.alpha = lastd ? inv_nk : 1.f; a.accumulate = lastd && run.j > 0;
+          }
+          a.x = r.p; a.y = dst.p;
+          const RowWindow w{y.lo, y.hi, r.lo + r.rows};
+          FS2_TRY(resstack(&a, s, &w, r.lo, org));
+        }
+        r = dst;
+      }
+      last = r_src;
+      continue;
+    }
     for (int j = 0; j < m->n_kernels; j++) {
       const int rb = i * m->n_kernels + j, k = m->rb_k[j];
       Rows R[FS2_MAX_DIL];                             // output rows of pair d
@@ -692,10 +816,10 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
         if (stage_pairs(m, i, C, k)) {
           const int id = add(FS2_VW_RB_PAIR, i, j, d, s1, R[d], x, r_src, r_src, f1c + f2c);
           if (ex) {
-            fs2_resstack_args p = resblock_pair(group, j, d);
+            fs2_resstack_args p = resblock_run(group, j, d, d + 1);
             p.x = r.p; p.y = dst.p; p.alpha = alpha; p.accumulate = accumulate;
             const RowWindow w{R[d].lo, R[d].hi, r.lo + r.rows};
-            FS2_TRY(resstack(&p, s, &w, r.lo, org));
+            FS2_TRY(resstack(&p, s, &w, r.lo, org, C == 128));
           }
           r_src = id;
         } else {
@@ -1002,6 +1126,17 @@ int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_st
   if (a->workspace_bytes < fs2_vocoder_streams_workspace_bytes(m, a->B, a->frames)) return FS2_ERR_ARG;
   Arena ar(a->workspace, a->workspace_bytes);
   return vocoder_streams_impl(m, a, S(st), ar);
+}
+
+static_assert(sizeof(fs2_resblock_run_t) == 32, "fs2_resblock_run_t: six int32 and a double");
+
+int fs2_vocoder_resblock_runs(const fs2_vocoder_model* m, int stage, fs2_resblock_run_t* out, int max_runs) {
+  if (!vocoder_ok(m) || stage < 0 || stage >= m->n_stages || max_runs < 0) return FS2_ERR_ARG;
+  if (!stage_fused(m, stage)) return 0;
+  RbRun runs[RB_MAX_RUNS];
+  const int n = stage_runs(m, stage, runs);
+  for (int q = 0; out && q < n && q < max_runs; q++) out[q] = runs[q];
+  return n;
 }
 
 int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, fs2_vocoder_window_launch_t* out, int max_launches) {

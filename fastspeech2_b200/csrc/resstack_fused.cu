@@ -388,6 +388,22 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_streams_kernel(
   resstack_body<CG, 16, 8, true, true, true>(tmx, tmy, p);
 }
 
+// The 128-channel stage's pairs (fs2_vocoder_model::pair_mask bit 8 + i): the same body at MT = 1 (MT * C = 128), with entry points
+// of their own.  fs2_resstack's public contract stays at 8 to 64 channels; the vocoder reaches these through resstack(.., wide = true).
+template <bool RAG>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_kernel(const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmy,
+                                                                      const RsP p) {
+  resstack_body<128, 128, 1, RAG>(tmx, tmy, p);
+}
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_window_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                             const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<128, 128, 1, true, true>(tmx, tmy, p);
+}
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_streams_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                              const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<128, 128, 1, true, true, true>(tmx, tmy, p);
+}
+
 // ------------------------------------------------------------------ host side
 static size_t rs_smem_bytes(int C, int MT, int SB, int TPS) {
   const size_t slab = (size_t)(C / 16) * 4 * (MT * 128) * 16;
@@ -395,9 +411,10 @@ static size_t rs_smem_bytes(int C, int MT, int SB, int TPS) {
 }
 
 // Launch plan (pure host logic, fs2_resstack_plan_t in fs2b200.h)
-int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out) {
+// wide: the vocoder's 128-channel pairs may use C = 128 (fs2_resstack_plan / fs2_resstack serve 8 to 64 channels)
+int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out, bool wide) {
   if (!a || a->B <= 0 || a->N <= 0 || num_sms <= 0) return FS2_ERR_ARG;
-  if (a->C != 8 && a->C != 16 && a->C != 32 && a->C != 64) return FS2_ERR_UNSUPPORTED;
+  if (a->C != 8 && a->C != 16 && a->C != 32 && a->C != 64 && !(wide && a->C == 128)) return FS2_ERR_UNSUPPORTED;
   const int Cm = a->C < 16 ? 16 : a->C;         // channels computed on chip (8 is zero-padded to 16)
   if (a->n_kernels <= 0 || a->n_kernels > RS_MAXK || a->n_dil <= 0 || a->n_dil > FS2_MAX_DIL) return FS2_ERR_ARG;
   int H = 0;
@@ -467,7 +484,7 @@ static int make_map(CUtensorMap* tm, const float* base, int B, int N, int C, int
 // win: NULL, or the windowed mode: a->x and a->y are then the window buffers [B][x1 - x0][C] and [B][yend - y0][C] (not biased), x0 /
 // x1 the logical rows a->x holds (win->xend is x1), and a->N the full logical length.  org (with win and a->lens): NULL, or the
 // per-utterance origins of the origin mode (origin_rows; rows are then window rows and a->N is not used).
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, int x0, const int* org) {
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, int x0, const int* org, bool wide) {
   if (!a || !a->x || !a->y) return FS2_ERR_ARG;
   if (!aligned16(a->x) || !aligned16(a->y)) return FS2_ERR_ARG;
   if (a->B <= 0 || a->N <= 0 || a->C <= 0) return FS2_ERR_ARG;
@@ -486,7 +503,7 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
   fs2_resstack_args rows = *a;                  // the plan's items: tiles of the y rows
   rows.N = yrows;
   fs2_resstack_plan_t plan;
-  FS2_TRY(resstack_plan(&rows, dv->num_sms.load(std::memory_order_relaxed), plan));
+  FS2_TRY(resstack_plan(&rows, dv->num_sms.load(std::memory_order_relaxed), plan, wide));
   FS2_TRY(dev_once(dv->fused_ready, [] {
     const int mx = 227 * 1024;
     cudaError_t e = cudaFuncSetAttribute(resstack_kernel<32, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
@@ -505,6 +522,10 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_streams_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_streams_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_streams_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     return e;
   }));
   RsP p{};
@@ -531,11 +552,13 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
   if (org) {
     if (a->C == 32) resstack_streams_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 64) resstack_streams_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 128) resstack_wide_streams_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 16) resstack_narrow_streams_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_narrow_streams_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   } else if (win) {
     if (a->C == 32) resstack_window_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 64) resstack_window_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 128) resstack_wide_window_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 16) resstack_narrow_window_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_narrow_window_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   } else if (a->C == 32) {
@@ -544,6 +567,9 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
   } else if (a->C == 64) {
     if (a->lens) resstack_kernel<64, 2, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_kernel<64, 2, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+  } else if (a->C == 128) {
+    if (a->lens) resstack_wide_kernel<true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_wide_kernel<false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   } else if (a->C == 16) {
     if (a->lens) resstack_narrow_kernel<16, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_narrow_kernel<16, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);

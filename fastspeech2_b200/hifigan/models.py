@@ -47,8 +47,10 @@ class Generator(nn.Module):
         # its input is the raw log-mel (|x| up to 11.5), where the E4M3 correction of the shipped universal checkpoint misses the 1e-4
         # waveform bar (tests/test_gpu_model.py::test_hifigan_real_checkpoint_vs_reference; CPU emulation: scripts/emul_split_precision.py).
         self.f8_mask = 0b11110
-        # Stages (bit i) whose ResBlock group runs as ONE persistent kernel with every intermediate on chip (fs2_resstack, available for
-        # the 64-, 32-, 16- and 8-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).  Default: every
+        # Stages (bit i) whose ResBlock group runs on the persistent fs2_resstack kernel with the intermediates of each launch on chip
+        # (available for the 64-, 32-, 16- and 8-channel stages; those stages use the f16 + f8 operand format regardless of f8_mask).
+        # The library cuts such a stage into the whole group or runs of each ResBlock's dilations, whichever its cost model of halo
+        # recompute rates fastest (fs2_vocoder_resblock_runs); every cut gives the same bits.  Default: every
         # stage it serves, 0b1100 for V1 (on an H100 SXM at 400 W, bench.py configs[2]: 127 ms per step against 133 ms with the
         # 64-channel stage on per-layer launches and fused k = 3 pairs) and 0b1111 for V2.
         self.fused_mask = self._fusable_stages()
@@ -58,6 +60,10 @@ class Generator(nn.Module):
         # fused_mask = 0 V2 still pairs that stage; clear pair_mask too for all-per-layer ResBlocks.
         self.pair_mask = 0b0100
         self.pair_kmax = 3
+        # The 128-channel stage (V1's second) too runs its pairs with kernel size <= pair_kmax as fs2_resstack launches (pair_mask bit
+        # 8 + i of the C ABI; its f16 + f8 tiles are then packed at 128 output channels per block).  Bit-identical to the per-layer
+        # convs, three launches instead of six; off by default (DESIGN.md section 5: 69.4 -> 68.1 ms for V1 at B = 16 x 1012).
+        self.wide_pairs = False
         populate(self, hifigan_spec(self._hd, weight_norm=True))
         with torch.no_grad():  # g = ||v|| so that the initial folded weight equals v, as torch's weight_norm does
             for base in self._bases():
@@ -111,10 +117,13 @@ class Generator(nn.Module):
     # ------------------------------------------------------------------ packing
     def _fusable_stages(self):
         """Bit i set when stage i's width (upsample_initial_channel / 2^(i+1)) is one fs2_resstack serves."""
+        return self._stages_of_width(*FUSED_WIDTHS)
+
+    def _stages_of_width(self, *widths):
         mask, ch = 0, self._hd["upsample_initial_channel"]
         for i in range(self.num_upsamples):
             ch //= 2
-            if ch in FUSED_WIDTHS:
+            if ch in widths:
                 mask |= 1 << i
         return mask
 
@@ -126,7 +135,8 @@ class Generator(nn.Module):
             return 0, 0, 0, 0
         fused = int(self.fused_mask) & self._fusable_stages()
         pair = int(self.pair_mask) & ~fused
-        return int(self.f8_mask) | (fused << 1) | (pair << 1), fused, pair, int(self.pair_kmax)
+        wide = self._stages_of_width(128) if self.wide_pairs else 0
+        return int(self.f8_mask) | (fused << 1) | (pair << 1) | (wide << 1), fused, pair | (wide << 8), int(self.pair_kmax)
 
     def _pack(self):
         L.lib()
@@ -151,8 +161,11 @@ class Generator(nn.Module):
                 raise L.Fs2Error("ConvTranspose1d stage needs kernel = 2*stride and even stride on the sm_90a path")
             m.rates[i], m.up_k[i] = u, k
         m.f8_mask, m.fused_mask, m.pair_mask, m.pair_kmax = self.effective_masks()
-        pk =packing.pack_vocoder(lambda b: self._folded(b).float(), lambda b: get(self, b + ".bias").detach().float(),
-                                  hd["upsample_rates"], m.n_stages * m.n_kernels, m.n_dil, f8_mask=m.f8_mask)
+        wide_keys = [f"rb.{i * m.n_kernels + j}.{d}.{w}" for i in range(m.n_stages) if (m.pair_mask >> (8 + i)) & 1
+                     for j in range(m.n_kernels) if m.rb_k[j] <= m.pair_kmax for d in range(m.n_dil) for w in ("w1", "w2")]
+        pk = packing.pack_vocoder(lambda b: self._folded(b).float(), lambda b: get(self, b + ".bias").detach().float(),
+                                  hd["upsample_rates"], m.n_stages * m.n_kernels, m.n_dil, f8_mask=m.f8_mask,
+                                  wide_keys=wide_keys if self.use_tensor_cores else ())
         P = lambda k: pk[k].data_ptr()
         m.w_pre, m.b_pre, m.w_post, m.b_post = P("w_pre"), P("b_pre"), P("w_post"), P("b_post")
         T = lambda k: pk[k + "_tc"].data_ptr() if (self.use_tensor_cores and k + "_tc" in pk) else 0

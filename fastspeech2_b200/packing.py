@@ -246,9 +246,11 @@ def split_conv_transpose(w: Tensor, u: int):
 
 
 def pack_vocoder(w_of: Callable[[str], Tensor], b_of: Callable[[str], Tensor], rates, n_resblocks: int, n_dil: int,
-                 f8_mask: int = 0) -> Dict[str, Tensor]:
+                 f8_mask: int = 0, wide_keys=()) -> Dict[str, Tensor]:
     """`w_of(base)` returns the folded weight of conv `base`, `b_of(base)` its bias.  f8_mask: bit 0 = conv_pre, bit 1+i = every conv of
-    upsample stage i uses the f16 + f8 operand format (fs2_vocoder_model.f8_mask)."""
+    upsample stage i uses the f16 + f8 operand format (fs2_vocoder_model.f8_mask).  wide_keys: ResBlock conv keys ('rb.<rb>.<d>.w1'
+    / '.w2') of a 128-channel stage that fs2_resstack runs (fs2_vocoder_model.pair_mask bit 8 + i): their f16 + f8 tiles are packed
+    at 128 output channels per block, the image that kernel reads, instead of the per-layer conv's 64."""
     pk: Dict[str, Tensor] = {"w_pre": conv_w(w_of("conv_pre")), "b_pre": b_of("conv_pre").contiguous()}
     for i, u in enumerate(rates):
         wa, wb = split_conv_transpose(w_of(f"ups.{i}"), u)
@@ -273,6 +275,9 @@ def pack_vocoder(w_of: Callable[[str], Tensor], b_of: Callable[[str], Tensor], r
         return idx if k.startswith("up.") else idx // nk
     f8_keys = [k for k in keys if f8_mask & (1 << (stage_of(k) + 1))]
     add_tc_tiles(pk, keys, f8_keys)
+    for k in wide_keys:
+        assert k in f8_keys and pk[k].shape[1:] == (128, 128), k
+        pk[k + "_tc"] = pack_conv_tc(pk[k], f8=True, nb=128)
     for k in f8_keys:                        # 8-channel ResBlock convs: the zero-padded tiles of fs2_resstack (fs2_vocoder_model)
         if k.startswith("rb.") and k + "_tc" not in pk:
             t = pack_conv_tc_pad16(pk[k])

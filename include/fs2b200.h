@@ -216,7 +216,7 @@ int fs2_conv_post(const fs2_conv_post_args* a, fs2_stream_t stream);
 /* HiFi-GAN multi-receptive-field ResBlock group of one upsample stage as ONE persistent kernel (hifigan/models.py:154-160, ResBlock.forward
  * :96-103):   y = (1/n_kernels) * sum_j R_j(x),   R_j: x <- conv_{k_j,1}( lrelu( conv_{k_j,dil_jd}( lrelu(x) ) + b1 ) ) + b2 + x  for d = 0..n_dil-1,
  * lrelu slope 0.1, "same" zero padding at the utterance ends.  x, y: contiguous [B][N][C], C in {8, 16, 32, 64} (the 64- to 8-channel
- * stages of HiFi-GAN V1 and V2); every intermediate stays in shared memory / registers (halo recompute), weights are the f16+f8 tiles of
+ * stages of HiFi-GAN V1 and V2; the vocoder also runs 128-channel pairs on the same body, see fs2_vocoder_model::pair_mask); every intermediate stays in shared memory / registers (halo recompute), weights are the f16+f8 tiles of
  * the per-layer kernel (FS2_TC_VARIANT_F8 with N = C: pack_conv_tc(w, f8=True)).  C = 8 is computed as 16 channels whose upper 8 are
  * zero: its weights are the f8 tiles of the conv zero-padded to 16 x 16 (packing.pack_conv_tc_pad16), while x and y stay [B][N][8] and
  * no byte of y outside them is written.  (k-1)*dil/2 <= 32 per conv.  Other shapes: FS2_ERR_UNSUPPORTED.
@@ -396,13 +396,35 @@ typedef struct fs2_vocoder_model {
   const float *w_pre_tc, *w_up_a_tc[FS2_MAX_STAGES], *w_up_b_tc[FS2_MAX_STAGES];
   const float *w_rb1_tc[FS2_MAX_RESBLOCKS][FS2_MAX_DIL], *w_rb2_tc[FS2_MAX_RESBLOCKS][FS2_MAX_DIL];
   int f8_mask; /* bit 0: w_pre_tc, bit 1+i: every *_tc tile of stage i is in the f16+f8 format (FS2_TC_VARIANT_F8) */
-  int fused_mask; /* bit i: the ResBlock group of stage i runs as one fs2_resstack launch (needs f8_mask bit 1+i and a width fs2_resstack
+  int fused_mask; /* bit i: the ResBlock group of stage i runs on fs2_resstack, as the launches fs2_vocoder_resblock_runs plans (the
+                     whole group, or runs of each ResBlock's dilations; needs f8_mask bit 1+i and a width fs2_resstack
                      serves: 8, 16, 32 or 64 channels, i.e. the last two stages of V1 and all four of V2).  In an 8-channel stage the
                      w_rb*_tc tiles are the 16 x 16 zero-padded ones fs2_resstack reads; its per-layer convs run on the exact kernel. */
   int pair_mask;  /* bit i: in stage i every (conv_k,d ; conv_k,1 ; +x) pair with k <= pair_kmax runs as one fs2_resstack launch (the
-                     HBM-bound small-kernel layers: the pair's intermediate stays on chip); same requirements as fused_mask */
+                     HBM-bound small-kernel layers: the pair's intermediate stays on chip); same requirements as fused_mask.
+                     bit 8 + i: the same for a 128-channel stage i (V1's second stage), whose pairs' w_rb*_tc tiles must then be the
+                     f16 + f8 tiles packed at 128 output channels per block (packing.pack_conv_tc(w, f8=True, nb=128)), not the
+                     64-column blocks the per-layer conv reads; needs f8_mask bit 1+i. */
   int pair_kmax;
 } fs2_vocoder_model;
+
+/* How a stage in fused_mask cuts its ResBlock group into fs2_resstack launches (fs2_vocoder_resblock_runs).  One launch per work item
+ * recomputes H halo rows on each side of its TILE output rows, so the whole group, whose H is its widest ResBlock's reach, pays for
+ * that reach in every conv of every ResBlock.  The planner picks, per stage, either the whole group or, for each ResBlock j in turn,
+ * consecutive runs of its dilations, each run one launch.  A run that is not the last of its ResBlock writes the fp32 residual stream
+ * (alpha 1, no accumulate) that the next run reads; the last one adds alpha = 1/n_kernels times it into the stage's output as the
+ * group does.  Every cut computes the same bits: each output row's sums run in the same order wherever its tile starts.  The choice
+ * minimises a cost model -- MMA work on the slab rows (MT * 128 per TILE output rows) plus one fp32 write and read of every
+ * intermediate -- that depends on the model only, so the offline, windowed and streams calls launch the same runs. */
+typedef struct fs2_resblock_run_t {
+  int32_t j;              /* kernel-size index; -1: the whole group (every kernel size, d0 = 0, d1 = n_dil) */
+  int32_t d0, d1;         /* dilations [d0, d1) of ResBlock j */
+  int32_t H, TILE, slab;  /* fs2_resstack_plan of the launch: halo rows per side, output rows per work item, slab rows (MT * 128) */
+  double cost;            /* modelled ns per output row of the stage */
+} fs2_resblock_run_t;
+/* The launches of stage `stage`'s ResBlocks in issue order: writes min(count, max_runs) records to out (may be NULL) and returns the
+ * count, 0 for a stage outside fused_mask, or FS2_ERR_ARG / FS2_ERR_UNSUPPORTED.  Pure host logic: no CUDA call, no pointer read. */
+int fs2_vocoder_resblock_runs(const fs2_vocoder_model* m, int stage, fs2_resblock_run_t* out, int max_runs);
 
 typedef struct fs2_vocoder_args {
   int B, T;
@@ -444,7 +466,9 @@ int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_win
 
 /* One launch of a window (fs2_vocoder_window_plan).  Rows are logical rows at the launch's rate, `scale` rows per mel frame, clipped to
  * the utterance's logical extent [0, T * scale); input and output share the rate (the ConvTranspose runs as two phase-group convs
- * whose row q holds the next rate's rows [q * u, q * u + u)). */
+ * whose row q holds the next rate's rows [q * u, q * u + u)).  FS2_VW_RB_GROUP is one run of fs2_vocoder_resblock_runs: j = -1 the
+ * whole group, else ResBlock j's dilations [d, d1), where d1 is the next record's d if that record is a run of the same ResBlock,
+ * else n_dil (the same records in the same order as fs2_vocoder_resblock_runs returns for the stage). */
 enum { FS2_VW_CONV_PRE = 0, FS2_VW_UP_A = 1, FS2_VW_UP_B = 2, FS2_VW_RB_CONV1 = 3, FS2_VW_RB_CONV2 = 4, FS2_VW_RB_PAIR = 5,
        FS2_VW_RB_GROUP = 6, FS2_VW_CONV_POST = 7 };
 typedef struct fs2_vocoder_window_launch_t {

@@ -20,8 +20,9 @@ from fastspeech2_b200.spec import fastspeech2_spec
 def bind(path):
     handle = C.CDLL(path)
     for name, (res, args) in L.EXPORTS.items():
-        fn = getattr(handle, name)
-        fn.restype, fn.argtypes = res, args
+        fn = getattr(handle, name, None)               # an older build may lack entry points this script does not call
+        if fn is not None:
+            fn.restype, fn.argtypes = res, args
     # the two builds may differ in ABI version; the structs this script passes must have the same layout in both
     for i, cls in ((0, L.Conv1dArgs), (9, L.AcousticModel), (10, L.EncodeArgs), (11, L.DecodeArgs), (12, L.VocoderModel), (13, L.VocoderArgs)):
         assert handle.fs2_struct_size(i) == C.sizeof(cls), (path, cls.__name__)

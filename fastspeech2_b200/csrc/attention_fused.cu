@@ -2,8 +2,10 @@
 // SubLayers.py:39-44): S = Q K^T, softmax and O = P V in ONE persistent wgmma kernel -- the score matrix lives in registers and
 // never reaches HBM (the reference writes S [2B][T][T] in fp32 four times).
 //
-//   pack_kv_tiles_kernel, once per layer: K and V of every (utterance, head) -> fp16 hi/lo operand tiles (three-MMA split: attention
-//   keeps fp32-class operands), one bulk-copy stage per 16 rows of the MMA's K dimension.
+//   pack_kv_tiles_kernel, once per layer: K and V of every (utterance, head) x AF_WSCALE -> fp16 hi/lo operand tiles, one bulk-copy
+//   stage per 16 rows of the MMA's K dimension.  Every MMA is the three-MMA split (DESIGN §3): 22 significant bits per operand while its
+//   lo part is a normal fp16 number, and an absolute floor below that -- 2^-25 for Q (split unscaled), 2^-29 for K and V (x 16), about
+//   2^-40 for P (x AF_PSCALE).  The converts saturate: the domain is |q| < 65504 and |k|, |v| < 4094, with no error beyond it.
 //   work item = (head h, utterance b, 128 query rows).
 //   pass 1: for every block of 128 keys  S = Q K_j^T (register accumulators)  ->  row maximum (a row's columns are spread over the
 //           four lanes of a quad: two shuffles).
@@ -29,6 +31,7 @@ constexpr int AF_THREADS = 288;
 constexpr int AF_SB = 8;                         // K / V stage ring depth
 constexpr uint32_t AF_STAGE = 8192;              // one stage: [hi | lo][2 chunks][128][16 B]
 constexpr float AF_WSCALE = 16.f;                // power-of-two operand scale of the packed K / V tiles (|k|, |v| < 4094 stay inside fp16)
+constexpr float AF_PSCALE = 32768.f;             // scale of p in (0, 1] before its split: lo stays normal down to p ~ 2^-18 (max 32768)
 constexpr int AF_MIN_ROWS = 128;                 // shortest utterance the ragged kernel takes (a B = 1 call takes T >= 128)
 
 // ------------------------------------------------------------------ K / V operand tiles
@@ -262,7 +265,8 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
       m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 1));
       m[h] = fmaxf(m[h], __shfl_xor_sync(0xffffffffu, m[h], 2));
     }
-    // ---- pass 2: p = exp2(s*c - m) -> P operand planes -> O += P V_j
+    // ---- pass 2: p = exp2(s*c - m) x AF_PSCALE -> P operand planes -> O += P V_j.  The scale is applied after exp2f, so that p itself
+    // rounds as it would unscaled; l carries it too, so O / l needs no correction.
     float oacc[64];
     float l[2] = {0.f, 0.f};
     const int prow = 64 * g + 16 * w + (lane >> 2);
@@ -277,7 +281,7 @@ __global__ void __launch_bounds__(AF_THREADS, 1) attention_fused_kernel(const Af
           float e[2];
 #pragma unroll
           for (int q = 0; q < 2; q++) {
-            e[q] = j * 128 + k0 + q < len ? exp2f(fmaf(sacc[4 * jj + 2 * h + q], c, -m[h])) : 0.f;
+            e[q] = j * 128 + k0 + q < len ? exp2f(fmaf(sacc[4 * jj + 2 * h + q], c, -m[h])) * AF_PSCALE : 0.f;
             l[h] += e[q];
           }
           uint32_t lw;

@@ -18,7 +18,7 @@ constexpr size_t ATT_SMEM = (size_t)(ATT_BQ * ATT_LD + ATT_BK * ATT_LD + ATT_BK 
 // (they are not computed upstream and may hold anything), query tiles wholly at or beyond len and the rows there are not written, and
 // an utterance with len >= fused_from (> 0) is left to the fused kernel.  A template parameter, so the padded kernel keeps its code.
 template <bool RAG>
-__global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attention_args a, int fused_from) {
+__global__ void __launch_bounds__(256, 1) attention_simt_kernel(const fs2_attention_args a, int fused_from) {
   extern __shared__ __align__(16) float smem[];
   float* Qs = smem;                       // [64][132]
   float* Ks = Qs + ATT_BQ * ATT_LD;       // [64][132]  (reused as P [64][68])
@@ -52,13 +52,16 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
     *reinterpret_cast<float4*>(Qs + r * ATT_LD + c * 4) = v;
   }
 
-  float m_run[4], l_run[4], o[4][8];
+  // O and l are compensated (Kahan) sums: oc / lc hold what their last adds rounded away.  A plain fp32 chain rounds the same way on
+  // every add when many keys share one weight and one value, and that error grows with the number of keys (tests/att_cases.py, plateau).
+  float m_run[4], l_run[4], lc[4], o[4][8], oc[4][8];
 #pragma unroll
   for (int i = 0; i < 4; i++) {
     m_run[i] = -INFINITY;
     l_run[i] = 0.f;
+    lc[i] = 0.f;
 #pragma unroll
-    for (int j = 0; j < 8; j++) o[i][j] = 0.f;
+    for (int j = 0; j < 8; j++) o[i][j] = oc[i][j] = 0.f;
   }
 
   const int n_tiles = (len + ATT_BK - 1) / ATT_BK;
@@ -127,7 +130,9 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
 #pragma unroll
       for (int o2 = 8; o2 > 0; o2 >>= 1) psum += __shfl_xor_sync(0xffffffffu, psum, o2);
       scale_o[i] = expf(m_run[i] - m_new);      // exp(-inf) = 0 on the first tile
-      l_run[i] = l_run[i] * scale_o[i] + psum;
+      const float l0 = l_run[i] * scale_o[i], y = psum - lc[i] * scale_o[i];
+      l_run[i] = l0 + y;
+      lc[i] = (l_run[i] - l0) - y;
       m_run[i] = m_new;
     }
     __syncthreads();
@@ -136,7 +141,10 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
 #pragma unroll
     for (int i = 0; i < 4; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) o[i][j] *= scale_o[i];
+      for (int j = 0; j < 8; j++) {
+        o[i][j] *= scale_o[i];
+        oc[i][j] *= scale_o[i];
+      }
 #pragma unroll 2
     for (int kk = 0; kk < ATT_BK; kk += 4) {
       float4 pr[4];
@@ -146,13 +154,16 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
       for (int u = 0; u < 4; u++) {
         const float4 v0 = *reinterpret_cast<const float4*>(Vs + (kk + u) * ATT_D + tx * 4);
         const float4 v1 = *reinterpret_cast<const float4*>(Vs + (kk + u) * ATT_D + 64 + tx * 4);
+        const float vv[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
 #pragma unroll
         for (int i = 0; i < 4; i++) {
           const float pv = u == 0 ? pr[i].x : (u == 1 ? pr[i].y : (u == 2 ? pr[i].z : pr[i].w));
-          o[i][0] = fmaf(pv, v0.x, o[i][0]); o[i][1] = fmaf(pv, v0.y, o[i][1]);
-          o[i][2] = fmaf(pv, v0.z, o[i][2]); o[i][3] = fmaf(pv, v0.w, o[i][3]);
-          o[i][4] = fmaf(pv, v1.x, o[i][4]); o[i][5] = fmaf(pv, v1.y, o[i][5]);
-          o[i][6] = fmaf(pv, v1.z, o[i][6]); o[i][7] = fmaf(pv, v1.w, o[i][7]);
+#pragma unroll
+          for (int j = 0; j < 8; j++) {
+            const float y = fmaf(pv, vv[j], -oc[i][j]), t = o[i][j] + y;
+            oc[i][j] = (t - o[i][j]) - y;
+            o[i][j] = t;
+          }
         }
       }
     }
@@ -168,9 +179,12 @@ __global__ void __launch_bounds__(256, 2) attention_simt_kernel(const fs2_attent
       *reinterpret_cast<float4*>(orow + 64 + tx * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
       continue;
     }
-    const float inv = 1.f / l_run[i];
-    *reinterpret_cast<float4*>(orow + tx * 4) = make_float4(o[i][0] * inv, o[i][1] * inv, o[i][2] * inv, o[i][3] * inv);
-    *reinterpret_cast<float4*>(orow + 64 + tx * 4) = make_float4(o[i][4] * inv, o[i][5] * inv, o[i][6] * inv, o[i][7] * inv);
+    const float inv = 1.f / (l_run[i] - lc[i]);
+    float r[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) r[j] = (o[i][j] - oc[i][j]) * inv;
+    *reinterpret_cast<float4*>(orow + tx * 4) = make_float4(r[0], r[1], r[2], r[3]);
+    *reinterpret_cast<float4*>(orow + 64 + tx * 4) = make_float4(r[4], r[5], r[6], r[7]);
   }
 }
 

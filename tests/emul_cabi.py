@@ -353,6 +353,106 @@ def attention(qkv, H, key_lens):
     return ctx.masked_fill((torch.arange(T)[None, :] >= key_lens[:, None])[..., None], 0.0)
 
 
+# ------------------------------------------------------------------ the fused attention kernel's operand formats and their bound
+#
+# attention_fused.cu multiplies fp16 hi / lo operands three MMAs at a time, as the convolutions do (Dh = 128, scale = 128^-1/2):
+#   S = Q_lo K_hi + Q_hi K_hi + Q_hi K_lo        Q split as it is, K split x AF_WSCALE = 16 (the packed tiles)
+#   p = exp2(S c - m) in fp32, l = the sum of the fp32 p, P = p x AF_PSCALE split into fp16 hi / lo
+#   O = (P_lo V_hi + P_hi V_hi + P_hi V_lo) / (16 AF_PSCALE l)        V split x 16
+# All converts saturate at +-65504, so the domain is |q| < 65504 and |k|, |v| < 4094; beyond it the operands clip without an error.
+#
+# R (attention_contract), per output element, bounds |O(rounded Q, K, V) - O64| from the stated precision of the three splits
+# (_split3_err: 2^-22 relative, the absolute floor 2^-25 of a subnormal lo; for K and V that floor is 2^-29 after the / 16):
+#   score:  q.k - S = q_lo k_lo + q ek + eq k - eq ek with |eq| <= e_q, |ek| <= e_k, so one key's scaled score is off by at most
+#           d_s = scale sum_d (|q_lo| |k_lo| + |q| e_k + e_q |k| + e_q e_k).
+#   softmax: scores off by eps_s (|eps_s| <= d_s) move O by sum_s w_s (e^eps_s - 1)(v_s - O) / sum_s w_s e^eps_s, w the exact weights:
+#           at most e^dmax sum_s w_s expm1(d_s) |v_s - O|.
+#   values: the perturbed weights (each <= w_s e^(2 dmax)) times the V error: at most e^(2 dmax) sum_s w_s e_v,s.
+# P is not in R.  It lies in (0, 1], and AF_PSCALE = 2^15 keeps its lo plane normal down to p ~ 2^-18, so P costs 2^-22 relative
+# (the dropped P_lo V_lo term as much again), which the bar of the tests absorbs.  Without the scale its lo plane is subnormal below
+# p ~ 2^-3 and each weight carries up to 2^-25 absolute: on a row whose keys share one score and one value those errors add up n
+# times while l, summed from the unrounded p, does not see them.  Charging that floor to R would make the bar vacuous at decoder
+# lengths; the kernel must not have it (tests/test_attention_precision_cpu.py).
+
+ATT_PSCALE = 2.0 ** 15       # AF_PSCALE of attention_fused.cu
+ATT_WSCALE = 16.0            # AF_WSCALE
+
+
+def _heads(qkv, H, b, n):
+    """q, k, v of utterance b's first n rows, [H][n][dh] each, as qkv's dtype."""
+    D = qkv.shape[2] // 3
+    return [qkv[b, :n, i * D:(i + 1) * D].reshape(n, H, D // H).transpose(0, 1) for i in range(3)]
+
+
+def _key_rows(key_lens, T, b):
+    return min(max(int(key_lens[b]), 0), T)
+
+
+def attention_contract(qkv, H, key_lens):
+    """The fused kernel's contract in fp64: (o64, R), both [B, T, D], o64 the exact attention (E.attention), R the bound above; both
+    zero on padded query rows."""
+    B, T, D3 = qkv.shape
+    D = D3 // 3
+    dh = D // H
+    scale = 1.0 / math.sqrt(dh)
+    o64 = torch.zeros(B, T, D, dtype=torch.float64)
+    R = torch.zeros_like(o64)
+    for b in range(B):
+        n = _key_rows(key_lens, T, b)
+        if n == 0:
+            continue
+        q, k, v = (t.float() for t in _heads(qkv, H, b, n))
+        q64, k64, v64 = q.double(), k.double(), v.double()
+        w = torch.softmax(q64 @ k64.transpose(-1, -2) * scale, -1)
+        o = w @ v64
+        ks, vs = k * ATT_WSCALE, v * ATT_WSCALE
+        lo = lambda t: _f16(t - _f16(t)).double().abs()
+        lq, lk = lo(q), lo(ks) / ATT_WSCALE
+        eq, ek, ev = _split3_err(q), _split3_err(ks) / ATT_WSCALE, _split3_err(vs) / ATT_WSCALE
+        d = scale * (torch.cat([lq, q64.abs(), eq, eq], -1) @ torch.cat([lk, ek, k64.abs(), ek], -1).transpose(-1, -2))
+        dmax = d.amax(-1, keepdim=True)
+        we = w * torch.expm1(d)
+        soft = torch.empty_like(o)                     # sum_s we_s |v_s - O|, in row chunks of at most 2^24 (row, key, d) terms
+        step = max(1, 2 ** 24 // (n * dh))
+        for h in range(H):
+            for t0 in range(0, n, step):
+                diff = (v64[h][None] - o[h, t0:t0 + step, None]).abs()
+                soft[h, t0:t0 + step] = (we[h, t0:t0 + step, None] @ diff)[:, 0]
+        r = torch.exp(dmax) * soft + torch.exp(2 * dmax) * (w @ ev)
+        o64[b, :n] = o.transpose(0, 1).reshape(n, D)
+        R[b, :n] = r.transpose(0, 1).reshape(n, D)
+    return o64, R
+
+
+def attention_fused_emul(qkv, H, key_lens, p_scale=ATT_PSCALE):
+    """The fused kernel's arithmetic with exact sums: fp16 splits as split_f16x2 rounds them, S rounded to fp32, p = exp2(S c - m)
+    in fp32 as the kernel forms it, l the fp64 sum of those p, P split x p_scale, O summed in fp64.  p_scale = 1 is the kernel
+    without AF_PSCALE.  Returns [B, T, D] fp64, zero on padded query rows."""
+    B, T, D3 = qkv.shape
+    D = D3 // 3
+    dh = D // H
+    f32 = lambda t: t.float().double()
+    c = f32(torch.tensor(dh ** -0.5, dtype=torch.float32) * (1.0 / ATT_WSCALE) * 1.4426950408889634)
+    out = torch.zeros(B, T, D, dtype=torch.float64)
+    for b in range(B):
+        n = _key_rows(key_lens, T, b)
+        if n == 0:
+            continue
+        q, k, v = (t.float() for t in _heads(qkv, H, b, n))
+        split = lambda t: (_f16(t), _f16(t - _f16(t)))
+        (qh, ql), (kh, kl), (vh, vl) = split(q), split(k * ATT_WSCALE), split(v * ATT_WSCALE)
+        mm = lambda a, bt: a.double() @ bt.double()
+        s = f32(mm(ql, kh.transpose(-1, -2)) + mm(qh, kh.transpose(-1, -2)) + mm(qh, kl.transpose(-1, -2)))
+        sc = f32(s * c)
+        m = sc.amax(-1, keepdim=True)
+        p = f32(torch.exp2(f32(s * c - m)))
+        l = p.sum(-1, keepdim=True)
+        ph, pl = split((p * p_scale).float())
+        o = (mm(pl, vh) + mm(ph, vh) + mm(ph, vl)) / (ATT_WSCALE * p_scale * l)
+        out[b, :n] = o.transpose(0, 1).reshape(n, D)
+    return out
+
+
 def fft_block(pk, pfx, x, lens, H, k1, k2):
     qkv = conv1d(x, pk[pfx + "w_qkv"][None], pk[pfx + "b_qkv"])
     ctx = attention(qkv, H, lens)

@@ -5,6 +5,7 @@ import torch
 
 from fastspeech2_b200 import ops, packing
 from tests import emul_cabi as E
+from tests.att_cases import ATT_EXACT_C, EDGE_LENS, attention_bar_scale, attention_normalised_err, attention_qkv
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -673,65 +674,6 @@ def test_add_positions():
     assert torch.equal(got.cpu(), x + pos[:517])
 
 
-def attention_qkv(kind, lens, T, seed=3):
-    """qkv [B, T, 768] (2 heads of 128).  "random": N(0, 1).  The others are adversarial for a softmax kernel: every query is
-    8 u + small noise for one unit vector u, so a key c u scores about 8 c / sqrt(128) nats against all of them, per utterance of n keys:
-      last_tile_max: key n - 1 scores 42 nats, every earlier one |s| < ~3: breaks a missing online-softmax rescale.
-      masked_max:    the keys at and past n score 140 nats: breaks a max taken before masking.
-      range80:       keys spread over [-80, 50] nats and key n // 2 at +80: the far keys' weights underflow to 0, O = that key's v.
-      tied:          keys 0 and n - 1 (different 64-key tiles) share the row max bit for bit: O = the mean of their v."""
-    B = len(lens)
-    if kind == "random":
-        return rnd(B, T, 768, seed=seed)
-    gen = g(seed)
-    dh = 128
-    u = torch.ones(dh) / dh ** 0.5
-    q = 8 * u + 0.01 * torch.randn(B, T, 2, dh, generator=gen)
-    k = torch.randn(B, T, 2, dh, generator=gen)
-    v = torch.randn(B, T, 2, dh, generator=gen)
-    nats = lambda s: s * dh ** 0.5 / 8 * u
-    for b, n in enumerate(lens):
-        n = min(max(n, 0), T)
-        if n == 0:
-            continue
-        if kind == "last_tile_max":
-            k[b, n - 1] = nats(42.0)
-        elif kind == "masked_max":
-            k[b, n:] = nats(140.0)
-        elif kind == "range80":
-            s = torch.rand(T, 2, 1, generator=gen, dtype=torch.float64).float() * 130 - 80
-            k[b] = s * nats(1.0)
-            k[b, n // 2] = nats(80.0)
-        elif kind == "tied":
-            k[b] = 0.1 * k[b]
-            k[b, 0] = nats(30.0)
-            k[b, n - 1] = nats(30.0)
-    return torch.cat([q.reshape(B, T, 256), k.reshape(B, T, 256), v.reshape(B, T, 256)], dim=2)
-
-
-def attention_bar_scale(qkv, key_lens):
-    """Per (utterance, query row, head): max_s |v_s| (1 + scale max_s sum_d |q_d| |k_sd|) over the valid keys s, in fp64."""
-    B, T, _ = qkv.shape
-    q, k, v = (qkv[..., i * 256:(i + 1) * 256].double().abs().reshape(B, T, 2, 128).permute(0, 2, 1, 3) for i in range(3))
-    valid = (torch.arange(T)[None, :] < key_lens.clamp(0, T)[:, None])[:, None, :, None]     # [B, 1, Tk, 1]
-    vmax = (v * valid).amax(dim=(2, 3))                                                    # [B, H]
-    qk = (q @ k.transpose(-1, -2)).masked_fill(~valid.transpose(-1, -2), 0.0).amax(dim=-1)   # [B, H, T]
-    return (vmax[..., None] * (1 + qk / 128 ** 0.5)).permute(0, 2, 1)                    # [B, T, H]
-
-
-def attention_normalised_err(got, want, scale):
-    """max over rows of max_d |got - want| / (2^-24 scale_row); rows of zero scale (no valid key) must be exact."""
-    B, T, _ = got.shape
-    d = (got.double() - want).abs().reshape(B, T, 2, 128).amax(-1)
-    r = torch.where(scale > 0, d / (U24 * scale.clamp_min(1e-300)), torch.where(d > 0, float("inf"), 0.0))
-    return torch.nan_to_num(r, nan=float("inf")).max().item()
-
-
-# per-row error bar of both attention backends in units of 2^-24 max|v| (1 + scale max sum|q||k|) (attention_bar_scale).  Largest
-# values measured over ATT_ADV_CASES and ATT_DECODER_CASES on an H100 80GB HBM3 (700 W power limit): 0.41 for the exact kernel, 3.9
-# for the fused one (its P and V pass through fp16 hi / lo operand planes: the range80 rows, O against the argmax key's v).
-ATT_EXACT_C = {0: 2.0, 2: 16.0}
-EDGE_LENS = [0, 1, 63, 64, 65, 127, 128, 129, 300, 10 ** 6, -3]            # T = 300: plus one past T and one negative (both clamped)
 ATT_ADV_CASES = [
     ("random", 256, [256, 200, 129, 128, 127, 77, 65, 64, 63, 40, 17, 9, 3, 1, 256, 250] * 4),     # encoder shape B = 64 (configs[3]-like)
     ("random", 300, EDGE_LENS),

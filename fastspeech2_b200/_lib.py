@@ -195,6 +195,37 @@ VOCODER_STREAMS_ARGS_SIZE = 64
 assert C.sizeof(VocoderStreamsArgs) == VOCODER_STREAMS_ARGS_SIZE
 
 
+class ResampleArgs(C.Structure):
+    """fs2_resample_args: offline sample-rate conversion of [B][N] rows (88 bytes, pinned by a static_assert in resample.cu)."""
+    _fields_ = [("B", i32), ("up", i32), ("down", i32), ("K", i32), ("taps", fp), ("x", fp), ("x_batch_stride", i64), ("N", i64),
+                ("lens", fp), ("lens_scale", i32), ("y", fp), ("y_batch_stride", i64), ("pcm16", i32), ("scale", f32)]
+
+
+class ResampleWindowArgs(C.Structure):
+    """fs2_resample_window_args: outputs [j0, j1) from input pieces [i0, i1) + [i1, i2) (144 bytes, pinned in resample.cu)."""
+    _fields_ = [("B", i32), ("up", i32), ("down", i32), ("K", i32), ("taps", fp),
+                ("x0", fp), ("x0_batch_stride", i64), ("x1", fp), ("x1_batch_stride", i64),
+                ("i0", i64), ("i1", i64), ("i2", i64), ("N", i64), ("lens", fp), ("lens_scale", i32),
+                ("j0", i64), ("j1", i64), ("y", fp), ("y_batch_stride", i64), ("pcm16", i32), ("scale", f32)]
+
+
+class ResampleStream(C.Structure):
+    """fs2_resample_stream_t: one stream's record of fs2_resample_streams, in device memory (64 bytes, pinned in resample.cu)."""
+    _fields_ = [("x0", fp), ("x1", fp)] + [(n, i64) for n in ("i0", "i1", "i2", "n", "j0", "j1")]
+
+
+class ResampleStreamsArgs(C.Structure):
+    """fs2_resample_streams_args: B streams at their own positions in one launch (64 bytes, pinned in resample.cu)."""
+    _fields_ = [("B", i32), ("up", i32), ("down", i32), ("K", i32), ("taps", fp), ("table", fp), ("max_out", i64),
+                ("y", fp), ("y_batch_stride", i64), ("pcm16", i32), ("scale", f32)]
+
+
+RESAMPLE_MAX_FACTOR = 2048
+RESAMPLE_ARGS_SIZE, RESAMPLE_WINDOW_ARGS_SIZE, RESAMPLE_STREAM_SIZE, RESAMPLE_STREAMS_ARGS_SIZE = 88, 144, 64, 64
+assert C.sizeof(ResampleArgs) == RESAMPLE_ARGS_SIZE and C.sizeof(ResampleWindowArgs) == RESAMPLE_WINDOW_ARGS_SIZE
+assert C.sizeof(ResampleStream) == RESAMPLE_STREAM_SIZE and C.sizeof(ResampleStreamsArgs) == RESAMPLE_STREAMS_ARGS_SIZE
+
+
 class ConvTcPlan(C.Structure):
     _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")]
 
@@ -257,6 +288,9 @@ EXPORTS = {
     "fs2_vocoder_resblock_runs": (i32, [C.POINTER(VocoderModel), i32, C.POINTER(ResblockRun), i32]),
     "fs2_vocoder_streams_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward_streams": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsArgs), fp]),
+    "fs2_resample": (i32, [C.POINTER(ResampleArgs), fp]),
+    "fs2_resample_window": (i32, [C.POINTER(ResampleWindowArgs), fp]),
+    "fs2_resample_streams": (i32, [C.POINTER(ResampleStreamsArgs), fp]),
 }
 
 _lib = None

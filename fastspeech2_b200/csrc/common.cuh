@@ -35,7 +35,7 @@ inline int cuda_status() {
 constexpr int FS2_MAX_DEVICES = 64;
 struct DevState {
   std::atomic<int> num_sms{0};
-  std::atomic<bool> conv_tc_ready{false}, att_simt_ready{false}, fused_ready{false}, att_fused_ready{false};
+  std::atomic<bool> conv_tc_ready{false}, att_simt_ready{false}, fused_ready{false}, att_fused_ready{false}, resample_ready{false};
 };
 DevState* dev_state(int* err);                       // NULL + *err on failure
 // Runs setup() under one process-wide lock unless `ready` is already set, and sets it when setup() succeeds.  Returns FS2_OK, or
@@ -89,6 +89,12 @@ struct ControlView {
   const float* v; int64_t sb, sl;
   const int32_t* rag;
 };
+
+// fp32 sample -> int16 PCM as numpy's (x * scale).astype("int16") on in-range values: truncation toward zero.  Values past the int16
+// range are clamped, not wrapped (fs2_wav_to_int16, fs2_resample*).
+__device__ __forceinline__ short pcm16_sample(float v, float scale) {
+  return (short)min(max(__float2int_rz(v * scale), -32768), 32767);
+}
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

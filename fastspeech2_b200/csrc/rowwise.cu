@@ -625,10 +625,10 @@ __global__ void wav_to_int16_kernel(const float* __restrict__ wav, long long wav
     const float4 a = __ldg(reinterpret_cast<const float4*>(src)), c = __ldg(reinterpret_cast<const float4*>(src) + 1);
     const float f[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
 #pragma unroll
-    for (int k = 0; k < 8; k++) v[k] = t0 + k < len ? (short)min(max(__float2int_rz(f[k] * scale), -32768), 32767) : (short)0;
+    for (int k = 0; k < 8; k++) v[k] = t0 + k < len ? pcm16_sample(f[k], scale) : (short)0;
   } else {
 #pragma unroll
-    for (int k = 0; k < 8; k++) v[k] = (t0 + k < N && t0 + k < len) ? (short)min(max(__float2int_rz(src[k] * scale), -32768), 32767) : (short)0;
+    for (int k = 0; k < 8; k++) v[k] = (t0 + k < N && t0 + k < len) ? pcm16_sample(src[k], scale) : (short)0;
   }
   short* dst = out + (long long)b * N + t0;
   if (t0 + 8 <= N && ((reinterpret_cast<uintptr_t>(dst) & 15u) == 0)) {

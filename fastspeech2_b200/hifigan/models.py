@@ -12,8 +12,9 @@ import torch
 import torch.nn as nn
 
 from .. import _lib as L
-from .. import packing
+from .. import ops, packing
 from .._modtree import get, populate
+from ..resample import Resampler
 from ..spec import hifigan_spec
 
 LRELU_SLOPE = 0.1
@@ -241,19 +242,60 @@ class Generator(nn.Module):
         return wav
 
     @torch.no_grad()
-    def stream(self, x, mel_lens=None, chunk_frames=64):
+    def stream(self, x, mel_lens=None, chunk_frames=64, sample_rate=None, pcm16=False):
         """Synthesise in chunks of `chunk_frames` mel frames: an iterator of (first_sample, wav_chunk[B, 1, n]), the chunks in order,
         whose concatenation along the last axis equals forward(x, mel_lens) bit for bit (fs2_vocoder_forward_window).  Each chunk is
         computed from the frames it needs plus the generator's receptive field, in a workspace that depends on B and chunk_frames, not
         on T, and is ready as soon as it is yielded (on the current stream), before the rest of the utterance is synthesised.  The
         arguments are those of forward and are checked, and the mel converted, once, when stream() is called; device mel_lens are
-        never read on the host, so every utterance runs the batch's T frames in lockstep (chunks past an utterance's end are zeros)."""
+        never read on the host, so every utterance runs the batch's T frames in lockstep (chunks past an utterance's end are zeros).
+
+        sample_rate (optional): yield the waveform at this rate instead of h.sampling_rate (resample.Resampler): one chunk per vocoder
+        chunk, holding the outputs whose support has arrived (the last chunk flushes the rest), with first_sample at the new rate.
+        Concatenated, they equal Resampler(h.sampling_rate, sample_rate)(forward(x, mel_lens), mel_lens * hop) bit for bit, hop =
+        prod(upsample_rates) (without mel_lens: of forward(x)); pcm16 yields that output's int16 conversion (x 32768, truncated,
+        clamped).  The lag behind the vocoder is about half_len / up input samples, under 1 ms at 8 to 48 kHz."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
+        rs = self._resampler(sample_rate, chunk_frames)
         dev = get(self, "conv_pre.bias").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
             inputs = self._inputs(x, mel_lens)
-        return self._stream(inputs, chunk_frames)
+        if rs is None and not pcm16:
+            return self._stream(inputs, chunk_frames)
+        return self._stream_resampled(inputs, chunk_frames, rs, pcm16)
+
+    def _resampler(self, sample_rate, chunk_frames):
+        """The Resampler from h.sampling_rate to sample_rate, or None (sample_rate None or equal).  A window needs Resampler.history
+        input samples before its first output's support, which the previous chunk must hold: ValueError otherwise."""
+        if sample_rate is None:
+            return None
+        rs = Resampler(_cfg(self.h, "sampling_rate"), sample_rate)
+        if rs.identity:
+            return None
+        hop = int(np.prod(self._hd["upsample_rates"]))
+        if chunk_frames * hop < rs.history:
+            raise ValueError(f"chunk_frames * {hop} samples must cover the resampler's history of {rs.history} samples")
+        return rs
+
+    def _stream_resampled(self, inputs, chunk_frames, rs, pcm16):
+        _m, _keep, dev, up, B, T, _mel, _bs, _rs, lens_d, _ = inputs
+        N = T * up
+        prev, emitted = None, 0
+        with torch.no_grad(), torch.cuda.device(dev):
+            for i1, wav in self._stream(inputs, chunk_frames):  # i1: the chunk's first sample
+                cur = wav[:, 0]
+                if rs is None:                                  # the generator's own rate, int16 (samples past mel_lens are zeros)
+                    yield i1, ops.wav_to_int16(cur).unsqueeze(1)
+                    continue
+                i2 = i1 + cur.shape[1]
+                r = rs.ready(i2, N, i2 >= N)
+                if r > emitted:
+                    y = rs.window(prev, cur, i1, N, emitted, r, lens=lens_d, lens_scale=up, pcm16=pcm16)
+                else:
+                    y = torch.empty(B, 0, dtype=torch.int16 if pcm16 else torch.float32, device=dev)
+                yield emitted, y.unsqueeze(1)
+                prev, emitted = cur, r
 
     def _stream(self, inputs, chunk_frames):
         lib = L.lib()
@@ -274,14 +316,20 @@ class Generator(nn.Module):
                         "fs2_vocoder_forward_window")
                 yield f0 * up, wav
 
-    def stream_pool(self, chunk_frames=64):
+    def stream_pool(self, chunk_frames=64, sample_rate=None, pcm16=False):
         """A pool of independent streams vocoded together (fs2_vocoder_forward_streams), for serving requests that arrive at different
         times: StreamPool.add(mel) admits a stream, and every StreamPool.step() synthesises the next `chunk_frames` frames of every live
         stream in one call, each at its own position.  Concatenated, one stream's chunks equal self(mel[None]) bit for bit, whatever else
         shares the pool.  It uses the weights packed at creation, like stream(); the workspace depends on the live count and
-        chunk_frames, not on any length."""
+        chunk_frames, not on any length.
+
+        sample_rate (optional): step() returns each stream's chunk at this rate, converted by one fs2_resample_streams launch after the
+        vocoder's call; a stream keeps its chunk count, each chunk holding the outputs whose support has arrived (the last flushes the
+        rest), and concatenated they equal Resampler(h.sampling_rate, sample_rate)(self(mel[None])) bit for bit.  pcm16: int16 chunks
+        (x 32768, truncated, clamped).  ValueError when chunk_frames * hop is below the resampler's history."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
+        rs = self._resampler(sample_rate, chunk_frames)
         if self.training:
             raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
         dev = get(self, "conv_pre.bias").device
@@ -312,7 +360,23 @@ class Generator(nn.Module):
                         "fs2_vocoder_forward_streams")
             return wav
 
-        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev)
+        resample = None
+        if rs is not None:
+            def resample(records, max_out):
+                with torch.cuda.device(dev):
+                    if max_out == 0:                   # no stream has a new output: no launch
+                        return torch.empty(len(records), 0, dtype=torch.int16 if pcm16 else torch.float32, device=dev)
+                    return rs.streams(records, max_out, dev, pcm16=pcm16)
+            resample.rs = rs
+        elif pcm16:                                    # the generator's own rate: the int16 conversion of each step's waveform
+            vocode = launch
+
+            def launch(ptrs, f0s, ns):
+                wav = vocode(ptrs, f0s, ns)
+                with torch.cuda.device(dev):
+                    return ops.wav_to_int16(wav)
+
+        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev, resample=resample)
         pool._keep = keep                              # the packed weights stay alive while the pool runs
         return pool
 
@@ -320,11 +384,17 @@ class Generator(nn.Module):
 class StreamPool:
     """Streams vocoded together in chunks of `chunk_frames` mel frames (Generator.stream_pool).  Streams are kept in admission order;
     each starts at frame 0 in the step after its add() and leaves after its last chunk.  `launch(ptrs, f0s, ns)` computes one step: the
-    [B, chunk_frames * up] waveform of the live streams, stream b from its frame f0s[b] of the ns[b] frames at device address ptrs[b]."""
+    [B, chunk_frames * up] waveform of the live streams, stream b from its frame f0s[b] of the ns[b] frames at device address ptrs[b].
 
-    def __init__(self, launch, n_mel, up, chunk_frames, device):
+    resample (optional): `resample(records, max_out)` converts one step's waveform to another rate in one call, its `.rs` the
+    resample.Resampler whose emission rule decides each stream's outputs: records[b] = (x0, x1, i0, i1, i2, n, j0, j1) gives stream b's
+    previous chunk (address x0, input samples [i0, i1)) and current chunk (x1, [i1, i2)) of its n samples, and the outputs [j0, j1) it
+    emits; the call returns a [B, >= max(j1 - j0)] tensor (max 0 included) whose row b starts with them."""
+
+    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None):
         self._launch, self.n_mel, self.up, self.chunk_frames, self.device = launch, n_mel, up, chunk_frames, torch.device(device)
-        self._live = []                                # [handle, channels-last mel view [n, n_mel], n, next frame]
+        self._resample = resample
+        self._live = []                                # [handle, channels-last mel view [n, n_mel], n, next frame, last chunk, emitted]
         self._next = 0
 
     def add(self, mel):
@@ -346,7 +416,7 @@ class StreamPool:
             rows = rows.to(torch.float32).contiguous()
         h = self._next
         self._next += 1
-        self._live.append([h, rows, n, 0])
+        self._live.append([h, rows, n, 0, None, 0])
         return h
 
     def cancel(self, h):
@@ -362,18 +432,38 @@ class StreamPool:
 
     def step(self):
         """One chunk of every live stream, in one launch call: a list of (handle, first_sample, wav [1, 1, m]) in admission order,
-        m = chunk_frames * up except on a stream's last chunk, which is trimmed to its end.  [] without a call when the pool is empty."""
+        m = chunk_frames * up except on a stream's last chunk, which is trimmed to its end.  [] without a call when the pool is empty.
+        With a resampler: first_sample and m at the new rate, the chunk holding the outputs that became ready (possibly none)."""
         if not self._live:
             return []
         live = self._live
         wav = self._launch([s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live])
+        if self._resample is not None:
+            wav, starts, widths = self._resampled(live, wav)
+        else:
+            starts = [s[3] * self.up for s in live]
+            widths = [min(self.chunk_frames, s[2] - s[3]) * self.up for s in live]
         out, keep = [], []
         for i, s in enumerate(live):
-            h, _, n, f0 = s
-            m = min(self.chunk_frames, n - f0) * self.up
-            out.append((h, f0 * self.up, wav[i:i + 1, :m].unsqueeze(0)))
-            s[3] = f0 + self.chunk_frames
-            if s[3] < n:
+            out.append((s[0], starts[i], wav[i:i + 1, :widths[i]].unsqueeze(0)))
+            s[3] += self.chunk_frames
+            if s[3] < s[2]:
                 keep.append(s)
         self._live = keep
         return out
+
+    def _resampled(self, live, wav):
+        """The resampler's call on this step's waveform: (its output, each stream's first output, each stream's output count)."""
+        rs, n1 = self._resample.rs, self.chunk_frames * self.up
+        records, starts, widths = [], [], []
+        for i, s in enumerate(live):
+            _, _, n, f0, prev, emitted = s
+            i1, N = f0 * self.up, n * self.up
+            r = rs.ready(min(i1 + n1, N), N, f0 + self.chunk_frames >= n)
+            cur = wav[i]
+            records.append((0 if prev is None else prev.data_ptr(), cur.data_ptr(), i1 - (0 if prev is None else n1), i1, i1 + n1, N,
+                            emitted, r))
+            starts.append(emitted)
+            widths.append(r - emitted)
+            s[4], s[5] = cur, r                        # the chunk stays alive as the next step's history
+        return self._resample(records, max(widths)), starts, widths

@@ -514,6 +514,73 @@ typedef struct fs2_vocoder_streams_args {
 size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, int frames);
 int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t stream);
 
+/* ------------------------------------------------------------------ sample-rate conversion of the waveform (scipy.signal.resample_poly)
+ *
+ * up / down is fs_out / fs_in reduced, max(up, down) <= FS2_RESAMPLE_MAX_FACTOR.  With half_len = 10 * max(up, down) and the
+ * (2 half_len + 1)-tap Kaiser(5.0) low-pass h that resample_poly designs (firwin(...) * up), output j of a row of n input samples is
+ *     y[j] = sum over ascending i of x[i] * h[j * down - i * up + half_len],  0 <= i < n,  0 <= j * down - i * up + half_len <= 2 half_len,
+ * for j < n_out = ceil(n * up / down), and 0 for j >= n_out (zero padding: inputs outside [0, n) are zero).  The sum runs in fp32, one
+ * fmaf per tap in descending tap order (ascending i), from fp32 taps, so an output's bits depend on its inputs only, never on where a
+ * window or chunk boundary falls.  Output j reads the K contiguous inputs [q - K + 1, q], q = floor((j * down + half_len) / up), with the
+ * taps of phase p = (j * down + half_len) mod up.
+ * taps: [up][K] fp32, taps[p * K + k] = h[p + k * up], zero where p + k * up > 2 half_len; K = ceil((2 half_len + 1) / up).
+ * pcm16 != 0 writes int16 (trunc(y * scale) clamped to [-32768, 32767], as fs2_wav_to_int16; resampled audio can ring past +-1, so the
+ * clamp is reachable here) instead of fp32.
+ * Every call returns FS2_ERR_ARG before any CUDA call for a ratio, K or pointer that breaks these rules, and FS2_ERR_UNSUPPORTED when the
+ * tap table does not fit the device's shared memory (it always fits an H100's for max(up, down) <= FS2_RESAMPLE_MAX_FACTOR). */
+#define FS2_RESAMPLE_MAX_FACTOR 2048
+
+/* Offline: every row of x [B][N] (batch stride in floats), row b over its own min(lens[b] * lens_scale, N) samples when lens is set
+ * (device int32, clamped, never read by the host), so that row b equals a B = 1 call on its first lens[b] * lens_scale samples and its
+ * outputs at or past ceil(lens[b] * lens_scale * up / down) are zeros.  y: [B][ceil(N * up / down)] with batch stride y_batch_stride
+ * (elements of fp32 or int16). */
+typedef struct fs2_resample_args {
+  int B, up, down, K;
+  const float* taps;
+  const float* x; int64_t x_batch_stride, N;
+  const int32_t* lens; int32_t lens_scale;
+  void* y; int64_t y_batch_stride;
+  int32_t pcm16; float scale;
+} fs2_resample_args;
+int fs2_resample(const fs2_resample_args* a, fs2_stream_t stream);
+
+/* Window: outputs [j0, j1) of every row (0 <= j0 < j1 <= ceil(N * up / down)), written to y[b * y_batch_stride + j - j0], from input
+ * samples [i0, i2) given in two pieces: x0 holds samples [i0, i1) (x0[b * x0_batch_stride + i - i0]), x1 holds [i1, i2) (may be NULL
+ * when i1 == i2) -- typically the previous chunk's tail and the current chunk.  N and lens bound the rows as in fs2_resample.  Every
+ * input of [0, N) the outputs read must lie in [i0, i2), else FS2_ERR_ARG (pure integer host check); inputs at or past a row's
+ * lens[b] * lens_scale are zeros whether given or not.  The outputs equal fs2_resample's bit for bit. */
+typedef struct fs2_resample_window_args {
+  int B, up, down, K;
+  const float* taps;
+  const float* x0; int64_t x0_batch_stride;
+  const float* x1; int64_t x1_batch_stride;
+  int64_t i0, i1, i2, N;
+  const int32_t* lens; int32_t lens_scale;
+  int64_t j0, j1;
+  void* y; int64_t y_batch_stride;
+  int32_t pcm16; float scale;
+} fs2_resample_window_args;
+int fs2_resample_window(const fs2_resample_window_args* a, fs2_stream_t stream);
+
+/* Streams: one device record per stream, each stream at its own position, in one launch (the resampling step of a stream pool).  Stream b
+ * writes its outputs [j0, j1) to y[b * y_batch_stride + j - j0] from its pieces x0 = samples [i0, i1) and x1 = samples [i1, i2) of a
+ * stream of n input samples, equal bit for bit to fs2_resample of that stream alone.  The host never reads the table: the grid is
+ * sized from max_out, j1 - j0 is clamped to [0, max_out], and an input of [0, n) outside [i0, i2) reads as zero (the caller provides
+ * every input its outputs need; Python's stream_pool does by construction). */
+typedef struct fs2_resample_stream_t {
+  const float *x0, *x1;
+  int64_t i0, i1, i2, n, j0, j1;
+} fs2_resample_stream_t;
+typedef struct fs2_resample_streams_args {
+  int B, up, down, K;
+  const float* taps;
+  const fs2_resample_stream_t* table;   /* [B] device */
+  int64_t max_out;
+  void* y; int64_t y_batch_stride;
+  int32_t pcm16; float scale;
+} fs2_resample_streams_args;
+int fs2_resample_streams(const fs2_resample_streams_args* a, fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ misc */
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
@@ -521,8 +588,9 @@ const char* fs2_build_info(void);          /* "sm_90a ..." */
 /* sizeof of a struct above (binding self-check), fs2_<name>[_args]: 0 conv1d, 1 layernorm, 2 attention, 3 embed, 4 rowbias,
  * 5 variance_head, 6 durations, 7 length_regulate, 8 conv_post, 9 acoustic_model, 10 encode, 11 decode, 12 vocoder_model,
  * 13 vocoder, 14 resstack, 15 wav_int16, 16 conv_tc_plan_t, 17 conv_simt_plan_t, 18 resstack_plan_t.  Like fs2_control_args,
- * fs2_vocoder_window_args (80 bytes), fs2_vocoder_window_launch_t (56 bytes) and fs2_vocoder_streams_args (64 bytes) are not in the
- * table: the binding pins their sizes. */
+ * fs2_vocoder_window_args (80 bytes), fs2_vocoder_window_launch_t (56 bytes), fs2_vocoder_streams_args (64 bytes) and the resampler's
+ * structs (fs2_resample_args 88, fs2_resample_window_args 144, fs2_resample_stream_t 64, fs2_resample_streams_args 64 bytes; added at
+ * ABI 12 without a bump, since no existing struct changed) are not in the table: the binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

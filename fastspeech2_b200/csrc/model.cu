@@ -423,7 +423,7 @@ static fs2_resstack_args resblock_run(const fs2_resstack_args& g, int j, int d0,
 
 static bool resstack_width(int C) { return C == 8 || C == 16 || C == 32 || C == 64; }   // the channel counts fs2_resstack serves
 
-// Stage i's operand format, and which of its ResBlock layers run as one fs2_resstack launch: the offline and the windowed walk share them
+// Stage i's operand format, and which of its ResBlock layers run as one fs2_resstack launch (window_walk, fs2_vocoder_resblock_runs)
 static unsigned stage_tcv(const fs2_vocoder_model* m, int i) { return (m->f8_mask & (2 << i)) ? FS2_TC_VARIANT_F8 : 0; }
 static bool stage_fused(const fs2_vocoder_model* m, int i) { return (m->fused_mask >> i) & 1; }
 // A 128-channel stage pairs only with pair_mask bit 8 + i (its tiles are then packed at NB = 128, see fs2_vocoder_model::pair_mask)
@@ -510,125 +510,12 @@ static int stage_runs(const fs2_vocoder_model* m, int i, RbRun* out) {
   return n;
 }
 
-static int vocoder_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, cudaStream_t s, Arena& ar) {
-  const int B = a->B, T = a->T;
-  size_t per_frame = (size_t)m->c0;  // floats per mel frame of the widest activation
-  {
-    int up = 1, ch = m->c0;
-    for (int i = 0; i < m->n_stages; i++) {
-      up *= m->rates[i];
-      ch /= 2;
-      per_frame = per_frame > (size_t)up * ch ? per_frame : (size_t)up * ch;
-    }
-  }
-  const size_t n = (size_t)B * T * per_frame;
-  float* bx = ar.f32(n);
-  float* bu = ar.f32(n);
-  float* bt = ar.f32(n);
-  float* r1 = ar.f32(n);
-  float* r2 = ar.f32(n);
-  if (ar.dry) return FS2_OK;
-  if (!bx || !bu || !bt || !r1 || !r2) return FS2_ERR_WORKSPACE;
-  // Ragged mode: every layer bounds utterance b by mel_lens[b] frames times its rows per mel frame (`scale`), so each utterance is
-  // synthesised as if alone and the tiles of the padding are never computed.  Rows beyond an utterance are left unspecified in the
-  // intermediates; conv_post writes them as zeros.
-  const int32_t* lens = a->mel_lens;
-  int scale = 1;
-
-  // conv_pre reads the (possibly strided) channels-last mel view
-  fs2_conv1d_args c = conv_args(a->mel, B, T, m->n_mel, m->c0, 7, bx);
-  c.x_batch_stride = a->mel_batch_stride; c.x_row_stride = a->mel_row_stride;
-  c.res_batch_stride = c.res_row_stride = 0;                        // no residual
-  c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
-  c.x_lens = lens; c.lens_scale = scale;
-  FS2_TRY(conv1d_dispatch(&c, s));
-  int Ti = T, C = m->c0;
-  const float inv_nk = 1.f / (float)m->n_kernels;
-  for (int i = 0; i < m->n_stages; i++) {
-    const int u = m->rates[i], Co = C / 2;
-    if (m->up_k[i] != 2 * u || (u & 1)) return FS2_ERR_UNSUPPORTED;
-    const unsigned tcv = stage_tcv(m, i);
-    // ---- lrelu + ConvTranspose1d as two 2-tap phase-group convolutions (hifigan/models.py:152-153)
-    for (int g = 0; g < 2; g++) {
-      const size_t off = (size_t)g * (u / 2) * Co;    // group g writes output channels [off, off + (u/2)*Co) of each [u*Co] row
-      c = conv_args(bx, B, Ti, C, (u / 2) * Co, 2, bu + off);
-      c.y_batch_stride = (int64_t)Ti * u * Co; c.y_row_stride = (int64_t)u * Co;
-      c.res_batch_stride = c.res_row_stride = 0;                    // no residual
-      c.pad_left = g == 0 ? 1 : 0;
-      c.w = g == 0 ? m->w_up_a[i] : m->w_up_b[i];
-      c.w_tc = g == 0 ? m->w_up_a_tc[i] : m->w_up_b_tc[i];
-      c.bias = m->b_up[i] + off;
-      c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
-      c.x_lens = lens; c.lens_scale = scale;          // [B][Ti][u*Co]: input and output rows have the same n_b
-      FS2_TRY(conv1d_dispatch(&c, s));
-    }
-    Ti *= u; C = Co; scale *= u;
-    // ---- mean of the multi-receptive-field ResBlocks (models.py:154-160, ResBlock.forward :96-103)
-    const fs2_resstack_args group = resblock_args(m, i, B, Ti, C, lens, scale);
-    if (stage_fused(m, i)) {                           // persistent kernels whose intermediates never leave the SM: the planner's runs
-      if (!tcv) return FS2_ERR_ARG;
-      RbRun runs[RB_MAX_RUNS];
-      const int nr = stage_runs(m, i, runs);
-      if (nr < 0) return nr;
-      const float* r = bu;
-      for (int q = 0; q < nr; q++) {
-        const RbRun& run = runs[q];
-        const bool last = run.d1 == m->n_dil;           // the last run of a ResBlock adds its share of the mean into bx
-        if (run.d0 == 0) r = bu;
-        float* dst = last ? bx : (r == r1 ? r2 : r1);
-        fs2_resstack_args a = group;                   // the whole group: alpha 0 (the mean), no accumulate
-        if (run.j >= 0) {
-          a = resblock_run(group, run.j, run.d0, run.d1);
-          a.alpha = last ? inv_nk : 1.f; a.accumulate = last && run.j > 0;
-        }
-        a.x = r; a.y = dst;
-        FS2_TRY(resstack(&a, s));
-        r = dst;
-      }
-      continue;
-    }
-    for (int j = 0; j < m->n_kernels; j++) {
-      const int rb = i * m->n_kernels + j, k = m->rb_k[j];
-      const float* r = bu;
-      const bool pairs = stage_pairs(m, i, C, k);
-      for (int d = 0; d < m->n_dil; d++) {
-        const bool last = d == m->n_dil - 1;            // the last layer adds its share of the mean over the n_kernels ResBlocks into bx
-        float* dst = last ? bx : (r == r1 ? r2 : r1);
-        const float alpha = last ? inv_nk : 1.f;
-        const int accumulate = last && j > 0;
-        if (pairs) {                                   // one launch per (dilated conv, conv, +x) pair: the intermediate stays on chip
-          fs2_resstack_args p = resblock_run(group, j, d, d + 1);
-          p.x = r; p.y = dst; p.alpha = alpha; p.accumulate = accumulate;
-          FS2_TRY(resstack(&p, s, nullptr, 0, nullptr, C == 128));
-        } else {                                       // the two convs through bt
-          const int dil = m->rb_dil[j][d];
-          c = conv_args(r, B, Ti, C, C, k, bt);
-          c.w = m->w_rb1[rb][d]; c.w_tc = m->w_rb1_tc[rb][d]; c.bias = m->b_rb1[rb][d]; c.tc_variant = tcv;
-          c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
-          c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
-          c.x_lens = lens; c.lens_scale = scale;
-          FS2_TRY(conv1d_dispatch(&c, s));
-          c = conv_args(bt, B, Ti, C, C, k, dst);
-          c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
-          c.res = r; c.alpha = alpha; c.accumulate = accumulate;
-          c.x_lens = lens; c.lens_scale = scale;
-          FS2_TRY(conv1d_dispatch(&c, s));
-        }
-        r = dst;
-      }
-    }
-  }
-  fs2_conv_post_args p{};
-  p.x = bx; p.B = B; p.T = Ti; p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f; p.wav = a->wav;
-  p.lens = lens; p.lens_scale = scale;
-  return conv_post(&p, s);
-}
-
-// ------------------------------------------------------------------ windowed vocoder (fs2_vocoder_forward_window)
+// ------------------------------------------------------------------ vocoder (fs2_vocoder_forward, _forward_window, _forward_streams)
 // A window [f0, f1) is walked backward from its output samples to the rows every layer must compute (each conv: its consumers' rows
-// widened by its radius, clipped to the utterance's logical extent), then forward in the offline call's launch order, every layer
-// computing only those rows with the kernels and arithmetic the offline call uses (RowWindow).  One walk makes both the plan
-// (fs2_vocoder_window_plan) and, given a WinExec, the launches, so the two cannot disagree.
+// widened by its radius, clipped to the utterance's logical extent), then forward in launch order, every layer computing only those
+// rows with the kernels and arithmetic of the whole batch (RowWindow).  One walk makes both the plan (fs2_vocoder_window_plan) and,
+// given a WinExec, the launches, so the two cannot disagree.  fs2_vocoder_forward is the window [0, T) of a T-frame batch: every range
+// is then [0, T * scale), every buffer [B][T * scale][C], and the walk runs the offline entry points (no RowWindow).
 
 struct Rows {
   int lo, hi;
@@ -642,6 +529,12 @@ static Rows widen(Rows r, int by, long long cap) {
 }
 static int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 static int pair_reach(const fs2_vocoder_model* m, int j, int d) { return (m->rb_k[j] - 1) * m->rb_dil[j][d] / 2 + (m->rb_k[j] - 1) / 2; }
+// rows per mel frame at stage i's input, prod(rates[0, i)); i = n_stages: waveform samples per mel frame
+static long long frame_rows(const fs2_vocoder_model* m, int i) {
+  long long r = 1;
+  for (int k = 0; k < i; k++) r *= m->rates[k];
+  return r;
+}
 
 // A window buffer: logical rows [lo, lo + rows) of C floats each, utterances `rows` rows apart.
 struct View {
@@ -651,10 +544,10 @@ struct View {
   int64_t bs() const { return (int64_t)rows * C; }
 };
 
-// What a walk issues: the batch's mel view and lengths, the waveform, and the offline call's five buffers, each B * width floats.
-// org: NULL (one window for the whole batch, fs2_vocoder_forward_window), or the per-utterance origin mode (fs2_vocoder_forward_streams):
-// the walk is then the unclipped plan of [0, frames), its rows are window rows, utterance b's window starts at its frame org[b]
-// (origin_rows), and the mel is the staged window buffer.
+// What a walk issues: the batch's mel view and lengths, the waveform, and five buffers, each B * width floats (window_plan).
+// org: NULL (one window for the whole batch), or the per-utterance origin mode (fs2_vocoder_forward_streams): the walk is then the
+// unclipped plan of [0, frames), its rows are window rows, utterance b's window starts at its frame org[b] (origin_rows), and the mel
+// is the staged window buffer.
 struct WinExec {
   int B; cudaStream_t s;
   const float* mel; int64_t mel_bs, mel_rs;
@@ -673,20 +566,23 @@ static fs2_conv1d_args win_conv_args(const float* x, int64_t xbs, int64_t xrs, i
 }
 
 // The launches of window [f0, f1) of a T-frame batch (f1 <= T), appended to L in issue order; with ex, also issued.  T < 0: the plan of
-// an unclipped [f0, f1) (no launches), whose row counts bound those of every window of f1 - f0 frames.
+// an unclipped [f0, f1) (no launches), whose row counts bound those of every window of f1 - f0 frames.  Refuses a model it cannot run
+// before its first launch.
 static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::vector<fs2_vocoder_window_launch_t>& L, const WinExec* ex) {
   const int n = m->n_stages;
   int sc[FS2_MAX_STAGES + 1];                          // rows per mel frame at stage i's input (sc[n]: the waveform)
-  sc[0] = 1;
+  for (int i = 0; i <= n; i++) sc[i] = (int)frame_rows(m, i);
   for (int i = 0; i < n; i++) {
     if (m->up_k[i] != 2 * m->rates[i] || (m->rates[i] & 1)) return FS2_ERR_UNSUPPORTED;
     if (stage_fused(m, i) && !stage_tcv(m, i)) return FS2_ERR_ARG;
-    sc[i + 1] = sc[i] * m->rates[i];
   }
   auto cap = [&](int scale) { return T < 0 ? -1LL : (long long)T * scale; };
   // the kernels' logical length at `scale` rows per frame; the origin mode bounds every utterance by itself (origin_rows)
   const int* org = ex ? ex->org : nullptr;
   auto len = [&](int scale) { return org ? ORIGIN_CAP : T * scale; };
+  // the whole batch [0, T) runs the offline entry points (the window ones compute the same bits; conv_post has one kernel)
+  const bool whole = !org && T >= 0 && f0 == 0 && f1 == T;
+  auto win = [&](const RowWindow& w) -> const RowWindow* { return whole ? nullptr : &w; };
   // ---- backward: O[i + 1] = the rows stage i's output must hold (O[0]: conv_pre's), U[i] = its ResBlocks' input, Q[i] = the
   // ConvTranspose's phase-group rows
   Rows O[FS2_MAX_STAGES + 1], U[FS2_MAX_STAGES], Q[FS2_MAX_STAGES];
@@ -723,14 +619,14 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     fs2_conv1d_args c = win_conv_args(ex->mel, ex->mel_bs, ex->mel_rs, B, len(1), m->n_mel, bx, C, 7);
     c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
     c.x_lens = lens; c.lens_scale = 1;
-    const RowWindow w{O[0].lo, O[0].hi, mel.hi};
-    FS2_TRY(conv1d_dispatch(&c, s, &w, org));
+    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi}), org));
   }
   const float inv_nk = 1.f / (float)m->n_kernels;
   for (int i = 0; i < n; i++) {
     const int u = m->rates[i], Co = C / 2, s0 = sc[i], s1 = sc[i + 1];
     const unsigned tcv = stage_tcv(m, i);
-    // ---- ConvTranspose phase groups: rows Q[i] of [u * Co] = the next rate's rows [Q.lo * u, Q.hi * u)
+    // ---- lrelu + ConvTranspose1d as two 2-tap phase-group convolutions (hifigan/models.py:152-153): rows Q[i] of [u * Co] = the
+    // next rate's rows [Q.lo * u, Q.hi * u)
     const double up_flops = 2.0 * Q[i].n() * C * 2 * (u / 2) * Co;
     const View bu{ex ? ex->bu : nullptr, Q[i].lo, Q[i].n(), u * Co};
     int up_src = -1;
@@ -738,7 +634,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       const Rows x = widen(Rows{Q[i].lo - (g == 0), Q[i].hi + (g == 1)}, 0, cap(s0));
       up_src = add(g == 0 ? FS2_VW_UP_A : FS2_VW_UP_B, i, -1, -1, s0, Q[i], x, last, -1, up_flops);
       if (!ex) continue;
-      const size_t off = (size_t)g * (u / 2) * Co;
+      const size_t off = (size_t)g * (u / 2) * Co;    // group g writes output channels [off, off + (u/2)*Co) of each [u*Co] row
       fs2_conv1d_args c = win_conv_args(bx.at(), bx.bs(), C, B, len(s0), C, bu, (u / 2) * Co, 2);
       c.y += off;
       c.pad_left = g == 0 ? 1 : 0;
@@ -747,111 +643,89 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       c.bias = m->b_up[i] + off;
       c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
       c.x_lens = lens; c.lens_scale = s0;
-      const RowWindow w{Q[i].lo, Q[i].hi, x.hi};
-      FS2_TRY(conv1d_dispatch(&c, s, &w, org));
+      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi}), org));
     }
     C = Co;
     const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
     const long long cap1 = cap(s1);
     bx = View{bx.p, O[i + 1].lo, O[i + 1].n(), C};
-    const fs2_resstack_args group = ex ? resblock_args(m, i, B, len(s1), C, lens, s1) : fs2_resstack_args{};
-    // output rows of ResBlock j's pair d (R[j][d]) and the algorithmic FLOPs of its two convs
-    auto pair_rows = [&](int j, Rows* R, double* fl) {
-      const int k = m->rb_k[j];
-      R[m->n_dil - 1] = O[i + 1];
-      for (int d = m->n_dil - 1; d > 0; d--) R[d - 1] = widen(R[d], pair_reach(m, j, d), cap1);
-      for (int d = 0; d < m->n_dil; d++) fl[d] = 2.0 * C * k * C * (widen(R[d], (k - 1) / 2, cap1).n() + R[d].n());
-    };
-    if (stage_fused(m, i)) {                           // the planner's runs (fs2_vocoder_resblock_runs), each widened by its total reach
-      RbRun runs[RB_MAX_RUNS];
-      const int nr = stage_runs(m, i, runs);
+    // ---- mean of the multi-receptive-field ResBlocks (models.py:154-160, ResBlock.forward :96-103).  Its launches: in a fused stage
+    // the planner's runs (fs2_vocoder_resblock_runs), each widened by its total reach; else one (j, d, d + 1) per layer, a fused pair
+    // (the intermediate stays on chip) or the two convs through bt.
+    const bool fused = stage_fused(m, i);
+    RbRun runs[RB_MAX_RUNS];
+    int nr = 0;
+    if (fused) {
+      nr = stage_runs(m, i, runs);
       if (nr < 0) return nr;
-      View r = in;
-      int r_src = up_src;
-      for (int q = 0; q < nr; q++) {
-        const RbRun& run = runs[q];
-        const bool lastd = run.d1 == m->n_dil;
-        Rows R[FS2_MAX_DIL], y = O[i + 1], x = U[i];
-        double fd[FS2_MAX_DIL], fl = 0;
-        for (int j = run.j < 0 ? 0 : run.j; j < (run.j < 0 ? m->n_kernels : run.j + 1); j++) {
-          pair_rows(j, R, fd);
-          for (int d = run.d0; d < run.d1; d++) fl += fd[d];
-        }
-        if (run.j >= 0) {
-          y = R[run.d1 - 1];
-          x = widen(R[run.d0], pair_reach(m, run.j, run.d0), cap1);
-        }
-        if (run.d0 == 0) { r = in; r_src = up_src; }
-        r_src = add(FS2_VW_RB_GROUP, i, run.j, run.j < 0 ? -1 : run.d0, s1, y, x, r_src, -1, fl);
-        const View dst{lastd ? bx.p : (ex && r.p == ex->r1 ? ex->r2 : (ex ? ex->r1 : nullptr)), y.lo, y.n(), C};
+    } else {
+      for (int j = 0; j < m->n_kernels; j++)
+        for (int d = 0; d < m->n_dil; d++) runs[nr++] = RbRun{j, d, d + 1, 0, 0, 0, 0};
+    }
+    const fs2_resstack_args group = ex ? resblock_args(m, i, B, len(s1), C, lens, s1) : fs2_resstack_args{};
+    auto conv_flops = [&](Rows y, int k) { return 2.0 * y.n() * C * k * C; };
+    View r = in;
+    int r_src = up_src;
+    for (int q = 0; q < nr; q++) {
+      const RbRun& run = runs[q];
+      const bool lastd = run.d1 == m->n_dil;          // the last layer of a ResBlock adds its share of the mean into bx
+      if (run.d0 == 0) { r = in; r_src = up_src; }
+      // R[d]: output rows of ResBlock j's pair d; the launch's FLOPs are its convs' over their rows
+      Rows R[FS2_MAX_DIL], y = O[i + 1], x = U[i];
+      double fl = 0;
+      for (int j = run.j < 0 ? 0 : run.j; j < (run.j < 0 ? m->n_kernels : run.j + 1); j++) {
+        const int k = m->rb_k[j];
+        R[m->n_dil - 1] = O[i + 1];
+        for (int d = m->n_dil - 1; d > 0; d--) R[d - 1] = widen(R[d], pair_reach(m, j, d), cap1);
+        for (int d = run.d0; d < run.d1; d++) fl += conv_flops(widen(R[d], (k - 1) / 2, cap1), k) + conv_flops(R[d], k);
+      }
+      if (run.j >= 0) {
+        y = R[run.d1 - 1];
+        x = widen(R[run.d0], pair_reach(m, run.j, run.d0), cap1);
+      }
+      const View dst{lastd ? bx.p : (ex && r.p == ex->r1 ? ex->r2 : (ex ? ex->r1 : nullptr)), y.lo, y.n(), C};
+      const float alpha = lastd ? inv_nk : 1.f;
+      const int accumulate = lastd && run.j > 0;
+      if (fused || stage_pairs(m, i, C, m->rb_k[run.j])) {
+        r_src = add(fused ? FS2_VW_RB_GROUP : FS2_VW_RB_PAIR, i, run.j, run.j < 0 ? -1 : run.d0, s1, y, x, r_src, fused ? -1 : r_src, fl);
         if (ex) {
           fs2_resstack_args a = group;                 // the whole group: alpha 0 (the mean), no accumulate
           if (run.j >= 0) {
             a = resblock_run(group, run.j, run.d0, run.d1);
-            a.alpha = lastd ? inv_nk : 1.f; a.accumulate = lastd && run.j > 0;
+            a.alpha = alpha; a.accumulate = accumulate;
           }
           a.x = r.p; a.y = dst.p;
-          const RowWindow w{y.lo, y.hi, r.lo + r.rows};
-          FS2_TRY(resstack(&a, s, &w, r.lo, org));
+          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}), r.lo, org, C == 128));
         }
-        r = dst;
-      }
-      last = r_src;
-      continue;
-    }
-    for (int j = 0; j < m->n_kernels; j++) {
-      const int rb = i * m->n_kernels + j, k = m->rb_k[j];
-      Rows R[FS2_MAX_DIL];                             // output rows of pair d
-      R[m->n_dil - 1] = O[i + 1];
-      for (int d = m->n_dil - 1; d > 0; d--) R[d - 1] = widen(R[d], pair_reach(m, j, d), cap1);
-      View r = in;
-      int r_src = up_src;
-      for (int d = 0; d < m->n_dil; d++) {
-        const bool lastd = d == m->n_dil - 1;
-        const Rows x = widen(R[d], pair_reach(m, j, d), cap1), mid = widen(R[d], (k - 1) / 2, cap1);
-        const double f1c = 2.0 * mid.n() * C * k * C, f2c = 2.0 * R[d].n() * C * k * C;
-        const View dst{lastd ? bx.p : (ex && r.p == ex->r1 ? ex->r2 : (ex ? ex->r1 : nullptr)), R[d].lo, R[d].n(), C};
-        const float alpha = lastd ? inv_nk : 1.f;
-        const int accumulate = lastd && j > 0;
-        if (stage_pairs(m, i, C, k)) {
-          const int id = add(FS2_VW_RB_PAIR, i, j, d, s1, R[d], x, r_src, r_src, f1c + f2c);
-          if (ex) {
-            fs2_resstack_args p = resblock_run(group, j, d, d + 1);
-            p.x = r.p; p.y = dst.p; p.alpha = alpha; p.accumulate = accumulate;
-            const RowWindow w{R[d].lo, R[d].hi, r.lo + r.rows};
-            FS2_TRY(resstack(&p, s, &w, r.lo, org, C == 128));
-          }
-          r_src = id;
-        } else {
-          const int c1 = add(FS2_VW_RB_CONV1, i, j, d, s1, mid, x, r_src, -1, f1c);
-          const int c2 = add(FS2_VW_RB_CONV2, i, j, d, s1, R[d], mid, c1, r_src, f2c);
-          if (ex) {
-            const int dil = m->rb_dil[j][d];
-            const View t{ex->bt, mid.lo, mid.n(), C};
-            fs2_conv1d_args c = win_conv_args(r.at(), r.bs(), C, B, len(s1), C, t, C, k);
-            c.w = m->w_rb1[rb][d]; c.w_tc = m->w_rb1_tc[rb][d]; c.bias = m->b_rb1[rb][d]; c.tc_variant = tcv;
-            c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
-            c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
-            c.x_lens = lens; c.lens_scale = s1;
-            const RowWindow w1{mid.lo, mid.hi, x.hi};
-            FS2_TRY(conv1d_dispatch(&c, s, &w1, org));
-            c = win_conv_args(t.at(), t.bs(), C, B, len(s1), C, dst, C, k);
-            c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
-            c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
-            c.alpha = alpha; c.accumulate = accumulate;
-            c.x_lens = lens; c.lens_scale = s1;
-            const RowWindow w2{R[d].lo, R[d].hi, mid.hi};
-            FS2_TRY(conv1d_dispatch(&c, s, &w2, org));
-          }
-          r_src = c2;
+      } else {
+        const int j = run.j, d = run.d0, rb = i * m->n_kernels + j, k = m->rb_k[j];
+        const Rows mid = widen(y, (k - 1) / 2, cap1);
+        const int c1 = add(FS2_VW_RB_CONV1, i, j, d, s1, mid, x, r_src, -1, conv_flops(mid, k));
+        r_src = add(FS2_VW_RB_CONV2, i, j, d, s1, y, mid, c1, r_src, conv_flops(y, k));
+        if (ex) {
+          const int dil = m->rb_dil[j][d];
+          const View t{ex->bt, mid.lo, mid.n(), C};
+          fs2_conv1d_args c = win_conv_args(r.at(), r.bs(), C, B, len(s1), C, t, C, k);
+          c.w = m->w_rb1[rb][d]; c.w_tc = m->w_rb1_tc[rb][d]; c.bias = m->b_rb1[rb][d]; c.tc_variant = tcv;
+          c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
+          c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
+          c.x_lens = lens; c.lens_scale = s1;
+          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi}), org));
+          c = win_conv_args(t.at(), t.bs(), C, B, len(s1), C, dst, C, k);
+          c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
+          c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
+          c.alpha = alpha; c.accumulate = accumulate;
+          c.x_lens = lens; c.lens_scale = s1;
+          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi}), org));
         }
-        r = dst;
       }
-      last = r_src;
+      r = dst;
     }
+    last = r_src;
   }
   add(FS2_VW_CONV_POST, -1, -1, -1, sc[n], post, O[n], last, -1, 2.0 * post.n() * C * 7);
   if (!ex) return FS2_OK;
+  // conv_post takes its window in every mode (a NULL one would ignore the batch strides); the whole batch's is {0, T * up, T * up}
   fs2_conv_post_args p{};
   p.x = bx.at(); p.B = B; p.T = len(sc[n]); p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
   p.wav = ex->wav - post.lo;                           // sample f0 * up is the caller's wav[0]
@@ -860,10 +734,10 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   return conv_post(&p, s, &w, bx.bs(), ex->wav_bs, org);
 }
 
-// Floats per utterance of each of the five buffers of a window of `frames` frames: the widest output of its unclipped plan
-static int window_width(const fs2_vocoder_model* m, int frames, size_t& width) {
-  std::vector<fs2_vocoder_window_launch_t> L;
-  FS2_TRY(window_walk(m, -1, 0, frames, L, nullptr));
+// The plan of [0, frames) clipped at T (T < 0: unclipped, the bound of every window of `frames` frames), and the floats per utterance
+// of each of the five buffers that hold it: the widest output of its launches
+static int window_plan(const fs2_vocoder_model* m, int T, int frames, std::vector<fs2_vocoder_window_launch_t>& L, size_t& width) {
+  FS2_TRY(window_walk(m, T, 0, frames, L, nullptr));
   width = 0;
   for (const auto& l : L) {
     size_t ch = 0;                                     // floats per output row
@@ -876,25 +750,39 @@ static int window_width(const fs2_vocoder_model* m, int frames, size_t& width) {
   return FS2_OK;
 }
 
-static int vocoder_window_impl(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, int frames, cudaStream_t s, Arena& ar) {
+// fs2_vocoder_forward: the window [0, T) of the batch, on buffers of B * T * max(c0, max_i prod(rates[0, i]) * c_i) floats
+static int vocoder_forward_impl(const fs2_vocoder_model* m, const fs2_vocoder_args* a, cudaStream_t s, Arena& ar) {
+  std::vector<fs2_vocoder_window_launch_t> L;
   size_t width = 0;
-  FS2_TRY(window_width(m, frames, width));
+  FS2_TRY(window_plan(m, a->T, a->T, L, width));
+  const size_t nf = (size_t)a->B * width;
+  WinExec ex{a->B, s, a->mel, a->mel_batch_stride, a->mel_row_stride, a->mel_lens, nullptr, a->wav, a->T * frame_rows(m, m->n_stages),
+             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
+  if (ar.dry) return FS2_OK;
+  if (!ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
+  L.clear();
+  return window_walk(m, a->T, 0, a->T, L, &ex);
+}
+
+static int vocoder_window_impl(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, int frames, cudaStream_t s, Arena& ar) {
+  std::vector<fs2_vocoder_window_launch_t> L;
+  size_t width = 0;
+  FS2_TRY(window_plan(m, -1, frames, L, width));
   const size_t nf = (size_t)a->B * width;
   WinExec ex{a->B, s, a->mel, a->mel_batch_stride, a->mel_row_stride, a->mel_lens, nullptr, a->wav, a->wav_batch_stride,
              ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
   if (ar.dry) return FS2_OK;
   if (!ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
-  std::vector<fs2_vocoder_window_launch_t> L;
+  L.clear();
   return window_walk(m, a->T, a->f0, a->f1 < a->T ? a->f1 : a->T, L, &ex);
 }
 
 // fs2_vocoder_forward_streams: the unclipped plan of [0, frames) once for the whole batch, each stream at its own origin.  The mel cone
 // (conv_pre's input rows [x0, x1) of that plan) is staged first, [B][x1 - x0][n_mel], so that conv_pre reads one batch-strided buffer.
 static int vocoder_streams_impl(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, cudaStream_t s, Arena& ar) {
-  size_t width = 0;
-  FS2_TRY(window_width(m, a->frames, width));
   std::vector<fs2_vocoder_window_launch_t> L;
-  FS2_TRY(window_walk(m, -1, 0, a->frames, L, nullptr));
+  size_t width = 0;
+  FS2_TRY(window_plan(m, -1, a->frames, L, width));
   const int x0 = L[0].x0, rows = L[0].x1 - L[0].x0;     // launch 0 is conv_pre
   const size_t nf = (size_t)a->B * width;
   float* mel = ar.f32((size_t)a->B * rows * m->n_mel);
@@ -1064,14 +952,14 @@ size_t fs2_vocoder_workspace_bytes(const fs2_vocoder_model* m, int B, int T) {
   Arena ar(nullptr, 0);
   fs2_vocoder_args a{};
   a.B = B; a.T = T;
-  vocoder_impl(m, &a, nullptr, ar);
+  if (vocoder_forward_impl(m, &a, nullptr, ar) != FS2_OK) return 0;
   return ar.off + 256;
 }
 
 int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, fs2_stream_t st) {
   if (!vocoder_ok(m) || !a || a->B <= 0 || a->T <= 0 || !a->mel || !a->wav || !a->workspace) return FS2_ERR_ARG;
   Arena ar(a->workspace, a->workspace_bytes);
-  return vocoder_impl(m, a, S(st), ar);
+  return vocoder_forward_impl(m, a, S(st), ar);
 }
 
 // fs2_vocoder_window_args and fs2_vocoder_window_launch_t are not in the fs2_struct_size table (it stays at 0..18): pinned here and in
@@ -1080,11 +968,7 @@ static_assert(sizeof(fs2_vocoder_window_args) == 80, "fs2_vocoder_window_args: f
 static_assert(sizeof(fs2_vocoder_window_launch_t) == 56, "fs2_vocoder_window_launch_t: twelve int32 and a double");
 
 // Row counts of a window must fit the kernels' int rows with the halo: frames (and T) times prod(rates) below 2^30
-static bool window_rows_ok(const fs2_vocoder_model* m, long long frames) {
-  long long up = 1;
-  for (int i = 0; i < m->n_stages; i++) up *= m->rates[i];
-  return frames * up < (1LL << 30);
-}
+static bool window_rows_ok(const fs2_vocoder_model* m, long long frames) { return frames * frame_rows(m, m->n_stages) < (1LL << 30); }
 
 size_t fs2_vocoder_window_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
   if (!vocoder_ok(m) || B <= 0 || frames <= 0 || !window_rows_ok(m, frames)) return 0;
@@ -1099,9 +983,7 @@ int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_win
   if (!vocoder_ok(m) || !a || a->B <= 0 || a->T <= 0 || !a->mel || !a->wav || !a->workspace) return FS2_ERR_ARG;
   if (a->f0 < 0 || a->f1 <= a->f0 || a->f0 >= a->T || !window_rows_ok(m, a->T)) return FS2_ERR_ARG;
   const int frames = (a->f1 < a->T ? a->f1 : a->T) - a->f0;
-  long long up = 1;
-  for (int i = 0; i < m->n_stages; i++) up *= m->rates[i];
-  if (a->B > 1 && a->wav_batch_stride < frames * up) return FS2_ERR_ARG;
+  if (a->B > 1 && a->wav_batch_stride < frames * frame_rows(m, m->n_stages)) return FS2_ERR_ARG;
   Arena ar(a->workspace, a->workspace_bytes);
   return vocoder_window_impl(m, a, frames, S(st), ar);
 }
@@ -1120,9 +1002,7 @@ size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, in
 int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t st) {
   if (!vocoder_ok(m) || !a || a->B <= 0 || a->frames <= 0 || !window_rows_ok(m, a->frames)) return FS2_ERR_ARG;
   if (!a->mel || !a->mel_lens || !a->f0 || !a->wav || !a->workspace) return FS2_ERR_ARG;
-  long long up = 1;
-  for (int i = 0; i < m->n_stages; i++) up *= m->rates[i];
-  if (a->B > 1 && a->wav_batch_stride < a->frames * up) return FS2_ERR_ARG;
+  if (a->B > 1 && a->wav_batch_stride < a->frames * frame_rows(m, m->n_stages)) return FS2_ERR_ARG;
   if (a->workspace_bytes < fs2_vocoder_streams_workspace_bytes(m, a->B, a->frames)) return FS2_ERR_ARG;
   Arena ar(a->workspace, a->workspace_bytes);
   return vocoder_streams_impl(m, a, S(st), ar);

@@ -437,6 +437,10 @@ typedef struct fs2_vocoder_args {
    * (fs2_conv1d x_lens / fs2_resstack lens / fs2_conv_post lens with the layer's frames-to-rows factor as lens_scale). */
   const int32_t* mel_lens;
 } fs2_vocoder_args;
+/* fs2_vocoder_forward issues the launches of fs2_vocoder_window_plan(m, T, 0, T), in five workspace buffers of B * T * max(c0,
+ * max_i prod(rates[0..i]) * (c0 >> (i + 1))) floats each.  A model it cannot run -- a stage with up_k != 2 * rate or an odd rate
+ * (FS2_ERR_UNSUPPORTED), or a fused_mask stage without f8_mask bit 1 + i (FS2_ERR_ARG) -- is refused before any CUDA call, and
+ * fs2_vocoder_workspace_bytes returns 0 for it. */
 size_t fs2_vocoder_workspace_bytes(const fs2_vocoder_model* m, int B, int T);
 int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, fs2_stream_t stream);
 
@@ -485,7 +489,8 @@ typedef struct fs2_vocoder_window_launch_t {
 /* The launches of the window [f0, f1) of a T-frame batch in issue order, walked backward from the output samples: conv_post +-3
  * rows, a ResBlock conv (k - 1) / 2 * dilation (a fused pair or group: its total reach), a ConvTranspose phase-group pair whose output
  * rows [a, b) at the next rate read input rows [floor(a / u) - 1, ceil(b / u) + 1), conv_pre +-3.  Writes min(count, max_launches)
- * records to out (may be NULL) and returns the count, or FS2_ERR_ARG.  Pure host logic: no CUDA call. */
+ * records to out (may be NULL) and returns the count, or FS2_ERR_ARG.  Pure host logic: no CUDA call.  The plan of [0, T) is
+ * fs2_vocoder_forward's launch list. */
 int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, fs2_vocoder_window_launch_t* out, int max_launches);
 
 /* Many independent streams in one call: stream b's window is its mel frames [f0[b], f0[b] + frames), each stream at its own position.

@@ -2,9 +2,12 @@
 passed on the command line (e.g. the previous commit built into scratch_ab/, which is not tracked).  Same inputs, same packed
 weights; every comparison must match bit for bit.
 
-  1. workspace sizes (no GPU needed): fs2_{encode,decode,vocoder}_workspace_bytes for the LJSpeech and LibriTTS model shapes.
-  2. whole forwards: every output of FastSpeech2 and Generator under several tensor-core / vocoder policies, the kernel launch
-     count and the per-class launches of fs2_profile_begin / fs2_profile_end.
+  1. host logic (no GPU needed): fs2_{encode,decode,vocoder}_workspace_bytes for the LJSpeech and LibriTTS model shapes; for V1, V2
+     and tests/test_stream_vocoder_cpu.py's other generator under each of its policies, the vocoder's launch plans
+     (fs2_vocoder_window_plan, record for record; the plan of [0, T) is fs2_vocoder_forward's launches), its ResBlock runs and its
+     offline, window and streams workspace sizes.
+  2. whole forwards: every output of FastSpeech2 and Generator (forward, stream, stream_pool) under several tensor-core / vocoder
+     policies, the kernel launch count and the per-class launches of fs2_profile_begin / fs2_profile_end.
   3. the tensor-core conv: ragged cases and every epilogue mode, then per-layer timing.
 
 usage: python scripts/ab_lib.py [old.so]
@@ -85,6 +88,39 @@ for B in BATCHES:
         assert ws["new"] == ws["old"] > 0, ("vocoder", B, n, ws)
         n_ws += 1
 print(f"workspace bytes: new == old for {n_ws} (model, B, L / T) queries", flush=True)
+
+from tests.test_stream_vocoder_cpu import CONFIGS, POLICIES as PLAN_POLICIES, _model, _windows
+
+
+def host(fn):
+    """fn() through the package binding on each library."""
+    got = {}
+    for name, lib in libs.items():
+        L._lib = lib
+        got[name] = fn(lib)
+    L._lib = None
+    return got
+
+
+n_plans = n_ws = 0
+for cfg, shape in CONFIGS.items():
+    for policy in PLAN_POLICIES:
+        vm, _ = _model(shape, policy)
+        for T in (1, 5, 40, 101, 1011):
+            for f0, f1 in _windows(T) + [(0, T)]:
+                if 0 <= f0 < T and f1 > f0:
+                    got = host(lambda lib: [bytes(l) for l in L.vocoder_window_plan(vm, T, f0, f1)])
+                    assert got["new"] == got["old"], ("window plan", cfg, policy, T, f0, f1)
+                    n_plans += 1
+        got = host(lambda lib: [[bytes(r) for r in L.vocoder_resblock_runs(vm, i)] for i in range(vm.n_stages)])
+        assert got["new"] == got["old"], ("resblock runs", cfg, policy)
+        for B in (1, 3, 16):
+            for n in (1, 7, 64, 127, 1011):
+                got = host(lambda lib: [f(C.byref(vm), B, n) for f in (lib.fs2_vocoder_workspace_bytes, lib.fs2_vocoder_window_workspace_bytes,
+                                                                      lib.fs2_vocoder_streams_workspace_bytes)])
+                assert got["new"] == got["old"] and min(got["new"]) > 0, ("vocoder workspaces", cfg, policy, B, n, got)
+                n_ws += 3
+print(f"vocoder host logic: new == old for {n_plans} window plans, the ResBlock runs and {n_ws} workspace queries", flush=True)
 if not torch.cuda.is_available():
     print("no GPU: skipping the forward and conv sections")
     sys.exit(0)
@@ -178,24 +214,53 @@ POLICIES = {                                           # tests/test_gpu_ragged_v
     "split3_everywhere": {"f8_mask": 0},
     "fp32_cuda_cores": {"use_tensor_cores": False},
 }
-h = AttrDict(configs.HIFIGAN_CONFIG)
-gen_sd = synth.hifigan_state_dict(h, seed=0)
 mel_cl = lj_out[1].transpose(1, 2)                     # [B, 80, T] channels-last view of postnet_mel
 mel_c = mel_cl.contiguous()                            # [B, 80, T] contiguous: the Generator transposes it first
 ml = lj_out[9]
-for policy, attrs in POLICIES.items():
+
+
+def generator(config, seed, **attrs):
+    h = AttrDict(config)
     gen = Generator(h)
-    gen.load_state_dict(gen_sd)
+    gen.load_state_dict(synth.hifigan_state_dict(h, seed=seed))
     gen.eval()
     gen.remove_weight_norm()
     gen = gen.to(DEV)
     for k, v in attrs.items():
         setattr(gen, k, v)
     gen._invalidate()
+    return gen
+
+
+def pool_run(gen):
+    """Three utterances through a stream pool of 32-frame chunks, the third admitted after the first step: each one's chunks, joined."""
+    pool, chunks = gen.stream_pool(chunk_frames=32), {}
+    mels = [mel_c[b, :, :int(ml[b])] for b in range(3)]
+    pool.add(mels[0]), pool.add(mels[1])
+    first = True
+    while len(pool):
+        for h, _, w in pool.step():
+            chunks.setdefault(h, []).append(w)
+        if first:
+            pool.add(mels[2])
+            first = False
+    return tuple(torch.cat(chunks[h], -1) for h in sorted(chunks))
+
+
+for policy, attrs in list(POLICIES.items()) + [("wide_pairs", {"wide_pairs": True})]:
+    gen = generator(configs.HIFIGAN_CONFIG, 0, **attrs)
     for layout, mel in (("channels-last", mel_cl), ("contiguous", mel_c)):
         ab(f"Generator {policy}, {layout}, padded", lambda: gen(mel))
         ab(f"Generator {policy}, {layout}, ragged", lambda: gen(mel, mel_lens=ml))
     del gen
+gen = generator(configs.HIFIGAN_V2_CONFIG, 1)
+ab("Generator V2, padded", lambda: gen(mel_c))
+ab("Generator V2, ragged", lambda: gen(mel_c, mel_lens=ml))
+del gen
+gen = generator(configs.HIFIGAN_CONFIG, 0)
+ab("Generator stream(chunk_frames=64), ragged", lambda: torch.cat([w for _, w in gen.stream(mel_c, mel_lens=ml, chunk_frames=64)], -1))
+ab("Generator stream_pool(chunk_frames=32), 3 streams", lambda: pool_run(gen))
+del gen
 L._lib = None
 print("whole forwards: new == old bit for bit, same launches", flush=True)
 

@@ -54,7 +54,7 @@ class Stage:
         self.runs = [(r.j, r.d0, r.d1) for r in L.vocoder_resblock_runs(m, i)]
 
     def launch(self, runs, lens=None):
-        """The launches of `runs` [(j, d0, d1)] (j = -1: the whole group), as model.cu's vocoder_impl issues them; returns y."""
+        """The launches of `runs` [(j, d0, d1)] (j = -1: the whole group), as fs2_vocoder_forward issues them; returns y."""
         return run_stage(self.m, self.pk, self.i, self.x, lens, runs, (self.y, self.r1, self.r2))
 
     def cuts(self, j):

@@ -548,7 +548,7 @@ def acoustic_forward(pk, cfg, speakers, texts, src_lens, p_control=1.0, d_contro
 
 
 def vocoder_forward(pk, rates, rb_k, rb_dil, mel_cl):
-    """Mirror of vocoder_impl in model.cu.  mel_cl: [B,T,80] channels-last."""
+    """Mirror of fs2_vocoder_forward (model.cu's window_walk over [0, T)).  mel_cl: [B,T,80] channels-last."""
     x = conv1d(mel_cl, pk["w_pre"], pk["b_pre"], pad_left=3)
     nk = len(rb_k)
     for i, u in enumerate(rates):

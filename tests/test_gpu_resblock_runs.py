@@ -20,8 +20,8 @@ def _rows_per_frame(m, i):
 
 def run_stage(m, pk, i, x, lens, runs, bufs=None):
     """Stage i's ResBlock group on x [B][N][C] issued as `runs` [(j, d0, d1)] (j = -1: the whole group), with the buffers and
-    arguments model.cu's vocoder_impl uses; bufs: (y, r1, r2) like x, or None for fresh NaN-filled ones.  Returns y.
-    (scripts/resblock_runs_bench.py times stages through this too.)"""
+    arguments fs2_vocoder_forward uses (model.cu's window_walk over [0, T)); bufs: (y, r1, r2) like x, or None for fresh NaN-filled
+    ones.  Returns y.  (scripts/resblock_runs_bench.py times stages through this too.)"""
     nk, nd, scale = m.n_kernels, m.n_dil, _rows_per_frame(m, i)
     ks = [m.rb_k[j] for j in range(nk)]
     dils = [[m.rb_dil[j][d] for d in range(nd)] for j in range(nk)]

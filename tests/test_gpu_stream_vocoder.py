@@ -12,6 +12,7 @@ import torch
 
 from fastspeech2_b200 import _lib as L, configs, synth
 from fastspeech2_b200.hifigan import AttrDict, Generator
+from tests.test_gpu_ragged_vocoder import POLICIES as RAGGED_POLICIES
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -64,6 +65,23 @@ def test_stream_equals_forward(cfg, policy, ragged, chunk):
     got = _streamed(gen, mel, lens, chunk)
     torch.cuda.synchronize()
     assert torch.equal(got, want)
+
+
+@pytest.mark.parametrize("ragged", [False, True])
+@pytest.mark.parametrize("policy", list(RAGGED_POLICIES) + ["wide_pairs"])
+@pytest.mark.parametrize("cfg", ["v1", "v2"])
+def test_forward_launches_the_plan_of_the_whole_batch(cfg, policy, ragged):
+    """forward issues fs2_vocoder_window_plan(m, T, 0, T): one kernel per record."""
+    gen = _generator(configs.HIFIGAN_CONFIG if cfg == "v1" else configs.HIFIGAN_V2_CONFIG,
+                     **({"wide_pairs": True} if policy == "wide_pairs" else RAGGED_POLICIES[policy]))
+    mel = _postnet_view(len(LENS), T, seed=22)          # a channels-last view: forward launches no transpose
+    lens = torch.tensor(LENS) if ragged else None
+    gen(mel, lens)                                      # packs the weights
+    torch.cuda.synchronize()
+    n0 = L.lib().fs2_kernel_launch_count()
+    gen(mel, lens)
+    launches = L.lib().fs2_kernel_launch_count() - n0
+    assert launches == len(L.vocoder_window_plan(gen._packed[0], T, 0, T))
 
 
 def test_stream_contiguous_mel_and_lengths_on_the_device():

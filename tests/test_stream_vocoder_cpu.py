@@ -115,6 +115,38 @@ def test_workspace_is_bounded_by_the_window_not_by_T(cfg):
         assert ws[64] * 50 < full
 
 
+@pytest.mark.parametrize("cfg", list(CONFIGS))
+def test_offline_workspace_is_five_buffers_of_the_widest_layer(cfg):
+    """fs2_vocoder_workspace_bytes: five 256-byte aligned buffers of B * T * max(c0, max_i up_i * c_i) floats, with up_i the rows per
+    mel frame after stage i and c_i = c0 >> (i + 1) its channels, plus 256 bytes."""
+    m, _ = _model(CONFIGS[cfg])
+    per_frame, up = m.c0, 1
+    for i in range(m.n_stages):
+        up *= m.rates[i]
+        per_frame = max(per_frame, up * (m.c0 >> (i + 1)))
+    for B in (1, 3, 16):
+        for T in (1, 7, 127, 1011):
+            n = 4 * B * T * per_frame
+            assert L.lib().fs2_vocoder_workspace_bytes(ctypes.byref(m), B, T) == 4 * ((n + 255) // 256 * 256) + n + 256, (B, T)
+
+
+def test_unsupported_models_are_refused_before_any_cuda_call():
+    """A model the walk cannot run is refused by forward before its first launch (the pointers below are never dereferenced), and
+    has no workspace size."""
+    h = L.lib()
+    T = 40
+    a = L.VocoderArgs(B=2, T=T, mel=0x1000, mel_batch_stride=T * 80, mel_row_stride=80, wav=0x1000, workspace=0x1000,
+                      workspace_bytes=1 << 40)
+    m, _ = _model(configs.HIFIGAN_CONFIG)
+    m.up_k[2] = 2 * m.rates[2] + 2                     # the ConvTranspose runs as two 2-tap phase groups only at up_k = 2 * rate
+    assert h.fs2_vocoder_workspace_bytes(ctypes.byref(m), 2, T) == 0
+    assert h.fs2_vocoder_forward(ctypes.byref(m), ctypes.byref(a), None) == -2     # FS2_ERR_UNSUPPORTED
+    m, _ = _model(configs.HIFIGAN_CONFIG)
+    m.fused_mask, m.f8_mask = 0b1000, m.f8_mask & ~(2 << 3)   # a fused stage without its f16 + f8 tiles
+    assert h.fs2_vocoder_workspace_bytes(ctypes.byref(m), 2, T) == 0
+    assert h.fs2_vocoder_forward(ctypes.byref(m), ctypes.byref(a), None) == -1     # FS2_ERR_ARG
+
+
 @pytest.mark.parametrize("cfg", ["v1", "v2"])
 def test_streamed_work_is_within_ten_percent_of_offline(cfg):
     """Algorithmic FLOPs (every conv over the rows its consumers need) of a 1012-frame utterance in 64-frame chunks."""

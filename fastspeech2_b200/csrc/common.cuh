@@ -65,16 +65,15 @@ __device__ __forceinline__ int ragged_rows(const int* lens, int scale, int cap, 
   return n <= 0 ? 0 : (n >= cap ? cap : (int)n);
 }
 
-// Windowed mode of one vocoder layer (fs2_vocoder_forward_window): the layer computes the logical output rows [y0, yend) and reads
-// logical input rows below xend only; rows outside [0, n_b) still read as zero, so the convs pad at the utterance ends and not at the
-// window's.  The host biases the buffer pointers by the windows' first rows, so kernels address logical rows.  The offline layer is
-// the window {0, cap, cap}.
+// The rows of one vocoder layer: it computes the output rows [y0, yend) and reads input rows below xend only; rows outside the
+// utterance still read as zero, so the convs pad at the utterance ends and not at the window's.  The host biases the buffer pointers
+// by the windows' first rows, so kernels address window rows.  The offline layer is the window {0, cap, cap}.
 struct RowWindow { int y0, yend, xend; };
 
-// Per-utterance origin mode of the windowed layers (fs2_vocoder_forward_streams): every utterance has its own window, and row r of the
-// window buffers is utterance b's logical row r + org[b] * scale.  Rows stay window-relative in the kernels, so only the bounds move:
-// utterance b's live rows are [lo, hi) = [-org[b] * scale, (max(lens[b], 0) - org[b]) * scale), clamped to +-ORIGIN_CAP, which lies
-// beyond every window's rows (an empty span when lens[b] <= 0).  Device values are clamped, never trusted.
+// Per-utterance origin mode of the windowed layers (fs2_vocoder_forward_window and _streams): every utterance has its own window, and
+// row r of the window buffers is utterance b's logical row r + org[b] * scale.  Rows stay window-relative in the kernels, so only the
+// bounds move: utterance b's live rows are [lo, hi) = [-org[b] * scale, (max(lens[b], 0) - org[b]) * scale), clamped to +-ORIGIN_CAP,
+// which lies beyond every window's rows (an empty span when lens[b] <= 0).  Device values are clamped, never trusted.
 constexpr int ORIGIN_CAP = 1 << 30;
 struct RowSpan { int lo, hi; };
 __device__ __forceinline__ int origin_clamp(long long v) { return v < -ORIGIN_CAP ? -ORIGIN_CAP : (v > ORIGIN_CAP ? ORIGIN_CAP : (int)v); }
@@ -82,6 +81,20 @@ __device__ __forceinline__ RowSpan origin_rows(const int* lens, const int* org, 
   const long long o = __ldg(org + b), n = max(__ldg(lens + b), 0);
   return RowSpan{origin_clamp(-o * scale), origin_clamp((n - o) * scale)};
 }
+
+// What a launcher takes in the windowed mode, NULL outside it: the layer's window rows and the utterances' origins, never one without
+// the other.
+struct OriginWindow { RowWindow rows; const int* org; };
+
+// The mel of the windowed vocoder's streams, staged by stage_mel: stream b's rows at table[b], n_mel floats apart (table != NULL), or at
+// mel + b * bs, rs floats apart; its first frame f0s[b], or f0 for every stream (f0s NULL); its length lens[b] clamped to [0, cap], or
+// cap (lens NULL).
+struct MelSource {
+  const float* const* table;
+  const float* mel; int64_t bs, rs;
+  const int32_t* f0s; int f0;
+  const int32_t* lens; int cap;
+};
 
 // A per-element control of fs2_control_args on the [B][L] rows of a variance head or of the durations: c[b, l] = v[b * sb + l * sl]
 // (strides in elements, 0 along a broadcast dimension).  rag: NULL, or the ragged mode's lengths -- columns l >= rag[b] are not read.

@@ -29,7 +29,7 @@ struct ConvP {
   int tiles_per_batch;
   const int* x_lens; int lens_scale;   // ragged batch (fs2_conv1d_args::x_lens) or NULL
   RowWindow win;                       // rows computed and read ({0, T, T} outside the windowed mode)
-  const int* org;                      // per-utterance origins (conv_simt_streams_kernel only), see origin_rows
+  const int* org;                      // the windowed mode's per-utterance origins (conv_simt_streams_kernel only), see origin_rows
 };
 
 // ORG: per-utterance origin mode (origin_rows): utterance b's rows below lo_b read as zero too, and n_b is hi_b
@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvP p) {
   conv_simt_body<BM, BN, ACT, false>(p);
 }
 
-// Per-utterance origin mode (fs2_vocoder_forward_streams): an entry point of its own, so that the other modes keep their code
+// Windowed mode (fs2_vocoder_forward_window and _streams): an entry point of its own, so that the offline one keeps its code
 template <int BM, int BN, int ACT>
 __global__ void __launch_bounds__(256) conv_simt_streams_kernel(const ConvP p) {
   conv_simt_body<BM, BN, ACT, true>(p);
@@ -234,10 +234,9 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* 
   return FS2_OK;
 }
 
-// win: NULL, or the windowed mode (RowWindow; a->T is then the full logical length): the tile is chosen for the window's rows.
+// win (with a->x_lens): NULL, or the windowed mode (OriginWindow; a->T is not used): the tile is chosen for the window's rows.
 // Every output element sums its taps and channels in the same order whatever the tile, so a window computes the offline bits.
-// org (with win and a->x_lens): NULL, or the per-utterance origins of the origin mode (origin_rows; a->T is not used).
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, const int* org) {
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
@@ -245,8 +244,8 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, 
   if (a->res && ((a->res_row_stride & 3) || (a->res_batch_stride & 3))) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
   if (a->in_act != FS2_ACT_NONE && a->in_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;
-  if (org && (!win || !a->x_lens)) return FS2_ERR_ARG;
-  if (org && a->out_act != FS2_ACT_NONE && a->out_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;   // the vocoder's activations
+  if (win && !a->x_lens) return FS2_ERR_ARG;
+  if (win && a->out_act != FS2_ACT_NONE && a->out_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;   // the vocoder's activations
   ConvP p;
   p.x = a->x; p.xbs = a->x_batch_stride; p.xrs = a->x_row_stride;
   p.B = a->B; p.T = a->T; p.Cin = a->Cin;
@@ -259,8 +258,8 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, 
   p.row_lens = a->row_lens;
   p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
-  p.win = win ? *win : RowWindow{0, a->T, a->T};
-  p.org = org;
+  p.win = win ? win->rows : RowWindow{0, a->T, a->T};
+  p.org = win ? win->org : nullptr;
   fs2_conv1d_args rows = *a;
   rows.T = p.win.yend - p.win.y0;
   if (rows.T <= 0) return FS2_ERR_ARG;
@@ -274,7 +273,7 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, 
   const dim3 grid((unsigned)plan.grid_x, (unsigned)plan.grid_y);
   prof_before(s);
 #define FS2_SIMT_ACT(BM_, BN_)                                                                            \
-  if (org) {                                                                                              \
+  if (win) {                                                                                              \
     if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); \
     else conv_simt_streams_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p);                        \
   } else {                                                                                                \

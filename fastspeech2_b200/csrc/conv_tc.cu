@@ -101,23 +101,22 @@ int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t
 }
 
 // a->w_tc must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h) in the format a->tc_variant names.
-// win: NULL, or the windowed mode (RowWindow; a->T is then the full logical length): the plan is made for the window's rows.
-// org (with win and a->x_lens): NULL, or the per-utterance origins of the origin mode (origin_rows; a->T is not used).
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, const int* org) {
+// win (with a->x_lens): NULL, or the windowed mode (OriginWindow; a->T is not used): the plan is made for the window's rows.
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win) {
   if (!a || !a->x || !a->w_tc || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w_tc) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
-  if (org && (!win || !a->x_lens)) return FS2_ERR_ARG;
+  if (win && !a->x_lens) return FS2_ERR_ARG;
   const unsigned variant = a->tc_variant;
   fs2_conv1d_args slice, rows;
   int nseg, seg_nkc;
   const fs2_conv1d_args* plan_args = conv_tc_segments(a, slice, nseg, seg_nkc);
   if (!plan_args) return FS2_ERR_UNSUPPORTED;
   if (win) {                                            // tiles of the window only
-    if (win->yend <= win->y0) return FS2_ERR_ARG;
+    if (win->rows.yend <= win->rows.y0) return FS2_ERR_ARG;
     rows = *plan_args;
-    rows.T = win->yend - win->y0;
+    rows.T = win->rows.yend - win->rows.y0;
     plan_args = &rows;
   }
   int derr = FS2_OK;
@@ -148,11 +147,11 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win, co
   FS2_TRY(conv_tc_plan(plan_args, nseg, g_num_sms, pl));
   p.SA = pl.SA; p.SB = pl.SB; p.TPS = pl.TPS; p.R = pl.R; p.tiles_per_batch = pl.tiles_per_batch; p.n_items = pl.n_items;
   p.stage_off = pl.smem - (int)tc_stage_bytes(pl.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));   // the staged inputs end the budget
-  p.win = win ? *win : RowWindow{0, a->T, a->T};
-  p.org = org;
+  p.win = win ? win->rows : RowWindow{0, a->T, a->T};
+  p.org = win ? win->org : nullptr;
   const unsigned grid = (unsigned)pl.grid;
   const size_t smem = (size_t)pl.smem;
-  const int w = org ? 2 : (win ? 1 : 0);
+  const bool w = win != nullptr;
   prof_before(s);
   switch (pl.NB) {
     case 16: conv_tc_launch_nb16(p, w, grid, smem, s); break;

@@ -75,8 +75,8 @@ struct TcP {
   const int* x_lens;               // ragged batch (fs2_conv1d_args::x_lens) or NULL
   int lens_scale;
   int stage_off;                   // shared-memory byte offset of the staged epilogue inputs (used only if tc_stage_tiles(...) > 0)
-  RowWindow win;                   // windowed mode (conv_tc_window_kernel only): rows computed and read, see RowWindow
-  const int* org;                  // per-utterance origins (conv_tc_streams_kernel only), see origin_rows
+  RowWindow win;                   // windowed mode (conv_tc_streams_kernel only): rows computed and read, see RowWindow
+  const int* org;                  // the windowed mode's per-utterance origins, see origin_rows
 };
 
 // Shared-memory epilogue tiles behind the ring barriers: [full, empty mbarrier per consumer warp][residual tile if res][sum tile if
@@ -237,10 +237,10 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 }
 
 // RAG: ragged batch (TcP::x_lens != NULL), see WorkList (every NB is at or near the 96-register cap of one 544-thread CTA per SM).
-// WIN: windowed mode, see WindowList: the tiles start at p.win.y0, rows at or beyond p.win.yend are not written and rows at or beyond
-// p.win.xend are not read (the host biases x, res and y by the window origins, so rows are logical here).
-// ORG (with WIN): per-utterance origin mode, see origin_rows: rows are window rows, and utterance b's rows below lo_b read as zero too.
-template <int NB, bool RAG, bool WIN, bool ORG = false>
+// WIN: windowed mode with per-utterance origins, see WindowList and origin_rows: the tiles start at p.win.y0, rows at or beyond
+// p.win.yend are not written and rows at or beyond p.win.xend are not read (the host biases x, res and y by the window origins, so rows
+// are window rows here), and utterance b's rows outside [lo_b, hi_b) read as zero.
+template <int NB, bool RAG, bool WIN>
 __device__ __forceinline__ void conv_tc_body(const TcP& p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -260,9 +260,9 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
-  // 128-row tiles x NB-channel blocks; windowed: item.rows bounds the stores, the transform warps bound their loads at min(n_b, xend)
-  std::conditional_t<WIN, WindowList<ORG>, WorkList<RAG>> work;
-  if constexpr (WIN) work.init(p.x_lens, p.lens_scale, p.T, p.B, 128, p.n_items / (p.B * p.tiles_per_batch), p.win.y0, p.win.yend, p.win.yend, p.org);
+  // 128-row tiles x NB-channel blocks; windowed: item.rows bounds the stores, the transform warps bound their loads at min(hi_b, xend)
+  std::conditional_t<WIN, WindowList, WorkList<RAG>> work;
+  if constexpr (WIN) work.init(p.x_lens, p.org, p.lens_scale, p.B, 128, p.n_items / (p.B * p.tiles_per_batch), p.win.y0, p.win.yend, p.win.yend);
   else work.init(p.x_lens, p.lens_scale, p.T, p.B, 128, p.tiles_per_batch, p.n_items);
 
   if (tid == 0) {
@@ -401,18 +401,18 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
     int l_item = blockIdx.x, l_kb = 0, l_seg = 0;
     const float* l_xrow = nullptr;                     // &x[b][t0 - pad][0]; rows outside [0, l_tend) are never dereferenced
     int l_tfirst = 0, l_tend = p.T;                    // l_tend: T, or n_b of a ragged batch
-    int l_tlo = 0;                                     // rows below it read as zero: 0, or lo_b in the origin mode
+    int l_tlo = 0;                                     // rows below it read as zero: 0, or lo_b in the windowed mode
     bool l_interior = false;                           // warp-uniform: every slab row of the item exists
     auto l_set_item = [&]() {
       if (l_item < work.count) {
         const Item it = work.item(l_item);
         if constexpr (WIN) l_tend = work.rows_of(it.b, p.win.xend);
         else l_tend = it.rows;
-        if constexpr (ORG) l_tlo = work.lo_of(it.b);
+        if constexpr (WIN) l_tlo = work.lo_of(it.b);
         const int s_tap = l_seg / p.seg_nkc, s_kc = l_seg - s_tap * p.seg_nkc;   // K-segment: one tap, one 256-channel chunk (0, 0 when nseg == 1)
         l_tfirst = it.t0 - p.pad + s_tap;
         l_xrow = p.x + (long long)it.b * p.xbs + (long long)l_tfirst * p.xrs + s_kc * p.Cin;
-        if constexpr (ORG) l_interior = l_tfirst >= l_tlo && l_tfirst + rows_needed <= l_tend;
+        if constexpr (WIN) l_interior = l_tfirst >= l_tlo && l_tfirst + rows_needed <= l_tend;
         else l_interior = l_tfirst >= 0 && l_tfirst + rows_needed <= l_tend;
       }
     };
@@ -428,7 +428,7 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
         for (int u = 0; u < LD; u++) {
           const int t = l_tfirst + rowu[u];
           bool in;
-          if constexpr (ORG) in = rowu[u] >= 0 && t >= l_tlo && t < l_tend;
+          if constexpr (WIN) in = rowu[u] >= 0 && t >= l_tlo && t < l_tend;
           else in = rowu[u] >= 0 && t >= 0 && t < l_tend;
           if (in) {
             ldg256(dst[u], xk + goff[u]);
@@ -479,24 +479,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const TcP p) {
   conv_tc_body<NB, RAG, false>(p);
 }
 
-// Windowed mode: its own entry point, so that the padded and ragged instantiations keep their code (lens may be NULL here).
+// Windowed mode (fs2_vocoder_forward_window and _streams): an entry point of its own, so that the padded and ragged instantiations keep
+// their code (p.org and the lens are not NULL here).
 template <int NB>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_window_kernel(const TcP p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_kernel(const TcP p) {
   conv_tc_body<NB, true, true>(p);
 }
 
-// Per-utterance origin mode (fs2_vocoder_forward_streams): an entry point of its own as well (p.org and the lens are not NULL here).
-template <int NB>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_kernel(const TcP p) {
-  conv_tc_body<NB, true, true, true>(p);
-}
-
 // The NB instantiations live in their own translation units (conv_tc_nb*.cu) so that the library builds in parallel.
-// conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.  window: 0 offline, 1 windowed
-// (conv_tc_window_kernel), 2 windowed with per-utterance origins (conv_tc_streams_kernel).
+// conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.  window: the windowed mode
+// (conv_tc_streams_kernel).
 #define FS2_CONV_TC_NB_DECL(nb)                        \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes); \
-  void conv_tc_launch_nb##nb(const TcP& p, int window, unsigned grid, size_t smem, cudaStream_t s);
+  void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s);
 FS2_CONV_TC_NB_DECL(16) FS2_CONV_TC_NB_DECL(32) FS2_CONV_TC_NB_DECL(48) FS2_CONV_TC_NB_DECL(64)
 FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CONV_TC_NB_DECL(128)
 #undef FS2_CONV_TC_NB_DECL
@@ -505,12 +500,10 @@ FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CON
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes) {                                                  \
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
     if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_window_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
     return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_streams_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
   }                                                                                                     \
-  void conv_tc_launch_nb##nb(const TcP& p, int window, unsigned grid, size_t smem, cudaStream_t s) {    \
-    if (window == 2) conv_tc_streams_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                     \
-    else if (window) conv_tc_window_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                      \
+  void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s) {   \
+    if (window) conv_tc_streams_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                          \
     else if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                     \
     else conv_tc_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);                                  \
   }

@@ -62,10 +62,10 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 }
 
 // kernels / launchers defined in the other translation units
-// win (the vocoder's windowed mode, RowWindow) and org (its per-utterance origins, origin_rows): NULL everywhere else
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr, const int* org = nullptr);
+// win: the vocoder's windowed mode (OriginWindow), NULL everywhere else
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr);
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr, const int* org = nullptr);
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
@@ -73,12 +73,12 @@ int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
 
 // backend dispatch of the fs2_conv1d contract
-static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const RowWindow* win = nullptr, const int* org = nullptr) {
+static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr) {
   if (!a) return FS2_ERR_ARG;
   if (a->x_lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win, org);
-  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win, org);
-  return conv1d_simt(a, s, win, org);
+  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win);
+  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win);
+  return conv1d_simt(a, s, win);
 }
 int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = false, int fused_from = 0);
 int embed_positions(const fs2_embed_args* a, cudaStream_t s);
@@ -87,12 +87,9 @@ int layernorm(const fs2_layernorm_args* a, cudaStream_t s);
 int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl = nullptr);
 int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr);
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0,
-              const int* org = nullptr);
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win = nullptr, int x0 = 0, const int* org = nullptr,
-             bool wide = false);
-int stage_mel(const float* const* mel, const int32_t* lens, const int32_t* org, int B, int x0, int rows, int n_mel, float* out,
-              cudaStream_t s);
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win = nullptr, int x0 = 0, bool wide = false);
+int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out, bool wide = false);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
@@ -513,9 +510,10 @@ static int stage_runs(const fs2_vocoder_model* m, int i, RbRun* out) {
 // ------------------------------------------------------------------ vocoder (fs2_vocoder_forward, _forward_window, _forward_streams)
 // A window [f0, f1) is walked backward from its output samples to the rows every layer must compute (each conv: its consumers' rows
 // widened by its radius, clipped to the utterance's logical extent), then forward in launch order, every layer computing only those
-// rows with the kernels and arithmetic of the whole batch (RowWindow).  One walk makes both the plan (fs2_vocoder_window_plan) and,
-// given a WinExec, the launches, so the two cannot disagree.  fs2_vocoder_forward is the window [0, T) of a T-frame batch: every range
-// is then [0, T * scale), every buffer [B][T * scale][C], and the walk runs the offline entry points (no RowWindow).
+// rows with the kernels and arithmetic of the whole batch.  One walk makes both the plan (fs2_vocoder_window_plan) and, given a
+// WinExec, the launches, so the two cannot disagree.  It issues two modes: fs2_vocoder_forward is the window [0, T) of a T-frame batch
+// (every range is then [0, T * scale), every buffer [B][T * scale][C], and the walk runs the offline entry points), and the windowed
+// calls run the unclipped plan of [0, frames) with every utterance at its own origin (OriginWindow).
 
 struct Rows {
   int lo, hi;
@@ -545,13 +543,14 @@ struct View {
 };
 
 // What a walk issues: the batch's mel view and lengths, the waveform, and five buffers, each B * width floats (window_plan).
-// org: NULL (one window for the whole batch), or the per-utterance origin mode (fs2_vocoder_forward_streams): the walk is then the
-// unclipped plan of [0, frames), its rows are window rows, utterance b's window starts at its frame org[b] (origin_rows), and the mel
-// is the staged window buffer.
+// org: NULL (the offline forward), or the windowed mode: the walk is then the unclipped plan of [0, frames), its rows are window rows,
+// utterance b's window starts at its frame org[b] (origin_rows), and the mel is the staged window buffer.  pre_tc: conv_pre's
+// tensor-core weights, or NULL where the caller's mel layout keeps conv_pre on the fp32 kernel.
 struct WinExec {
   int B; cudaStream_t s;
   const float* mel; int64_t mel_bs, mel_rs;
   const int32_t* lens; const int32_t* org;
+  const float* pre_tc;
   float* wav; int64_t wav_bs;
   float *bx, *bu, *bt, *r1, *r2;
 };
@@ -577,12 +576,12 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     if (stage_fused(m, i) && !stage_tcv(m, i)) return FS2_ERR_ARG;
   }
   auto cap = [&](int scale) { return T < 0 ? -1LL : (long long)T * scale; };
-  // the kernels' logical length at `scale` rows per frame; the origin mode bounds every utterance by itself (origin_rows)
+  // the kernels' logical length at `scale` rows per frame, and a launch's window: the windowed mode bounds every utterance by itself
+  // (origin_rows); the offline forward passes no window, so it runs the offline entry points
   const int* org = ex ? ex->org : nullptr;
   auto len = [&](int scale) { return org ? ORIGIN_CAP : T * scale; };
-  // the whole batch [0, T) runs the offline entry points (the window ones compute the same bits; conv_post has one kernel)
-  const bool whole = !org && T >= 0 && f0 == 0 && f1 == T;
-  auto win = [&](const RowWindow& w) -> const RowWindow* { return whole ? nullptr : &w; };
+  OriginWindow ow{};
+  auto win = [&](const RowWindow& w) -> const OriginWindow* { ow = OriginWindow{w, org}; return org ? &ow : nullptr; };
   // ---- backward: O[i + 1] = the rows stage i's output must hold (O[0]: conv_pre's), U[i] = its ResBlocks' input, Q[i] = the
   // ConvTranspose's phase-group rows
   Rows O[FS2_MAX_STAGES + 1], U[FS2_MAX_STAGES], Q[FS2_MAX_STAGES];
@@ -617,9 +616,9 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   View bx{ex ? ex->bx : nullptr, O[0].lo, O[0].n(), C};
   if (ex) {
     fs2_conv1d_args c = win_conv_args(ex->mel, ex->mel_bs, ex->mel_rs, B, len(1), m->n_mel, bx, C, 7);
-    c.w = m->w_pre; c.w_tc = m->w_pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
+    c.w = m->w_pre; c.w_tc = ex->pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
     c.x_lens = lens; c.lens_scale = 1;
-    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi}), org));
+    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi})));
   }
   const float inv_nk = 1.f / (float)m->n_kernels;
   for (int i = 0; i < n; i++) {
@@ -643,7 +642,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       c.bias = m->b_up[i] + off;
       c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
       c.x_lens = lens; c.lens_scale = s0;
-      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi}), org));
+      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi})));
     }
     C = Co;
     const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
@@ -695,7 +694,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
             a.alpha = alpha; a.accumulate = accumulate;
           }
           a.x = r.p; a.y = dst.p;
-          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}), r.lo, org, C == 128));
+          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}), r.lo, C == 128));
         }
       } else {
         const int j = run.j, d = run.d0, rb = i * m->n_kernels + j, k = m->rb_k[j];
@@ -710,13 +709,13 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
           c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
           c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
           c.x_lens = lens; c.lens_scale = s1;
-          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi}), org));
+          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi})));
           c = win_conv_args(t.at(), t.bs(), C, B, len(s1), C, dst, C, k);
           c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
           c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
           c.alpha = alpha; c.accumulate = accumulate;
           c.x_lens = lens; c.lens_scale = s1;
-          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi}), org));
+          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi})));
         }
       }
       r = dst;
@@ -725,13 +724,11 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   }
   add(FS2_VW_CONV_POST, -1, -1, -1, sc[n], post, O[n], last, -1, 2.0 * post.n() * C * 7);
   if (!ex) return FS2_OK;
-  // conv_post takes its window in every mode (a NULL one would ignore the batch strides); the whole batch's is {0, T * up, T * up}
   fs2_conv_post_args p{};
   p.x = bx.at(); p.B = B; p.T = len(sc[n]); p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
   p.wav = ex->wav - post.lo;                           // sample f0 * up is the caller's wav[0]
   p.lens = lens; p.lens_scale = sc[n];
-  const RowWindow w{post.lo, post.hi, O[n].hi};
-  return conv_post(&p, s, &w, bx.bs(), ex->wav_bs, org);
+  return conv_post(&p, s, win({post.lo, post.hi, O[n].hi}), bx.bs(), ex->wav_bs);   // offline: the strides are its defaults
 }
 
 // The plan of [0, frames) clipped at T (T < 0: unclipped, the bound of every window of `frames` frames), and the floats per utterance
@@ -756,44 +753,35 @@ static int vocoder_forward_impl(const fs2_vocoder_model* m, const fs2_vocoder_ar
   size_t width = 0;
   FS2_TRY(window_plan(m, a->T, a->T, L, width));
   const size_t nf = (size_t)a->B * width;
-  WinExec ex{a->B, s, a->mel, a->mel_batch_stride, a->mel_row_stride, a->mel_lens, nullptr, a->wav, a->T * frame_rows(m, m->n_stages),
-             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
+  WinExec ex{a->B, s, a->mel, a->mel_batch_stride, a->mel_row_stride, a->mel_lens, nullptr, m->w_pre_tc, a->wav,
+             a->T * frame_rows(m, m->n_stages), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
   if (ar.dry) return FS2_OK;
   if (!ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
   L.clear();
   return window_walk(m, a->T, 0, a->T, L, &ex);
 }
 
-static int vocoder_window_impl(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, int frames, cudaStream_t s, Arena& ar) {
+// fs2_vocoder_forward_window and _streams: the unclipped plan of [0, frames) once for the whole batch, each stream at its own origin.
+// The mel cone (conv_pre's input rows [x0, x1) of that plan) is staged first, [B][x1 - x0][n_mel], with the streams' origins and
+// lengths, so that conv_pre reads one batch-strided buffer and every launch the same two tables whichever call passed them.
+static int vocoder_windowed_impl(const fs2_vocoder_model* m, const MelSource& src, int B, int frames, float* wav, int64_t wav_bs,
+                                 const float* pre_tc, cudaStream_t s, Arena& ar) {
   std::vector<fs2_vocoder_window_launch_t> L;
   size_t width = 0;
   FS2_TRY(window_plan(m, -1, frames, L, width));
-  const size_t nf = (size_t)a->B * width;
-  WinExec ex{a->B, s, a->mel, a->mel_batch_stride, a->mel_row_stride, a->mel_lens, nullptr, a->wav, a->wav_batch_stride,
-             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
-  if (ar.dry) return FS2_OK;
-  if (!ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
-  L.clear();
-  return window_walk(m, a->T, a->f0, a->f1 < a->T ? a->f1 : a->T, L, &ex);
-}
-
-// fs2_vocoder_forward_streams: the unclipped plan of [0, frames) once for the whole batch, each stream at its own origin.  The mel cone
-// (conv_pre's input rows [x0, x1) of that plan) is staged first, [B][x1 - x0][n_mel], so that conv_pre reads one batch-strided buffer.
-static int vocoder_streams_impl(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, cudaStream_t s, Arena& ar) {
-  std::vector<fs2_vocoder_window_launch_t> L;
-  size_t width = 0;
-  FS2_TRY(window_plan(m, -1, a->frames, L, width));
   const int x0 = L[0].x0, rows = L[0].x1 - L[0].x0;     // launch 0 is conv_pre
-  const size_t nf = (size_t)a->B * width;
-  float* mel = ar.f32((size_t)a->B * rows * m->n_mel);
-  WinExec ex{a->B, s, nullptr, (int64_t)rows * m->n_mel, m->n_mel, a->mel_lens, a->f0, a->wav, a->wav_batch_stride,
+  const size_t nf = (size_t)B * width;
+  float* mel = ar.f32((size_t)B * rows * m->n_mel);
+  int32_t* org = (int32_t*)ar.take((size_t)B * sizeof(int32_t));
+  int32_t* lens = (int32_t*)ar.take((size_t)B * sizeof(int32_t));
+  WinExec ex{B, s, nullptr, (int64_t)rows * m->n_mel, m->n_mel, lens, org, pre_tc, wav, wav_bs,
              ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
   if (ar.dry) return FS2_OK;
-  if (!mel || !ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
-  FS2_TRY(stage_mel(a->mel, a->mel_lens, a->f0, a->B, x0, rows, m->n_mel, mel, s));
+  if (!mel || !org || !lens || !ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
+  FS2_TRY(stage_mel(src, B, x0, rows, m->n_mel, mel, org, lens, s));
   ex.mel = mel - (ptrdiff_t)x0 * m->n_mel;             // window row 0 of stream 0 (the conv reads rows [x0, x1) only)
   L.clear();
-  return window_walk(m, -1, 0, a->frames, L, &ex);
+  return window_walk(m, -1, 0, frames, L, &ex);
 }
 
 }  // namespace fs2
@@ -970,13 +958,15 @@ static_assert(sizeof(fs2_vocoder_window_launch_t) == 56, "fs2_vocoder_window_lau
 // Row counts of a window must fit the kernels' int rows with the halo: frames (and T) times prod(rates) below 2^30
 static bool window_rows_ok(const fs2_vocoder_model* m, long long frames) { return frames * frame_rows(m, m->n_stages) < (1LL << 30); }
 
-size_t fs2_vocoder_window_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
+size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
   if (!vocoder_ok(m) || B <= 0 || frames <= 0 || !window_rows_ok(m, frames)) return 0;
   Arena ar(nullptr, 0);
-  fs2_vocoder_window_args a{};
-  a.B = B;
-  if (vocoder_window_impl(m, &a, frames, nullptr, ar) != FS2_OK) return 0;
+  if (vocoder_windowed_impl(m, MelSource{}, B, frames, nullptr, 0, nullptr, nullptr, ar) != FS2_OK) return 0;
   return ar.off + 256;
+}
+
+size_t fs2_vocoder_window_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
+  return fs2_vocoder_streams_workspace_bytes(m, B, frames);
 }
 
 int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_window_args* a, fs2_stream_t st) {
@@ -984,28 +974,26 @@ int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_win
   if (a->f0 < 0 || a->f1 <= a->f0 || a->f0 >= a->T || !window_rows_ok(m, a->T)) return FS2_ERR_ARG;
   const int frames = (a->f1 < a->T ? a->f1 : a->T) - a->f0;
   if (a->B > 1 && a->wav_batch_stride < frames * frame_rows(m, m->n_stages)) return FS2_ERR_ARG;
+  // every stream starts at f0 and has clamp(mel_lens[b], 0, T) frames (T without mel_lens): the kernels read no row at or past T
+  const MelSource src{nullptr, a->mel, a->mel_batch_stride, a->mel_row_stride, nullptr, a->f0, a->mel_lens, a->T};
+  // conv_pre runs on the backend the caller's mel layout selects, as fs2_vocoder_forward's does on the same mel
+  fs2_conv1d_args pre = conv_args(a->mel, a->B, a->T, m->n_mel, m->c0, 7, nullptr);
+  pre.x_batch_stride = a->mel_batch_stride; pre.x_row_stride = a->mel_row_stride;
   Arena ar(a->workspace, a->workspace_bytes);
-  return vocoder_window_impl(m, a, frames, S(st), ar);
+  return vocoder_windowed_impl(m, src, a->B, frames, a->wav, a->wav_batch_stride, conv_tc_supported(&pre) ? m->w_pre_tc : nullptr, S(st),
+                               ar);
 }
 
 static_assert(sizeof(fs2_vocoder_streams_args) == 64, "fs2_vocoder_streams_args: two int32, five pointers, an int64 and a size_t");
-
-size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, int frames) {
-  if (!vocoder_ok(m) || B <= 0 || frames <= 0 || !window_rows_ok(m, frames)) return 0;
-  Arena ar(nullptr, 0);
-  fs2_vocoder_streams_args a{};
-  a.B = B; a.frames = frames;
-  if (vocoder_streams_impl(m, &a, nullptr, ar) != FS2_OK) return 0;
-  return ar.off + 256;
-}
 
 int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t st) {
   if (!vocoder_ok(m) || !a || a->B <= 0 || a->frames <= 0 || !window_rows_ok(m, a->frames)) return FS2_ERR_ARG;
   if (!a->mel || !a->mel_lens || !a->f0 || !a->wav || !a->workspace) return FS2_ERR_ARG;
   if (a->B > 1 && a->wav_batch_stride < a->frames * frame_rows(m, m->n_stages)) return FS2_ERR_ARG;
   if (a->workspace_bytes < fs2_vocoder_streams_workspace_bytes(m, a->B, a->frames)) return FS2_ERR_ARG;
+  const MelSource src{a->mel, nullptr, 0, 0, a->f0, 0, a->mel_lens, INT32_MAX};
   Arena ar(a->workspace, a->workspace_bytes);
-  return vocoder_streams_impl(m, a, S(st), ar);
+  return vocoder_windowed_impl(m, src, a->B, a->frames, a->wav, a->wav_batch_stride, m->w_pre_tc, S(st), ar);
 }
 
 static_assert(sizeof(fs2_resblock_run_t) == 32, "fs2_resblock_run_t: six int32 and a double");

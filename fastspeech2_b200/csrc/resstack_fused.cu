@@ -54,9 +54,9 @@ struct RsP {
   int TPS;                       // conv taps per weight stage (one bulk copy / one handshake)
   int accumulate;                // the first kernel size reduce-adds into y too
   const int* lens; int lens_scale;   // ragged batch (fs2_resstack_args::lens) or NULL
-  int x0;                            // windowed mode: logical row of the x map's row 0 (the y map's row 0 is win.y0)
+  int x0;                            // windowed mode: window row of the x map's row 0 (the y map's row 0 is win.y0)
   RowWindow win;                     // windowed mode: rows computed (win.xend is not read: the x map ends the input)
-  const int* org;                    // per-utterance origins (the streams entry points only), see origin_rows
+  const int* org;                    // the windowed mode's per-utterance origins, see origin_rows
 };
 
 // ------------------------------------------------------------------ TMA (tensor-map) wrappers
@@ -108,12 +108,12 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
 // weights are then the 16 x 16 zero-padded tiles, and channels CG..C-1 are held at exact zero in both slabs).  Global rows of 128 bytes
 // or more travel as [128 rows][32 channels] boxes with the 128-byte swizzle; narrower rows (CG = 16: 64 B, CG = 8: 32 B) as one
 // unswizzled [rows][CG] box per 128 rows.  RAG: ragged batch (RsP::lens != NULL), see WorkList.
-// WIN (with RAG): windowed mode, see WindowList.  The tensor maps span the window buffers: the x map's row 0 is logical row p.x0, the
-// y map's is p.win.y0.  Its zero fill beyond the x window only reaches slab rows whose results are never stored (the host sizes the x
-// window to the stored rows' receptive field), and the y map clips the stores to the window.
-// ORG (with WIN): per-utterance origin mode, see origin_rows.  The zero fill covers only the buffer edges, so the slab rows of x below
-// lo_b are zeroed like those at or past n_b, and every conv's rows outside [lo_b, hi_b) are held at zero as outside [0, n_b).
-template <int CG, int C, int MT, bool RAG, bool WIN = false, bool ORG = false>
+// WIN (with RAG): windowed mode with per-utterance origins, see WindowList and origin_rows.  The tensor maps span the window buffers:
+// the x map's row 0 is window row p.x0, the y map's is p.win.y0.  Its zero fill beyond the x window only reaches slab rows whose
+// results are never stored (the host sizes the x window to the stored rows' receptive field), and the y map clips the stores to the
+// window.  The zero fill covers only the buffer edges, so the slab rows of x below lo_b are zeroed like those at or past hi_b, and every
+// conv's rows outside [lo_b, hi_b) are held at zero as outside [0, n_b) offline.
+template <int CG, int C, int MT, bool RAG, bool WIN = false>
 __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUtensorMap& tmy, const RsP& p) {
   constexpr int KB = C / 16, R = MT * 128, NJ = C / 8;                // NJ: 8-column fragment groups of a row
   constexpr int BOXC = CG < 32 ? CG : 32, NH = CG / BOXC;             // channels per TMA box, boxes across a row
@@ -148,8 +148,8 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
   }
   fence_proxy_async();
   __syncthreads();
-  std::conditional_t<WIN, WindowList<ORG>, WorkList<RAG>> work;   // TILE-row tiles of each utterance
-  if constexpr (WIN) work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, 1, p.win.y0, p.win.yend, p.N, p.org);
+  std::conditional_t<WIN, WindowList, WorkList<RAG>> work;   // TILE-row tiles of each utterance
+  if constexpr (WIN) work.init(p.lens, p.org, p.lens_scale, p.B, p.TILE, 1, p.win.y0, p.win.yend, p.N);
   else work.init(p.lens, p.lens_scale, p.N, p.B, p.TILE, p.tiles_per_b, p.n_items);
   const int xorg = WIN ? p.x0 : 0, yorg = WIN ? p.win.y0 : 0;   // map row 0
 
@@ -189,8 +189,8 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
   for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
     const Item it = work.item(item);
     const int b = it.b, t0 = it.t0, nrows = it.rows;   // nrows: rows of utterance b (n_b of a ragged batch); the convs pad at its end
-    int lo = 0;                                        // and at its first row: 0, or lo_b in the origin mode
-    if constexpr (ORG) lo = work.lo_of(b);
+    int lo = 0;                                        // and at its first row: 0, or lo_b in the windowed mode
+    if constexpr (WIN) lo = work.lo_of(b);
     for (int j = 0; j < p.n_kernels; j++) {
       // ---- input: TMA boxes of x -> XT (idle: the last conv that read it has retired), then residual stream -> registers, lrelu(x) -> XA
       if (io) {
@@ -212,7 +212,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
             const int c = cbase + 8 * jj;
             if (8 * jj >= CG) { rs_store2(xa, CHUNK, row, c, 0.f, 0.f); continue; }   // zero-padded channels
             float2 u = *reinterpret_cast<const float2*>(xt + (size_t)((c / BOXC) * MT + m) * XBOX + rs_box_off<SW, BOXC>(r128, c));
-            if (RAG && (t0 - p.H + row >= nrows || (ORG && t0 - p.H + row < lo))) u = make_float2(0.f, 0.f);   // the padding of a ragged batch reads as zero
+            if (RAG && (t0 - p.H + row >= nrows || (WIN && t0 - p.H + row < lo))) u = make_float2(0.f, 0.f);   // the padding of a ragged batch reads as zero
             xr(i, 4 * jj + 2 * h) = u.x;
             xr(i, 4 * jj + 2 * h + 1) = u.y;
             rs_store2(xa, CHUNK, row, c, rs_lrelu(u.x), rs_lrelu(u.y));   // rows outside the utterance arrive as zeros (TMA fill)
@@ -364,28 +364,17 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_kernel(const __
   resstack_body<CG, 16, 8, RAG>(tmx, tmy, p);
 }
 
-// Windowed mode: entry points of their own, so that the padded and ragged instantiations keep their code (lens may be NULL here)
-template <int C, int MT>
-__global__ void __launch_bounds__(RS_THREADS, 1) resstack_window_kernel(const __grid_constant__ CUtensorMap tmx,
-                                                                        const __grid_constant__ CUtensorMap tmy, const RsP p) {
-  resstack_body<C, C, MT, true, true>(tmx, tmy, p);
-}
-template <int CG>
-__global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_window_kernel(const __grid_constant__ CUtensorMap tmx,
-                                                                               const __grid_constant__ CUtensorMap tmy, const RsP p) {
-  resstack_body<CG, 16, 8, true, true>(tmx, tmy, p);
-}
-
-// Per-utterance origin mode (fs2_vocoder_forward_streams): entry points of their own as well (p.org and the lens are not NULL here)
+// Windowed mode (fs2_vocoder_forward_window and _streams): entry points of their own, so that the padded and ragged instantiations
+// keep their code (p.org and the lens are not NULL here)
 template <int C, int MT>
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_streams_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                          const __grid_constant__ CUtensorMap tmy, const RsP p) {
-  resstack_body<C, C, MT, true, true, true>(tmx, tmy, p);
+  resstack_body<C, C, MT, true, true>(tmx, tmy, p);
 }
 template <int CG>
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_narrow_streams_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                                 const __grid_constant__ CUtensorMap tmy, const RsP p) {
-  resstack_body<CG, 16, 8, true, true, true>(tmx, tmy, p);
+  resstack_body<CG, 16, 8, true, true>(tmx, tmy, p);
 }
 
 // The 128-channel stage's pairs (fs2_vocoder_model::pair_mask bit 8 + i): the same body at MT = 1 (MT * C = 128), with entry points
@@ -395,13 +384,9 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_kernel(const __gr
                                                                       const RsP p) {
   resstack_body<128, 128, 1, RAG>(tmx, tmy, p);
 }
-__global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_window_kernel(const __grid_constant__ CUtensorMap tmx,
-                                                                             const __grid_constant__ CUtensorMap tmy, const RsP p) {
-  resstack_body<128, 128, 1, true, true>(tmx, tmy, p);
-}
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_streams_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                               const __grid_constant__ CUtensorMap tmy, const RsP p) {
-  resstack_body<128, 128, 1, true, true, true>(tmx, tmy, p);
+  resstack_body<128, 128, 1, true, true>(tmx, tmy, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -481,16 +466,15 @@ static int make_map(CUtensorMap* tm, const float* base, int B, int N, int C, int
   return r == CUDA_SUCCESS ? FS2_OK : FS2_ERR_CUDA - 1;
 }
 
-// win: NULL, or the windowed mode: a->x and a->y are then the window buffers [B][x1 - x0][C] and [B][yend - y0][C] (not biased), x0 /
-// x1 the logical rows a->x holds (win->xend is x1), and a->N the full logical length.  org (with win and a->lens): NULL, or the
-// per-utterance origins of the origin mode (origin_rows; rows are then window rows and a->N is not used).
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, int x0, const int* org, bool wide) {
+// win (with a->lens): NULL, or the windowed mode (OriginWindow; a->N is not used): a->x and a->y are then the window buffers
+// [B][x1 - x0][C] and [B][yend - y0][C] (not biased), x0 / x1 the window rows a->x holds (win->rows.xend is x1).
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win, int x0, bool wide) {
   if (!a || !a->x || !a->y) return FS2_ERR_ARG;
   if (!aligned16(a->x) || !aligned16(a->y)) return FS2_ERR_ARG;
   if (a->B <= 0 || a->N <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (org && (!win || !a->lens)) return FS2_ERR_ARG;
-  const int xrows = win ? win->xend - x0 : a->N, yrows = win ? win->yend - win->y0 : a->N;   // rows of the x and y buffers
+  if (win && !a->lens) return FS2_ERR_ARG;
+  const int xrows = win ? win->rows.xend - x0 : a->N, yrows = win ? win->rows.yend - win->rows.y0 : a->N;   // rows of the x and y buffers
   if (xrows <= 0 || yrows <= 0) return FS2_ERR_ARG;
   {  // not in place: a work item re-reads halo rows of x that its neighbours' results would already have overwritten
     const unsigned char *xb = reinterpret_cast<const unsigned char*>(a->x), *yb = reinterpret_cast<const unsigned char*>(a->y);
@@ -514,17 +498,12 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_window_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_window_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_window_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_window_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_streams_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_streams_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_streams_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_narrow_streams_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     return e;
   }));
@@ -543,24 +522,18 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const RowWindow* win, i
   p.H = plan.H; p.TILE = plan.TILE; p.tiles_per_b = plan.n_items / a->B; p.n_items = plan.n_items; p.SB = plan.SB; p.OBOX = plan.OBOX; p.n_oboxes = plan.n_oboxes; p.TPS = plan.TPS;
   p.alpha = a->alpha > 0.f ? a->alpha : 1.f / (float)a->n_kernels; p.accumulate = a->accumulate;
   p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
-  p.x0 = x0; p.win = win ? *win : RowWindow{0, a->N, a->N};
-  p.org = org;
+  p.x0 = x0; p.win = win ? win->rows : RowWindow{0, a->N, a->N};
+  p.org = win ? win->org : nullptr;
   alignas(64) CUtensorMap tmx, tmy;
   FS2_TRY(make_map(&tmx, a->x, a->B, xrows, a->C, 128));
   FS2_TRY(make_map(&tmy, a->y, a->B, yrows, a->C, p.OBOX));
   prof_before(s);
-  if (org) {
+  if (win) {
     if (a->C == 32) resstack_streams_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 64) resstack_streams_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 128) resstack_wide_streams_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 16) resstack_narrow_streams_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_narrow_streams_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
-  } else if (win) {
-    if (a->C == 32) resstack_window_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
-    else if (a->C == 64) resstack_window_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
-    else if (a->C == 128) resstack_wide_window_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
-    else if (a->C == 16) resstack_narrow_window_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
-    else resstack_narrow_window_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
   } else if (a->C == 32) {
     if (a->lens) resstack_kernel<32, 4, true><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else resstack_kernel<32, 4, false><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);

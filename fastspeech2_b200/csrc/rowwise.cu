@@ -366,9 +366,9 @@ int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s) {
 // 256 + taps - 1 activated rows in shared memory with fully coalesced float4 loads (row stride C+1 floats -> conflict-free
 // column walks), then each thread reduces its own output sample from shared memory.
 constexpr int CP_ROWS = 256;
-// Batch strides of x and wav and the rows computed and read: {T * C, T} and {0, T, T} outside the windowed mode (RowWindow; a.T is then
-// the full logical length, and x / wav are biased by the windows' first rows).
-// org: NULL, or the per-utterance origins of the origin mode (origin_rows): rows and samples outside [lo_b, hi_b) read and write zero.
+// Batch strides of x and wav and the rows computed and read: {T * C, T} and {0, T, T} outside the windowed mode (RowWindow; x / wav
+// are then biased by the windows' first rows).
+// org: NULL, or the windowed mode's per-utterance origins (origin_rows): rows and samples outside [lo_b, hi_b) read and write zero.
 struct PostRows { long long xbs, wbs; RowWindow win; const int* org; };
 template <bool ORG>
 __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
@@ -422,7 +422,7 @@ __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int t
 __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
   conv_post_body<false>(a, tiles_per_batch, pr);
 }
-// Per-utterance origin mode (fs2_vocoder_forward_streams): entry points of their own, so that the other modes keep their code
+// Windowed mode (fs2_vocoder_forward_window and _streams): entry points of their own, so that the offline ones keep their code
 __global__ void __launch_bounds__(CP_ROWS) conv_post_streams_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
   conv_post_body<true>(a, tiles_per_batch, pr);
 }
@@ -435,7 +435,7 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_streams_kernel(const fs2_co
 // B = 16 x 259k samples; this one is bound by the single read of x.)
 constexpr int CPF_BLOCKS = 18;                         // row blocks of TAPS rows per 8-lane group
 // RAG: ragged batch (a.lens != NULL); a template parameter so that the padded path keeps its code and registers.  ORG (with RAG): the
-// per-utterance origin mode.
+// windowed mode's per-utterance origins.
 template <int TAPS, bool RAG, bool ORG>
 __device__ __forceinline__ void conv_post_c32_body(const fs2_conv_post_args a, int groups_per_batch, long long n_groups, const PostRows pr) {
   constexpr int PAD = (TAPS - 1) / 2, ROWS = CPF_BLOCKS * TAPS - 2 * PAD;     // output rows per group (120 for 7 taps: a multiple of 8)
@@ -515,14 +515,14 @@ __global__ void __launch_bounds__(256) conv_post_c32_streams_kernel(const fs2_co
   conv_post_c32_body<TAPS, true, true>(a, groups_per_batch, n_groups, pr);
 }
 
-// win: NULL, or the windowed mode (a->T is then the full logical length, a->x and a->wav are biased by the windows' first rows and
-// their batch strides are x_bs and wav_bs).  Both kernels add every output's taps in the same order wherever its tile starts.
-// org (with win and a->lens): NULL, or the per-utterance origins of the origin mode (origin_rows; a->T is not used).
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win, long long x_bs, long long wav_bs, const int* org) {
+// win (with a->lens): NULL, or the windowed mode (OriginWindow; a->T is not used, a->x and a->wav are biased by the windows' first rows
+// and their batch strides are x_bs and wav_bs).  Both kernels add every output's taps in the same order wherever its tile starts.
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win, long long x_bs, long long wav_bs) {
   if (!a || !a->x || !a->w || !a->bias || !a->wav || a->B <= 0 || a->T <= 0 || a->C <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (org && (!win || !a->lens)) return FS2_ERR_ARG;
-  const PostRows pr = win ? PostRows{x_bs, wav_bs, *win, org} : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr};
+  if (win && !a->lens) return FS2_ERR_ARG;
+  const PostRows pr = win ? PostRows{x_bs, wav_bs, win->rows, win->org}
+                          : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr};
   const int rows = pr.win.yend - pr.win.y0;
   if (rows <= 0) return FS2_ERR_ARG;
   if (a->C == 32 && a->taps == 7 && (reinterpret_cast<uintptr_t>(a->x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15u) == 0) {
@@ -531,7 +531,7 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win,
     const long long n_groups = (long long)gpb * a->B, blocks = (n_groups * 8 + 255) / 256;
     if (blocks > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
     prof_before(s);
-    if (org) conv_post_c32_streams_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    if (win) conv_post_c32_streams_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     prof_after(s, 3, 2.0 * (double)a->B * rows * a->taps * a->C);
@@ -544,39 +544,45 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const RowWindow* win,
   const long long n = (long long)a->B * rows;
   if ((long long)tiles * a->B > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   prof_before(s);
-  if (org) conv_post_streams_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
+  if (win) conv_post_streams_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   else conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   prof_after(s, 3, 2.0 * n * a->taps * a->C);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
-// ------------------------------------------------------------------ mel staging of fs2_vocoder_forward_streams
-// out[b][r] = stream b's mel row org[b] + x0 + r for r < rows, zeros where that row lies outside [0, max(lens[b], 0)): the one kernel
-// that reads the per-stream pointer table, so the window kernels after it see one batch-strided buffer.  n_mel % 4 == 0 and 16-byte
-// aligned rows (float4 loads); rows outside the utterance are never dereferenced.
-__global__ void stage_mel_kernel(const float* const* mel, const int* lens, const int* org, int x0, int rows, int n4, float4* out,
-                                 long long total) {
+// ------------------------------------------------------------------ mel staging of the windowed vocoder
+// out[b][r] = stream b's mel row o_b + x0 + r for r < rows, zeros where that row lies outside [0, n_b), with o_b and n_b the origin and
+// length of MelSource; org[b] = o_b and lens[b] = n_b.  The one kernel that reads the caller's mel and lengths, so the window kernels
+// after it see one batch-strided buffer and two tables.  n_mel % 4 == 0 and 16-byte aligned rows (float4 loads); rows outside the
+// utterance are never dereferenced.
+__global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, int n4, float4* out, int* org, int* lens, long long total) {
+  auto origin = [&](int b) { return src.f0s ? __ldg(src.f0s + b) : src.f0; };
+  auto length = [&](int b) { return src.lens ? min(max(__ldg(src.lens + b), 0), src.cap) : src.cap; };
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long br = i / n4;
     const int c4 = (int)(i - br * n4);
     const int b = (int)(br / rows), r = (int)(br - (long long)b * rows);
-    const long long t = (long long)__ldg(org + b) + x0 + r;
+    const long long t = (long long)origin(b) + x0 + r;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t >= 0 && t < __ldg(lens + b)) v = __ldg(reinterpret_cast<const float4*>(mel[b]) + t * n4 + c4);
+    if (t >= 0 && t < length(b)) {
+      const float* row = src.table ? src.table[b] + t * n4 * 4 : src.mel + b * src.bs + t * src.rs;
+      v = __ldg(reinterpret_cast<const float4*>(row) + c4);
+    }
     out[i] = v;
+    if (i < B) { org[i] = origin((int)i); lens[i] = length((int)i); }
   }
 }
 
-int stage_mel(const float* const* mel, const int32_t* lens, const int32_t* org, int B, int x0, int rows, int n_mel, float* out,
-              cudaStream_t s) {
-  if (!mel || !lens || !org || !out || B <= 0 || rows <= 0 || n_mel <= 0) return FS2_ERR_ARG;
-  if (n_mel % 4 || !aligned16(out)) return FS2_ERR_UNSUPPORTED;
+int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, cudaStream_t s) {
+  if (!(src.table || src.mel) || !out || !org || !lens || B <= 0 || rows <= 0 || n_mel <= 0) return FS2_ERR_ARG;
+  if (n_mel % 4 || !aligned16(out) || (!src.table && ((src.bs | src.rs) & 3))) return FS2_ERR_UNSUPPORTED;
+  if (!src.table && !aligned16(src.mel)) return FS2_ERR_ARG;
   const long long total = (long long)B * rows * (n_mel / 4);
   const long long blocks = (total + 255) / 256;
   prof_before(s);
-  stage_mel_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(mel, lens, org, x0, rows, n_mel / 4,
-                                                                             reinterpret_cast<float4*>(out), total);
+  stage_mel_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(src, B, x0, rows, n_mel / 4, reinterpret_cast<float4*>(out),
+                                                                             org, lens, total);
   prof_after(s, 3, 0.0);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

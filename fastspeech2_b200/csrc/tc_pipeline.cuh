@@ -198,47 +198,13 @@ struct WorkList<true, MIN_ROWS> {
   }
 };
 
-// Windowed mode (fs2_vocoder_forward_window): only the logical rows [y0, yend) of each utterance are computed, in `tile`-row tiles
-// that start at y0, and only where they hold a row < n_b.  n_b = ragged_rows(lens, scale, cap, b), or cap when lens is NULL (every
-// utterance cap rows long).  An item's t0 is its tile's first logical row and its `rows` is min(n_b, lim), lim >= yend: the bound of the
-// rows the kernel stores (conv_tc), or cap (resstack, whose tensor maps bound its loads and stores); rows_of(b, end) gives another.
-// The cursor is the ragged one's.
-// WindowList<true>: the per-utterance origin mode (origin_rows; fs2_vocoder_forward_streams).  Utterance b's rows are [lo_b, hi_b) of
-// the window buffers instead of [0, n_b): `rows` is min(hi_b, lim), lo_of(b) gives lo_b, and cap is not used.  Only the tiles that
-// overlap [max(y0, lo_b), min(yend, hi_b)) are items; the tile grid still starts at y0, so every utterance's tiles cover the same
-// window rows and every role walks the same monotone item sequence.
-template <bool ORG = false>
+// Windowed mode, per-utterance origins (origin_rows; fs2_vocoder_forward_window and _streams): only the window rows [y0, yend) are
+// computed, in `tile`-row tiles that start at y0.  Utterance b's rows are [lo_b, hi_b) of the window buffers; only the tiles that
+// overlap [max(y0, lo_b), min(yend, hi_b)) are items, and the tile grid still starts at y0, so every utterance's tiles cover the same
+// window rows and every role walks the same monotone item sequence.  An item's t0 is its tile's first window row and its `rows` is
+// min(hi_b, lim), lim >= yend: the bound of the rows the kernel stores (conv_tc), or the layer's length (resstack, whose tensor maps
+// bound its loads and stores); rows_of(b, end) gives another, lo_of(b) gives lo_b.  The cursor is the ragged one's.
 struct WindowList {
-  const int* lens; int scale, cap, tile, y0, yend, lim;
-  int count, live;
-  int nblk, b, before, rows;       // cursor; rows = min(n_b, lim)
-  __device__ __forceinline__ int rows_of(int u, int end) const { return min(lens ? ragged_rows(lens, scale, cap, u) : cap, end); }
-  __device__ __forceinline__ int rows_of(int u) const { return rows_of(u, lim); }
-  __device__ __forceinline__ int tiles_of(int r) const { return max(0, min(r, yend) - y0 + tile - 1) / tile; }
-  __device__ __forceinline__ void init(const int* lens_, int scale_, int cap_, int B, int tile_, int blocks, int y0_, int yend_, int lim_,
-                                       const int* = nullptr) {
-    lens = lens_; scale = scale_; cap = cap_; tile = tile_; y0 = y0_; yend = yend_; lim = lim_;
-    live = 0;
-    for (int u = 0; u < B; u++) live += tiles_of(rows_of(u));
-    count = live * blocks;
-    nblk = 0; b = 0; before = 0; rows = rows_of(0);
-  }
-  __device__ __forceinline__ int lo_of(int) const { return 0; }
-  __device__ __forceinline__ Item item(int i) {   // i < count, and not below the previous call's i
-    const int blk = i / live, rem = i - blk * live;
-    if (blk != nblk) { nblk = blk; b = 0; before = 0; rows = rows_of(0); }
-    for (int nt = tiles_of(rows); rem >= before + nt; nt = tiles_of(rows)) {
-      before += nt;
-      rows = rows_of(++b);
-    }
-    Item it;
-    it.nblk = blk; it.b = b; it.t0 = y0 + (rem - before) * tile; it.rows = rows;
-    return it;
-  }
-};
-
-template <>
-struct WindowList<true> {
   const int* lens; const int* org; int scale, tile, y0, yend, lim;
   int count, live;
   int nblk, b, before, rows, first;   // cursor; rows = min(hi_b, lim), first = utterance b's first live tile
@@ -247,8 +213,8 @@ struct WindowList<true> {
   __device__ __forceinline__ int lo_of(int u) const { return origin_rows(lens, org, scale, u).lo; }
   __device__ __forceinline__ int first_of(int u) const { return max(0, lo_of(u) - y0) / tile; }
   __device__ __forceinline__ int tiles_of(int r, int f) const { return max(0, max(0, min(r, yend) - y0 + tile - 1) / tile - f); }
-  __device__ __forceinline__ void init(const int* lens_, int scale_, int, int B, int tile_, int blocks, int y0_, int yend_, int lim_,
-                                       const int* org_) {
+  __device__ __forceinline__ void init(const int* lens_, const int* org_, int scale_, int B, int tile_, int blocks, int y0_, int yend_,
+                                       int lim_) {
     lens = lens_; org = org_; scale = scale_; tile = tile_; y0 = y0_; yend = yend_; lim = lim_;
     live = 0;
     for (int u = 0; u < B; u++) live += tiles_of(rows_of(u), first_of(u));

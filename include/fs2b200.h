@@ -453,9 +453,14 @@ int fs2_vocoder_forward(const fs2_vocoder_model* m, const fs2_vocoder_args* a, f
  *   - stateless: a window depends only on mel, mel_lens, [f0, f1) and the weights; windows may be computed in any order, or twice;
  *   - every layer computes only the rows later layers need (fs2_vocoder_window_plan): a window reads the mel frames
  *     [f0 - halo, f1 + halo) of [0, mel_lens[b]) and nothing else, every intermediate likewise;
- *   - the workspace, fs2_vocoder_window_workspace_bytes(m, B, f1 - f0) or that of any wider window, does not depend on T.
+ *   - the workspace, fs2_vocoder_window_workspace_bytes(m, B, f1 - f0) or that of any wider window, does not depend on T:
+ *     fs2_vocoder_window_workspace_bytes(m, B, frames) equals fs2_vocoder_streams_workspace_bytes(m, B, frames);
+ *   - it issues the launches of a fs2_vocoder_forward_streams call of frames = min(f1, T) - f0 in which every stream starts at f0
+ *     and has clamp(mel_lens[b], 0, T) frames (T without mel_lens): one launch stages the mel cone, then the unclipped plan of
+ *     [0, frames).  Strides that are not multiples of 4 floats are FS2_ERR_UNSUPPORTED, a mel that is not 16-byte aligned FS2_ERR_ARG.
  * Every layer pads at the utterance's ends, not at the window's, and keeps the offline call's kernel choice and arithmetic per
- * output row (f8_mask, fused_mask, pair_mask, pair_kmax and the *_tc pointers apply unchanged). */
+ * output row (f8_mask, fused_mask, pair_mask, pair_kmax and the *_tc pointers apply unchanged; conv_pre runs on the backend the
+ * caller's mel layout selects in fs2_vocoder_forward). */
 typedef struct fs2_vocoder_window_args {
   int B, T;
   const float* mel; int64_t mel_batch_stride, mel_row_stride; /* channels-last view [B][T][n_mel], as in fs2_vocoder_args */
@@ -503,11 +508,11 @@ int fs2_vocoder_window_plan(const fs2_vocoder_model* m, int T, int f0, int f1, f
  *     0 <= r + f0[b] * scale < n_b * scale;
  *   - any device values are memory-safe: stream b's mel is read only at rows of [0, n_b) inside its window's cone; f0[b] >= n_b or
  *     n_b <= 0 gives an all-zero chunk, and rows before a negative f0[b] read as zero;
- *   - one launch stages every stream's mel cone into the workspace ([B][cone rows][n_mel]); the rest are the launches of one
- *     fs2_vocoder_forward_window of `frames` frames;
+ *   - one launch stages every stream's mel cone ([B][cone rows][n_mel]), f0 and mel_lens into the workspace; the rest are the
+ *     launches of the unclipped plan of [0, frames);
  *   - B <= 0, frames <= 0, a NULL pointer, wav_batch_stride < frames * up with B > 1, or a workspace below
  *     fs2_vocoder_streams_workspace_bytes(m, B, frames) is FS2_ERR_ARG before any CUDA call.  That bound depends on B and frames only:
- *     the window's, plus the staged mel cone. */
+ *     the plan's five buffers, the staged mel cone and two [B] int32 tables. */
 typedef struct fs2_vocoder_streams_args {
   int B, frames;                  /* B streams, `frames` mel frames each */
   const float* const* mel;        /* [B] device array: stream b's mel rows, n_mel contiguous floats per row, 16-byte aligned */

@@ -5,9 +5,11 @@ weights; every comparison must match bit for bit.
   1. host logic (no GPU needed): fs2_{encode,decode,vocoder}_workspace_bytes for the LJSpeech and LibriTTS model shapes; for V1, V2
      and tests/test_stream_vocoder_cpu.py's other generator under each of its policies, the vocoder's launch plans
      (fs2_vocoder_window_plan, record for record; the plan of [0, T) is fs2_vocoder_forward's launches), its ResBlock runs and its
-     offline, window and streams workspace sizes.
+     offline and streams workspace sizes.  The new library stages the streams' origins and lengths into two [B] int32 tables of the
+     streams workspace, and its window workspace equals its streams workspace.
   2. whole forwards: every output of FastSpeech2 and Generator (forward, stream, stream_pool) under several tensor-core / vocoder
-     policies, the kernel launch count and the per-class launches of fs2_profile_begin / fs2_profile_end.
+     policies, the kernel launch count and the per-class launches of fs2_profile_begin / fs2_profile_end.  The new library's window
+     call issues one staging launch (class 3) more than the old one's: stream() is expected to launch one more kernel per chunk.
   3. the tensor-core conv: ragged cases and every epilogue mode, then per-layer timing.
 
 usage: python scripts/ab_lib.py [old.so]
@@ -116,11 +118,13 @@ for cfg, shape in CONFIGS.items():
         assert got["new"] == got["old"], ("resblock runs", cfg, policy)
         for B in (1, 3, 16):
             for n in (1, 7, 64, 127, 1011):
-                got = host(lambda lib: [f(C.byref(vm), B, n) for f in (lib.fs2_vocoder_workspace_bytes, lib.fs2_vocoder_window_workspace_bytes,
-                                                                      lib.fs2_vocoder_streams_workspace_bytes)])
-                assert got["new"] == got["old"] and min(got["new"]) > 0, ("vocoder workspaces", cfg, policy, B, n, got)
+                got = host(lambda lib: [f(C.byref(vm), B, n) for f in (lib.fs2_vocoder_workspace_bytes, lib.fs2_vocoder_streams_workspace_bytes,
+                                                                      lib.fs2_vocoder_window_workspace_bytes)])
+                tables = 2 * ((4 * B + 255) // 256 * 256)
+                assert got["new"][:2] == [got["old"][0], got["old"][1] + tables] and min(got["new"]) > 0, ("vocoder workspaces", cfg, policy, B, n, got)
+                assert got["new"][2] == got["new"][1], ("window workspace == streams workspace", cfg, policy, B, n, got)
                 n_ws += 3
-print(f"vocoder host logic: new == old for {n_plans} window plans, the ResBlock runs and {n_ws} workspace queries", flush=True)
+print(f"vocoder host logic: new == old for {n_plans} window plans and the ResBlock runs; {n_ws} workspace queries as expected", flush=True)
 if not torch.cuda.is_available():
     print("no GPU: skipping the forward and conv sections")
     sys.exit(0)
@@ -138,8 +142,9 @@ def same(a, b):
     return a == b
 
 
-def ab(label, fn):
-    """Run fn() once on each library (through the package binding) and assert identical outputs and launches."""
+def ab(label, fn, extra=0):
+    """Run fn() once on each library (through the package binding) and assert identical outputs, and identical launches but for
+    `extra` more class-3 launches in the new library."""
     got = {}
     for name in ("old", "new"):
         lib = libs[name]
@@ -156,8 +161,8 @@ def ab(label, fn):
         got[name] = (out, n, list(launches))
     (o_old, n_old, c_old), (o_new, n_new, c_new) = got["old"], got["new"]
     assert len(o_old) == len(o_new) and all(same(a, b) for a, b in zip(o_old, o_new)), f"{label}: outputs differ"
-    assert n_old == n_new, f"{label}: launch count {n_old} (old) vs {n_new} (new)"
-    assert c_old == c_new, f"{label}: per-class launches {c_old} (old) vs {c_new} (new)"
+    assert n_old + extra == n_new, f"{label}: launch count {n_old} (old) vs {n_new} (new), expected {extra} more"
+    assert [c + (extra if k == 3 else 0) for k, c in enumerate(c_old)] == c_new, f"{label}: per-class launches {c_old} (old) vs {c_new} (new)"
     print(f"{label:58s} identical, {n_new} launches, per class {c_new}", flush=True)
 
 
@@ -258,7 +263,8 @@ ab("Generator V2, padded", lambda: gen(mel_c))
 ab("Generator V2, ragged", lambda: gen(mel_c, mel_lens=ml))
 del gen
 gen = generator(configs.HIFIGAN_CONFIG, 0)
-ab("Generator stream(chunk_frames=64), ragged", lambda: torch.cat([w for _, w in gen.stream(mel_c, mel_lens=ml, chunk_frames=64)], -1))
+ab("Generator stream(chunk_frames=64), ragged", lambda: torch.cat([w for _, w in gen.stream(mel_c, mel_lens=ml, chunk_frames=64)], -1),
+   extra=-(-mel_c.shape[2] // 64))                    # the staging launch of every window
 ab("Generator stream_pool(chunk_frames=32), 3 streams", lambda: pool_run(gen))
 del gen
 L._lib = None

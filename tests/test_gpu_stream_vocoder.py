@@ -113,16 +113,23 @@ def _window_call(gen, mel_cl, lens_d, f0, f1, out, out_bs, ws):
     L.check(L.lib().fs2_vocoder_forward_window(ctypes.byref(m), ctypes.byref(a), torch.cuda.current_stream().cuda_stream), "window")
 
 
-@pytest.mark.parametrize("ragged", [False, True])
+@pytest.mark.parametrize("ragged", [False, True, "clamped"])
 @pytest.mark.parametrize("cfg", ["v1", "v2"])
 def test_windows_in_reverse_order_into_the_full_waveform(cfg, ragged):
     """Stateless windows, written straight into a preallocated waveform at sample f0 * up (wav_batch_stride = T * up), last first
-    and the first one twice."""
+    and the first one twice.  clamped: device lengths outside [0, T], read as clamped to it, and mel rows 84 floats apart (forward
+    runs conv_pre on the fp32 kernel for that layout, and so must the window)."""
     gen = _generator(configs.HIFIGAN_CONFIG if cfg == "v1" else configs.HIFIGAN_V2_CONFIG)
     m, _keep, _dev, up = gen._pack()
     mel = _postnet_view(len(LENS), T, seed=24)
     lens_d = torch.tensor(LENS, dtype=torch.int32, device=DEV) if ragged else None
     want = gen(mel, lens_d)
+    if ragged == "clamped":
+        wide = torch.full((len(LENS), T, 84), NAN, device=DEV)
+        wide[:, :, :80] = mel.transpose(1, 2)
+        mel = wide[:, :, :80].transpose(1, 2)
+        lens_d = torch.tensor((T + 7, -3, 40), dtype=torch.int32, device=DEV)
+        want = gen(mel, torch.tensor((T, 0, 40)))
     mel_cl = mel.transpose(1, 2)
     chunk = 13
     ws = torch.empty(L.lib().fs2_vocoder_window_workspace_bytes(ctypes.byref(m), len(LENS), chunk), dtype=torch.uint8, device=DEV)

@@ -28,19 +28,26 @@ def _cone(m, frames):
 
 
 @pytest.mark.parametrize("cfg", list(CONFIGS))
-def test_workspace_is_the_window_bound_plus_the_staged_cone(cfg):
-    """The bound depends on B and frames only, is the window's plus the staged [B][x1 - x0][80] mel cone, and grows linearly in B."""
+def test_workspace_is_the_plan_buffers_plus_the_staged_cone_and_tables(cfg):
+    """The bound depends on B and frames only, equals the window call's, is the plan's five buffers plus the staged [B][x1 - x0][80]
+    mel cone and the [B] origin and length tables, and grows linearly in B."""
     h = L.lib()
     m, _up = _model(CONFIGS[cfg])
+    align = lambda n: (n + 255) // 256 * 256           # the workspace arena's alignment of every buffer
     for frames in (1, 7, 32, 64):
         x0, x1 = _cone(m, frames)
         assert x0 < 0 < frames < x1
+        width = 0                                      # floats per utterance of each buffer: the widest output of the unclipped plan
+        for l in L.vocoder_window_plan(m, 1 << 20, 1000, 1000 + frames)[:-1]:
+            ch = m.c0 if l.layer == L.VW_CONV_PRE else (m.c0 >> (l.stage + 1)) * (
+                m.rates[l.stage] if l.layer in (L.VW_UP_A, L.VW_UP_B) else 1)
+            width = max(width, (l.y1 - l.y0) * ch)
         sizes = []
         for B in (1, 2, 3, 16):
             s = h.fs2_vocoder_streams_workspace_bytes(ctypes.byref(m), B, frames)
             w = h.fs2_vocoder_window_workspace_bytes(ctypes.byref(m), B, frames)
             cone = B * (x1 - x0) * 80 * 4
-            assert s >= w and s - w == (cone + 255) // 256 * 256, (frames, B)
+            assert s == w == 5 * align(4 * B * width) + align(cone) + 2 * align(4 * B) + 256, (frames, B)
             sizes.append(s)
         # linear in B (up to the arena's 256-byte alignment of each of the six buffers)
         per_b = sizes[1] - sizes[0]

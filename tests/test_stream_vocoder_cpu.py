@@ -203,9 +203,10 @@ def test_receptive_field_against_the_oracle(cfg, T):
             assert reads[f].x0 <= j < reads[f].x1, (j, f, reads[f].x0, reads[f].x1)
 
 
-# The windowed modes' own entry points (conv_tc_window_kernel, resstack_window_kernel, resstack_narrow_window_kernel) get the checks
-# tests/test_sass_pipeline.py makes of the padded and ragged ones: pipelined wgmma groups, and no spills in the conv kernel.
-WINDOW_KERNELS = {"conv_tc_window_kernel": 8, "resstack_window_kernel": 2, "resstack_narrow_window_kernel": 2}
+# The windowed mode's own entry points (conv_tc_streams_kernel, resstack_streams_kernel, resstack_narrow_streams_kernel), which the
+# window and streams calls run, get the checks tests/test_sass_pipeline.py makes of the padded and ragged ones: pipelined wgmma groups,
+# and no spills in the conv kernel.
+WINDOW_KERNELS = {"conv_tc_streams_kernel": 8, "resstack_streams_kernel": 2, "resstack_narrow_streams_kernel": 2}
 
 
 @pytest.fixture(scope="module")
@@ -236,7 +237,7 @@ def window_sass():
     return {k: "\n".join(v) for k, v in funcs.items()}, usage
 
 
-def test_window_kernels_are_pipelined_and_the_conv_does_not_spill(window_sass):
+def test_windowed_entry_points_are_pipelined_and_the_conv_does_not_spill(window_sass):
     import re
     sass, usage = window_sass
     for kernel, n in WINDOW_KERNELS.items():
@@ -246,5 +247,5 @@ def test_window_kernels_are_pipelined_and_the_conv_does_not_spill(window_sass):
             mmas = len(re.findall(r"\b[HQ]GMMA\.", sass[f]))
             full_waits = len(re.findall(r"WARPGROUP\.DEPBAR\.LE gsb0, 0x0\b", sass[f]))
             assert mmas > 0 and full_waits * 4 <= mmas, (f, mmas, full_waits)
-            if kernel == "conv_tc_window_kernel":
+            if kernel == "conv_tc_streams_kernel":
                 assert usage[f]["STACK"] == 0 and usage[f]["LOCAL"] == 0, (f, usage[f])

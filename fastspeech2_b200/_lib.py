@@ -225,6 +225,31 @@ RESAMPLE_ARGS_SIZE, RESAMPLE_WINDOW_ARGS_SIZE, RESAMPLE_STREAM_SIZE, RESAMPLE_ST
 assert C.sizeof(ResampleArgs) == RESAMPLE_ARGS_SIZE and C.sizeof(ResampleWindowArgs) == RESAMPLE_WINDOW_ARGS_SIZE
 assert C.sizeof(ResampleStream) == RESAMPLE_STREAM_SIZE and C.sizeof(ResampleStreamsArgs) == RESAMPLE_STREAMS_ARGS_SIZE
 
+RESAMPLE_MAX_FILTERS = 8
+RESAMPLE_F32, RESAMPLE_PCM16, RESAMPLE_ULAW, RESAMPLE_ALAW = 0, 1, 2, 3
+
+
+class ResampleFilter(C.Structure):
+    """fs2_resample_filter_t: one filter of fs2_resample_streams_mixed's table (24 bytes, pinned in resample.cu)."""
+    _fields_ = [("up", i32), ("down", i32), ("K", i32), ("taps", fp)]
+
+
+class ResampleMixedStream(C.Structure):
+    """fs2_resample_mixed_stream_t: one stream's record of fs2_resample_streams_mixed, in device memory (80 bytes, pinned in
+    resample.cu)."""
+    _fields_ = ResampleStream._fields_ + [("filter", i32), ("encoding", i32), ("y_offset", i64)]
+
+
+class ResampleMixedArgs(C.Structure):
+    """fs2_resample_mixed_args: B streams, each with its own filter and encoding, in one launch (232 bytes, pinned in resample.cu)."""
+    _fields_ = [("B", i32), ("n_filters", i32), ("filters", ResampleFilter * RESAMPLE_MAX_FILTERS), ("table", fp), ("max_out", i64),
+                ("y", fp), ("scale", f32)]
+
+
+RESAMPLE_FILTER_SIZE, RESAMPLE_MIXED_STREAM_SIZE, RESAMPLE_MIXED_ARGS_SIZE = 24, 80, 232
+assert C.sizeof(ResampleFilter) == RESAMPLE_FILTER_SIZE and C.sizeof(ResampleMixedStream) == RESAMPLE_MIXED_STREAM_SIZE
+assert C.sizeof(ResampleMixedArgs) == RESAMPLE_MIXED_ARGS_SIZE
+
 
 class ConvTcPlan(C.Structure):
     _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")]
@@ -291,6 +316,7 @@ EXPORTS = {
     "fs2_resample": (i32, [C.POINTER(ResampleArgs), fp]),
     "fs2_resample_window": (i32, [C.POINTER(ResampleWindowArgs), fp]),
     "fs2_resample_streams": (i32, [C.POINTER(ResampleStreamsArgs), fp]),
+    "fs2_resample_streams_mixed": (i32, [C.POINTER(ResampleMixedArgs), fp]),
 }
 
 _lib = None

@@ -109,6 +109,28 @@ __device__ __forceinline__ short pcm16_sample(float v, float scale) {
   return (short)min(max(__float2int_rz(v * scale), -32768), 32767);
 }
 
+// ITU-T G.711 codes of an int16 PCM sample (fs2_resample_streams_mixed), as audioop.lin2ulaw / lin2alaw compute them on 16-bit input.
+// mu-law: the 14-bit magnitude of s >> 2 (arithmetic), clipped to 8159 and biased by 33, lies in [32, 8192]; its segment is the position
+// of its leading bit less 5 (8192, past segment 7, is the largest code), the mantissa the next four bits; every bit is inverted, the
+// sign bit set for s >= 0.
+__device__ __forceinline__ unsigned char ulaw_byte(short s) {
+  const int v = s >> 2;
+  const int mag = min(v < 0 ? -v : v, 8159) + 33;
+  const int seg = 26 - __clz(mag);
+  const int u = seg > 7 ? 0x7F : (seg << 4) | ((mag >> (seg + 1)) & 0xF);
+  return (unsigned char)(u ^ (v < 0 ? 0x7F : 0xFF));
+}
+
+// A-law: the 13-bit s >> 3 (arithmetic), magnitude -v - 1 when negative, in [0, 4095]; segment = position of its leading bit less 4,
+// at least 0; mantissa = four bits below it (bits 1..4 in segments 0 and 1); even bits inverted (xor 0x55), sign bit set for v >= 0.
+__device__ __forceinline__ unsigned char alaw_byte(short s) {
+  const int v = s >> 3;
+  const int mag = v < 0 ? -v - 1 : v;
+  const int seg = max(27 - __clz(mag), 0);
+  const int a = (seg << 4) | ((mag >> (seg < 2 ? 1 : seg)) & 0xF);
+  return (unsigned char)(a ^ (v < 0 ? 0x55 : 0xD5));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -14,7 +14,7 @@ import torch.nn as nn
 from .. import _lib as L
 from .. import ops, packing
 from .._modtree import get, populate
-from ..resample import Resampler
+from ..resample import ENCODINGS, Resampler
 from ..spec import hifigan_spec
 
 LRELU_SLOPE = 0.1
@@ -323,10 +323,12 @@ class Generator(nn.Module):
         shares the pool.  It uses the weights packed at creation, like stream(); the workspace depends on the live count and
         chunk_frames, not on any length.
 
-        sample_rate (optional): step() returns each stream's chunk at this rate, converted by one fs2_resample_streams launch after the
-        vocoder's call; a stream keeps its chunk count, each chunk holding the outputs whose support has arrived (the last flushes the
-        rest), and concatenated they equal Resampler(h.sampling_rate, sample_rate)(self(mel[None])) bit for bit.  pcm16: int16 chunks
-        (x 32768, truncated, clamped).  ValueError when chunk_frames * hop is below the resampler's history."""
+        sample_rate (optional): step() returns each stream's chunk at this rate, converted after the vocoder's call; a stream keeps its
+        chunk count, each chunk holding the outputs whose support has arrived (the last flushes the rest), and concatenated they equal
+        Resampler(h.sampling_rate, sample_rate)(self(mel[None])) bit for bit.  pcm16: int16 chunks (x 32768, truncated, clamped).
+        ValueError when chunk_frames * hop is below the resampler's history.  These are the defaults of StreamPool.add, which can give
+        each stream its own rate and encoding ("f32", "pcm16", "ulaw", "alaw"); every stream that is not at h.sampling_rate in fp32 is
+        converted by one fs2_resample_streams_mixed launch per step, whatever its format."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
         rs = self._resampler(sample_rate, chunk_frames)
@@ -360,23 +362,12 @@ class Generator(nn.Module):
                         "fs2_vocoder_forward_streams")
             return wav
 
-        resample = None
-        if rs is not None:
-            def resample(records, max_out):
-                with torch.cuda.device(dev):
-                    if max_out == 0:                   # no stream has a new output: no launch
-                        return torch.empty(len(records), 0, dtype=torch.int16 if pcm16 else torch.float32, device=dev)
-                    return rs.streams(records, max_out, dev, pcm16=pcm16)
-            resample.rs = rs
-        elif pcm16:                                    # the generator's own rate: the int16 conversion of each step's waveform
-            vocode = launch
-
-            def launch(ptrs, f0s, ns):
-                wav = vocode(ptrs, f0s, ns)
-                with torch.cuda.device(dev):
-                    return ops.wav_to_int16(wav)
-
-        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev, resample=resample)
+        def resample(records, max_out):
+            with torch.cuda.device(dev):
+                return Resampler.mixed(records, max_out, dev)[1]
+        fs = _cfg(self.h, "sampling_rate")
+        resample.rs = rs or Resampler(fs, fs)
+        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev, resample=resample, encoding="pcm16" if pcm16 else "f32")
         pool._keep = keep                              # the packed weights stay alive while the pool runs
         return pool
 
@@ -386,20 +377,55 @@ class StreamPool:
     each starts at frame 0 in the step after its add() and leaves after its last chunk.  `launch(ptrs, f0s, ns)` computes one step: the
     [B, chunk_frames * up] waveform of the live streams, stream b from its frame f0s[b] of the ns[b] frames at device address ptrs[b].
 
-    resample (optional): `resample(records, max_out)` converts one step's waveform to another rate in one call, its `.rs` the
-    resample.Resampler whose emission rule decides each stream's outputs: records[b] = (x0, x1, i0, i1, i2, n, j0, j1) gives stream b's
-    previous chunk (address x0, input samples [i0, i1)) and current chunk (x1, [i1, i2)) of its n samples, and the outputs [j0, j1) it
-    emits; the call returns a [B, >= max(j1 - j0)] tensor (max 0 included) whose row b starts with them."""
+    resample (optional): `resample(records, max_out)` converts one step's waveform, in one call, for every live stream whose format is
+    not the waveform's own rate in fp32 (those take their slice of the waveform): records[b] = (x0, x1, i0, i1, i2, n, j0, j1,
+    resampler, encoding) gives stream b's previous chunk (address x0, input samples [i0, i1)) and current chunk (x1, [i1, i2)) of its n
+    samples, the outputs [j0, j1) it emits, its resample.Resampler (the identity at the waveform's rate) and its L.RESAMPLE_* encoding;
+    the call returns rows indexable by b (a [B, >= max(j1 - j0)] tensor, or a list of tensors), row b starting with stream b's outputs.
+    Its `.rs`, a Resampler from the waveform's rate, and `encoding` ("f32", "pcm16", "ulaw" or "alaw") are the defaults of add(); a
+    pool without `resample` only vocodes."""
 
-    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None):
+    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None, encoding="f32"):
         self._launch, self.n_mel, self.up, self.chunk_frames, self.device = launch, n_mel, up, chunk_frames, torch.device(device)
         self._resample = resample
-        self._live = []                                # [handle, channels-last mel view [n, n_mel], n, next frame, last chunk, emitted]
+        rs = getattr(resample, "rs", None)
+        self._rates = {} if rs is None else {rs.fs_out: rs}   # output rate -> its Resampler, one per rate
+        self._default = (rs, self._encoding(encoding))
+        # [handle, channels-last mel view [n, n_mel], n, next frame, last chunk, emitted, Resampler or None, encoding]
+        self._live = []
         self._next = 0
 
-    def add(self, mel):
+    def _encoding(self, name):
+        if name not in ENCODINGS:
+            raise ValueError(f"encoding must be one of {sorted(ENCODINGS)}, got {name!r}")
+        if ENCODINGS[name] != L.RESAMPLE_F32 and self._resample is None:
+            raise ValueError(f"this pool has no conversion call for encoding {name!r}")
+        return ENCODINGS[name]
+
+    def _resampler(self, sample_rate):
+        """The Resampler of an output rate (None: the pool's default), checked against the pool's limits."""
+        if sample_rate is None:
+            return self._default[0]
+        default = self._default[0]
+        if default is None:
+            raise ValueError("this pool has no conversion call: it cannot change a stream's rate")
+        rs = Resampler(default.fs_in, sample_rate)
+        rs = self._rates.setdefault(rs.fs_out, rs)
+        if self.chunk_frames * self.up < rs.history:
+            raise ValueError(f"chunk_frames * {self.up} samples must cover the resampler's history of {rs.history} samples")
+        return rs
+
+    @staticmethod
+    def _native(s):
+        """The stream takes its slice of the waveform: its rate is the waveform's and its encoding fp32."""
+        return (s[6] is None or s[6].identity) and s[7] == L.RESAMPLE_F32
+
+    def add(self, mel, sample_rate=None, encoding=None):
         """Admits a stream.  mel: [n_mel, n] or [1, n_mel, n] on the pool's device, n >= 1.  A channels-last view with row stride n_mel
-        (FastSpeech2's postnet_mel[b, :n].T is one) is kept without a copy; any other layout is converted once.  Returns the handle."""
+        (FastSpeech2's postnet_mel[b, :n].T is one) is kept without a copy; any other layout is converted once.  sample_rate and encoding
+        ("f32", "pcm16", "ulaw" or "alaw"): the stream's output format, None for the pool's.  ValueError for a rate Resampler refuses, a
+        resampler history longer than chunk_frames * up, an unknown encoding, or a ninth distinct output rate among the live streams.
+        Returns the handle."""
         if not isinstance(mel, torch.Tensor):
             raise ValueError("mel must be a tensor")
         if mel.dim() == 3 and mel.shape[0] == 1:
@@ -411,12 +437,17 @@ class StreamPool:
         n = mel.shape[1]
         if n < 1:
             raise ValueError("mel has no frames")
+        rs = self._resampler(sample_rate)
+        enc = self._default[1] if encoding is None else self._encoding(encoding)
+        rates = {s[6].fs_out for s in self._live if s[6] is not None}
+        if rs is not None and rs.fs_out not in rates and len(rates) >= L.RESAMPLE_MAX_FILTERS:
+            raise ValueError(f"the live streams already use {len(rates)} output rates; at most {L.RESAMPLE_MAX_FILTERS}")
         rows = mel.T
         if not (rows.dtype == torch.float32 and rows.stride(1) == 1 and (n == 1 or rows.stride(0) == self.n_mel) and rows.data_ptr() % 16 == 0):
             rows = rows.to(torch.float32).contiguous()
         h = self._next
         self._next += 1
-        self._live.append([h, rows, n, 0, None, 0])
+        self._live.append([h, rows, n, 0, None, 0, rs, enc])
         return h
 
     def cancel(self, h):
@@ -431,39 +462,51 @@ class StreamPool:
         return len(self._live)
 
     def step(self):
-        """One chunk of every live stream, in one launch call: a list of (handle, first_sample, wav [1, 1, m]) in admission order,
+        """One chunk of every live stream, in one launch call: a list of (handle, first_sample, chunk [1, 1, m]) in admission order,
         m = chunk_frames * up except on a stream's last chunk, which is trimmed to its end.  [] without a call when the pool is empty.
-        With a resampler: first_sample and m at the new rate, the chunk holding the outputs that became ready (possibly none)."""
+        A converted stream: first_sample and m at its own rate, the chunk holding the outputs that became ready (possibly none), of its
+        encoding's dtype; at most one conversion call per step, none when every live stream is at the waveform's rate in fp32."""
         if not self._live:
             return []
         live = self._live
         wav = self._launch([s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live])
-        if self._resample is not None:
-            wav, starts, widths = self._resampled(live, wav)
-        else:
-            starts = [s[3] * self.up for s in live]
-            widths = [min(self.chunk_frames, s[2] - s[3]) * self.up for s in live]
+        rows = [(wav, i) for i in range(len(live))]     # where each stream's chunk is: (rows, index)
+        starts = [s[3] * self.up for s in live]
+        widths = [min(self.chunk_frames, s[2] - s[3]) * self.up for s in live]
+        conv = [i for i, s in enumerate(live) if not self._native(s)]
+        if conv:
+            y = self._converted(live, conv, wav, starts, widths)
+            for k, i in enumerate(conv):
+                rows[i] = (y, k)
         out, keep = [], []
         for i, s in enumerate(live):
-            out.append((s[0], starts[i], wav[i:i + 1, :widths[i]].unsqueeze(0)))
+            t, k = rows[i]
+            out.append((s[0], starts[i], t[k][None, None, :widths[i]]))
             s[3] += self.chunk_frames
             if s[3] < s[2]:
                 keep.append(s)
         self._live = keep
         return out
 
-    def _resampled(self, live, wav):
-        """The resampler's call on this step's waveform: (its output, each stream's first output, each stream's output count)."""
-        rs, n1 = self._resample.rs, self.chunk_frames * self.up
-        records, starts, widths = [], [], []
-        for i, s in enumerate(live):
-            _, _, n, f0, prev, emitted = s
+    def _converted(self, live, conv, wav, starts, widths):
+        """The conversion call for streams `conv` on this step's waveform; sets their first output and output count in starts and
+        widths."""
+        n1 = self.chunk_frames * self.up
+        records = []
+        for i in conv:
+            s = live[i]
+            _, _, n, f0, prev, emitted, rs, enc = s
             i1, N = f0 * self.up, n * self.up
             r = rs.ready(min(i1 + n1, N), N, f0 + self.chunk_frames >= n)
             cur = wav[i]
             records.append((0 if prev is None else prev.data_ptr(), cur.data_ptr(), i1 - (0 if prev is None else n1), i1, i1 + n1, N,
-                            emitted, r))
-            starts.append(emitted)
-            widths.append(r - emitted)
-            s[4], s[5] = cur, r                        # the chunk stays alive as the next step's history
-        return self._resample(records, max(widths)), starts, widths
+                            emitted, r, rs, enc))
+            starts[i], widths[i] = emitted, r - emitted
+            s[5] = r
+        y = self._resample(records, max(widths[i] for i in conv))
+        # Each chunk stays alive as the next step's history.  The previous chunks are released only now: the call is enqueued, so a
+        # later allocation that reuses their memory is written after the call has read them (released before, the call's own table
+        # upload or output could take that memory first).
+        for i in conv:
+            live[i][4] = wav[i]
+        return y

@@ -3,6 +3,10 @@ window and zero padding, computed by the polyphase FIR kernel behind fs2_resampl
 (include/fs2b200.h states the formula and the order of the fp32 sums).  The taps are designed here in fp64 with numpy, as
 scipy.signal.firwin designs them, so the runtime needs no scipy.
 
+Mixed streams (Resampler.mixed, fs2_resample_streams_mixed): streams at different rates and encodings -- fp32, int16 PCM, or the
+ITU-T G.711 mu-law / A-law byte of that PCM -- in one launch; a stream at the input rate that wants PCM or G.711 runs the identity
+filter.  Generator.stream_pool converts every stream of a step this way.
+
 Streaming: after m input samples of a stream have arrived, output j is ready iff floor((j * down + half_len) / up) < m, or the stream
 has ended (Resampler.ready).  Generator.stream and Generator.stream_pool emit exactly the ready outputs on each chunk; an output's
 arithmetic never depends on where a chunk boundary falls, so the concatenated chunks equal the offline call bit for bit.
@@ -17,6 +21,11 @@ import numpy as np
 import torch
 
 from . import _lib as L
+
+# output encodings of the mixed call, by name; a stream's chunk has the dtype of its encoding
+ENCODINGS = {"f32": L.RESAMPLE_F32, "pcm16": L.RESAMPLE_PCM16, "ulaw": L.RESAMPLE_ULAW, "alaw": L.RESAMPLE_ALAW}
+DTYPES = {L.RESAMPLE_F32: torch.float32, L.RESAMPLE_PCM16: torch.int16, L.RESAMPLE_ULAW: torch.uint8, L.RESAMPLE_ALAW: torch.uint8}
+_UNIT_TAP = np.ones((1, 1), dtype=np.float32)       # the identity filter: up = down = K = 1
 
 
 def _rate(v, name):
@@ -81,14 +90,15 @@ class Resampler:
         return min(self.n_out(n), max(0, -(-(m * self.up - self.half_len) // self.down)))
 
     def device_taps(self, device):
+        """The [up][K] taps on `device` (the identity: the one-tap table of 1.0 that the mixed call runs), uploaded once."""
         device = torch.device(device)
         t = self._dev_taps.get(device)
         if t is None:
-            t = self._dev_taps[device] = torch.from_numpy(self.taps).to(device)
+            t = self._dev_taps[device] = torch.from_numpy(_UNIT_TAP if self.identity else self.taps).to(device)
         return t
 
     def _filter(self, device):
-        return dict(up=self.up, down=self.down, K=self.K, taps=self.device_taps(device).data_ptr())
+        return dict(up=self.up, down=self.down, K=1 if self.identity else self.K, taps=self.device_taps(device).data_ptr())
 
     @torch.no_grad()
     def __call__(self, wav, lengths=None, pcm16=False, scale=32768.0):
@@ -161,3 +171,56 @@ class Resampler:
                                   pcm16=int(bool(pcm16)), scale=float(scale), **self._filter(dev))
         L.check(L.lib().fs2_resample_streams(C.byref(a), torch.cuda.current_stream(dev).cuda_stream), "fs2_resample_streams")
         return y
+
+    @staticmethod
+    def mixed_table(records, max_out):
+        """The host side of Resampler.mixed, without device work: (filters, table, offsets, nbytes).  filters: the distinct ratios'
+        Resamplers in order of first use (at most 8, else ValueError); table: int64 [B, 10], row b the fs2_resample_mixed_stream_t of
+        stream b (its filter index and encoding packed as two int32 in column 8); offsets: stream b's byte offset in the output, each a
+        multiple of 16, the streams back to back; nbytes: the output's size."""
+        filters, index = [], {}
+        table = np.zeros((len(records), 10), dtype=np.int64)
+        offsets, off = [], 0
+        for b, rec in enumerate(records):
+            rs, enc = rec[8], rec[9]
+            if enc not in DTYPES:
+                raise ValueError(f"unknown encoding {enc!r}")
+            k = index.get((rs.up, rs.down))
+            if k is None:
+                k = index[(rs.up, rs.down)] = len(filters)
+                filters.append(rs)
+            table[b, :8] = rec[:8]
+            table[b, 8] = k | (enc << 32)
+            table[b, 9] = off
+            offsets.append(off)
+            width = min(max(rec[7] - rec[6], 0), max_out) * DTYPES[enc].itemsize
+            off += -(-width // 16) * 16
+        if len(filters) > L.RESAMPLE_MAX_FILTERS:
+            raise ValueError(f"{len(filters)} filters in one call; at most {L.RESAMPLE_MAX_FILTERS}")
+        return filters, table, offsets, off
+
+    @staticmethod
+    def mixed(records, max_out, device, scale=32768.0):
+        """One fs2_resample_streams_mixed launch on the current stream: records[b] = (x0, x1, i0, i1, i2, n, j0, j1, resampler,
+        encoding) -- the fields of Resampler.streams' records, then stream b's Resampler (the identity included) and its encoding (an
+        L.RESAMPLE_* code).  The records are uploaded from a fresh pinned block with one non_blocking copy (no host sync).  Returns
+        (y, views): one uint8 buffer holding every stream's outputs, and stream b's min(j1 - j0, max_out) outputs as a view of it
+        typed by its encoding (fp32, int16 or uint8).  max_out == 0: no launch, empty views."""
+        dev = torch.device(device)
+        filters, table, offsets, nbytes = Resampler.mixed_table(records, max_out)
+        y = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+        views = []
+        for rec, off in zip(records, offsets):
+            dt = DTYPES[rec[9]]
+            views.append(y[off:off + min(max(rec[7] - rec[6], 0), max_out) * dt.itemsize].view(dt))
+        if max_out > 0 and records:
+            host = torch.empty(table.size, dtype=torch.int64, pin_memory=True)
+            host.numpy()[:] = table.reshape(-1)
+            dtable = host.to(dev, non_blocking=True)
+            a = L.ResampleMixedArgs(B=len(records), n_filters=len(filters), table=dtable.data_ptr(), max_out=max_out, y=y.data_ptr(),
+                                    scale=float(scale))
+            for i, rs in enumerate(filters):
+                a.filters[i] = L.ResampleFilter(**rs._filter(dev))
+            L.check(L.lib().fs2_resample_streams_mixed(C.byref(a), torch.cuda.current_stream(dev).cuda_stream),
+                    "fs2_resample_streams_mixed")
+        return y, views

@@ -591,6 +591,41 @@ typedef struct fs2_resample_streams_args {
 } fs2_resample_streams_args;
 int fs2_resample_streams(const fs2_resample_streams_args* a, fs2_stream_t stream);
 
+/* Mixed streams: as fs2_resample_streams, but each stream names its own filter in a table of n_filters (1..FS2_RESAMPLE_MAX_FILTERS)
+ * filters passed by value, and its own output encoding, so that streams at different rates and sample types share one launch.
+ * Encodings: FS2_RESAMPLE_F32 writes fp32; FS2_RESAMPLE_PCM16 int16 as pcm16 above; FS2_RESAMPLE_ULAW / FS2_RESAMPLE_ALAW one byte,
+ * the ITU-T G.711 mu-law / A-law code of that int16 sample (equal to Python's audioop.lin2ulaw / lin2alaw on 16-bit input).
+ * A filter is a ratio with its taps as above, or the identity: up == down == 1, K == 1 and taps a one-tap table of 1.0f, whose output
+ * j is input j (with PCM16, fs2_wav_to_int16's bits; with F32, x + 0.0f, so -0.0f becomes +0.0f).  The identity is accepted here only.
+ * Stream b writes outputs [j0, j1) (j1 - j0 clamped to [0, max_out]) to the bytes at y + y_offset, elements of its encoding.  The host
+ * never reads the table; a record whose filter is outside [0, n_filters), whose encoding is unknown, or whose y_offset is negative or
+ * not a multiple of 16 writes nothing.  The host refuses before any CUDA call (FS2_ERR_ARG) a bad B, n_filters, ratio, K or taps, a
+ * NULL table, max_out < 1, and a y that is NULL or not 16-byte aligned.  Dynamic shared memory is the largest of the filters' needs. */
+#define FS2_RESAMPLE_MAX_FILTERS 8
+#define FS2_RESAMPLE_F32 0
+#define FS2_RESAMPLE_PCM16 1
+#define FS2_RESAMPLE_ULAW 2
+#define FS2_RESAMPLE_ALAW 3
+typedef struct fs2_resample_filter_t {
+  int32_t up, down, K;
+  const float* taps;                    /* [up][K] device */
+} fs2_resample_filter_t;
+typedef struct fs2_resample_mixed_stream_t {
+  const float *x0, *x1;
+  int64_t i0, i1, i2, n, j0, j1;        /* as fs2_resample_stream_t */
+  int32_t filter, encoding;
+  int64_t y_offset;                     /* bytes from y */
+} fs2_resample_mixed_stream_t;
+typedef struct fs2_resample_mixed_args {
+  int B, n_filters;
+  fs2_resample_filter_t filters[FS2_RESAMPLE_MAX_FILTERS];
+  const fs2_resample_mixed_stream_t* table;   /* [B] device */
+  int64_t max_out;
+  void* y;
+  float scale;
+} fs2_resample_mixed_args;
+int fs2_resample_streams_mixed(const fs2_resample_mixed_args* a, fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ misc */
 int fs2_abi_version(void);                 /* bumps when any struct above changes */
 int64_t fs2_kernel_launch_count(void);     /* kernels launched by this library since load (process-wide) */
@@ -600,7 +635,8 @@ const char* fs2_build_info(void);          /* "sm_90a ..." */
  * 13 vocoder, 14 resstack, 15 wav_int16, 16 conv_tc_plan_t, 17 conv_simt_plan_t, 18 resstack_plan_t.  Like fs2_control_args,
  * fs2_vocoder_window_args (80 bytes), fs2_vocoder_window_launch_t (56 bytes), fs2_vocoder_streams_args (64 bytes) and the resampler's
  * structs (fs2_resample_args 88, fs2_resample_window_args 144, fs2_resample_stream_t 64, fs2_resample_streams_args 64 bytes; added at
- * ABI 12 without a bump, since no existing struct changed) are not in the table: the binding pins their sizes. */
+ * ABI 12 without a bump, since no existing struct changed; then fs2_resample_filter_t 24, fs2_resample_mixed_stream_t 80 and
+ * fs2_resample_mixed_args 232 bytes, likewise) are not in the table: the binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

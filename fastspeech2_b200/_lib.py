@@ -195,6 +195,27 @@ VOCODER_STREAMS_ARGS_SIZE = 64
 assert C.sizeof(VocoderStreamsArgs) == VOCODER_STREAMS_ARGS_SIZE
 
 
+class VocoderStreamsRingArgs(C.Structure):
+    """fs2_vocoder_streams_ring_args: the streams call on mel rings of cap[b] rows (72 bytes, pinned by a static_assert in model.cu)."""
+    _fields_ = VocoderStreamsArgs._fields_ + [("cap", fp)]
+
+
+class MelRingRecord(C.Structure):
+    """fs2_mel_ring_record_t: one record of fs2_mel_ring_append, in device memory (56 bytes, pinned in model.cu)."""
+    _fields_ = [("src", fp), ("frame_stride", i64), ("channel_stride", i64), ("src_frame", i64), ("ring", fp), ("dst_frame", i64),
+                ("cap", i32), ("count", i32)]
+
+
+class MelRingAppendArgs(C.Structure):
+    """fs2_mel_ring_append_args: n_records appends in one launch (24 bytes, pinned in model.cu)."""
+    _fields_ = [("table", fp), ("n_records", i32), ("n_mel", i32), ("max_count", i32)]
+
+
+VOCODER_STREAMS_RING_ARGS_SIZE, MEL_RING_RECORD_SIZE, MEL_RING_APPEND_ARGS_SIZE = 72, 56, 24
+assert C.sizeof(VocoderStreamsRingArgs) == VOCODER_STREAMS_RING_ARGS_SIZE and C.sizeof(MelRingRecord) == MEL_RING_RECORD_SIZE
+assert C.sizeof(MelRingAppendArgs) == MEL_RING_APPEND_ARGS_SIZE
+
+
 class ResampleArgs(C.Structure):
     """fs2_resample_args: offline sample-rate conversion of [B][N] rows (88 bytes, pinned by a static_assert in resample.cu)."""
     _fields_ = [("B", i32), ("up", i32), ("down", i32), ("K", i32), ("taps", fp), ("x", fp), ("x_batch_stride", i64), ("N", i64),
@@ -313,6 +334,8 @@ EXPORTS = {
     "fs2_vocoder_resblock_runs": (i32, [C.POINTER(VocoderModel), i32, C.POINTER(ResblockRun), i32]),
     "fs2_vocoder_streams_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward_streams": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsArgs), fp]),
+    "fs2_vocoder_forward_streams_ring": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsRingArgs), fp]),
+    "fs2_mel_ring_append": (i32, [C.POINTER(MelRingAppendArgs), fp]),
     "fs2_resample": (i32, [C.POINTER(ResampleArgs), fp]),
     "fs2_resample_window": (i32, [C.POINTER(ResampleWindowArgs), fp]),
     "fs2_resample_streams": (i32, [C.POINTER(ResampleStreamsArgs), fp]),

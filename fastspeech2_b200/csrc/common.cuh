@@ -88,12 +88,14 @@ struct OriginWindow { RowWindow rows; const int* org; };
 
 // The mel of the windowed vocoder's streams, staged by stage_mel: stream b's rows at table[b], n_mel floats apart (table != NULL), or at
 // mel + b * bs, rs floats apart; its first frame f0s[b], or f0 for every stream (f0s NULL); its length lens[b] clamped to [0, cap], or
-// cap (lens NULL).
+// cap (lens NULL).  ring (with table, may be NULL): stream b's frame t lives at row t mod ring[b] of table[b], and ring[b] <= 0 makes its
+// length 0.
 struct MelSource {
   const float* const* table;
   const float* mel; int64_t bs, rs;
   const int32_t* f0s; int f0;
   const int32_t* lens; int cap;
+  const int32_t* ring;
 };
 
 // A per-element control of fs2_control_args on the [B][L] rows of a variance head or of the durations: c[b, l] = v[b * sb + l * sl]

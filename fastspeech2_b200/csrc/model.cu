@@ -90,6 +90,7 @@ int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
 int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win = nullptr, int x0 = 0, bool wide = false);
 int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, cudaStream_t s);
+int mel_ring_append(const fs2_mel_ring_append_args* a, cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out, bool wide = false);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
@@ -986,15 +987,33 @@ int fs2_vocoder_forward_window(const fs2_vocoder_model* m, const fs2_vocoder_win
 
 static_assert(sizeof(fs2_vocoder_streams_args) == 64, "fs2_vocoder_streams_args: two int32, five pointers, an int64 and a size_t");
 
-int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t st) {
+// The streams call, its mel rows addressed as rings of ring[b] rows when ring is set (fs2_vocoder_forward_streams_ring)
+static int vocoder_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, const int32_t* ring, fs2_stream_t st) {
   if (!vocoder_ok(m) || !a || a->B <= 0 || a->frames <= 0 || !window_rows_ok(m, a->frames)) return FS2_ERR_ARG;
   if (!a->mel || !a->mel_lens || !a->f0 || !a->wav || !a->workspace) return FS2_ERR_ARG;
   if (a->B > 1 && a->wav_batch_stride < a->frames * frame_rows(m, m->n_stages)) return FS2_ERR_ARG;
   if (a->workspace_bytes < fs2_vocoder_streams_workspace_bytes(m, a->B, a->frames)) return FS2_ERR_ARG;
-  const MelSource src{a->mel, nullptr, 0, 0, a->f0, 0, a->mel_lens, INT32_MAX};
+  const MelSource src{a->mel, nullptr, 0, 0, a->f0, 0, a->mel_lens, INT32_MAX, ring};
   Arena ar(a->workspace, a->workspace_bytes);
   return vocoder_windowed_impl(m, src, a->B, a->frames, a->wav, a->wav_batch_stride, m->w_pre_tc, S(st), ar);
 }
+
+int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t st) {
+  return vocoder_streams(m, a, nullptr, st);
+}
+
+static_assert(sizeof(fs2_vocoder_streams_ring_args) == 72, "fs2_vocoder_streams_ring_args: fs2_vocoder_streams_args' fields and cap");
+static_assert(sizeof(fs2_mel_ring_record_t) == 56, "fs2_mel_ring_record_t: a pointer, three int64, a pointer, an int64, two int32");
+static_assert(sizeof(fs2_mel_ring_append_args) == 24, "fs2_mel_ring_append_args: a pointer and three int32");
+
+int fs2_vocoder_forward_streams_ring(const fs2_vocoder_model* m, const fs2_vocoder_streams_ring_args* a, fs2_stream_t st) {
+  if (!a || !a->cap) return FS2_ERR_ARG;
+  const fs2_vocoder_streams_args s{a->B, a->frames, a->mel, a->mel_lens, a->f0, a->wav, a->wav_batch_stride, a->workspace,
+                                   a->workspace_bytes};
+  return vocoder_streams(m, &s, a->cap, st);
+}
+
+int fs2_mel_ring_append(const fs2_mel_ring_append_args* a, fs2_stream_t st) { return mel_ring_append(a, S(st)); }
 
 static_assert(sizeof(fs2_resblock_run_t) == 32, "fs2_resblock_run_t: six int32 and a double");
 

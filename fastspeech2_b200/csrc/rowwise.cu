@@ -555,10 +555,13 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
 // out[b][r] = stream b's mel row o_b + x0 + r for r < rows, zeros where that row lies outside [0, n_b), with o_b and n_b the origin and
 // length of MelSource; org[b] = o_b and lens[b] = n_b.  The one kernel that reads the caller's mel and lengths, so the window kernels
 // after it see one batch-strided buffer and two tables.  n_mel % 4 == 0 and 16-byte aligned rows (float4 loads); rows outside the
-// utterance are never dereferenced.
+// utterance are never dereferenced, and a ring's rows are read at t mod ring[b] only.
 __global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, int n4, float4* out, int* org, int* lens, long long total) {
   auto origin = [&](int b) { return src.f0s ? __ldg(src.f0s + b) : src.f0; };
-  auto length = [&](int b) { return src.lens ? min(max(__ldg(src.lens + b), 0), src.cap) : src.cap; };
+  auto length = [&](int b) {
+    if (src.ring && __ldg(src.ring + b) <= 0) return 0;
+    return src.lens ? min(max(__ldg(src.lens + b), 0), src.cap) : src.cap;
+  };
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long br = i / n4;
     const int c4 = (int)(i - br * n4);
@@ -566,7 +569,8 @@ __global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, i
     const long long t = (long long)origin(b) + x0 + r;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (t >= 0 && t < length(b)) {
-      const float* row = src.table ? src.table[b] + t * n4 * 4 : src.mel + b * src.bs + t * src.rs;
+      const long long tr = src.ring ? t % __ldg(src.ring + b) : t;     // length(b) > 0 implies ring[b] > 0
+      const float* row = src.table ? src.table[b] + tr * n4 * 4 : src.mel + b * src.bs + t * src.rs;
       v = __ldg(reinterpret_cast<const float4*>(row) + c4);
     }
     out[i] = v;
@@ -575,7 +579,7 @@ __global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, i
 }
 
 int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, cudaStream_t s) {
-  if (!(src.table || src.mel) || !out || !org || !lens || B <= 0 || rows <= 0 || n_mel <= 0) return FS2_ERR_ARG;
+  if (!(src.table || src.mel) || (src.ring && !src.table) || !out || !org || !lens || B <= 0 || rows <= 0 || n_mel <= 0) return FS2_ERR_ARG;
   if (n_mel % 4 || !aligned16(out) || (!src.table && ((src.bs | src.rs) & 3))) return FS2_ERR_UNSUPPORTED;
   if (!src.table && !aligned16(src.mel)) return FS2_ERR_ARG;
   const long long total = (long long)B * rows * (n_mel / 4);
@@ -583,6 +587,47 @@ int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* o
   prof_before(s);
   stage_mel_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(src, B, x0, rows, n_mel / 4, reinterpret_cast<float4*>(out),
                                                                              org, lens, total);
+  prof_after(s, 3, 0.0);
+  FS2_LAUNCH_CHECK();
+  return FS2_OK;
+}
+
+// ------------------------------------------------------------------ appending arriving mel frames to the streams' rings
+// Block (r, y) copies its share of record r's frames, one float4 (four channels of one frame) per element: channels fastest from a
+// channels-last source (float4 loads and stores both coalesced), frames fastest from any other (a channel-major block's four scalar
+// loads are then coalesced along its frames).  Only the last cap frames of a longer record are copied, so no two elements of a record
+// store to the same ring row.
+__global__ void mel_ring_append_kernel(const fs2_mel_ring_record_t* __restrict__ table, int n4, int max_count) {
+  const fs2_mel_ring_record_t rec = table[blockIdx.x];
+  const int cap = rec.cap;
+  if (cap <= 0 || (reinterpret_cast<uintptr_t>(rec.ring) & 15u)) return;
+  const int cnt = min(max(rec.count, 0), max_count);
+  const int skip = cnt > cap ? cnt - cap : 0, frames = cnt - skip;
+  const long long fs = rec.frame_stride, cs = rec.channel_stride;
+  const bool vec = cs == 1 && (fs & 3) == 0 && (reinterpret_cast<uintptr_t>(rec.src) & 15u) == 0;
+  const long long total = (long long)frames * n4;
+  for (long long e = (long long)blockIdx.y * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.y * blockDim.x) {
+    const int i = skip + (int)(vec ? e / n4 : e % frames), c4 = (int)(vec ? e % n4 : e / frames);
+    const float* s = rec.src + (rec.src_frame + i) * fs + (long long)c4 * 4 * cs;
+    float4 v;
+    if (vec) {
+      v = __ldg(reinterpret_cast<const float4*>(s));
+    } else {
+      v.x = __ldg(s); v.y = __ldg(s + cs); v.z = __ldg(s + 2 * cs); v.w = __ldg(s + 3 * cs);
+    }
+    long long row = (rec.dst_frame + i) % cap;
+    if (row < 0) row += cap;
+    reinterpret_cast<float4*>(rec.ring + row * n4 * 4)[c4] = v;
+  }
+}
+
+int mel_ring_append(const fs2_mel_ring_append_args* a, cudaStream_t s) {
+  if (!a || !a->table || a->n_records <= 0 || a->max_count <= 0) return FS2_ERR_ARG;
+  if (a->n_mel <= 0 || a->n_mel % 4) return FS2_ERR_UNSUPPORTED;
+  const int n4 = a->n_mel / 4;
+  const long long per = ((long long)a->max_count * n4 + 255) / 256;
+  prof_before(s);
+  mel_ring_append_kernel<<<dim3((unsigned)a->n_records, (unsigned)(per < 65535 ? per : 65535)), 256, 0, s>>>(a->table, n4, a->max_count);
   prof_after(s, 3, 0.0);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

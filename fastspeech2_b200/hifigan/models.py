@@ -4,6 +4,7 @@
 """
 from __future__ import annotations
 
+import collections
 import contextlib
 import ctypes as C
 
@@ -328,7 +329,11 @@ class Generator(nn.Module):
         Resampler(h.sampling_rate, sample_rate)(self(mel[None])) bit for bit.  pcm16: int16 chunks (x 32768, truncated, clamped).
         ValueError when chunk_frames * hop is below the resampler's history.  These are the defaults of StreamPool.add, which can give
         each stream its own rate and encoding ("f32", "pcm16", "ulaw", "alaw"); every stream that is not at h.sampling_rate in fp32 is
-        converted by one fs2_resample_streams_mixed launch per step, whatever its format."""
+        converted by one fs2_resample_streams_mixed launch per step, whatever its format.
+
+        A stream whose mel arrives in pieces: h = pool.open(); pool.feed(h, block) as blocks arrive; pool.close(h) after the last.
+        Its chunks, concatenated, equal self(cat(blocks)[None]) (and the conversion of that) bit for bit; its mel is held in a ring
+        of StreamPool.ring_frames rows that depends on chunk_frames only, filled by one fs2_mel_ring_append launch per step."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
         rs = self._resampler(sample_rate, chunk_frames)
@@ -340,36 +345,73 @@ class Generator(nn.Module):
         lib = L.lib()
         ws = [None]
 
-        def launch(ptrs, f0s, ns):
-            """One fs2_vocoder_forward_streams call on the current stream: uploads the (pointer, f0, n) table from a fresh pinned block
-            with one non_blocking copy (the caching host allocator keeps the block until the copy is done; no host sync)."""
+        def launch(ptrs, f0s, ns, caps=None):
+            """One fs2_vocoder_forward_streams call on the current stream (fs2_vocoder_forward_streams_ring with caps): uploads the
+            (pointer, f0, n[, cap]) table from a fresh pinned block with one non_blocking copy (the caching host allocator keeps the
+            block until the copy is done; no host sync)."""
             B, n = len(ptrs), chunk_frames * up
             with torch.cuda.device(dev):
-                host = torch.empty(4 * B, dtype=torch.int32, pin_memory=True)
+                host = torch.empty((4 if caps is None else 5) * B, dtype=torch.int32, pin_memory=True)
                 h = host.numpy()
                 h[:2 * B].view(np.int64)[:] = ptrs
                 h[2 * B:3 * B] = f0s
-                h[3 * B:] = ns
+                h[3 * B:4 * B] = ns
+                if caps is not None:
+                    h[4 * B:] = caps
                 table = host.to(dev, non_blocking=True)
                 need = lib.fs2_vocoder_streams_workspace_bytes(C.byref(m), B, chunk_frames)
                 if ws[0] is None or ws[0].numel() < need:
                     ws[0] = torch.empty(need, dtype=torch.uint8, device=dev)
                 wav = torch.empty(B, n, dtype=torch.float32, device=dev)
                 base = table.data_ptr()
-                sa = L.VocoderStreamsArgs(B=B, frames=chunk_frames, mel=base, mel_lens=base + 12 * B, f0=base + 8 * B, wav=wav.data_ptr(),
-                                          wav_batch_stride=n, workspace=ws[0].data_ptr(), workspace_bytes=ws[0].numel())
-                L.check(lib.fs2_vocoder_forward_streams(C.byref(m), C.byref(sa), torch.cuda.current_stream(dev).cuda_stream),
-                        "fs2_vocoder_forward_streams")
+                args = dict(B=B, frames=chunk_frames, mel=base, mel_lens=base + 12 * B, f0=base + 8 * B, wav=wav.data_ptr(),
+                            wav_batch_stride=n, workspace=ws[0].data_ptr(), workspace_bytes=ws[0].numel())
+                st = torch.cuda.current_stream(dev).cuda_stream
+                if caps is None:
+                    L.check(lib.fs2_vocoder_forward_streams(C.byref(m), C.byref(L.VocoderStreamsArgs(**args)), st),
+                            "fs2_vocoder_forward_streams")
+                else:
+                    L.check(lib.fs2_vocoder_forward_streams_ring(C.byref(m), C.byref(L.VocoderStreamsRingArgs(cap=base + 16 * B, **args)),
+                                                                 st), "fs2_vocoder_forward_streams_ring")
             return wav
+
+        def append(records):
+            """One fs2_mel_ring_append launch on the current stream, its records uploaded as launch's table is."""
+            with torch.cuda.device(dev):
+                host = torch.empty(7 * len(records), dtype=torch.int64, pin_memory=True)
+                t = host.numpy().reshape(-1, 7)
+                t[:, :6] = [r[:6] for r in records]
+                t[:, 6] = [r[6] | (r[7] << 32) for r in records]       # cap and count: two int32, cap first
+                table = host.to(dev, non_blocking=True)
+                a = L.MelRingAppendArgs(table=table.data_ptr(), n_records=len(records), n_mel=m.n_mel, max_count=max(r[7] for r in records))
+                L.check(lib.fs2_mel_ring_append(C.byref(a), torch.cuda.current_stream(dev).cuda_stream), "fs2_mel_ring_append")
 
         def resample(records, max_out):
             with torch.cuda.device(dev):
                 return Resampler.mixed(records, max_out, dev)[1]
         fs = _cfg(self.h, "sampling_rate")
         resample.rs = rs or Resampler(fs, fs)
-        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev, resample=resample, encoding="pcm16" if pcm16 else "f32")
+        pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev, resample=resample, encoding="pcm16" if pcm16 else "f32", append=append,
+                          reach=mel_reach(m, chunk_frames))
         pool._keep = keep                              # the packed weights stay alive while the pool runs
         return pool
+
+
+def mel_reach(m, chunk_frames):
+    """(left, right): the mel frames a chunk [f0, f0 + chunk_frames) of model m reads before f0 and past f0 + chunk_frames -- conv_pre's
+    input rows of the plan of a window that neither utterance end clips (L.vocoder_window_plan)."""
+    f0 = 1 << 16
+    pre = L.vocoder_window_plan(m, 1 << 20, f0, f0 + chunk_frames)[0]
+    return f0 - pre.x0, pre.x1 - f0 - chunk_frames
+
+
+class _Feed:
+    """An open stream's state: the frames in its ring, the caller's blocks not yet appended ([tensor [n_mel, m], frames appended]),
+    and whether it is closed."""
+    __slots__ = ("written", "blocks", "closed")
+
+    def __init__(self):
+        self.written, self.blocks, self.closed = 0, collections.deque(), False
 
 
 class StreamPool:
@@ -383,15 +425,27 @@ class StreamPool:
     samples, the outputs [j0, j1) it emits, its resample.Resampler (the identity at the waveform's rate) and its L.RESAMPLE_* encoding;
     the call returns rows indexable by b (a [B, >= max(j1 - j0)] tensor, or a list of tensors), row b starting with stream b's outputs.
     Its `.rs`, a Resampler from the waveform's rate, and `encoding` ("f32", "pcm16", "ulaw" or "alaw") are the defaults of add(); a
-    pool without `resample` only vocodes."""
+    pool without `resample` only vocodes.
 
-    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None, encoding="f32"):
+    append (optional): what open streams (open / feed / close) need.  `append(records)` copies arriving mel frames into the streams'
+    rings, in one call: records[r] = (src, frame_stride, channel_stride, src_frame, ring, dst_frame, cap, count) copies `count` frames,
+    source frame src_frame + i at element src_frame + i times frame_stride, plus c times channel_stride for channel c, of the tensor at
+    address src, to row (dst_frame + i) mod cap of the [cap, n_mel] ring at address ring (fs2_mel_ring_append).  reach = (left, right):
+    the mel frames a chunk [f0, f0 + chunk_frames) reads before f0 and past its end (mel_reach).  In a step in which a stream opened
+    with open() takes part, launch is called as launch(ptrs, f0s, ns, caps=caps): stream b's frame t at row t mod caps[b] of ptrs[b]
+    (caps[b] = ns[b] for an add()ed stream, which never wraps)."""
+
+    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None, encoding="f32", append=None, reach=(0, 0)):
         self._launch, self.n_mel, self.up, self.chunk_frames, self.device = launch, n_mel, up, chunk_frames, torch.device(device)
         self._resample = resample
         rs = getattr(resample, "rs", None)
         self._rates = {} if rs is None else {rs.fs_out: rs}   # output rate -> its Resampler, one per rate
         self._default = (rs, self._encoding(encoding))
-        # [handle, channels-last mel view [n, n_mel], n, next frame, last chunk, emitted, Resampler or None, encoding]
+        self._append, self.reach = append, tuple(reach)
+        # an open stream's ring holds the cone of its current chunk: the frames written last are at most f0 + chunk_frames + right
+        self.ring_frames = -(-(self.reach[0] + chunk_frames + self.reach[1]) // 8) * 8
+        # [handle, channels-last mel view [n, n_mel] (an open stream: its ring [ring_frames, n_mel]), n (an open stream: the frames fed
+        #  so far), next frame, last chunk, emitted, Resampler or None, encoding, _Feed (None for an add()ed stream)]
         self._live = []
         self._next = 0
 
@@ -437,18 +491,79 @@ class StreamPool:
         n = mel.shape[1]
         if n < 1:
             raise ValueError("mel has no frames")
+        rs, enc = self._format(sample_rate, encoding)
+        rows = mel.T
+        if not (rows.dtype == torch.float32 and rows.stride(1) == 1 and (n == 1 or rows.stride(0) == self.n_mel) and rows.data_ptr() % 16 == 0):
+            rows = rows.to(torch.float32).contiguous()
+        return self._admit(rows, n, rs, enc, None)
+
+    def _format(self, sample_rate, encoding):
+        """A new stream's (Resampler or None, encoding), checked as add() documents."""
         rs = self._resampler(sample_rate)
         enc = self._default[1] if encoding is None else self._encoding(encoding)
         rates = {s[6].fs_out for s in self._live if s[6] is not None}
         if rs is not None and rs.fs_out not in rates and len(rates) >= L.RESAMPLE_MAX_FILTERS:
             raise ValueError(f"the live streams already use {len(rates)} output rates; at most {L.RESAMPLE_MAX_FILTERS}")
-        rows = mel.T
-        if not (rows.dtype == torch.float32 and rows.stride(1) == 1 and (n == 1 or rows.stride(0) == self.n_mel) and rows.data_ptr() % 16 == 0):
-            rows = rows.to(torch.float32).contiguous()
+        return rs, enc
+
+    def _admit(self, rows, n, rs, enc, feed):
         h = self._next
         self._next += 1
-        self._live.append([h, rows, n, 0, None, 0, rs, enc])
+        self._live.append([h, rows, n, 0, None, 0, rs, enc, feed])
         return h
+
+    def open(self, sample_rate=None, encoding=None):
+        """Admits a stream whose mel has not arrived yet: feed(h, block) appends frames, close(h) fixes its length.  It takes part in a
+        step once its next chunk's cone has arrived, and concatenated its chunks equal those of add() on the concatenated blocks bit
+        for bit.  Its mel lives in a ring of ring_frames rows, whatever its length.  sample_rate and encoding as in add().  ValueError
+        in a pool without an append call.  Returns the handle."""
+        if self._append is None:
+            raise ValueError("this pool has no append call: it cannot take open streams")
+        rs, enc = self._format(sample_rate, encoding)
+        ring = torch.empty(self.ring_frames, self.n_mel, dtype=torch.float32, device=self.device)
+        return self._admit(ring, 0, rs, enc, _Feed())
+
+    def _open_stream(self, h):
+        for s in self._live:
+            if s[0] == h:
+                if s[8] is None:
+                    raise ValueError(f"stream {h} was admitted whole by add()")
+                if s[8].closed:
+                    raise ValueError(f"stream {h} is closed")
+                return s
+        raise KeyError(h)
+
+    def feed(self, h, mel):
+        """Queues the next frames of open stream h: mel [n_mel, m] or [1, n_mel, m], m >= 1, on the pool's device, in any layout
+        (FastSpeech2's postnet_mel[b, a:z].T and a channel-major [n_mel, m] block are both read in place).  The pool keeps a reference
+        to the tensor until its last frame has been copied into the ring; the caller must not write it before then.  A floating
+        block that is not fp32 is converted once.  KeyError for a handle that is not live, ValueError for a closed or add()ed stream
+        or a bad block."""
+        s = self._open_stream(h)
+        if not isinstance(mel, torch.Tensor):
+            raise ValueError("mel must be a tensor")
+        if mel.dim() == 3 and mel.shape[0] == 1:
+            mel = mel[0]
+        if mel.dim() != 2 or mel.shape[0] != self.n_mel:
+            raise ValueError(f"expected mel of shape [{self.n_mel}, m] or [1, {self.n_mel}, m]")
+        if mel.device != self.device:
+            raise ValueError(f"mel is on {mel.device}, the vocoder on {self.device}")
+        if not mel.dtype.is_floating_point:
+            raise ValueError(f"mel must be floating point, got {mel.dtype}")
+        if mel.shape[1] < 1:
+            raise ValueError("mel has no frames")
+        if mel.dtype != torch.float32:
+            mel = mel.to(torch.float32)
+        s[8].blocks.append([mel, 0])
+        s[2] += mel.shape[1]
+
+    def close(self, h):
+        """Fixes open stream h's length at the frames fed so far; its remaining chunks then take part in every step, the last trimmed
+        to its end.  A stream closed with no frames leaves without output.  KeyError / ValueError as feed()."""
+        s = self._open_stream(h)
+        s[8].closed = True
+        if s[3] >= s[2]:
+            self._live = [x for x in self._live if x is not s]
 
     def cancel(self, h):
         """Drops a live stream (KeyError if it is not live)."""
@@ -465,11 +580,21 @@ class StreamPool:
         """One chunk of every live stream, in one launch call: a list of (handle, first_sample, chunk [1, 1, m]) in admission order,
         m = chunk_frames * up except on a stream's last chunk, which is trimmed to its end.  [] without a call when the pool is empty.
         A converted stream: first_sample and m at its own rate, the chunk holding the outputs that became ready (possibly none), of its
-        encoding's dtype; at most one conversion call per step, none when every live stream is at the waveform's rate in fp32."""
-        if not self._live:
+        encoding's dtype; at most one conversion call per step, none when every live stream is at the waveform's rate in fp32.
+
+        An open stream takes part only once the cone of its next chunk has arrived (fed >= f0 + chunk_frames + reach[1]), or once it is
+        closed; a starved one yields nothing and holds nobody back, and a step in which no stream takes part makes no call.  In a step
+        with a stream from open(), one append call first copies into the rings the frames this step's chunks read, then the launch
+        runs every stream that takes part on rings (launch's caps)."""
+        live = [s for s in self._live if s[8] is None or s[8].closed or s[2] >= s[3] + self.chunk_frames + self.reach[1]]
+        if not live:
             return []
-        live = self._live
-        wav = self._launch([s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live])
+        ptrs, f0s, ns = [s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live]
+        if any(s[8] is not None for s in live):
+            self._fill(live)
+            wav = self._launch(ptrs, f0s, ns, caps=[n if s[8] is None else self.ring_frames for s, n in zip(live, ns)])
+        else:
+            wav = self._launch(ptrs, f0s, ns)
         rows = [(wav, i) for i in range(len(live))]     # where each stream's chunk is: (rows, index)
         starts = [s[3] * self.up for s in live]
         widths = [min(self.chunk_frames, s[2] - s[3]) * self.up for s in live]
@@ -478,15 +603,36 @@ class StreamPool:
             y = self._converted(live, conv, wav, starts, widths)
             for k, i in enumerate(conv):
                 rows[i] = (y, k)
-        out, keep = [], []
+        out = []
         for i, s in enumerate(live):
             t, k = rows[i]
             out.append((s[0], starts[i], t[k][None, None, :widths[i]]))
             s[3] += self.chunk_frames
-            if s[3] < s[2]:
-                keep.append(s)
-        self._live = keep
+        self._live = [s for s in self._live if (s[8] is not None and not s[8].closed) or s[3] < s[2]]
         return out
+
+    def _fill(self, live):
+        """One append call copying, for each stream from open() among `live`, its frames up to the end of this step's cone (or its
+        end) that are not in its ring yet."""
+        records, done = [], []
+        for s in live:
+            f = s[8]
+            if f is None:
+                continue
+            target = min(s[3] + self.chunk_frames + self.reach[1], s[2])
+            while f.written < target:
+                blk = f.blocks[0]
+                mel, off = blk
+                k = min(mel.shape[1] - off, target - f.written)
+                records.append((mel.data_ptr(), mel.stride(1), mel.stride(0), off, s[1].data_ptr(), f.written, self.ring_frames, k))
+                f.written += k
+                blk[1] = off + k
+                if blk[1] == mel.shape[1]:
+                    done.append(f.blocks.popleft())
+        if records:
+            self._append(records)
+        # The blocks appended in full are released only now, after the call is enqueued (the rule _converted states for its chunks).
+        del done
 
     def _converted(self, live, conv, wav, starts, widths):
         """The conversion call for streams `conv` on this step's waveform; sets their first output and output count in starts and
@@ -495,9 +641,10 @@ class StreamPool:
         records = []
         for i in conv:
             s = live[i]
-            _, _, n, f0, prev, emitted, rs, enc = s
-            i1, N = f0 * self.up, n * self.up
-            r = rs.ready(min(i1 + n1, N), N, f0 + self.chunk_frames >= n)
+            _, _, n, f0, prev, emitted, rs, enc, feed = s
+            i1, N = f0 * self.up, n * self.up              # an open stream: N covers every input its ready outputs read
+            is_open = feed is not None and not feed.closed
+            r = rs.ready(min(i1 + n1, N), None if is_open else N, not is_open and f0 + self.chunk_frames >= n)
             cur = wav[i]
             records.append((0 if prev is None else prev.data_ptr(), cur.data_ptr(), i1 - (0 if prev is None else n1), i1, i1 + n1, N,
                             emitted, r, rs, enc))

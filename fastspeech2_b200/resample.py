@@ -80,14 +80,14 @@ class Resampler:
         """Input samples before the first not-yet-emitted output's support that a window may still need: K - 1."""
         return 0 if self.identity else self.K - 1
 
-    def ready(self, m: int, n: int, ended: bool) -> int:
+    def ready(self, m: int, n: int | None, ended: bool) -> int:
         """Outputs ready once m of a stream's n input samples have arrived: j is ready iff floor((j down + half_len) / up) < m, or
-        the stream has ended (then all n_out(n))."""
+        the stream has ended (then all n_out(n)).  n None: a stream whose length is not known yet, which has not ended; its ready
+        outputs are not capped at n_out(n)."""
         if ended:
             return self.n_out(n)
-        if self.identity:
-            return min(m, n)
-        return min(self.n_out(n), max(0, -(-(m * self.up - self.half_len) // self.down)))
+        r = m if self.identity else max(0, -(-(m * self.up - self.half_len) // self.down))
+        return r if n is None else min(self.n_out(n), r)
 
     def device_taps(self, device):
         """The [up][K] taps on `device` (the identity: the one-tap table of 1.0 that the mixed call runs), uploaded once."""

@@ -524,6 +524,48 @@ typedef struct fs2_vocoder_streams_args {
 size_t fs2_vocoder_streams_workspace_bytes(const fs2_vocoder_model* m, int B, int frames);
 int fs2_vocoder_forward_streams(const fs2_vocoder_model* m, const fs2_vocoder_streams_args* a, fs2_stream_t stream);
 
+/* Streams whose mel is a ring: fs2_vocoder_forward_streams, but stream b's frame t lives at row t mod cap[b] of its cap[b]-row buffer
+ * mel[b] (n_mel contiguous floats per row, 16-byte aligned).  With n_b = mel_lens[b], the output equals fs2_vocoder_forward_streams on
+ * the stream's unwrapped frames bit for bit, provided every frame of the window's cone inside [0, n_b) is still in the ring (within the
+ * last cap[b] frames written).  A finished mel is the ring cap[b] = n_b, which never wraps.
+ *   - the host never reads cap: the row index is reduced mod cap[b] on the device, so the reads stay inside the cap[b] rows at
+ *     mel[b]; cap[b] <= 0 gives an all-zero chunk;
+ *   - the launches, workspace bound (fs2_vocoder_streams_workspace_bytes) and argument checks are those of
+ *     fs2_vocoder_forward_streams, plus FS2_ERR_ARG for a NULL cap. */
+typedef struct fs2_vocoder_streams_ring_args {
+  int B, frames;
+  const float* const* mel;        /* [B] device array: stream b's ring of cap[b] rows */
+  const int32_t* mel_lens;        /* [B] device: frames of stream b that exist (written so far, or its total) */
+  const int32_t* f0;              /* [B] device: stream b's first frame in this call */
+  float* wav; int64_t wav_batch_stride;
+  void* workspace; size_t workspace_bytes;
+  const int32_t* cap;             /* [B] device: ring rows of stream b */
+} fs2_vocoder_streams_ring_args;
+int fs2_vocoder_forward_streams_ring(const fs2_vocoder_model* m, const fs2_vocoder_streams_ring_args* a, fs2_stream_t stream);
+
+/* Appending arriving mel frames to rings, every stream's in one launch: record r copies `count` frames, source frame src_frame + i at
+ * src + (src_frame + i) * frame_stride + c * channel_stride (floats) for channel c, to ring row (dst_frame + i) mod cap of `ring`
+ * ([cap][n_mel] channels-last, 16-byte aligned), for i < count.  Any strides: FastSpeech2's postnet_mel[b] is frame_stride n_mel,
+ * channel_stride 1 (float4 loads when aligned), an [n_mel, m] channel-major block frame_stride 1, channel_stride m (transposed on the
+ * way in).  Every ring row is written with float4 stores.
+ *   - the host never reads the table: the grid is sized from n_records and max_count, count is clamped to [0, max_count], and a count
+ *     past cap copies only its last cap frames (what copying in order would leave); a record with cap <= 0 or a ring that is not
+ *     16-byte aligned writes nothing;
+ *   - a NULL table, n_records <= 0 or max_count <= 0 is FS2_ERR_ARG, n_mel not a positive multiple of 4 FS2_ERR_UNSUPPORTED, before any
+ *     CUDA call.  Records of one launch must not write the same ring rows. */
+typedef struct fs2_mel_ring_record_t {
+  const float* src;
+  int64_t frame_stride, channel_stride, src_frame;
+  float* ring;
+  int64_t dst_frame;
+  int32_t cap, count;
+} fs2_mel_ring_record_t;
+typedef struct fs2_mel_ring_append_args {
+  const fs2_mel_ring_record_t* table;   /* [n_records] device */
+  int n_records, n_mel, max_count;
+} fs2_mel_ring_append_args;
+int fs2_mel_ring_append(const fs2_mel_ring_append_args* a, fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ sample-rate conversion of the waveform (scipy.signal.resample_poly)
  *
  * up / down is fs_out / fs_in reduced, max(up, down) <= FS2_RESAMPLE_MAX_FACTOR.  With half_len = 10 * max(up, down) and the
@@ -636,7 +678,8 @@ const char* fs2_build_info(void);          /* "sm_90a ..." */
  * fs2_vocoder_window_args (80 bytes), fs2_vocoder_window_launch_t (56 bytes), fs2_vocoder_streams_args (64 bytes) and the resampler's
  * structs (fs2_resample_args 88, fs2_resample_window_args 144, fs2_resample_stream_t 64, fs2_resample_streams_args 64 bytes; added at
  * ABI 12 without a bump, since no existing struct changed; then fs2_resample_filter_t 24, fs2_resample_mixed_stream_t 80 and
- * fs2_resample_mixed_args 232 bytes, likewise) are not in the table: the binding pins their sizes. */
+ * fs2_resample_mixed_args 232 bytes, likewise; then fs2_vocoder_streams_ring_args 72, fs2_mel_ring_record_t 56 and
+ * fs2_mel_ring_append_args 24 bytes, likewise) are not in the table: the binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

@@ -182,11 +182,12 @@ __global__ void variance_head_kernel(const fs2_variance_head_args a, const Contr
   }
   if (lane == 0) a.pred_out[row] = pred;
   if (!a.bins) return;
-  // torch.bucketize(right=False): number of edges strictly below key
+  // torch.bucketize(right=False) in ATen's form: the number of edges strictly below an ordered key, and n_edges for a NaN key (no
+  // edge compares >= NaN), which is the bucket the reference picks for a NaN prediction, control or target
   int lo = 0, hi = a.n_edges;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
-    if (__ldg(a.bins + mid) < key) lo = mid + 1; else hi = mid;
+    if (!(__ldg(a.bins + mid) >= key)) lo = mid + 1; else hi = mid;
   }
   const float4* e = reinterpret_cast<const float4*>(a.emb) + (long long)lo * (a.D / 4);
   float4* x = reinterpret_cast<float4*>(a.x) + (long long)row * (a.D / 4);
@@ -236,12 +237,14 @@ __global__ void durations_kernel(const fs2_durations_args a, const int* __restri
         d = s;
       } else {
         const float dc = CTL ? __ldg(ctl.v + b * ctl.sb + l * ctl.sl) : a.d_control;
-        d = fmaxf(rintf(expf(s) - 1.f) * dc, 0.f);
+        const float v = rintf(expf(s) - 1.f) * dc;
+        d = v <= 0.f ? 0.f : v;  // torch.clamp(min=0) keeps NaN (fmaxf would make it 0); -0 and below give +0 as fmaxf did
         if (a.d_rounded) a.d_rounded[(long long)b * a.L + l] = d;
       }
-      // int() truncation toward zero.  A NaN / inf / absurd duration (the reference raises on int(inf) or dies allocating) is counted
-      // in len_stats[2] and contributes no frames, so the caller can fail loudly instead of sizing a gigantic output.
-      const bool wild = !(d <= 1.0e6f);
+      // int() truncation toward zero.  A NaN / +-inf / absurd duration (the reference raises on int(nan) and int(+-inf), or dies
+      // allocating) is counted in len_stats[2] and contributes no frames, so the caller can fail loudly instead of sizing a gigantic
+      // output.
+      const bool wild = !(d <= 1.0e6f && d > -INFINITY);
       if (wild) atomicAdd(a.len_stats + 2, 1);
       reps = wild ? 0 : max((int)d, 0);
     }
@@ -388,7 +391,10 @@ __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int t
   const int nin = min(n_b, pr.win.xend);
   for (int i = threadIdx.x; i < a.taps * C; i += blockDim.x) wsm[i] = a.w[i];
   const int rows = CP_ROWS + a.taps - 1, C4 = C / 4;
-  const float4* xb = reinterpret_cast<const float4*>(a.x + (long long)b * pr.xbs);
+  const float* xf = a.x + (long long)b * pr.xbs;
+  const float4* xb = reinterpret_cast<const float4*>(xf);
+  // x need not be 16-byte aligned here (the dispatcher sends such an x to this kernel, e.g. a view at an odd float offset): scalar loads
+  const bool vec = (reinterpret_cast<uintptr_t>(xf) & 15u) == 0;
   for (int i = threadIdx.x; i < rows * C4; i += blockDim.x) {
     const int r = i / C4, c4 = i - r * C4;
     const int t = t0 - pad + r;
@@ -397,7 +403,12 @@ __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int t
     if constexpr (ORG) in = t >= lo_b && t < nin;
     else in = t >= 0 && t < nin;
     if (in) {
-      v = __ldg(xb + (long long)t * C4 + c4);
+      if (vec) {
+        v = __ldg(xb + (long long)t * C4 + c4);
+      } else {
+        const float* p = xf + (long long)t * C + c4 * 4;
+        v = make_float4(__ldg(p), __ldg(p + 1), __ldg(p + 2), __ldg(p + 3));
+      }
       v.x = v.x > 0.f ? v.x : v.x * a.in_slope;
       v.y = v.y > 0.f ? v.y : v.y * a.in_slope;
       v.z = v.z > 0.f ? v.z : v.z * a.in_slope;

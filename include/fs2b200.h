@@ -174,8 +174,8 @@ typedef struct fs2_rowbias_args { float* x; const float* table; const int64_t* i
 int fs2_add_speaker(const fs2_rowbias_args* a, fs2_stream_t stream);
 
 /* pred[b,l] = (h[b,l,:].w + *b), 0 where l >= lens[b]; if bins != NULL:
- *   v = target ? target[b,l] : pred*control (pred_out then holds the scaled value),  i = #edges < v (torch.bucketize right=False),
- *   x[b,l,:] += emb[i]. */
+ *   v = target ? target[b,l] : pred*control (pred_out then holds the scaled value),  i = #edges < v (torch.bucketize right=False:
+ *   -inf -> 0, +inf -> #edges < inf, NaN -> n_edges, as ATen's search picks),  x[b,l,:] += emb[i]. */
 typedef struct fs2_variance_head_args {
   const float* h; const float* w; const float* b; int B, L, C;
   const int32_t* lens; float control; const float* target;
@@ -184,9 +184,11 @@ typedef struct fs2_variance_head_args {
 } fs2_variance_head_args;
 int fs2_variance_head(const fs2_variance_head_args* a, fs2_stream_t stream);
 
-/* d = use_target ? src[b,l] : max(rint(exp(src[b,l]) - 1) * d_control, 0); reps = max((int)d, 0);
+/* d = use_target ? src[b,l] : clamp(rint(exp(src[b,l]) - 1) * d_control, min=0) (torch.clamp: NaN stays NaN, so d_rounded holds NaN
+ * where the reference's does); reps = max((int)d, 0);
  * cum[b,l] = inclusive prefix sum of reps; mel_lens[b] = cum[b,L-1]; len_stats[0] = max_b mel_lens, [1] = sum_b mel_lens,
- * [2] = number of non-finite / > 1e6 durations (those contribute 0 frames; the reference raises on them).  The call zeroes len_stats. */
+ * [2] = number of NaN / +-inf / > 1e6 durations (those contribute 0 frames; the reference's int() raises on them).  The call zeroes
+ * len_stats. */
 typedef struct fs2_durations_args {
   const float* src; int use_target; float d_control; int B, L;
   float* d_rounded;     /* [B][L] or NULL */
@@ -322,7 +324,7 @@ typedef struct fs2_encode_args {
   int32_t* mel_lens32;       /* [B] */
   int32_t* cum_dur;          /* [B][L] */
   float* x_adapted;          /* [B][L][D]: input of the length regulator */
-  int32_t* len_stats;        /* device [3]: max and sum of mel_lens, count of non-finite durations */
+  int32_t* len_stats;        /* device [3]: max and sum of mel_lens, count of NaN / +-inf / > 1e6 durations */
   int32_t* len_stats_host;   /* pinned host [3] or NULL: async D2H copy is enqueued on the stream */
   void* workspace; size_t workspace_bytes;
 } fs2_encode_args;

@@ -473,7 +473,7 @@ def variance_head(h, w, b, lens, control, target, bins, emb, x):
     else:
         pred = pred * control
         key = pred
-    idx = (bins[None, None, :] < key[..., None]).sum(-1)
+    idx = (~(bins[None, None, :] >= key[..., None])).sum(-1)    # torch.bucketize(right=False): NaN -> len(bins), like ATen's search
     return pred, x + emb[idx]
 
 
@@ -490,11 +490,13 @@ def durations(src, use_target, d_control):
         d = src
         d_rounded = None
     else:
-        d = torch.clamp(torch.round(torch.exp(src) - 1) * d_control, min=0)
+        d = torch.clamp(torch.round(torch.exp(src) - 1) * d_control, min=0)     # torch.clamp keeps NaN
         d_rounded = d
-    reps = d.trunc().clamp(min=0).to(torch.int32)
+    # the reference's int() raises on NaN and +-inf (a -inf target too); those and durations past 1e6 frames count as wild, 0 frames
+    wild = ~((d <= 1.0e6) & (d > -math.inf))
+    reps = torch.where(wild, torch.zeros_like(d), d).trunc().clamp(min=0).to(torch.int32)
     cum = torch.cumsum(reps, dim=1).to(torch.int32)
-    return d_rounded, cum, cum[:, -1].long()
+    return d_rounded, cum, cum[:, -1].long(), int(wild.sum())
 
 
 def length_regulate(x, cum, pos, T):
@@ -523,7 +525,7 @@ def acoustic_forward(pk, cfg, speakers, texts, src_lens, p_control=1.0, d_contro
         p_pred, x = predictor(pk, "pitch", x, lens, k, p_control, p_target, pk["pitch_bins"], pk["pitch_emb"], x)
     if not energy_frame:
         e_pred, x = predictor(pk, "energy", x, lens, k, p_control, e_target, pk["energy_bins"], pk["energy_emb"], x)
-    d_rounded, cum, mel_len = durations(d_target if d_target is not None else logd, d_target is not None, d_control)
+    d_rounded, cum, mel_len, _ = durations(d_target if d_target is not None else logd, d_target is not None, d_control)
     T = int(max_mel_len) if max_mel_len is not None else int(mel_len.max())
     mask_lens = (mel_lens if mel_lens is not None else mel_len).to(torch.int32)
     if pitch_frame or energy_frame:                  # decode_impl: LR without positions, frame-level heads, then fs2_add_positions

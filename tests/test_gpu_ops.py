@@ -807,9 +807,10 @@ def test_variance_head():
 
 
 def test_bucketize_edges_exact():
-    """torch.bucketize(right=False): a value equal to an edge goes to that edge's index."""
+    """torch.bucketize(right=False): a value equal to an edge goes to that edge's index, NaN past the last edge (ATen's search)."""
     bins = torch.linspace(-1.0, 1.0, 255)
-    vals = torch.cat([bins[[0, 1, 100, 254]], torch.tensor([-5.0, 5.0, 0.0])])
+    vals = torch.cat([bins[[0, 1, 100, 254]], torch.tensor([-5.0, 5.0, 0.0, -0.0, float("nan"), float("inf"), float("-inf")]),
+                      torch.nextafter(bins[[0, 127, 254]], torch.tensor(2.0)), torch.nextafter(bins[[0, 127, 254]], torch.tensor(-2.0))])
     n = vals.numel()
     h = torch.zeros(1, n, 4); h[0, :, 0] = vals
     w = torch.tensor([1.0, 0, 0, 0]); b = torch.zeros(1)
@@ -825,7 +826,7 @@ def test_durations_and_length_regulate(L, d_control):
     logd = rnd(B, L, seed=1, scale=0.6) + 1.2
     logd[1, L // 2:] = 0.0                                    # padded phonemes predict log-duration 0 -> d = 0
     logd[0, :5] = torch.log(torch.tensor([3.5, 4.5, 1.5, 2.5, 1.0]))   # round-half-even cases
-    wd, wcum, wlen = E.durations(logd, False, d_control)
+    wd, wcum, wlen, _ = E.durations(logd, False, d_control)
     d, cum, mel_lens, mel_lens32, stats = ops.durations(logd.to(DEV), False, d_control)
     assert torch.equal(d.cpu(), wd) and torch.equal(cum.cpu(), wcum) and torch.equal(mel_lens.cpu(), wlen)
     assert stats.cpu().tolist() == [int(wlen.max()), int(wlen.sum()), 0]          # max, sum, count of non-finite durations
@@ -837,7 +838,7 @@ def test_durations_and_length_regulate(L, d_control):
         assert torch.equal(got.cpu(), want)                   # gather + one add: bit exact
     # integer targets (teacher forcing)
     tgt = torch.randint(0, 9, (B, L), generator=g(4)).float()
-    _, wcum2, wlen2 = E.durations(tgt, True, 1.0)
+    _, wcum2, wlen2, _ = E.durations(tgt, True, 1.0)
     _, cum2, ml2, _, _ = ops.durations(tgt.to(DEV), True, 1.0)
     assert torch.equal(cum2.cpu(), wcum2) and torch.equal(ml2.cpu(), wlen2)
 

@@ -211,6 +211,16 @@ class MelRingAppendArgs(C.Structure):
     _fields_ = [("table", fp), ("n_records", i32), ("n_mel", i32), ("max_count", i32)]
 
 
+class VocoderStreamsMultiArgs(C.Structure):
+    """fs2_vocoder_streams_multi_args: the streams call with a generator per stream, cap NULL or rings (88 bytes, pinned by a
+    static_assert in model.cu)."""
+    _fields_ = VocoderStreamsRingArgs._fields_ + [("gen", fp), ("models_dev", fp)]
+
+
+MAX_GENERATORS = 8
+VOCODER_STREAMS_MULTI_ARGS_SIZE = 88
+assert C.sizeof(VocoderStreamsMultiArgs) == VOCODER_STREAMS_MULTI_ARGS_SIZE
+
 VOCODER_STREAMS_RING_ARGS_SIZE, MEL_RING_RECORD_SIZE, MEL_RING_APPEND_ARGS_SIZE = 72, 56, 24
 assert C.sizeof(VocoderStreamsRingArgs) == VOCODER_STREAMS_RING_ARGS_SIZE and C.sizeof(MelRingRecord) == MEL_RING_RECORD_SIZE
 assert C.sizeof(MelRingAppendArgs) == MEL_RING_APPEND_ARGS_SIZE
@@ -335,6 +345,8 @@ EXPORTS = {
     "fs2_vocoder_streams_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward_streams": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsArgs), fp]),
     "fs2_vocoder_forward_streams_ring": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderStreamsRingArgs), fp]),
+    "fs2_vocoder_streams_multi_workspace_bytes": (C.c_size_t, [C.POINTER(C.POINTER(VocoderModel)), i32, i32, i32]),
+    "fs2_vocoder_forward_streams_multi": (i32, [C.POINTER(C.POINTER(VocoderModel)), i32, C.POINTER(VocoderStreamsMultiArgs), fp]),
     "fs2_mel_ring_append": (i32, [C.POINTER(MelRingAppendArgs), fp]),
     "fs2_resample": (i32, [C.POINTER(ResampleArgs), fp]),
     "fs2_resample_window": (i32, [C.POINTER(ResampleWindowArgs), fp]),
@@ -395,6 +407,11 @@ def vocoder_resblock_runs(m, stage):
     out = (ResblockRun * max(n, 1))()
     check(min(0, lib().fs2_vocoder_resblock_runs(C.byref(m), stage, out, n)), "fs2_vocoder_resblock_runs")
     return list(out)[:n]
+
+
+def model_array(models):
+    """The host array of model pointers fs2_vocoder_forward_streams_multi takes (the structs must outlive it)."""
+    return (C.POINTER(VocoderModel) * len(models))(*[C.pointer(m) for m in models])
 
 
 def ptr(t):

@@ -82,9 +82,23 @@ __device__ __forceinline__ RowSpan origin_rows(const int* lens, const int* org, 
   return RowSpan{origin_clamp(-o * scale), origin_clamp((n - o) * scale)};
 }
 
+// Multi-generator mode of the windowed layers (fs2_vocoder_forward_streams_multi): stream b's weights are those of generator gen[b] of
+// the device array `models` (gen as stage_mel staged it: always in range).  A launch names each weight it reads by a GenRef -- the
+// byte offset of its pointer field in fs2_vocoder_model and a float offset past that pointer -- and every work item loads the pointer
+// from its own stream's generator.  models == NULL outside this mode.
+struct GenRef { int32_t off, add; };
+struct Generators { const fs2_vocoder_model* models; const int* gen; };
+__device__ __forceinline__ const float* gen_weight(const Generators& g, int b, GenRef r) {
+  const unsigned char* m = reinterpret_cast<const unsigned char*>(g.models + __ldg(g.gen + b));
+  return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(m + r.off))) + r.add;
+}
+// The weights of one windowed launch in the multi-generator mode: a conv's fp32 weights, tiles and bias; a fused ResBlock launch's
+// pairs, its arguments' (j, d) being ResBlock rb + j at dilation d0 + d of every generator.
+struct GenLaunch { Generators gens; GenRef w, wt, bias; int rb, d0; };
+
 // What a launcher takes in the windowed mode, NULL outside it: the layer's window rows and the utterances' origins, never one without
-// the other.
-struct OriginWindow { RowWindow rows; const int* org; };
+// the other, and the launch's weights per generator in the multi-generator mode (multi.gens.models != NULL).
+struct OriginWindow { RowWindow rows; const int* org; GenLaunch multi; };
 
 // The mel of the windowed vocoder's streams, staged by stage_mel: stream b's rows at table[b], n_mel floats apart (table != NULL), or at
 // mel + b * bs, rs floats apart; its first frame f0s[b], or f0 for every stream (f0s NULL); its length lens[b] clamped to [0, cap], or

@@ -213,6 +213,15 @@ template <int BM, int BN, int ACT>
 __global__ void __launch_bounds__(256) conv_simt_streams_kernel(const ConvP p) {
   conv_simt_body<BM, BN, ACT, true>(p);
 }
+// Multi-generator mode (fs2_vocoder_forward_streams_multi): a CTA serves one utterance, so it runs the windowed body on the weights and
+// bias of that utterance's generator (g: w and bias; p.bias stays the "has a bias" flag)
+template <int BM, int BN, int ACT>
+__global__ void __launch_bounds__(256) conv_simt_streams_multi_kernel(ConvP p, const GenLaunch g) {
+  const int b = blockIdx.x / p.tiles_per_batch;
+  p.w = gen_weight(g.gens, b, g.w);
+  if (p.bias) p.bias = gen_weight(g.gens, b, g.bias);
+  conv_simt_body<BM, BN, ACT, true>(p);
+}
 
 // Tile choice of the launcher (pure host logic, no CUDA call; exposed as fs2_conv_simt_plan so that the GPU tests' coverage of the six
 // (BM, BN) instantiations is checkable without a GPU).
@@ -260,6 +269,7 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
   p.win = win ? win->rows : RowWindow{0, a->T, a->T};
   p.org = win ? win->org : nullptr;
+  const bool multi = win && win->multi.gens.models;     // a->w and a->bias are generator 0's, checked above
   fs2_conv1d_args rows = *a;
   rows.T = p.win.yend - p.win.y0;
   if (rows.T <= 0) return FS2_ERR_ARG;
@@ -273,7 +283,10 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   const dim3 grid((unsigned)plan.grid_x, (unsigned)plan.grid_y);
   prof_before(s);
 #define FS2_SIMT_ACT(BM_, BN_)                                                                            \
-  if (win) {                                                                                              \
+  if (multi) {                                                                                            \
+    if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_multi_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p, win->multi); \
+    else conv_simt_streams_multi_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p, win->multi);      \
+  } else if (win) {                                                                                       \
     if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); \
     else conv_simt_streams_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p);                        \
   } else {                                                                                                \

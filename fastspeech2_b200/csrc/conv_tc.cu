@@ -149,8 +149,15 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win)
   p.stage_off = pl.smem - (int)tc_stage_bytes(pl.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));   // the staged inputs end the budget
   p.win = win ? win->rows : RowWindow{0, a->T, a->T};
   p.org = win ? win->org : nullptr;
+  size_t smem = (size_t)pl.smem;
+  if (win && win->multi.gens.models) {                  // a->w_tc and a->bias are generator 0's: checked above, read per item below
+    if (nseg != 1) return FS2_ERR_UNSUPPORTED;           // one weight-scale header per item (TcGenSlot)
+    p.gens = win->multi.gens; p.wt_ref = win->multi.wt; p.bias_ref = win->multi.bias;
+    static_assert(226 * 1024 + TC_GEN_BYTES <= 227 * 1024, "the slot ring fits between the plan's budget and the opt-in");
+    p.gen_off = pl.smem;                                // the slot ring follows the plan's budget, within the 227 KB opt-in
+    smem += TC_GEN_BYTES;
+  }
   const unsigned grid = (unsigned)pl.grid;
-  const size_t smem = (size_t)pl.smem;
   const bool w = win != nullptr;
   prof_before(s);
   switch (pl.NB) {

@@ -77,7 +77,21 @@ struct TcP {
   int stage_off;                   // shared-memory byte offset of the staged epilogue inputs (used only if tc_stage_tiles(...) > 0)
   RowWindow win;                   // windowed mode (conv_tc_streams_kernel only): rows computed and read, see RowWindow
   const int* org;                  // the windowed mode's per-utterance origins, see origin_rows
+  Generators gens;                 // multi-generator mode (conv_tc_streams_multi_kernel only): wt and bias per work item, see GenRef
+  GenRef wt_ref, bias_ref;         // (bias stays the "has a bias" flag)
+  int gen_off;                     // multi-generator mode: shared-memory byte offset of the TcGenSlot ring, past the plan's budget
 };
+
+// Multi-generator mode: the weight producer resolves each work item's generator -- its tiles' weight-scale header and its bias -- into
+// a slot of a small shared-memory ring before it pushes the item's first weight stage, whose full barrier then publishes the slot to the
+// consumers; they read it in the item's epilogue (their own loads of it there push the 96-register warpgroups into spills).  The
+// producer runs at most TC_SB_MAX stages, so at most TC_SB_MAX items, ahead of an epilogue: TC_GEN_SLOTS > TC_SB_MAX + 1 slots.
+struct TcGenSlot { const float* bias; float inv_ws; int pad_; };
+constexpr int TC_GEN_SLOTS = 16;
+constexpr int TC_GEN_BYTES = TC_GEN_SLOTS * (int)sizeof(TcGenSlot);
+__device__ __forceinline__ TcGenSlot& tc_gen_slot(const TcP& p, unsigned char* smem, int k) {
+  return reinterpret_cast<TcGenSlot*>(smem + p.gen_off)[k % TC_GEN_SLOTS];
+}
 
 // Shared-memory epilogue tiles behind the ring barriers: [full, empty mbarrier per consumer warp][residual tile if res][sum tile if
 // accumulate or nseg > 1],
@@ -240,7 +254,9 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 // WIN: windowed mode with per-utterance origins, see WindowList and origin_rows: the tiles start at p.win.y0, rows at or beyond
 // p.win.yend are not written and rows at or beyond p.win.xend are not read (the host biases x, res and y by the window origins, so rows
 // are window rows here), and utterance b's rows outside [lo_b, hi_b) read as zero.
-template <int NB, bool RAG, bool WIN>
+// MULTI (with WIN): multi-generator mode: each work item reads the tiles, weight-scale header and bias of its utterance's generator
+// (p.gens), loaded once per item instead of once per CTA.
+template <int NB, bool RAG, bool WIN, bool MULTI = false>
 __device__ __forceinline__ void conv_tc_body(const TcP& p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -278,10 +294,18 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
     if (lane == 0) {
       const uint32_t stage_bytes = 2 * b_plane;   // one tap of one K-block (hi + lo)
       Ring rb;
-      for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
-        const int nblk = work.item(item).nblk;
+      for (int item = blockIdx.x, k = 0; item < work.count; item += gridDim.x, k++) {
+        const Item pit = work.item(item);
+        const int nblk = pit.nblk;
+        const float* wt = p.wt;
+        if constexpr (MULTI) {                         // before the item's first stage: its full barrier publishes the slot
+          wt = gen_weight(p.gens, pit.b, p.wt_ref);
+          TcGenSlot& gs = tc_gen_slot(p, smem_raw, k);
+          gs.inv_ws = __ldg(wt);
+          gs.bias = p.bias ? gen_weight(p.gens, pit.b, p.bias_ref) : nullptr;
+        }
         for (int seg = 0; seg < p.nseg; seg++) {
-          const unsigned char* src = reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes + TC_HDR +
+          const unsigned char* src = reinterpret_cast<const unsigned char*>(wt) + (long long)seg * p.seg_wbytes + TC_HDR +
                                      (size_t)nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
           for (int kb = 0; kb < KBLOCKS; kb++) {
             for (int tap = 0; tap < p.taps; tap += p.TPS) {
@@ -351,8 +375,13 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
         const float* bias = first ? p.bias : nullptr;
         const int* lens = last ? p.row_lens : nullptr;
         const bool use_res = last && p.res, sum_in = !first || p.accumulate, sum_out = !last;
-        const float inv_ws = p.nseg == 1 ? inv_ws0
+        float inv_ws = p.nseg == 1 ? inv_ws0
             : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes));
+        if constexpr (MULTI) {                         // this item's generator's, from the producer (one segment: checked on the host)
+          const TcGenSlot& gs = tc_gen_slot(p, smem_raw, (item - (int)blockIdx.x) / (int)gridDim.x);
+          inv_ws = gs.inv_ws;
+          if (bias) bias = gs.bias;
+        }
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
         switch (p.out_act) {                           // uniform branch: keeps tanhf out of the other variants' inner loops
           case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
@@ -486,9 +515,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_kernel(const Tc
   conv_tc_body<NB, true, true>(p);
 }
 
+// Multi-generator mode (fs2_vocoder_forward_streams_multi): the windowed mode with each item's weights from its stream's generator
+template <int NB>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_multi_kernel(const TcP p) {
+  conv_tc_body<NB, true, true, true>(p);
+}
+
 // The NB instantiations live in their own translation units (conv_tc_nb*.cu) so that the library builds in parallel.
 // conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.  window: the windowed mode
-// (conv_tc_streams_kernel).
+// (conv_tc_streams_kernel; conv_tc_streams_multi_kernel when p.gens.models is set).
 #define FS2_CONV_TC_NB_DECL(nb)                        \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes); \
   void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s);
@@ -500,10 +535,12 @@ FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CON
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes) {                                                  \
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
     if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_streams_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_streams_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+    return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_streams_multi_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
   }                                                                                                     \
   void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s) {   \
-    if (window) conv_tc_streams_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                          \
+    if (window && p.gens.models) conv_tc_streams_multi_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);   \
+    else if (window) conv_tc_streams_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                     \
     else if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                     \
     else conv_tc_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);                                  \
   }

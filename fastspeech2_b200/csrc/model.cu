@@ -89,7 +89,8 @@ int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_le
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
 int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win = nullptr, int x0 = 0, bool wide = false);
-int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, cudaStream_t s);
+int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, const int32_t* gen_in,
+              int n_gen, int32_t* gen, cudaStream_t s);
 int mel_ring_append(const fs2_mel_ring_append_args* a, cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out, bool wide = false);
@@ -546,7 +547,8 @@ struct View {
 // What a walk issues: the batch's mel view and lengths, the waveform, and five buffers, each B * width floats (window_plan).
 // org: NULL (the offline forward), or the windowed mode: the walk is then the unclipped plan of [0, frames), its rows are window rows,
 // utterance b's window starts at its frame org[b] (origin_rows), and the mel is the staged window buffer.  pre_tc: conv_pre's
-// tensor-core weights, or NULL where the caller's mel layout keeps conv_pre on the fp32 kernel.
+// tensor-core weights, or NULL where the caller's mel layout keeps conv_pre on the fp32 kernel.  gens (windowed mode only): the
+// multi-generator mode's generators and staged table (models NULL outside it); the walk plans and checks on m, generator 0.
 struct WinExec {
   int B; cudaStream_t s;
   const float* mel; int64_t mel_bs, mel_rs;
@@ -554,6 +556,7 @@ struct WinExec {
   const float* pre_tc;
   float* wav; int64_t wav_bs;
   float *bx, *bu, *bt, *r1, *r2;
+  Generators gens;
 };
 
 // fs2_conv1d arguments of a windowed launch: `cap` (a.T) is the layer's full logical length; residual off, as conv_args leaves it
@@ -582,7 +585,14 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   const int* org = ex ? ex->org : nullptr;
   auto len = [&](int scale) { return org ? ORIGIN_CAP : T * scale; };
   OriginWindow ow{};
-  auto win = [&](const RowWindow& w) -> const OriginWindow* { ow = OriginWindow{w, org}; return org ? &ow : nullptr; };
+  // g: the launch's weights as fields of fs2_vocoder_model, which the multi-generator mode reads per work item (GenLaunch)
+  const Generators gens = ex ? ex->gens : Generators{};
+  auto win = [&](const RowWindow& w, GenLaunch g) -> const OriginWindow* {
+    g.gens = gens;
+    ow = OriginWindow{w, org, gens.models ? g : GenLaunch{}};
+    return org ? &ow : nullptr;
+  };
+  auto ref = [&](const void* field, int add = 0) { return GenRef{(int32_t)((const char*)field - (const char*)m), add}; };
   // ---- backward: O[i + 1] = the rows stage i's output must hold (O[0]: conv_pre's), U[i] = its ResBlocks' input, Q[i] = the
   // ConvTranspose's phase-group rows
   Rows O[FS2_MAX_STAGES + 1], U[FS2_MAX_STAGES], Q[FS2_MAX_STAGES];
@@ -619,7 +629,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     fs2_conv1d_args c = win_conv_args(ex->mel, ex->mel_bs, ex->mel_rs, B, len(1), m->n_mel, bx, C, 7);
     c.w = m->w_pre; c.w_tc = ex->pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
     c.x_lens = lens; c.lens_scale = 1;
-    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi})));
+    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi}, GenLaunch{{}, ref(&m->w_pre), ref(&m->w_pre_tc), ref(&m->b_pre), 0, 0})));
   }
   const float inv_nk = 1.f / (float)m->n_kernels;
   for (int i = 0; i < n; i++) {
@@ -643,7 +653,9 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       c.bias = m->b_up[i] + off;
       c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
       c.x_lens = lens; c.lens_scale = s0;
-      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi})));
+      const GenLaunch gl{{}, ref(g == 0 ? &m->w_up_a[i] : &m->w_up_b[i]), ref(g == 0 ? &m->w_up_a_tc[i] : &m->w_up_b_tc[i]),
+                         ref(&m->b_up[i], (int)off), 0, 0};
+      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi}, gl)));
     }
     C = Co;
     const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
@@ -695,7 +707,8 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
             a.alpha = alpha; a.accumulate = accumulate;
           }
           a.x = r.p; a.y = dst.p;
-          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}), r.lo, C == 128));
+          const GenLaunch gl{{}, {}, {}, {}, i * m->n_kernels + (run.j < 0 ? 0 : run.j), run.j < 0 ? 0 : run.d0};
+          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}, gl), r.lo, C == 128));
         }
       } else {
         const int j = run.j, d = run.d0, rb = i * m->n_kernels + j, k = m->rb_k[j];
@@ -710,13 +723,15 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
           c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
           c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
           c.x_lens = lens; c.lens_scale = s1;
-          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi})));
+          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi},
+                                             GenLaunch{{}, ref(&m->w_rb1[rb][d]), ref(&m->w_rb1_tc[rb][d]), ref(&m->b_rb1[rb][d]), 0, 0})));
           c = win_conv_args(t.at(), t.bs(), C, B, len(s1), C, dst, C, k);
           c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
           c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
           c.alpha = alpha; c.accumulate = accumulate;
           c.x_lens = lens; c.lens_scale = s1;
-          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi})));
+          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi},
+                                             GenLaunch{{}, ref(&m->w_rb2[rb][d]), ref(&m->w_rb2_tc[rb][d]), ref(&m->b_rb2[rb][d]), 0, 0})));
         }
       }
       r = dst;
@@ -729,7 +744,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   p.x = bx.at(); p.B = B; p.T = len(sc[n]); p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
   p.wav = ex->wav - post.lo;                           // sample f0 * up is the caller's wav[0]
   p.lens = lens; p.lens_scale = sc[n];
-  return conv_post(&p, s, win({post.lo, post.hi, O[n].hi}), bx.bs(), ex->wav_bs);   // offline: the strides are its defaults
+  return conv_post(&p, s, win({post.lo, post.hi, O[n].hi}, GenLaunch{{}, ref(&m->w_post), {}, ref(&m->b_post), 0, 0}), bx.bs(), ex->wav_bs);   // offline: the strides are its defaults
 }
 
 // The plan of [0, frames) clipped at T (T < 0: unclipped, the bound of every window of `frames` frames), and the floats per utterance
@@ -765,8 +780,10 @@ static int vocoder_forward_impl(const fs2_vocoder_model* m, const fs2_vocoder_ar
 // fs2_vocoder_forward_window and _streams: the unclipped plan of [0, frames) once for the whole batch, each stream at its own origin.
 // The mel cone (conv_pre's input rows [x0, x1) of that plan) is staged first, [B][x1 - x0][n_mel], with the streams' origins and
 // lengths, so that conv_pre reads one batch-strided buffer and every launch the same two tables whichever call passed them.
+// mg (gen set): the multi-generator mode, whose staged generator table is a third one.
+struct MultiGen { const fs2_vocoder_model* models_dev; const int32_t* gen; int n; };
 static int vocoder_windowed_impl(const fs2_vocoder_model* m, const MelSource& src, int B, int frames, float* wav, int64_t wav_bs,
-                                 const float* pre_tc, cudaStream_t s, Arena& ar) {
+                                 const float* pre_tc, cudaStream_t s, Arena& ar, const MultiGen& mg = MultiGen{}) {
   std::vector<fs2_vocoder_window_launch_t> L;
   size_t width = 0;
   FS2_TRY(window_plan(m, -1, frames, L, width));
@@ -775,11 +792,12 @@ static int vocoder_windowed_impl(const fs2_vocoder_model* m, const MelSource& sr
   float* mel = ar.f32((size_t)B * rows * m->n_mel);
   int32_t* org = (int32_t*)ar.take((size_t)B * sizeof(int32_t));
   int32_t* lens = (int32_t*)ar.take((size_t)B * sizeof(int32_t));
+  int32_t* gen = mg.gen ? (int32_t*)ar.take((size_t)B * sizeof(int32_t)) : nullptr;
   WinExec ex{B, s, nullptr, (int64_t)rows * m->n_mel, m->n_mel, lens, org, pre_tc, wav, wav_bs,
-             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf)};
+             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), Generators{mg.gen ? mg.models_dev : nullptr, gen}};
   if (ar.dry) return FS2_OK;
-  if (!mel || !org || !lens || !ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
-  FS2_TRY(stage_mel(src, B, x0, rows, m->n_mel, mel, org, lens, s));
+  if (!mel || !org || !lens || (mg.gen && !gen) || !ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
+  FS2_TRY(stage_mel(src, B, x0, rows, m->n_mel, mel, org, lens, mg.gen, mg.n, gen, s));
   ex.mel = mel - (ptrdiff_t)x0 * m->n_mel;             // window row 0 of stream 0 (the conv reads rows [x0, x1) only)
   L.clear();
   return window_walk(m, -1, 0, frames, L, &ex);
@@ -1014,6 +1032,64 @@ int fs2_vocoder_forward_streams_ring(const fs2_vocoder_model* m, const fs2_vocod
 }
 
 int fs2_mel_ring_append(const fs2_mel_ring_append_args* a, fs2_stream_t st) { return mel_ring_append(a, S(st)); }
+
+static_assert(sizeof(fs2_vocoder_streams_multi_args) == 88,
+              "fs2_vocoder_streams_multi_args: fs2_vocoder_streams_ring_args' fields, gen and models_dev");
+
+// Generator k of a multi-generator call runs on generator 0's plan and kernels: the same architecture and masks, and every weight
+// pointer NULL where generator 0's is, else at the same address modulo 16 (the format choices and alignment checks made on generator 0).
+static bool same_generator_layout(const fs2_vocoder_model* a, const fs2_vocoder_model* b) {
+  if (a->n_mel != b->n_mel || a->c0 != b->c0 || a->n_stages != b->n_stages || a->n_kernels != b->n_kernels || a->n_dil != b->n_dil ||
+      a->f8_mask != b->f8_mask || a->fused_mask != b->fused_mask || a->pair_mask != b->pair_mask || a->pair_kmax != b->pair_kmax)
+    return false;
+  for (int i = 0; i < a->n_stages; i++)
+    if (a->rates[i] != b->rates[i] || a->up_k[i] != b->up_k[i]) return false;
+  for (int j = 0; j < a->n_kernels; j++) {
+    if (a->rb_k[j] != b->rb_k[j]) return false;
+    for (int d = 0; d < a->n_dil; d++)
+      if (a->rb_dil[j][d] != b->rb_dil[j][d]) return false;
+  }
+  auto same = [](const float* p, const float* q) { return !p == !q && ((uintptr_t)p & 15u) == ((uintptr_t)q & 15u); };
+  bool ok = same(a->w_pre, b->w_pre) && same(a->b_pre, b->b_pre) && same(a->w_post, b->w_post) && same(a->b_post, b->b_post) &&
+            same(a->w_pre_tc, b->w_pre_tc);
+  for (int i = 0; i < a->n_stages; i++)
+    ok = ok && same(a->w_up_a[i], b->w_up_a[i]) && same(a->w_up_b[i], b->w_up_b[i]) && same(a->b_up[i], b->b_up[i]) &&
+         same(a->w_up_a_tc[i], b->w_up_a_tc[i]) && same(a->w_up_b_tc[i], b->w_up_b_tc[i]);
+  for (int rb = 0; rb < a->n_stages * a->n_kernels; rb++)
+    for (int d = 0; d < a->n_dil; d++)
+      ok = ok && same(a->w_rb1[rb][d], b->w_rb1[rb][d]) && same(a->b_rb1[rb][d], b->b_rb1[rb][d]) && same(a->w_rb2[rb][d], b->w_rb2[rb][d]) &&
+           same(a->b_rb2[rb][d], b->b_rb2[rb][d]) && same(a->w_rb1_tc[rb][d], b->w_rb1_tc[rb][d]) && same(a->w_rb2_tc[rb][d], b->w_rb2_tc[rb][d]);
+  return ok;
+}
+
+static bool generators_ok(const fs2_vocoder_model* const* models, int n_models) {
+  if (!models || n_models < 1 || n_models > FS2_MAX_GENERATORS) return false;
+  for (int k = 0; k < n_models; k++)
+    if (!vocoder_ok(models[k]) || !same_generator_layout(models[0], models[k])) return false;
+  return true;
+}
+
+size_t fs2_vocoder_streams_multi_workspace_bytes(const fs2_vocoder_model* const* models, int n_models, int B, int frames) {
+  if (!generators_ok(models, n_models) || B <= 0 || frames <= 0 || !window_rows_ok(models[0], frames)) return 0;
+  Arena ar(nullptr, 0);
+  const MultiGen dry{nullptr, reinterpret_cast<const int32_t*>(16), n_models};   // a dry run counts the generator table's bytes only
+  if (vocoder_windowed_impl(models[0], MelSource{}, B, frames, nullptr, 0, nullptr, nullptr, ar, dry) != FS2_OK) return 0;
+  return ar.off + 256;
+}
+
+int fs2_vocoder_forward_streams_multi(const fs2_vocoder_model* const* models, int n_models, const fs2_vocoder_streams_multi_args* a,
+                                      fs2_stream_t st) {
+  if (!generators_ok(models, n_models) || !a || !a->gen || !a->models_dev) return FS2_ERR_ARG;
+  const fs2_vocoder_model* m = models[0];
+  if (a->B <= 0 || a->frames <= 0 || !window_rows_ok(m, a->frames)) return FS2_ERR_ARG;
+  if (!a->mel || !a->mel_lens || !a->f0 || !a->wav || !a->workspace) return FS2_ERR_ARG;
+  if (a->B > 1 && a->wav_batch_stride < a->frames * frame_rows(m, m->n_stages)) return FS2_ERR_ARG;
+  if (a->workspace_bytes < fs2_vocoder_streams_multi_workspace_bytes(models, n_models, a->B, a->frames)) return FS2_ERR_ARG;
+  const MelSource src{a->mel, nullptr, 0, 0, a->f0, 0, a->mel_lens, INT32_MAX, a->cap};
+  Arena ar(a->workspace, a->workspace_bytes);
+  return vocoder_windowed_impl(m, src, a->B, a->frames, a->wav, a->wav_batch_stride, m->w_pre_tc, S(st), ar,
+                               MultiGen{a->models_dev, a->gen, n_models});
+}
 
 static_assert(sizeof(fs2_resblock_run_t) == 32, "fs2_resblock_run_t: six int32 and a double");
 

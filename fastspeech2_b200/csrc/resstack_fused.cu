@@ -31,6 +31,7 @@
 // Roles: warps 0-7 two consumer warpgroups (conversion, MMAs, epilogues; thread 0 issues the tensor-map copies), warp 8 weight producer.
 #include <cuda.h>
 
+#include <cstddef>
 #include <type_traits>
 
 #include "tc_pipeline.cuh"
@@ -57,7 +58,19 @@ struct RsP {
   int x0;                            // windowed mode: window row of the x map's row 0 (the y map's row 0 is win.y0)
   RowWindow win;                     // windowed mode: rows computed (win.xend is not read: the x map ends the input)
   const int* org;                    // the windowed mode's per-utterance origins, see origin_rows
+  Generators gens; int rb, d0;       // multi-generator mode (the resstack_multi_*kernel entry points): conv[j][d]'s tiles and biases
+                                     // per work item, ResBlock rb + j's at dilation d0 + d of the item's generator (GenLaunch)
 };
+
+// Multi-generator mode: pair (j, d)'s conv c2 (0: dilated, 1: dilation 1) of utterance b's generator -- its tiles and its bias
+__device__ __forceinline__ RsConv rs_gen_conv(const RsP& p, RsConv cv, int b, int j, int d, int c2) {
+  const int slot = ((p.rb + j) * FS2_MAX_DIL + p.d0 + d) * (int)sizeof(void*);
+  const int w = (int)(c2 ? offsetof(fs2_vocoder_model, w_rb2_tc) : offsetof(fs2_vocoder_model, w_rb1_tc)) + slot;
+  const int bias = (int)(c2 ? offsetof(fs2_vocoder_model, b_rb2) : offsetof(fs2_vocoder_model, b_rb1)) + slot;
+  cv.w = reinterpret_cast<const unsigned char*>(gen_weight(p.gens, b, GenRef{w, 0}));
+  cv.b = gen_weight(p.gens, b, GenRef{bias, 0});
+  return cv;
+}
 
 // ------------------------------------------------------------------ TMA (tensor-map) wrappers
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* tm, int c0, int n0, int b, uint64_t* bar) {
@@ -113,7 +126,9 @@ __device__ __forceinline__ void rs_store2(unsigned char* slab, uint32_t chunk_by
 // results are never stored (the host sizes the x window to the stored rows' receptive field), and the y map clips the stores to the
 // window.  The zero fill covers only the buffer edges, so the slab rows of x below lo_b are zeroed like those at or past hi_b, and every
 // conv's rows outside [lo_b, hi_b) are held at zero as outside [0, n_b) offline.
-template <int CG, int C, int MT, bool RAG, bool WIN = false>
+// MULTI (with WIN): multi-generator mode, every work item streams the tiles and reads the weight-scale headers and biases of its
+// utterance's generator (rs_gen_conv).
+template <int CG, int C, int MT, bool RAG, bool WIN = false, bool MULTI = false>
 __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUtensorMap& tmy, const RsP& p) {
   constexpr int KB = C / 16, R = MT * 128, NJ = C / 8;                // NJ: 8-column fragment groups of a row
   constexpr int BOXC = CG < 32 ? CG : 32, NH = CG / BOXC;             // channels per TMA box, boxes across a row
@@ -157,11 +172,14 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
     // ===================== weight producer: every conv's stages once per work item and kernel size =====================
     if (lane == 0) {
       Ring rb;
-      for (int item = blockIdx.x; item < work.count; item += gridDim.x)
+      for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+        int b = 0;
+        if constexpr (MULTI) b = work.item(item).b;
         for (int j = 0; j < p.n_kernels; j++)
           for (int d = 0; d < p.n_dil; d++)
             for (int c2 = 0; c2 < 2; c2++) {
-              const RsConv cv = p.conv[j][d][c2];
+              RsConv cv = p.conv[j][d][c2];
+              if constexpr (MULTI) cv = rs_gen_conv(p, cv, b, j, d, c2);
               const unsigned char* src = cv.w + TC_HDR;   // tiles are ordered [kb][tap]: the taps of one K-block are contiguous
               for (int kb = 0; kb < KB; kb++)
                 for (int tap = 0; tap < cv.taps; tap += p.TPS) {
@@ -170,6 +188,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
                   src += bytes;
                 }
             }
+      }
     }
     return;
   }
@@ -251,8 +270,10 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
           ring_drain(emptyB, pend);
 #pragma unroll
           for (int i = 0; i < MT; i++) { wgmma_keep<C>(acc[i]); wgmma_keep<C>(corr[i]); }
-          // ---- epilogue straight from the fragments
-          const float inv_s = __ldg(reinterpret_cast<const float*>(cv.w));
+          // ---- epilogue straight from the fragments (in the multi-generator mode with the item's generator's header and bias, loaded
+          // only here so that they hold no register across the MMAs)
+          const RsConv ce = MULTI ? rs_gen_conv(p, cv, b, j, d, c2) : cv;
+          const float inv_s = __ldg(reinterpret_cast<const float*>(ce.w));
           // The same epilogue in two loop orders.  MT = 8 (the narrow widths) walks rows outer: with column groups outer, the 16 rows'
           // addresses and predicates stay live across both groups and push per-item state out of the 168 registers (stack spills).  The
           // wide widths keep column groups outer, the order their register allocation was tuned in.
@@ -271,7 +292,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
                     if (c2 == 0 || !last) rs_store2(c2 == 0 ? xt : xa, CHUNK, row, c, 0.f, 0.f);
                     continue;
                   }
-                  const float2 bv = __ldg(reinterpret_cast<const float2*>(cv.b + c));
+                  const float2 bv = __ldg(reinterpret_cast<const float2*>(ce.b + c));
                   const float s0 = acc[i][4 * jj + 2 * h] + corr[i][4 * jj + 2 * h], s1 = acc[i][4 * jj + 2 * h + 1] + corr[i][4 * jj + 2 * h + 1];
                   float v0 = fmaf(s0, inv_s, bv.x), v1 = fmaf(s1, inv_s, bv.y);
                   if (c2 == 0) {
@@ -301,7 +322,7 @@ __device__ __forceinline__ void resstack_body(const CUtensorMap& tmx, const CUte
                     for (int h = 0; h < 2; h++) rs_store2(c2 == 0 ? xt : xa, CHUNK, rbase + 64 * i + 8 * h, c, 0.f, 0.f);
                 continue;
               }
-              const float2 bv = __ldg(reinterpret_cast<const float2*>(cv.b + c));
+              const float2 bv = __ldg(reinterpret_cast<const float2*>(ce.b + c));
 #pragma unroll
               for (int i = 0; i < MT; i++)
 #pragma unroll
@@ -387,6 +408,22 @@ __global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_kernel(const __gr
 __global__ void __launch_bounds__(RS_THREADS, 1) resstack_wide_streams_kernel(const __grid_constant__ CUtensorMap tmx,
                                                                               const __grid_constant__ CUtensorMap tmy, const RsP p) {
   resstack_body<128, 128, 1, true, true>(tmx, tmy, p);
+}
+
+// Multi-generator mode (fs2_vocoder_forward_streams_multi) of the three windowed entry points above
+template <int C, int MT>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_multi_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                               const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<C, C, MT, true, true, true>(tmx, tmy, p);
+}
+template <int CG>
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_multi_narrow_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                                      const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<CG, 16, 8, true, true, true>(tmx, tmy, p);
+}
+__global__ void __launch_bounds__(RS_THREADS, 1) resstack_multi_wide_kernel(const __grid_constant__ CUtensorMap tmx,
+                                                                                    const __grid_constant__ CUtensorMap tmy, const RsP p) {
+  resstack_body<128, 128, 1, true, true, true>(tmx, tmy, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -505,6 +542,11 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_wide_streams_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_multi_kernel<32, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_multi_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_multi_narrow_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_multi_narrow_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(resstack_multi_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, mx);
     return e;
   }));
   RsP p{};
@@ -524,11 +566,20 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win
   p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
   p.x0 = x0; p.win = win ? win->rows : RowWindow{0, a->N, a->N};
   p.org = win ? win->org : nullptr;
+  if (win && win->multi.gens.models) {                 // a's tiles and biases are generator 0's, checked above
+    p.gens = win->multi.gens; p.rb = win->multi.rb; p.d0 = win->multi.d0;
+  }
   alignas(64) CUtensorMap tmx, tmy;
   FS2_TRY(make_map(&tmx, a->x, a->B, xrows, a->C, 128));
   FS2_TRY(make_map(&tmy, a->y, a->B, yrows, a->C, p.OBOX));
   prof_before(s);
-  if (win) {
+  if (win && p.gens.models) {
+    if (a->C == 32) resstack_multi_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 64) resstack_multi_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 128) resstack_multi_wide_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else if (a->C == 16) resstack_multi_narrow_kernel<16><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+    else resstack_multi_narrow_kernel<8><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
+  } else if (win) {
     if (a->C == 32) resstack_streams_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 64) resstack_streams_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 128) resstack_wide_streams_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);

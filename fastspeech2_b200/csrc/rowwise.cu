@@ -372,8 +372,18 @@ constexpr int CP_ROWS = 256;
 // Batch strides of x and wav and the rows computed and read: {T * C, T} and {0, T, T} outside the windowed mode (RowWindow; x / wav
 // are then biased by the windows' first rows).
 // org: NULL, or the windowed mode's per-utterance origins (origin_rows): rows and samples outside [lo_b, hi_b) read and write zero.
-struct PostRows { long long xbs, wbs; RowWindow win; const int* org; };
-template <bool ORG>
+// multi: the multi-generator mode's weights (the *_streams_multi_kernel entry points): w and bias of utterance b's generator.
+struct PostRows { long long xbs, wbs; RowWindow win; const int* org; GenLaunch multi; };
+// The conv's weights and bias: the call's, or in the multi-generator mode those of utterance b's generator
+template <bool MULTI>
+__device__ __forceinline__ void conv_post_weights(const fs2_conv_post_args& a, const PostRows& pr, int b, const float*& w, const float*& bias) {
+  w = a.w; bias = a.bias;
+  if constexpr (MULTI) {
+    w = gen_weight(pr.multi.gens, b, pr.multi.w);
+    bias = gen_weight(pr.multi.gens, b, pr.multi.bias);
+  }
+}
+template <bool ORG, bool MULTI = false>
 __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
   extern __shared__ float cp_smem[];
   const int C = a.C, ld = C + 1, pad = (a.taps - 1) / 2;
@@ -389,7 +399,9 @@ __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int t
     n_b = a.lens ? ragged_rows(a.lens, a.lens_scale, a.T, b) : a.T;   // ragged batch: rows >= n_b read as zero, wav there is 0
   }
   const int nin = min(n_b, pr.win.xend);
-  for (int i = threadIdx.x; i < a.taps * C; i += blockDim.x) wsm[i] = a.w[i];
+  const float *w, *bias;
+  conv_post_weights<MULTI>(a, pr, b, w, bias);
+  for (int i = threadIdx.x; i < a.taps * C; i += blockDim.x) wsm[i] = w[i];
   const int rows = CP_ROWS + a.taps - 1, C4 = C / 4;
   const float* xf = a.x + (long long)b * pr.xbs;
   const float4* xb = reinterpret_cast<const float4*>(xf);
@@ -420,7 +432,7 @@ __device__ __forceinline__ void conv_post_body(const fs2_conv_post_args a, int t
   __syncthreads();
   const int t = t0 + threadIdx.x;
   if (t >= pr.win.yend) return;
-  float acc = __ldg(a.bias);
+  float acc = __ldg(bias);
   for (int j = 0; j < a.taps; j++) {
     const float* xr = xs + (threadIdx.x + j) * ld;
     const float* wj = wsm + j * C;
@@ -437,6 +449,9 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_kernel(const fs2_conv_post_
 __global__ void __launch_bounds__(CP_ROWS) conv_post_streams_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
   conv_post_body<true>(a, tiles_per_batch, pr);
 }
+__global__ void __launch_bounds__(CP_ROWS) conv_post_streams_multi_kernel(const fs2_conv_post_args a, int tiles_per_batch, const PostRows pr) {
+  conv_post_body<true, true>(a, tiles_per_batch, pr);
+}
 
 // The generator's own shape (32 channels, 7 taps, hifigan/models.py:131): no shared memory at all.  Eight lanes own one time row (one
 // float4 of channels each: a warp reads 4 full 128-byte lines per load instruction, each row exactly once per group plus a 6-row halo),
@@ -446,8 +461,8 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post_streams_kernel(const fs2_co
 // B = 16 x 259k samples; this one is bound by the single read of x.)
 constexpr int CPF_BLOCKS = 18;                         // row blocks of TAPS rows per 8-lane group
 // RAG: ragged batch (a.lens != NULL); a template parameter so that the padded path keeps its code and registers.  ORG (with RAG): the
-// windowed mode's per-utterance origins.
-template <int TAPS, bool RAG, bool ORG>
+// windowed mode's per-utterance origins.  MULTI (with ORG): the multi-generator mode.
+template <int TAPS, bool RAG, bool ORG, bool MULTI = false>
 __device__ __forceinline__ void conv_post_c32_body(const fs2_conv_post_args a, int groups_per_batch, long long n_groups, const PostRows pr) {
   constexpr int PAD = (TAPS - 1) / 2, ROWS = CPF_BLOCKS * TAPS - 2 * PAD;     // output rows per group (120 for 7 taps: a multiple of 8)
   static_assert(ROWS % 8 == 0, "full 8-sample stores");
@@ -467,10 +482,12 @@ __device__ __forceinline__ void conv_post_c32_body(const fs2_conv_post_args a, i
     n_b = RAG ? ragged_rows(a.lens, a.lens_scale, T, b) : T;   // ragged batch: rows >= n_b read as zero, wav there is 0
   }
   const int nin = min(n_b, pr.win.xend);
+  const float *wp, *bp;
+  conv_post_weights<MULTI>(a, pr, b, wp, bp);
   float4 w[TAPS];
 #pragma unroll
-  for (int j = 0; j < TAPS; j++) w[j] = __ldg(reinterpret_cast<const float4*>(a.w + j * 32) + sub);
-  const float bias = __ldg(a.bias), slope = a.in_slope;
+  for (int j = 0; j < TAPS; j++) w[j] = __ldg(reinterpret_cast<const float4*>(wp + j * 32) + sub);
+  const float bias = __ldg(bp), slope = a.in_slope;
   const float4* xb = reinterpret_cast<const float4*>(a.x + (long long)b * pr.xbs) + sub;
   float* wb = a.wav + (long long)b * pr.wbs;
   float s[TAPS];
@@ -525,6 +542,11 @@ __global__ void __launch_bounds__(256) conv_post_c32_streams_kernel(const fs2_co
                                                                     const PostRows pr) {
   conv_post_c32_body<TAPS, true, true>(a, groups_per_batch, n_groups, pr);
 }
+template <int TAPS>
+__global__ void __launch_bounds__(256) conv_post_c32_streams_multi_kernel(const fs2_conv_post_args a, int groups_per_batch, long long n_groups,
+                                                                          const PostRows pr) {
+  conv_post_c32_body<TAPS, true, true, true>(a, groups_per_batch, n_groups, pr);
+}
 
 // win (with a->lens): NULL, or the windowed mode (OriginWindow; a->T is not used, a->x and a->wav are biased by the windows' first rows
 // and their batch strides are x_bs and wav_bs).  Both kernels add every output's taps in the same order wherever its tile starts.
@@ -532,8 +554,9 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
   if (!a || !a->x || !a->w || !a->bias || !a->wav || a->B <= 0 || a->T <= 0 || a->C <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
   if (win && !a->lens) return FS2_ERR_ARG;
-  const PostRows pr = win ? PostRows{x_bs, wav_bs, win->rows, win->org}
-                          : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr};
+  const PostRows pr = win ? PostRows{x_bs, wav_bs, win->rows, win->org, win->multi}
+                          : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr, GenLaunch{}};
+  const bool multi = win && win->multi.gens.models;     // a->w and a->bias are generator 0's, checked above
   const int rows = pr.win.yend - pr.win.y0;
   if (rows <= 0) return FS2_ERR_ARG;
   if (a->C == 32 && a->taps == 7 && (reinterpret_cast<uintptr_t>(a->x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15u) == 0) {
@@ -542,7 +565,8 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
     const long long n_groups = (long long)gpb * a->B, blocks = (n_groups * 8 + 255) / 256;
     if (blocks > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
     prof_before(s);
-    if (win) conv_post_c32_streams_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    if (multi) conv_post_c32_streams_multi_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    else if (win) conv_post_c32_streams_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     prof_after(s, 3, 2.0 * (double)a->B * rows * a->taps * a->C);
@@ -555,7 +579,8 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
   const long long n = (long long)a->B * rows;
   if ((long long)tiles * a->B > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   prof_before(s);
-  if (win) conv_post_streams_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
+  if (multi) conv_post_streams_multi_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
+  else if (win) conv_post_streams_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   else conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   prof_after(s, 3, 2.0 * n * a->taps * a->C);
   FS2_LAUNCH_CHECK();
@@ -566,11 +591,22 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
 // out[b][r] = stream b's mel row o_b + x0 + r for r < rows, zeros where that row lies outside [0, n_b), with o_b and n_b the origin and
 // length of MelSource; org[b] = o_b and lens[b] = n_b.  The one kernel that reads the caller's mel and lengths, so the window kernels
 // after it see one batch-strided buffer and two tables.  n_mel % 4 == 0 and 16-byte aligned rows (float4 loads); rows outside the
-// utterance are never dereferenced, and a ring's rows are read at t mod ring[b] only.
-__global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, int n4, float4* out, int* org, int* lens, long long total) {
+// utterance are never dereferenced, and a ring's rows are read at t mod ring[b] only.  MULTI: gen[b] = stream b's generator index
+// gen_in[b], or 0 -- and length 0 -- for one outside [0, n_gen), so that the window kernels index the generators with it unchecked.
+template <bool MULTI>
+__device__ __forceinline__ void stage_mel_body(const MelSource& src, int B, int x0, int rows, int n4, float4* out, int* org, int* lens,
+                                               const int* gen_in, int n_gen, int* gen, long long total) {
   auto origin = [&](int b) { return src.f0s ? __ldg(src.f0s + b) : src.f0; };
+  auto gen_ok = [&](int b) {
+    if constexpr (MULTI) {
+      const int g = __ldg(gen_in + b);
+      return g >= 0 && g < n_gen;
+    }
+    return true;
+  };
   auto length = [&](int b) {
     if (src.ring && __ldg(src.ring + b) <= 0) return 0;
+    if (!gen_ok(b)) return 0;
     return src.lens ? min(max(__ldg(src.lens + b), 0), src.cap) : src.cap;
   };
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -585,19 +621,34 @@ __global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, i
       v = __ldg(reinterpret_cast<const float4*>(row) + c4);
     }
     out[i] = v;
-    if (i < B) { org[i] = origin((int)i); lens[i] = length((int)i); }
+    if (i < B) {
+      org[i] = origin((int)i); lens[i] = length((int)i);
+      if constexpr (MULTI) gen[i] = gen_ok((int)i) ? __ldg(gen_in + i) : 0;
+    }
   }
 }
+__global__ void stage_mel_kernel(const MelSource src, int B, int x0, int rows, int n4, float4* out, int* org, int* lens, long long total) {
+  stage_mel_body<false>(src, B, x0, rows, n4, out, org, lens, nullptr, 0, nullptr, total);
+}
+__global__ void stage_mel_multi_kernel(const MelSource src, int B, int x0, int rows, int n4, float4* out, int* org, int* lens,
+                                       const int* gen_in, int n_gen, int* gen, long long total) {
+  stage_mel_body<true>(src, B, x0, rows, n4, out, org, lens, gen_in, n_gen, gen, total);
+}
 
-int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, cudaStream_t s) {
+// gen: NULL, or the multi-generator mode's staged table of gen_in's n_gen generators (src.table set)
+int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, const int32_t* gen_in,
+              int n_gen, int32_t* gen, cudaStream_t s) {
   if (!(src.table || src.mel) || (src.ring && !src.table) || !out || !org || !lens || B <= 0 || rows <= 0 || n_mel <= 0) return FS2_ERR_ARG;
+  if (gen && !(gen_in && src.table)) return FS2_ERR_ARG;
   if (n_mel % 4 || !aligned16(out) || (!src.table && ((src.bs | src.rs) & 3))) return FS2_ERR_UNSUPPORTED;
   if (!src.table && !aligned16(src.mel)) return FS2_ERR_ARG;
   const long long total = (long long)B * rows * (n_mel / 4);
   const long long blocks = (total + 255) / 256;
   prof_before(s);
-  stage_mel_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(src, B, x0, rows, n_mel / 4, reinterpret_cast<float4*>(out),
-                                                                             org, lens, total);
+  const unsigned grid = (unsigned)(blocks < 4096 ? blocks : 4096);
+  if (gen)
+    stage_mel_multi_kernel<<<grid, 256, 0, s>>>(src, B, x0, rows, n_mel / 4, reinterpret_cast<float4*>(out), org, lens, gen_in, n_gen, gen, total);
+  else stage_mel_kernel<<<grid, 256, 0, s>>>(src, B, x0, rows, n_mel / 4, reinterpret_cast<float4*>(out), org, lens, total);
   prof_after(s, 3, 0.0);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

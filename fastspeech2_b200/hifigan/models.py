@@ -317,7 +317,7 @@ class Generator(nn.Module):
                         "fs2_vocoder_forward_window")
                 yield f0 * up, wav
 
-    def stream_pool(self, chunk_frames=64, sample_rate=None, pcm16=False):
+    def stream_pool(self, chunk_frames=64, sample_rate=None, pcm16=False, generators=()):
         """A pool of independent streams vocoded together (fs2_vocoder_forward_streams), for serving requests that arrive at different
         times: StreamPool.add(mel) admits a stream, and every StreamPool.step() synthesises the next `chunk_frames` frames of every live
         stream in one call, each at its own position.  Concatenated, one stream's chunks equal self(mel[None]) bit for bit, whatever else
@@ -333,22 +333,65 @@ class Generator(nn.Module):
 
         A stream whose mel arrives in pieces: h = pool.open(); pool.feed(h, block) as blocks arrive; pool.close(h) after the last.
         Its chunks, concatenated, equal self(cat(blocks)[None]) (and the conversion of that) bit for bit; its mel is held in a ring
-        of StreamPool.ring_frames rows that depends on chunk_frames only, filled by one fs2_mel_ring_append launch per step."""
+        of StreamPool.ring_frames rows that depends on chunk_frames only, filled by one fs2_mel_ring_append launch per step.
+
+        generators: more generators of this one's architecture (fine-tuned voices, or the reference's LJSpeech and universal
+        checkpoints), vocoded in the same calls: the pool's generators are (self, *generators), and StreamPool.add / open take the
+        index of a stream's generator (0, self, by default).  A stream's chunks then equal generators[k](mel[None]) bit for bit,
+        whatever the other streams' generators, and a step still makes one call with the launches of a one-generator step
+        (fs2_vocoder_forward_streams_multi).  Each must match self in its config (upsample_*, resblock_*, sampling_rate),
+        effective_masks(), use_tensor_cores, wide_pairs and device, and be in eval mode; ValueError otherwise, and for more than
+        L.MAX_GENERATORS in all.  Each is packed once, here."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
         rs = self._resampler(sample_rate, chunk_frames)
         if self.training:
             raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
         dev = get(self, "conv_pre.bias").device
+        gens = (self, *generators)
+        self._check_pool_generators(gens, dev)
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
-            m, keep, dev, up = self._packed or self._pack()
+            packs = [g._packed or g._pack() for g in gens]
+        m, keep, dev, up = packs[0]
         lib = L.lib()
         ws = [None]
+        models = L.model_array([p[0] for p in packs])
+        # the generators' structs in device memory, read per work item by the multi-generator call (one upload, at its first call)
+        models_dev = [None]
 
-        def launch(ptrs, f0s, ns, caps=None):
+        def launch_multi(ptrs, f0s, ns, caps, gen):
+            """One fs2_vocoder_forward_streams_multi call: stream b vocoded by generator gen[b] (its ring of caps[b] rows with caps)."""
+            B, n = len(ptrs), chunk_frames * up
+            with torch.cuda.device(dev):
+                if models_dev[0] is None:
+                    models_dev[0] = torch.frombuffer(bytearray(b"".join(bytes(p[0]) for p in packs)), dtype=torch.uint8).to(dev)
+                host = torch.empty((5 if caps is None else 6) * B, dtype=torch.int32, pin_memory=True)
+                h = host.numpy()
+                h[:2 * B].view(np.int64)[:] = ptrs
+                h[2 * B:3 * B] = f0s
+                h[3 * B:4 * B] = ns
+                h[4 * B:5 * B] = gen
+                if caps is not None:
+                    h[5 * B:] = caps
+                table = host.to(dev, non_blocking=True)
+                need = lib.fs2_vocoder_streams_multi_workspace_bytes(models, len(packs), B, chunk_frames)
+                if ws[0] is None or ws[0].numel() < need:
+                    ws[0] = torch.empty(need, dtype=torch.uint8, device=dev)
+                wav = torch.empty(B, n, dtype=torch.float32, device=dev)
+                base = table.data_ptr()
+                a = L.VocoderStreamsMultiArgs(B=B, frames=chunk_frames, mel=base, mel_lens=base + 12 * B, f0=base + 8 * B, wav=wav.data_ptr(),
+                                              wav_batch_stride=n, workspace=ws[0].data_ptr(), workspace_bytes=ws[0].numel(),
+                                              cap=0 if caps is None else base + 20 * B, gen=base + 16 * B, models_dev=models_dev[0].data_ptr())
+                L.check(lib.fs2_vocoder_forward_streams_multi(models, len(packs), C.byref(a), torch.cuda.current_stream(dev).cuda_stream),
+                        "fs2_vocoder_forward_streams_multi")
+            return wav
+
+        def launch(ptrs, f0s, ns, caps=None, gens=None):
             """One fs2_vocoder_forward_streams call on the current stream (fs2_vocoder_forward_streams_ring with caps): uploads the
             (pointer, f0, n[, cap]) table from a fresh pinned block with one non_blocking copy (the caching host allocator keeps the
-            block until the copy is done; no host sync)."""
+            block until the copy is done; no host sync).  gens (a pool of several generators): fs2_vocoder_forward_streams_multi."""
+            if gens is not None:
+                return launch_multi(ptrs, f0s, ns, caps, gens)
             B, n = len(ptrs), chunk_frames * up
             with torch.cuda.device(dev):
                 host = torch.empty((4 if caps is None else 5) * B, dtype=torch.int32, pin_memory=True)
@@ -392,9 +435,28 @@ class Generator(nn.Module):
         fs = _cfg(self.h, "sampling_rate")
         resample.rs = rs or Resampler(fs, fs)
         pool = StreamPool(launch, m.n_mel, up, chunk_frames, dev, resample=resample, encoding="pcm16" if pcm16 else "f32", append=append,
-                          reach=mel_reach(m, chunk_frames))
-        pool._keep = keep                              # the packed weights stay alive while the pool runs
+                          reach=mel_reach(m, chunk_frames), n_generators=len(gens))
+        pool._keep = (packs, models, models_dev)       # the packed weights and the model tables stay alive while the pool runs
         return pool
+
+    def _check_pool_generators(self, gens, dev):
+        """ValueError unless every generator can share self's plan in one stream pool (stream_pool's generators)."""
+        if len(gens) > L.MAX_GENERATORS:
+            raise ValueError(f"a stream pool takes at most {L.MAX_GENERATORS} generators, got {len(gens)}")
+        keys = ("upsample_rates", "upsample_kernel_sizes", "upsample_initial_channel", "resblock", "resblock_kernel_sizes",
+                "resblock_dilation_sizes", "sampling_rate")
+        for k, g in enumerate(gens[1:], 1):
+            if not isinstance(g, Generator):
+                raise ValueError(f"generators[{k}] is not a hifigan Generator")
+            if g.training:
+                raise ValueError(f"generators[{k}] is in training mode: call .eval()")
+            if any(str(_cfg(g.h, n)) != str(_cfg(self.h, n)) for n in keys):
+                raise ValueError(f"generators[{k}] has another architecture or sampling rate than generators[0]")
+            if (g.effective_masks() != self.effective_masks() or bool(g.use_tensor_cores) != bool(self.use_tensor_cores)
+                    or bool(g.wide_pairs) != bool(self.wide_pairs)):
+                raise ValueError(f"generators[{k}]'s masks, use_tensor_cores or wide_pairs differ from generators[0]'s")
+            if get(g, "conv_pre.bias").device != dev:
+                raise ValueError(f"generators[{k}] is on {get(g, 'conv_pre.bias').device}, generators[0] on {dev}")
 
 
 def mel_reach(m, chunk_frames):
@@ -433,9 +495,13 @@ class StreamPool:
     address src, to row (dst_frame + i) mod cap of the [cap, n_mel] ring at address ring (fs2_mel_ring_append).  reach = (left, right):
     the mel frames a chunk [f0, f0 + chunk_frames) reads before f0 and past its end (mel_reach).  In a step in which a stream opened
     with open() takes part, launch is called as launch(ptrs, f0s, ns, caps=caps): stream b's frame t at row t mod caps[b] of ptrs[b]
-    (caps[b] = ns[b] for an add()ed stream, which never wraps)."""
+    (caps[b] = ns[b] for an add()ed stream, which never wraps).
 
-    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None, encoding="f32", append=None, reach=(0, 0)):
+    n_generators: the generators the launch call serves (Generator.stream_pool's generators).  With more than one, add() and open()
+    take each stream's generator index, and launch is called with gens=[the live streams' indices] as a keyword; a one-generator
+    pool calls launch(ptrs, f0s, ns[, caps]) as above."""
+
+    def __init__(self, launch, n_mel, up, chunk_frames, device, resample=None, encoding="f32", append=None, reach=(0, 0), n_generators=1):
         self._launch, self.n_mel, self.up, self.chunk_frames, self.device = launch, n_mel, up, chunk_frames, torch.device(device)
         self._resample = resample
         rs = getattr(resample, "rs", None)
@@ -444,8 +510,9 @@ class StreamPool:
         self._append, self.reach = append, tuple(reach)
         # an open stream's ring holds the cone of its current chunk: the frames written last are at most f0 + chunk_frames + right
         self.ring_frames = -(-(self.reach[0] + chunk_frames + self.reach[1]) // 8) * 8
+        self.n_generators = n_generators
         # [handle, channels-last mel view [n, n_mel] (an open stream: its ring [ring_frames, n_mel]), n (an open stream: the frames fed
-        #  so far), next frame, last chunk, emitted, Resampler or None, encoding, _Feed (None for an add()ed stream)]
+        #  so far), next frame, last chunk, emitted, Resampler or None, encoding, _Feed (None for an add()ed stream), generator index]
         self._live = []
         self._next = 0
 
@@ -474,12 +541,19 @@ class StreamPool:
         """The stream takes its slice of the waveform: its rate is the waveform's and its encoding fp32."""
         return (s[6] is None or s[6].identity) and s[7] == L.RESAMPLE_F32
 
-    def add(self, mel, sample_rate=None, encoding=None):
+    def _generator(self, generator):
+        """A new stream's generator index, checked against the pool's generators."""
+        if isinstance(generator, bool) or not isinstance(generator, int) or not 0 <= generator < self.n_generators:
+            raise ValueError(f"generator must be an int in [0, {self.n_generators}), got {generator!r}")
+        return generator
+
+    def add(self, mel, sample_rate=None, encoding=None, generator=0):
         """Admits a stream.  mel: [n_mel, n] or [1, n_mel, n] on the pool's device, n >= 1.  A channels-last view with row stride n_mel
         (FastSpeech2's postnet_mel[b, :n].T is one) is kept without a copy; any other layout is converted once.  sample_rate and encoding
         ("f32", "pcm16", "ulaw" or "alaw"): the stream's output format, None for the pool's.  ValueError for a rate Resampler refuses, a
         resampler history longer than chunk_frames * up, an unknown encoding, or a ninth distinct output rate among the live streams.
-        Returns the handle."""
+        generator: the index of the stream's generator in the pool's (ValueError outside them).  Returns the handle."""
+        generator = self._generator(generator)
         if not isinstance(mel, torch.Tensor):
             raise ValueError("mel must be a tensor")
         if mel.dim() == 3 and mel.shape[0] == 1:
@@ -495,7 +569,7 @@ class StreamPool:
         rows = mel.T
         if not (rows.dtype == torch.float32 and rows.stride(1) == 1 and (n == 1 or rows.stride(0) == self.n_mel) and rows.data_ptr() % 16 == 0):
             rows = rows.to(torch.float32).contiguous()
-        return self._admit(rows, n, rs, enc, None)
+        return self._admit(rows, n, rs, enc, None, generator)
 
     def _format(self, sample_rate, encoding):
         """A new stream's (Resampler or None, encoding), checked as add() documents."""
@@ -506,22 +580,23 @@ class StreamPool:
             raise ValueError(f"the live streams already use {len(rates)} output rates; at most {L.RESAMPLE_MAX_FILTERS}")
         return rs, enc
 
-    def _admit(self, rows, n, rs, enc, feed):
+    def _admit(self, rows, n, rs, enc, feed, generator):
         h = self._next
         self._next += 1
-        self._live.append([h, rows, n, 0, None, 0, rs, enc, feed])
+        self._live.append([h, rows, n, 0, None, 0, rs, enc, feed, generator])
         return h
 
-    def open(self, sample_rate=None, encoding=None):
+    def open(self, sample_rate=None, encoding=None, generator=0):
         """Admits a stream whose mel has not arrived yet: feed(h, block) appends frames, close(h) fixes its length.  It takes part in a
         step once its next chunk's cone has arrived, and concatenated its chunks equal those of add() on the concatenated blocks bit
-        for bit.  Its mel lives in a ring of ring_frames rows, whatever its length.  sample_rate and encoding as in add().  ValueError
-        in a pool without an append call.  Returns the handle."""
+        for bit.  Its mel lives in a ring of ring_frames rows, whatever its length.  sample_rate, encoding and generator as in add().
+        ValueError in a pool without an append call.  Returns the handle."""
+        generator = self._generator(generator)
         if self._append is None:
             raise ValueError("this pool has no append call: it cannot take open streams")
         rs, enc = self._format(sample_rate, encoding)
         ring = torch.empty(self.ring_frames, self.n_mel, dtype=torch.float32, device=self.device)
-        return self._admit(ring, 0, rs, enc, _Feed())
+        return self._admit(ring, 0, rs, enc, _Feed(), generator)
 
     def _open_stream(self, h):
         for s in self._live:
@@ -590,11 +665,12 @@ class StreamPool:
         if not live:
             return []
         ptrs, f0s, ns = [s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live]
+        gens = {} if self.n_generators == 1 else {"gens": [s[9] for s in live]}
         if any(s[8] is not None for s in live):
             self._fill(live)
-            wav = self._launch(ptrs, f0s, ns, caps=[n if s[8] is None else self.ring_frames for s, n in zip(live, ns)])
+            wav = self._launch(ptrs, f0s, ns, caps=[n if s[8] is None else self.ring_frames for s, n in zip(live, ns)], **gens)
         else:
-            wav = self._launch(ptrs, f0s, ns)
+            wav = self._launch(ptrs, f0s, ns, **gens)
         rows = [(wav, i) for i in range(len(live))]     # where each stream's chunk is: (rows, index)
         starts = [s[3] * self.up for s in live]
         widths = [min(self.chunk_frames, s[2] - s[3]) * self.up for s in live]
@@ -641,7 +717,7 @@ class StreamPool:
         records = []
         for i in conv:
             s = live[i]
-            _, _, n, f0, prev, emitted, rs, enc, feed = s
+            _, _, n, f0, prev, emitted, rs, enc, feed, _ = s
             i1, N = f0 * self.up, n * self.up              # an open stream: N covers every input its ready outputs read
             is_open = feed is not None and not feed.closed
             r = rs.ready(min(i1 + n1, N), None if is_open else N, not is_open and f0 + self.chunk_frames >= n)

@@ -545,6 +545,37 @@ typedef struct fs2_vocoder_streams_ring_args {
 } fs2_vocoder_streams_ring_args;
 int fs2_vocoder_forward_streams_ring(const fs2_vocoder_model* m, const fs2_vocoder_streams_ring_args* a, fs2_stream_t stream);
 
+/* Streams of several generators in one call: fs2_vocoder_forward_streams_ring (cap may be NULL: no rings, as
+ * fs2_vocoder_forward_streams), but stream b is vocoded with generator gen[b] of models[0 .. n_models): its output equals that call with
+ * models[gen[b]] alone bit for bit, whatever the other streams' generators.  The generators share one architecture and weight format
+ * (fine-tuned copies of one checkpoint, or V1 checkpoints trained apart), so the call plans once, on models[0]: its launches, grid and
+ * launch count are those of fs2_vocoder_forward_streams at the same B and frames, and every work item reads its own stream's weights.
+ *   - models_dev: a device copy of the n_models structs models points at (the pointers inside are device pointers anyway); the kernels
+ *     read each weight's pointer from models_dev[gen[b]], so it must stay equal to the host array while the call runs;
+ *   - the host never reads gen: the staging launch clamps it with the origin and length tables, and a stream whose gen[b] lies outside
+ *     [0, n_models) gets an all-zero chunk (as cap[b] <= 0 does) without changing the other streams;
+ *   - FS2_ERR_ARG before any CUDA call for n_models outside [1, FS2_MAX_GENERATORS], a NULL model, gen or models_dev, and a model whose
+ *     architecture (n_mel, c0, stages, rates, up_k, ResBlock kernels and dilations), masks (f8_mask, fused_mask, pair_mask, pair_kmax) or
+ *     weight format differs from models[0]'s -- every weight pointer must be NULL where models[0]'s is (which *_tc tiles exist, and so
+ *     which convs, conv_pre included, take the tensor cores) and otherwise lie at the same address modulo 16; then the checks of
+ *     fs2_vocoder_forward_streams.  The workspace bound, fs2_vocoder_streams_multi_workspace_bytes (0 for models the call refuses), is
+ *     fs2_vocoder_streams_workspace_bytes of models[0] plus the staged generator table. */
+#define FS2_MAX_GENERATORS 8
+typedef struct fs2_vocoder_streams_multi_args {
+  int B, frames;
+  const float* const* mel;        /* [B] device array: stream b's mel rows (its ring of cap[b] rows when cap is set) */
+  const int32_t* mel_lens;        /* [B] device */
+  const int32_t* f0;              /* [B] device */
+  float* wav; int64_t wav_batch_stride;
+  void* workspace; size_t workspace_bytes;
+  const int32_t* cap;             /* [B] device, or NULL */
+  const int32_t* gen;             /* [B] device: stream b's generator index */
+  const fs2_vocoder_model* models_dev;   /* [n_models] device copy of the models' structs */
+} fs2_vocoder_streams_multi_args;
+size_t fs2_vocoder_streams_multi_workspace_bytes(const fs2_vocoder_model* const* models, int n_models, int B, int frames);
+int fs2_vocoder_forward_streams_multi(const fs2_vocoder_model* const* models, int n_models, const fs2_vocoder_streams_multi_args* a,
+                                      fs2_stream_t stream);
+
 /* Appending arriving mel frames to rings, every stream's in one launch: record r copies `count` frames, source frame src_frame + i at
  * src + (src_frame + i) * frame_stride + c * channel_stride (floats) for channel c, to ring row (dst_frame + i) mod cap of `ring`
  * ([cap][n_mel] channels-last, 16-byte aligned), for i < count.  Any strides: FastSpeech2's postnet_mel[b] is frame_stride n_mel,
@@ -681,7 +712,8 @@ const char* fs2_build_info(void);          /* "sm_90a ..." */
  * structs (fs2_resample_args 88, fs2_resample_window_args 144, fs2_resample_stream_t 64, fs2_resample_streams_args 64 bytes; added at
  * ABI 12 without a bump, since no existing struct changed; then fs2_resample_filter_t 24, fs2_resample_mixed_stream_t 80 and
  * fs2_resample_mixed_args 232 bytes, likewise; then fs2_vocoder_streams_ring_args 72, fs2_mel_ring_record_t 56 and
- * fs2_mel_ring_append_args 24 bytes, likewise) are not in the table: the binding pins their sizes. */
+ * fs2_mel_ring_append_args 24 bytes, likewise; then fs2_vocoder_streams_multi_args 88 bytes, likewise) are not in the table: the
+ * binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

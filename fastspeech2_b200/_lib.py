@@ -283,7 +283,7 @@ assert C.sizeof(ResampleMixedArgs) == RESAMPLE_MIXED_ARGS_SIZE
 
 
 class ConvTcPlan(C.Structure):
-    _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem")]
+    _fields_ = [(n, i32) for n in ("NB", "TG", "SA", "SB", "TPS", "R", "acc_regs", "tiles_per_batch", "n_items", "grid", "smem", "NG")]
 
 
 class ConvSimtPlan(C.Structure):
@@ -311,7 +311,8 @@ EXPORTS = {
     "fs2_conv_tc_block": (i32, [i32]),
     "fs2_conv_tc_block_f8": (i32, [i32]),
     # plan queries write a ConvTcPlan / ConvSimtPlan / ResstackPlan; the out pointer stays untyped so that a caller's int32 buffer of
-    # the plan's layout (the fields in order, as ABI 11 returned them) is still accepted
+    # the plan's layout (the fields in order) is accepted.  ConvTcPlan has twelve int32 since NG was appended: a buffer of the eleven
+    # earlier fields is too small (fs2_struct_size(16) gives the size; ABI_VERSION did not change with it)
     "fs2_conv_tc_plan": (i32, [C.POINTER(Conv1dArgs), i32, C.c_void_p]),
     "fs2_conv_simt_plan": (i32, [C.POINTER(Conv1dArgs), i32, C.c_void_p]),
     "fs2_layernorm": (i32, [C.POINTER(LayerNormArgs), fp]),

@@ -77,13 +77,28 @@ static int conv_tc_plan(const fs2_conv1d_args* a, int nseg, int num_sms, fs2_con
   while (fixed + sa * a_stage + sb * b_stage > budget && sa > 2) sa--;
   while (fixed + sa * a_stage + sb * b_stage > budget && sb > 2) sb--;
   if (fixed + sa * a_stage + sb * b_stage > budget) return FS2_ERR_UNSUPPORTED;
-  p.SA = sa; p.SB = sb;
-  p.smem = (int)(fixed + sa * a_stage + sb * b_stage);   // [slab stages][weight stages][ring barriers][staged inputs]
   p.tiles_per_batch = (a->T + 127) / 128;
   const long long n_items = (long long)(a->N / p.NB) * a->B * p.tiles_per_batch;
   if (n_items > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   p.n_items = (int)n_items;
-  p.grid = n_items < num_sms ? (int)n_items : num_sms;
+  // Channel-block groups: a work item computes NG blocks from one resident slab (all kblocks stages), so the transform warps load and
+  // split each input tile once instead of N / NB times, and read it from HBM once.  The largest NG that fits the budget with a weight ring
+  // of >= 2 stages, keeps >= 4 waves of items (the tail wave's idle SMs stay <= 1/4 of the launch) and divides the blocks.
+  p.NG = 1;
+  const int nblocks = a->N / p.NB;
+  if (nseg == 1 && kblocks <= TC_SA_MAX)
+    for (int ng = nblocks; ng > 1 && p.NG == 1; ng--) {
+      if (nblocks % ng || n_items / ng < 4LL * num_sms) continue;
+      int gsa = TC_SA_MAX, gsb = sb;
+      while (fixed + gsa * a_stage + gsb * b_stage > budget && gsa > kblocks) gsa--;
+      while (fixed + gsa * a_stage + gsb * b_stage > budget && gsb > 2) gsb--;
+      if (fixed + gsa * a_stage + gsb * b_stage > budget) continue;
+      p.NG = ng; sa = gsa; sb = gsb;
+    }
+  p.SA = sa; p.SB = sb;
+  p.smem = (int)(fixed + sa * a_stage + sb * b_stage);   // [slab stages][weight stages][ring barriers][staged inputs]
+  const long long ctas = n_items / p.NG;
+  p.grid = ctas < num_sms ? (int)ctas : num_sms;
   return FS2_OK;
 }
 
@@ -145,17 +160,17 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win)
   p.x_lens = a->x_lens; p.lens_scale = a->lens_scale;   // the plan below stays the padded one: the host never reads device lengths
   fs2_conv_tc_plan_t pl{};
   FS2_TRY(conv_tc_plan(plan_args, nseg, g_num_sms, pl));
-  p.SA = pl.SA; p.SB = pl.SB; p.TPS = pl.TPS; p.R = pl.R; p.tiles_per_batch = pl.tiles_per_batch; p.n_items = pl.n_items;
+  p.SA = pl.SA; p.SB = pl.SB; p.TPS = pl.TPS; p.R = pl.R; p.tiles_per_batch = pl.tiles_per_batch;
+  p.NG = pl.NG; p.n_items = pl.n_items / pl.NG;         // the kernel's items: tiles x groups of NG channel blocks
   p.stage_off = pl.smem - (int)tc_stage_bytes(pl.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));   // the staged inputs end the budget
   p.win = win ? win->rows : RowWindow{0, a->T, a->T};
   p.org = win ? win->org : nullptr;
-  size_t smem = (size_t)pl.smem;
+  static_assert(226 * 1024 + TC_SLOT_BYTES <= 227 * 1024, "the slot ring fits between the plan's budget and the opt-in");
+  p.slot_off = pl.smem;                                 // the unit slot ring (TcSlot) follows the plan's budget, within the 227 KB opt-in
+  const size_t smem = (size_t)pl.smem + TC_SLOT_BYTES;
   if (win && win->multi.gens.models) {                  // a->w_tc and a->bias are generator 0's: checked above, read per item below
-    if (nseg != 1) return FS2_ERR_UNSUPPORTED;           // one weight-scale header per item (TcGenSlot)
+    if (nseg != 1) return FS2_ERR_UNSUPPORTED;           // one weight-scale header per unit (TcSlot)
     p.gens = win->multi.gens; p.wt_ref = win->multi.wt; p.bias_ref = win->multi.bias;
-    static_assert(226 * 1024 + TC_GEN_BYTES <= 227 * 1024, "the slot ring fits between the plan's budget and the opt-in");
-    p.gen_off = pl.smem;                                // the slot ring follows the plan's budget, within the 227 KB opt-in
-    smem += TC_GEN_BYTES;
   }
   const unsigned grid = (unsigned)pl.grid;
   const bool w = win != nullptr;

@@ -12,8 +12,8 @@
 // ABSOLUTE error < 3e-8).  Emulated end to end on the CPU (exact accumulation) this split is as accurate as fp32 convolution
 // on both the synthetic and the shipped HiFi-GAN checkpoint; on the GPU the tensor core's truncating accumulator is what remains.
 //
-// Persistent, warp-specialised kernel: one CTA per SM walks a list of work items (one 128-row time tile of one utterance x one
-// block of NB <= 128 output channels); four roles overlap through mbarrier rings:
+// Persistent, warp-specialised kernel: one CTA per SM walks a list of work items (one 128-row time tile of one utterance x NG
+// blocks of NB <= 128 output channels); four roles overlap through mbarrier rings:
 //   warp 8      weight producer: every (tap, 16-channel K-block) weight stage is ONE cp.async.bulk (TMA bulk engine) of a
 //               host-pre-split, host-pre-tiled smem image  [hi|lo][16-byte K-chunk][n][8 halfs].
 //   warps 9-16  activation transform: read the [128 + (taps-1)*dil] x 16-channel slab of a K-block ONCE from global
@@ -21,6 +21,9 @@
 //               split hi/lo and store both in the no-swizzle K-major layout [16-byte K-chunk][row][8 halfs].  There a core
 //               matrix (8 rows x 16 B) starting at ANY row is 128 contiguous bytes, so each conv tap is just the same slab with
 //               the descriptor start address advanced by tap*dil rows: the slab is loaded and split once per K-block, not once per tap.
+//               With NG > 1 the item's Cin/16 K-block slabs stay resident (SA >= Cin/16, one plan field) while the consumers run
+//               the K loop once per channel block, so the slab is loaded and split once per tile rather than once per block, and
+//               the tile's input is read from global once; each stage is released on the item's last block (ring_release_last).
 //   warps 0-7   two consumer warpgroups, 64 output rows each: per weight stage 3 (split terms) wgmma m64nNBk16 with register
 //               accumulators (or one FP16 + one E4M3 K = 32 MMA, TcP::f8), then the epilogue straight from the accumulator
 //               fragments: bias / activation / residual / alpha / accumulate / pad-row mask -> global stores.  The residual and
@@ -65,7 +68,7 @@ struct TcP {
   int SA, SB;                      // ring depths
   int TPS;                         // conv taps per weight stage (small NB: several taps share one bulk copy / one handshake)
   int R;                           // slab rows held in smem (>= 128 + (taps-1)*dil, R % 8 == 4)
-  int tiles_per_batch, n_items;    // work items of the padded shape: per utterance ceil(T / 128), in all (N/NB) * B * tiles_per_batch
+  int tiles_per_batch, n_items;    // work items of the padded shape: per utterance ceil(T / 128), in all (N/(NG*NB)) * B * tiles_per_batch
   int nseg;                       // K-segments per output tile (1 = plain conv).  > 1: the conv is the sum of nseg one-tap slices over p.Cin (= 256)
                                    // input channels each, slice s = (tap = s / seg_nkc, channel chunk = s % seg_nkc); every slice is its own work unit with a
                                    // fresh accumulator, and the units of one tile run back to back on one CTA, adding into y in fp32 (FS2_TC_VARIANT_SEGMENTED)
@@ -79,18 +82,20 @@ struct TcP {
   const int* org;                  // the windowed mode's per-utterance origins, see origin_rows
   Generators gens;                 // multi-generator mode (conv_tc_streams_multi_kernel only): wt and bias per work item, see GenRef
   GenRef wt_ref, bias_ref;         // (bias stays the "has a bias" flag)
-  int gen_off;                     // multi-generator mode: shared-memory byte offset of the TcGenSlot ring, past the plan's budget
+  int slot_off;                    // shared-memory byte offset of the TcSlot ring, past the plan's budget
+  int NG;                          // NB-channel blocks per work item, computed one after another from the item's slab (see conv_tc_body)
 };
 
-// Multi-generator mode: the weight producer resolves each work item's generator -- its tiles' weight-scale header and its bias -- into
-// a slot of a small shared-memory ring before it pushes the item's first weight stage, whose full barrier then publishes the slot to the
-// consumers; they read it in the item's epilogue (their own loads of it there push the 96-register warpgroups into spills).  The
-// producer runs at most TC_SB_MAX stages, so at most TC_SB_MAX items, ahead of an epilogue: TC_GEN_SLOTS > TC_SB_MAX + 1 slots.
-struct TcGenSlot { const float* bias; float inv_ws; int pad_; };
-constexpr int TC_GEN_SLOTS = 16;
-constexpr int TC_GEN_BYTES = TC_GEN_SLOTS * (int)sizeof(TcGenSlot);
-__device__ __forceinline__ TcGenSlot& tc_gen_slot(const TcP& p, unsigned char* smem, int k) {
-  return reinterpret_cast<TcGenSlot*>(smem + p.gen_off)[k % TC_GEN_SLOTS];
+// The weight producer decodes each unit (work item, channel block) -- its tile and block, and its generator's weight-scale header and
+// bias in the multi-generator mode -- into a slot of a small shared-memory ring before it pushes the unit's first weight stage, whose
+// full barrier then publishes the slot to the consumers; they read it in the unit's epilogue.  So the consumer warpgroups hold no
+// work-list cursor (with one, the ragged and windowed cursors' state pushes the 96-register warpgroups into spills).  The producer runs
+// at most TC_SB_MAX stages, so at most TC_SB_MAX units, ahead of an epilogue: TC_SLOTS > TC_SB_MAX + 1 slots.
+struct TcSlot { Item it; const float* bias; float inv_ws; int pad_; };
+constexpr int TC_SLOTS = 16;
+constexpr int TC_SLOT_BYTES = TC_SLOTS * (int)sizeof(TcSlot);
+__device__ __forceinline__ TcSlot& tc_slot(const TcP& p, unsigned char* smem, int u) {
+  return reinterpret_cast<TcSlot*>(smem + p.slot_off)[u % TC_SLOTS];
 }
 
 // Shared-memory epilogue tiles behind the ring barriers: [full, empty mbarrier per consumer warp][residual tile if res][sum tile if
@@ -180,8 +185,9 @@ struct TcStage {
   static __device__ __forceinline__ float* sum_tile(const TcP& p, unsigned char* smem) {
     return res_tile(p, smem) + (p.res ? tc_stage_tile_bytes(NB) / 4 : 0);
   }
-  // Staging warp, work item `it`: for each consumer warp w, once w has released its rows of the previous item, bulk-copy the residual /
-  // old y rows of its 16 tile rows below it.rows (one copy per row and tile), completing on full[w].  `phase`: parity of this CTA's item.
+  // Staging warp, channel block it.nblk of a work item: for each consumer warp w, once w has released its rows of the previous block, bulk-copy
+  // the residual / old y rows of its 16 tile rows below it.rows (one copy per row and tile), completing on full[w].  `phase`: parity of
+  // this CTA's (item, block) count.
   static __device__ __forceinline__ void fill(const TcP& p, unsigned char* smem, const Item& it, uint32_t phase) {
     const int lane = threadIdx.x & 31;
     const uint32_t row_bytes = NB * 4, per_row = (p.res ? row_bytes : 0u) + (p.accumulate ? row_bytes : 0u);
@@ -276,6 +282,7 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
+  const int NG = p.NG;
   // 128-row tiles x NB-channel blocks; windowed: item.rows bounds the stores, the transform warps bound their loads at min(hi_b, xend)
   std::conditional_t<WIN, WindowList, WorkList<RAG>> work;
   if constexpr (WIN) work.init(p.x_lens, p.org, p.lens_scale, p.B, 128, p.n_items / (p.B * p.tiles_per_batch), p.win.y0, p.win.yend, p.win.yend);
@@ -294,24 +301,31 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
     if (lane == 0) {
       const uint32_t stage_bytes = 2 * b_plane;   // one tap of one K-block (hi + lo)
       Ring rb;
-      for (int item = blockIdx.x, k = 0; item < work.count; item += gridDim.x, k++) {
+      const float inv_ws0 = __ldg(p.wt);               // header: 1 / (power-of-two weight scale)
+      for (int item = blockIdx.x, u = 0; item < work.count; item += gridDim.x) {
         const Item pit = work.item(item);
-        const int nblk = pit.nblk;
         const float* wt = p.wt;
-        if constexpr (MULTI) {                         // before the item's first stage: its full barrier publishes the slot
+        const float* bias = p.bias;
+        float inv_ws = inv_ws0;
+        if constexpr (MULTI) {                         // the item's generator's
           wt = gen_weight(p.gens, pit.b, p.wt_ref);
-          TcGenSlot& gs = tc_gen_slot(p, smem_raw, k);
-          gs.inv_ws = __ldg(wt);
-          gs.bias = p.bias ? gen_weight(p.gens, pit.b, p.bias_ref) : nullptr;
+          bias = p.bias ? gen_weight(p.gens, pit.b, p.bias_ref) : nullptr;
+          inv_ws = __ldg(wt);
         }
-        for (int seg = 0; seg < p.nseg; seg++) {
-          const unsigned char* src = reinterpret_cast<const unsigned char*>(wt) + (long long)seg * p.seg_wbytes + TC_HDR +
-                                     (size_t)nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
-          for (int kb = 0; kb < KBLOCKS; kb++) {
-            for (int tap = 0; tap < p.taps; tap += p.TPS) {
-              const uint32_t bytes = (uint32_t)min(p.TPS, p.taps - tap) * stage_bytes;
-              ring_push(fullB, emptyB, rb, SB, b_base + (size_t)rb.idx * p.TPS * stage_bytes, src, bytes);
-              src += bytes;
+        for (int j = 0; j < NG; j++, u++) {            // the item's blocks, in the consumers' order
+          TcSlot& slot = tc_slot(p, smem_raw, u);       // before the unit's first stage: its full barrier publishes the slot
+          slot.it = Item{pit.nblk * NG + j, pit.b, pit.t0, pit.rows};
+          slot.bias = bias;
+          slot.inv_ws = inv_ws;
+          for (int seg = 0; seg < p.nseg; seg++) {
+            const unsigned char* src = reinterpret_cast<const unsigned char*>(wt) + (long long)seg * p.seg_wbytes + TC_HDR +
+                                       (size_t)slot.it.nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
+            for (int kb = 0; kb < KBLOCKS; kb++) {
+              for (int tap = 0; tap < p.taps; tap += p.TPS) {
+                const uint32_t bytes = (uint32_t)min(p.TPS, p.taps - tap) * stage_bytes;
+                ring_push(fullB, emptyB, rb, SB, b_base + (size_t)rb.idx * p.TPS * stage_bytes, src, bytes);
+                src += bytes;
+              }
             }
           }
         }
@@ -322,10 +336,13 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
     // Every operand is a precomputed descriptor base plus a constant.
     const int g = warp >> 2;                             // 64-row half of the tile
     const uint64_t a_const = wgmma_desc(0, (uint32_t)R * 16, 128), b_const = wgmma_desc(0, (uint32_t)NB * 16, 128);
-    const float inv_ws0 = __ldg(p.wt);                 // header: 1 / (power-of-two weight scale)
     Ring ra, rb;
-    for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
-      const Item it = work.item(item);
+    // This CTA's units (work item, channel block): the item's NG blocks one after another, each a full pass over the item's slab stages
+    // (NG > 1: nseg == 1 and SA >= KBLOCKS, planned on the host).  Every pass but the last rewinds the slab cursor and keeps the stages
+    // full.  The unit's tile and block come from the producer's slot (TcSlot).
+    const int units = (work.count - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x * NG;
+    for (int unit = 0, blk = 0; unit < units; unit++, blk = blk == NG - 1 ? 0 : blk + 1) {   // blk: the unit's block in its item
+      const bool last_pass = blk == NG - 1;
       for (int seg = 0; seg < p.nseg; seg++) {
         float acc[TG][NB / 2];
 #pragma unroll
@@ -357,7 +374,7 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
                 }
               }
             });
-            if (pend_a >= 0) { tc_release(&emptyA[pend_a]); pend_a = -1; }   // its last group retired in ring_step
+            ring_release_last(emptyA, pend_a, last_pass);   // its last group retired in ring_step
           }
           pend_a = (int)sa;
         }
@@ -365,23 +382,22 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
 #pragma unroll
         for (int gg = 0; gg < TG; gg++) wgmma_keep<NB>(acc[gg]);
         if (pend_b >= 0) tc_release(&emptyB[pend_b]);
-        if (pend_a >= 0) tc_release(&emptyA[pend_a]);
+        ring_release_last(emptyA, pend_a, last_pass);
+        if (!last_pass) ra.rewind(SA, KBLOCKS);
         // K-segmented conv: unit (item, seg) adds slice seg of the tile into the sum tile -- bias with the first slice; residual,
         // alpha-free sum, the pad-row mask and the store to y with the last.  The same thread owns the same outputs in every unit, so the
         // fp32 read-modify-write of the sum tile needs no further ordering.  No output activation (checked on the host).
         const bool first = seg == 0, last = seg == p.nseg - 1;
-        // the staging barrier completes one phase per work item of this CTA (phase parity from the item index: no register held)
-        if (staged && first) mbar_wait(Stage::full(p, smem_raw, warp), (uint32_t)((item - (int)blockIdx.x) / (int)gridDim.x) & 1u);
-        const float* bias = first ? p.bias : nullptr;
+        const TcSlot& slot = tc_slot(p, smem_raw, unit);
+        const Item it = slot.it;
+        // the staging barrier completes one phase per unit of this CTA
+        if (staged && first) mbar_wait(Stage::full(p, smem_raw, warp), (uint32_t)unit & 1u);
+        const float* bias = first ? slot.bias : nullptr;
         const int* lens = last ? p.row_lens : nullptr;
         const bool use_res = last && p.res, sum_in = !first || p.accumulate, sum_out = !last;
-        float inv_ws = p.nseg == 1 ? inv_ws0
+        // header: 1 / (power-of-two weight scale) of the unit's generator (multi-generator mode: one segment, checked on the host)
+        const float inv_ws = p.nseg == 1 ? slot.inv_ws
             : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes));
-        if constexpr (MULTI) {                         // this item's generator's, from the producer (one segment: checked on the host)
-          const TcGenSlot& gs = tc_gen_slot(p, smem_raw, (item - (int)blockIdx.x) / (int)gridDim.x);
-          inv_ws = gs.inv_ws;
-          if (bias) bias = gs.bias;
-        }
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
         switch (p.out_act) {                           // uniform branch: keeps tanhf out of the other variants' inner loops
           case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
@@ -396,10 +412,13 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
       }
     }
   } else if (warp == TC_THREADS / 32 - 1) {
-    // ===================== staging warp: residual / old-y rows of each work item -> shared memory (TcStage) =====================
+    // ===================== staging warp: residual / old-y rows of each work item and block -> shared memory (TcStage) ================
     if (staged) {
       uint32_t phase = 0;
-      for (int item = blockIdx.x; item < work.count; item += gridDim.x, phase ^= 1u) Stage::fill(p, smem_raw, work.item(item), phase);
+      for (int item = blockIdx.x; item < work.count; item += gridDim.x) {
+        const Item it = work.item(item);
+        for (int j = 0; j < NG; j++, phase ^= 1u) Stage::fill(p, smem_raw, Item{it.nblk * NG + j, it.b, it.t0, it.rows}, phase);
+      }
     }
   } else {
     // ===================== transform warps (activation + fp16 hi/lo split) =====================

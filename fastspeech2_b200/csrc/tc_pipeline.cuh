@@ -91,6 +91,11 @@ struct Ring {
   __device__ __forceinline__ void advance(uint32_t n) {
     if (++idx == n) { idx = 0; phase ^= 1u; }
   }
+  // back over the last `steps` <= n stages: the next pass of a consumer that reads them more than once (ring_release_last)
+  __device__ __forceinline__ void rewind(uint32_t n, uint32_t steps) {
+    if (idx < steps) { idx += n; phase ^= 1u; }
+    idx -= steps;
+  }
 };
 
 // One thread initialises the barrier pairs of an n-stage ring; mbar_init_fence() then orders every init before the barriers' use.
@@ -125,6 +130,14 @@ __device__ __forceinline__ void ring_step(uint64_t* full, uint64_t* empty, const
   wgmma_wait<1>();
   if (pend >= 0) tc_release(&empty[pend]);
   pend = (int)r.idx;
+}
+
+// Consumer that reads a span of stages in several passes (the conv's slab: once per channel block of a work item): pend, a stage whose
+// reads have retired, is released only on the last pass, so the producer cannot refill it while a later pass still needs it; earlier
+// passes find it still full (the same phase) after Ring::rewind.  The ring needs at least as many stages as the span.
+__device__ __forceinline__ void ring_release_last(uint64_t* empty, int& pend, bool last) {
+  if (pend >= 0 && last) tc_release(&empty[pend]);
+  pend = -1;
 }
 
 // After at least one ring_step: waits for every wgmma group and releases the last stage; then wgmma_keep the accumulators.

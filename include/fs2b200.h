@@ -74,17 +74,19 @@ enum { FS2_TC_VARIANT_F8 = 1,
 int fs2_conv_tc_block(int N);    /* 0 when N is not supported by the tensor-core kernel */
 int fs2_conv_tc_block_f8(int N); /* the same for FS2_TC_VARIANT_F8 tiles: the largest multiple of 16 <= 64 that divides N (N itself if N <= 64) */
 struct fs2_conv1d_args;
-/* Launch plan of the tensor-core kernel; a work item is one 128-row tile x NB output channels. */
+/* Launch plan of the tensor-core kernel; a work item is one 128-row tile x NG blocks of NB output channels, computed one block after
+ * another from the tile's input slab, which stays in shared memory (SA >= C_in / 16 when NG > 1). */
 typedef struct fs2_conv_tc_plan_t {
-  int32_t NB;              /* output channels per work item */
+  int32_t NB;              /* output channels per block */
   int32_t TG;              /* accumulators per tile: 1 = all split terms together, 2 = {hi*hi | the cross terms} */
   int32_t SA, SB;          /* activation slab stages, weight stages */
   int32_t TPS;             /* conv taps per weight stage */
   int32_t R;               /* slab rows */
   int32_t acc_regs;        /* accumulator registers per consumer thread */
-  int32_t tiles_per_batch; /* work items per utterance and channel block */
-  int32_t n_items, grid;   /* work items (of the padded shape), CTAs */
+  int32_t tiles_per_batch; /* 128-row tiles per utterance */
+  int32_t n_items, grid;   /* (tile, block) pairs of the padded shape, i.e. NG x the work items; CTAs */
   int32_t smem;            /* dynamic shared memory bytes */
+  int32_t NG;              /* channel blocks per work item */
 } fs2_conv_tc_plan_t;
 /* The plan the tensor-core kernel would use for this call on a device with num_sms SMs (pure host logic, no CUDA call, pointers are
  * only checked for alignment).  Returns FS2_ERR_UNSUPPORTED for shapes the kernel does not take. */

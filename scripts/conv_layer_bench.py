@@ -1,7 +1,7 @@
 """Warm timings of single fs2_conv1d layers on the tensor-core kernel, grouped by epilogue: plain (LeakyReLU out), residual, and
 residual + accumulate into y (the last conv of every ResBlock after the first), at the shapes the vocoder runs through per-layer
-launches (stages 0 and 1 of HiFi-GAN V1: B = 16 x 1 017 mel frames, every kernel size and dilation), plus the K-segmented convs of
-an encoder FFT block.  The same layer with and without the residual / accumulate input shows what reading those costs.
+launches (stages 0 and 1 of HiFi-GAN V1: B = 16 x 1 017 mel frames, every kernel size and dilation, and the two stages'
+ConvTranspose phase groups), plus the K-segmented convs of an encoder FFT block.  The same layer with and without the residual / accumulate input shows what reading those costs.
 
 usage: python scripts/conv_layer_bench.py [--quick] [other.so ...]
   other.so: further builds of libfs2b200.so (same ABI) timed on the same inputs, alternating with the in-tree library
@@ -67,6 +67,20 @@ def vocoder_layer(stage, C, up, k, dil, f8, mode, n=10):
     report(f"s{stage} C={C:3d} k={k:2d} dil={dil} {'f16+f8' if f8 else 'split3':6s} {mode:7s}", timed(fn, n), 2.0 * B * N * C * C * k)
 
 
+def upsample_group(stage, Cin, rows, rate, n=10):
+    """one ConvTranspose1d phase group as the vocoder runs it: LeakyReLU in, 2 taps, Cin -> (rate / 2) * Cin / 2 channels at the stage's
+    input rows (T0 * rows), f16 + f8"""
+    T, N = T0 * rows, (rate // 2) * (Cin // 2)
+    x = torch.randn(B, T, Cin, generator=g).to(DEV)
+    w = torch.randn(2, Cin, N, generator=g) * (Cin * 2) ** -0.5
+    b = torch.randn(N, generator=g).to(DEV) * 0.05
+    wt = packing.pack_conv_tc(w, f8=True).to(DEV)
+    wd = w.to(DEV)
+    y = torch.empty(B, T, N, device=DEV)
+    fn = lambda: ops.conv1d(x, wd, b, pad_left=1, in_act=3, in_slope=0.1, out=y, w_tc=wt, backend=2, tc_variant=1)
+    report(f"s{stage} upsample group Cin={Cin} N={N} k=2 f16+f8", timed(fn, n), 2.0 * B * T * Cin * N * 2)
+
+
 def segmented_layer(label, T, Cin, N, k, res, n=20):
     """K-segmented encoder conv (FS2_TC_VARIANT_NB64 | SEGMENTED): every (tap, 256-channel) slice is one work unit summed in fp32"""
     x = torch.randn(B, T, Cin, generator=g).to(DEV)
@@ -87,6 +101,8 @@ for stage, C, up in ((0, 256, 8), (1, 128, 64)):
         for dil in ((1,) if quick else (1, 3, 5)):
             for mode in ("plain", "res", "res+acc"):
                 vocoder_layer(stage, C, up, k, dil, True, mode)
+for stage, Cin, rows in ((0, 512, 1), (1, 256, 8)):      # the ConvTranspose phase groups of stages 0 and 1 (rate 8 each)
+    upsample_group(stage, Cin, rows, 8)
 for mode in ("plain", "res", "res+acc"):                 # split-fp16 at 128 output channels per work item
     vocoder_layer(1, 128, 64, 11, 1, False, mode)
 segmented_layer("enc ffn1 256->1024 k=9 segmented", 128, 256, 1024, 9, False)

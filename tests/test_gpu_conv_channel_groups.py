@@ -1,14 +1,16 @@
 """GPU: channel-block groups (fs2_conv_tc_plan_t::NG) change which CTA computes a block, never the bits.
 
 A conv planned at NG = 2 must equal, bit for bit, the same conv computed one 64-channel block at a time (N = 64 per launch: one block,
-so NG = 1), in the padded layout with every epilogue mode.  The windowed entry points are checked through Generator: stream() in one
+so NG = 1), each block's launch reading its tiles from the same packed buffer, in the padded layout with every epilogue mode.  Plans
+are made with the device's own SM count.  The windowed entry points are checked through Generator: stream() in one
 window whose 128-channel stage is planned at NG = 2 against short windows planned at NG = 1, and a multi-generator pool large enough
 for NG = 2 against each stream's own forward."""
 import pytest
 import torch
 
 from fastspeech2_b200 import _lib as L, configs, ops, packing, synth
-from tests.test_conv_channel_groups_cpu import _plan
+from tests.test_conv_channel_groups_cpu import _plan as _plan_at
+from tests.test_gpu_conv_groups import block_tiles, device_sms
 from tests.test_gpu_stream_multi import _run
 from tests.test_gpu_stream_vocoder import _generator, _streamed
 
@@ -16,10 +18,13 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
 
-def _conv(x, w, b, dil, res, y, alpha, acc, out_act):
+def _plan(*a, **k):
+    return _plan_at(*a, num_sms=device_sms(), **k)
+
+
+def _conv(x, w, b, dil, res, y, alpha, acc, out_act, w_tc):
     ops.conv1d(x, w, b, dilation=dil, pad_left=(w.shape[0] - 1) * dil // 2, in_act=L.ACT_LRELU, in_slope=0.1, out_act=out_act,
-               out_slope=0.1, res=res, alpha=alpha, out=y, accumulate=acc, w_tc=packing.pack_conv_tc(w.cpu(), f8=True).to(DEV),
-               backend=L.CONV_TC, tc_variant=L.TC_VARIANT_F8)
+               out_slope=0.1, res=res, alpha=alpha, out=y, accumulate=acc, w_tc=w_tc, backend=L.CONV_TC, tc_variant=L.TC_VARIANT_F8)
 
 
 @pytest.mark.parametrize("k,dil", [(3, 1), (11, 5)])
@@ -36,10 +41,11 @@ def test_grouped_blocks_equal_one_block_per_launch(k, dil, mode):
     y0 = torch.randn(Bn, T, C, generator=g).to(DEV)
     acc, alpha, out_act = mode == "res+acc", (1 / 3 if mode == "res+acc" else 1.0), (L.ACT_LRELU if mode == "plain" else L.ACT_NONE)
     grouped, split = y0.clone(), y0.clone()
-    _conv(x, w, b, dil, res, grouped, alpha, acc, out_act)
+    w_tc = packing.pack_conv_tc(w.cpu(), f8=True).to(DEV)
+    _conv(x, w, b, dil, res, grouped, alpha, acc, out_act, w_tc)
     for n in (0, 64):
         _conv(x, w[:, :, n:n + 64].contiguous(), b[n:n + 64], dil, None if res is None else res[:, :, n:n + 64], split[:, :, n:n + 64],
-              alpha, acc, out_act)
+              alpha, acc, out_act, block_tiles(w_tc, n // 64, k, C, 64))
     torch.cuda.synchronize()
     assert torch.equal(grouped, split)
 

@@ -13,6 +13,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib as L
+from .. import _streams
 from .. import ops, packing
 from .._modtree import get, populate
 from ..resample import ENCODINGS, Resampler
@@ -72,7 +73,8 @@ class Generator(nn.Module):
                 v = get(self, base + ".weight_v")
                 get(self, base + ".weight_g").copy_(v.reshape(v.shape[0], -1).norm(dim=1).reshape(-1, *([1] * (v.dim() - 1))))
         self._packed = None
-        self._ws = None
+        self._packed_state = None      # _streams.StreamState of the packed weights: made on the stream of the call that packed them
+        self._ws, self._ws_stream = None, None     # the last forward's workspace and the stream it was allocated on (_streams.workspace)
 
     # ------------------------------------------------------------------ weight-norm handling
     def _bases(self):
@@ -103,8 +105,10 @@ class Generator(nn.Module):
         self._invalidate()
 
     def _invalidate(self):
+        if self._packed is not None:
+            self._packed_state.release(*self._packed[1].values())
         self._packed = None
-        self._ws = None
+        self._ws = self._ws_stream = None
 
     def load_state_dict(self, *a, **k):
         out = super().load_state_dict(*a, **k)
@@ -184,7 +188,14 @@ class Generator(nn.Module):
         for u in hd["upsample_rates"]:
             up *= u
         self._packed = (m, pk, dev, up)
+        self._packed_state = _streams.made(dev)
         return self._packed
+
+    def _packed_on_stream(self):
+        """_packed (packing it first if needed), ready on the current stream."""
+        packed = self._packed or self._pack()
+        self._packed_state.enter()
+        return packed
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
@@ -196,7 +207,12 @@ class Generator(nn.Module):
         at or beyond mel_lens[b] are never read, the vocoder skips the work of the padding, and wav[b, 0, t] = 0 for
         t >= mel_lens[b] * prod(upsample_rates).  The output shape stays [B, 1, prod(upsample_rates) * T].  Without mel_lens every
         utterance is synthesised over all T frames, padding included, as the reference does.  A CPU tensor is range-checked
-        (ValueError outside [0, T]); device values are clamped to [0, T] by the kernels."""
+        (ValueError outside [0, T]); device values are clamped to [0, T] by the kernels.
+
+        CUDA streams: the call enqueues all of its device work on the stream current at the call.  Its workspace is cached for the next
+        call on the same stream only: a call on another stream allocates its own, so calls on two streams never share one.  x, mel_lens
+        and the returned waveform follow torch's usual rule: the caller orders them across streams.  The weights packed by the first
+        call are ready on whatever stream a later call uses, and are not freed while another stream's queued work reads them."""
         dev = get(self, "conv_pre.bias").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):   # per-device kernel setup: CURRENT device
             return self._forward(x, mel_lens)
@@ -207,7 +223,7 @@ class Generator(nn.Module):
         if self.training:
             raise NotImplementedError("H100-native hifigan.Generator is inference-only: call .eval() (utils/model.py:67)")
         lib = L.lib()
-        m, keep, dev, up = self._packed or self._pack()
+        m, keep, dev, up = self._packed_on_stream()
         if x.dim() != 3 or x.shape[1] != m.n_mel:
             raise ValueError(f"expected mel of shape [B, {m.n_mel}, T]")
         x = x.to(device=dev, dtype=torch.float32)
@@ -234,11 +250,11 @@ class Generator(nn.Module):
         lib = L.lib()
         m, _keep, dev, up, B, T, mel_cl, bs, rs, lens_d, stream = self._inputs(x, mel_lens)
         wav = torch.empty(B, 1, T * up, dtype=torch.float32, device=dev)
-        need = lib.fs2_vocoder_workspace_bytes(C.byref(m), B, T)
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
+        self._ws, self._ws_stream = _streams.workspace((self._ws, self._ws_stream), lib.fs2_vocoder_workspace_bytes(C.byref(m), B, T),
+                                                       dev, slack=1024)
+        ws = self._ws
         va = L.VocoderArgs(B=B, T=T, mel=mel_cl.data_ptr(), mel_batch_stride=bs, mel_row_stride=rs, wav=wav.data_ptr(),
-                           workspace=self._ws.data_ptr(), workspace_bytes=self._ws.numel(), mel_lens=L.ptr(lens_d))
+                           workspace=ws.data_ptr(), workspace_bytes=ws.numel(), mel_lens=L.ptr(lens_d))
         L.check(lib.fs2_vocoder_forward(C.byref(m), C.byref(va), stream), "fs2_vocoder_forward")
         return wav
 
@@ -255,16 +271,22 @@ class Generator(nn.Module):
         chunk, holding the outputs whose support has arrived (the last chunk flushes the rest), with first_sample at the new rate.
         Concatenated, they equal Resampler(h.sampling_rate, sample_rate)(forward(x, mel_lens), mel_lens * hop) bit for bit, hop =
         prod(upsample_rates) (without mel_lens: of forward(x)); pcm16 yields that output's int16 conversion (x 32768, truncated,
-        clamped).  The lag behind the vocoder is about half_len / up input samples, under 1 ms at 8 to 48 kHz."""
+        clamped).  The lag behind the vocoder is about half_len / up input samples, under 1 ms at 8 to 48 kHz.
+
+        CUDA streams: stream() enqueues the mel's conversion on the stream current when it is called, and each next() enqueues its
+        chunk on the stream current at that next(), after the iterator's earlier work on any other stream (converted mel, previous
+        chunk), with no host sync.  x, mel_lens and the yielded chunks follow torch's usual rule: the caller orders them across
+        streams.  The iterator's own tensors are not freed while a stream it ran on still has queued work that reads them."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
         rs = self._resampler(sample_rate, chunk_frames)
         dev = get(self, "conv_pre.bias").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
             inputs = self._inputs(x, mel_lens)
+            state = _streams.made(dev)             # the iterator's last enqueued work: the mel's conversion, then each chunk
         if rs is None and not pcm16:
-            return self._stream(inputs, chunk_frames)
-        return self._stream_resampled(inputs, chunk_frames, rs, pcm16)
+            return self._stream(inputs, chunk_frames, state)
+        return self._stream_resampled(inputs, chunk_frames, rs, pcm16, state)
 
     def _resampler(self, sample_rate, chunk_frames):
         """The Resampler from h.sampling_rate to sample_rate, or None (sample_rate None or equal).  A window needs Resampler.history
@@ -279,15 +301,18 @@ class Generator(nn.Module):
             raise ValueError(f"chunk_frames * {hop} samples must cover the resampler's history of {rs.history} samples")
         return rs
 
-    def _stream_resampled(self, inputs, chunk_frames, rs, pcm16):
+    def _stream_resampled(self, inputs, chunk_frames, rs, pcm16, state):
         _m, _keep, dev, up, B, T, _mel, _bs, _rs, lens_d, _ = inputs
         N = T * up
         prev, emitted = None, 0
         with torch.no_grad(), torch.cuda.device(dev):
-            for i1, wav in self._stream(inputs, chunk_frames):  # i1: the chunk's first sample
+            # _stream enters the iterator's state before each chunk; the chunk's conversion is recorded here, before it is yielded
+            for i1, wav in self._stream(inputs, chunk_frames, state, record=False):  # i1: the chunk's first sample
                 cur = wav[:, 0]
                 if rs is None:                                  # the generator's own rate, int16 (samples past mel_lens are zeros)
-                    yield i1, ops.wav_to_int16(cur).unsqueeze(1)
+                    y = ops.wav_to_int16(cur)
+                    state.record()
+                    yield i1, y.unsqueeze(1)
                     continue
                 i2 = i1 + cur.shape[1]
                 r = rs.ready(i2, N, i2 >= N)
@@ -295,27 +320,33 @@ class Generator(nn.Module):
                     y = rs.window(prev, cur, i1, N, emitted, r, lens=lens_d, lens_scale=up, pcm16=pcm16)
                 else:
                     y = torch.empty(B, 0, dtype=torch.int16 if pcm16 else torch.float32, device=dev)
-                yield emitted, y.unsqueeze(1)
-                prev, emitted = cur, r
+                state.record()
+                state.release(prev)
+                j0, prev, emitted = emitted, cur, r
+                yield j0, y.unsqueeze(1)
 
-    def _stream(self, inputs, chunk_frames):
+    def _stream(self, inputs, chunk_frames, state, record=True):
+        """The chunks of stream(): each enqueued on the current stream after the iterator's earlier work (state), and recorded in
+        state unless the caller records its own work on the chunk."""
         lib = L.lib()
         m, _keep, dev, up, B, T, mel_cl, bs, rs, lens_d, _ = inputs    # _keep: the packed weights stay alive while the stream runs
         with torch.no_grad(), torch.cuda.device(dev):
-            ws = None
-            for f0 in range(0, T, chunk_frames):
-                f1 = min(f0 + chunk_frames, T)
-                if ws is None:                                 # one workspace for every chunk
-                    need = lib.fs2_vocoder_window_workspace_bytes(C.byref(m), B, f1 - f0)
-                    ws = torch.empty(need, dtype=torch.uint8, device=dev)
-                n = (f1 - f0) * up
-                wav = torch.empty(B, 1, n, dtype=torch.float32, device=dev)
-                wa = L.VocoderWindowArgs(B=B, T=T, mel=mel_cl.data_ptr(), mel_batch_stride=bs, mel_row_stride=rs, wav=wav.data_ptr(),
-                                         workspace=ws.data_ptr(), workspace_bytes=ws.numel(), mel_lens=L.ptr(lens_d),
-                                         f0=f0, f1=f1, wav_batch_stride=n)
-                L.check(lib.fs2_vocoder_forward_window(C.byref(m), C.byref(wa), torch.cuda.current_stream(dev).cuda_stream),
-                        "fs2_vocoder_forward_window")
-                yield f0 * up, wav
+            try:
+                for f0 in range(0, T, chunk_frames):
+                    f1 = min(f0 + chunk_frames, T)
+                    stream = state.enter()                     # after the packing and the mel's conversion, whatever their stream
+                    ws = torch.empty(lib.fs2_vocoder_window_workspace_bytes(C.byref(m), B, f1 - f0), dtype=torch.uint8, device=dev)
+                    n = (f1 - f0) * up
+                    wav = torch.empty(B, 1, n, dtype=torch.float32, device=dev)
+                    wa = L.VocoderWindowArgs(B=B, T=T, mel=mel_cl.data_ptr(), mel_batch_stride=bs, mel_row_stride=rs, wav=wav.data_ptr(),
+                                             workspace=ws.data_ptr(), workspace_bytes=ws.numel(), mel_lens=L.ptr(lens_d),
+                                             f0=f0, f1=f1, wav_batch_stride=n)
+                    L.check(lib.fs2_vocoder_forward_window(C.byref(m), C.byref(wa), stream.cuda_stream), "fs2_vocoder_forward_window")
+                    if record:
+                        state.record()
+                    yield f0 * up, wav
+            finally:
+                state.release(mel_cl, lens_d)
 
     def stream_pool(self, chunk_frames=64, sample_rate=None, pcm16=False, generators=()):
         """A pool of independent streams vocoded together (fs2_vocoder_forward_streams), for serving requests that arrive at different
@@ -341,7 +372,13 @@ class Generator(nn.Module):
         whatever the other streams' generators, and a step still makes one call with the launches of a one-generator step
         (fs2_vocoder_forward_streams_multi).  Each must match self in its config (upsample_*, resblock_*, sampling_rate),
         effective_masks(), use_tensor_cores, wide_pairs and device, and be in eval mode; ValueError otherwise, and for more than
-        L.MAX_GENERATORS in all.  Each is packed once, here."""
+        L.MAX_GENERATORS in all.  Each is packed once, here.
+
+        CUDA streams: every add, feed and step enqueues its device work on the stream current at that call, after the pool's earlier
+        work on any other stream (its mel conversions, rings, previous chunks and generator table), with no host sync; one pool may
+        be driven from several streams.  The mels the caller passes in and the chunks it gets back follow torch's usual rule: the
+        caller orders them across streams.  The pool's own tensors are not freed while a stream it ran on still has queued work that
+        reads them, and its workspace is allocated per step on the step's stream."""
         if isinstance(chunk_frames, bool) or not isinstance(chunk_frames, int) or chunk_frames < 1:
             raise ValueError("chunk_frames must be a positive int")
         rs = self._resampler(sample_rate, chunk_frames)
@@ -351,10 +388,9 @@ class Generator(nn.Module):
         gens = (self, *generators)
         self._check_pool_generators(gens, dev)
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
-            packs = [g._packed or g._pack() for g in gens]
+            packs = [g._packed_on_stream() for g in gens]
         m, keep, dev, up = packs[0]
         lib = L.lib()
-        ws = [None]
         models = L.model_array([p[0] for p in packs])
         # the generators' structs in device memory, read per work item by the multi-generator call (one upload, at its first call)
         models_dev = [None]
@@ -374,13 +410,12 @@ class Generator(nn.Module):
                 if caps is not None:
                     h[5 * B:] = caps
                 table = host.to(dev, non_blocking=True)
-                need = lib.fs2_vocoder_streams_multi_workspace_bytes(models, len(packs), B, chunk_frames)
-                if ws[0] is None or ws[0].numel() < need:
-                    ws[0] = torch.empty(need, dtype=torch.uint8, device=dev)
+                ws = torch.empty(lib.fs2_vocoder_streams_multi_workspace_bytes(models, len(packs), B, chunk_frames), dtype=torch.uint8,
+                                 device=dev)
                 wav = torch.empty(B, n, dtype=torch.float32, device=dev)
                 base = table.data_ptr()
                 a = L.VocoderStreamsMultiArgs(B=B, frames=chunk_frames, mel=base, mel_lens=base + 12 * B, f0=base + 8 * B, wav=wav.data_ptr(),
-                                              wav_batch_stride=n, workspace=ws[0].data_ptr(), workspace_bytes=ws[0].numel(),
+                                              wav_batch_stride=n, workspace=ws.data_ptr(), workspace_bytes=ws.numel(),
                                               cap=0 if caps is None else base + 20 * B, gen=base + 16 * B, models_dev=models_dev[0].data_ptr())
                 L.check(lib.fs2_vocoder_forward_streams_multi(models, len(packs), C.byref(a), torch.cuda.current_stream(dev).cuda_stream),
                         "fs2_vocoder_forward_streams_multi")
@@ -402,13 +437,11 @@ class Generator(nn.Module):
                 if caps is not None:
                     h[4 * B:] = caps
                 table = host.to(dev, non_blocking=True)
-                need = lib.fs2_vocoder_streams_workspace_bytes(C.byref(m), B, chunk_frames)
-                if ws[0] is None or ws[0].numel() < need:
-                    ws[0] = torch.empty(need, dtype=torch.uint8, device=dev)
+                ws = torch.empty(lib.fs2_vocoder_streams_workspace_bytes(C.byref(m), B, chunk_frames), dtype=torch.uint8, device=dev)
                 wav = torch.empty(B, n, dtype=torch.float32, device=dev)
                 base = table.data_ptr()
                 args = dict(B=B, frames=chunk_frames, mel=base, mel_lens=base + 12 * B, f0=base + 8 * B, wav=wav.data_ptr(),
-                            wav_batch_stride=n, workspace=ws[0].data_ptr(), workspace_bytes=ws[0].numel())
+                            wav_batch_stride=n, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
                 st = torch.cuda.current_stream(dev).cuda_stream
                 if caps is None:
                     L.check(lib.fs2_vocoder_forward_streams(C.byref(m), C.byref(L.VocoderStreamsArgs(**args)), st),
@@ -515,6 +548,9 @@ class StreamPool:
         #  so far), next frame, last chunk, emitted, Resampler or None, encoding, _Feed (None for an add()ed stream), generator index]
         self._live = []
         self._next = 0
+        # the pool's last enqueued work (creation: the packed weights; then every conversion, append, launch and resampling), which
+        # work on another stream waits for, and the streams the pool has used, on which dropped tensors are recorded
+        self._state = _streams.made(self.device)
 
     def _encoding(self, name):
         if name not in ENCODINGS:
@@ -568,7 +604,9 @@ class StreamPool:
         rs, enc = self._format(sample_rate, encoding)
         rows = mel.T
         if not (rows.dtype == torch.float32 and rows.stride(1) == 1 and (n == 1 or rows.stride(0) == self.n_mel) and rows.data_ptr() % 16 == 0):
+            self._state.enter()
             rows = rows.to(torch.float32).contiguous()
+            self._state.record()
         return self._admit(rows, n, rs, enc, None, generator)
 
     def _format(self, sample_rate, encoding):
@@ -628,7 +666,9 @@ class StreamPool:
         if mel.shape[1] < 1:
             raise ValueError("mel has no frames")
         if mel.dtype != torch.float32:
+            self._state.enter()
             mel = mel.to(torch.float32)
+            self._state.record()
         s[8].blocks.append([mel, 0])
         s[2] += mel.shape[1]
 
@@ -639,14 +679,20 @@ class StreamPool:
         s[8].closed = True
         if s[3] >= s[2]:
             self._live = [x for x in self._live if x is not s]
+            self._drop(s)
 
     def cancel(self, h):
         """Drops a live stream (KeyError if it is not live)."""
         for i, s in enumerate(self._live):
             if s[0] == h:
                 del self._live[i]
+                self._drop(s)
                 return
         raise KeyError(h)
+
+    def _drop(self, s):
+        """Releases the device tensors of stream record s, which has left the pool."""
+        self._state.release(s[1], s[4], *(b[0] for b in (s[8].blocks if s[8] is not None else ())))
 
     def __len__(self):
         return len(self._live)
@@ -664,6 +710,7 @@ class StreamPool:
         live = [s for s in self._live if s[8] is None or s[8].closed or s[2] >= s[3] + self.chunk_frames + self.reach[1]]
         if not live:
             return []
+        self._state.enter()
         ptrs, f0s, ns = [s[1].data_ptr() for s in live], [s[3] for s in live], [s[2] for s in live]
         gens = {} if self.n_generators == 1 else {"gens": [s[9] for s in live]}
         if any(s[8] is not None for s in live):
@@ -684,7 +731,12 @@ class StreamPool:
             t, k = rows[i]
             out.append((s[0], starts[i], t[k][None, None, :widths[i]]))
             s[3] += self.chunk_frames
-        self._live = [s for s in self._live if (s[8] is not None and not s[8].closed) or s[3] < s[2]]
+        self._state.record()
+        keep = [s for s in self._live if (s[8] is not None and not s[8].closed) or s[3] < s[2]]
+        for s in live:
+            if (s[8] is None or s[8].closed) and s[3] >= s[2]:
+                self._drop(s)
+        self._live = keep
         return out
 
     def _fill(self, live):
@@ -708,6 +760,7 @@ class StreamPool:
         if records:
             self._append(records)
         # The blocks appended in full are released only now, after the call is enqueued (the rule _converted states for its chunks).
+        self._state.release(*(b[0] for b in done))
         del done
 
     def _converted(self, live, conv, wav, starts, widths):
@@ -730,6 +783,7 @@ class StreamPool:
         # Each chunk stays alive as the next step's history.  The previous chunks are released only now: the call is enqueued, so a
         # later allocation that reuses their memory is written after the call has read them (released before, the call's own table
         # upload or output could take that memory first).
+        self._state.release(*(live[i][4] for i in conv))
         for i in conv:
             live[i][4] = wav[i]
         return y

@@ -11,6 +11,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib as L
+from .. import _streams
 from .. import packing
 from .._modtree import get, populate
 from ..spec import fastspeech2_spec, read_dataset_files
@@ -101,14 +102,17 @@ class FastSpeech2(nn.Module):
         #    back to the fp32 kernels' level (scripts/flip_census.py).  Clear the two bits for the fp32 kernels.
         self.tc_mask = (L.TC_DECODER | L.TC_POSTNET | L.TC_DECODER_F8 | L.TC_POSTNET_F8 | L.TC_ENCODER | L.TC_PREDICTORS)
         self._packed = None          # (AcousticModel struct, keep-alive tensors, device)
-        self._pos_long = {}          # device position tables longer than max_seq_len, keyed by width
-        self._ws = None
-        self._stats_host = None
+        self._packed_state = None    # _streams.StreamState of the packed weights: made on the stream of the call that packed them
+        self._pos_long = {}          # width -> (device position table longer than max_seq_len, its StreamState)
+        self._ws, self._ws_stream = None, None     # the last call's workspace and the stream it was allocated on (_streams.workspace)
+        self._stats_host = None      # the last call's len_stats [max, sum of mel_lens, wild durations], pinned, final once its stream syncs
 
     # ------------------------------------------------------------------ packing
     def _invalidate(self):
+        if self._packed is not None:
+            self._packed_state.release(*self._packed[1].values())
         self._packed = None
-        self._ws = None
+        self._ws = self._ws_stream = None
 
     def load_state_dict(self, *a, **k):
         out = super().load_state_dict(*a, **k)
@@ -178,6 +182,7 @@ class FastSpeech2(nn.Module):
             m.w_post[i], m.b_post[i] = w.data_ptr(), P(f"post.{i}.b")
             m.post_k, m.post_cin[i], m.post_cout[i] = w.shape[0], w.shape[1], w.shape[2]
         self._packed = (m, pk, dev)
+        self._packed_state = _streams.made(dev)
         return self._packed
 
     def _keys(self):
@@ -190,16 +195,19 @@ class FastSpeech2(nn.Module):
         reference recomputes the table on the fly (transformer/Models.py:82-87,:145-152) -- same here, cached by size."""
         if n <= self.max_seq_len:
             return self._pos_ptrs[which], self.max_seq_len + 1
-        tab = self._pos_long.get(width)
-        if tab is None or tab.shape[0] < n or tab.device != dev:
+        old = self._pos_long.get(width)
+        if old is None or old[0].shape[0] < n or old[0].device != dev:
+            if old is not None:
+                old[1].release(old[0])
             rows = max(2048, 1 << (n - 1).bit_length())
             tab = sinusoid_table(rows, width).to(dev)
-            self._pos_long[width] = tab
+            self._pos_long[width] = (tab, _streams.made(dev))      # the upload is ordered on the current stream only
+        tab, state = self._pos_long[width]
+        state.enter()
         return tab.data_ptr(), tab.shape[0]
 
     def _workspace(self, nbytes: int, dev):
-        if self._ws is None or self._ws.numel() < nbytes or self._ws.device != dev:
-            self._ws = torch.empty(int(nbytes * 1.25) + 1024, dtype=torch.uint8, device=dev)
+        self._ws, self._ws_stream = _streams.workspace((self._ws, self._ws_stream), nbytes, dev, grow=1.25, slack=1024)
         return self._ws
 
     # ------------------------------------------------------------------ forward
@@ -218,7 +226,14 @@ class FastSpeech2(nn.Module):
         d_control with d_targets.  Tensor values are rounded to fp32 on the model's device without a host synchronisation; the one
         deviation from the reference is a float64 control, which the reference would let promote the prediction to float64.  Ragged
         mode: utterance b equals its solo call with c[b] ([B, 1]) or c[b:b+1, :src_lens[b]] ([B, L]), and control columns beyond an
-        utterance's length are never read."""
+        utterance's length are never read.
+
+        CUDA streams: the call enqueues all of its device work on the stream current at the call; without max_mel_len it synchronises
+        that stream once, to read the output length.  Its workspace is cached for the next call on the same stream only: a call on
+        another stream allocates its own, so calls on two streams never share one.  The arguments and the returned tensors follow
+        torch's usual rule: the caller orders them across streams.  The weights packed by the first call and the position tables
+        longer than max_seq_len are ready on whatever stream a later call uses, and are not freed while another stream's queued work
+        reads them."""
         # the C ABI sets up per-device kernel attributes for the CURRENT device: make the model's device current
         dev = get(self, "mel_linear.weight").device
         with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
@@ -233,6 +248,7 @@ class FastSpeech2(nn.Module):
         e_frame = self.energy_feature_level == "frame_level"
         lib = L.lib()
         m, _keep, dev = self._packed or self._pack()
+        self._packed_state.enter()
         B, Lmax = int(texts.shape[0]), int(max_src_len)
         if texts.shape[1] != Lmax:
             raise ValueError("texts.shape[1] must equal max_src_len")
@@ -253,8 +269,9 @@ class FastSpeech2(nn.Module):
         cum = torch.empty(B, Lmax, dtype=torch.int32, device=dev)
         x_adapted = torch.empty(B, Lmax, m.d_model, **f32)
         stats_dev = torch.empty(3, dtype=torch.int32, device=dev)
-        if self._stats_host is None:
-            self._stats_host = torch.zeros(3, dtype=torch.int32).pin_memory()
+        # a pinned block of this call's own, filled by a torch copy on the call's stream: the caching host allocator then keeps the block
+        # from reuse until that copy is done, whenever the block is dropped
+        stats_host = torch.empty(3, dtype=torch.int32, pin_memory=True)
         tgt = lambda t: None if t is None else t.to(**f32).contiguous()
         p_t, e_t, d_t = tgt(p_targets), tgt(e_targets), tgt(d_targets)
         # p_control scales the predictors without a target; e_control is never read (model/modules.py:124)
@@ -264,26 +281,27 @@ class FastSpeech2(nn.Module):
         d_ctl = normalize_control(d_control, (B, Lmax), dev, "d_control") if d_t is None else _UNREAD_CONTROL
 
         m.enc_pos, m.enc_pos_rows = self._position(0, Lmax, m.d_model, dev)
-        ws_bytes = lib.fs2_encode_workspace_bytes(C.byref(m), B, Lmax)
-        ws = self._workspace(ws_bytes, dev)
+        ws = self._workspace(lib.fs2_encode_workspace_bytes(C.byref(m), B, Lmax), dev)
         ea = L.EncodeArgs(B=B, L=Lmax, texts=texts.data_ptr(), speakers=L.ptr(speakers_d), src_lens=src_lens32.data_ptr(),
                           p_control=p_enc[1], e_control=1.0, d_control=d_ctl[1],
                           p_target=0 if p_frame else L.ptr(p_t), e_target=0 if e_frame else L.ptr(e_t), d_target=L.ptr(d_t),
                           p_pred=0 if p_frame else p_pred.data_ptr(), e_pred=0 if e_frame else e_pred.data_ptr(), logd_pred=logd.data_ptr(),
                           d_rounded=d_rounded.data_ptr(), mel_lens=mel_lens_out.data_ptr(), mel_lens32=mel_lens32.data_ptr(),
                           cum_dur=cum.data_ptr(), x_adapted=x_adapted.data_ptr(), len_stats=stats_dev.data_ptr(),
-                          len_stats_host=self._stats_host.data_ptr(), workspace=ws.data_ptr(), workspace_bytes=ws.numel())
+                          len_stats_host=0, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
         ctl = _control_args(p_enc, d_ctl)
         L.check(lib.fs2_acoustic_encode_ctl(C.byref(m), C.byref(ea), C.byref(ctl), int(ragged), stream), "fs2_acoustic_encode")
+        stats_host.copy_(stats_dev, non_blocking=True)
+        self._stats_host = stats_host
 
         if max_mel_len is not None:
             T = int(max_mel_len)
         else:
             # the one unavoidable host sync: the output shape depends on the predicted durations (utils/tools.py:94)
             torch.cuda.current_stream(dev).synchronize()
-            T = int(self._stats_host[0])
-            if int(self._stats_host[2]) != 0:
-                raise L.Fs2Error(f"{int(self._stats_host[2])} predicted durations are NaN / inf / > 1e6 frames "
+            T = int(stats_host[0])
+            if int(stats_host[2]) != 0:
+                raise L.Fs2Error(f"{int(stats_host[2])} predicted durations are NaN / inf / > 1e6 frames "
                                  "(the reference raises on them too, model/modules.py:186)")
         if T <= 0:
             raise L.Fs2Error("all predicted durations are zero: nothing to decode")
@@ -304,8 +322,7 @@ class FastSpeech2(nn.Module):
             if e_t is not None and tuple(e_t.shape) != (B, T):
                 raise ValueError("frame-level e_targets must be [B, max_mel_len]")
         p_dec = normalize_control(p_control, (B, T), dev, "p_control") if p_read_dec else _UNREAD_CONTROL
-        ws_bytes = lib.fs2_decode_workspace_bytes(C.byref(m), B, T)
-        ws = self._workspace(ws_bytes, dev)
+        ws = self._workspace(lib.fs2_decode_workspace_bytes(C.byref(m), B, T), dev)
         da = L.DecodeArgs(B=B, L=Lmax, T=T, x_adapted=x_adapted.data_ptr(), cum_dur=cum.data_ptr(),
                           mel_mask_lens=mask_lens32.data_ptr(), p_control=p_dec[1],
                           p_target_frames=L.ptr(p_t) if p_frame else 0, e_target_frames=L.ptr(e_t) if e_frame else 0,

@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import _streams
 
 # output encodings of the mixed call, by name; a stream's chunk has the dtype of its encoding
 ENCODINGS = {"f32": L.RESAMPLE_F32, "pcm16": L.RESAMPLE_PCM16, "ulaw": L.RESAMPLE_ULAW, "alaw": L.RESAMPLE_ALAW}
@@ -56,7 +57,11 @@ def polyphase(h: np.ndarray, up: int) -> np.ndarray:
 
 class Resampler:
     """Converts waveforms from fs_in to fs_out Hz (up / down = fs_out / fs_in reduced).  fs_out == fs_in is the identity: the input is
-    returned unchanged, with no launch.  Refuses non-positive or non-integer rates and max(up, down) > 2048 with ValueError."""
+    returned unchanged, with no launch.  Refuses non-positive or non-integer rates and max(up, down) > 2048 with ValueError.
+
+    CUDA streams: every call (__call__, window, streams, mixed) enqueues all of its device work on the stream current at that call.
+    The waveforms, lengths and records the caller passes in and the outputs it gets back follow torch's usual rule: the caller orders
+    them across streams.  The taps, uploaded to a device by the first call there, are ready on whatever stream a later call uses."""
 
     def __init__(self, fs_in, fs_out):
         self.fs_in, self.fs_out = _rate(fs_in, "fs_in"), _rate(fs_out, "fs_out")
@@ -94,8 +99,10 @@ class Resampler:
         device = torch.device(device)
         t = self._dev_taps.get(device)
         if t is None:
-            t = self._dev_taps[device] = torch.from_numpy(_UNIT_TAP if self.identity else self.taps).to(device)
-        return t
+            tab = torch.from_numpy(_UNIT_TAP if self.identity else self.taps).to(device)
+            t = self._dev_taps[device] = (tab, _streams.made(device))     # the upload is ordered on the current stream only
+        t[1].enter()
+        return t[0]
 
     def _filter(self, device):
         return dict(up=self.up, down=self.down, K=1 if self.identity else self.K, taps=self.device_taps(device).data_ptr())

@@ -221,6 +221,16 @@ MAX_GENERATORS = 8
 VOCODER_STREAMS_MULTI_ARGS_SIZE = 88
 assert C.sizeof(VocoderStreamsMultiArgs) == VOCODER_STREAMS_MULTI_ARGS_SIZE
 
+class AcousticVoices(C.Structure):
+    """fs2_acoustic_voices: the voices of fs2_acoustic_{encode,decode}_voices (32 bytes, pinned by a static_assert in model.cu).
+    models: the address of a host array of AcousticModel pointers (acoustic_model_array)."""
+    _fields_ = [("n", i32), ("models", fp), ("models_dev", fp), ("voice", fp)]
+
+
+MAX_VOICES = 8
+ACOUSTIC_VOICES_SIZE = 32
+assert C.sizeof(AcousticVoices) == ACOUSTIC_VOICES_SIZE
+
 VOCODER_STREAMS_RING_ARGS_SIZE, MEL_RING_RECORD_SIZE, MEL_RING_APPEND_ARGS_SIZE = 72, 56, 24
 assert C.sizeof(VocoderStreamsRingArgs) == VOCODER_STREAMS_RING_ARGS_SIZE and C.sizeof(MelRingRecord) == MEL_RING_RECORD_SIZE
 assert C.sizeof(MelRingAppendArgs) == MEL_RING_APPEND_ARGS_SIZE
@@ -337,6 +347,10 @@ EXPORTS = {
     "fs2_acoustic_decode_ragged": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), fp]),
     "fs2_acoustic_encode_ctl": (i32, [C.POINTER(AcousticModel), C.POINTER(EncodeArgs), C.POINTER(ControlArgs), i32, fp]),
     "fs2_acoustic_decode_ctl": (i32, [C.POINTER(AcousticModel), C.POINTER(DecodeArgs), C.POINTER(ControlArgs), i32, fp]),
+    "fs2_encode_voices_workspace_bytes": (C.c_size_t, [C.POINTER(AcousticVoices), i32, i32]),
+    "fs2_decode_voices_workspace_bytes": (C.c_size_t, [C.POINTER(AcousticVoices), i32, i32]),
+    "fs2_acoustic_encode_voices": (i32, [C.POINTER(AcousticVoices), C.POINTER(EncodeArgs), C.POINTER(ControlArgs), i32, fp]),
+    "fs2_acoustic_decode_voices": (i32, [C.POINTER(AcousticVoices), C.POINTER(DecodeArgs), C.POINTER(ControlArgs), i32, fp]),
     "fs2_vocoder_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
     "fs2_vocoder_forward": (i32, [C.POINTER(VocoderModel), C.POINTER(VocoderArgs), fp]),
     "fs2_vocoder_window_workspace_bytes": (C.c_size_t, [C.POINTER(VocoderModel), i32, i32]),
@@ -413,6 +427,11 @@ def vocoder_resblock_runs(m, stage):
 def model_array(models):
     """The host array of model pointers fs2_vocoder_forward_streams_multi takes (the structs must outlive it)."""
     return (C.POINTER(VocoderModel) * len(models))(*[C.pointer(m) for m in models])
+
+
+def acoustic_model_array(models):
+    """The host array of AcousticModel pointers fs2_acoustic_voices.models points at (the structs must outlive it)."""
+    return (C.POINTER(AcousticModel) * len(models))(*[C.pointer(m) for m in models])
 
 
 def ptr(t):

@@ -87,10 +87,38 @@ __device__ __forceinline__ RowSpan origin_rows(const int* lens, const int* org, 
 // byte offset of its pointer field in fs2_vocoder_model and a float offset past that pointer -- and every work item loads the pointer
 // from its own stream's generator.  models == NULL outside this mode.
 struct GenRef { int32_t off, add; };
-struct Generators { const fs2_vocoder_model* models; const int* gen; };
-__device__ __forceinline__ const float* gen_weight(const Generators& g, int b, GenRef r) {
+template <class M> struct ModelTable { const M* models; const int* gen; };
+using Generators = ModelTable<fs2_vocoder_model>;
+template <class M>
+__device__ __forceinline__ const float* gen_weight(const ModelTable<M>& g, int b, GenRef r) {
   const unsigned char* m = reinterpret_cast<const unsigned char*>(g.models + __ldg(g.gen + b));
   return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(m + r.off))) + r.add;
+}
+
+// Voices mode of the acoustic layers (fs2_acoustic_{encode,decode}_voices): utterance b reads its weights from voice gen[b] of the
+// device array `models` (gen: the phase's staged table, always in range), through the same field lookup as the generators above.  A
+// conv names its fp32 weights, tiles and bias (VoiceLaunch); a row kernel up to four tables (VoiceRow).  models == NULL outside it.
+using Voices = ModelTable<fs2_acoustic_model>;
+struct VoiceLaunch { Voices voices; GenRef w, wt, bias; };
+// in (the phase's first launch only): the caller's voice indices.  That launch reads them itself, clamped to voice 0 outside [0, n),
+// and stages the table the later launches read: out[b] = the clamped index, out[B + b] = 1 if in[b] was in range, else 0.
+struct VoiceRow { Voices voices; GenRef r[4]; const int* in; int n; int* out; };
+__device__ __forceinline__ int voice_of(const VoiceRow& v, int b) {
+  if (!v.in) return __ldg(v.voices.gen + b);
+  const int k = __ldg(v.in + b);
+  return k >= 0 && k < v.n ? k : 0;
+}
+__device__ __forceinline__ const float* voice_table(const VoiceRow& v, int b, int i) {
+  const unsigned char* m = reinterpret_cast<const unsigned char*>(v.voices.models + voice_of(v, b));
+  return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(m + v.r[i].off))) + v.r[i].add;
+}
+__device__ __forceinline__ void voice_stage(const VoiceRow& v, int B) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v.in && i < B) {
+    const int k = __ldg(v.in + i);
+    v.out[i] = voice_of(v, i);
+    v.out[B + i] = k >= 0 && k < v.n;
+  }
 }
 // The weights of one windowed launch in the multi-generator mode: a conv's fp32 weights, tiles and bias; a fused ResBlock launch's
 // pairs, its arguments' (j, d) being ResBlock rb + j at dilation d0 + d of every generator.

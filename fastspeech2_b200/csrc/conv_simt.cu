@@ -223,6 +223,15 @@ __global__ void __launch_bounds__(256) conv_simt_streams_multi_kernel(ConvP p, c
   conv_simt_body<BM, BN, ACT, true>(p);
 }
 
+// Voices mode (fs2_acoustic_{encode,decode}_voices): the offline body on the weights and bias of the CTA's utterance's voice
+template <int BM, int BN, int ACT>
+__global__ void __launch_bounds__(256) conv_simt_voices_kernel(ConvP p, const VoiceLaunch v) {
+  const int b = blockIdx.x / p.tiles_per_batch;
+  p.w = gen_weight(v.voices, b, v.w);
+  if (p.bias) p.bias = gen_weight(v.voices, b, v.bias);
+  conv_simt_body<BM, BN, ACT, false>(p);
+}
+
 // Tile choice of the launcher (pure host logic, no CUDA call; exposed as fs2_conv_simt_plan so that the GPU tests' coverage of the six
 // (BM, BN) instantiations is checkable without a GPU).
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out) {
@@ -245,7 +254,8 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* 
 
 // win (with a->x_lens): NULL, or the windowed mode (OriginWindow; a->T is not used): the tile is chosen for the window's rows.
 // Every output element sums its taps and channels in the same order whatever the tile, so a window computes the offline bits.
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win) {
+// voices: NULL, or the voices mode (VoiceLaunch, offline only): a->w and a->bias are voice 0's.
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win, const VoiceLaunch* voices) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
@@ -253,7 +263,8 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   if (a->res && ((a->res_row_stride & 3) || (a->res_batch_stride & 3))) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
   if (a->in_act != FS2_ACT_NONE && a->in_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;
-  if (win && !a->x_lens) return FS2_ERR_ARG;
+  if ((win && !a->x_lens) || (win && voices)) return FS2_ERR_ARG;
+  if (voices && a->out_act == FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;                              // the acoustic model's activations
   if (win && a->out_act != FS2_ACT_NONE && a->out_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;   // the vocoder's activations
   ConvP p;
   p.x = a->x; p.xbs = a->x_batch_stride; p.xrs = a->x_row_stride;
@@ -289,6 +300,12 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   } else if (win) {                                                                                       \
     if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); \
     else conv_simt_streams_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p);                        \
+  } else if (voices) {                                                                                    \
+    switch (a->out_act) {                                                                                 \
+      case FS2_ACT_RELU: conv_simt_voices_kernel<BM_, BN_, FS2_ACT_RELU><<<grid, 256, 0, s>>>(p, *voices); break; \
+      case FS2_ACT_TANH: conv_simt_voices_kernel<BM_, BN_, FS2_ACT_TANH><<<grid, 256, 0, s>>>(p, *voices); break; \
+      default: conv_simt_voices_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p, *voices); break;   \
+    }                                                                                                     \
   } else {                                                                                                \
     switch (a->out_act) {                                                                                 \
       case FS2_ACT_RELU: conv_simt_kernel<BM_, BN_, FS2_ACT_RELU><<<grid, 256, 0, s>>>(p); break;         \

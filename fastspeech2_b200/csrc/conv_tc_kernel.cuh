@@ -84,6 +84,7 @@ struct TcP {
   GenRef wt_ref, bias_ref;         // (bias stays the "has a bias" flag)
   int slot_off;                    // shared-memory byte offset of the TcSlot ring, past the plan's budget
   int NG;                          // NB-channel blocks per work item, computed one after another from the item's slab (see conv_tc_body)
+  Voices voices;                   // voices mode (conv_tc_voices_kernel only): wt and bias per work item through wt_ref / bias_ref
 };
 
 // The weight producer decodes each unit (work item, channel block) -- its tile and block, and its generator's weight-scale header and
@@ -91,11 +92,15 @@ struct TcP {
 // full barrier then publishes the slot to the consumers; they read it in the unit's epilogue.  So the consumer warpgroups hold no
 // work-list cursor (with one, the ragged and windowed cursors' state pushes the 96-register warpgroups into spills).  The producer runs
 // at most TC_SB_MAX stages, so at most TC_SB_MAX units, ahead of an epilogue: TC_SLOTS > TC_SB_MAX + 1 slots.
+// The voices mode's slot also carries the unit's tile base: a K-segmented conv's consumers read segment seg's weight-scale header there.
 struct TcSlot { Item it; const float* bias; float inv_ws; int pad_; };
+struct TcVoiceSlot : TcSlot { const float* wt; };
 constexpr int TC_SLOTS = 16;
 constexpr int TC_SLOT_BYTES = TC_SLOTS * (int)sizeof(TcSlot);
-__device__ __forceinline__ TcSlot& tc_slot(const TcP& p, unsigned char* smem, int u) {
-  return reinterpret_cast<TcSlot*>(smem + p.slot_off)[u % TC_SLOTS];
+constexpr int TC_VOICE_SLOT_BYTES = TC_SLOTS * (int)sizeof(TcVoiceSlot);
+template <class S = TcSlot>
+__device__ __forceinline__ S& tc_slot(const TcP& p, unsigned char* smem, int u) {
+  return reinterpret_cast<S*>(smem + p.slot_off)[u % TC_SLOTS];
 }
 
 // Shared-memory epilogue tiles behind the ring barriers: [full, empty mbarrier per consumer warp][residual tile if res][sum tile if
@@ -262,7 +267,9 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 // are window rows here), and utterance b's rows outside [lo_b, hi_b) read as zero.
 // MULTI (with WIN): multi-generator mode: each work item reads the tiles, weight-scale header and bias of its utterance's generator
 // (p.gens), loaded once per item instead of once per CTA.
-template <int NB, bool RAG, bool WIN, bool MULTI = false>
+// VOICE (offline, padded or ragged): voices mode: each work item reads the tiles, weight-scale headers and bias of its utterance's voice
+// (p.voices), K-segmented convs included.
+template <int NB, bool RAG, bool WIN, bool MULTI = false, bool VOICE = false>
 __device__ __forceinline__ void conv_tc_body(const TcP& p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -279,6 +286,7 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
   uint64_t* emptyB = fullB + TC_SB_MAX;    // [SB_MAX]
   const bool staged = tc_stage_tiles(p.res != nullptr, p.accumulate != 0, p.nseg) > 0;   // the host budgeted tc_stage_bytes
   using Stage = TcStage<NB>;
+  using Slot = std::conditional_t<VOICE, TcVoiceSlot, TcSlot>;
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
@@ -312,11 +320,17 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
           bias = p.bias ? gen_weight(p.gens, pit.b, p.bias_ref) : nullptr;
           inv_ws = __ldg(wt);
         }
+        if constexpr (VOICE) {                         // the item's voice's
+          wt = gen_weight(p.voices, pit.b, p.wt_ref);
+          bias = p.bias ? gen_weight(p.voices, pit.b, p.bias_ref) : nullptr;
+          inv_ws = __ldg(wt);
+        }
         for (int j = 0; j < NG; j++, u++) {            // the item's blocks, in the consumers' order
-          TcSlot& slot = tc_slot(p, smem_raw, u);       // before the unit's first stage: its full barrier publishes the slot
+          Slot& slot = tc_slot<Slot>(p, smem_raw, u);   // before the unit's first stage: its full barrier publishes the slot
           slot.it = Item{pit.nblk * NG + j, pit.b, pit.t0, pit.rows};
           slot.bias = bias;
           slot.inv_ws = inv_ws;
+          if constexpr (VOICE) slot.wt = wt;
           for (int seg = 0; seg < p.nseg; seg++) {
             const unsigned char* src = reinterpret_cast<const unsigned char*>(wt) + (long long)seg * p.seg_wbytes + TC_HDR +
                                        (size_t)slot.it.nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
@@ -388,16 +402,19 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
         // alpha-free sum, the pad-row mask and the store to y with the last.  The same thread owns the same outputs in every unit, so the
         // fp32 read-modify-write of the sum tile needs no further ordering.  No output activation (checked on the host).
         const bool first = seg == 0, last = seg == p.nseg - 1;
-        const TcSlot& slot = tc_slot(p, smem_raw, unit);
+        const Slot& slot = tc_slot<Slot>(p, smem_raw, unit);
         const Item it = slot.it;
         // the staging barrier completes one phase per unit of this CTA
         if (staged && first) mbar_wait(Stage::full(p, smem_raw, warp), (uint32_t)unit & 1u);
         const float* bias = first ? slot.bias : nullptr;
         const int* lens = last ? p.row_lens : nullptr;
         const bool use_res = last && p.res, sum_in = !first || p.accumulate, sum_out = !last;
-        // header: 1 / (power-of-two weight scale) of the unit's generator (multi-generator mode: one segment, checked on the host)
+        // header: 1 / (power-of-two weight scale) of the unit's generator (multi-generator mode: one segment, checked on the host) or
+        // voice; a K-segmented conv's segment seg has its own
+        const float* hdr = p.wt;
+        if constexpr (VOICE) hdr = slot.wt;
         const float inv_ws = p.nseg == 1 ? slot.inv_ws
-            : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(p.wt) + (long long)seg * p.seg_wbytes));
+            : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(hdr) + (long long)seg * p.seg_wbytes));
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
         switch (p.out_act) {                           // uniform branch: keeps tanhf out of the other variants' inner loops
           case FS2_ACT_RELU: tc_epilogue<FS2_ACT_RELU, NB, TG>(p, acc, it, row_base, bias, lens, smem_raw, use_res, sum_in, sum_out, inv_ws); break;
@@ -540,9 +557,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_multi_kernel(co
   conv_tc_body<NB, true, true, true>(p);
 }
 
+// Voices mode (fs2_acoustic_{encode,decode}_voices): the offline padded (RAG false) or ragged conv with each item's weights from its
+// utterance's voice
+template <int NB, bool RAG>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_voices_kernel(const TcP p) {
+  conv_tc_body<NB, RAG, false, false, true>(p);
+}
+
 // The NB instantiations live in their own translation units (conv_tc_nb*.cu) so that the library builds in parallel.
 // conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.  window: the windowed mode
-// (conv_tc_streams_kernel; conv_tc_streams_multi_kernel when p.gens.models is set).
+// (conv_tc_streams_kernel; conv_tc_streams_multi_kernel when p.gens.models is set); p.voices.models set: conv_tc_voices_kernel.
 #define FS2_CONV_TC_NB_DECL(nb)                        \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes); \
   void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s);
@@ -555,10 +579,14 @@ FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CON
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
     if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
     if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_streams_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_voices_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_voices_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
     return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_streams_multi_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
   }                                                                                                     \
   void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s) {   \
-    if (window && p.gens.models) conv_tc_streams_multi_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);   \
+    if (p.voices.models && p.x_lens) conv_tc_voices_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p); \
+    else if (p.voices.models) conv_tc_voices_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);      \
+    else if (window && p.gens.models) conv_tc_streams_multi_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p); \
     else if (window) conv_tc_streams_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                     \
     else if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                     \
     else conv_tc_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);                                  \

@@ -62,10 +62,11 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 }
 
 // kernels / launchers defined in the other translation units
-// win: the vocoder's windowed mode (OriginWindow), NULL everywhere else
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr);
+// win: the vocoder's windowed mode (OriginWindow), NULL everywhere else.  voices / vr: the acoustic voices mode (VoiceLaunch, VoiceRow),
+// NULL everywhere else
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const VoiceLaunch* voices = nullptr);
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr);
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const VoiceLaunch* voices = nullptr);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
@@ -73,20 +74,21 @@ int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
 
 // backend dispatch of the fs2_conv1d contract
-static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr) {
+static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const VoiceLaunch* voices = nullptr) {
   if (!a) return FS2_ERR_ARG;
   if (a->x_lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win);
-  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win);
-  return conv1d_simt(a, s, win);
+  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win, voices);
+  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win, voices);
+  return conv1d_simt(a, s, win, voices);
 }
 int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = false, int fused_from = 0);
-int embed_positions(const fs2_embed_args* a, cudaStream_t s);
-int add_speaker(const fs2_rowbias_args* a, cudaStream_t s);
-int layernorm(const fs2_layernorm_args* a, cudaStream_t s);
-int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl = nullptr);
-int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr);
-int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s);
+int embed_positions(const fs2_embed_args* a, cudaStream_t s, const VoiceRow* vr = nullptr);
+int add_speaker(const fs2_rowbias_args* a, cudaStream_t s, const VoiceRow* vr = nullptr);
+int layernorm(const fs2_layernorm_args* a, cudaStream_t s, const VoiceRow* vr = nullptr);
+int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl = nullptr, const VoiceRow* vr = nullptr);
+int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr,
+              const int32_t* valid = nullptr);
+int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s, const VoiceRow* vr = nullptr);
 int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
 int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win = nullptr, int x0 = 0, bool wide = false);
 int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, const int32_t* gen_in,
@@ -95,7 +97,7 @@ int mel_ring_append(const fs2_mel_ring_append_args* a, cudaStream_t s);
 int wav_to_int16(const fs2_wav_int16_args* a, cudaStream_t s);
 int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& out, bool wide = false);
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
-int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s);
+int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s, const VoiceRow* vr = nullptr);
 int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cudaStream_t s);
 
 // ------------------------------------------------------------------ workspace bump allocator
@@ -139,16 +141,44 @@ static fs2_conv1d_args conv_args(const float* x, int B, int T, int Cin, int N, i
 //             fp32 CUDA-core kernel's level (scripts/flip_census.py).  w_tc: taps * (Cin/256) tile buffers of 128 + 1024*N bytes
 //             (packing.pack_conv_tc_segments).  No output activation: a following ReLU is applied by the consumer (in_act of the
 //             next conv / pre_relu of the LayerNorm).
+// The voices mode (fs2_acoustic_{encode,decode}_voices): the phase plans and checks on m = models[0] and names each weight a launch reads
+// by its field in *m; utterance b reads that field of voice staged[b] of models_dev.  staged: the phase's [2B] table (VoiceRow::out),
+// staged from the caller's `in` by the phase's first launch.  Each launch's VoiceRow / VoiceLaunch is built right before it.
+struct VoiceSet {
+  const fs2_acoustic_model* m;
+  const fs2_acoustic_model* models_dev;
+  int32_t* staged;
+  const int32_t* in; int n;
+  mutable VoiceRow vr;
+  mutable VoiceLaunch vl;
+  GenRef ref(const void* field) const { return GenRef{(int32_t)((const char*)field - (const char*)m), 0}; }
+  const VoiceRow* row(const void* f0, const void* f1 = nullptr, const void* f2 = nullptr, const void* f3 = nullptr, bool first = false) const {
+    vr = VoiceRow{{models_dev, staged}, {ref(f0), f1 ? ref(f1) : GenRef{}, f2 ? ref(f2) : GenRef{}, f3 ? ref(f3) : GenRef{}},
+                  first ? in : nullptr, n, first ? staged : nullptr};
+    return &vr;
+  }
+  const VoiceLaunch* conv(const void* w, const void* w_tc, const void* bias) const {
+    vl = VoiceLaunch{{models_dev, staged}, ref(w), ref(w_tc), ref(bias)};
+    return &vl;
+  }
+};
+// The row tables of a launch: NULL outside the voices mode
+template <class... F>
+static const VoiceRow* voice_row(const VoiceSet* vs, F... fields) { return vs ? vs->row(fields...) : nullptr; }
+
 struct ConvMode {
   enum { EXACT, TC, SEGMENTED } path;
   unsigned tcv;
-  void weights(fs2_conv1d_args& a, const float* w, const float* w_tc, const float* bias) const {
+  const VoiceSet* vs;     // the voices mode, or NULL
+  // Runs `a` with these weights (fields of the model: in the voices mode each utterance reads them from its own voice).
+  int run(fs2_conv1d_args& a, const float* const& w, const float* const& w_tc, const float* const& bias, cudaStream_t s) const {
     a.bias = bias;
     if (path == SEGMENTED) {
       a.w = nullptr; a.w_tc = w_tc; a.backend = FS2_CONV_TC; a.tc_variant = FS2_TC_VARIANT_NB64 | FS2_TC_VARIANT_SEGMENTED;
     } else {
       a.w = w; a.w_tc = path == TC ? w_tc : nullptr; a.tc_variant = tcv;
     }
+    return conv1d_dispatch(&a, s, nullptr, vs ? vs->conv(&w, &w_tc, &bias) : nullptr);
   }
 };
 
@@ -167,9 +197,8 @@ static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_
   const int32_t* rag = ragged_lens(ragged, lens);
   if (seg && (!w.w_qkv_tc || !w.w_o_tc || !w.w_1_tc || !w.w_2_tc || m->k2 != 1)) return FS2_ERR_ARG;
   fs2_conv1d_args c = conv_args(f.x, B, T, D, 3 * D, 1, f.qkv);
-  mode.weights(c, w.w_qkv, w.w_qkv_tc, w.b_qkv);
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(mode.run(c, w.w_qkv, w.w_qkv_tc, w.b_qkv, s));
   fs2_attention_args at{};
   at.qkv = f.qkv; at.ctx = f.ctx; at.B = B; at.T = T; at.H = m->n_head; at.Dh = D / m->n_head; at.key_lens = lens;
   at.scale = 1.0f / sqrtf((float)(D / m->n_head));
@@ -181,28 +210,25 @@ static int fft_block(cudaStream_t s, const fs2_acoustic_model* m, const fs2_fft_
     FS2_TRY(attention_simt(&at, s, ragged, 0));
   }
   c = conv_args(f.ctx, B, T, D, D, 1, f.tmp);
-  mode.weights(c, w.w_o, w.w_o_tc, w.b_o);
   c.res = f.x;
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(mode.run(c, w.w_o, w.w_o_tc, w.b_o, s));
   fs2_layernorm_args n{};                                           // both LayerNorms: tmp -> x, padded rows zeroed
   n.x = f.tmp; n.y = f.x; n.B = B; n.T = T; n.C = D; n.eps = 1e-5f; n.row_lens = lens;
   n.gamma = w.ln1_g; n.beta = w.ln1_b;
-  FS2_TRY(layernorm(&n, s));
+  FS2_TRY(layernorm(&n, s, voice_row(mode.vs, &w.ln1_g, &w.ln1_b)));
   // conv-FFN.  K-segmented: w_1 leaves the pre-activation hidden and the ReLU is w_2's input activation (leaky_relu with slope 0)
   c = conv_args(f.x, B, T, D, F, m->k1, f.hid);
-  mode.weights(c, w.w_1, w.w_1_tc, w.b_1);
   if (!seg) c.out_act = FS2_ACT_RELU;
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(mode.run(c, w.w_1, w.w_1_tc, w.b_1, s));
   c = conv_args(f.hid, B, T, F, D, m->k2, f.tmp);
-  mode.weights(c, w.w_2, w.w_2_tc, w.b_2);
   c.res = f.x;
   if (seg) { c.in_act = FS2_ACT_LRELU; c.in_slope = 0.f; }
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(mode.run(c, w.w_2, w.w_2_tc, w.b_2, s));
   n.gamma = w.ln2_g; n.beta = w.ln2_b;
-  return layernorm(&n, s);
+  return layernorm(&n, s, voice_row(mode.vs, &w.ln2_g, &w.ln2_b));
 }
 
 static bool model_ok(const fs2_acoustic_model* m) {
@@ -229,32 +255,33 @@ static FftBufs fft_bufs(Arena& ar, const fs2_acoustic_model* m, size_t rows, int
 // VariancePredictor.forward (+ bucketize / embedding add when bins != NULL) on rows [B][T]  (model/modules.py:242-250, :80-100).
 // `head` carries the caller's part of the head's arguments: B, L = T, lens, control, target, bins, emb, pred_out, and x, which is
 // both the predictor's input and where the embedding is added.  Ragged: the convs and LayerNorms are bounded by head.lens.
-// ctl: the per-element control that replaces head.control (ctl.v NULL: the scalar).
+// ctl: the per-element control that replaces head.control (ctl.v NULL: the scalar).  vs: the voices mode, or NULL (w is then one of m's
+// predictors, and head.bins / head.emb m's tables of the same quantity).
 static int run_predictor(cudaStream_t s, const fs2_acoustic_model* m, const fs2_predictor_weights& w, fs2_variance_head_args head,
-                         float* h1, float* h2, bool ragged, const ControlView& ctl = ControlView{}) {
+                         float* h1, float* h2, bool ragged, const ControlView& ctl, const VoiceSet* vs) {
   const int B = head.B, T = head.L, k = m->vp_kernel, D = m->d_model, VF = m->vp_filter;
   const bool seg = (m->tc_mask & FS2_TC_PREDICTORS) && w.w_c1_tc && w.w_c2_tc;   // K-segmented: the ReLU is applied by the LayerNorm
-  const ConvMode mode{seg ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};
+  const ConvMode mode{seg ? ConvMode::SEGMENTED : ConvMode::EXACT, 0, vs};
   const int32_t* rag = ragged_lens(ragged, head.lens);
   fs2_layernorm_args n{};                                           // both LayerNorms: h1 -> h2, unmasked (ragged: masked)
   n.x = h1; n.y = h2; n.B = B; n.T = T; n.C = VF; n.eps = 1e-5f; n.pre_relu = seg; n.row_lens = rag;
   fs2_conv1d_args c = conv_args(head.x, B, T, D, VF, k, h1);
-  mode.weights(c, w.w_c1, w.w_c1_tc, w.b_c1);
   if (!seg) c.out_act = FS2_ACT_RELU;
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(mode.run(c, w.w_c1, w.w_c1_tc, w.b_c1, s));
   n.gamma = w.ln1_g; n.beta = w.ln1_b;
-  FS2_TRY(layernorm(&n, s));
+  FS2_TRY(layernorm(&n, s, voice_row(vs, &w.ln1_g, &w.ln1_b)));
   c = conv_args(h2, B, T, VF, VF, k, h1);
-  mode.weights(c, w.w_c2, w.w_c2_tc, w.b_c2);
   c.pad_left = 1;                                                   // padding=1 is hard-coded upstream
   if (!seg) c.out_act = FS2_ACT_RELU;
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(mode.run(c, w.w_c2, w.w_c2_tc, w.b_c2, s));
   n.gamma = w.ln2_g; n.beta = w.ln2_b;
-  FS2_TRY(layernorm(&n, s));
+  FS2_TRY(layernorm(&n, s, voice_row(vs, &w.ln2_g, &w.ln2_b)));
   head.h = h2; head.w = w.w_out; head.b = w.b_out; head.C = VF; head.n_edges = m->n_bins - 1; head.D = D;
-  return variance_head(&head, s, &ctl);
+  const bool pitch = &w == &m->pitch;                              // the bins and embedding of the predictor's quantity (none: durations)
+  return variance_head(&head, s, &ctl, voice_row(vs, &w.w_out, &w.b_out, pitch ? &m->pitch_bins : &m->energy_bins,
+                                                 pitch ? &m->pitch_emb : &m->energy_emb));
 }
 
 // The p (pitch / energy) or d (durations) control of fs2_control_args on the phase's [B][L] rows; ragged: columns l >= lens[b] are not read.
@@ -265,27 +292,32 @@ static ControlView control_view(const float* v, int64_t sb, int64_t sl, bool rag
 // ------------------------------------------------------------------ phase 1
 // ragged: utterance b has src_lens[b] phonemes; x_adapted rows at or beyond it are left unspecified.
 // ctl: NULL, or the per-element p / d controls that replace a->p_control / a->d_control where their pointers are set.
+// voices: NULL, or the voices mode (m = voices->models[0]): the staged table is the workspace's first allocation, so the workspace is the
+// single model's plus that table.
 static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, cudaStream_t s, Arena& ar,
-                       bool ragged) {
+                       bool ragged, const fs2_acoustic_voices* voices = nullptr) {
   const int B = a->B, L = a->L, D = m->d_model, VF = m->vp_filter;
   const size_t rows = (size_t)B * L;
+  int32_t* staged = voices ? (int32_t*)ar.take((size_t)2 * B * sizeof(int32_t)) : nullptr;
   FftBufs f = fft_bufs(ar, m, rows);
   float* h1 = ar.f32(rows * VF);
   float* h2 = ar.f32(rows * VF);
   if (ar.dry) return FS2_OK;
-  if (!f.x || !f.tmp || !f.qkv || !f.ctx || !f.hid || !h1 || !h2) return FS2_ERR_WORKSPACE;
+  if (!f.x || !f.tmp || !f.qkv || !f.ctx || !f.hid || !h1 || !h2 || (voices && !staged)) return FS2_ERR_WORKSPACE;
   if (L > m->enc_pos_rows) return FS2_ERR_ARG;
+  const VoiceSet vset{m, voices ? voices->models_dev : nullptr, staged, voices ? voices->voice : nullptr, voices ? voices->n : 0, {}, {}};
+  const VoiceSet* vs = voices ? &vset : nullptr;
 
   fs2_embed_args e{};
   e.ids = a->texts; e.table = m->word_emb; e.pos = m->enc_pos; e.y = f.x; e.B = B; e.L = L; e.D = D; e.n_vocab = m->n_vocab;
-  FS2_TRY(embed_positions(&e, s));
-  const ConvMode enc_mode{(m->tc_mask & FS2_TC_ENCODER) ? ConvMode::SEGMENTED : ConvMode::EXACT, 0};   // exact attention either way
+  FS2_TRY(embed_positions(&e, s, vs ? vs->row(&m->word_emb, &m->enc_pos, nullptr, nullptr, true) : nullptr));
+  const ConvMode enc_mode{(m->tc_mask & FS2_TC_ENCODER) ? ConvMode::SEGMENTED : ConvMode::EXACT, 0, vs};   // exact attention either way
   for (int i = 0; i < m->n_enc; i++) FS2_TRY(fft_block(s, m, m->enc[i], f, B, L, a->src_lens, enc_mode, ragged));
   if (m->spk_emb) {
     if (!a->speakers) return FS2_ERR_ARG;
     fs2_rowbias_args r{};
     r.x = f.x; r.table = m->spk_emb; r.idx = a->speakers; r.B = B; r.L = L; r.D = D; r.n_rows = m->n_speakers;
-    FS2_TRY(add_speaker(&r, s));
+    FS2_TRY(add_speaker(&r, s, voice_row(vs, &m->spk_emb)));
   }
   // x_adapted starts as the encoder output; pitch / energy embeddings are added in place (modules.py:117-126)
   cudaError_t ce = cudaMemcpyAsync(a->x_adapted, f.x, rows * D * sizeof(float), cudaMemcpyDeviceToDevice, s);
@@ -294,18 +326,18 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, co
   // duration on the un-embedded x; pitch on x; energy on x + pitch embedding.  energy uses p_control (modules.py:124).
   fs2_variance_head_args v{};
   v.x = a->x_adapted; v.B = B; v.L = L; v.lens = a->src_lens; v.control = 1.f; v.pred_out = a->logd_pred;
-  FS2_TRY(run_predictor(s, m, m->dur, v, h1, h2, ragged));
+  FS2_TRY(run_predictor(s, m, m->dur, v, h1, h2, ragged, ControlView{}, vs));
   v.control = a->p_control;
   const ControlView p_ctl = ctl ? control_view(ctl->p, ctl->p_stride_b, ctl->p_stride_l, ragged, a->src_lens) : ControlView{};
   if (!m->pitch_frame_level) {
     if (!a->p_pred) return FS2_ERR_ARG;
     v.target = a->p_target; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred;
-    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged, p_ctl));
+    FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged, p_ctl, vs));
   }
   if (!m->energy_frame_level) {
     if (!a->e_pred) return FS2_ERR_ARG;
     v.target = a->e_target; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred;
-    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged, p_ctl));
+    FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged, p_ctl, vs));
   }
 
   fs2_durations_args d{};
@@ -313,7 +345,7 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, co
   d.B = B; d.L = L; d.d_rounded = a->d_target ? nullptr : a->d_rounded; d.cum = a->cum_dur; d.mel_lens = a->mel_lens;
   d.mel_lens32 = a->mel_lens32; d.len_stats = a->len_stats;
   const ControlView d_ctl = ctl ? control_view(ctl->d, ctl->d_stride_b, ctl->d_stride_l, ragged, a->src_lens) : ControlView{};
-  FS2_TRY(durations(&d, s, ragged_lens(ragged, a->src_lens), &d_ctl));
+  FS2_TRY(durations(&d, s, ragged_lens(ragged, a->src_lens), &d_ctl, vs ? staged + B : nullptr));
   if (a->len_stats_host) {
     ce = cudaMemcpyAsync(a->len_stats_host, a->len_stats, 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
     if (ce != cudaSuccess) return FS2_ERR_CUDA - (int)ce;
@@ -324,23 +356,27 @@ static int encode_impl(const fs2_acoustic_model* m, const fs2_encode_args* a, co
 // ------------------------------------------------------------------ phase 2
 // ragged: utterance b has mel_mask_lens[b] frames; mel and postnet_mel rows at or beyond it are zeroed.
 // ctl: NULL, or the per-frame p control that replaces a->p_control when ctl->p is set (ctl->d is not read).
+// voices: NULL, or the voices mode, as in encode_impl.
 static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, cudaStream_t s, Arena& ar,
-                       bool ragged) {
+                       bool ragged, const fs2_acoustic_voices* voices = nullptr) {
   const int B = a->B, T = a->T, D = m->d_model;
   const size_t rows = (size_t)B * T;
+  int32_t* staged = voices ? (int32_t*)ar.take((size_t)2 * B * sizeof(int32_t)) : nullptr;
   FftBufs f = fft_bufs(ar, m, rows, B, T, (m->tc_mask & FS2_TC_DECODER) != 0);
   int pc = 0;
   for (int i = 0; i < m->n_postnet; i++) pc = pc > m->post_cout[i] ? pc : m->post_cout[i];
   float* pa = ar.f32(rows * pc);
   float* pb = ar.f32(rows * pc);
   if (ar.dry) return FS2_OK;
-  if (!f.x || !f.tmp || !f.qkv || !f.ctx || !f.hid || !pa || !pb || (f.att_bytes && !f.att_ws)) return FS2_ERR_WORKSPACE;
+  if (!f.x || !f.tmp || !f.qkv || !f.ctx || !f.hid || !pa || !pb || (f.att_bytes && !f.att_ws) || (voices && !staged)) return FS2_ERR_WORKSPACE;
   if (T > m->dec_pos_rows) return FS2_ERR_ARG;
+  const VoiceSet vset{m, voices ? voices->models_dev : nullptr, staged, voices ? voices->voice : nullptr, voices ? voices->n : 0, {}, {}};
+  const VoiceSet* vs = voices ? &vset : nullptr;
 
   const bool frame_level = m->pitch_frame_level || m->energy_frame_level;
   fs2_length_regulate_args lr{};
   lr.x = a->x_adapted; lr.cum = a->cum_dur; lr.pos = frame_level ? nullptr : m->dec_pos; lr.y = f.x; lr.B = B; lr.L = a->L; lr.T = T; lr.D = D;
-  FS2_TRY(length_regulate(&lr, s));
+  FS2_TRY(length_regulate(&lr, s, vs ? vs->row(&m->dec_pos, nullptr, nullptr, nullptr, true) : nullptr));
   if (frame_level) {                                   // frame-level pitch / energy (model/modules.py:139-148), then the position add
     float* h1 = f.hid;                                 // [rows][d_inner] is free here and d_inner >= 2 * vp_filter is checked below
     float* h2 = f.hid + rows * m->vp_filter;
@@ -351,36 +387,34 @@ static int decode_impl(const fs2_acoustic_model* m, const fs2_decode_args* a, co
     if (m->pitch_frame_level) {
       if (!a->p_pred_frames) return FS2_ERR_ARG;
       v.target = a->p_target_frames; v.bins = m->pitch_bins; v.emb = m->pitch_emb; v.pred_out = a->p_pred_frames;
-      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged, p_ctl));
+      FS2_TRY(run_predictor(s, m, m->pitch, v, h1, h2, ragged, p_ctl, vs));
     }
     if (m->energy_frame_level) {
       if (!a->e_pred_frames) return FS2_ERR_ARG;
       v.target = a->e_target_frames; v.bins = m->energy_bins; v.emb = m->energy_emb; v.pred_out = a->e_pred_frames;
-      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged, p_ctl));
+      FS2_TRY(run_predictor(s, m, m->energy, v, h1, h2, ragged, p_ctl, vs));
     }
-    FS2_TRY(add_positions(f.x, m->dec_pos, B, T, D, s));
+    FS2_TRY(add_positions(f.x, m->dec_pos, B, T, D, s, voice_row(vs, &m->dec_pos)));
   }
   const ConvMode dec_mode{(m->tc_mask & FS2_TC_DECODER) ? ConvMode::TC : ConvMode::EXACT,
-                          (m->tc_mask & FS2_TC_DECODER_F8) ? FS2_TC_VARIANT_F8 : 0u};
+                          (m->tc_mask & FS2_TC_DECODER_F8) ? FS2_TC_VARIANT_F8 : 0u, vs};
   for (int i = 0; i < m->n_dec; i++) FS2_TRY(fft_block(s, m, m->dec[i], f, B, T, a->mel_mask_lens, dec_mode, ragged));
   const ConvMode post_mode{(m->tc_mask & FS2_TC_POSTNET) ? ConvMode::TC : ConvMode::EXACT,
-                           (m->tc_mask & FS2_TC_POSTNET_F8) ? FS2_TC_VARIANT_F8 : 0u};
+                           (m->tc_mask & FS2_TC_POSTNET_F8) ? FS2_TC_VARIANT_F8 : 0u, vs};
   const int32_t* rag = ragged_lens(ragged, a->mel_mask_lens);
   fs2_conv1d_args c = conv_args(f.x, B, T, D, m->n_mel, 1, a->mel);
-  post_mode.weights(c, m->w_mel, m->w_mel_tc, m->b_mel);
   c.x_lens = rag;
-  FS2_TRY(conv1d_dispatch(&c, s));
+  FS2_TRY(post_mode.run(c, m->w_mel, m->w_mel_tc, m->b_mel, s));
   // PostNet: eval BatchNorm folded into (w, b) by the packer; unmasked, tanh on all but the last (Layers.py:129-137)
   const float* cur = a->mel;
   for (int i = 0; i < m->n_postnet; i++) {
     const bool last = i == m->n_postnet - 1;
     float* dst = last ? a->postnet_mel : ((i & 1) ? pb : pa);
     c = conv_args(cur, B, T, m->post_cin[i], m->post_cout[i], m->post_k, dst);
-    post_mode.weights(c, m->w_post[i], m->w_post_tc[i], m->b_post[i]);
     if (last) c.res = a->mel;
     else c.out_act = FS2_ACT_TANH;
     c.x_lens = rag;
-    FS2_TRY(conv1d_dispatch(&c, s));
+    FS2_TRY(post_mode.run(c, m->w_post[i], m->w_post_tc[i], m->b_post[i], s));
     cur = dst;
   }
   if (ragged) return zero_tail(a->mel, a->postnet_mel, a->mel_mask_lens, B, T, m->n_mel, s);   // the convs left those rows unspecified
@@ -907,7 +941,9 @@ static bool control_ok(const fs2_control_args* c, int ragged) {
          (!c || (c->p_stride_b >= 0 && c->p_stride_l >= 0 && c->d_stride_b >= 0 && c->d_stride_l >= 0));
 }
 
-int fs2_acoustic_encode_ctl(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st) {
+// voices: NULL, or the voices mode (m = voices->models[0], checked by the caller)
+static int encode_call(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st,
+                       const fs2_acoustic_voices* voices = nullptr) {
   if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0 || !control_ok(ctl, ragged)) return FS2_ERR_ARG;
   if (!a->texts || !a->src_lens || !a->logd_pred || !a->mel_lens || !a->cum_dur || !a->x_adapted ||
       !a->len_stats || !a->workspace)
@@ -915,7 +951,10 @@ int fs2_acoustic_encode_ctl(const fs2_acoustic_model* m, const fs2_encode_args* 
   if (!a->d_target && !a->d_rounded) return FS2_ERR_ARG;
   if (m->d_model / m->n_head != 128) return FS2_ERR_UNSUPPORTED;
   Arena ar(a->workspace, a->workspace_bytes);
-  return encode_impl(m, a, ctl, S(st), ar, ragged != 0);
+  return encode_impl(m, a, ctl, S(st), ar, ragged != 0, voices);
+}
+int fs2_acoustic_encode_ctl(const fs2_acoustic_model* m, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st) {
+  return encode_call(m, a, ctl, ragged, st);
 }
 int fs2_acoustic_encode(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return fs2_acoustic_encode_ctl(m, a, nullptr, 0, st); }
 int fs2_acoustic_encode_ragged(const fs2_acoustic_model* m, const fs2_encode_args* a, fs2_stream_t st) { return fs2_acoustic_encode_ctl(m, a, nullptr, 1, st); }
@@ -929,15 +968,94 @@ size_t fs2_decode_workspace_bytes(const fs2_acoustic_model* m, int B, int T) {
   return ar.off + 256;
 }
 
-int fs2_acoustic_decode_ctl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st) {
+static int decode_call(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st,
+                       const fs2_acoustic_voices* voices = nullptr) {
   if (!model_ok(m) || !a || a->B <= 0 || a->L <= 0 || a->T <= 0 || !control_ok(ctl, ragged)) return FS2_ERR_ARG;
   if (!a->x_adapted || !a->cum_dur || !a->mel_mask_lens || !a->mel || !a->postnet_mel || !a->workspace) return FS2_ERR_ARG;
   if (m->d_model / m->n_head != 128) return FS2_ERR_UNSUPPORTED;
   Arena ar(a->workspace, a->workspace_bytes);
-  return decode_impl(m, a, ctl, S(st), ar, ragged != 0);
+  return decode_impl(m, a, ctl, S(st), ar, ragged != 0, voices);
+}
+int fs2_acoustic_decode_ctl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged, fs2_stream_t st) {
+  return decode_call(m, a, ctl, ragged, st);
 }
 int fs2_acoustic_decode(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return fs2_acoustic_decode_ctl(m, a, nullptr, 0, st); }
 int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_args* a, fs2_stream_t st) { return fs2_acoustic_decode_ctl(m, a, nullptr, 1, st); }
+
+static_assert(sizeof(fs2_acoustic_voices) == 32, "fs2_acoustic_voices: an int32 and three pointers");
+
+// Voice k of a voices call runs on voice 0's plan and kernels: the same config and precision policy, and every weight pointer NULL
+// where voice 0's is, else at the same address modulo 16 (the format choices and alignment checks made on voice 0).
+static bool same_acoustic_layout(const fs2_acoustic_model* a, const fs2_acoustic_model* b) {
+  if (a->d_model != b->d_model || a->n_head != b->n_head || a->d_inner != b->d_inner || a->k1 != b->k1 || a->k2 != b->k2 ||
+      a->n_enc != b->n_enc || a->n_dec != b->n_dec || a->n_mel != b->n_mel || a->vp_filter != b->vp_filter ||
+      a->vp_kernel != b->vp_kernel || a->n_bins != b->n_bins || a->n_vocab != b->n_vocab || a->n_speakers != b->n_speakers ||
+      a->tc_mask != b->tc_mask || a->pitch_frame_level != b->pitch_frame_level || a->energy_frame_level != b->energy_frame_level ||
+      a->n_postnet != b->n_postnet || a->post_k != b->post_k)
+    return false;
+  for (int i = 0; i < a->n_postnet; i++)
+    if (a->post_cin[i] != b->post_cin[i] || a->post_cout[i] != b->post_cout[i]) return false;
+  auto same = [](const float* p, const float* q) { return !p == !q && ((uintptr_t)p & 15u) == ((uintptr_t)q & 15u); };
+  // the weight structs hold pointers only: compared as arrays of them
+  auto same_all = [&](const void* p, const void* q, size_t bytes) {
+    bool ok = true;
+    for (size_t i = 0; i < bytes / sizeof(const float*); i++) ok = ok && same(((const float* const*)p)[i], ((const float* const*)q)[i]);
+    return ok;
+  };
+  bool ok = same(a->word_emb, b->word_emb) && same(a->enc_pos, b->enc_pos) && same(a->dec_pos, b->dec_pos) &&
+            same(a->spk_emb, b->spk_emb) && same(a->pitch_bins, b->pitch_bins) && same(a->energy_bins, b->energy_bins) &&
+            same(a->pitch_emb, b->pitch_emb) && same(a->energy_emb, b->energy_emb) && same(a->w_mel, b->w_mel) &&
+            same(a->b_mel, b->b_mel) && same(a->w_mel_tc, b->w_mel_tc);
+  for (int i = 0; i < a->n_enc; i++) ok = ok && same_all(&a->enc[i], &b->enc[i], sizeof(fs2_fft_block_weights));
+  for (int i = 0; i < a->n_dec; i++) ok = ok && same_all(&a->dec[i], &b->dec[i], sizeof(fs2_fft_block_weights));
+  ok = ok && same_all(&a->dur, &b->dur, sizeof(fs2_predictor_weights)) && same_all(&a->pitch, &b->pitch, sizeof(fs2_predictor_weights)) &&
+       same_all(&a->energy, &b->energy, sizeof(fs2_predictor_weights));
+  for (int i = 0; i < a->n_postnet; i++)
+    ok = ok && same(a->w_post[i], b->w_post[i]) && same(a->b_post[i], b->b_post[i]) && same(a->w_post_tc[i], b->w_post_tc[i]);
+  return ok;
+}
+
+// n, the models and their layouts (what the workspace bounds need); calls also need models_dev and voice
+static bool voice_models_ok(const fs2_acoustic_voices* v) {
+  if (!v || v->n < 1 || v->n > FS2_MAX_VOICES || !v->models) return false;
+  for (int k = 0; k < v->n; k++)
+    if (!model_ok(v->models[k]) || !same_acoustic_layout(v->models[0], v->models[k])) return false;
+  return true;
+}
+
+size_t fs2_encode_voices_workspace_bytes(const fs2_acoustic_voices* v, int B, int L) {
+  if (!voice_models_ok(v) || B <= 0 || L <= 0) return 0;
+  Arena ar(nullptr, 0);
+  fs2_encode_args a{};
+  a.B = B; a.L = L;
+  encode_impl(v->models[0], &a, nullptr, nullptr, ar, false, v);
+  return ar.off + 256;
+}
+
+size_t fs2_decode_voices_workspace_bytes(const fs2_acoustic_voices* v, int B, int T) {
+  if (!voice_models_ok(v) || B <= 0 || T <= 0) return 0;
+  Arena ar(nullptr, 0);
+  fs2_decode_args a{};
+  a.B = B; a.T = T;
+  decode_impl(v->models[0], &a, nullptr, nullptr, ar, false, v);
+  return ar.off + 256;
+}
+
+int fs2_acoustic_encode_voices(const fs2_acoustic_voices* v, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged,
+                               fs2_stream_t st) {
+  if (!voice_models_ok(v) || !v->models_dev || !v->voice || !a) return FS2_ERR_ARG;
+  for (int k = 0; k < v->n; k++)
+    if (a->L > v->models[k]->enc_pos_rows) return FS2_ERR_ARG;
+  return encode_call(v->models[0], a, ctl, ragged, st, v);
+}
+
+int fs2_acoustic_decode_voices(const fs2_acoustic_voices* v, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged,
+                               fs2_stream_t st) {
+  if (!voice_models_ok(v) || !v->models_dev || !v->voice || !a) return FS2_ERR_ARG;
+  for (int k = 0; k < v->n; k++)
+    if (a->T > v->models[k]->dec_pos_rows) return FS2_ERR_ARG;
+  return decode_call(v->models[0], a, ctl, ragged, st, v);
+}
 
 static bool vocoder_ok(const fs2_vocoder_model* m) {
   if (!(m && m->n_stages > 0 && m->n_stages <= FS2_MAX_STAGES && m->n_kernels > 0 && m->n_kernels <= FS2_MAX_DIL + 4 &&

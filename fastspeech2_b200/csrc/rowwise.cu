@@ -5,13 +5,23 @@
 
 namespace fs2 {
 
+// VOICE (the row kernels' template parameter): the voices mode, vr naming the tables each utterance reads from its voice (VoiceRow).
+// An instantiation of its own, so that the offline one keeps its code.
+
 // ------------------------------------------------------------------ embedding + position (Models.py:89-91)
+// Voices mode: the first launch of phase 1, which stages the voice table; r[0] the word embedding, r[1] the positions.
+template <bool VOICE>
 __global__ void embed_kernel(const long long* __restrict__ ids, const float* __restrict__ table,
-                             const float* __restrict__ pos, float* __restrict__ y, int B, int L, int D4, int n_vocab) {
+                             const float* __restrict__ pos, float* __restrict__ y, int B, int L, int D4, int n_vocab, const VoiceRow vr) {
+  if constexpr (VOICE) voice_stage(vr, B);
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= B * L) return;
   const int lane = threadIdx.x & 31;
   const int l = row % L;
+  if constexpr (VOICE) {
+    table = voice_table(vr, row / L, 0);
+    pos = voice_table(vr, row / L, 1);
+  }
   long long id = ids[row];
   if (id < 0 || id >= n_vocab) id = 0;  // the reference would raise; stay in bounds
   const float4* e = reinterpret_cast<const float4*>(table) + id * D4;
@@ -23,22 +33,26 @@ __global__ void embed_kernel(const long long* __restrict__ ids, const float* __r
   }
 }
 
-int embed_positions(const fs2_embed_args* a, cudaStream_t s) {
+int embed_positions(const fs2_embed_args* a, cudaStream_t s, const VoiceRow* vr) {
   if (!a || !a->ids || !a->table || !a->pos || !a->y || a->B <= 0 || a->L <= 0 || a->D <= 0) return FS2_ERR_ARG;
   if (a->D % 4) return FS2_ERR_UNSUPPORTED;
   const int rows = a->B * a->L;
-  embed_kernel<<<(rows + 7) / 8, 256, 0, s>>>(reinterpret_cast<const long long*>(a->ids), a->table, a->pos, a->y, a->B, a->L,
-                                              a->D / 4, a->n_vocab);
+  const long long* ids = reinterpret_cast<const long long*>(a->ids);
+  if (vr) embed_kernel<true><<<(rows + 7) / 8, 256, 0, s>>>(ids, a->table, a->pos, a->y, a->B, a->L, a->D / 4, a->n_vocab, *vr);
+  else embed_kernel<false><<<(rows + 7) / 8, 256, 0, s>>>(ids, a->table, a->pos, a->y, a->B, a->L, a->D / 4, a->n_vocab, VoiceRow{});
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
 // ------------------------------------------------------------------ speaker add (fastspeech2.py:68-71)
+// Voices mode: r[0] the speaker table
+template <bool VOICE>
 __global__ void rowbias_kernel(float* __restrict__ x, const float* __restrict__ table, const long long* __restrict__ idx, int B,
-                               int L, int D4, int n_rows) {
+                               int L, int D4, int n_rows, const VoiceRow vr) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= B * L) return;
   const int lane = threadIdx.x & 31;
+  if constexpr (VOICE) table = voice_table(vr, row / L, 0);
   long long id = idx[row / L];
   if (id < 0 || id >= n_rows) id = 0;
   const float4* e = reinterpret_cast<const float4*>(table) + id * D4;
@@ -51,22 +65,26 @@ __global__ void rowbias_kernel(float* __restrict__ x, const float* __restrict__ 
   }
 }
 
-int add_speaker(const fs2_rowbias_args* a, cudaStream_t s) {
+int add_speaker(const fs2_rowbias_args* a, cudaStream_t s, const VoiceRow* vr) {
   if (!a || !a->x || !a->table || !a->idx || a->B <= 0 || a->L <= 0 || a->D <= 0) return FS2_ERR_ARG;
   if (a->D % 4) return FS2_ERR_UNSUPPORTED;
   const int rows = a->B * a->L;
-  rowbias_kernel<<<(rows + 7) / 8, 256, 0, s>>>(a->x, a->table, reinterpret_cast<const long long*>(a->idx), a->B, a->L, a->D / 4,
-                                                a->n_rows);
+  const long long* idx = reinterpret_cast<const long long*>(a->idx);
+  if (vr) rowbias_kernel<true><<<(rows + 7) / 8, 256, 0, s>>>(a->x, a->table, idx, a->B, a->L, a->D / 4, a->n_rows, *vr);
+  else rowbias_kernel<false><<<(rows + 7) / 8, 256, 0, s>>>(a->x, a->table, idx, a->B, a->L, a->D / 4, a->n_rows, VoiceRow{});
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
 // ------------------------------------------------------------------ x[b,t,:] += pos[t,:]
-__global__ void add_positions_kernel(float* __restrict__ x, const float* __restrict__ pos, long long rows, int T, int D4) {
+// Voices mode: r[0] the positions
+template <bool VOICE>
+__global__ void add_positions_kernel(float* __restrict__ x, const float* __restrict__ pos, long long rows, int T, int D4, const VoiceRow vr) {
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   const int t = (int)(row % T);
+  if constexpr (VOICE) pos = voice_table(vr, (int)(row / T), 0);
   float4* o = reinterpret_cast<float4*>(x) + row * D4;
   const float4* p = reinterpret_cast<const float4*>(pos) + (long long)t * D4;
   for (int c = lane; c < D4; c += 32) {
@@ -77,20 +95,23 @@ __global__ void add_positions_kernel(float* __restrict__ x, const float* __restr
   }
 }
 
-int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s) {
+int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s, const VoiceRow* vr) {
   if (!x || !pos || B <= 0 || T <= 0 || D <= 0) return FS2_ERR_ARG;
   if (D % 4) return FS2_ERR_UNSUPPORTED;
   const long long rows = (long long)B * T;
-  add_positions_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(x, pos, rows, T, D / 4);
+  if (vr) add_positions_kernel<true><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(x, pos, rows, T, D / 4, *vr);
+  else add_positions_kernel<false><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(x, pos, rows, T, D / 4, VoiceRow{});
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
 
 // ------------------------------------------------------------------ LayerNorm + pad-row zeroing
 // One warp per row; the row lives in registers (C <= 1024), two-pass mean / variance like ATen's CPU kernel.
+// Voices mode: r[0] gamma, r[1] beta.
+template <bool VOICE>
 __global__ void layernorm_kernel(const float* __restrict__ x, float* __restrict__ y, int rows, int T, int C4,
                                  const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                                 const int* __restrict__ row_lens, int pre_relu) {
+                                 const int* __restrict__ row_lens, int pre_relu, const VoiceRow vr) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -126,6 +147,10 @@ __global__ void layernorm_kernel(const float* __restrict__ x, float* __restrict_
     }
   }
   const float rstd = rsqrtf(warp_sum(sq) * inv_c + eps);
+  if constexpr (VOICE) {
+    gamma = voice_table(vr, row / T, 0);
+    beta = voice_table(vr, row / T, 1);
+  }
   const float4* g4 = reinterpret_cast<const float4*>(gamma);
   const float4* b4 = reinterpret_cast<const float4*>(beta);
 #pragma unroll
@@ -139,14 +164,18 @@ __global__ void layernorm_kernel(const float* __restrict__ x, float* __restrict_
   }
 }
 
-int layernorm(const fs2_layernorm_args* a, cudaStream_t s) {
+int layernorm(const fs2_layernorm_args* a, cudaStream_t s, const VoiceRow* vr) {
   if (!a || !a->x || !a->y || !a->gamma || !a->beta || a->B <= 0 || a->T <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->C % 4 || a->C > 1024) return FS2_ERR_UNSUPPORTED;
   const long long rows = (long long)a->B * a->T;
   if (rows > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   prof_before(s);
-  layernorm_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(a->x, a->y, (int)rows, a->T, a->C / 4, a->gamma, a->beta, a->eps,
-                                                             a->row_lens, a->pre_relu);
+  if (vr)
+    layernorm_kernel<true><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(a->x, a->y, (int)rows, a->T, a->C / 4, a->gamma, a->beta, a->eps,
+                                                                     a->row_lens, a->pre_relu, *vr);
+  else
+    layernorm_kernel<false><<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(a->x, a->y, (int)rows, a->T, a->C / 4, a->gamma, a->beta, a->eps,
+                                                                      a->row_lens, a->pre_relu, VoiceRow{});
   prof_after(s, 2, 0.0);
   FS2_LAUNCH_CHECK();
   return FS2_OK;
@@ -155,12 +184,18 @@ int layernorm(const fs2_layernorm_args* a, cudaStream_t s) {
 // ------------------------------------------------------------------ variance head (modules.py:80-100, :246-250)
 // CTL: the prediction is scaled by the per-element control ctl instead of the scalar a.control (a template parameter so that the
 // scalar path keeps its code and registers).  Both are one fp32 multiply: a control array of fp32(c) gives the scalar c's bits.
-template <bool CTL>
-__global__ void variance_head_kernel(const fs2_variance_head_args a, const ControlView ctl) {
+// Voices mode: r[0] w, r[1] b, r[2] bins, r[3] emb.
+template <bool CTL, bool VOICE>
+__global__ void variance_head_kernel(fs2_variance_head_args a, const ControlView ctl, const VoiceRow vr) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= a.B * a.L) return;
   const int lane = threadIdx.x & 31;
   const int b = row / a.L, l = row - b * a.L;
+  if constexpr (VOICE) {
+    a.w = voice_table(vr, b, 0);
+    a.b = voice_table(vr, b, 1);
+    if (a.bins) { a.bins = voice_table(vr, b, 2); a.emb = voice_table(vr, b, 3); }
+  }
   const float4* h = reinterpret_cast<const float4*>(a.h) + (long long)row * (a.C / 4);
   const float4* w = reinterpret_cast<const float4*>(a.w);
   float acc = 0.f;
@@ -200,13 +235,16 @@ __global__ void variance_head_kernel(const fs2_variance_head_args a, const Contr
 }
 
 // ctl: NULL or ctl->v NULL for the scalar a->control
-int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl) {
+int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const ControlView* ctl, const VoiceRow* vr) {
   if (!a || !a->h || !a->w || !a->b || !a->pred_out || a->B <= 0 || a->L <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->C % 4) return FS2_ERR_UNSUPPORTED;
   if (a->bins && (!a->emb || !a->x || a->n_edges <= 0 || a->D <= 0 || a->D % 4)) return FS2_ERR_ARG;
   const int rows = a->B * a->L;
-  if (ctl && ctl->v) variance_head_kernel<true><<<(rows + 7) / 8, 256, 0, s>>>(*a, *ctl);
-  else variance_head_kernel<false><<<(rows + 7) / 8, 256, 0, s>>>(*a, ControlView{});
+  const bool c = ctl && ctl->v;
+  if (vr && c) variance_head_kernel<true, true><<<(rows + 7) / 8, 256, 0, s>>>(*a, *ctl, *vr);
+  else if (vr) variance_head_kernel<false, true><<<(rows + 7) / 8, 256, 0, s>>>(*a, ControlView{}, *vr);
+  else if (c) variance_head_kernel<true, false><<<(rows + 7) / 8, 256, 0, s>>>(*a, *ctl, VoiceRow{});
+  else variance_head_kernel<false, false><<<(rows + 7) / 8, 256, 0, s>>>(*a, ControlView{}, VoiceRow{});
   FS2_LAUNCH_CHECK();
   return FS2_OK;
 }
@@ -215,20 +253,23 @@ int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const Control
 // One CTA per utterance: round-half-even (rintf == torch.round), truncate, block-wide inclusive scan.
 // RAG: ragged batch, columns l >= src_lens[b] do not exist: they are not read, count as 0 frames and d_rounded there is 0.
 // CTL: the per-element control ctl scales the rounded durations in place of the scalar a.d_control (predicted durations only).
-template <bool RAG, bool CTL>
-__global__ void durations_kernel(const fs2_durations_args a, const int* __restrict__ src_lens, const ControlView ctl) {
+// VOICE: voices mode: an utterance whose valid[b] is 0 (its voice index was out of range) has no columns, so 0 frames.
+template <bool RAG, bool CTL, bool VOICE>
+__global__ void durations_kernel(const fs2_durations_args a, const int* __restrict__ src_lens, const ControlView ctl,
+                                 const int* __restrict__ valid) {
   __shared__ int warp_tot[32];
   __shared__ int carry_s;
   const int b = blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int nw = blockDim.x >> 5;
-  const int n = RAG ? ragged_rows(src_lens, 1, a.L, b) : a.L;
+  int n = RAG ? ragged_rows(src_lens, 1, a.L, b) : a.L;
+  if (VOICE && !__ldg(valid + b)) n = 0;
   if (tid == 0) carry_s = 0;
   __syncthreads();
   for (int base = 0; base < a.L; base += blockDim.x) {
     const int l = base + tid;
     int reps = 0;
-    if (RAG && l >= n && l < a.L) {
+    if ((RAG || VOICE) && l >= n && l < a.L) {
       if (!a.use_target && a.d_rounded) a.d_rounded[(long long)b * a.L + l] = 0.f;
     } else if (l < a.L) {
       const float s = a.src[(long long)b * a.L + l];
@@ -283,17 +324,26 @@ __global__ void durations_kernel(const fs2_durations_args a, const int* __restri
 }
 
 // src_lens: the ragged mode's lengths or NULL.  ctl: NULL or ctl->v NULL for the scalar a->d_control; ignored with use_target.
-int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens, const ControlView* ctl) {
+// valid: NULL, or the voices mode's validity flags.
+int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens, const ControlView* ctl, const int32_t* valid) {
   if (!a || !a->src || !a->cum || !a->mel_lens || !a->len_stats || a->B <= 0 || a->L <= 0) return FS2_ERR_ARG;
   cudaError_t e = cudaMemsetAsync(a->len_stats, 0, 3 * sizeof(int), s);
   if (e != cudaSuccess) return FS2_ERR_CUDA - (int)e;
   const ControlView c = (ctl && !a->use_target) ? *ctl : ControlView{};
-  if (c.v) {
-    if (src_lens) durations_kernel<true, true><<<a->B, 256, 0, s>>>(*a, src_lens, c);
-    else durations_kernel<false, true><<<a->B, 256, 0, s>>>(*a, nullptr, c);
+  if (valid) {
+    if (c.v) {
+      if (src_lens) durations_kernel<true, true, true><<<a->B, 256, 0, s>>>(*a, src_lens, c, valid);
+      else durations_kernel<false, true, true><<<a->B, 256, 0, s>>>(*a, nullptr, c, valid);
+    } else {
+      if (src_lens) durations_kernel<true, false, true><<<a->B, 256, 0, s>>>(*a, src_lens, c, valid);
+      else durations_kernel<false, false, true><<<a->B, 256, 0, s>>>(*a, nullptr, c, valid);
+    }
+  } else if (c.v) {
+    if (src_lens) durations_kernel<true, true, false><<<a->B, 256, 0, s>>>(*a, src_lens, c, nullptr);
+    else durations_kernel<false, true, false><<<a->B, 256, 0, s>>>(*a, nullptr, c, nullptr);
   } else {
-    if (src_lens) durations_kernel<true, false><<<a->B, 256, 0, s>>>(*a, src_lens, c);
-    else durations_kernel<false, false><<<a->B, 256, 0, s>>>(*a, nullptr, c);
+    if (src_lens) durations_kernel<true, false, false><<<a->B, 256, 0, s>>>(*a, src_lens, c, nullptr);
+    else durations_kernel<false, false, false><<<a->B, 256, 0, s>>>(*a, nullptr, c, nullptr);
   }
   FS2_LAUNCH_CHECK();
   return FS2_OK;
@@ -323,11 +373,15 @@ int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cu
 // ------------------------------------------------------------------ length regulator gather (modules.py:167-194)
 // One warp per output frame: binary search of the inclusive duration prefix sums (L2/L1 resident, 4*L bytes per utterance),
 // then a coalesced float4 copy of the source phoneme row with the decoder position row added (Models.py:158-160).
-__global__ void length_regulate_kernel(const fs2_length_regulate_args a) {
+// Voices mode: the first launch of phase 2, which stages the voice table; r[0] the positions.
+template <bool VOICE>
+__global__ void length_regulate_kernel(fs2_length_regulate_args a, const VoiceRow vr) {
+  if constexpr (VOICE) voice_stage(vr, a.B);
   const long long frame = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (frame >= (long long)a.B * a.T) return;
   const int lane = threadIdx.x & 31;
   const int b = (int)(frame / a.T), t = (int)(frame - (long long)b * a.T);
+  if constexpr (VOICE) if (a.pos) a.pos = voice_table(vr, b, 0);
   const int* cum = a.cum + (long long)b * a.L;
   const int total = __ldg(cum + a.L - 1);
   const int D4 = a.D / 4;
@@ -353,12 +407,13 @@ __global__ void length_regulate_kernel(const fs2_length_regulate_args a) {
   }
 }
 
-int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s) {
+int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s, const VoiceRow* vr) {
   if (!a || !a->x || !a->cum || !a->y || a->B <= 0 || a->L <= 0 || a->T <= 0 || a->D <= 0) return FS2_ERR_ARG;
   if (a->D % 4) return FS2_ERR_UNSUPPORTED;
   const long long frames = (long long)a->B * a->T;
   prof_before(s);
-  length_regulate_kernel<<<(unsigned)((frames + 7) / 8), 256, 0, s>>>(*a);
+  if (vr) length_regulate_kernel<true><<<(unsigned)((frames + 7) / 8), 256, 0, s>>>(*a, *vr);
+  else length_regulate_kernel<false><<<(unsigned)((frames + 7) / 8), 256, 0, s>>>(*a, VoiceRow{});
   prof_after(s, 3, 0.0);
   FS2_LAUNCH_CHECK();
   return FS2_OK;

@@ -241,14 +241,20 @@ class FastSpeech2(nn.Module):
                                  p_control, e_control, d_control, self.ragged if ragged is None else bool(ragged))
 
     def _forward(self, speakers, texts, src_lens, max_src_len, mels=None, mel_lens=None, max_mel_len=None,
-                 p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0, ragged=False):
-        if self.training:
-            raise NotImplementedError("H100-native FastSpeech2 is inference-only: call .eval() (utils/model.py:32)")
+                 p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0, ragged=False, voices=None):
+        """forward, or with voices = (bank, voice) the VoiceBank call whose voice 0 is self."""
+        for mk in (self,) if voices is None else voices[0].models:
+            if mk.training:
+                raise NotImplementedError("H100-native FastSpeech2 is inference-only: call .eval() (utils/model.py:32)")
         p_frame = self.pitch_feature_level == "frame_level"
         e_frame = self.energy_feature_level == "frame_level"
-        lib = L.lib()
-        m, _keep, dev = self._packed or self._pack()
-        self._packed_state.enter()
+        L.lib()
+        if voices is not None:                         # checked before any packing or device work
+            voices = (voices[0], voices[0]._voice_table(voices[1], int(texts.shape[0]), get(self, "mel_linear.weight").device))
+        for mk in (self,) if voices is None else voices[0].models:
+            mk._packed or mk._pack()
+            mk._packed_state.enter()
+        m, _keep, dev = self._packed
         B, Lmax = int(texts.shape[0]), int(max_src_len)
         if texts.shape[1] != Lmax:
             raise ValueError("texts.shape[1] must equal max_src_len")
@@ -280,17 +286,14 @@ class FastSpeech2(nn.Module):
         p_enc = normalize_control(p_control, (B, Lmax), dev, "p_control") if p_read_enc else _UNREAD_CONTROL
         d_ctl = normalize_control(d_control, (B, Lmax), dev, "d_control") if d_t is None else _UNREAD_CONTROL
 
-        m.enc_pos, m.enc_pos_rows = self._position(0, Lmax, m.d_model, dev)
-        ws = self._workspace(lib.fs2_encode_workspace_bytes(C.byref(m), B, Lmax), dev)
         ea = L.EncodeArgs(B=B, L=Lmax, texts=texts.data_ptr(), speakers=L.ptr(speakers_d), src_lens=src_lens32.data_ptr(),
                           p_control=p_enc[1], e_control=1.0, d_control=d_ctl[1],
                           p_target=0 if p_frame else L.ptr(p_t), e_target=0 if e_frame else L.ptr(e_t), d_target=L.ptr(d_t),
                           p_pred=0 if p_frame else p_pred.data_ptr(), e_pred=0 if e_frame else e_pred.data_ptr(), logd_pred=logd.data_ptr(),
                           d_rounded=d_rounded.data_ptr(), mel_lens=mel_lens_out.data_ptr(), mel_lens32=mel_lens32.data_ptr(),
                           cum_dur=cum.data_ptr(), x_adapted=x_adapted.data_ptr(), len_stats=stats_dev.data_ptr(),
-                          len_stats_host=0, workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        ctl = _control_args(p_enc, d_ctl)
-        L.check(lib.fs2_acoustic_encode_ctl(C.byref(m), C.byref(ea), C.byref(ctl), int(ragged), stream), "fs2_acoustic_encode")
+                          len_stats_host=0)
+        self._phase("encode", B, Lmax, ea, _control_args(p_enc, d_ctl), ragged, stream, dev, voices)
         stats_host.copy_(stats_dev, non_blocking=True)
         self._stats_host = stats_host
 
@@ -310,7 +313,6 @@ class FastSpeech2(nn.Module):
         else:
             mask_lens32 = mel_lens32       # free-running: the adaptor rebuilds the mask from the predicted lengths (modules.py:132-137)
 
-        m.dec_pos, m.dec_pos_rows = self._position(1, T, m.d_model, dev)
         mel = torch.empty(B, T, m.n_mel, **f32)
         post = torch.empty(B, T, m.n_mel, **f32)
         if p_frame:                                    # frame-level predictions have the mel time axis (model/modules.py:139-148)
@@ -322,17 +324,119 @@ class FastSpeech2(nn.Module):
             if e_t is not None and tuple(e_t.shape) != (B, T):
                 raise ValueError("frame-level e_targets must be [B, max_mel_len]")
         p_dec = normalize_control(p_control, (B, T), dev, "p_control") if p_read_dec else _UNREAD_CONTROL
-        ws = self._workspace(lib.fs2_decode_workspace_bytes(C.byref(m), B, T), dev)
         da = L.DecodeArgs(B=B, L=Lmax, T=T, x_adapted=x_adapted.data_ptr(), cum_dur=cum.data_ptr(),
                           mel_mask_lens=mask_lens32.data_ptr(), p_control=p_dec[1],
                           p_target_frames=L.ptr(p_t) if p_frame else 0, e_target_frames=L.ptr(e_t) if e_frame else 0,
                           p_pred_frames=p_pred.data_ptr() if p_frame else 0, e_pred_frames=e_pred.data_ptr() if e_frame else 0,
-                          mel=mel.data_ptr(), postnet_mel=post.data_ptr(),
-                          workspace=ws.data_ptr(), workspace_bytes=ws.numel())
-        ctl = _control_args(p_dec, _UNREAD_CONTROL)
-        L.check(lib.fs2_acoustic_decode_ctl(C.byref(m), C.byref(da), C.byref(ctl), int(ragged), stream), "fs2_acoustic_decode")
+                          mel=mel.data_ptr(), postnet_mel=post.data_ptr())
+        self._phase("decode", B, T, da, _control_args(p_dec, _UNREAD_CONTROL), ragged, stream, dev, voices)
 
         src_masks = torch.arange(Lmax, device=dev)[None, :] >= src_lens32[:, None]
         mel_masks = torch.arange(T, device=dev)[None, :] >= mask_lens32[:, None]
         return (mel, post, p_pred, e_pred, logd, d_targets if d_targets is not None else d_rounded,
                 src_masks, mel_masks, src_lens_in, mel_lens_out)
+
+    def _phase(self, kind, B, n, args, ctl, ragged, stream, dev, voices):
+        """Phase `kind` of the call ("encode": n = L phonemes, "decode": n = T frames) on self, or with voices = (bank, device voice
+        table) on the bank's voices: each model's position table of >= n rows, the workspace, the call."""
+        lib = L.lib()
+        enc = kind == "encode"
+        for mk in (self,) if voices is None else voices[0].models:
+            m = mk._packed[0]
+            if enc:
+                m.enc_pos, m.enc_pos_rows = mk._position(0, n, m.d_model, dev)
+            else:
+                m.dec_pos, m.dec_pos_rows = mk._position(1, n, m.d_model, dev)
+        if voices is None:
+            target, owner, keep = C.byref(self._packed[0]), self, None
+            size, run = getattr(lib, f"fs2_{kind}_workspace_bytes"), getattr(lib, f"fs2_acoustic_{kind}_ctl")
+        else:
+            owner = voices[0]
+            va, keep = owner._upload(voices[1], dev)
+            target = C.byref(va)
+            size, run = getattr(lib, f"fs2_{kind}_voices_workspace_bytes"), getattr(lib, f"fs2_acoustic_{kind}_voices")
+        ws = owner._workspace(size(target, B, n), dev)
+        args.workspace, args.workspace_bytes = ws.data_ptr(), ws.numel()
+        L.check(run(target, C.byref(args), C.byref(ctl), int(ragged), stream), f"fs2_acoustic_{kind}")
+        del keep
+
+
+def _layout(model):
+    """What shapes a FastSpeech2's packed struct: its state's keys and shapes and the variance feature levels"""
+    return (model.pitch_feature_level, model.energy_feature_level, tuple((k, tuple(v.shape)) for k, v in model.state_dict().items()))
+
+
+class VoiceBank:
+    """Several FastSpeech2 voices of one config in one acoustic call: utterance b of a batch is synthesised by models[voice[b]].
+
+    models: 1 to L.MAX_VOICES FastSpeech2 modules of one config (the same state keys and shapes, feature levels and tc_mask), on one
+    device and in eval mode, such as one fine-tuned checkpoint per voice; voice 0 is models[0].  Each voice keeps its own weights and
+    tables: word and speaker embeddings, pitch / energy bins (from its own stats.json) and embeddings, and position tables.
+
+    bank(voice, speakers, texts, src_lens, max_src_len, ...) takes FastSpeech2.forward's arguments after `voice`, an integer tensor [B]
+    on any device, and returns forward's 10-tuple:
+      * ragged: utterance b equals models[voice[b]] called alone on its slice with ragged=True, bit for bit;
+      * padded: with T the call's output length, row b of every output equals row b of models[voice[b]] called on the same batch with
+        max_mel_len=T (no kernel mixes batch rows, only where the weights come from changes).
+    The call makes the launches of models[0].forward at the same B, L and T, whatever the voice mix, and never reads a device `voice`
+    on the host: an index outside [0, len(models)) there gives that utterance mel_lens 0 and zero durations, leaves the others
+    unchanged, and leaves its other outputs unspecified.  A CPU `voice` is checked: an index out of range raises ValueError.
+    CUDA streams as in forward: the call enqueues on the current stream, synchronises it once without max_mel_len, and caches its
+    workspace per stream; every voice's packed weights are ready on the calling stream."""
+
+    def __init__(self, models):
+        models = tuple(models)
+        if not 1 <= len(models) <= L.MAX_VOICES:
+            raise ValueError(f"a VoiceBank takes 1 to {L.MAX_VOICES} FastSpeech2 models, got {len(models)}")
+        m0 = models[0]
+        for k, mk in enumerate(models):
+            if not isinstance(mk, FastSpeech2):
+                raise ValueError(f"models[{k}] is not a FastSpeech2")
+            if mk.training:
+                raise ValueError(f"models[{k}] is in training mode: call .eval()")
+            if _layout(mk) != _layout(m0):
+                raise ValueError(f"models[{k}]'s config (state shapes or feature levels) differs from models[0]'s")
+            if mk.tc_mask != m0.tc_mask:
+                raise ValueError(f"models[{k}].tc_mask differs from models[0]'s")
+            if get(mk, "mel_linear.weight").device != get(m0, "mel_linear.weight").device:
+                raise ValueError(f"models[{k}] is on {get(mk, 'mel_linear.weight').device}, models[0] on {get(m0, 'mel_linear.weight').device}")
+        self.models = models
+        self._ws, self._ws_stream = None, None     # as FastSpeech2's: the last call's workspace and its stream
+
+    def __call__(self, voice, speakers, texts, src_lens, max_src_len, mels=None, mel_lens=None, max_mel_len=None,
+                 p_targets=None, e_targets=None, d_targets=None, p_control=1.0, e_control=1.0, d_control=1.0, ragged=None):
+        m0 = self.models[0]
+        dev = get(m0, "mel_linear.weight").device
+        with (torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()):
+            return m0._forward(speakers, texts, src_lens, max_src_len, mels, mel_lens, max_mel_len, p_targets, e_targets, d_targets,
+                               p_control, e_control, d_control, m0.ragged if ragged is None else bool(ragged), voices=(self, voice))
+
+    def _voice_table(self, voice, B, dev):
+        """`voice` as the int32 device table the C ABI reads; ValueError for a wrong shape or dtype, or a CPU index out of range."""
+        if not torch.is_tensor(voice) or voice.dtype == torch.bool or voice.is_floating_point() or voice.is_complex():
+            raise ValueError(f"voice must be an integer tensor, got {voice.dtype if torch.is_tensor(voice) else type(voice).__name__}")
+        if tuple(voice.shape) != (B,):
+            raise ValueError(f"voice must have shape [{B}] (one voice per utterance), got {tuple(voice.shape)}")
+        n = len(self.models)
+        if voice.device.type == "cpu" and B and not (0 <= int(voice.min()) and int(voice.max()) < n):
+            raise ValueError(f"voice indices must lie in [0, {n}), got {voice.tolist()}")
+        if voice.dtype != torch.int32:
+            voice = voice.clamp(-1, n)                 # a wide index stays out of range in int32
+        return voice.to(device=dev, dtype=torch.int32).contiguous()
+
+    def _upload(self, voice, dev):
+        """The fs2_acoustic_voices of this phase: the voices' structs (their per-call position pointers included) uploaded from a
+        fresh pinned block with one non_blocking copy (the caching host allocator keeps the block until the copy is done), and what
+        must stay alive while the call is made."""
+        structs = [mk._packed[0] for mk in self.models]
+        raw = bytearray(b"".join(bytes(m) for m in structs))
+        host = torch.empty(len(raw), dtype=torch.uint8, pin_memory=True)
+        host.copy_(torch.frombuffer(raw, dtype=torch.uint8))
+        table = host.to(dev, non_blocking=True)
+        arr = L.acoustic_model_array(structs)
+        va = L.AcousticVoices(n=len(structs), models=C.addressof(arr), models_dev=table.data_ptr(), voice=voice.data_ptr())
+        return va, (arr, table)
+
+    def _workspace(self, nbytes: int, dev):
+        self._ws, self._ws_stream = _streams.workspace((self._ws, self._ws_stream), nbytes, dev, grow=1.25, slack=1024)
+        return self._ws

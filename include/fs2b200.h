@@ -382,6 +382,37 @@ int fs2_acoustic_encode_ctl(const fs2_acoustic_model* m, const fs2_encode_args* 
 int fs2_acoustic_decode_ctl(const fs2_acoustic_model* m, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged,
                             fs2_stream_t stream);
 
+/* Utterances of several voices in one call: fs2_acoustic_{encode,decode}_ctl, but utterance b runs on voice voice[b] of models[0 .. n):
+ * one FastSpeech2 checkpoint per voice, all of one config (fine-tuned copies, or voices trained apart).  The call plans once, on models[0]:
+ * its launches, grids and launch count are those of the single-model call at the same B, L and T, and every launch reads each weight
+ * and table -- convs, LayerNorms, word / speaker / pitch / energy embeddings, bins, position tables -- from the utterance's own voice.
+ * So utterance b equals models[voice[b]] called alone on the same batch, bit for bit: in ragged mode, as that voice's ragged call on its
+ * own slice; padded, as row b of that voice's call on the whole batch (no kernel mixes batch rows).
+ *   - models_dev: a device copy of the n structs models points at; the kernels read each weight's pointer from models_dev[voice[b]], so
+ *     it must stay equal to the host array while the call runs (each voice's per-call position pointers included);
+ *   - the host never reads voice: each phase's first launch stages it into the workspace clamped to voice 0, with a validity flag; an
+ *     utterance whose voice[b] lies outside [0, n) gets 0 frames (mel_lens[b] = 0, d_rounded[b] = 0) without changing the others, and
+ *     its other outputs are unspecified;
+ *   - FS2_ERR_ARG before any CUDA call for n outside [1, FS2_MAX_VOICES], a NULL models, models_dev, voice or model, ragged not 0 or 1,
+ *     a voice whose position tables have fewer than L (encode) or T (decode) rows, and a model whose layout differs from models[0]'s:
+ *     every int field (widths, layers, kernels, n_bins, n_vocab, n_speakers, tc_mask, frame levels, PostNet shape) must be equal, and
+ *     every weight pointer NULL exactly where models[0]'s is and otherwise at the same address modulo 16; then the checks of the
+ *     single-model call.
+ * The workspace bounds (0 for models the call refuses) are the single-model bounds of models[0] plus the staged [2B] int32 table. */
+#define FS2_MAX_VOICES 8
+typedef struct fs2_acoustic_voices {
+  int n;                                     /* [1, FS2_MAX_VOICES] */
+  const fs2_acoustic_model* const* models;   /* host array; models[0] plans and is checked as in the single-model call */
+  const fs2_acoustic_model* models_dev;      /* device copy of the n structs, read per work item */
+  const int32_t* voice;                      /* [B] device */
+} fs2_acoustic_voices;
+size_t fs2_encode_voices_workspace_bytes(const fs2_acoustic_voices* v, int B, int L);
+size_t fs2_decode_voices_workspace_bytes(const fs2_acoustic_voices* v, int B, int T);
+int fs2_acoustic_encode_voices(const fs2_acoustic_voices* v, const fs2_encode_args* a, const fs2_control_args* ctl, int ragged,
+                               fs2_stream_t stream);
+int fs2_acoustic_decode_voices(const fs2_acoustic_voices* v, const fs2_decode_args* a, const fs2_control_args* ctl, int ragged,
+                               fs2_stream_t stream);
+
 /* ------------------------------------------------------------------ vocoder (hifigan Generator.forward) */
 
 typedef struct fs2_vocoder_model {
@@ -714,8 +745,8 @@ const char* fs2_build_info(void);          /* "sm_90a ..." */
  * structs (fs2_resample_args 88, fs2_resample_window_args 144, fs2_resample_stream_t 64, fs2_resample_streams_args 64 bytes; added at
  * ABI 12 without a bump, since no existing struct changed; then fs2_resample_filter_t 24, fs2_resample_mixed_stream_t 80 and
  * fs2_resample_mixed_args 232 bytes, likewise; then fs2_vocoder_streams_ring_args 72, fs2_mel_ring_record_t 56 and
- * fs2_mel_ring_append_args 24 bytes, likewise; then fs2_vocoder_streams_multi_args 88 bytes, likewise) are not in the table: the
- * binding pins their sizes. */
+ * fs2_mel_ring_append_args 24 bytes, likewise; then fs2_vocoder_streams_multi_args 88 bytes, likewise; then fs2_acoustic_voices 32 bytes,
+ * likewise) are not in the table: the binding pins their sizes. */
 size_t fs2_struct_size(int which);
 /* Re-entrancy: the library keeps no mutable process-wide state behind these calls except (a) a per-device table of one-time
  * cudaFuncSetAttribute opt-ins and SM counts, filled under a mutex for the device that is CURRENT when a call is made -- make the

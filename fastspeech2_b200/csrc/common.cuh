@@ -82,36 +82,37 @@ __device__ __forceinline__ RowSpan origin_rows(const int* lens, const int* org, 
   return RowSpan{origin_clamp(-o * scale), origin_clamp((n - o) * scale)};
 }
 
-// Multi-generator mode of the windowed layers (fs2_vocoder_forward_streams_multi): stream b's weights are those of generator gen[b] of
-// the device array `models` (gen as stage_mel staged it: always in range).  A launch names each weight it reads by a GenRef -- the
-// byte offset of its pointer field in fs2_vocoder_model and a float offset past that pointer -- and every work item loads the pointer
-// from its own stream's generator.  models == NULL outside this mode.
-struct GenRef { int32_t off, add; };
-template <class M> struct ModelTable { const M* models; const int* gen; };
-using Generators = ModelTable<fs2_vocoder_model>;
-template <class M>
-__device__ __forceinline__ const float* gen_weight(const ModelTable<M>& g, int b, GenRef r) {
-  const unsigned char* m = reinterpret_cast<const unsigned char*>(g.models + __ldg(g.gen + b));
-  return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(m + r.off))) + r.add;
-}
+// What a launcher takes in the windowed mode, NULL outside it: the layer's window rows and the utterances' origins, never one without
+// the other.
+struct OriginWindow { RowWindow rows; const int* org; };
 
-// Voices mode of the acoustic layers (fs2_acoustic_{encode,decode}_voices): utterance b reads its weights from voice gen[b] of the
-// device array `models` (gen: the phase's staged table, always in range), through the same field lookup as the generators above.  A
-// conv names its fp32 weights, tiles and bias (VoiceLaunch); a row kernel up to four tables (VoiceRow).  models == NULL outside it.
-using Voices = ModelTable<fs2_acoustic_model>;
-struct VoiceLaunch { Voices voices; GenRef w, wt, bias; };
-// in (the phase's first launch only): the caller's voice indices.  That launch reads them itself, clamped to voice 0 outside [0, n),
-// and stages the table the later launches read: out[b] = the clamped index, out[B + b] = 1 if in[b] was in range, else 0.
-struct VoiceRow { Voices voices; GenRef r[4]; const int* in; int n; int* out; };
+// Model table: per-utterance weights, for the vocoder's multi-generator pool (fs2_vocoder_forward_streams_multi, windowed) and the
+// acoustic voices mode (fs2_acoustic_{encode,decode}_voices, offline).  Row b of a launch reads its weights from model sel[b] of the
+// device array of model structs (fs2_vocoder_model or fs2_acoustic_model) at `models`, `stride` bytes apart; sel is a staged table,
+// always in range.  A launch names each weight it reads by a FieldRef -- the byte offset of its pointer field in the model struct and
+// a float offset past that pointer -- and every row loads the pointer from its own model.  models == NULL outside these modes.
+struct FieldRef { int32_t off, add; };
+struct ModelTable { const unsigned char* models; const int* sel; int stride; };
+// model k's weight r.  The byte offset is an int: at most FS2_MAX_GENERATORS / FS2_MAX_VOICES models of a few KB each.
+__device__ __forceinline__ const float* model_weight(const ModelTable& t, int k, FieldRef r) {
+  return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(t.models + (k * t.stride + r.off)))) + r.add;
+}
+// row b's weight r
+__device__ __forceinline__ const float* row_weight(const ModelTable& t, int b, FieldRef r) { return model_weight(t, __ldg(t.sel + b), r); }
+// The weights of one launch in the table mode, NULL outside it: a conv's fp32 weights, tiles and bias; a fused ResBlock launch's pairs,
+// its arguments' (j, d) being ResBlock rb + j at dilation d0 + d of every generator.
+struct LaunchWeights { ModelTable t; FieldRef w, wt, bias; int rb, d0; };
+
+// A row kernel of the voices mode names up to four tables.  in (the phase's first launch only): the caller's voice indices.  That
+// launch reads them itself, clamped to voice 0 outside [0, n), and stages the table the later launches read (t.sel): out[b] = the
+// clamped index, out[B + b] = 1 if in[b] was in range, else 0.
+struct VoiceRow { ModelTable t; FieldRef r[4]; const int* in; int n; int* out; };
 __device__ __forceinline__ int voice_of(const VoiceRow& v, int b) {
-  if (!v.in) return __ldg(v.voices.gen + b);
+  if (!v.in) return __ldg(v.t.sel + b);
   const int k = __ldg(v.in + b);
   return k >= 0 && k < v.n ? k : 0;
 }
-__device__ __forceinline__ const float* voice_table(const VoiceRow& v, int b, int i) {
-  const unsigned char* m = reinterpret_cast<const unsigned char*>(v.voices.models + voice_of(v, b));
-  return reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(m + v.r[i].off))) + v.r[i].add;
-}
+__device__ __forceinline__ const float* voice_table(const VoiceRow& v, int b, int i) { return model_weight(v.t, voice_of(v, b), v.r[i]); }
 __device__ __forceinline__ void voice_stage(const VoiceRow& v, int B) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (v.in && i < B) {
@@ -120,13 +121,6 @@ __device__ __forceinline__ void voice_stage(const VoiceRow& v, int B) {
     v.out[B + i] = k >= 0 && k < v.n;
   }
 }
-// The weights of one windowed launch in the multi-generator mode: a conv's fp32 weights, tiles and bias; a fused ResBlock launch's
-// pairs, its arguments' (j, d) being ResBlock rb + j at dilation d0 + d of every generator.
-struct GenLaunch { Generators gens; GenRef w, wt, bias; int rb, d0; };
-
-// What a launcher takes in the windowed mode, NULL outside it: the layer's window rows and the utterances' origins, never one without
-// the other, and the launch's weights per generator in the multi-generator mode (multi.gens.models != NULL).
-struct OriginWindow { RowWindow rows; const int* org; GenLaunch multi; };
 
 // The mel of the windowed vocoder's streams, staged by stage_mel: stream b's rows at table[b], n_mel floats apart (table != NULL), or at
 // mel + b * bs, rs floats apart; its first frame f0s[b], or f0 for every stream (f0s NULL); its length lens[b] clamped to [0, cap], or

@@ -213,23 +213,14 @@ template <int BM, int BN, int ACT>
 __global__ void __launch_bounds__(256) conv_simt_streams_kernel(const ConvP p) {
   conv_simt_body<BM, BN, ACT, true>(p);
 }
-// Multi-generator mode (fs2_vocoder_forward_streams_multi): a CTA serves one utterance, so it runs the windowed body on the weights and
-// bias of that utterance's generator (g: w and bias; p.bias stays the "has a bias" flag)
-template <int BM, int BN, int ACT>
-__global__ void __launch_bounds__(256) conv_simt_streams_multi_kernel(ConvP p, const GenLaunch g) {
+// Table mode (ModelTable; windowed or offline): a CTA serves one utterance, so it runs the body on the weights and bias of that
+// utterance's model (lw: w and bias; p.bias stays the "has a bias" flag)
+template <int BM, int BN, int ACT, bool WIN>
+__global__ void __launch_bounds__(256) conv_simt_table_kernel(ConvP p, const LaunchWeights lw) {
   const int b = blockIdx.x / p.tiles_per_batch;
-  p.w = gen_weight(g.gens, b, g.w);
-  if (p.bias) p.bias = gen_weight(g.gens, b, g.bias);
-  conv_simt_body<BM, BN, ACT, true>(p);
-}
-
-// Voices mode (fs2_acoustic_{encode,decode}_voices): the offline body on the weights and bias of the CTA's utterance's voice
-template <int BM, int BN, int ACT>
-__global__ void __launch_bounds__(256) conv_simt_voices_kernel(ConvP p, const VoiceLaunch v) {
-  const int b = blockIdx.x / p.tiles_per_batch;
-  p.w = gen_weight(v.voices, b, v.w);
-  if (p.bias) p.bias = gen_weight(v.voices, b, v.bias);
-  conv_simt_body<BM, BN, ACT, false>(p);
+  p.w = row_weight(lw.t, b, lw.w);
+  if (p.bias) p.bias = row_weight(lw.t, b, lw.bias);
+  conv_simt_body<BM, BN, ACT, WIN>(p);
 }
 
 // Tile choice of the launcher (pure host logic, no CUDA call; exposed as fs2_conv_simt_plan so that the GPU tests' coverage of the six
@@ -254,8 +245,8 @@ int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* 
 
 // win (with a->x_lens): NULL, or the windowed mode (OriginWindow; a->T is not used): the tile is chosen for the window's rows.
 // Every output element sums its taps and channels in the same order whatever the tile, so a window computes the offline bits.
-// voices: NULL, or the voices mode (VoiceLaunch, offline only): a->w and a->bias are voice 0's.
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win, const VoiceLaunch* voices) {
+// lw: NULL, or the table mode (LaunchWeights): a->w and a->bias are model 0's.
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win, const LaunchWeights* lw) {
   if (!a || !a->x || !a->w || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if ((a->Cin % BK != 0 && a->Cin != 8) || a->N % 4 != 0) return FS2_ERR_UNSUPPORTED;
@@ -263,8 +254,8 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   if (a->res && ((a->res_row_stride & 3) || (a->res_batch_stride & 3))) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
   if (a->in_act != FS2_ACT_NONE && a->in_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;
-  if ((win && !a->x_lens) || (win && voices)) return FS2_ERR_ARG;
-  if (voices && a->out_act == FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;                              // the acoustic model's activations
+  if (win && !a->x_lens) return FS2_ERR_ARG;
+  if (lw && !win && a->out_act == FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;                         // the acoustic model's activations
   if (win && a->out_act != FS2_ACT_NONE && a->out_act != FS2_ACT_LRELU) return FS2_ERR_UNSUPPORTED;   // the vocoder's activations
   ConvP p;
   p.x = a->x; p.xbs = a->x_batch_stride; p.xrs = a->x_row_stride;
@@ -280,7 +271,6 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   p.y = a->y; p.ybs = a->y_batch_stride; p.yrs = a->y_row_stride;
   p.win = win ? win->rows : RowWindow{0, a->T, a->T};
   p.org = win ? win->org : nullptr;
-  const bool multi = win && win->multi.gens.models;     // a->w and a->bias are generator 0's, checked above
   fs2_conv1d_args rows = *a;
   rows.T = p.win.yend - p.win.y0;
   if (rows.T <= 0) return FS2_ERR_ARG;
@@ -294,17 +284,17 @@ int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* wi
   const dim3 grid((unsigned)plan.grid_x, (unsigned)plan.grid_y);
   prof_before(s);
 #define FS2_SIMT_ACT(BM_, BN_)                                                                            \
-  if (multi) {                                                                                            \
-    if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_multi_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p, win->multi); \
-    else conv_simt_streams_multi_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p, win->multi);      \
+  if (lw && win) {                                                                                        \
+    if (a->out_act == FS2_ACT_LRELU) conv_simt_table_kernel<BM_, BN_, FS2_ACT_LRELU, true><<<grid, 256, 0, s>>>(p, *lw); \
+    else conv_simt_table_kernel<BM_, BN_, FS2_ACT_NONE, true><<<grid, 256, 0, s>>>(p, *lw);              \
   } else if (win) {                                                                                       \
     if (a->out_act == FS2_ACT_LRELU) conv_simt_streams_kernel<BM_, BN_, FS2_ACT_LRELU><<<grid, 256, 0, s>>>(p); \
     else conv_simt_streams_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p);                        \
-  } else if (voices) {                                                                                    \
+  } else if (lw) {                                                                                        \
     switch (a->out_act) {                                                                                 \
-      case FS2_ACT_RELU: conv_simt_voices_kernel<BM_, BN_, FS2_ACT_RELU><<<grid, 256, 0, s>>>(p, *voices); break; \
-      case FS2_ACT_TANH: conv_simt_voices_kernel<BM_, BN_, FS2_ACT_TANH><<<grid, 256, 0, s>>>(p, *voices); break; \
-      default: conv_simt_voices_kernel<BM_, BN_, FS2_ACT_NONE><<<grid, 256, 0, s>>>(p, *voices); break;   \
+      case FS2_ACT_RELU: conv_simt_table_kernel<BM_, BN_, FS2_ACT_RELU, false><<<grid, 256, 0, s>>>(p, *lw); break; \
+      case FS2_ACT_TANH: conv_simt_table_kernel<BM_, BN_, FS2_ACT_TANH, false><<<grid, 256, 0, s>>>(p, *lw); break; \
+      default: conv_simt_table_kernel<BM_, BN_, FS2_ACT_NONE, false><<<grid, 256, 0, s>>>(p, *lw); break; \
     }                                                                                                     \
   } else {                                                                                                \
     switch (a->out_act) {                                                                                 \

@@ -117,13 +117,13 @@ int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t
 
 // a->w_tc must be the tiled layout produced by fastspeech2_b200.packing.pack_conv_tc (see fs2b200.h) in the format a->tc_variant names.
 // win (with a->x_lens): NULL, or the windowed mode (OriginWindow; a->T is not used): the plan is made for the window's rows.
-// voices: NULL, or the voices mode (VoiceLaunch, offline only): a->w_tc and a->bias are voice 0's, every work item reads its voice's.
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win, const VoiceLaunch* voices) {
+// lw: NULL, or the table mode (LaunchWeights): a->w_tc and a->bias are model 0's, every work item reads its utterance's model's.
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win, const LaunchWeights* lw) {
   if (!a || !a->x || !a->w_tc || !a->y) return FS2_ERR_ARG;
   if (a->B <= 0 || a->T <= 0 || a->Cin <= 0 || a->N <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (!conv_tc_supported(a)) return FS2_ERR_UNSUPPORTED;
   if (!aligned16(a->x) || !aligned16(a->w_tc) || !aligned16(a->y) || (a->res && !aligned16(a->res))) return FS2_ERR_ARG;
-  if ((win && !a->x_lens) || (win && voices)) return FS2_ERR_ARG;
+  if (win && !a->x_lens) return FS2_ERR_ARG;
   const unsigned variant = a->tc_variant;
   fs2_conv1d_args slice, rows;
   int nseg, seg_nkc;
@@ -166,14 +166,10 @@ int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win,
   p.stage_off = pl.smem - (int)tc_stage_bytes(pl.NB, tc_stage_tiles(a->res != nullptr, a->accumulate != 0, nseg));   // the staged inputs end the budget
   p.win = win ? win->rows : RowWindow{0, a->T, a->T};
   p.org = win ? win->org : nullptr;
-  static_assert(226 * 1024 + TC_VOICE_SLOT_BYTES <= 227 * 1024, "the slot ring fits between the plan's budget and the opt-in");
+  static_assert(226 * 1024 + TC_TABLE_SLOT_BYTES <= 227 * 1024, "the slot ring fits between the plan's budget and the opt-in");
   p.slot_off = pl.smem;                                 // the unit slot ring (TcSlot) follows the plan's budget, within the 227 KB opt-in
-  const size_t smem = (size_t)pl.smem + (voices ? TC_VOICE_SLOT_BYTES : TC_SLOT_BYTES);
-  if (voices) { p.voices = voices->voices; p.wt_ref = voices->wt; p.bias_ref = voices->bias; }
-  if (win && win->multi.gens.models) {                  // a->w_tc and a->bias are generator 0's: checked above, read per item below
-    if (nseg != 1) return FS2_ERR_UNSUPPORTED;           // one weight-scale header per unit (TcSlot)
-    p.gens = win->multi.gens; p.wt_ref = win->multi.wt; p.bias_ref = win->multi.bias;
-  }
+  const size_t smem = (size_t)pl.smem + (lw ? TC_TABLE_SLOT_BYTES : TC_SLOT_BYTES);
+  if (lw) { p.table = lw->t; p.wt_ref = lw->wt; p.bias_ref = lw->bias; }
   const unsigned grid = (unsigned)pl.grid;
   const bool w = win != nullptr;
   prof_before(s);

@@ -80,24 +80,23 @@ struct TcP {
   int stage_off;                   // shared-memory byte offset of the staged epilogue inputs (used only if tc_stage_tiles(...) > 0)
   RowWindow win;                   // windowed mode (conv_tc_streams_kernel only): rows computed and read, see RowWindow
   const int* org;                  // the windowed mode's per-utterance origins, see origin_rows
-  Generators gens;                 // multi-generator mode (conv_tc_streams_multi_kernel only): wt and bias per work item, see GenRef
-  GenRef wt_ref, bias_ref;         // (bias stays the "has a bias" flag)
+  ModelTable table;                // table mode (conv_tc_table_kernel only): wt and bias per work item, see FieldRef
+  FieldRef wt_ref, bias_ref;       // (bias stays the "has a bias" flag)
   int slot_off;                    // shared-memory byte offset of the TcSlot ring, past the plan's budget
   int NG;                          // NB-channel blocks per work item, computed one after another from the item's slab (see conv_tc_body)
-  Voices voices;                   // voices mode (conv_tc_voices_kernel only): wt and bias per work item through wt_ref / bias_ref
 };
 
-// The weight producer decodes each unit (work item, channel block) -- its tile and block, and its generator's weight-scale header and
-// bias in the multi-generator mode -- into a slot of a small shared-memory ring before it pushes the unit's first weight stage, whose
+// The weight producer decodes each unit (work item, channel block) -- its tile and block, and its model's weight-scale header and
+// bias in the table mode -- into a slot of a small shared-memory ring before it pushes the unit's first weight stage, whose
 // full barrier then publishes the slot to the consumers; they read it in the unit's epilogue.  So the consumer warpgroups hold no
 // work-list cursor (with one, the ragged and windowed cursors' state pushes the 96-register warpgroups into spills).  The producer runs
 // at most TC_SB_MAX stages, so at most TC_SB_MAX units, ahead of an epilogue: TC_SLOTS > TC_SB_MAX + 1 slots.
-// The voices mode's slot also carries the unit's tile base: a K-segmented conv's consumers read segment seg's weight-scale header there.
+// The table mode's slot also carries the unit's tile base: a K-segmented conv's consumers read segment seg's weight-scale header there.
 struct TcSlot { Item it; const float* bias; float inv_ws; int pad_; };
-struct TcVoiceSlot : TcSlot { const float* wt; };
+struct TcTableSlot : TcSlot { const float* wt; };
 constexpr int TC_SLOTS = 16;
 constexpr int TC_SLOT_BYTES = TC_SLOTS * (int)sizeof(TcSlot);
-constexpr int TC_VOICE_SLOT_BYTES = TC_SLOTS * (int)sizeof(TcVoiceSlot);
+constexpr int TC_TABLE_SLOT_BYTES = TC_SLOTS * (int)sizeof(TcTableSlot);
 template <class S = TcSlot>
 __device__ __forceinline__ S& tc_slot(const TcP& p, unsigned char* smem, int u) {
   return reinterpret_cast<S*>(smem + p.slot_off)[u % TC_SLOTS];
@@ -265,11 +264,9 @@ __device__ __forceinline__ void tc_epilogue(const TcP& p, float (&acc)[TG][NB / 
 // WIN: windowed mode with per-utterance origins, see WindowList and origin_rows: the tiles start at p.win.y0, rows at or beyond
 // p.win.yend are not written and rows at or beyond p.win.xend are not read (the host biases x, res and y by the window origins, so rows
 // are window rows here), and utterance b's rows outside [lo_b, hi_b) read as zero.
-// MULTI (with WIN): multi-generator mode: each work item reads the tiles, weight-scale header and bias of its utterance's generator
-// (p.gens), loaded once per item instead of once per CTA.
-// VOICE (offline, padded or ragged): voices mode: each work item reads the tiles, weight-scale headers and bias of its utterance's voice
-// (p.voices), K-segmented convs included.
-template <int NB, bool RAG, bool WIN, bool MULTI = false, bool VOICE = false>
+// TABLE: table mode: each work item reads the tiles, weight-scale headers and bias of its utterance's model (p.table), loaded once
+// per item instead of once per CTA, K-segmented convs included.
+template <int NB, bool RAG, bool WIN, bool TABLE = false>
 __device__ __forceinline__ void conv_tc_body(const TcP& p) {
   constexpr int TG = NB <= 64 ? 2 : 1;
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -286,7 +283,7 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
   uint64_t* emptyB = fullB + TC_SB_MAX;    // [SB_MAX]
   const bool staged = tc_stage_tiles(p.res != nullptr, p.accumulate != 0, p.nseg) > 0;   // the host budgeted tc_stage_bytes
   using Stage = TcStage<NB>;
-  using Slot = std::conditional_t<VOICE, TcVoiceSlot, TcSlot>;
+  using Slot = std::conditional_t<TABLE, TcTableSlot, TcSlot>;
 
   const int KBLOCKS = p.Cin / TC_KB;
   constexpr int CWARPS = TC_CTHREADS / 32;
@@ -315,14 +312,9 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
         const float* wt = p.wt;
         const float* bias = p.bias;
         float inv_ws = inv_ws0;
-        if constexpr (MULTI) {                         // the item's generator's
-          wt = gen_weight(p.gens, pit.b, p.wt_ref);
-          bias = p.bias ? gen_weight(p.gens, pit.b, p.bias_ref) : nullptr;
-          inv_ws = __ldg(wt);
-        }
-        if constexpr (VOICE) {                         // the item's voice's
-          wt = gen_weight(p.voices, pit.b, p.wt_ref);
-          bias = p.bias ? gen_weight(p.voices, pit.b, p.bias_ref) : nullptr;
+        if constexpr (TABLE) {                         // the item's model's
+          wt = row_weight(p.table, pit.b, p.wt_ref);
+          bias = p.bias ? row_weight(p.table, pit.b, p.bias_ref) : nullptr;
           inv_ws = __ldg(wt);
         }
         for (int j = 0; j < NG; j++, u++) {            // the item's blocks, in the consumers' order
@@ -330,7 +322,7 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
           slot.it = Item{pit.nblk * NG + j, pit.b, pit.t0, pit.rows};
           slot.bias = bias;
           slot.inv_ws = inv_ws;
-          if constexpr (VOICE) slot.wt = wt;
+          if constexpr (TABLE) slot.wt = wt;
           for (int seg = 0; seg < p.nseg; seg++) {
             const unsigned char* src = reinterpret_cast<const unsigned char*>(wt) + (long long)seg * p.seg_wbytes + TC_HDR +
                                        (size_t)slot.it.nblk * p.taps * KBLOCKS * stage_bytes;   // tiles are ordered [kb][tap]
@@ -409,10 +401,9 @@ __device__ __forceinline__ void conv_tc_body(const TcP& p) {
         const float* bias = first ? slot.bias : nullptr;
         const int* lens = last ? p.row_lens : nullptr;
         const bool use_res = last && p.res, sum_in = !first || p.accumulate, sum_out = !last;
-        // header: 1 / (power-of-two weight scale) of the unit's generator (multi-generator mode: one segment, checked on the host) or
-        // voice; a K-segmented conv's segment seg has its own
+        // header: 1 / (power-of-two weight scale) of the unit's model; a K-segmented conv's segment seg has its own
         const float* hdr = p.wt;
-        if constexpr (VOICE) hdr = slot.wt;
+        if constexpr (TABLE) hdr = slot.wt;
         const float inv_ws = p.nseg == 1 ? slot.inv_ws
             : __ldg(reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(hdr) + (long long)seg * p.seg_wbytes));
         const int row_base = it.t0 + 64 * g + 16 * (warp & 3);
@@ -551,22 +542,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_kernel(const Tc
   conv_tc_body<NB, true, true>(p);
 }
 
-// Multi-generator mode (fs2_vocoder_forward_streams_multi): the windowed mode with each item's weights from its stream's generator
-template <int NB>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_streams_multi_kernel(const TcP p) {
-  conv_tc_body<NB, true, true, true>(p);
-}
-
-// Voices mode (fs2_acoustic_{encode,decode}_voices): the offline padded (RAG false) or ragged conv with each item's weights from its
-// utterance's voice
-template <int NB, bool RAG>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_voices_kernel(const TcP p) {
-  conv_tc_body<NB, RAG, false, false, true>(p);
+// Table mode (ModelTable): the windowed conv (multi-generator pool) or the offline padded or ragged one (voices) with each item's
+// weights from its utterance's model
+template <int NB, bool RAG, bool WIN>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_table_kernel(const TcP p) {
+  conv_tc_body<NB, RAG, WIN, true>(p);
 }
 
 // The NB instantiations live in their own translation units (conv_tc_nb*.cu) so that the library builds in parallel.
-// conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.  window: the windowed mode
-// (conv_tc_streams_kernel; conv_tc_streams_multi_kernel when p.gens.models is set); p.voices.models set: conv_tc_voices_kernel.
+// conv_tc_prepare_nb / conv_tc_launch_nb return cudaErrorInvalidValue for an NB they do not instantiate.  The entry point follows from
+// the mode: window (the windowed mode), p.table.models (the table mode) and p.x_lens (a ragged offline batch).
 #define FS2_CONV_TC_NB_DECL(nb)                        \
   cudaError_t conv_tc_prepare_nb##nb(int smem_bytes); \
   void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s);
@@ -574,22 +559,21 @@ FS2_CONV_TC_NB_DECL(16) FS2_CONV_TC_NB_DECL(32) FS2_CONV_TC_NB_DECL(48) FS2_CONV
 FS2_CONV_TC_NB_DECL(80) FS2_CONV_TC_NB_DECL(96) FS2_CONV_TC_NB_DECL(112) FS2_CONV_TC_NB_DECL(128)
 #undef FS2_CONV_TC_NB_DECL
 
-#define FS2_CONV_TC_NB_DEF(nb)                                                                          \
-  cudaError_t conv_tc_prepare_nb##nb(int smem_bytes) {                                                  \
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_streams_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_voices_kernel<nb, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_voices_kernel<nb, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes); \
-    return e == cudaSuccess ? cudaFuncSetAttribute(conv_tc_streams_multi_kernel<nb>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) : e; \
-  }                                                                                                     \
-  void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s) {   \
-    if (p.voices.models && p.x_lens) conv_tc_voices_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p); \
-    else if (p.voices.models) conv_tc_voices_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);      \
-    else if (window && p.gens.models) conv_tc_streams_multi_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p); \
-    else if (window) conv_tc_streams_kernel<nb><<<grid, TC_THREADS, smem, s>>>(p);                     \
-    else if (p.x_lens) conv_tc_kernel<nb, true><<<grid, TC_THREADS, smem, s>>>(p);                     \
-    else conv_tc_kernel<nb, false><<<grid, TC_THREADS, smem, s>>>(p);                                  \
+#define FS2_CONV_TC_NB_DEF(nb)                                                                                            \
+  cudaError_t conv_tc_prepare_nb##nb(int smem_bytes) {                                                                    \
+    cudaError_t e = cudaSuccess;                                                                                          \
+    for (const void* k : {(const void*)conv_tc_kernel<nb, false>, (const void*)conv_tc_kernel<nb, true>,                   \
+                          (const void*)conv_tc_streams_kernel<nb>, (const void*)conv_tc_table_kernel<nb, false, false>,    \
+                          (const void*)conv_tc_table_kernel<nb, true, false>, (const void*)conv_tc_table_kernel<nb, true, true>}) \
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);        \
+    return e;                                                                                                             \
+  }                                                                                                                       \
+  void conv_tc_launch_nb##nb(const TcP& p, bool window, unsigned grid, size_t smem, cudaStream_t s) {                     \
+    void (*k)(const TcP);                                                                                                 \
+    if (p.table.models) k = window ? conv_tc_table_kernel<nb, true, true>                                                 \
+                            : p.x_lens ? conv_tc_table_kernel<nb, true, false> : conv_tc_table_kernel<nb, false, false>;    \
+    else k = window ? conv_tc_streams_kernel<nb> : p.x_lens ? conv_tc_kernel<nb, true> : conv_tc_kernel<nb, false>;       \
+    k<<<grid, TC_THREADS, smem, s>>>(p);                                                                                  \
   }
 
 }  // namespace fs2

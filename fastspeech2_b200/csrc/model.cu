@@ -62,11 +62,11 @@ void prof_after(cudaStream_t s, int cls, double flops) {
 }
 
 // kernels / launchers defined in the other translation units
-// win: the vocoder's windowed mode (OriginWindow), NULL everywhere else.  voices / vr: the acoustic voices mode (VoiceLaunch, VoiceRow),
-// NULL everywhere else
-int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const VoiceLaunch* voices = nullptr);
+// win: the vocoder's windowed mode (OriginWindow), NULL everywhere else.  lw / vr: the table mode (LaunchWeights, VoiceRow: the
+// multi-generator pool, the acoustic voices mode), NULL everywhere else
+int conv1d_simt(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const LaunchWeights* lw = nullptr);
 int conv_simt_plan(const fs2_conv1d_args* a, int num_sms, fs2_conv_simt_plan_t* out);
-int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const VoiceLaunch* voices = nullptr);
+int conv1d_tc(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const LaunchWeights* lw = nullptr);
 int attention_fused(const fs2_attention_args* a, void* ws, size_t ws_bytes, cudaStream_t s, bool ragged = false);
 size_t attention_fused_workspace(int B, int T, int H);
 bool conv_tc_supported(const fs2_conv1d_args* a);
@@ -74,12 +74,12 @@ int conv_tc_nb(int N, int nb_max);
 int conv_tc_plan_query(const fs2_conv1d_args* a, int num_sms, fs2_conv_tc_plan_t* out);
 
 // backend dispatch of the fs2_conv1d contract
-static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const VoiceLaunch* voices = nullptr) {
+static int conv1d_dispatch(const fs2_conv1d_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const LaunchWeights* lw = nullptr) {
   if (!a) return FS2_ERR_ARG;
   if (a->x_lens && a->lens_scale < 1) return FS2_ERR_ARG;
-  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win, voices);
-  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win, voices);
-  return conv1d_simt(a, s, win, voices);
+  if (a->backend == FS2_CONV_TC) return conv1d_tc(a, s, win, lw);
+  if (a->backend == FS2_CONV_AUTO && a->w_tc && conv_tc_supported(a)) return conv1d_tc(a, s, win, lw);
+  return conv1d_simt(a, s, win, lw);
 }
 int attention_simt(const fs2_attention_args* a, cudaStream_t s, bool ragged = false, int fused_from = 0);
 int embed_positions(const fs2_embed_args* a, cudaStream_t s, const VoiceRow* vr = nullptr);
@@ -89,8 +89,10 @@ int variance_head(const fs2_variance_head_args* a, cudaStream_t s, const Control
 int durations(const fs2_durations_args* a, cudaStream_t s, const int32_t* src_lens = nullptr, const ControlView* ctl = nullptr,
               const int32_t* valid = nullptr);
 int length_regulate(const fs2_length_regulate_args* a, cudaStream_t s, const VoiceRow* vr = nullptr);
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win = nullptr, long long x_bs = 0, long long wav_bs = 0);
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win = nullptr, int x0 = 0, bool wide = false);
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const LaunchWeights* lw = nullptr,
+              long long x_bs = 0, long long wav_bs = 0);
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win = nullptr, const LaunchWeights* lw = nullptr, int x0 = 0,
+             bool wide = false);
 int stage_mel(const MelSource& src, int B, int x0, int rows, int n_mel, float* out, int32_t* org, int32_t* lens, const int32_t* gen_in,
               int n_gen, int32_t* gen, cudaStream_t s);
 int mel_ring_append(const fs2_mel_ring_append_args* a, cudaStream_t s);
@@ -99,6 +101,17 @@ int resstack_plan(const fs2_resstack_args* a, int num_sms, fs2_resstack_plan_t& 
 int transpose_bct_to_btc(const float* in, float* out, int B, int C, int T, cudaStream_t s);
 int add_positions(float* x, const float* pos, int B, int T, int D, cudaStream_t s, const VoiceRow* vr = nullptr);
 int zero_tail(float* y0, float* y1, const int32_t* lens, int B, int T, int C, cudaStream_t s);
+
+// The table mode (ModelTable): the device array of models M and the staged table of each row's model, and a field's ref relative to
+// model 0 (m)
+template <class M>
+static ModelTable model_table(const M* models_dev, const int32_t* sel) {
+  return ModelTable{reinterpret_cast<const unsigned char*>(models_dev), sel, (int)sizeof(M)};
+}
+template <class M>
+static FieldRef field_ref(const M* m, const void* field, int add = 0) {
+  return FieldRef{(int32_t)((const char*)field - (const char*)m), add};
+}
 
 // ------------------------------------------------------------------ workspace bump allocator
 struct Arena {
@@ -143,23 +156,22 @@ static fs2_conv1d_args conv_args(const float* x, int B, int T, int Cin, int N, i
 //             next conv / pre_relu of the LayerNorm).
 // The voices mode (fs2_acoustic_{encode,decode}_voices): the phase plans and checks on m = models[0] and names each weight a launch reads
 // by its field in *m; utterance b reads that field of voice staged[b] of models_dev.  staged: the phase's [2B] table (VoiceRow::out),
-// staged from the caller's `in` by the phase's first launch.  Each launch's VoiceRow / VoiceLaunch is built right before it.
+// staged from the caller's `in` by the phase's first launch.  Each launch's VoiceRow / LaunchWeights is built right before it.
 struct VoiceSet {
   const fs2_acoustic_model* m;
   const fs2_acoustic_model* models_dev;
   int32_t* staged;
   const int32_t* in; int n;
   mutable VoiceRow vr;
-  mutable VoiceLaunch vl;
-  GenRef ref(const void* field) const { return GenRef{(int32_t)((const char*)field - (const char*)m), 0}; }
+  mutable LaunchWeights lw;
+  FieldRef ref(const void* field) const { return field ? field_ref(m, field) : FieldRef{}; }
   const VoiceRow* row(const void* f0, const void* f1 = nullptr, const void* f2 = nullptr, const void* f3 = nullptr, bool first = false) const {
-    vr = VoiceRow{{models_dev, staged}, {ref(f0), f1 ? ref(f1) : GenRef{}, f2 ? ref(f2) : GenRef{}, f3 ? ref(f3) : GenRef{}},
-                  first ? in : nullptr, n, first ? staged : nullptr};
+    vr = VoiceRow{model_table(models_dev, staged), {ref(f0), ref(f1), ref(f2), ref(f3)}, first ? in : nullptr, n, first ? staged : nullptr};
     return &vr;
   }
-  const VoiceLaunch* conv(const void* w, const void* w_tc, const void* bias) const {
-    vl = VoiceLaunch{{models_dev, staged}, ref(w), ref(w_tc), ref(bias)};
-    return &vl;
+  const LaunchWeights* conv(const void* w, const void* w_tc, const void* bias) const {
+    lw = LaunchWeights{model_table(models_dev, staged), ref(w), ref(w_tc), ref(bias), 0, 0};
+    return &lw;
   }
 };
 // The row tables of a launch: NULL outside the voices mode
@@ -581,7 +593,7 @@ struct View {
 // What a walk issues: the batch's mel view and lengths, the waveform, and five buffers, each B * width floats (window_plan).
 // org: NULL (the offline forward), or the windowed mode: the walk is then the unclipped plan of [0, frames), its rows are window rows,
 // utterance b's window starts at its frame org[b] (origin_rows), and the mel is the staged window buffer.  pre_tc: conv_pre's
-// tensor-core weights, or NULL where the caller's mel layout keeps conv_pre on the fp32 kernel.  gens (windowed mode only): the
+// tensor-core weights, or NULL where the caller's mel layout keeps conv_pre on the fp32 kernel.  table (windowed mode only): the
 // multi-generator mode's generators and staged table (models NULL outside it); the walk plans and checks on m, generator 0.
 struct WinExec {
   int B; cudaStream_t s;
@@ -590,7 +602,7 @@ struct WinExec {
   const float* pre_tc;
   float* wav; int64_t wav_bs;
   float *bx, *bu, *bt, *r1, *r2;
-  Generators gens;
+  ModelTable table;
 };
 
 // fs2_conv1d arguments of a windowed launch: `cap` (a.T) is the layer's full logical length; residual off, as conv_args leaves it
@@ -619,14 +631,18 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   const int* org = ex ? ex->org : nullptr;
   auto len = [&](int scale) { return org ? ORIGIN_CAP : T * scale; };
   OriginWindow ow{};
-  // g: the launch's weights as fields of fs2_vocoder_model, which the multi-generator mode reads per work item (GenLaunch)
-  const Generators gens = ex ? ex->gens : Generators{};
-  auto win = [&](const RowWindow& w, GenLaunch g) -> const OriginWindow* {
-    g.gens = gens;
-    ow = OriginWindow{w, org, gens.models ? g : GenLaunch{}};
+  auto win = [&](const RowWindow& w) -> const OriginWindow* {
+    ow = OriginWindow{w, org};
     return org ? &ow : nullptr;
   };
-  auto ref = [&](const void* field, int add = 0) { return GenRef{(int32_t)((const char*)field - (const char*)m), add}; };
+  // the launch's weights as fields of fs2_vocoder_model, which the multi-generator mode reads per work item
+  LaunchWeights lw{};
+  const ModelTable table = ex ? ex->table : ModelTable{};
+  auto weights = [&](FieldRef w, FieldRef wt, FieldRef bias, int rb = 0, int d0 = 0) -> const LaunchWeights* {
+    lw = LaunchWeights{table, w, wt, bias, rb, d0};
+    return table.models ? &lw : nullptr;
+  };
+  auto ref = [&](const void* field, int add = 0) { return field_ref(m, field, add); };
   // ---- backward: O[i + 1] = the rows stage i's output must hold (O[0]: conv_pre's), U[i] = its ResBlocks' input, Q[i] = the
   // ConvTranspose's phase-group rows
   Rows O[FS2_MAX_STAGES + 1], U[FS2_MAX_STAGES], Q[FS2_MAX_STAGES];
@@ -663,7 +679,7 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
     fs2_conv1d_args c = win_conv_args(ex->mel, ex->mel_bs, ex->mel_rs, B, len(1), m->n_mel, bx, C, 7);
     c.w = m->w_pre; c.w_tc = ex->pre_tc; c.bias = m->b_pre; c.tc_variant = (m->f8_mask & 1) ? FS2_TC_VARIANT_F8 : 0;
     c.x_lens = lens; c.lens_scale = 1;
-    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi}, GenLaunch{{}, ref(&m->w_pre), ref(&m->w_pre_tc), ref(&m->b_pre), 0, 0})));
+    FS2_TRY(conv1d_dispatch(&c, s, win({O[0].lo, O[0].hi, mel.hi}), weights(ref(&m->w_pre), ref(&m->w_pre_tc), ref(&m->b_pre))));
   }
   const float inv_nk = 1.f / (float)m->n_kernels;
   for (int i = 0; i < n; i++) {
@@ -687,9 +703,9 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
       c.bias = m->b_up[i] + off;
       c.in_act = FS2_ACT_LRELU; c.in_slope = 0.1f; c.tc_variant = tcv;
       c.x_lens = lens; c.lens_scale = s0;
-      const GenLaunch gl{{}, ref(g == 0 ? &m->w_up_a[i] : &m->w_up_b[i]), ref(g == 0 ? &m->w_up_a_tc[i] : &m->w_up_b_tc[i]),
-                         ref(&m->b_up[i], (int)off), 0, 0};
-      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi}, gl)));
+      FS2_TRY(conv1d_dispatch(&c, s, win({Q[i].lo, Q[i].hi, x.hi}),
+                              weights(ref(g == 0 ? &m->w_up_a[i] : &m->w_up_b[i]), ref(g == 0 ? &m->w_up_a_tc[i] : &m->w_up_b_tc[i]),
+                                      ref(&m->b_up[i], (int)off))));
     }
     C = Co;
     const View in{bu.p, bu.lo * u, bu.rows * u, C};    // the same buffer at the ResBlocks' rate
@@ -741,8 +757,8 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
             a.alpha = alpha; a.accumulate = accumulate;
           }
           a.x = r.p; a.y = dst.p;
-          const GenLaunch gl{{}, {}, {}, {}, i * m->n_kernels + (run.j < 0 ? 0 : run.j), run.j < 0 ? 0 : run.d0};
-          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}, gl), r.lo, C == 128));
+          FS2_TRY(resstack(&a, s, win({y.lo, y.hi, r.lo + r.rows}),
+                           weights({}, {}, {}, i * m->n_kernels + (run.j < 0 ? 0 : run.j), run.j < 0 ? 0 : run.d0), r.lo, C == 128));
         }
       } else {
         const int j = run.j, d = run.d0, rb = i * m->n_kernels + j, k = m->rb_k[j];
@@ -757,15 +773,13 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
           c.dilation = dil; c.pad_left = (k * dil - dil) / 2;
           c.in_act = c.out_act = FS2_ACT_LRELU; c.in_slope = c.out_slope = 0.1f;
           c.x_lens = lens; c.lens_scale = s1;
-          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi},
-                                             GenLaunch{{}, ref(&m->w_rb1[rb][d]), ref(&m->w_rb1_tc[rb][d]), ref(&m->b_rb1[rb][d]), 0, 0})));
+          FS2_TRY(conv1d_dispatch(&c, s, win({mid.lo, mid.hi, x.hi}), weights(ref(&m->w_rb1[rb][d]), ref(&m->w_rb1_tc[rb][d]), ref(&m->b_rb1[rb][d]))));
           c = win_conv_args(t.at(), t.bs(), C, B, len(s1), C, dst, C, k);
           c.w = m->w_rb2[rb][d]; c.w_tc = m->w_rb2_tc[rb][d]; c.bias = m->b_rb2[rb][d]; c.tc_variant = tcv;
           c.res = r.at(); c.res_batch_stride = r.bs(); c.res_row_stride = C;
           c.alpha = alpha; c.accumulate = accumulate;
           c.x_lens = lens; c.lens_scale = s1;
-          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi},
-                                             GenLaunch{{}, ref(&m->w_rb2[rb][d]), ref(&m->w_rb2_tc[rb][d]), ref(&m->b_rb2[rb][d]), 0, 0})));
+          FS2_TRY(conv1d_dispatch(&c, s, win({y.lo, y.hi, mid.hi}), weights(ref(&m->w_rb2[rb][d]), ref(&m->w_rb2_tc[rb][d]), ref(&m->b_rb2[rb][d]))));
         }
       }
       r = dst;
@@ -778,7 +792,8 @@ static int window_walk(const fs2_vocoder_model* m, int T, int f0, int f1, std::v
   p.x = bx.at(); p.B = B; p.T = len(sc[n]); p.C = C; p.w = m->w_post; p.bias = m->b_post; p.taps = 7; p.in_slope = 0.01f;
   p.wav = ex->wav - post.lo;                           // sample f0 * up is the caller's wav[0]
   p.lens = lens; p.lens_scale = sc[n];
-  return conv_post(&p, s, win({post.lo, post.hi, O[n].hi}, GenLaunch{{}, ref(&m->w_post), {}, ref(&m->b_post), 0, 0}), bx.bs(), ex->wav_bs);   // offline: the strides are its defaults
+  return conv_post(&p, s, win({post.lo, post.hi, O[n].hi}), weights(ref(&m->w_post), {}, ref(&m->b_post)), bx.bs(),
+                   ex->wav_bs);   // offline: the strides are its defaults
 }
 
 // The plan of [0, frames) clipped at T (T < 0: unclipped, the bound of every window of `frames` frames), and the floats per utterance
@@ -828,7 +843,7 @@ static int vocoder_windowed_impl(const fs2_vocoder_model* m, const MelSource& sr
   int32_t* lens = (int32_t*)ar.take((size_t)B * sizeof(int32_t));
   int32_t* gen = mg.gen ? (int32_t*)ar.take((size_t)B * sizeof(int32_t)) : nullptr;
   WinExec ex{B, s, nullptr, (int64_t)rows * m->n_mel, m->n_mel, lens, org, pre_tc, wav, wav_bs,
-             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), Generators{mg.gen ? mg.models_dev : nullptr, gen}};
+             ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), ar.f32(nf), model_table(mg.gen ? mg.models_dev : nullptr, gen)};
   if (ar.dry) return FS2_OK;
   if (!mel || !org || !lens || (mg.gen && !gen) || !ex.bx || !ex.bu || !ex.bt || !ex.r1 || !ex.r2) return FS2_ERR_WORKSPACE;
   FS2_TRY(stage_mel(src, B, x0, rows, m->n_mel, mel, org, lens, mg.gen, mg.n, gen, s));
@@ -984,8 +999,11 @@ int fs2_acoustic_decode_ragged(const fs2_acoustic_model* m, const fs2_decode_arg
 
 static_assert(sizeof(fs2_acoustic_voices) == 32, "fs2_acoustic_voices: an int32 and three pointers");
 
-// Voice k of a voices call runs on voice 0's plan and kernels: the same config and precision policy, and every weight pointer NULL
-// where voice 0's is, else at the same address modulo 16 (the format choices and alignment checks made on voice 0).
+// Model k of a table call (voices, generators) runs on model 0's plan and kernels, so each of its weight pointers q must be NULL where
+// model 0's p is, else at the same address modulo 16 (the format choices and alignment checks made on model 0).
+static bool same_ptr(const float* p, const float* q) { return !p == !q && ((uintptr_t)p & 15u) == ((uintptr_t)q & 15u); }
+
+// Voice k of a voices call: the same config and precision policy as voice 0, and its pointers as same_ptr asks.
 static bool same_acoustic_layout(const fs2_acoustic_model* a, const fs2_acoustic_model* b) {
   if (a->d_model != b->d_model || a->n_head != b->n_head || a->d_inner != b->d_inner || a->k1 != b->k1 || a->k2 != b->k2 ||
       a->n_enc != b->n_enc || a->n_dec != b->n_dec || a->n_mel != b->n_mel || a->vp_filter != b->vp_filter ||
@@ -995,23 +1013,22 @@ static bool same_acoustic_layout(const fs2_acoustic_model* a, const fs2_acoustic
     return false;
   for (int i = 0; i < a->n_postnet; i++)
     if (a->post_cin[i] != b->post_cin[i] || a->post_cout[i] != b->post_cout[i]) return false;
-  auto same = [](const float* p, const float* q) { return !p == !q && ((uintptr_t)p & 15u) == ((uintptr_t)q & 15u); };
   // the weight structs hold pointers only: compared as arrays of them
-  auto same_all = [&](const void* p, const void* q, size_t bytes) {
+  auto same_all = [](const void* p, const void* q, size_t bytes) {
     bool ok = true;
-    for (size_t i = 0; i < bytes / sizeof(const float*); i++) ok = ok && same(((const float* const*)p)[i], ((const float* const*)q)[i]);
+    for (size_t i = 0; i < bytes / sizeof(const float*); i++) ok = ok && same_ptr(((const float* const*)p)[i], ((const float* const*)q)[i]);
     return ok;
   };
-  bool ok = same(a->word_emb, b->word_emb) && same(a->enc_pos, b->enc_pos) && same(a->dec_pos, b->dec_pos) &&
-            same(a->spk_emb, b->spk_emb) && same(a->pitch_bins, b->pitch_bins) && same(a->energy_bins, b->energy_bins) &&
-            same(a->pitch_emb, b->pitch_emb) && same(a->energy_emb, b->energy_emb) && same(a->w_mel, b->w_mel) &&
-            same(a->b_mel, b->b_mel) && same(a->w_mel_tc, b->w_mel_tc);
+  bool ok = same_ptr(a->word_emb, b->word_emb) && same_ptr(a->enc_pos, b->enc_pos) && same_ptr(a->dec_pos, b->dec_pos) &&
+            same_ptr(a->spk_emb, b->spk_emb) && same_ptr(a->pitch_bins, b->pitch_bins) && same_ptr(a->energy_bins, b->energy_bins) &&
+            same_ptr(a->pitch_emb, b->pitch_emb) && same_ptr(a->energy_emb, b->energy_emb) && same_ptr(a->w_mel, b->w_mel) &&
+            same_ptr(a->b_mel, b->b_mel) && same_ptr(a->w_mel_tc, b->w_mel_tc);
   for (int i = 0; i < a->n_enc; i++) ok = ok && same_all(&a->enc[i], &b->enc[i], sizeof(fs2_fft_block_weights));
   for (int i = 0; i < a->n_dec; i++) ok = ok && same_all(&a->dec[i], &b->dec[i], sizeof(fs2_fft_block_weights));
   ok = ok && same_all(&a->dur, &b->dur, sizeof(fs2_predictor_weights)) && same_all(&a->pitch, &b->pitch, sizeof(fs2_predictor_weights)) &&
        same_all(&a->energy, &b->energy, sizeof(fs2_predictor_weights));
   for (int i = 0; i < a->n_postnet; i++)
-    ok = ok && same(a->w_post[i], b->w_post[i]) && same(a->b_post[i], b->b_post[i]) && same(a->w_post_tc[i], b->w_post_tc[i]);
+    ok = ok && same_ptr(a->w_post[i], b->w_post[i]) && same_ptr(a->b_post[i], b->b_post[i]) && same_ptr(a->w_post_tc[i], b->w_post_tc[i]);
   return ok;
 }
 
@@ -1154,8 +1171,7 @@ int fs2_mel_ring_append(const fs2_mel_ring_append_args* a, fs2_stream_t st) { re
 static_assert(sizeof(fs2_vocoder_streams_multi_args) == 88,
               "fs2_vocoder_streams_multi_args: fs2_vocoder_streams_ring_args' fields, gen and models_dev");
 
-// Generator k of a multi-generator call runs on generator 0's plan and kernels: the same architecture and masks, and every weight
-// pointer NULL where generator 0's is, else at the same address modulo 16 (the format choices and alignment checks made on generator 0).
+// Generator k of a multi-generator call: the same architecture and masks as generator 0, and its pointers as same_ptr asks.
 static bool same_generator_layout(const fs2_vocoder_model* a, const fs2_vocoder_model* b) {
   if (a->n_mel != b->n_mel || a->c0 != b->c0 || a->n_stages != b->n_stages || a->n_kernels != b->n_kernels || a->n_dil != b->n_dil ||
       a->f8_mask != b->f8_mask || a->fused_mask != b->fused_mask || a->pair_mask != b->pair_mask || a->pair_kmax != b->pair_kmax)
@@ -1167,16 +1183,15 @@ static bool same_generator_layout(const fs2_vocoder_model* a, const fs2_vocoder_
     for (int d = 0; d < a->n_dil; d++)
       if (a->rb_dil[j][d] != b->rb_dil[j][d]) return false;
   }
-  auto same = [](const float* p, const float* q) { return !p == !q && ((uintptr_t)p & 15u) == ((uintptr_t)q & 15u); };
-  bool ok = same(a->w_pre, b->w_pre) && same(a->b_pre, b->b_pre) && same(a->w_post, b->w_post) && same(a->b_post, b->b_post) &&
-            same(a->w_pre_tc, b->w_pre_tc);
+  bool ok = same_ptr(a->w_pre, b->w_pre) && same_ptr(a->b_pre, b->b_pre) && same_ptr(a->w_post, b->w_post) && same_ptr(a->b_post, b->b_post) &&
+            same_ptr(a->w_pre_tc, b->w_pre_tc);
   for (int i = 0; i < a->n_stages; i++)
-    ok = ok && same(a->w_up_a[i], b->w_up_a[i]) && same(a->w_up_b[i], b->w_up_b[i]) && same(a->b_up[i], b->b_up[i]) &&
-         same(a->w_up_a_tc[i], b->w_up_a_tc[i]) && same(a->w_up_b_tc[i], b->w_up_b_tc[i]);
+    ok = ok && same_ptr(a->w_up_a[i], b->w_up_a[i]) && same_ptr(a->w_up_b[i], b->w_up_b[i]) && same_ptr(a->b_up[i], b->b_up[i]) &&
+         same_ptr(a->w_up_a_tc[i], b->w_up_a_tc[i]) && same_ptr(a->w_up_b_tc[i], b->w_up_b_tc[i]);
   for (int rb = 0; rb < a->n_stages * a->n_kernels; rb++)
     for (int d = 0; d < a->n_dil; d++)
-      ok = ok && same(a->w_rb1[rb][d], b->w_rb1[rb][d]) && same(a->b_rb1[rb][d], b->b_rb1[rb][d]) && same(a->w_rb2[rb][d], b->w_rb2[rb][d]) &&
-           same(a->b_rb2[rb][d], b->b_rb2[rb][d]) && same(a->w_rb1_tc[rb][d], b->w_rb1_tc[rb][d]) && same(a->w_rb2_tc[rb][d], b->w_rb2_tc[rb][d]);
+      ok = ok && same_ptr(a->w_rb1[rb][d], b->w_rb1[rb][d]) && same_ptr(a->b_rb1[rb][d], b->b_rb1[rb][d]) && same_ptr(a->w_rb2[rb][d], b->w_rb2[rb][d]) &&
+           same_ptr(a->b_rb2[rb][d], b->b_rb2[rb][d]) && same_ptr(a->w_rb1_tc[rb][d], b->w_rb1_tc[rb][d]) && same_ptr(a->w_rb2_tc[rb][d], b->w_rb2_tc[rb][d]);
   return ok;
 }
 

@@ -58,17 +58,17 @@ struct RsP {
   int x0;                            // windowed mode: window row of the x map's row 0 (the y map's row 0 is win.y0)
   RowWindow win;                     // windowed mode: rows computed (win.xend is not read: the x map ends the input)
   const int* org;                    // the windowed mode's per-utterance origins, see origin_rows
-  Generators gens; int rb, d0;       // multi-generator mode (the resstack_multi_*kernel entry points): conv[j][d]'s tiles and biases
-                                     // per work item, ResBlock rb + j's at dilation d0 + d of the item's generator (GenLaunch)
+  ModelTable table; int rb, d0;      // table mode (the resstack_multi_*kernel entry points): conv[j][d]'s tiles and biases per work
+                                     // item, ResBlock rb + j's at dilation d0 + d of the item's generator (LaunchWeights)
 };
 
-// Multi-generator mode: pair (j, d)'s conv c2 (0: dilated, 1: dilation 1) of utterance b's generator -- its tiles and its bias
+// Table mode: pair (j, d)'s conv c2 (0: dilated, 1: dilation 1) of utterance b's generator -- its tiles and its bias
 __device__ __forceinline__ RsConv rs_gen_conv(const RsP& p, RsConv cv, int b, int j, int d, int c2) {
   const int slot = ((p.rb + j) * FS2_MAX_DIL + p.d0 + d) * (int)sizeof(void*);
   const int w = (int)(c2 ? offsetof(fs2_vocoder_model, w_rb2_tc) : offsetof(fs2_vocoder_model, w_rb1_tc)) + slot;
   const int bias = (int)(c2 ? offsetof(fs2_vocoder_model, b_rb2) : offsetof(fs2_vocoder_model, b_rb1)) + slot;
-  cv.w = reinterpret_cast<const unsigned char*>(gen_weight(p.gens, b, GenRef{w, 0}));
-  cv.b = gen_weight(p.gens, b, GenRef{bias, 0});
+  cv.w = reinterpret_cast<const unsigned char*>(row_weight(p.table, b, FieldRef{w, 0}));
+  cv.b = row_weight(p.table, b, FieldRef{bias, 0});
   return cv;
 }
 
@@ -505,12 +505,14 @@ static int make_map(CUtensorMap* tm, const float* base, int B, int N, int C, int
 
 // win (with a->lens): NULL, or the windowed mode (OriginWindow; a->N is not used): a->x and a->y are then the window buffers
 // [B][x1 - x0][C] and [B][yend - y0][C] (not biased), x0 / x1 the window rows a->x holds (win->rows.xend is x1).
-int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win, int x0, bool wide) {
+// lw (with win): NULL, or the table mode (LaunchWeights: t, rb, d0): a's tiles and biases are model 0's.
+int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win, const LaunchWeights* lw, int x0, bool wide) {
   if (!a || !a->x || !a->y) return FS2_ERR_ARG;
   if (!aligned16(a->x) || !aligned16(a->y)) return FS2_ERR_ARG;
   if (a->B <= 0 || a->N <= 0 || a->C <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
   if (win && !a->lens) return FS2_ERR_ARG;
+  if (lw && !win) return FS2_ERR_UNSUPPORTED;           // the table mode's entry points are windowed
   const int xrows = win ? win->rows.xend - x0 : a->N, yrows = win ? win->rows.yend - win->rows.y0 : a->N;   // rows of the x and y buffers
   if (xrows <= 0 || yrows <= 0) return FS2_ERR_ARG;
   {  // not in place: a work item re-reads halo rows of x that its neighbours' results would already have overwritten
@@ -566,14 +568,12 @@ int resstack(const fs2_resstack_args* a, cudaStream_t s, const OriginWindow* win
   p.lens = a->lens; p.lens_scale = a->lens_scale;   // the grid stays the padded plan's: the host never reads device lengths
   p.x0 = x0; p.win = win ? win->rows : RowWindow{0, a->N, a->N};
   p.org = win ? win->org : nullptr;
-  if (win && win->multi.gens.models) {                 // a's tiles and biases are generator 0's, checked above
-    p.gens = win->multi.gens; p.rb = win->multi.rb; p.d0 = win->multi.d0;
-  }
+  if (lw) { p.table = lw->t; p.rb = lw->rb; p.d0 = lw->d0; }
   alignas(64) CUtensorMap tmx, tmy;
   FS2_TRY(make_map(&tmx, a->x, a->B, xrows, a->C, 128));
   FS2_TRY(make_map(&tmy, a->y, a->B, yrows, a->C, p.OBOX));
   prof_before(s);
-  if (win && p.gens.models) {
+  if (lw) {
     if (a->C == 32) resstack_multi_kernel<32, 4><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 64) resstack_multi_kernel<64, 2><<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);
     else if (a->C == 128) resstack_multi_wide_kernel<<<plan.grid, RS_THREADS, plan.smem, s>>>(tmx, tmy, p);

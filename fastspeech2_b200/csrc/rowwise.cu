@@ -427,15 +427,15 @@ constexpr int CP_ROWS = 256;
 // Batch strides of x and wav and the rows computed and read: {T * C, T} and {0, T, T} outside the windowed mode (RowWindow; x / wav
 // are then biased by the windows' first rows).
 // org: NULL, or the windowed mode's per-utterance origins (origin_rows): rows and samples outside [lo_b, hi_b) read and write zero.
-// multi: the multi-generator mode's weights (the *_streams_multi_kernel entry points): w and bias of utterance b's generator.
-struct PostRows { long long xbs, wbs; RowWindow win; const int* org; GenLaunch multi; };
-// The conv's weights and bias: the call's, or in the multi-generator mode those of utterance b's generator
+// lw: the table mode's weights (the *_streams_multi_kernel entry points): w and bias of utterance b's generator.
+struct PostRows { long long xbs, wbs; RowWindow win; const int* org; LaunchWeights lw; };
+// The conv's weights and bias: the call's, or in the table mode those of utterance b's generator
 template <bool MULTI>
 __device__ __forceinline__ void conv_post_weights(const fs2_conv_post_args& a, const PostRows& pr, int b, const float*& w, const float*& bias) {
   w = a.w; bias = a.bias;
   if constexpr (MULTI) {
-    w = gen_weight(pr.multi.gens, b, pr.multi.w);
-    bias = gen_weight(pr.multi.gens, b, pr.multi.bias);
+    w = row_weight(pr.lw.t, b, pr.lw.w);
+    bias = row_weight(pr.lw.t, b, pr.lw.bias);
   }
 }
 template <bool ORG, bool MULTI = false>
@@ -605,13 +605,14 @@ __global__ void __launch_bounds__(256) conv_post_c32_streams_multi_kernel(const 
 
 // win (with a->lens): NULL, or the windowed mode (OriginWindow; a->T is not used, a->x and a->wav are biased by the windows' first rows
 // and their batch strides are x_bs and wav_bs).  Both kernels add every output's taps in the same order wherever its tile starts.
-int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win, long long x_bs, long long wav_bs) {
+// lw (with win): NULL, or the table mode (LaunchWeights): a->w and a->bias are model 0's.
+int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* win, const LaunchWeights* lw, long long x_bs, long long wav_bs) {
   if (!a || !a->x || !a->w || !a->bias || !a->wav || a->B <= 0 || a->T <= 0 || a->C <= 0 || a->taps <= 0) return FS2_ERR_ARG;
   if (a->lens && a->lens_scale < 1) return FS2_ERR_ARG;
   if (win && !a->lens) return FS2_ERR_ARG;
-  const PostRows pr = win ? PostRows{x_bs, wav_bs, win->rows, win->org, win->multi}
-                          : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr, GenLaunch{}};
-  const bool multi = win && win->multi.gens.models;     // a->w and a->bias are generator 0's, checked above
+  if (lw && !win) return FS2_ERR_UNSUPPORTED;           // the table mode's entry points are windowed
+  const PostRows pr = win ? PostRows{x_bs, wav_bs, win->rows, win->org, lw ? *lw : LaunchWeights{}}
+                          : PostRows{(long long)a->T * a->C, a->T, RowWindow{0, a->T, a->T}, nullptr, LaunchWeights{}};
   const int rows = pr.win.yend - pr.win.y0;
   if (rows <= 0) return FS2_ERR_ARG;
   if (a->C == 32 && a->taps == 7 && (reinterpret_cast<uintptr_t>(a->x) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a->w) & 15u) == 0) {
@@ -620,7 +621,7 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
     const long long n_groups = (long long)gpb * a->B, blocks = (n_groups * 8 + 255) / 256;
     if (blocks > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
     prof_before(s);
-    if (multi) conv_post_c32_streams_multi_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
+    if (lw) conv_post_c32_streams_multi_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else if (win) conv_post_c32_streams_kernel<7><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else if (a->lens) conv_post_c32_kernel<7, true><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
     else conv_post_c32_kernel<7, false><<<(unsigned)blocks, 256, 0, s>>>(*a, gpb, n_groups, pr);
@@ -634,7 +635,7 @@ int conv_post(const fs2_conv_post_args* a, cudaStream_t s, const OriginWindow* w
   const long long n = (long long)a->B * rows;
   if ((long long)tiles * a->B > 0x7fffffffLL) return FS2_ERR_UNSUPPORTED;
   prof_before(s);
-  if (multi) conv_post_streams_multi_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
+  if (lw) conv_post_streams_multi_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   else if (win) conv_post_streams_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   else conv_post_kernel<<<(unsigned)(tiles * a->B), CP_ROWS, smem, s>>>(*a, tiles, pr);
   prof_after(s, 3, 2.0 * n * a->taps * a->C);

@@ -200,32 +200,12 @@ def test_bank_in_training_mode_raises(lj):
 
 
 # --------------------------------------------------------------------------------------------------------------- SASS of the entry points
-def test_voices_conv_entry_points_are_pipelined_and_do_not_spill():
-    from tests.test_sass_pipeline import LIB, _cuobjdump
-    tool = _cuobjdump()
-    if tool is None or not os.path.isfile(LIB):
-        pytest.skip("cuobjdump or the built library not found")
-    sass, name = {}, None
-    for line in subprocess.run([tool, "-sass", LIB], capture_output=True, text=True, check=True).stdout.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if "conv_tc_voices_kernel" in m.group(1) else None
-            if name:
-                sass[name] = []
-        elif name:
-            sass[name].append(line)
-    usage, name = {}, None
-    for line in subprocess.run([tool, "-res-usage", LIB], capture_output=True, text=True, check=True).stdout.splitlines():
-        m = re.match(r"\s*Function (\S+):", line)
-        if m:
-            name = m.group(1) if "conv_tc_voices_kernel" in m.group(1) else None
-        elif name and "REG:" in line:
-            usage[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", line)}
-            name = None
+def test_offline_table_conv_entry_points_are_pipelined_and_do_not_spill():
+    from tests.test_sass_pipeline import mmas_and_full_waits, res_usage_of, sass_of
+    keep = re.compile(r"\dconv_tc_table_kernelILi\d+ELb[01]ELb0E").search     # the offline ones: conv_tc_table_kernel<NB, RAG, false>
+    sass, usage = sass_of(keep), res_usage_of(keep)
     assert len(sass) == 16 and set(usage) == set(sass)       # 8 NB x (padded, ragged)
-    for f, lines in sass.items():
-        text = "\n".join(lines)
-        mmas = len(re.findall(r"\b[HQ]GMMA\.", text))
-        full_waits = len(re.findall(r"WARPGROUP\.DEPBAR\.LE gsb0, 0x0\b", text))
+    for f, text in sass.items():
+        mmas, full_waits = mmas_and_full_waits(text)
         assert mmas > 0 and full_waits * 4 <= mmas, (f, mmas, full_waits)
         assert usage[f]["STACK"] == 0 and usage[f]["LOCAL"] == 0, (f, usage[f])

@@ -66,7 +66,7 @@ def test_windowed_vocoder_with_groups_equals_short_windows(ragged):
 
 
 def test_multi_generator_pool_with_groups_equals_each_forward():
-    """64 streams of two generators in one pool (conv_tc_streams_multi_kernel, NG = 2 from the first tick's window on) against each
+    """64 streams of two generators in one pool (windowed conv_tc_table_kernel, NG = 2 from the first tick's window on) against each
     stream's own generator's forward on that stream alone (one utterance: NG = 1)."""
     gens = [_generator(configs.HIFIGAN_CONFIG, seed=s) for s in (3, 11)]
     n, frames, chunk = 64, 80, 32

@@ -5,7 +5,8 @@ commit group late (wgmma.wait_group 1), so the tensor core has the next stage's 
 only holds if ptxas sees the MMAs in warp-uniform control flow.  When it does not (warning C7520), it wraps every MMA in its own
 warpgroup arrive + full wait (`WARPGROUP.DEPBAR.LE gsb0, 0x0`): the code still computes the same thing, several times slower, and
 the extra live ranges push the 96-register conv kernels into local-memory spills.  Nothing but the SASS shows it, so it is checked
-here: per kernel, full waits must be rare next to the MMAs, and the conv kernels must not spill.
+here: per kernel, full waits must be rare next to the MMAs, and the conv kernels must not spill.  The parser below also serves the
+SASS checks of the table mode's entry points (test_stream_multi_cpu.py, test_acoustic_voices_cpu.py).
 """
 import os
 import re
@@ -39,18 +40,13 @@ def _dump(flag):
     return subprocess.run([tool, flag, LIB], capture_output=True, text=True, check=True).stdout
 
 
-def _kernel(mangled):
-    return next((k for k in KERNELS if k in mangled), None)
-
-
-@pytest.fixture(scope="module")
-def sass():
-    """{mangled name: SASS text} of every tensor-core kernel"""
+def sass_of(keep):
+    """{mangled name: SASS text} of every function of the library whose mangled name keep(name) accepts"""
     funcs, name = {}, None
     for line in _dump("-sass").splitlines():
         m = re.match(r"\s*Function : (\S+)", line)
         if m:
-            name = m.group(1) if _kernel(m.group(1)) else None
+            name = m.group(1) if keep(m.group(1)) else None
             if name:
                 funcs[name] = []
         elif name:
@@ -58,18 +54,39 @@ def sass():
     return {k: "\n".join(v) for k, v in funcs.items()}
 
 
-@pytest.fixture(scope="module")
-def res_usage():
-    """{mangled name: {resource: value}} of every tensor-core kernel"""
+def res_usage_of(keep):
+    """{mangled name: {resource: value}} of every function of the library whose mangled name keep(name) accepts"""
     out, name = {}, None
     for line in _dump("-res-usage").splitlines():
         m = re.match(r"\s*Function (\S+):", line)
         if m:
-            name = m.group(1) if _kernel(m.group(1)) else None
+            name = m.group(1) if keep(m.group(1)) else None
         elif name and "REG:" in line:
             out[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", line)}
             name = None
     return out
+
+
+def mmas_and_full_waits(text):
+    """wgmma instructions and full wgmma waits in one function's SASS; pipelined: one full wait per accumulator hand-off to an
+    epilogue, a handful per kernel (full_waits * 4 <= mmas); serialised: one per MMA"""
+    return len(re.findall(r"\b[HQ]GMMA\.", text)), len(re.findall(r"WARPGROUP\.DEPBAR\.LE gsb0, 0x0\b", text))
+
+
+def _kernel(mangled):
+    return next((k for k in KERNELS if k in mangled), None)
+
+
+@pytest.fixture(scope="module")
+def sass():
+    """{mangled name: SASS text} of every tensor-core kernel"""
+    return sass_of(_kernel)
+
+
+@pytest.fixture(scope="module")
+def res_usage():
+    """{mangled name: {resource: value}} of every tensor-core kernel"""
+    return res_usage_of(_kernel)
 
 
 def test_every_instantiation_is_found(sass, res_usage):
@@ -83,10 +100,8 @@ def test_mmas_are_not_serialised(sass, kernel):
     for name, text in sass.items():
         if _kernel(name) != kernel:
             continue
-        mmas = len(re.findall(r"\b[HQ]GMMA\.", text))
-        full_waits = len(re.findall(r"WARPGROUP\.DEPBAR\.LE gsb0, 0x0\b", text))
+        mmas, full_waits = mmas_and_full_waits(text)
         assert mmas > 0, name
-        # pipelined: one full wait per accumulator hand-off to an epilogue, a handful per kernel; serialised: one per MMA
         assert full_waits * 4 <= mmas, f"{name}: {full_waits} full wgmma waits for {mmas} MMAs (serialised pipeline)"
 
 

@@ -2,7 +2,6 @@
 checks, workspace), the pool's bookkeeping with a substituted launch call, and the SASS of the multi-generator entry points."""
 import ctypes
 import re
-import subprocess
 
 import pytest
 import torch
@@ -193,44 +192,20 @@ def test_pool_creation_refuses_more_than_max_generators():
 
 
 # --------------------------------------------------------------------------- SASS of the multi-generator entry points
-MULTI_KERNELS = {"conv_tc_streams_multi_kernel": 8, "resstack_multi_kernel": 2, "resstack_multi_narrow_kernel": 2,
-                 "resstack_multi_wide_kernel": 1}
+# the table mode's windowed entry points (mangled-name patterns): conv_tc_table_kernel<NB, true, true> and the fused ResBlock ones
+MULTI_KERNELS = {r"\dconv_tc_table_kernelILi\d+ELb1ELb1E": 8, r"\dresstack_multi_kernelI": 2, r"\dresstack_multi_narrow_kernelI": 2,
+                 r"\dresstack_multi_wide_kernelE": 1}
 
 
-@pytest.fixture(scope="module")
-def multi_sass():
-    from tests.test_sass_pipeline import LIB, _cuobjdump
-    tool = _cuobjdump()
-    if tool is None:
-        pytest.skip("cuobjdump not found")
-    funcs, name = {}, None
-    for line in subprocess.run([tool, "-sass", LIB], capture_output=True, text=True, check=True).stdout.splitlines():
-        m = re.match(r"\s*Function : (\S+)", line)
-        if m:
-            name = m.group(1) if any(k in m.group(1) for k in MULTI_KERNELS) else None
-            if name:
-                funcs[name] = []
-        elif name:
-            funcs[name].append(line)
-    usage, name = {}, None
-    for line in subprocess.run([tool, "-res-usage", LIB], capture_output=True, text=True, check=True).stdout.splitlines():
-        m = re.match(r"\s*Function (\S+):", line)
-        if m:
-            name = m.group(1) if any(k in m.group(1) for k in MULTI_KERNELS) else None
-        elif name and "REG:" in line:
-            usage[name] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", line)}
-            name = None
-    return {k: "\n".join(v) for k, v in funcs.items()}, usage
-
-
-def test_multi_entry_points_are_pipelined_and_the_conv_does_not_spill(multi_sass):
-    sass, usage = multi_sass
+def test_windowed_table_entry_points_are_pipelined_and_the_conv_does_not_spill():
+    from tests.test_sass_pipeline import mmas_and_full_waits, res_usage_of, sass_of
+    keep = re.compile("|".join(MULTI_KERNELS)).search
+    sass, usage = sass_of(keep), res_usage_of(keep)
     for kernel, n in MULTI_KERNELS.items():
-        names = [f for f in sass if re.search(r"\d" + kernel + r"(I|E)", f)]
-        assert len(names) == n and sum(bool(re.search(r"\d" + kernel + r"(I|E)", f)) for f in usage) == n, kernel
+        names = [f for f in sass if re.search(kernel, f)]
+        assert len(names) == n and sum(bool(re.search(kernel, f)) for f in usage) == n, kernel
         for f in names:
-            mmas = len(re.findall(r"\b[HQ]GMMA\.", sass[f]))
-            full_waits = len(re.findall(r"WARPGROUP\.DEPBAR\.LE gsb0, 0x0\b", sass[f]))
+            mmas, full_waits = mmas_and_full_waits(sass[f])
             assert mmas > 0 and full_waits * 4 <= mmas, (f, mmas, full_waits)
-            if kernel == "conv_tc_streams_multi_kernel":
+            if "conv_tc_table_kernel" in kernel:
                 assert usage[f]["STACK"] == 0 and usage[f]["LOCAL"] == 0, (f, usage[f])
